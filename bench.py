@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """bench.py -- views/sec forward+backward of the feature-Gaussian rasterizer (BASELINE.json metric).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--config c3]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--config c3] [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 \
            --master-port P bench.py --gpus N --steps K --warmup W
 
@@ -20,8 +20,13 @@ JSON keys beyond the base contract:
             region (f3dgs_profile_*), against MEASURED_PEAKS.json hbm_gbs.
   cpu_baseline  the CPU oracle (oracle/, a port: the reference has no CPU implementation) on a bounded tile
             sample of the same workload, all host cores, rank 0 at N=1 only.
-`--impl reference` runs the UNMODIFIED reference CUDA extension (oracle/_ref, built from /root/reference's own
-sources for sm_100a) through the identical procedure: the north star compares against "the reference's own
+`--dump-outputs DIR` writes, after the timed steps of `value`, what the last timed step computed (the last view's
+colour / feature / depth maps and radii, the step's accumulated gradients) as DIR/<name>.npy in float32; arrays
+above 512K elements are stored as a fixed, seeded sample of flat indices
+(numpy default_rng(0).integers(0, numel, 512K), sorted).  Inputs are
+seeded, so two builds can be compared output for output.
+`--impl reference` runs the UNMODIFIED reference CUDA extension (oracle/_ref, built from the reference's own
+sources for sm_90a) through the identical procedure: the north star compares against "the reference's own
 rasterizer timed on the same box".  If oracle/_ref is missing it falls back to timing the CPU oracle port.
 """
 import argparse
@@ -50,7 +55,7 @@ def log(*a):
 
 
 class ClockSampler:
-    """nvidia-smi clocks/throttle reasons DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks/throttle reasons DURING the timed region."""
 
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,"
          "clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
@@ -135,6 +140,20 @@ def cpu_baseline(scene, cfg, sample_div=16):
                       f"{cfg}"}
 
 
+def dump_outputs(out_dir, arrays, cap=1 << 19):
+    """name -> tensor, written as float32 DIR/<name>.npy; above `cap` elements a fixed, seeded sample of flat indices
+    (the same for every run and build, so it is not stored)."""
+    import torch
+
+    os.makedirs(out_dir, exist_ok=True)
+    for name, v in arrays.items():
+        a = v.detach().float().reshape(-1)
+        if a.numel() > cap:
+            idx = np.sort(np.random.default_rng(0).integers(0, a.numel(), cap))
+            a = a[torch.from_numpy(idx).long().to(a.device)]
+        np.save(os.path.join(out_dir, name + ".npy"), a.cpu().numpy().astype(np.float32))
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
@@ -153,6 +172,8 @@ def main():
                     help="config c4 only: size of the view batch sharded over the ranks (BASELINE: 64)")
     ap.add_argument("--l2-flush", action="store_true",
                     help="write a 512 MB buffer between timed steps (outside the per-step event pairs)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the outputs of the last timed step as DIR/<name>.npy (float32, at most 64 MB in all)")
     ap.add_argument("--ref-debug", action="store_true",
                     help="reference arm only: debug=True, the reference scripts' default (arguments/__init__.py:71)")
     args = ap.parse_args()
@@ -257,7 +278,7 @@ def main():
 
     # teacher feature map at the teacher's resolution (reference train.py:99: viewpoint_cam.semantic_feature), resident
     Hg, Wg = max(int(round(H / 2.25)), 1), max(int(round(W / 2.25)), 1)
-    gt_feat = torch.rand(C, Hg, Wg, device=dev) if C else None
+    gt_feat = torch.rand(C, Hg, Wg, device=dev, generator=torch.Generator(dev).manual_seed(0)) if C else None
 
     stats = {}
     use_batch = args.impl == "ours" and args.api == "batch" and not fwd_only
@@ -276,6 +297,7 @@ def main():
                 color, feat, radii, depth, ctx = vb.forward(settings_of(cam, cam_dev[i]))
                 vb.backward(ctx, gc, gf if C else None, gd, last=(i == len(cams) - 1))
                 stats["radii"] = radii
+                stats["maps"] = (color, feat, depth)
             vb.all_reduce()
 
         from diff_gaussian_rasterization import feature_head as fh
@@ -307,6 +329,7 @@ def main():
                 for i, cam in enumerate(cams):
                     color, feat, radii, depth = render(cam, cam_dev[i])
                     stats["radii"] = radii
+                    stats["maps"] = (color, feat, depth)
             return
         flat.zero_()
         for i, cam in enumerate(cams):
@@ -317,6 +340,7 @@ def main():
                 gos.append(gf)
             torch.autograd.backward(outs, gos)
             stats["radii"] = radii
+            stats["maps"] = (color, feat, depth)
         flat.all_reduce()
 
     h2d_bytes = sum(h.numel() * 4 for h in cam_host)
@@ -366,7 +390,7 @@ def main():
             barrier()
             total_ms = e0.elapsed_time(e1)
         else:
-            # one event pair per step; the L2 flush (a 512 MB fill, 4x the 126 MB L2) sits between the pairs
+            # one event pair per step; the L2 flush (a 512 MB fill, 10x the 50 MB L2) sits between the pairs
             pairs = []
             for _ in range(steps):
                 flush_buf.fill_(1)
@@ -401,6 +425,17 @@ def main():
         stage_ms, stage_cnt = _C.profile_read()
     views_per_step = n_views
     value = views_per_step * args.steps / (ms_total / 1000.0)
+    if args.dump_outputs and rank == 0:
+        color, feat, depth = stats["maps"]
+        arrays = {"color": color, "depth": depth, "radii": stats["radii"]}
+        if C:
+            arrays["feature_map"] = feat
+        if use_batch:
+            arrays.update({"grad_" + k: v for k, v in vb.grads.items()})
+            arrays.update(grad_accum=vb.grad_accum, denom=vb.denom)
+        elif not fwd_only:
+            arrays.update({"grad_" + k: v.grad for k, v in t.items() if torch.is_tensor(v) and v.grad is not None})
+        dump_outputs(args.dump_outputs, arrays)
 
     # ---------------- timed region 2: end to end
     ms_e2e = timed(step_e2e_batch if use_batch else step_e2e, args.steps, max(args.warmup, 3))
@@ -432,7 +467,7 @@ def main():
         "config": {"workload": cfg_str, "views_per_rank_per_step": VPR, "views_per_step": views_per_step,
                    "parallelism": f"view-sharded dp{world}, 1 grad all-reduce/step" if distributed else "single GPU",
                    "l2": ("explicit flush: 512 MB fill between timed steps, outside the per-step event pairs" if args.l2_flush
-                          else "inputs exceed the 126 MB L2 (per view: features P*C*4 B, upstream grads C*H*W*4 B); no explicit flush"),
+                          else "inputs exceed the 50 MB L2 (per view: features P*C*4 B, upstream grads C*H*W*4 B); no explicit flush"),
                    "api": ("ViewBatch: _C.rasterize_gaussians forward + in-kernel gradient accumulation "
                            "(f3dgs_backward_accum) into one flat buffer, densification statistics folded in" if use_batch else
                            "GaussianRasterizer autograd API (forward" + ("" if fwd_only else " + torch.autograd.backward") + ")"),
@@ -450,9 +485,9 @@ def main():
     }
     if args.impl == "reference":
         out["impl"] = "reference"
-        out["config"]["reference_kind"] = ("unmodified reference CUDA kernels + _C binding (oracle/_ref, sm_100a build), debug="
+        out["config"]["reference_kind"] = ("unmodified reference CUDA kernels + _C binding (oracle/_ref, sm_90a build), debug="
                                            + str(bool(args.ref_debug)) + "; its 60-line Python autograd shim is restated "
-                                           "in oracle/ref_wrapper.py (the reference tree does not travel to the GPU box)")
+                                           "in oracle/ref_wrapper.py (the reference tree is not needed at run time)")
         maps = open("/proc/self/maps").read()
         mine = sorted({ln.split("/")[-1] for ln in maps.splitlines()
                        if "libf3dgs_b200" in ln or "diff_gaussian_rasterization/_C" in ln})
@@ -477,17 +512,11 @@ def main():
             peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
         except Exception:
             pass
-        peak = float(peaks.get("hbm_gbs", 6650.0))
+        peak = float(peaks.get("hbm_gbs", 3350.0))
         achieved = alg[dom] / (per_launch[dom] * 1e-3) / 1e9 if per_launch[dom] > 0 else 0.0
-        traffic = None  # the ncu --set full capture under profiles/ was taken at config 3: null for the other configs
-        try:
-            if args.config == "c3":
-                traffic = json.load(open(os.path.join(ROOT, "profiles", "traffic.json"))).get(dom)
-        except Exception:
-            pass
         out["roofline"] = {"bound": "hbm", "kernel": dom, "achieved": achieved, "peak": peak, "unit": "GB/s",
-                           "frac": achieved / peak, "traffic": traffic,
-                           "peak_source": "MEASURED_PEAKS.json hbm_gbs (of measured)" if peaks else "fallback 6650 (of fallback)",
+                           "frac": achieved / peak,
+                           "peak_source": "MEASURED_PEAKS.json hbm_gbs (of measured)" if peaks else "H100 SXM data sheet 3350 (not measured)",
                            "algorithmic_bytes_per_launch": alg[dom], "launch_ms": per_launch[dom],
                            "V": V, "R": R, "stage_ms_per_launch": per_launch,
                            "other": {k: {"achieved": alg[k] / (per_launch[k] * 1e-3) / 1e9 if per_launch[k] else 0.0,

@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""In-tree build of the two native artefacts (no torch JIT cache, so they travel with gpurun):
+"""In-tree build of the two native artefacts (no torch JIT cache: they live next to the package):
 
-  feature-3dgs_b200/libf3dgs_b200.so           CUDA kernels + C ABI (include/f3dgs_b200.h); nvcc, sm_100a only
+  feature-3dgs_b200/libf3dgs_b200.so           CUDA kernels + C ABI (include/f3dgs_b200.h); nvcc, sm_90a only
   feature-3dgs_b200/diff_gaussian_rasterization/_C*.so   torch/pybind11 binding over the C ABI; g++ only
 
 Usage: python feature-3dgs_b200/build.py [--force]
@@ -19,9 +19,9 @@ OBJ = os.path.join(PKG, "build")
 LIB = os.path.join(PKG, "libf3dgs_b200.so")
 EXT = os.path.join(PKG, "diff_gaussian_rasterization", "_C" + sysconfig.get_config_var("EXT_SUFFIX"))
 CU = ["api.cu", "preprocess.cu", "binning.cu", "composite_fwd.cu", "composite_bwd.cu", "feature_bwd.cu",
-      "composite_fwd_tc.cu", "feature_head.cu", "optimizer.cu"]
+      "feature_head.cu", "optimizer.cu"]
 HDRS = ["common.cuh", "kernels.h", "composite_common.cuh", "tc_common.cuh", os.path.join(ROOT, "include", "f3dgs_b200.h")]
-NVCC_FLAGS = ["-std=c++17", "-O3", "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo",
+NVCC_FLAGS = ["-std=c++17", "-O3", "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo",
               "-Xcompiler", "-fPIC", "-Xptxas", "-v", "--expt-relaxed-constexpr"]
 NVCC_FLAGS += os.environ.get("F3DGS_EXTRA_NVCC_FLAGS", "").split()  # experiments: -DF3DGS_STAGES=6 -DF3DGS_WSLOTS=3 ...
 if os.environ.get("F3DGS_TIMING_BUILD") == "1":  # per-role cycle counters in the composite kernels (debug builds only)
@@ -76,7 +76,7 @@ def build_lib(force=False):
     with ThreadPoolExecutor(max(1, min(len(jobs), os.cpu_count() or 1))) as ex:
         list(ex.map(lambda j: _run(*j), jobs))
     if force or jobs or not os.path.exists(LIB):
-        _run(["nvcc", "-shared", "-o", LIB] + objs + ["-gencode", "arch=compute_100a,code=sm_100a", "-cudart", "static"])
+        _run(["nvcc", "-shared", "-o", LIB] + objs + ["-gencode", "arch=compute_90a,code=sm_90a", "-cudart", "static"])
     return LIB
 
 

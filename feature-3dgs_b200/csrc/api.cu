@@ -25,7 +25,7 @@
 #define F3DGS_BWD2_DEFAULT 1
 #endif
 #ifndef F3DGS_TC_DEFAULT
-#define F3DGS_TC_DEFAULT 1
+#define F3DGS_TC_DEFAULT 0  // H100, config 3: composite_fwd 2.68 ms on the fp32 pipe, 4.32 ms with F3DGS_TC=1
 #endif
 
 namespace f3dgs {
@@ -134,7 +134,7 @@ struct ListLayout {
 
 // Two-kernel backward (default): geometric gradients from the alpha-only kernel at two CTAs per SM, which also emits the
 // blend weights per (tile, block); the feature gradient is a second, streaming kernel over those lists
-// (feature_bwd.cu).  Measured at config 3: 2.80 ms against 3.47 ms for the fused kernel (profiles/r02_variants.jsonl).
+// (feature_bwd.cu).
 // F3DGS_BWD2=0|1 overrides the default per process (A/B runs; both settings are covered by the GPU test-suite).
 inline bool bwd2_mode() {
     static int on = -1;
@@ -145,7 +145,7 @@ inline bool bwd2_mode() {
     return on != 0;
 }
 
-// Tensor-core feature contraction (composite_fwd_tc.cu).  F3DGS_TC=0|1 overrides the default per process (experiments).
+// Tensor-core feature contraction (composite_fwd.cu, launch_composite_fwd_tc).  F3DGS_TC=0|1 overrides the default per process (experiments).
 inline bool tc_mode(int C, const float* features) {
     static int on = -1;
     if (on < 0) {
@@ -155,7 +155,7 @@ inline bool tc_mode(int C, const float* features) {
     static int min_c = -1;  // F3DGS_TC_MIN_C overrides the narrowest width that takes the tensor-core kernel
     if (min_c < 0) {
         const char* e = getenv("F3DGS_TC_MIN_C");
-        min_c = e ? atoi(e) : 33;  // measured: C = 64 (c5, c3 at C = 64) 32% faster on the tensor cores, C = 16 slightly slower
+        min_c = e ? atoi(e) : 33;  // narrower widths fill less than a quarter of the 128-channel MMA tile
     }
     return on && C >= min_c && C % 4 == 0 && (reinterpret_cast<uintptr_t>(features) & 15) == 0;
 }

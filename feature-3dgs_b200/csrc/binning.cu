@@ -7,7 +7,7 @@
 // the Gaussian's rectangle starting at offsets[i-1]; the sort (cub::DeviceRadixSort, api.cu) is
 // stable, so equal keys keep ascending Gaussian order.
 //
-// B200 notes: emission is warp-cooperative -- a warp owns 32 consecutive Gaussians and spreads
+// Notes: emission is warp-cooperative -- a warp owns 32 consecutive Gaussians and spreads
 // the (Gaussian, tile) instances of all of them over its lanes, so one huge splat does not
 // serialise a thread (the reference loops per thread) and the 12-byte-per-instance stores are
 // coalesced runs.

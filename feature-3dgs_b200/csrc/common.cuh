@@ -1,4 +1,4 @@
-// Shared device helpers for the f3dgs_b200 kernels (sm_100a).
+// Shared device helpers for the f3dgs kernels (sm_90a).
 //
 // Numerics contract.  The tile/key indexing of this library must be bit-identical to the
 // reference extension built by nvcc with default flags (-fmad=true, IEEE div/sqrt).  Where a*b+c
@@ -27,6 +27,11 @@ __device__ __forceinline__ float fmar(float a, float b, float c) { return __fmaf
 __device__ __forceinline__ float divr(float a, float b) { return __fdiv_rn(a, b); }
 __device__ __forceinline__ float rcpr(float a) { return __frcp_rn(a); }
 __device__ __forceinline__ float sqrtr(float a) { return __fsqrt_rn(a); }
+// Two independent fma.rn on a pair of accumulators.  The feature loops keep the two pixels of a quad row in one float2;
+// each half is an IEEE fma.rn, so the result is bit-identical to two scalar fmaf calls.
+__device__ __forceinline__ float2 fma2_rn(float2 a, float2 b, float2 c) {
+    return make_float2(__fmaf_rn(a.x, b.x, c.x), __fmaf_rn(a.y, b.y, c.y));
+}
 
 // a0*b0 + a1*b1 + a2*b2 as nvcc contracts it in the reference (GLM mat3 products, dot(),
 // transformPoint): the middle product is a plain multiply, the other two are fused.
@@ -86,7 +91,7 @@ __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
 }
 // The whole wait loop is one asm block: written as a C loop the compiler re-materialises the barrier address (S2R
 // SR_CgaCtaId, LEA, ...) inside it, 17 instructions per poll, and waiting warps then take a quarter of the SM's issue
-// slots from the warps they wait for (ncu source counters, profiles/r01d_*).  Here a poll is TRYWAIT + NANOSLEEP + BRA.
+// slots from the warps they wait for (ncu source counters).  Here a poll is TRYWAIT + NANOSLEEP + BRA.
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
     asm volatile(
         "{\n\t.reg .pred p;\n\t"
@@ -101,7 +106,7 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
 // Wait with a real sleep between polls, for roles that are far ahead of / behind their partner (epilogue waiting for a whole
 // tile, producer waiting for a free stage, ...).  The poll loop of mbar_wait costs three issue slots every ~20 cycles per
 // waiting warp: with ten waiting warps per SM that was 43% of all instructions executed by the tensor-core forward kernel
-// (ncu source counters, profiles/r02_*), taken from the warps on the critical path.  `ns` bounds the added wake-up latency.
+// (ncu source counters), taken from the warps on the critical path.  `ns` bounds the added wake-up latency.
 __device__ __forceinline__ void mbar_wait_sleep(uint64_t* bar, uint32_t parity, uint32_t ns) {
     asm volatile(
         "{\n\t.reg .pred p;\n\t"
@@ -148,11 +153,10 @@ __device__ __forceinline__ void st_na_f4(float* p, float4 v) {
                  "f"(v.w)
                  : "memory");
 }
-// 256-bit store (sm_100: STG.E.ENL2.256): one full 32-byte sector per lane
+// one full 32-byte sector per lane, as two 128-bit stores (the widest global store of sm_90); p 32-byte aligned
 __device__ __forceinline__ void st_na_f8(float* p, float4 a, float4 b) {
-    asm volatile("st.global.L1::no_allocate.v8.f32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};" ::"l"(p), "f"(a.x), "f"(a.y),
-                 "f"(a.z), "f"(a.w), "f"(b.x), "f"(b.y), "f"(b.z), "f"(b.w)
-                 : "memory");
+    st_na_f4(p, a);
+    st_na_f4(p + 4, b);
 }
 __device__ __forceinline__ float4 ld_nc_f4(const float* p) {
     float4 v;

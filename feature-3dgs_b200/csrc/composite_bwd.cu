@@ -42,10 +42,10 @@ static constexpr bool kTimingB = F3DGS_TIMING_BUILD != 0;
 #define BTICK() ((kTimingB && args.dbg) ? clock64() : 0ll)
 
 #ifndef F3DGS_PAIR_SKIP
-#define F3DGS_PAIR_SKIP 1   // 1 (with F3DGS_FFMA2): skip the FFMA2 group of a quad row whose two pixels did not blend
+#define F3DGS_PAIR_SKIP 1   // 1 (with F3DGS_FFMA2): skip the paired FMAs of a quad row whose two pixels did not blend
 #endif
 #ifndef F3DGS_FFMA2
-#define F3DGS_FFMA2 1   // 1: feature-gradient loop on packed fp32 FMAs (fma.rn.f32x2 -> FFMA2), see composite_fwd.cu
+#define F3DGS_FFMA2 1   // 1: feature-gradient loop on paired accumulators (fma2_rn), see composite_fwd.cu
 #endif
 
 #ifndef F3DGS_RED_SLOTS
@@ -427,7 +427,7 @@ composite_bwd_kernel(const BwdArgs args) {
         const int grp = lane / LPR, cl = lane % LPR;
         // upstream feature gradient: [quad][pixel in quad][channel]; with F3DGS_FFMA2 the two pixels of a quad row share a
         // 64-bit register pair (they arrive adjacent from the 128-bit loads, as do their weights from the LDS.128), so one
-        // FFMA2 (weight pair x dO pair + g pair) replaces two FFMAs; g.x / g.y collect the even / odd pixel columns
+        // paired FMA (weight pair x dO pair + g pair, fma2_rn) covers both; g.x / g.y collect the even / odd pixel columns
 #if F3DGS_FFMA2
         float2 dO2[NQ][2][4];
 #define DO(q, i, c) (((i) & 1) ? dO2[q][(i) >> 1][c].y : dO2[q][(i) >> 1][c].x)
@@ -524,14 +524,14 @@ composite_bwd_kernel(const BwdArgs args) {
 #endif
                         {
 #pragma unroll
-                            for (int c = 0; c < 4; c++) gp[c] = __ffma2_rn(w01, dO2[qi][0][c], gp[c]);
+                            for (int c = 0; c < 4; c++) gp[c] = fma2_rn(w01, dO2[qi][0][c], gp[c]);
                         }
 #if F3DGS_PAIR_SKIP
                         if ((pm >> (4 * q)) & 0xCu)
 #endif
                         {
 #pragma unroll
-                            for (int c = 0; c < 4; c++) gp[c] = __ffma2_rn(w23, dO2[qi][1][c], gp[c]);
+                            for (int c = 0; c < 4; c++) gp[c] = fma2_rn(w23, dO2[qi][1][c], gp[c]);
                         }
                     }
                 }
@@ -607,7 +607,7 @@ static cudaError_t launch_bwd_t(const ViewParams& vp, BwdArgs a, cudaStream_t s)
         if (e != cudaSuccess) return e;
         int n = 0;
         cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-        sms_of_device[dev].store(n > 0 ? n : 148);
+        sms_of_device[dev].store(n > 0 ? n : 132);
     }
     const int num_sms = sms_of_device[dev].load();
     a.pa.chunks = CH > 0 ? (vp.C + CH - 1) / CH : 1;
@@ -664,7 +664,7 @@ cudaError_t launch_composite_bwd_geom_slim(const ViewParams& vp, const uint2* ra
         if (e != cudaSuccess) return e;
         int n = 0;
         cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-        sms_of_device[dev].store(n > 0 ? n : 148);
+        sms_of_device[dev].store(n > 0 ? n : 132);
     }
     BwdArgs a;
     a.pa.ranges = ranges; a.pa.point_list = point_list; a.pa.rec = rec; a.pa.features = nullptr;

@@ -235,8 +235,8 @@ struct ProducerArgs {
 // COPYWARP = true: the producer only walks, culls and compacts; it hands each stage's id list to copy_loop() (a
 // second warp of the producer group) through `listed[s]`, and that warp issues the stage's bulk copies.  Issuing a bulk
 // copy costs the issuing warp ~9 instructions and an R2UR round trip per row (UBLKCP takes uniform registers, so the
-// compiler serialises the lanes); with 2.4 M rows per view at config 3 that was ~45% of the producer's instructions
-// and the producer was busy 85% of the time, i.e. the pipeline's critical path (ncu source counters, round 1).
+// compiler serialises the lanes), a large share of the producer's instructions when a stage's rows are many, and the
+// producer is on the pipeline's critical path.
 template <int CH, bool REVERSE, bool COPYWARP = false, typename RING = RingV2<CH>>
 __device__ __forceinline__ void producer_loop(RING& ring, const ProducerArgs& pa) {
     const int lane = threadIdx.x & 31;

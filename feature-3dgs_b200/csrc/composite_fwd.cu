@@ -15,12 +15,17 @@
 //                  the mask, 2x2-pixel quads at a time: one broadcast LDS.128 of weights feeds
 //                  16 FFMAs; the feature float4 is loaded once per instance.  All 32 pixels x 4
 //                  channels (= 128 accumulators per lane at CH = 128) live in registers.
+//   TC feature warps (launch_composite_fwd_tc): the same roles, with the block's contraction
+//                  D[ch, px] = sum_k f[k, ch] * w[k, px] on the tensor cores: per 8 staged instances
+//                  three mma.sync m16n8k8 TF32 products per 16 channels x 8 pixels (3xTF32, tc_common.cuh),
+//                  fp32 accumulators in registers (CH x 32 per warp, as in the fp32 loop).
 // Channel counts above 128 are split into chunks of 128 (extra work items); chunk 0 also writes
 // colour, depth, final_T and n_contrib.
 #include <cstdio>
 #include <cstdlib>
 
 #include "composite_common.cuh"
+#include "tc_common.cuh"
 
 namespace f3dgs {
 
@@ -35,13 +40,13 @@ namespace f3dgs {
 #define F3DGS_FWD_F1 152
 #endif
 #ifndef F3DGS_FFMA2
-#define F3DGS_FFMA2 1          // 1: feature loop on packed fp32 FMAs (fma.rn.f32x2 -> FFMA2): half the FMA issue slots
+#define F3DGS_FFMA2 1          // 1: feature loop on paired accumulators (fma2_rn, common.cuh: two scalar fma.rn on sm_90)
 #endif
 #ifndef F3DGS_DIAG_NO_FMA
 #define F3DGS_DIAG_NO_FMA 0    // diagnostic builds only (WRONG RESULTS): feature warps consume their slots without the FMAs
 #endif
 #ifndef F3DGS_PAIR_SKIP
-#define F3DGS_PAIR_SKIP 1      // 1 (with F3DGS_FFMA2): skip the FFMA2 group of a quad row whose two pixels did not blend
+#define F3DGS_PAIR_SKIP 1      // 1 (with F3DGS_FFMA2): skip the paired FMAs of a quad row whose two pixels did not blend
 #endif
 #ifndef F3DGS_FEAT_PREFETCH
 #define F3DGS_FEAT_PREFETCH 1  // 1: software-pipeline the sparse feature loop by one instance (mask + feature float4)
@@ -63,16 +68,18 @@ struct FwdArgs {
 
 // Forward register budget.  BPA == 1 (20 warps, launched at 96 regs/thread = 61440 in the CTA pool):
 // 4x32x40 + 8x32x64 + 8x32x152 = 60416, feature warps run the sparse quad loop.  The alternative 40/48/168 with the
-// dense hoisted loop (-DF3DGS_FWD_A1=48 -DF3DGS_FWD_F1=168) measured 2.37 ms vs 2.19 ms at c3: the extra FFMA issue
-// of the dense loop takes more from the alpha warps sharing the SMSP than the hoisted loads give back.
-template <int BPA>
+// dense hoisted loop (-DF3DGS_FWD_A1=48 -DF3DGS_FWD_F1=168) is kept as a build option; its extra FMA issue competes
+// with the alpha warps sharing the SMSP.
+// The TC feature warps hold the same CH x 32 accumulators plus the split operand fragments of one K = 8 step:
+// 4x32x40 + 8x32x56 + 8x32x160 = 60416.
+template <int BPA, bool TC = false>
 struct FwdLayout : Layout<BPA> {
-    static constexpr int kRegsAlpha = BPA == 2 ? 104 : F3DGS_FWD_A1;
-    static constexpr int kRegsFeature = BPA == 2 ? 184 : F3DGS_FWD_F1;
+    static constexpr int kRegsAlpha = TC ? 56 : (BPA == 2 ? 104 : F3DGS_FWD_A1);
+    static constexpr int kRegsFeature = TC ? 160 : (BPA == 2 ? 184 : F3DGS_FWD_F1);
     static constexpr bool kPrefetchW = BPA == 2 || F3DGS_FWD_F1 >= 168;
 };
 
-template <int CH, int BPA>
+template <int CH, int BPA, bool TC>
 __global__ void __launch_bounds__(Layout<BPA>::kThreads, 1)
 composite_fwd_kernel(const FwdArgs args) {
     extern __shared__ __align__(128) unsigned char smem_raw[];
@@ -86,7 +93,7 @@ composite_fwd_kernel(const FwdArgs args) {
     const int W = args.pa.W, H = args.pa.H, C = args.pa.C;
     const size_t HW = (size_t)H * W;
 
-    using L = FwdLayout<BPA>;
+    using L = FwdLayout<BPA, TC>;
     constexpr bool kCopyWarp = CH > 0 && F3DGS_FWD_COPYWARP;  // see producer_loop<>
     ring_init<CH>(ring, CH > 0 ? L::kAlphaWarps + kBlocksPerTile : L::kAlphaWarps, CH > 0, kCopyWarp ? 2 : 1);
     __syncthreads();
@@ -392,6 +399,116 @@ composite_fwd_kernel(const FwdArgs args) {
     // ======================================================================== feature warps
     if (CH == 0) return;
     reg_inc<L::kRegsFeature>();
+    if constexpr (TC) {
+        // Tensor-core contraction.  B column n of n-tile ni is pixel (x = 2 ni + (n & 1), y = n >> 1) of the block, so the
+        // accumulators of a lane (columns 2t, 2t + 1 of the four n-tiles) are the 8 pixels of block row t.  Instances of
+        // the stage that did not blend in this block (km bit clear) and rows past the stage's end enter as zeros.
+        constexpr int MT = CH / 16;  // m-tiles of 16 channels
+        const int b = warp - L::kFeatWarp0;
+        const int g = lane >> 2, t = lane & 3;
+        int bcol[4];  // column of ws.w (alpha-warp lane, see lane_px / lane_py) holding pixel (2 ni + (g & 1), g >> 1)
+#pragma unroll
+        for (int ni = 0; ni < 4; ni++) bcol[ni] = ((g >> 2) << 4) | (ni << 2) | (((g >> 1) & 1) << 1) | (g & 1);
+        float d[MT][4][4];
+#pragma unroll
+        for (int mi = 0; mi < MT; mi++)
+#pragma unroll
+            for (int ni = 0; ni < 4; ni++)
+#pragma unroll
+                for (int e = 0; e < 4; e++) d[mi][ni][e] = 0.f;
+        int s = 0, j = 0;
+        uint32_t parity = 0, wparity = 0;
+        for (;;) {
+            mbar_wait(&ring.wfull[b][j], wparity);
+            const WSlot& ws = ring.ws[b][j];
+            const int work = ws.work;
+            if (work < 0) break;
+            const uint32_t km = ws.km, last = ws.last;
+            mbar_wait(&ring.full[s], parity);  // feature rows landed
+            const Stage<CH>& st = ring.stage[s];
+#pragma unroll 1
+            for (int k0 = 0; k0 < kStageEntries; k0 += 8) {
+                const uint32_t kb = (km >> k0) & 0xFFu;
+                if (!kb) continue;  // warp-uniform
+                const int ka = k0 + t, kc = ka + 4;
+                const bool va = (kb >> t) & 1u, vc = (kb >> (t + 4)) & 1u;
+                float bw[4][2];  // raw weights; the hi / lo split is redone at each use (registers go to the accumulators)
+#pragma unroll
+                for (int ni = 0; ni < 4; ni++) {
+                    bw[ni][0] = va ? ws.w[ka][bcol[ni]] : 0.f;
+                    bw[ni][1] = vc ? ws.w[kc][bcol[ni]] : 0.f;
+                }
+#pragma unroll
+                for (int mi = 0; mi < MT; mi++) {
+                    const int c0 = 16 * mi + g;
+                    const float f[4] = {va ? st.feat[ka][c0] : 0.f, va ? st.feat[ka][c0 + 8] : 0.f,
+                                        vc ? st.feat[kc][c0] : 0.f, vc ? st.feat[kc][c0 + 8] : 0.f};
+                    uint32_t ah[4], al[4];
+#pragma unroll
+                    for (int r = 0; r < 4; r++) {
+                        const float hi = tf32_hi(f[r]);
+                        ah[r] = __float_as_uint(hi);
+                        al[r] = __float_as_uint(f[r] - hi);
+                    }
+#pragma unroll
+                    for (int ni = 0; ni < 4; ni++) {
+                        uint32_t bh[2], bl[2];
+#pragma unroll
+                        for (int r = 0; r < 2; r++) {
+                            const float hi = tf32_hi(bw[ni][r]);
+                            bh[r] = __float_as_uint(hi);
+                            bl[r] = __float_as_uint(bw[ni][r] - hi);
+                        }
+                        mma_tf32_16x8x8(d[mi][ni], ah, bh);
+                        mma_tf32_16x8x8(d[mi][ni], ah, bl);
+                        mma_tf32_16x8x8(d[mi][ni], al, bh);
+                    }
+                }
+            }
+            __syncwarp();
+            if (lane == 0) {
+                mbar_arrive(&ring.wempty[b][j]);
+                mbar_arrive(&ring.empty[s]);
+            }
+            if (last) {
+                // ---- epilogue: lane (g, t) writes channels 16 mi + g (+ 8) of block row t, 8 pixels each
+                const int tile = work / args.pa.chunks, chunk = work - tile * args.pa.chunks;
+                const int tile_x = tile % args.pa.tiles_x, tile_y = tile / args.pa.tiles_x;
+                const int bx0 = tile_x * 16 + (b & 1) * 8, yy = tile_y * 16 + (b >> 1) * 4 + t;
+                if (yy < H) {
+#pragma unroll
+                    for (int mi = 0; mi < MT; mi++)
+#pragma unroll
+                        for (int h = 0; h < 2; h++) {
+                            const int ch = chunk * CH + 16 * mi + g + 8 * h;
+                            float* row = args.out_feature + (size_t)ch * HW + (size_t)yy * W + bx0;
+                            if (ch >= C) {
+                            } else if ((args.vec_store & 1) && bx0 + 8 <= W) {
+                                st_na_f4(row, make_float4(d[mi][0][2 * h], d[mi][0][2 * h + 1], d[mi][1][2 * h],
+                                                          d[mi][1][2 * h + 1]));
+                                st_na_f4(row + 4, make_float4(d[mi][2][2 * h], d[mi][2][2 * h + 1], d[mi][3][2 * h],
+                                                              d[mi][3][2 * h + 1]));
+                            } else {
+#pragma unroll
+                                for (int ni = 0; ni < 4; ni++)
+#pragma unroll
+                                    for (int e = 0; e < 2; e++)
+                                        if (bx0 + 2 * ni + e < W) row[2 * ni + e] = d[mi][ni][2 * h + e];
+                            }
+                        }
+                }
+#pragma unroll
+                for (int mi = 0; mi < MT; mi++)
+#pragma unroll
+                    for (int ni = 0; ni < 4; ni++)
+#pragma unroll
+                        for (int e = 0; e < 4; e++) d[mi][ni][e] = 0.f;
+            }
+            if (++s == kStages) { s = 0; parity ^= 1; }
+            if (++j == kWSlots) { j = 0; wparity ^= 1; }
+        }
+        return;
+    }
     {
         constexpr int LPR = CH > 0 ? CH / 4 : 32;  // lanes per feature row
         constexpr int G = 32 / LPR;                // lane groups sharing the 32 pixels
@@ -399,8 +516,8 @@ composite_fwd_kernel(const FwdArgs args) {
         const int b = warp - L::kFeatWarp0;
         const int grp = lane / LPR, cl = lane % LPR;
         // Accumulators [quad][pixel in quad][channel].  With F3DGS_FFMA2 the two pixels of a quad row share a 64-bit
-        // register pair, so one FFMA2 (feature channel broadcast x weight pair + accumulator pair) does the work of two
-        // FFMAs; each half of an f32x2 FMA is an IEEE fma.rn, so the results are bit-identical to the scalar loop.
+        // register pair and one paired FMA (fma2_rn: feature channel broadcast x weight pair + accumulator pair) covers
+        // both; each half is an IEEE fma.rn, so the results are bit-identical to the scalar loop.
 #if F3DGS_FFMA2
         float2 acc2[NQ][2][4];  // [quad][pixel pair (row of the 2x2 quad)][channel]
 #define ACC(q, i, c) (((i) & 1) ? acc2[q][(i) >> 1][c].y : acc2[q][(i) >> 1][c].x)
@@ -419,7 +536,7 @@ composite_fwd_kernel(const FwdArgs args) {
         const float2 w2_ = (W2);                                                                     \
         const float fr_[4] = {f.x, f.y, f.z, f.w};                                                   \
         _Pragma("unroll") for (int c_ = 0; c_ < 4; c_++)                                             \
-            acc2[Q][ROW][c_] = __ffma2_rn(make_float2(fr_[c_], fr_[c_]), w2_, acc2[Q][ROW][c_]);     \
+            acc2[Q][ROW][c_] = fma2_rn(make_float2(fr_[c_], fr_[c_]), w2_, acc2[Q][ROW][c_]);     \
     } while (0)
 #if F3DGS_FFMA2
 #define FEAT_QUAD_FMA(Q, W4)                                                                         \
@@ -428,8 +545,8 @@ composite_fwd_kernel(const FwdArgs args) {
         const float fc_[4] = {f.x, f.y, f.z, f.w};                                                   \
         _Pragma("unroll") for (int c_ = 0; c_ < 4; c_++) {                                           \
             const float2 fb_ = make_float2(fc_[c_], fc_[c_]);                                        \
-            acc2[Q][0][c_] = __ffma2_rn(fb_, w01_, acc2[Q][0][c_]);                                  \
-            acc2[Q][1][c_] = __ffma2_rn(fb_, w23_, acc2[Q][1][c_]);                                  \
+            acc2[Q][0][c_] = fma2_rn(fb_, w01_, acc2[Q][0][c_]);                                  \
+            acc2[Q][1][c_] = fma2_rn(fb_, w23_, acc2[Q][1][c_]);                                  \
         }                                                                                            \
     } while (0)
 #else
@@ -592,9 +709,9 @@ composite_fwd_kernel(const FwdArgs args) {
     }
 }
 
-// Warp layout (see Layout<> in composite_common.cuh): 8 alpha warps x 1 block (BPA = 1).  The 4 x 2 layout measured slower
-// at c3 in round 1 (forward 2.41 vs 2.19 ms, backward 5.5 vs 4.2 ms) and is no longer instantiated.
-template <int CH, int BPA>
+// Warp layout (see Layout<> in composite_common.cuh): 8 alpha warps x 1 block (BPA = 1).  The 4 x 2 layout is not
+// instantiated.
+template <int CH, int BPA, bool TC>
 static cudaError_t launch_fwd_t(const ViewParams& vp, const uint2* ranges, const uint32_t* point_list,
                                 const SplatRec* rec, const float* features, const float* bg, float* final_T,
                                 uint32_t* n_contrib, float* out_color, float* out_feature, float* out_depth,
@@ -607,12 +724,12 @@ static cudaError_t launch_fwd_t(const ViewParams& vp, const uint2* ranges, const
     cudaGetDevice(&dev);
     if (dev < 0 || dev >= 64) return cudaErrorInvalidDevice;
     if (sms_of_device[dev].load() == 0) {
-        cudaError_t e = cudaFuncSetAttribute(composite_fwd_kernel<CH, BPA>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+        cudaError_t e = cudaFuncSetAttribute(composite_fwd_kernel<CH, BPA, TC>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                              (int)smem);
         if (e != cudaSuccess) return e;
         int n = 0;
         cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-        sms_of_device[dev].store(n > 0 ? n : 148);
+        sms_of_device[dev].store(n > 0 ? n : 132);
     }
     const int num_sms = sms_of_device[dev].load();
     FwdArgs a;
@@ -637,7 +754,7 @@ static cudaError_t launch_fwd_t(const ViewParams& vp, const uint2* ranges, const
     if (timing && !dbg) cudaMalloc(&dbg, 256 * 32 * 8 * sizeof(long long));
     a.dbg = timing ? dbg : nullptr;
     if (timing) cudaMemsetAsync(dbg, 0, 256 * 32 * 8 * sizeof(long long), s);
-    composite_fwd_kernel<CH, BPA><<<grid, Layout<BPA>::kThreads, smem, s>>>(a);
+    composite_fwd_kernel<CH, BPA, TC><<<grid, Layout<BPA>::kThreads, smem, s>>>(a);
     g_launches++;
     if (timing) {
         static long long host[256 * 32 * 8];
@@ -657,18 +774,28 @@ static cudaError_t launch_fwd_t(const ViewParams& vp, const uint2* ranges, const
     return cudaGetLastError();
 }
 
-#define F3DGS_FWD_DISPATCH(CHV)                                                                              \
-    launch_fwd_t<CHV, 1>(vp, ranges, point_list, rec, features, bg, final_T, n_contrib, out_color, out_feature, \
+#define F3DGS_FWD_DISPATCH(CHV, TC)                                                                          \
+    launch_fwd_t<CHV, 1, TC>(vp, ranges, point_list, rec, features, bg, final_T, n_contrib, out_color, out_feature, \
                          out_depth, work_counter, s)
 
 cudaError_t launch_composite_fwd(const ViewParams& vp, const uint2* ranges, const uint32_t* point_list,
                                  const SplatRec* rec, const float* features, const float* bg,
                                  float* final_T, uint32_t* n_contrib, float* out_color,
                                  float* out_feature, float* out_depth, int* work_counter, cudaStream_t s) {
-    if (vp.C == 0) return F3DGS_FWD_DISPATCH(0);
-    if (vp.C <= 32) return F3DGS_FWD_DISPATCH(32);
-    if (vp.C <= 64) return F3DGS_FWD_DISPATCH(64);
-    return F3DGS_FWD_DISPATCH(128);
+    if (vp.C == 0) return F3DGS_FWD_DISPATCH(0, false);
+    if (vp.C <= 32) return F3DGS_FWD_DISPATCH(32, false);
+    if (vp.C <= 64) return F3DGS_FWD_DISPATCH(64, false);
+    return F3DGS_FWD_DISPATCH(128, false);
+}
+
+// Preconditions checked by the caller (api.cu): C % 4 == 0 and a 16-byte aligned feature matrix (the feature rows arrive
+// by bulk copies); every other shape takes launch_composite_fwd.
+cudaError_t launch_composite_fwd_tc(const ViewParams& vp, const uint2* ranges, const uint32_t* point_list,
+                                    const SplatRec* rec, const float* features, const float* bg,
+                                    float* final_T, uint32_t* n_contrib, float* out_color,
+                                    float* out_feature, float* out_depth, int* work_counter, cudaStream_t s) {
+    if (vp.C <= 64) return F3DGS_FWD_DISPATCH(64, true);
+    return F3DGS_FWD_DISPATCH(128, true);
 }
 
 }  // namespace f3dgs

@@ -9,7 +9,7 @@
 // feature_bwd_kernel<CH> (here): every warp is an independent worker that pulls (tile, channel chunk, block) items from an
 // atomic counter, keeps the block's upstream gradient dL/dfeature_map (32 pixels x 4 channels per lane) in registers,
 // streams the block's list through a double-buffered cp.async ring (8 entries per step) and forms
-// dL/df[g] += sum_pixels w * dL/dO with the FFMA2 quad loop of composite_bwd.cu, one red.global.add.v4 per lane and
+// dL/df[g] += sum_pixels w * dL/dO with the paired-FMA quad loop of composite_bwd.cu, one red.global.add.v4 per lane and
 // entry.  No inter-warp synchronisation at all; 12 warps per SM.  Channel counts above 128 reuse the same lists for
 // every 128-channel chunk (the alpha evaluation is not repeated per chunk).
 // Reference semantics: backward.cu:565-575 (feature gradient; the feature loss does not feed dL/dalpha, :575 disabled).
@@ -21,10 +21,8 @@
 
 namespace f3dgs {
 
-// (An L2 prefetch of the next chunk's gradient rows ahead of their reductions was measured and lost: 3.06 vs 2.96 ms for the
-// whole backward at config 3, profiles/r02_fwd_tc_diag.txt.)
 #ifndef F3DGS_LIST_CHUNK
-#define F3DGS_LIST_CHUNK 16   // 16: 2.94 ms, 8: 2.96 ms for the whole backward at config 3
+#define F3DGS_LIST_CHUNK 16
 #endif
 constexpr int kListChunk = F3DGS_LIST_CHUNK;   // list entries staged per pipeline step (<= 32)
 constexpr int kFeatWarps = 4;   // independent worker warps per CTA
@@ -184,9 +182,9 @@ __global__ void __launch_bounds__(kFeatWarps * 32, 3) feature_bwd_kernel(const F
                         const float4 w4 = *reinterpret_cast<const float4*>(&sm.w[buf][i][4 * q]);
                         const float2 w01 = make_float2(w4.x, w4.y), w23 = make_float2(w4.z, w4.w);
 #pragma unroll
-                        for (int ch = 0; ch < 4; ch++) gp[ch] = __ffma2_rn(w01, dO2[qi][0][ch], gp[ch]);
+                        for (int ch = 0; ch < 4; ch++) gp[ch] = fma2_rn(w01, dO2[qi][0][ch], gp[ch]);
 #pragma unroll
-                        for (int ch = 0; ch < 4; ch++) gp[ch] = __ffma2_rn(w23, dO2[qi][1][ch], gp[ch]);
+                        for (int ch = 0; ch < 4; ch++) gp[ch] = fma2_rn(w23, dO2[qi][1][ch], gp[ch]);
                     }
                 }
                 float g0 = gp[0].x + gp[0].y, g1 = gp[1].x + gp[1].y, g2 = gp[2].x + gp[2].y, g3 = gp[3].x + gp[3].y;
@@ -216,368 +214,141 @@ __global__ void __launch_bounds__(kFeatWarps * 32, 3) feature_bwd_kernel(const F
 }
 
 // ------------------------------------------------------------------------------------------------ tensor-core variant
-// The same lists, with the per-block contraction on the tensor cores:  D[entry, ch] = sum_px W[entry, px] * dO[ch, px]
-// is, per (tile, block, 128-channel chunk) and per 128 list entries, a GEMM with M = 128 entries, N = 128 channels,
-// K = 32 pixels -- four K = 8 steps of three tcgen05.mma each (3xTF32, tc_common.cuh): 12 MMAs of ~108 cycles
-// (profiles/r02_tc_rate.txt) per 128 entries, where the fp32 kernel above spends 128 x 64 FFMA2.  Both operands are K-major
-// SWIZZLE_128B ([row][32 floats], 16-byte chunk ^ (row & 7)): A = the list rows as they lie in memory (one row = the 32
-// weights of an entry), B = the block's upstream gradient transposed to [channel][pixel] in the list's pixel order.
-//
-// One CTA per SM, 16 warps:
-//   two LOADER groups of four warps, each owning one operand slot and one accumulator: fetch an item, stage B once per item
-//     and A per 128 entries (hi / lo split on the way, the A rows prefetched into registers before the slot is free), then
-//     the group's first thread issues the 12 MMAs and commits them to d_full;
-//   four EPILOGUE warps (tcgen05.ld: lane = entry, registers = channels) transpose their 32 entries through shared memory
-//     so that one red.global.add.v4 instruction covers one entry's 512-byte gradient row, release the accumulator
-//     (d_empty), and issue the REDs of the even rows;
-//   four HELPER warps issue the REDs of the odd rows (a warp's REDs go out one after the other: twice the warps, twice
-//     the REDs in flight).
-namespace {
-
-constexpr int kFbHelp0 = 0, kFbLoad0 = 4, kFbLoadWarpsPerGroup = 4, kFbGroups = 2;
-constexpr int kFbEpi0 = 12, kFbEpiN = 4;
-constexpr int kFbThreads = (kFbEpi0 + kFbEpiN) * 32;
-constexpr int kFbRows = 128;  // list entries per MMA group
-constexpr int kFbTrStride = 132;  // floats; 16-byte aligned rows, conflict-free for lane = row STS.128 and lane = column LDS.128
-
-struct alignas(1024) FbSlot {
-    float Ahi[kFbRows][32];   // list rows (entries x 32 pixels), K-major SWIZZLE_128B
-    float Alo[kFbRows][32];
-    float Bhi[128][32];       // upstream gradient (channels x 32 pixels), K-major SWIZZLE_128B
-    float Blo[128][32];
+// The same work items and lists, with the per-block contraction on the tensor cores:  D[entry, ch] = sum_px W[entry, px] *
+// dO[ch, px]  is, per staged chunk of 16 list entries, a GEMM with M = 16 entries, N = CH channels, K = 32 pixels: four
+// K = 8 steps of three mma.sync m16n8k8 TF32 products per 8 channels (3xTF32, tc_common.cuh).  A = the list rows as they
+// lie in memory (one row = the 32 weights of an entry, zero where the pixel did not blend); B = the block's upstream
+// gradient, staged once per item in shared memory as [channel][pixel] in the list's pixel order (row stride 36 floats:
+// the fragment loads of a warp hit 32 different banks).  Each lane adds its two channels of an entry with one red.v2.
+constexpr int kDoStride = 36;
+template <int CH>
+struct alignas(128) FeatSmemTc {  // per warp
+    float w[2][kListChunk][32];
+    float dO[CH][kDoStride];
 };
-static_assert(sizeof(FbSlot) == 64 * 1024, "operand slot is 64 KB");
+static_assert(kListChunk == 16, "the tensor-core variant stages one m16 tile of entries per chunk");
 
-struct alignas(1024) FbSmem {
-    FbSlot slot[kFbGroups];
-    float tr[kFbEpiN][32][kFbTrStride];  // epilogue transpose: [entry][channel], so that one RED covers one entry's row
-    uint32_t tr_gid[kFbEpiN][32];
-    int32_t tr_rows[kFbEpiN];   // rows of tr[ew] to reduce; < 0: no more work (helper exits)
-    int32_t tr_ch0[kFbEpiN];
-    uint32_t gid[kFbGroups][kFbRows];
-    int32_t cnt[kFbGroups];     // rows of this hand-over; < 0: this group has no more work
-    int32_t ch0[kFbGroups];     // first channel of the chunk
-    int32_t item[kFbGroups];    // work item broadcast inside a loader group
-    uint64_t d_full[kFbGroups], d_empty[kFbGroups];
-    uint32_t tmem_base;
-};
-
-__device__ __forceinline__ void group_sync(int g) {  // named barrier 1 + g over the 128 threads of loader group g
-    asm volatile("bar.sync %0, %1;" ::"r"(1 + g), "r"(kFbLoadWarpsPerGroup * 32) : "memory");
-}
-__device__ __forceinline__ void pair_sync(int ew) {  // named barrier 3 + ew: epilogue warp ew and its helper
-    asm volatile("bar.sync %0, %1;" ::"r"(3 + ew), "r"(64) : "memory");
+__device__ __forceinline__ void red_add_f2(float* p, float a, float b) {
+    asm volatile("red.global.add.v2.f32 [%0], {%1,%2};" ::"l"(p), "f"(a), "f"(b) : "memory");
 }
 
-// REDs of rows first, first + step, ... of one transposed quarter
-__device__ __forceinline__ void fb_reduce_rows(const FbSmem& sm, int ew, int lane, int first, int step, int rows, int ch0,
-                                               const FeatArgs& a) {
-    const bool col_ok = ch0 + lane * 4 < a.C;  // C % 4 == 0 on this path
-    if (!col_ok) return;
-    float* dst = a.dL_dfeature + ch0 + lane * 4;
-    int r = first;
-    for (; r + 3 * step < rows; r += 4 * step) {
-        float4 v[4];
-        uint32_t gid[4];
-#pragma unroll
-        for (int u = 0; u < 4; u++) {
-            gid[u] = sm.tr_gid[ew][r + u * step];
-            v[u] = *reinterpret_cast<const float4*>(&sm.tr[ew][r + u * step][lane * 4]);
-        }
-#pragma unroll
-        for (int u = 0; u < 4; u++) red_add_f4(dst + (size_t)gid[u] * a.C, v[u]);
-    }
-    for (; r < rows; r += step)
-        red_add_f4(dst + (size_t)sm.tr_gid[ew][r] * a.C, *reinterpret_cast<const float4*>(&sm.tr[ew][r][lane * 4]));
-}
-
-// development counters (F3DGS_FBTC_DIAG=1): cycles summed over CTAs -- loader group 0: loop, waiting for its slot;
-// epilogue warp 0: loop, waiting for an accumulator, transposing + reducing
-__device__ unsigned long long fbtc_diag[8];
-
-__device__ __forceinline__ void prefetch_l2(const void* p) { asm volatile("prefetch.global.L2 [%0];" ::"l"(p)); }
-
-constexpr int kFbHelpers = 1, kFbDiag = 2, kFbPrefetch = 4;
-
-__global__ void __launch_bounds__(kFbThreads, 1) feature_bwd_tc_kernel(const FeatArgs a, const int flags) {
-    const int helpers = flags & kFbHelpers;
-    extern __shared__ unsigned char fb_smem_dyn[];
-    FbSmem& sm = *reinterpret_cast<FbSmem*>(fb_smem_dyn + ((1024u - (smem_u32(fb_smem_dyn) & 1023u)) & 1023u));
+template <int CH>
+__global__ void __launch_bounds__(kFeatWarps * 32, 2) feature_bwd_tc_kernel(const FeatArgs a) {
+    extern __shared__ __align__(128) unsigned char smem_raw[];
     const int warp = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0), lane = threadIdx.x & 31;
+    FeatSmemTc<CH>& sm = reinterpret_cast<FeatSmemTc<CH>*>(smem_raw)[warp];
+    constexpr int NT = CH / 8;  // n-tiles of 8 channels
+    const int g = lane >> 2, t = lane & 3;
     const int W = a.W, H = a.H, C = a.C;
     const size_t HW = (size_t)H * W;
 
-    if (threadIdx.x == 0) {
-        for (int g = 0; g < kFbGroups; g++) {
-            mbar_init(&sm.d_full[g], 1);
-            mbar_init(&sm.d_empty[g], kFbEpiN);
-        }
-        mbar_fence_init();
-    }
-    if (warp == 0) tmem_alloc<256>(&sm.tmem_base);
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem = sm.tmem_base;
+    const int items = a.num_tiles * a.chunks * kBlocksPerTile;
+    for (;;) {
+        int item = 0;
+        if (lane == 0) item = atomicAdd(a.work_counter, 1);
+        item = __shfl_sync(0xffffffffu, item, 0);
+        if (item >= items) break;
+        const ItemPos ip = decode_item(item, a);
+        const uint32_t rx = __shfl_sync(0xffffffffu, a.ranges[ip.tile].x, 0);
+        const uint32_t ry = __shfl_sync(0xffffffffu, a.ranges[ip.tile].y, 0);
+        const size_t base = 8 * (size_t)rx + (size_t)ip.b * (ry - rx);
+        const uint32_t n = __shfl_sync(0xffffffffu, a.list_cnt[(size_t)ip.tile * kBlocksPerTile + ip.b], 0);
+        if (n == 0) continue;
+        const int chunk0 = ip.chunk * CH;
+        const uint32_t nch = (n + kListChunk - 1) / kListChunk;
 
-    if (warp >= kFbLoad0 && warp < kFbLoad0 + kFbGroups * kFbLoadWarpsPerGroup) {
-        // ==================================================================== loader groups
-        const int g = (warp - kFbLoad0) / kFbLoadWarpsPerGroup;
-        const int t = threadIdx.x - (kFbLoad0 + g * kFbLoadWarpsPerGroup) * 32;  // 0..127 inside the group
-        const int gw = t >> 5;
-        FbSlot& sl = sm.slot[g];
-        const int items = a.num_tiles * a.chunks * kBlocksPerTile;
-        constexpr uint32_t kIdesc = umma_idesc_tf32(128, 128, 0, 0);
-        uint32_t use = 0;
-        long long c_wait = 0;
-        const long long c_start = clock64();
-        // two items in hand: `item` is staged while the lists and gradient block of `next` are pulled into L2
-        if (t == 0) sm.item[g] = atomicAdd(a.work_counter, 1);
-        group_sync(g);
-        int item = sm.item[g];
-        group_sync(g);
-        if (t == 0) sm.item[g] = atomicAdd(a.work_counter, 1);
-        group_sync(g);
-        int next = sm.item[g];
-        size_t base = 0;
-        uint32_t n = 0;
-        if (item < items) {
-            const ItemPos ip = decode_item(item, a);
-            const uint32_t rx = a.ranges[ip.tile].x, ry = a.ranges[ip.tile].y;
-            base = 8 * (size_t)rx + (size_t)ip.b * (ry - rx);
-            n = a.list_cnt[(size_t)ip.tile * kBlocksPerTile + ip.b];
-        }
-        while (item < items) {
-            group_sync(g);  // everyone has read the index
-            if (t == 0) sm.item[g] = atomicAdd(a.work_counter, 1);
-            const ItemPos ip = decode_item(item, a);
-            const bool has_next = next < items;
-            const ItemPos ip2 = decode_item(has_next ? next : 0, a);
-            size_t nbase = 0;
-            uint32_t nn = 0;
-            if (has_next) {
-                const uint32_t rx = a.ranges[ip2.tile].x, ry = a.ranges[ip2.tile].y;
-                nbase = 8 * (size_t)rx + (size_t)ip2.b * (ry - rx);
-                nn = a.list_cnt[(size_t)ip2.tile * kBlocksPerTile + ip2.b];
+        auto issue = [&](uint32_t c, int buf) {
+            const uint32_t cnt = min((uint32_t)kListChunk, n - c * kListChunk);
+            const float* wsrc = a.list_w + (base + (size_t)c * kListChunk) * 32;
+            for (uint32_t j = lane; j < cnt * 8; j += 32) cp_async16(&sm.w[buf][0][0] + j * 4, wsrc + j * 4);
+            cp_async_commit();
+        };
+        issue(0, 0);
+        {   // upstream gradient of the block: lane = pixel (list order, see lane_px / lane_py), one channel per trip
+            const int xx = ip.bx0 + lane_px(lane), yy = ip.by0 + lane_py(lane);
+            const bool in = xx < W && yy < H;
+            for (int c = 0; c < CH; c++) {
+                const int ch = chunk0 + c;
+                sm.dO[c][lane] = (in && ch < C) ? __ldg(a.dL_dfeat_pix + (size_t)ch * HW + (size_t)yy * W + xx) : 0.f;
             }
-            for (uint32_t e0 = 0; e0 < n; e0 += kFbRows, use++) {
-                const uint32_t cnt = min((uint32_t)kFbRows, n - e0);
-                // ---- A: 128 list rows of 128 bytes; a warp instruction moves four rows (8 lanes x 16 bytes each).  Loaded
-                // before the slot is free: the global latency overlaps the previous group's MMAs and accumulator read.
-                const float* wsrc = a.list_w + (base + e0) * 32;
-                float4 q[kFbRows / 16];
-#pragma unroll
-                for (int it = 0; it < kFbRows / 16; it++) {
-                    const int row = it * 16 + gw * 4 + (lane >> 3);
-                    q[it] = make_float4(0.f, 0.f, 0.f, 0.f);
-                    if (row < (int)cnt) q[it] = __ldg(reinterpret_cast<const float4*>(wsrc + (size_t)row * 32) + (lane & 7));
-                }
-                const uint32_t my_gid = t < (int)cnt ? __ldg(&a.list_meta[base + e0 + t]).x : 0u;
-                if (e0 == 0 && has_next && (flags & kFbPrefetch)) {
-                    if ((uint32_t)t < nn) prefetch_l2(a.list_w + (nbase + t) * 32);
-                    if ((uint32_t)t + 128u < nn) prefetch_l2(a.list_w + (nbase + 128 + t) * 32);
-                    if ((uint32_t)t * 16u < min(nn, 256u)) prefetch_l2(a.list_meta + nbase + t * 16);
-                    const int ch2 = ip2.chunk * 128 + t;
-                    if (ch2 < C) {
-#pragma unroll
-                        for (int y = 0; y < 4; y++)
-                            if (ip2.by0 + y < H) prefetch_l2(a.dL_dfeat_pix + (size_t)ch2 * HW + (size_t)(ip2.by0 + y) * W + ip2.bx0);
-                    }
-                }
-                const long long c0 = clock64();
-                mbar_wait_sleep(&sm.d_empty[g], (use & 1u) ^ 1u, 32);
-                c_wait += clock64() - c0;
-#pragma unroll
-                for (int it = 0; it < kFbRows / 16; it++) {
-                    const int row = it * 16 + gw * 4 + (lane >> 3), c16 = lane & 7;
-                    const float4 hi = make_float4(tf32_hi(q[it].x), tf32_hi(q[it].y), tf32_hi(q[it].z), tf32_hi(q[it].w));
-                    const float4 lo = make_float4(q[it].x - hi.x, q[it].y - hi.y, q[it].z - hi.z, q[it].w - hi.w);
-                    const int o = row * 32 + ((c16 ^ (row & 7)) << 2);
-                    *reinterpret_cast<float4*>(&sl.Ahi[0][0] + o) = hi;
-                    *reinterpret_cast<float4*>(&sl.Alo[0][0] + o) = lo;
-                }
-                sm.gid[g][t] = my_gid;
-                if (e0 == 0) {
-                    // ---- B: this thread's channel, 32 pixels of the block, transposed into the list's pixel order
-                    const int ch = ip.chunk * 128 + t;
-                    float v[4][8];
-#pragma unroll
-                    for (int y = 0; y < 4; y++)
-#pragma unroll
-                        for (int x = 0; x < 8; x++) v[y][x] = 0.f;
-                    if (ch < C) {
-                        const float* plane = a.dL_dfeat_pix + (size_t)ch * HW;
-#pragma unroll
-                        for (int y = 0; y < 4; y++) {
-                            const int yy = ip.by0 + y;
-                            if (yy >= H) continue;
-                            if ((a.vec & 2) && ip.bx0 + 8 <= W) {
-                                const float4 p0 = ld_nc_f4(plane + (size_t)yy * W + ip.bx0);
-                                const float4 p1 = ld_nc_f4(plane + (size_t)yy * W + ip.bx0 + 4);
-                                v[y][0] = p0.x; v[y][1] = p0.y; v[y][2] = p0.z; v[y][3] = p0.w;
-                                v[y][4] = p1.x; v[y][5] = p1.y; v[y][6] = p1.z; v[y][7] = p1.w;
-                            } else {
-#pragma unroll
-                                for (int x = 0; x < 8; x++)
-                                    if (ip.bx0 + x < W) v[y][x] = __ldg(plane + (size_t)yy * W + ip.bx0 + x);
-                            }
-                        }
-                    }
-                    // chunk j of the row = list lanes 4j .. 4j+3 = the 2x2 quad at (px0, py0) = ((j & 3) * 2, (j >> 2) * 2)
-#pragma unroll
-                    for (int j = 0; j < 8; j++) {
-                        const int px0 = (j & 3) * 2, py0 = (j >> 2) * 2;
-                        const float4 p = make_float4(v[py0][px0], v[py0][px0 + 1], v[py0 + 1][px0], v[py0 + 1][px0 + 1]);
-                        const float4 hi = make_float4(tf32_hi(p.x), tf32_hi(p.y), tf32_hi(p.z), tf32_hi(p.w));
-                        const float4 lo = make_float4(p.x - hi.x, p.y - hi.y, p.z - hi.z, p.w - hi.w);
-                        const int o = t * 32 + ((j ^ (t & 7)) << 2);
-                        *reinterpret_cast<float4*>(&sl.Bhi[0][0] + o) = hi;
-                        *reinterpret_cast<float4*>(&sl.Blo[0][0] + o) = lo;
-                    }
-                }
-                if (t == 0) {
-                    sm.cnt[g] = (int)cnt;
-                    sm.ch0[g] = ip.chunk * 128;
-                }
-                fence_async_smem();
-                group_sync(g);
-                if (t == 0) {
-                    tc_fence_after();
-                    const uint32_t ah = smem_u32(&sl.Ahi[0][0]), al = smem_u32(&sl.Alo[0][0]);
-                    const uint32_t bh = smem_u32(&sl.Bhi[0][0]), bl = smem_u32(&sl.Blo[0][0]);
-                    const uint32_t d = tmem + (uint32_t)g * 128u;
-#pragma unroll
-                    for (int k = 0; k < 4; k++) {  // 8 pixels = 32 bytes inside the swizzled 128-byte rows
-                        const uint64_t a_hi = umma_desc(ah + k * 32, 16, 1024, kUmmaSw128), a_lo = umma_desc(al + k * 32, 16, 1024, kUmmaSw128);
-                        const uint64_t b_hi = umma_desc(bh + k * 32, 16, 1024, kUmmaSw128), b_lo = umma_desc(bl + k * 32, 16, 1024, kUmmaSw128);
-                        umma_tf32_ss(d, a_hi, b_hi, kIdesc, k == 0 ? 0u : 1u);
-                        umma_tf32_ss(d, a_hi, b_lo, kIdesc, 1u);
-                        umma_tf32_ss(d, a_lo, b_hi, kIdesc, 1u);
-                    }
-                    umma_commit(&sm.d_full[g]);
-                }
-            }
-            group_sync(g);
-            item = next;
-            next = sm.item[g];
-            base = nbase;
-            n = nn;
         }
-        if ((flags & kFbDiag) && g == 0 && t == 0) {
-            atomicAdd(&fbtc_diag[0], (unsigned long long)(clock64() - c_start));
-            atomicAdd(&fbtc_diag[1], (unsigned long long)c_wait);
-            atomicAdd(&fbtc_diag[2], (unsigned long long)use);
-        }
-        // no more work for this group: tell the epilogue once the last accumulator has been read
-        mbar_wait_sleep(&sm.d_empty[g], (use & 1u) ^ 1u, 32);
-        if (t == 0) {
-            sm.cnt[g] = -1;
-            __threadfence_block();
-            mbar_arrive(&sm.d_full[g]);
-        }
-    } else if (warp >= kFbEpi0) {
-        // ==================================================================== epilogue warps
-        const int ew = warp - kFbEpi0;
-        uint32_t use[kFbGroups] = {0, 0}, alive = (1u << kFbGroups) - 1;
-        int g = 0;
-        long long c_wait = 0, c_red = 0;
-        const long long c_start = clock64();
-        while (alive) {
-            if (!((alive >> g) & 1u)) { g ^= 1; continue; }
-            const long long c0 = clock64();
-            mbar_wait_sleep(&sm.d_full[g], use[g] & 1u, 32);
-            const long long c1 = clock64();
-            c_wait += c1 - c0;
-            tc_fence_after();
-            const int cnt = *reinterpret_cast<volatile int32_t*>(&sm.cnt[g]);
-            if (cnt < 0) {
-                alive &= ~(1u << g);
-                use[g]++;
-                g ^= 1;
-                continue;
+        uint2 m_cur = (lane < kListChunk && (uint32_t)lane < n) ? __ldg(&a.list_meta[base + lane]) : make_uint2(0u, 0u);
+        for (uint32_t c = 0; c < nch; c++) {
+            const int buf = c & 1;
+            const uint32_t e_nxt = (c + 1) * kListChunk + lane;
+            const uint2 m_nxt = (lane < kListChunk && e_nxt < n) ? __ldg(&a.list_meta[base + e_nxt]) : make_uint2(0u, 0u);
+            if (c + 1 < nch) {
+                issue(c + 1, buf ^ 1);
+                cp_async_wait<1>();
+            } else {
+                cp_async_wait<0>();
             }
-            const int ch0 = *reinterpret_cast<volatile int32_t*>(&sm.ch0[g]);
-            const int rows = min(32, cnt - 32 * ew);  // this warp's quarter of the accumulator: entries 32 ew .. 32 ew + 31
-            if (rows > 0) {
-#pragma unroll 1
-                for (int j = 0; j < 4; j++) {
-                    uint32_t r[32];
-                    tmem_ld_x32(tmem + ((uint32_t)(32 * ew) << 16) + (uint32_t)(g * 128 + j * 32), r);
-                    tmem_ld_wait();
-#pragma unroll
-                    for (int q = 0; q < 8; q++)
-                        *reinterpret_cast<float4*>(&sm.tr[ew][lane][j * 32 + q * 4]) =
-                            make_float4(__uint_as_float(r[4 * q]), __uint_as_float(r[4 * q + 1]), __uint_as_float(r[4 * q + 2]),
-                                        __uint_as_float(r[4 * q + 3]));
-                }
-                sm.tr_gid[ew][lane] = lane < rows ? sm.gid[g][32 * ew + lane] : 0u;
-                if (lane == 0) {
-                    sm.tr_rows[ew] = rows;
-                    sm.tr_ch0[ew] = ch0;
-                }
-            }
-            tc_fence_before();
             __syncwarp();
-            if (lane == 0) mbar_arrive(&sm.d_empty[g]);  // accumulator and ids are out: the slot can be refilled
-            if (rows > 0) {
-                if (helpers) {
-                    pair_sync(ew);  // rows are in shared memory
-                    fb_reduce_rows(sm, ew, lane, 0, 2, rows, ch0, a);
-                    __syncwarp();
-                    pair_sync(ew);  // both halves are out: tr[ew] can be overwritten
-                } else {
-                    fb_reduce_rows(sm, ew, lane, 0, 1, rows, ch0, a);
-                    __syncwarp();
+            const uint32_t cnt = min((uint32_t)kListChunk, n - c * kListChunk);
+            const bool v0 = (uint32_t)g < cnt, v1 = (uint32_t)(g + 8) < cnt;  // rows past the chunk's end enter as zeros
+            float d[NT][4];
+#pragma unroll
+            for (int ni = 0; ni < NT; ni++)
+#pragma unroll
+                for (int e = 0; e < 4; e++) d[ni][e] = 0.f;
+#pragma unroll
+            for (int k0 = 0; k0 < 32; k0 += 8) {
+                const float av[4] = {v0 ? sm.w[buf][g][k0 + t] : 0.f, v1 ? sm.w[buf][g + 8][k0 + t] : 0.f,
+                                     v0 ? sm.w[buf][g][k0 + t + 4] : 0.f, v1 ? sm.w[buf][g + 8][k0 + t + 4] : 0.f};
+                uint32_t ah[4], al[4];
+#pragma unroll
+                for (int r = 0; r < 4; r++) {
+                    const float hi = tf32_hi(av[r]);
+                    ah[r] = __float_as_uint(hi);
+                    al[r] = __float_as_uint(av[r] - hi);
+                }
+#pragma unroll
+                for (int ni = 0; ni < NT; ni++) {
+                    const float bv[2] = {sm.dO[8 * ni + g][k0 + t], sm.dO[8 * ni + g][k0 + t + 4]};
+                    uint32_t bh[2], bl[2];
+#pragma unroll
+                    for (int r = 0; r < 2; r++) {
+                        const float hi = tf32_hi(bv[r]);
+                        bh[r] = __float_as_uint(hi);
+                        bl[r] = __float_as_uint(bv[r] - hi);
+                    }
+                    mma_tf32_16x8x8(d[ni], ah, bh);
+                    mma_tf32_16x8x8(d[ni], ah, bl);
+                    mma_tf32_16x8x8(d[ni], al, bh);
                 }
             }
-            c_red += clock64() - c1;
-            use[g]++;
-            g ^= 1;
-        }
-        if ((flags & kFbDiag) && ew == 0 && lane == 0) {
-            atomicAdd(&fbtc_diag[3], (unsigned long long)(clock64() - c_start));
-            atomicAdd(&fbtc_diag[4], (unsigned long long)c_wait);
-            atomicAdd(&fbtc_diag[5], (unsigned long long)c_red);
-        }
-        if (helpers) {
-            if (lane == 0) sm.tr_rows[ew] = -1;
+            // rows g, g + 8 = entries; columns 2t, 2t + 1 of n-tile ni = channels 8 ni + 2t (+ 1) of the chunk
+            const uint32_t gid0 = __shfl_sync(0xffffffffu, m_cur.x, g), gid1 = __shfl_sync(0xffffffffu, m_cur.x, g + 8);
+#pragma unroll
+            for (int h = 0; h < 2; h++) {
+                if (!(h ? v1 : v0)) continue;
+                float* row = a.dL_dfeature + (size_t)(h ? gid1 : gid0) * C + chunk0;
+#pragma unroll
+                for (int ni = 0; ni < NT; ni++) {
+                    const int ch = 8 * ni + 2 * t;
+                    if (chunk0 + ch + 1 < C) {
+                        red_add_f2(row + ch, d[ni][2 * h], d[ni][2 * h + 1]);
+                    } else if (chunk0 + ch < C) {
+                        red_add_f1(row + ch, d[ni][2 * h]);
+                    }
+                }
+            }
             __syncwarp();
-            pair_sync(ew);
+            m_cur = m_nxt;
         }
-    } else if (helpers) {
-        // ==================================================================== helper warps
-        const int ew = warp - kFbHelp0;
-        for (;;) {
-            pair_sync(ew);
-            const int rows = *reinterpret_cast<volatile int32_t*>(&sm.tr_rows[ew]);
-            if (rows < 0) break;
-            const int ch0 = *reinterpret_cast<volatile int32_t*>(&sm.tr_ch0[ew]);
-            fb_reduce_rows(sm, ew, lane, 1, 2, rows, ch0, a);
-            __syncwarp();
-            pair_sync(ew);
-        }
-    }
-
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 0) {
-        tc_fence_after();
-        tmem_dealloc<256>(tmem);
     }
 }
-
-}  // namespace
 
 // ------------------------------------------------------------------------------------------------ launchers
 static int workers_grid() {
     static std::atomic<int> sms_of_device[64];  // zero-initialised; set once per device (idempotent)
     int dev = 0;
     cudaGetDevice(&dev);
-    if (dev < 0 || dev >= 64) return 148 * 3;
+    if (dev < 0 || dev >= 64) return 132 * 3;
     if (sms_of_device[dev].load() == 0) {
         int n = 0;
         cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-        sms_of_device[dev].store(n > 0 ? n : 148);
+        sms_of_device[dev].store(n > 0 ? n : 132);
     }
     return sms_of_device[dev].load() * 3;  // __launch_bounds__(128, 3): three CTAs of four workers per SM
 }
@@ -588,6 +359,18 @@ static cudaError_t launch_feat_bwd_t(const FeatArgs& a, cudaStream_t s) {
     const int items = a.num_tiles * a.chunks * kBlocksPerTile;
     const int grid = min((items + kFeatWarps - 1) / kFeatWarps, workers_grid());
     feature_bwd_kernel<CH><<<grid, kFeatWarps * 32, smem, s>>>(a);
+    g_launches++;
+    return cudaGetLastError();
+}
+
+template <int CH>
+static cudaError_t launch_feat_bwd_tc_t(const FeatArgs& a, cudaStream_t s) {
+    const size_t smem = kFeatWarps * sizeof(FeatSmemTc<CH>);
+    cudaError_t e = cudaFuncSetAttribute(feature_bwd_tc_kernel<CH>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e != cudaSuccess) return e;
+    const int items = a.num_tiles * a.chunks * kBlocksPerTile;
+    const int grid = min((items + kFeatWarps - 1) / kFeatWarps, workers_grid());
+    feature_bwd_tc_kernel<CH><<<grid, kFeatWarps * 32, smem, s>>>(a);
     g_launches++;
     return cudaGetLastError();
 }
@@ -609,45 +392,7 @@ cudaError_t launch_feature_bwd(const ViewParams& vp, const uint2* ranges, const 
     if (vp.W % 4 == 0 && (reinterpret_cast<uintptr_t>(dL_dfeat_pix) & 15) == 0) a.vec |= 2;
     cudaError_t e = cudaMemsetAsync(work_counter, 0, sizeof(int), s);
     if (e != cudaSuccess) return e;
-    if (use_tc && (a.vec & 1)) {
-        a.chunks = (vp.C + 127) / 128;
-        const size_t smem = sizeof(FbSmem) + 1024;
-        static std::atomic<int> sms_of_device[64];
-        int dev = 0;
-        cudaGetDevice(&dev);
-        if (dev < 0 || dev >= 64) return cudaErrorInvalidDevice;
-        if (sms_of_device[dev].load() == 0) {
-            e = cudaFuncSetAttribute(feature_bwd_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-            if (e != cudaSuccess) return e;
-            int n = 0;
-            cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-            sms_of_device[dev].store(n > 0 ? n : 148);
-        }
-        const int items = a.num_tiles * a.chunks * kBlocksPerTile;
-        static const int flags = [] {
-            auto on = [](const char* name, int dflt) {
-                const char* e = getenv(name);
-                return (e ? atoi(e) : dflt) != 0;
-            };
-            return (on("F3DGS_FBTC_HELPERS", 1) ? kFbHelpers : 0) | (on("F3DGS_FBTC_DIAG", 0) ? kFbDiag : 0) |
-                   (on("F3DGS_FBTC_PREFETCH", 1) ? kFbPrefetch : 0);
-        }();
-        const int grid = min(items, sms_of_device[dev].load());
-        feature_bwd_tc_kernel<<<grid, kFbThreads, smem, s>>>(a, flags);
-        g_launches++;
-        e = cudaGetLastError();
-        if (e == cudaSuccess && (flags & kFbDiag)) {  // development: per-CTA mean cycles of the roles, once per launch
-            unsigned long long d[8] = {0};
-            const unsigned long long zero[8] = {0};
-            cudaStreamSynchronize(s);
-            cudaMemcpyFromSymbol(d, fbtc_diag, sizeof(d));
-            cudaMemcpyToSymbol(fbtc_diag, zero, sizeof(zero));
-            fprintf(stderr, "fbtc_diag: loader0 loop %.0f wait_slot %.0f handovers %.1f | epi0 loop %.0f wait_acc %.0f drain %.0f (cycles per CTA, %d CTAs)\n",
-                    (double)d[0] / grid, (double)d[1] / grid, (double)d[2] / grid, (double)d[3] / grid, (double)d[4] / grid,
-                    (double)d[5] / grid, grid);
-        }
-        return e;
-    }
+    if (use_tc && CH >= 64 && (a.vec & 1)) return CH == 64 ? launch_feat_bwd_tc_t<64>(a, s) : launch_feat_bwd_tc_t<128>(a, s);
     if (CH == 32) return launch_feat_bwd_t<32>(a, s);
     if (CH == 64) return launch_feat_bwd_t<64>(a, s);
     return launch_feat_bwd_t<128>(a, s);

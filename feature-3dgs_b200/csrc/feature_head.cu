@@ -264,7 +264,7 @@ cudaError_t launch_feature_resize_fwd(int C, int H, int W, int Hg, int Wg, const
                                       float grad_scale, float* out, float* loss_sum, cudaStream_t s) {
     const size_t n = (size_t)C * Hg * Wg;
     if (n == 0) return cudaSuccess;
-    int dev = 0, sms = 148;
+    int dev = 0, sms = 132;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     const size_t rows = (size_t)C * Hg;

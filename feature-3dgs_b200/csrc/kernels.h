@@ -52,7 +52,7 @@ cudaError_t launch_composite_fwd(const ViewParams& vp, const uint2* ranges, cons
                                  float* final_T, uint32_t* n_contrib, float* out_color,
                                  float* out_feature, float* out_depth, int* work_counter, cudaStream_t s);
 
-// composite_fwd_tc.cu: the same contract with the feature contraction on the tensor cores (tcgen05, 3xTF32);
+// the same contract with the feature contraction on the tensor cores (composite_fwd.cu, mma.sync 3xTF32);
 // needs C % 4 == 0 and a 16-byte aligned feature matrix
 cudaError_t launch_composite_fwd_tc(const ViewParams& vp, const uint2* ranges, const uint32_t* point_list,
                                     const SplatRec* rec, const float* features, const float* bg,

@@ -1,24 +1,13 @@
-// tcgen05 / tensor-memory helpers of the tensor-core composite kernels (composite_fwd_tc.cu, composite_bwd_tc.cu).
+// Tensor-core helpers of the forward composite's feature contraction (composite_fwd.cu, TC feature warps).
 //
-// The feature contraction of a tile,  out[ch, px] = sum_k f[k, ch] * w[k, px]  (forward) and
-// dF[k, ch] = sum_px w[k, px] * dO[ch, px]  (backward), is a dense GEMM per tile once the blend weights of the pairs that
-// did not blend are written as zeros.  It runs on the 5th-generation tensor cores as an ERROR-COMPENSATED TF32 product:
-// every fp32 operand x is split into hi = x with the 13 low mantissa bits cleared (exactly a TF32 number) and
-// lo = x - hi (exact in fp32, <= 13 significant bits), and
-//      a * b  ~=  a_hi * b_hi + a_hi * b_lo + a_lo * b_hi                    (three kind::tf32 MMAs, fp32 accumulate in TMEM)
+// The feature contraction of a pixel block,  out[ch, px] = sum_k f[k, ch] * w[k, px]  over the block's instances, is a
+// dense GEMM once the blend weights of the pairs that did not blend are written as zeros.  It runs on the tensor cores
+// (warp-level mma.sync m16n8k8, TF32 inputs, fp32 accumulate) as an ERROR-COMPENSATED TF32 product: every fp32 operand
+// x is split into hi = x with the 13 low mantissa bits cleared (exactly a TF32 number) and lo = x - hi (exact in fp32),
+// and
+//      a * b  ~=  a_hi * b_hi + a_hi * b_lo + a_lo * b_hi                    (three TF32 MMAs, fp32 accumulate)
 // The dropped a_lo * b_lo term and the truncation of the lo parts to TF32 are each <= 2^-21 |a b|; the three products
 // themselves are exact in fp32 (11 x 11 significant bits).  That is ~200x inside the 1e-4 relative parity bound.
-//
-// Shared-memory operand layouts, region[block of 32 elements][row][32 floats] with 128-byte rows:
-//   K-major operand (a row is one m / n, the 32 floats run along K): SWIZZLE_128B, atoms of 8 rows, physical 16-byte
-//       chunk = logical chunk ^ (row & 7); SBO = 1024 (next 8 rows), LBO unused; a K = 8 step is 32 bytes inside the row.
-//   MN-major operand (a row is one k, the 32 floats run along M / N): for 32-bit types the only legal swizzle is
-//       SWIZZLE_128B_BASE32B, atoms of 4 rows, physical 32-byte chunk = logical chunk ^ (row & 3); LBO = next block of 32
-//       along M / N, SBO = 512 (next 4 k); a K = 8 step is two atoms = 1024 bytes.
-// Descriptor fields as in the PTX ISA "matrix descriptor" / CUTLASS cute/arch/mma_sm100_desc.hpp: start address, LBO, SBO
-// in 16-byte units, version 1, layout type 2 (SWIZZLE_128B) or 1 (SWIZZLE_128B_BASE32B).
-// tools/micro/tc_probe.cu checks exactly these layouts and encodings against a float64 product on the GPU
-// (profiles/r02_tc_probe.txt: 7.8e-7 / 9.3e-7 of sum|terms| for the compensated product, 2e-4 for a single TF32 MMA).
 #pragma once
 #include <stdint.h>
 
@@ -26,95 +15,18 @@
 
 namespace f3dgs {
 
-constexpr uint32_t kUmmaSw128 = 2, kUmmaSw128Base32 = 1;
-__device__ __forceinline__ uint64_t umma_desc(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes,
-                                              uint32_t layout_type) {
-    uint64_t d = 0;
-    d |= (uint64_t)((smem_addr >> 4) & 0x3FFF);
-    d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;
-    d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;
-    d |= (uint64_t)1 << 46;  // descriptor version: Blackwell
-    d |= (uint64_t)layout_type << 61;
-    return d;
-}
-// instruction descriptor: D = f32, A = B = tf32, dense, no negate
-constexpr uint32_t umma_idesc_tf32(int M, int N, int a_mn_major, int b_mn_major) {
-    return (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)a_mn_major << 15) | ((uint32_t)b_mn_major << 16) |
-           ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
-// D[tmem] (+)= A[smem] * B[smem]
-__device__ __forceinline__ void umma_tf32_ss(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                             uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}" ::"r"(d_tmem),
-        "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-// D[tmem] (+)= A[tmem] * B[smem]   (A: lane = row, 32-bit column = k)
-__device__ __forceinline__ void umma_tf32_ts(uint32_t d_tmem, uint32_t a_tmem, uint64_t bdesc, uint32_t idesc,
-                                             uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::tf32 [%0], [%1], %2, %3, p;\n\t}" ::"r"(d_tmem),
-        "r"(a_tmem), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-// all tcgen05 operations issued so far by this thread arrive on `bar` when they have completed
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-                 : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-// generic-proxy shared-memory stores -> visible to the async proxy (tensor-core operand reads)
-__device__ __forceinline__ void fence_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-
-template <int COLS>
-__device__ __forceinline__ void tmem_alloc(uint32_t* slot_in_smem) {  // one full warp; COLS a power of two >= 32
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(slot_in_smem)),
-                 "n"(COLS)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-template <int COLS>
-__device__ __forceinline__ void tmem_dealloc(uint32_t tmem_base) {  // the allocating warp
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "n"(COLS) : "memory");
-}
-// 32 lanes x 32 consecutive 32-bit columns: thread t of the warp gets lane (32*(warp%4) + t)
-__device__ __forceinline__ void tmem_ld_x32(uint32_t taddr, uint32_t (&r)[32]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,"
-        "%30,%31}, [%32];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-          "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-          "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-          "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-        : "r"(taddr));
-}
-__device__ __forceinline__ void tmem_ld_x16(uint32_t taddr, uint32_t (&r)[16]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-          "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-        : "r"(taddr));
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void tmem_st_x8(uint32_t taddr, const uint32_t (&r)[8]) {
-    asm volatile("tcgen05.st.sync.aligned.32x32b.x8.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};" ::"r"(taddr), "r"(r[0]),
-                 "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7])
-                 : "memory");
-}
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-
 // hi / lo split of an fp32 value for the compensated TF32 product
 __device__ __forceinline__ float tf32_hi(float x) { return __uint_as_float(__float_as_uint(x) & 0xFFFFE000u); }
 
-// float index of element c (0..31) of row r inside a [rows][32 floats] region (1024-byte aligned)
-//   K-major, SWIZZLE_128B:             16-byte chunks ^ (r & 7)
-//   MN-major, SWIZZLE_128B_BASE32B:    32-byte chunks ^ (r & 3)
-__device__ __forceinline__ int sw128_idx(int r, int c) { return r * 32 + ((((c >> 2) ^ (r & 7)) << 2) | (c & 3)); }
-__device__ __forceinline__ int sw32b_idx(int r, int c) { return r * 32 + ((((c >> 3) ^ (r & 3)) << 3) | (c & 7)); }
+// d (+)= a * b, m16n8k8, A row-major 16x8 (4 regs), B column-major 8x8 (2 regs), D 16x8 fp32 (4 regs).  Fragments
+// (PTX ISA, mma.m16n8k8 .tf32), g = lane >> 2, t = lane & 3:
+//   a0 (g, t)  a1 (g + 8, t)  a2 (g, t + 4)  a3 (g + 8, t + 4)      b0 (k = t, n = g)  b1 (k = t + 4, n = g)
+//   d0 (g, 2t) d1 (g, 2t + 1) d2 (g + 8, 2t) d3 (g + 8, 2t + 1)
+__device__ __forceinline__ void mma_tf32_16x8x8(float (&d)[4], const uint32_t (&a)[4], const uint32_t (&b)[2]) {
+    asm volatile(
+        "mma.sync.aligned.m16n8k8.row.col.f32.tf32.tf32.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b[0]), "r"(b[1]));
+}
 
 }  // namespace f3dgs

@@ -1,4 +1,4 @@
-"""Drop-in `diff_gaussian_rasterization` on the B200-native rasterizer (libf3dgs_b200.so).
+"""Drop-in `diff_gaussian_rasterization` on the H100-native rasterizer (libf3dgs_b200.so).
 
 Public surface = the reference extension's
 (submodules/diff-gaussian-rasterization-feature/diff_gaussian_rasterization/__init__.py):
@@ -32,7 +32,7 @@ try:
 except ImportError as exc:  # pragma: no cover - exercised only on a broken install
     raise ImportError(
         "diff_gaussian_rasterization._C (f3dgs_b200) is not built. Run "
-        "`python feature-3dgs_b200/build.py` (needs nvcc, targets sm_100a). "
+        "`python feature-3dgs_b200/build.py` (needs nvcc, targets sm_90a). "
         "There is no CPU fallback. Original error: %s" % (exc,)
     ) from exc
 

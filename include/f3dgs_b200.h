@@ -1,5 +1,5 @@
 /*
- * f3dgs_b200 -- C ABI of the B200-native feature-Gaussian rasterizer (libf3dgs_b200.so).
+ * f3dgs_b200 -- C ABI of the H100-native feature-Gaussian rasterizer (libf3dgs_b200.so).
  *
  * This is the drop-in boundary below the Python/torch surface.  Every entry point takes plain
  * device pointers and sizes -- no torch, no C++ types -- and replaces one member of the

@@ -1,4 +1,4 @@
-"""oracle -- CPU checker for the B200 rasterizer.  TEST INFRASTRUCTURE ONLY.
+"""oracle -- CPU checker for the H100 rasterizer.  TEST INFRASTRUCTURE ONLY.
 
 Only tests/, __graft_entry__.smoke() and bench.py's cpu_baseline / --impl reference legs import
 this package; the product (feature-3dgs_b200/) never does.
@@ -11,7 +11,7 @@ this package; the product (feature-3dgs_b200/) never does.
 Backed by oracle/f3dgs_oracle.c (plain C restatement of the reference CUDA algorithm, each
 function citing the reference file:line), compiled on first use into oracle/libf3dgs_oracle.so.
 Parity pin: tests/golden/*.npz were produced by the UNMODIFIED reference extension (oracle/_ref)
-on a B200 via oracle/make_golden.py; tests/test_oracle_golden.py checks this restatement against
+via oracle/make_golden.py; tests/test_oracle_golden.py checks this restatement against
 them.
 """
 import ctypes

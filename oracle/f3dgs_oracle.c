@@ -6,13 +6,13 @@
  *
  * The reference has no CPU implementation (SURVEY.md section 0); this is a plain-C restatement of its
  * CUDA algorithm, function by function, each citing the reference file:line it follows
- * (DGR = /root/reference/submodules/diff-gaussian-rasterization-feature).  Pinning: the reference
+ * (DGR = <reference checkout>/submodules/diff-gaussian-rasterization-feature).  Pinning: the reference
  * ships no golden vectors, so the oracle is pinned against outputs of the reference extension
  * itself (oracle/_ref, built from the unmodified sources by oracle/build_ref.py and run on the
- * B200 by oracle/make_golden.py); the vectors are committed under tests/golden/.
+ * GPU by oracle/make_golden.py); the vectors are committed under tests/golden/.
  *
  * Numerics: the forward per-Gaussian stage reproduces the exact fp32 operation sequence of the
- * reference's sm_100a build (FMA placement read off its PTX *and* SASS -- ptxas fuses further
+ * reference's build (FMA placement read off its PTX *and* SASS -- ptxas fuses further
  * mul/add pairs the PTX still shows separately; fmaf() here, -ffp-contract=off), so radii / tile
  * rectangles / depth keys / point_list / ranges are bit-identical to the GPU.
  * expf() comes from libm and differs from CUDA's by <= 2 ulp, so images agree to ~1e-6 and

@@ -2,8 +2,7 @@
 """Generate the golden vectors under tests/golden/ by running the UNMODIFIED reference CUDA extension
 (oracle/_ref, see oracle/build_ref.py) on seeded scenegen scenes.  Needs a GPU:
 
-    gpurun -- python oracle/make_golden.py        # writes gpurun_out/golden/<name>.npz
-    cp gpurun_out/golden/*.npz tests/golden/      # then commit
+    python oracle/make_golden.py [OUT_DIR]        # writes OUT_DIR/<name>.npz (default: tests/golden)
 
 Inputs are not stored: tests regenerate them bit-identically from scenegen (numpy PCG64) with the
 recorded (config name, seed).  Stored per case: images, all bit-exact index structures, the
@@ -26,7 +25,7 @@ CASES = [("tiny", 1), ("tiny", 7), ("small", 2)]
 def main():
     import torch
 
-    out_dir = os.path.join(ROOT, "gpurun_out", "golden")
+    out_dir = sys.argv[1] if len(sys.argv) > 1 else os.path.join(ROOT, "tests", "golden")
     os.makedirs(out_dir, exist_ok=True)
     for name, seed in CASES:
         sc = scenegen.make_config(name, seed=seed)

@@ -1,7 +1,7 @@
-"""Loader + autograd wrapper for oracle/_ref: the UNMODIFIED reference CUDA rasterizer (sm_100a build).
+"""Loader + autograd wrapper for oracle/_ref: the UNMODIFIED reference CUDA rasterizer (sm_90a build).
 
 TEST / BENCH INFRASTRUCTURE ONLY (needs a GPU; the modules are built in the CPU container by
-oracle/build_ref.py and travel to the B200 box with gpurun).
+oracle/build_ref.py and are loaded on the GPU machine).
 
 The reference fixes the feature width at compile time, so `load(C)` picks the module built for
 that width (C = 0 is served by the C = 1 build with an all-zero feature column: colour, depth and

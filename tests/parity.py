@@ -152,6 +152,14 @@ def run_oracle(scene, cam, grads=None, threads=None, **kw):
     return out
 
 
+def golden_pair(g, key, ours):
+    """(ours, stored) for array `key` of a golden file.  Large arrays are stored as every n-th element of the flattened
+    array (`<key>_stride` = n, keeping the files small); `ours` is sampled the same way."""
+    if key + "_stride" in g.files:
+        return np.asarray(ours).reshape(-1)[:: int(g[key + "_stride"])], g[key]
+    return ours, g[key]
+
+
 def float_mismatch(a, b, rtol=RTOL, atol_rel=ATOL_REL):
     """-> (max violation ratio, max abs err, scale).  ratio <= 1 means within tolerance."""
     a = np.asarray(a, np.float64)

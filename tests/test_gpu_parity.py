@@ -1,12 +1,11 @@
 """GPU parity tests proper (-m gpu): this repo's CUDA path, called through the public Python API -> torch
 binding -> C ABI, against
-  * the UNMODIFIED reference CUDA extension (oracle/_ref, where a build for that feature width travels), and
+  * the UNMODIFIED reference CUDA extension (oracle/_ref, where a build for that feature width exists), and
   * the CPU oracle (oracle/) for every case small enough,
 on identical seeded inputs.  Bars (BASELINE.json north_star): bit-exact tile/key indexing (radii,
 num_rendered, point_list, ranges, n_contrib); RGB/feature/depth/gradients within 1e-4 relative
 (parity.RTOL + ATOL_REL floor).  On top of the bar, colour / depth / final_T are asserted BIT-identical to
 the reference build (same fp32 operation sequence), the feature map to 5e-6 of its scale.
-Nothing here reads /root/reference.
 """
 import copy
 
@@ -62,11 +61,11 @@ def test_small_configs_vs_reference_and_oracle(name):
 
 def test_c2_vs_reference():
     sc = scenegen.make_config("c2")
-    _check(sc, sc.cameras[0], vs_oracle=False)
+    _check(sc, sc.cameras[0])
 
 
 def test_golden_fixtures_match_gpu():
-    """The committed golden vectors (reference outputs from an earlier B200 run) against today's GPU result."""
+    """The committed golden vectors (outputs of the unmodified reference extension) against today's GPU result."""
     import glob
     import os
 
@@ -79,9 +78,9 @@ def test_golden_fixtures_match_gpu():
             assert np.array_equal(np.asarray(ours[k]).astype(np.int64), g[k].astype(np.int64)), (path, k)
         for k in ("color", "depth", "final_T"):
             assert np.array_equal(ours[k], g[k]), (path, k)
-        assert parity.float_mismatch(ours["feature_map"], g["feature_map"])[0] <= 1.0
+        assert parity.float_mismatch(*parity.golden_pair(g, "feature_map", ours["feature_map"]))[0] <= 1.0
         for k in ("means3D", "means2D", "sh", "semantic_feature", "opacities", "scales", "rotations"):
-            assert parity.float_mismatch(ours["grads"][k], g["grad_" + k])[0] <= 1.0, (path, k)
+            assert parity.float_mismatch(*parity.golden_pair(g, "grad_" + k, ours["grads"][k]))[0] <= 1.0, (path, k)
 
 
 # ------------------------------------------------------------------------------------------- feature widths
@@ -300,43 +299,87 @@ def c3_scene():
 
 
 def _full_size_vs_reference(sc, with_grads, label):
-    """Device-side comparison of one full-size view against the reference build; prints the worst violation ratio
-    (|a-b| / tolerance, <= 1 passes) of every float tensor so the margin is on record in the test log."""
+    """One full-size view, compared on the device; prints the worst violation ratio (|a-b| / tolerance, <= 1 passes) of
+    every float tensor so the margin is on record in the test log.
+
+    Against the unmodified reference build (oracle/_ref, where a reference checkout was there to build it): indices and
+    colour / depth / final_T bit-identical, feature map and gradients within the parity bar.  Without it, against the CPU
+    oracle (oracle/: the reference algorithm restated in C, pinned to the reference's outputs by test_oracle_golden.py)
+    with parity.compare's threshold-tie rule: libm's expf differs from CUDA's by <= 2 ulp, so up to max(2, 1e-4 * pixels)
+    pixels may differ in n_contrib; those are masked out of the images and widen the gradient bar 50x.  Every blend
+    weight then carries those ulps, so the feature map's relative bar applies to the sum of its terms' magnitudes
+    (the oracle's map of |features|) rather than to the possibly cancelled sum."""
+    import os
+
     import torch
     from oracle import ref_wrapper as rw
 
-    if not rw.available(sc.C):
-        pytest.skip(f"no reference build for C={sc.C} on this box")
     cam = sc.cameras[0]
     grads = scenegen.upstream_grads(cam.image_height, cam.image_width, sc.C) if with_grads else None
     ours = parity.run_ours(sc, cam, grads=grads)
-    ref = parity.run_ref(sc, cam, grads=grads)
-    for k in ("radii", "point_list", "ranges", "n_contrib"):
-        assert np.array_equal(ours[k], ref[k]), k
+    vs_ref = rw.available(sc.C)
+    ref = parity.run_ref(sc, cam, grads=grads) if vs_ref else parity.run_oracle(sc, cam, grads=grads,
+                                                                                 threads=os.cpu_count())
+    for k in ("radii", "point_list", "ranges"):
+        assert np.array_equal(np.asarray(ours[k]).astype(np.int64), np.asarray(ref[k]).astype(np.int64)), k
     assert int(ours["num_rendered"]) == int(ref["num_rendered"])
-    for k in ("color", "depth", "final_T"):
-        assert np.array_equal(ours[k], ref[k]), k
+    ties = np.asarray(ours["n_contrib"]).astype(np.int64) != np.asarray(ref["n_contrib"]).astype(np.int64)
+    n_ties = int(ties.sum())
+    if vs_ref:
+        assert n_ties == 0
+        for k in ("color", "depth", "final_T"):
+            assert np.array_equal(ours[k], ref[k]), k
+    else:
+        assert n_ties <= max(2, int(1e-4 * ties.size)), n_ties
+    keep = torch.from_numpy(~ties).cuda()
+    extra = []  # image pixels outside the bar with n_contrib unchanged (oracle only)
 
-    def viol(a, b, atol):
-        a, b = torch.from_numpy(a).cuda().double(), torch.from_numpy(b).cuda().double()
-        tol = parity.RTOL * b.abs() + atol * b.abs().max()
-        return float(((a - b).abs() / tol).max())
+    def viol(a, b, atol, widen=1.0, mask=None, mag=None):
+        a = torch.from_numpy(np.ascontiguousarray(a)).cuda().double()
+        b = torch.from_numpy(np.ascontiguousarray(b)).cuda().double()
+        if mask is not None:
+            a = torch.where(mask, a, b)
+        m = b.abs() if mag is None else torch.from_numpy(np.ascontiguousarray(mag)).cuda().double()
+        tol = widen * (parity.RTOL * m + atol * b.abs().max())
+        r = (a - b).abs() / tol
+        if not vs_ref and r.dim() >= 2 and r.shape[-2:] == keep.shape:
+            # a blend flipped at the threshold before the pixel's last contributor leaves n_contrib unchanged: such
+            # pixels count against the same tie budget and must stay within the 50x bar of a tie
+            px = r.reshape(-1, *r.shape[-2:]).amax(0)
+            extra.append(px > 1.0)
+            assert float(px.max()) <= 50.0, float(px.max())
+            r = torch.where(px > 1.0, 0.0, px)
+        return float(r.max())
 
     worst = {}
+    if not vs_ref:
+        for k in ("color", "depth", "final_T"):
+            worst[k] = viol(ours[k], ref[k], parity.ATOL_REL, mask=keep)
     if sc.C:
-        worst["feature_map"] = viol(ours["feature_map"], ref["feature_map"], parity.ATOL_REL)
+        mag = None
+        if not vs_ref:
+            sc_abs = copy.copy(sc)
+            sc_abs.features = np.abs(sc.features)
+            mag = parity.run_oracle(sc_abs, cam, threads=os.cpu_count())["feature_map"]
+        worst["feature_map"] = viol(ours["feature_map"], ref["feature_map"], parity.ATOL_REL, mask=keep, mag=mag)
     if with_grads:
         for k in ("means3D", "means2D", "sh", "semantic_feature", "opacities", "scales", "rotations"):
             if k in ours["grads"]:
-                worst["grad_" + k] = viol(ours["grads"][k], ref["grads"][k], parity.GRAD_ATOL_REL)
-    print(f"[{label}] V={int((ours['radii'] > 0).sum())} R={int(ours['num_rendered'])} worst viol per tensor: "
+                worst["grad_" + k] = viol(ours["grads"][k], ref["grads"][k], parity.GRAD_ATOL_REL,
+                                          widen=50.0 if n_ties else 1.0)
+    if extra:
+        flipped = torch.stack(extra).any(0) & keep
+        n_ties += int(flipped.sum())
+        assert n_ties <= max(2, int(1e-4 * ties.size)), n_ties
+    print(f"[{label} vs {'reference build' if vs_ref else 'CPU oracle'}] V={int((ours['radii'] > 0).sum())} "
+          f"R={int(ours['num_rendered'])} n_contrib ties={n_ties} worst viol per tensor: "
           + ", ".join(f"{k}={v:.3g}" for k, v in worst.items()))
     for k, v in worst.items():
         assert v <= 1.0, (k, v)
 
 
 def test_c3_full_size_vs_reference(c3_scene):
-    """BASELINE.json's metric configuration itself: 1M Gaussians, 1080p, C=128 (device-side comparison)."""
+    """BASELINE.json's metric configuration itself: 1M Gaussians, 1080p, C=128, forward + backward."""
     _full_size_vs_reference(c3_scene, True, "c3")
 
 
@@ -450,11 +493,11 @@ def test_view_batch_accumulates_like_autograd(name):
 
 # ------------------------------------------------------------------------------------------- per-process overrides
 @pytest.mark.parametrize("env", [{"F3DGS_TC": "0"}, {"F3DGS_BWD2": "0"}, {"F3DGS_TC": "0", "F3DGS_BWD2": "0"},
-                                 {"F3DGS_TC_MIN_C": "16"}, {"F3DGS_FBWD_TC": "1"}])
+                                 {"F3DGS_TC": "1", "F3DGS_TC_MIN_C": "16"}, {"F3DGS_FBWD_TC": "1"}])
 def test_kernel_selection_overrides_keep_parity(env):
     """F3DGS_TC / F3DGS_BWD2 / F3DGS_TC_MIN_C / F3DGS_FBWD_TC are read once per process, so each setting runs in its own
-    interpreter: the fp32-pipe forward, the fused single-kernel backward, the tensor-core path at narrow widths and the
-    opt-in tensor-core feature-gradient kernel must all pass the same parity checks as the defaults."""
+    interpreter: the fp32-pipe forward, the fused single-kernel backward, the tensor-core forward (at every width from 16)
+    and the opt-in tensor-core feature-gradient kernel must all pass the same parity checks as the defaults."""
     import os
     import subprocess
     import sys

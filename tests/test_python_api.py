@@ -5,6 +5,7 @@ only production caller gaussian_renderer/__init__.py (keyword call sites :75-88,
 """
 import ast
 import inspect
+import json
 import os
 
 import pytest
@@ -13,9 +14,9 @@ import torch
 import diff_gaussian_rasterization as dgr
 from diff_gaussian_rasterization import GaussianRasterizationSettings, GaussianRasterizer, rasterize_gaussians
 
-REF_RENDERER = "/root/reference/gaussian_renderer/__init__.py"
-REF_WRAPPER = "/root/reference/submodules/diff-gaussian-rasterization-feature/diff_gaussian_rasterization/__init__.py"
-
+# Keyword call sites of the reference's unmodified renderer and the positional arity of its wrapper's native calls, read
+# from the reference sources (paths and line ranges inside the file).
+REF_API = json.load(open(os.path.join(os.path.dirname(__file__), "golden", "reference_api.json")))
 
 def _settings(**over):
     kw = dict(image_height=32, image_width=32, tanfovx=0.5, tanfovy=0.5, bg=torch.zeros(3), scale_modifier=1.0,
@@ -90,32 +91,21 @@ def test_cpu_deep_copy_tuple():
     assert out[1] == 1.5 and out[2] == "x" and torch.equal(out[0], t) and out[0].data_ptr() != t.data_ptr()
 
 
-@pytest.mark.skipif(not os.path.exists(REF_RENDERER), reason="reference tree not mounted on this box")
 def test_every_reference_call_site_binds_to_our_signatures():
-    """Statically bind each GaussianRasterizationSettings(...)/rasterizer(...) call of the reference's unmodified
-    renderer against our signatures."""
-    tree = ast.parse(open(REF_RENDERER).read())
+    """Bind each GaussianRasterizationSettings(...) / rasterizer(...) call of the reference's unmodified renderer (keywords
+    recorded in golden/reference_api.json) against our signatures."""
     fwd = inspect.signature(GaussianRasterizer.forward)
-    n_settings = n_calls = 0
-    for node in ast.walk(tree):
-        if not isinstance(node, ast.Call):
-            continue
-        name = getattr(node.func, "id", None)
-        kws = {k.arg for k in node.keywords}
-        if name == "GaussianRasterizationSettings":
-            assert kws == set(GaussianRasterizationSettings._fields)
-            n_settings += 1
-        elif name == "rasterizer":
-            fwd.bind(None, **{k: None for k in kws})
-            n_calls += 1
-    assert n_settings >= 2 and n_calls >= 2
+    for site in REF_API["settings_calls"]:
+        assert set(site["keywords"]) == set(GaussianRasterizationSettings._fields), site["lines"]
+    for site in REF_API["rasterizer_calls"]:
+        fwd.bind(None, **{k: None for k in site["keywords"]})
+    assert len(REF_API["settings_calls"]) >= 2 and len(REF_API["rasterizer_calls"]) >= 2
 
 
-@pytest.mark.skipif(not os.path.exists(REF_WRAPPER), reason="reference tree not mounted on this box")
 def test_native_call_arity_matches_reference_wrapper():
-    """The reference wrapper calls _C positionally: count the arguments it passes."""
-    src = open(REF_WRAPPER).read()
-    tree = ast.parse(src)
+    """The reference wrapper calls _C positionally (20 arguments forward, 24 backward): ours must pass the same counts."""
+    tree = ast.parse(open(inspect.getsourcefile(dgr)).read())
     tuples = [n for n in ast.walk(tree) if isinstance(n, ast.Assign) and getattr(n.targets[0], "id", "") == "args"]
     arities = sorted(len(t.value.elts) for t in tuples)
-    assert arities == [20, 24]  # forward, backward
+    want = REF_API["native_call_arities"]
+    assert arities == sorted([want["forward"], want["backward"]])

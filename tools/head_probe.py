@@ -1,5 +1,5 @@
 """Two calls of the fused feature head at the config-3 shape (C = 128, 822x1237 -> 365x549), for an ncu capture:
-    ncu --set full --clock-control none -k regex:resize_ -c 3 -o gpurun_out/r02_head python tools/head_probe.py
+    ncu --set full --clock-control none -k regex:resize_ -c 3 -o r02_head python tools/head_probe.py
 Development tool, not product code."""
 import os
 import sys

@@ -1,6 +1,6 @@
 """ncu `--page raw --csv` export -> profiles/<tag>_ncu.json (per kernel: time, DRAM bytes, issue utilisation, stalls, ...)
 and profiles/traffic.json (DRAM bytes per launch of the composite stages, read by bench.py for roofline.traffic).
-usage: python tools/ncu_to_profiles.py gpurun_out/prof_raw.csv r02_c3"""
+usage: python tools/ncu_to_profiles.py prof_raw.csv r02_c3"""
 import csv
 import json
 import os

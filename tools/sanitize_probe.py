@@ -1,5 +1,5 @@
 """One small forward + backward through the autograd API and one feature-head call, for compute-sanitizer:
-    F3DGS_FBWD_TC=1 compute-sanitizer --tool memcheck python tools/sanitize_probe.py small128
+    compute-sanitizer --tool memcheck python tools/sanitize_probe.py small128
 Development tool, not product code."""
 import os
 import sys

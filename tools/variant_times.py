@@ -131,18 +131,6 @@ def main():
             os.environ["F3DGS_TC"] = "1"  # tensor-core feature contraction (read once per library instance)
         if "+notc" in name:
             os.environ["F3DGS_TC"] = "0"
-        os.environ.pop("F3DGS_FBWD_TC", None)
-        os.environ.pop("F3DGS_FBTC_HELPERS", None)
-        os.environ.pop("F3DGS_FBTC_PREFETCH", None)
-        os.environ.pop("F3DGS_FBTC_DIAG", None)
-        if "+nopf" in name:
-            os.environ["F3DGS_FBTC_PREFETCH"] = "0"
-        if "+diag" in name:
-            os.environ["F3DGS_FBTC_DIAG"] = "1"
-        if "+nohelp" in name:
-            os.environ["F3DGS_FBTC_HELPERS"] = "0"
-        if "+fbtc" in name:
-            os.environ["F3DGS_FBWD_TC"] = "1"  # tensor-core feature-gradient kernel
         os.environ.pop("F3DGS_BWD2", None)
         if "+bwd1" in name:
             os.environ["F3DGS_BWD2"] = "0"  # fused single-kernel backward
