@@ -20,12 +20,9 @@ LIB = os.path.join(PKG, "libf3dgs_b200.so")
 EXT = os.path.join(PKG, "diff_gaussian_rasterization", "_C" + sysconfig.get_config_var("EXT_SUFFIX"))
 CU = ["api.cu", "preprocess.cu", "binning.cu", "composite_fwd.cu", "composite_bwd.cu", "feature_bwd.cu",
       "feature_head.cu", "optimizer.cu"]
-HDRS = ["common.cuh", "kernels.h", "composite_common.cuh", "tc_common.cuh", os.path.join(ROOT, "include", "f3dgs_b200.h")]
+HDRS = ["common.cuh", "kernels.h", "composite_common.cuh", os.path.join(ROOT, "include", "f3dgs_b200.h")]
 NVCC_FLAGS = ["-std=c++17", "-O3", "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo",
               "-Xcompiler", "-fPIC", "-Xptxas", "-v", "--expt-relaxed-constexpr"]
-NVCC_FLAGS += os.environ.get("F3DGS_EXTRA_NVCC_FLAGS", "").split()  # experiments: -DF3DGS_STAGES=6 -DF3DGS_WSLOTS=3 ...
-if os.environ.get("F3DGS_TIMING_BUILD") == "1":  # per-role cycle counters in the composite kernels (debug builds only)
-    NVCC_FLAGS.append("-DF3DGS_TIMING_BUILD=1")
 
 
 def _run(cmd, log=None):
@@ -47,7 +44,7 @@ def _newer(target, deps):
 
 
 def _flags_changed():
-    """Objects are only reusable for the flags they were built with (experiment / timing builds change the code)."""
+    """Objects are only reusable for the flags they were built with."""
     import hashlib
 
     h = hashlib.sha256(" ".join(NVCC_FLAGS).encode()).hexdigest()
@@ -62,9 +59,6 @@ def _flags_changed():
 
 def build_lib(force=False):
     os.makedirs(OBJ, exist_ok=True)
-    if any("F3DGS_DIAG_" in f for f in NVCC_FLAGS):
-        raise RuntimeError("F3DGS_DIAG_* builds produce wrong results on purpose: build them with tools/build_variants.sh "
-                           "into feature-3dgs_b200/variants/, never as the product library")
     force = _flags_changed() or force
     hdrs = [h if os.path.isabs(h) else os.path.join(CSRC, h) for h in HDRS]
     jobs, objs = [], []

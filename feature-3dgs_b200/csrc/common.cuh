@@ -78,17 +78,6 @@ __device__ __forceinline__ void mbar_arrive_expect_tx(uint64_t* bar, uint32_t by
 }
 // try_wait with a suspend-time hint: the warp is parked by the hardware until the phase completes
 // (or the hint expires) instead of spinning and stealing issue slots from the warps it waits for.
-__device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
-    uint32_t ok;
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2, %3;\n\t"
-        "selp.u32 %0, 1, 0, p;\n\t}"
-        : "=r"(ok)
-        : "r"(smem_u32(bar)), "r"(parity), "r"(0x989680u)
-        : "memory");
-    return ok != 0;
-}
 // The whole wait loop is one asm block: written as a C loop the compiler re-materialises the barrier address (S2R
 // SR_CgaCtaId, LEA, ...) inside it, 17 instructions per poll, and waiting warps then take a quarter of the SM's issue
 // slots from the warps they wait for (ncu source counters).  Here a poll is TRYWAIT + NANOSLEEP + BRA.
@@ -105,7 +94,7 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
 }
 // Wait with a real sleep between polls, for roles that are far ahead of / behind their partner (epilogue waiting for a whole
 // tile, producer waiting for a free stage, ...).  The poll loop of mbar_wait costs three issue slots every ~20 cycles per
-// waiting warp: with ten waiting warps per SM that was 43% of all instructions executed by the tensor-core forward kernel
+// waiting warp: with ten waiting warps per SM that was 43% of all instructions executed by a forward composite kernel
 // (ncu source counters), taken from the warps on the critical path.  `ns` bounds the added wake-up latency.
 __device__ __forceinline__ void mbar_wait_sleep(uint64_t* bar, uint32_t parity, uint32_t ns) {
     asm volatile(
@@ -118,18 +107,6 @@ __device__ __forceinline__ void mbar_wait_sleep(uint64_t* bar, uint32_t parity, 
         "F3DGS_SDONE_%=:\n\t}" ::"r"(smem_u32(bar)),
         "r"(parity), "r"(ns)
         : "memory");
-}
-// non-blocking probe of a phase (helper warps that serve several barriers round-robin)
-__device__ __forceinline__ bool mbar_test(uint64_t* bar, uint32_t parity) {
-    uint32_t ok;
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "mbarrier.test_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-        "selp.u32 %0, 1, 0, p;\n\t}"
-        : "=r"(ok)
-        : "r"(smem_u32(bar)), "r"(parity)
-        : "memory");
-    return ok != 0;
 }
 // 1-D TMA bulk copy global -> shared, completion signalled on an mbarrier (SASS: UBLKCP).
 // dst/src 16-byte aligned, bytes a multiple of 16.

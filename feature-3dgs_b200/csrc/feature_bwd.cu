@@ -8,26 +8,21 @@
 //
 // feature_bwd_kernel<CH> (here): every warp is an independent worker that pulls (tile, channel chunk, block) items from an
 // atomic counter, keeps the block's upstream gradient dL/dfeature_map (32 pixels x 4 channels per lane) in registers,
-// streams the block's list through a double-buffered cp.async ring (8 entries per step) and forms
-// dL/df[g] += sum_pixels w * dL/dO with the paired-FMA quad loop of composite_bwd.cu, one red.global.add.v4 per lane and
-// entry.  No inter-warp synchronisation at all; 12 warps per SM.  Channel counts above 128 reuse the same lists for
-// every 128-channel chunk (the alpha evaluation is not repeated per chunk).
+// streams the block's list through a double-buffered cp.async ring (16 entries per step) and forms
+// dL/df[g] += sum_pixels w * dL/dO with paired FMAs (fma2_rn) over the 2x2-pixel quads that blended, one red.global.add.v4
+// per lane and entry.  No inter-warp synchronisation at all; 12 warps per SM.  Channel counts above 128 reuse the same
+// lists for every 128-channel chunk (the alpha evaluation is not repeated per chunk).
 // Reference semantics: backward.cu:565-575 (feature gradient; the feature loss does not feed dL/dalpha, :575 disabled).
 #include <cstdio>
 #include <cstdlib>
 
 #include "composite_common.cuh"
-#include "tc_common.cuh"
 
 namespace f3dgs {
 
-#ifndef F3DGS_LIST_CHUNK
-#define F3DGS_LIST_CHUNK 16
-#endif
-constexpr int kListChunk = F3DGS_LIST_CHUNK;   // list entries staged per pipeline step (<= 32)
+constexpr int kListChunk = 16;  // list entries staged per pipeline step (<= 32)
 constexpr int kFeatWarps = 4;   // independent worker warps per CTA
 
-template <int CH, bool WITH_ROWS>
 struct alignas(128) FeatSmem {  // per warp
     float w[2][kListChunk][32];
 };
@@ -41,7 +36,7 @@ struct FeatArgs {
     float* dL_dfeature;         // backward: [P, C]
     int* work_counter;
     int W, H, C, tiles_x, num_tiles, chunks;
-    int vec;  // bit0: feature / gradient rows are 16-byte aligned and C % 4 == 0; bit1: 128-bit image rows; bit2: 256-bit
+    int vec;  // bit0: gradient rows are 16-byte aligned and C % 4 == 0; bit1: 128-bit image rows
 };
 
 __device__ __forceinline__ void cp_async16(void* dst_smem, const void* src_gmem) {
@@ -75,7 +70,7 @@ template <int CH>
 __global__ void __launch_bounds__(kFeatWarps * 32, 3) feature_bwd_kernel(const FeatArgs a) {
     extern __shared__ __align__(128) unsigned char smem_raw[];
     const int warp = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0), lane = threadIdx.x & 31;
-    FeatSmem<CH, false>& sm = reinterpret_cast<FeatSmem<CH, false>*>(smem_raw)[warp];
+    FeatSmem& sm = reinterpret_cast<FeatSmem*>(smem_raw)[warp];
     constexpr int LPR = CH / 4;
     constexpr int G = 32 / LPR;
     constexpr int NQ = 8 / G;
@@ -113,7 +108,8 @@ __global__ void __launch_bounds__(kFeatWarps * 32, 3) feature_bwd_kernel(const F
         uint2 m_cur = load_meta(0);
         issue(0, 0);
 
-        // upstream gradient of the block's 32 pixels x 4 channels: [quad][pixel pair][channel], pairs as in composite_bwd.cu
+        // upstream gradient of the block's 32 pixels x 4 channels: [quad][pixel pair][channel]: the two pixels of a
+        // quad row share a 64-bit register pair, as do their weights in the LDS.128
         float2 dO2[NQ][2][4];
 #define DOB(q, i, c) (((i) & 1) ? dO2[q][(i) >> 1][c].y : dO2[q][(i) >> 1][c].x)
 #pragma unroll
@@ -213,132 +209,6 @@ __global__ void __launch_bounds__(kFeatWarps * 32, 3) feature_bwd_kernel(const F
     }
 }
 
-// ------------------------------------------------------------------------------------------------ tensor-core variant
-// The same work items and lists, with the per-block contraction on the tensor cores:  D[entry, ch] = sum_px W[entry, px] *
-// dO[ch, px]  is, per staged chunk of 16 list entries, a GEMM with M = 16 entries, N = CH channels, K = 32 pixels: four
-// K = 8 steps of three mma.sync m16n8k8 TF32 products per 8 channels (3xTF32, tc_common.cuh).  A = the list rows as they
-// lie in memory (one row = the 32 weights of an entry, zero where the pixel did not blend); B = the block's upstream
-// gradient, staged once per item in shared memory as [channel][pixel] in the list's pixel order (row stride 36 floats:
-// the fragment loads of a warp hit 32 different banks).  Each lane adds its two channels of an entry with one red.v2.
-constexpr int kDoStride = 36;
-template <int CH>
-struct alignas(128) FeatSmemTc {  // per warp
-    float w[2][kListChunk][32];
-    float dO[CH][kDoStride];
-};
-static_assert(kListChunk == 16, "the tensor-core variant stages one m16 tile of entries per chunk");
-
-__device__ __forceinline__ void red_add_f2(float* p, float a, float b) {
-    asm volatile("red.global.add.v2.f32 [%0], {%1,%2};" ::"l"(p), "f"(a), "f"(b) : "memory");
-}
-
-template <int CH>
-__global__ void __launch_bounds__(kFeatWarps * 32, 2) feature_bwd_tc_kernel(const FeatArgs a) {
-    extern __shared__ __align__(128) unsigned char smem_raw[];
-    const int warp = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0), lane = threadIdx.x & 31;
-    FeatSmemTc<CH>& sm = reinterpret_cast<FeatSmemTc<CH>*>(smem_raw)[warp];
-    constexpr int NT = CH / 8;  // n-tiles of 8 channels
-    const int g = lane >> 2, t = lane & 3;
-    const int W = a.W, H = a.H, C = a.C;
-    const size_t HW = (size_t)H * W;
-
-    const int items = a.num_tiles * a.chunks * kBlocksPerTile;
-    for (;;) {
-        int item = 0;
-        if (lane == 0) item = atomicAdd(a.work_counter, 1);
-        item = __shfl_sync(0xffffffffu, item, 0);
-        if (item >= items) break;
-        const ItemPos ip = decode_item(item, a);
-        const uint32_t rx = __shfl_sync(0xffffffffu, a.ranges[ip.tile].x, 0);
-        const uint32_t ry = __shfl_sync(0xffffffffu, a.ranges[ip.tile].y, 0);
-        const size_t base = 8 * (size_t)rx + (size_t)ip.b * (ry - rx);
-        const uint32_t n = __shfl_sync(0xffffffffu, a.list_cnt[(size_t)ip.tile * kBlocksPerTile + ip.b], 0);
-        if (n == 0) continue;
-        const int chunk0 = ip.chunk * CH;
-        const uint32_t nch = (n + kListChunk - 1) / kListChunk;
-
-        auto issue = [&](uint32_t c, int buf) {
-            const uint32_t cnt = min((uint32_t)kListChunk, n - c * kListChunk);
-            const float* wsrc = a.list_w + (base + (size_t)c * kListChunk) * 32;
-            for (uint32_t j = lane; j < cnt * 8; j += 32) cp_async16(&sm.w[buf][0][0] + j * 4, wsrc + j * 4);
-            cp_async_commit();
-        };
-        issue(0, 0);
-        {   // upstream gradient of the block: lane = pixel (list order, see lane_px / lane_py), one channel per trip
-            const int xx = ip.bx0 + lane_px(lane), yy = ip.by0 + lane_py(lane);
-            const bool in = xx < W && yy < H;
-            for (int c = 0; c < CH; c++) {
-                const int ch = chunk0 + c;
-                sm.dO[c][lane] = (in && ch < C) ? __ldg(a.dL_dfeat_pix + (size_t)ch * HW + (size_t)yy * W + xx) : 0.f;
-            }
-        }
-        uint2 m_cur = (lane < kListChunk && (uint32_t)lane < n) ? __ldg(&a.list_meta[base + lane]) : make_uint2(0u, 0u);
-        for (uint32_t c = 0; c < nch; c++) {
-            const int buf = c & 1;
-            const uint32_t e_nxt = (c + 1) * kListChunk + lane;
-            const uint2 m_nxt = (lane < kListChunk && e_nxt < n) ? __ldg(&a.list_meta[base + e_nxt]) : make_uint2(0u, 0u);
-            if (c + 1 < nch) {
-                issue(c + 1, buf ^ 1);
-                cp_async_wait<1>();
-            } else {
-                cp_async_wait<0>();
-            }
-            __syncwarp();
-            const uint32_t cnt = min((uint32_t)kListChunk, n - c * kListChunk);
-            const bool v0 = (uint32_t)g < cnt, v1 = (uint32_t)(g + 8) < cnt;  // rows past the chunk's end enter as zeros
-            float d[NT][4];
-#pragma unroll
-            for (int ni = 0; ni < NT; ni++)
-#pragma unroll
-                for (int e = 0; e < 4; e++) d[ni][e] = 0.f;
-#pragma unroll
-            for (int k0 = 0; k0 < 32; k0 += 8) {
-                const float av[4] = {v0 ? sm.w[buf][g][k0 + t] : 0.f, v1 ? sm.w[buf][g + 8][k0 + t] : 0.f,
-                                     v0 ? sm.w[buf][g][k0 + t + 4] : 0.f, v1 ? sm.w[buf][g + 8][k0 + t + 4] : 0.f};
-                uint32_t ah[4], al[4];
-#pragma unroll
-                for (int r = 0; r < 4; r++) {
-                    const float hi = tf32_hi(av[r]);
-                    ah[r] = __float_as_uint(hi);
-                    al[r] = __float_as_uint(av[r] - hi);
-                }
-#pragma unroll
-                for (int ni = 0; ni < NT; ni++) {
-                    const float bv[2] = {sm.dO[8 * ni + g][k0 + t], sm.dO[8 * ni + g][k0 + t + 4]};
-                    uint32_t bh[2], bl[2];
-#pragma unroll
-                    for (int r = 0; r < 2; r++) {
-                        const float hi = tf32_hi(bv[r]);
-                        bh[r] = __float_as_uint(hi);
-                        bl[r] = __float_as_uint(bv[r] - hi);
-                    }
-                    mma_tf32_16x8x8(d[ni], ah, bh);
-                    mma_tf32_16x8x8(d[ni], ah, bl);
-                    mma_tf32_16x8x8(d[ni], al, bh);
-                }
-            }
-            // rows g, g + 8 = entries; columns 2t, 2t + 1 of n-tile ni = channels 8 ni + 2t (+ 1) of the chunk
-            const uint32_t gid0 = __shfl_sync(0xffffffffu, m_cur.x, g), gid1 = __shfl_sync(0xffffffffu, m_cur.x, g + 8);
-#pragma unroll
-            for (int h = 0; h < 2; h++) {
-                if (!(h ? v1 : v0)) continue;
-                float* row = a.dL_dfeature + (size_t)(h ? gid1 : gid0) * C + chunk0;
-#pragma unroll
-                for (int ni = 0; ni < NT; ni++) {
-                    const int ch = 8 * ni + 2 * t;
-                    if (chunk0 + ch + 1 < C) {
-                        red_add_f2(row + ch, d[ni][2 * h], d[ni][2 * h + 1]);
-                    } else if (chunk0 + ch < C) {
-                        red_add_f1(row + ch, d[ni][2 * h]);
-                    }
-                }
-            }
-            __syncwarp();
-            m_cur = m_nxt;
-        }
-    }
-}
-
 // ------------------------------------------------------------------------------------------------ launchers
 static int workers_grid() {
     static std::atomic<int> sms_of_device[64];  // zero-initialised; set once per device (idempotent)
@@ -355,22 +225,10 @@ static int workers_grid() {
 
 template <int CH>
 static cudaError_t launch_feat_bwd_t(const FeatArgs& a, cudaStream_t s) {
-    const size_t smem = kFeatWarps * sizeof(FeatSmem<CH, false>);
+    const size_t smem = kFeatWarps * sizeof(FeatSmem);
     const int items = a.num_tiles * a.chunks * kBlocksPerTile;
     const int grid = min((items + kFeatWarps - 1) / kFeatWarps, workers_grid());
     feature_bwd_kernel<CH><<<grid, kFeatWarps * 32, smem, s>>>(a);
-    g_launches++;
-    return cudaGetLastError();
-}
-
-template <int CH>
-static cudaError_t launch_feat_bwd_tc_t(const FeatArgs& a, cudaStream_t s) {
-    const size_t smem = kFeatWarps * sizeof(FeatSmemTc<CH>);
-    cudaError_t e = cudaFuncSetAttribute(feature_bwd_tc_kernel<CH>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return e;
-    const int items = a.num_tiles * a.chunks * kBlocksPerTile;
-    const int grid = min((items + kFeatWarps - 1) / kFeatWarps, workers_grid());
-    feature_bwd_tc_kernel<CH><<<grid, kFeatWarps * 32, smem, s>>>(a);
     g_launches++;
     return cudaGetLastError();
 }
@@ -379,7 +237,7 @@ static int feat_ch(int C) { return C <= 32 ? 32 : (C <= 64 ? 64 : 128); }
 
 cudaError_t launch_feature_bwd(const ViewParams& vp, const uint2* ranges, const float* list_w, const uint2* list_meta,
                                const uint32_t* list_cnt, const float* dL_dfeat_pix, float* dL_dfeature,
-                               int* work_counter, cudaStream_t s, bool use_tc) {
+                               int* work_counter, cudaStream_t s) {
     FeatArgs a;
     a.ranges = ranges; a.list_w = list_w; a.list_meta = list_meta; a.list_cnt = list_cnt;
     a.dL_dfeat_pix = dL_dfeat_pix; a.dL_dfeature = dL_dfeature;
@@ -392,7 +250,6 @@ cudaError_t launch_feature_bwd(const ViewParams& vp, const uint2* ranges, const 
     if (vp.W % 4 == 0 && (reinterpret_cast<uintptr_t>(dL_dfeat_pix) & 15) == 0) a.vec |= 2;
     cudaError_t e = cudaMemsetAsync(work_counter, 0, sizeof(int), s);
     if (e != cudaSuccess) return e;
-    if (use_tc && CH >= 64 && (a.vec & 1)) return CH == 64 ? launch_feat_bwd_tc_t<64>(a, s) : launch_feat_bwd_tc_t<128>(a, s);
     if (CH == 32) return launch_feat_bwd_t<32>(a, s);
     if (CH == 64) return launch_feat_bwd_t<64>(a, s);
     return launch_feat_bwd_t<128>(a, s);

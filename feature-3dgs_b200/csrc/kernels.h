@@ -52,34 +52,19 @@ cudaError_t launch_composite_fwd(const ViewParams& vp, const uint2* ranges, cons
                                  float* final_T, uint32_t* n_contrib, float* out_color,
                                  float* out_feature, float* out_depth, int* work_counter, cudaStream_t s);
 
-// the same contract with the feature contraction on the tensor cores (composite_fwd.cu, mma.sync 3xTF32);
-// needs C % 4 == 0 and a 16-byte aligned feature matrix
-cudaError_t launch_composite_fwd_tc(const ViewParams& vp, const uint2* ranges, const uint32_t* point_list,
-                                    const SplatRec* rec, const float* features, const float* bg,
-                                    float* final_T, uint32_t* n_contrib, float* out_color,
-                                    float* out_feature, float* out_depth, int* work_counter, cudaStream_t s);
-
-// geometric-gradient kernel of the two-kernel backward (composite_bwd.cu): alpha-only, two CTAs per SM; with list pointers it
+// ---- composite_bwd.cu: geometric-gradient kernel of the two-kernel backward, two CTAs per SM; with list pointers it
 // also emits the per-(tile, block) blend weights for launch_feature_bwd
-cudaError_t launch_composite_bwd_geom_slim(const ViewParams& vp, const uint2* ranges, const uint32_t* point_list,
-                                           const SplatRec* rec, const float* bg, const float* final_T,
-                                           const uint32_t* n_contrib, const float* dL_dpix, const float* dL_ddepth,
-                                           float* dL_dmean2D, float* dL_dconic, float* dL_dopacity, float* dL_dcolor,
-                                           float* dL_dz, int* work_counter, cudaStream_t s, float* list_w = nullptr,
-                                           uint2* list_meta = nullptr, uint32_t* list_cnt = nullptr);
+cudaError_t launch_composite_bwd_geom(const ViewParams& vp, const uint2* ranges, const uint32_t* point_list,
+                                      const SplatRec* rec, const float* bg, const float* final_T,
+                                      const uint32_t* n_contrib, const float* dL_dpix, const float* dL_ddepth,
+                                      float* dL_dmean2D, float* dL_dconic, float* dL_dopacity, float* dL_dcolor,
+                                      float* dL_dz, int* work_counter, cudaStream_t s, float* list_w = nullptr,
+                                      uint2* list_meta = nullptr, uint32_t* list_cnt = nullptr);
 
 // ---- feature_bwd.cu: feature gradient from the instance lists (second kernel of the two-kernel backward)
 cudaError_t launch_feature_bwd(const ViewParams& vp, const uint2* ranges, const float* list_w, const uint2* list_meta,
                                const uint32_t* list_cnt, const float* dL_dfeat_pix, float* dL_dfeature,
-                               int* work_counter, cudaStream_t s, bool use_tc = false);
-
-// ---- composite_bwd.cu
-cudaError_t launch_composite_bwd(const ViewParams& vp, const uint2* ranges, const uint32_t* point_list,
-                                 const SplatRec* rec, const float* bg, const float* final_T,
-                                 const uint32_t* n_contrib, const float* dL_dpix, const float* dL_dfeat_pix,
-                                 const float* dL_ddepth, float* dL_dmean2D, float* dL_dconic,
-                                 float* dL_dopacity, float* dL_dcolor, float* dL_dfeature, float* dL_dz,
-                                 int* work_counter, cudaStream_t s);
+                               int* work_counter, cudaStream_t s);
 
 // ---- feature_head.cu
 cudaError_t launch_feature_resize_fwd(int C, int H, int W, int Hg, int Wg, const float* fm, const float* gt,

@@ -33,7 +33,7 @@ CONFIGS: Dict[str, dict] = {
     # small cases for parity tests / golden fixtures
     "tiny": dict(P=600, W=80, H=56, C=8, sh_degree=3, views=1),
     "small": dict(P=4000, W=160, H=112, C=16, sh_degree=2, views=1),
-    # small cases wide enough for the tensor-core feature path (C > 64), odd image size, two channel chunks
+    # small cases with wide features: a full 128-channel chunk, and an odd image size with two channel chunks
     "small128": dict(P=4000, W=160, H=112, C=128, sh_degree=2, views=1),
     "small200": dict(P=3000, W=150, H=100, C=200, sh_degree=1, views=1),
 }

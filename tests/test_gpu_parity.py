@@ -5,7 +5,7 @@ binding -> C ABI, against
 on identical seeded inputs.  Bars (BASELINE.json north_star): bit-exact tile/key indexing (radii,
 num_rendered, point_list, ranges, n_contrib); RGB/feature/depth/gradients within 1e-4 relative
 (parity.RTOL + ATOL_REL floor).  On top of the bar, colour / depth / final_T are asserted BIT-identical to
-the reference build (same fp32 operation sequence), the feature map to 5e-6 of its scale.
+the reference build (same fp32 operation sequence), the feature map to 2e-6 of its scale.
 """
 import copy
 
@@ -36,9 +36,9 @@ def _check(sc, cam, with_grads=True, vs_ref=True, vs_oracle=True, exact_vs_ref=T
             for k in ("color", "depth", "final_T"):
                 assert np.array_equal(ours[k], ref[k]), f"{k} not bit-identical to the reference build"
             if sc.C:
-                # fp32-pipe kernel: <= 2e-6 of scale; tensor-core path (C > 64, compensated 3xTF32): <= 5e-6 of scale.
-                # Both are ~20-50x inside the 1e-4 bar checked by parity.compare above.
-                assert rep["feature_map"]["max_abs_err"] <= 5e-6 * max(rep["feature_map"]["scale"], 1e-6)
+                # the feature accumulation differs from the reference by one rounding per term (composite_fwd.cu):
+                # <= 2e-6 of scale, ~50x inside the 1e-4 bar checked by parity.compare above
+                assert rep["feature_map"]["max_abs_err"] <= 2e-6 * max(rep["feature_map"]["scale"], 1e-6)
         n += 1
     if vs_oracle:
         okw = {k: v for k, v in kw.items() if k in ("colors_precomp", "cov3D_precomp")}
@@ -53,7 +53,7 @@ def _check(sc, cam, with_grads=True, vs_ref=True, vs_oracle=True, exact_vs_ref=T
 
 
 # ------------------------------------------------------------------------------------------- configs
-@pytest.mark.parametrize("name", ["tiny", "small", "c1"])
+@pytest.mark.parametrize("name", ["tiny", "small", "c1", "small128", "small200"])
 def test_small_configs_vs_reference_and_oracle(name):
     sc = scenegen.make_config(name)
     _check(sc, sc.cameras[0])
@@ -489,26 +489,3 @@ def test_view_batch_accumulates_like_autograd(name):
         assert r <= 1.0, (k, r)
     assert torch.equal(vb.denom, denom)
     assert parity.float_mismatch(vb.grad_accum.cpu().numpy(), accum.cpu().numpy(), atol_rel=parity.GRAD_ATOL_REL)[0] <= 1.0
-
-
-# ------------------------------------------------------------------------------------------- per-process overrides
-@pytest.mark.parametrize("env", [{"F3DGS_TC": "0"}, {"F3DGS_BWD2": "0"}, {"F3DGS_TC": "0", "F3DGS_BWD2": "0"},
-                                 {"F3DGS_TC": "1", "F3DGS_TC_MIN_C": "16"}, {"F3DGS_FBWD_TC": "1"}])
-def test_kernel_selection_overrides_keep_parity(env):
-    """F3DGS_TC / F3DGS_BWD2 / F3DGS_TC_MIN_C / F3DGS_FBWD_TC are read once per process, so each setting runs in its own
-    interpreter: the fp32-pipe forward, the fused single-kernel backward, the tensor-core forward (at every width from 16)
-    and the opt-in tensor-core feature-gradient kernel must all pass the same parity checks as the defaults."""
-    import os
-    import subprocess
-    import sys
-
-    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    code = (
-        "import sys; sys.path[:0] = [%r, %r, %r]\n"
-        "import scenegen, parity\n"
-        "from test_gpu_parity import _check\n"
-        "for name in ('small', 'small128', 'small200'):\n"
-        "    sc = scenegen.make_config(name); _check(sc, sc.cameras[0], vs_ref=(name == 'small'))\n"
-        "print('OVERRIDE OK')\n" % (root, os.path.join(root, "feature-3dgs_b200"), os.path.join(root, "tests")))
-    r = subprocess.run([sys.executable, "-c", code], env={**os.environ, **env}, capture_output=True, text=True, timeout=600)
-    assert r.returncode == 0 and "OVERRIDE OK" in r.stdout, r.stdout[-2000:] + r.stderr[-2000:]

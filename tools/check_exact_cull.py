@@ -1,4 +1,4 @@
-"""CPU check of the exact ellipse-vs-rectangle footprint test (composite_common.cuh: footprint_hits_rect, F3DGS_EXACT_CULL)
+"""CPU check of the exact ellipse-vs-rectangle footprint test (composite_common.cuh: footprint_hits_rect)
 restated in numpy float32: on a tile sample of a config it must keep EVERY (8x4 block, instance) pair in which at least
 one pixel passes the reference's blend conditions (power <= 0 and alpha >= 1/255), and every (tile, instance) pair likewise.
 Also reports how many pairs it removes relative to the AABB test.  Development tool (not product code)."""
