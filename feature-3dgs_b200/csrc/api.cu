@@ -535,6 +535,25 @@ int f3dgs_feature_resize_bwd(int C, int H, int W, int Hg, int Wg, const float* d
     return 0;
 }
 
+int f3dgs_image_loss(int planes, int H, int W, const float* image, const float* gt, float w_l1, float w_ssim, float* sums,
+                     float* dL_dimage, void* cuda_stream) {
+    t_error.clear();
+    if (planes < 0 || H <= 0 || W <= 0) return fail(F3DGS_ERR_INVALID_ARGUMENT, "f3dgs_image_loss: bad sizes");
+    if (planes == 0) return 0;
+    if (!image_loss_grid_ok(planes, H, W))
+        return fail(F3DGS_ERR_INVALID_ARGUMENT, "f3dgs_image_loss: sizes exceed the launch grid limits");
+    if (!image || !gt || !sums) return fail(F3DGS_ERR_INVALID_ARGUMENT, "f3dgs_image_loss: NULL pointer");
+    if (dL_dimage) {  // a CTA reads its neighbours' pixels (the window halo), so the gradient cannot overwrite an input
+        const uintptr_t n = (uintptr_t)planes * H * W * sizeof(float), d = (uintptr_t)dL_dimage;
+        auto overlaps = [&](const float* p) { return d < (uintptr_t)p + n && (uintptr_t)p < d + n; };
+        if (overlaps(image) || overlaps(gt))
+            return fail(F3DGS_ERR_INVALID_ARGUMENT, "f3dgs_image_loss: dL_dimage overlaps image or gt");
+    }
+    cudaError_t e = launch_image_loss(planes, H, W, image, gt, w_l1, w_ssim, sums, dL_dimage, (cudaStream_t)cuda_stream);
+    if (e != cudaSuccess) return fail(F3DGS_ERR_CUDA, std::string("image_loss: ") + cudaGetErrorString(e));
+    return 0;
+}
+
 int f3dgs_mark_visible(int P, const float* means3D, const float* viewmatrix, const float* projmatrix,
                        uint8_t* present, void* cuda_stream) {
     (void)projmatrix;  // the reference's frustum side test is commented out (auxiliary.h:160)

@@ -71,4 +71,9 @@ cudaError_t launch_feature_resize_fwd(int C, int H, int W, int Hg, int Wg, const
                                       float grad_scale, float* out, float* loss_sum, cudaStream_t s);
 cudaError_t launch_feature_resize_bwd(int C, int H, int W, int Hg, int Wg, const float* dout, float* dfm, cudaStream_t s);
 
+// ---- image_loss.cu: fused L1 + SSIM sums and, with dL_dimage != nullptr, the gradient w.r.t. image
+bool image_loss_grid_ok(int planes, int H, int W);  // the launch grid fits CUDA's limits
+cudaError_t launch_image_loss(int planes, int H, int W, const float* image, const float* gt, float w_l1, float w_ssim,
+                              float* sums, float* dL_dimage, cudaStream_t s);
+
 }  // namespace f3dgs

@@ -286,6 +286,29 @@ torch::Tensor featureResizeBwd(const torch::Tensor& dout, int64_t H, int64_t W) 
     return dfm;
 }
 
+// ---- photometric loss (f3dgs_image_loss): image, gt [C,H,W] or [B,C,H,W]
+// -> (sums [2] = (sum |image - gt|, sum ssim_map), dL/dimage shaped like image, or an empty tensor without need_grad)
+std::tuple<torch::Tensor, torch::Tensor> imageLoss(const torch::Tensor& image, const torch::Tensor& gt, double w_l1,
+                                                   double w_ssim, bool need_grad) {
+    TORCH_CHECK(image.is_cuda() && image.scalar_type() == torch::kFloat32 && (image.dim() == 3 || image.dim() == 4),
+                "image must be a float32 CUDA tensor [C,H,W] or [B,C,H,W]");
+    TORCH_CHECK(gt.device() == image.device() && gt.scalar_type() == torch::kFloat32 && gt.sizes() == image.sizes(),
+                "gt must be a float32 tensor on ", image.device(), " with the shape of image");
+    const c10::cuda::CUDAGuard guard(image.device());
+    auto x = image.contiguous(), y = gt.contiguous();
+    const int64_t H = x.size(-2), W = x.size(-1);
+    TORCH_CHECK(H > 0 && W > 0 && H <= INT32_MAX && W <= INT32_MAX, "image must have H, W >= 1");
+    const int64_t planes = x.numel() / (H * W);
+    TORCH_CHECK(planes <= INT32_MAX, "too many planes");
+    torch::Tensor sums = planes ? torch::empty({2}, x.options()) : torch::zeros({2}, x.options());
+    torch::Tensor grad = need_grad ? torch::empty_like(x) : torch::empty({0}, x.options());
+    cudaStream_t stream = c10::cuda::getCurrentCUDAStream().stream();
+    check_rc(f3dgs_image_loss((int)planes, (int)H, (int)W, fptr(x), fptr(y), (float)w_l1, (float)w_ssim,
+                              sums.data_ptr<float>(), need_grad && planes ? grad.data_ptr<float>() : nullptr, (void*)stream),
+             "f3dgs_image_loss");
+    return std::make_tuple(sums, grad);
+}
+
 // ---- activation prologue + fused optimizer step (f3dgs_activate / f3dgs_adam_step): in-place on the caller's tensors
 void activateParams(const torch::Tensor& raw_opacity, const torch::Tensor& raw_scaling, const torch::Tensor& raw_rotation,
                     const torch::Tensor& f_dc, const torch::Tensor& f_rest, torch::Tensor opacity, torch::Tensor scales,
@@ -347,6 +370,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     m.def("rasterize_gaussians_backward_accum", &RasterizeGaussiansBackwardAccumCUDA);
     m.def("feature_resize_fwd", &featureResizeFwd);
     m.def("feature_resize_bwd", &featureResizeBwd);
+    m.def("image_loss", &imageLoss);
     m.def("activate", &activateParams);
     m.def("adam_step", &adamStep);
     m.def("backward_scratch_bytes", [](int P) { return (unsigned long long)f3dgs_backward_scratch_bytes(P); });

@@ -151,6 +151,17 @@ int f3dgs_feature_resize_fwd(int C, int H, int W, int Hg, int Wg, const float* f
 int f3dgs_feature_resize_bwd(int C, int H, int W, int Hg, int Wg, const float* dout, float* dL_dfeature_map,
                              void* cuda_stream);
 
+/* ---- photometric loss: reference train.py (colour term), utils/loss_utils.py l1_loss + ssim(window_size=11) ---------
+ * loss = (1 - lambda_dssim) * l1_loss(image, gt) + lambda_dssim * (1 - ssim(image, gt)).  image, gt [planes,H,W]; the
+ * SSIM window is the 11-tap Gaussian (sigma 1.5) per plane with zero padding, C1 = 0.01^2, C2 = 0.03^2.
+ *   sums       device float[2]: sum |image - gt|, sum of the SSIM map (WRITTEN, not accumulated)
+ *   dL_dimage  [planes,H,W] or NULL (value only): w_l1 * sign(image - gt) + w_ssim * d(sum ssim_map)/d image, every
+ *              element written; must not overlap image or gt.  The reference loss takes w_l1 = (1 - lambda) / N and
+ *              w_ssim = -lambda / N with N = planes * H * W.
+ * Deterministic: the same inputs give bitwise-identical sums and gradient.  planes == 0 is a no-op. */
+int f3dgs_image_loss(int planes, int H, int W, const float* image, const float* gt, float w_l1, float w_ssim,
+                     float* sums, float* dL_dimage, void* cuda_stream);
+
 /* ---- activation prologue: reference scene/gaussian_model.py:98-121 ------------------------------------------------
  * opacity = sigmoid(raw_opacity[P]); scales = exp(raw_scaling[P,3]); rotations = normalize(raw_rotation[P,4]);
  * shs[P,M,3] = cat(features_dc[P,1,3], features_rest[P,M-1,3]).  Any raw pointer may be NULL (group skipped). */
