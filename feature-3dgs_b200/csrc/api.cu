@@ -554,6 +554,55 @@ int f3dgs_image_loss(int planes, int H, int W, const float* image, const float* 
     return 0;
 }
 
+namespace {
+bool ranges_overlap(const void* a, size_t na, const void* b, size_t nb) {
+    if (!a || !b) return false;
+    const uintptr_t x = (uintptr_t)a, y = (uintptr_t)b;
+    return x < y + nb && y < x + na;
+}
+}  // namespace
+
+int f3dgs_decoder_forward(int Cin, int Cout, int N, const float* weight, const float* bias, const float* x, float* y,
+                          void* cuda_stream) {
+    t_error.clear();
+    if (Cin < 1 || Cin > kDecoderMaxCin || Cout < 1 || Cout > kDecoderMaxCout || N < 1)
+        return fail(F3DGS_ERR_INVALID_ARGUMENT, "f3dgs_decoder_forward: bad sizes (1 <= Cin <= 256, 1 <= Cout <= 4096, N >= 1)");
+    if (!decoder_grid_ok(Cin, Cout, N))
+        return fail(F3DGS_ERR_INVALID_ARGUMENT, "f3dgs_decoder_forward: sizes exceed the launch grid limits");
+    if (!weight || !x || !y) return fail(F3DGS_ERR_INVALID_ARGUMENT, "f3dgs_decoder_forward: NULL pointer");
+    const size_t ny = (size_t)Cout * N * 4;
+    if (ranges_overlap(y, ny, weight, (size_t)Cout * Cin * 4) || ranges_overlap(y, ny, bias, (size_t)Cout * 4) ||
+        ranges_overlap(y, ny, x, (size_t)Cin * N * 4))
+        return fail(F3DGS_ERR_INVALID_ARGUMENT, "f3dgs_decoder_forward: y overlaps an input");
+    cudaError_t e = launch_decoder_forward(Cin, Cout, N, weight, bias, x, y, (cudaStream_t)cuda_stream);
+    if (e != cudaSuccess) return fail(F3DGS_ERR_CUDA, std::string("decoder_forward: ") + cudaGetErrorString(e));
+    return 0;
+}
+
+int f3dgs_decoder_l1(int Cin, int Cout, int N, const float* weight, const float* bias, const float* x, const float* gt,
+                     float grad_scale, float* loss_sum, float* dL_dx, float* dL_dweight, float* dL_dbias,
+                     void* cuda_stream) {
+    t_error.clear();
+    if (Cin < 1 || Cin > kDecoderMaxCin || Cout < 1 || Cout > kDecoderMaxCout || N < 1)
+        return fail(F3DGS_ERR_INVALID_ARGUMENT, "f3dgs_decoder_l1: bad sizes (1 <= Cin <= 256, 1 <= Cout <= 4096, N >= 1)");
+    if (!decoder_grid_ok(Cin, Cout, N))
+        return fail(F3DGS_ERR_INVALID_ARGUMENT, "f3dgs_decoder_l1: sizes exceed the launch grid limits");
+    if (!weight || !x || !gt || !loss_sum || !dL_dx || !dL_dweight)
+        return fail(F3DGS_ERR_INVALID_ARGUMENT, "f3dgs_decoder_l1: NULL pointer");
+    if ((bias == nullptr) != (dL_dbias == nullptr))
+        return fail(F3DGS_ERR_INVALID_ARGUMENT, "f3dgs_decoder_l1: NULL pointer (dL_dbias goes with bias)");
+    const size_t nx = (size_t)Cin * N * 4, nw = (size_t)Cout * Cin * 4, nb = (size_t)Cout * 4;
+    // a warp reads x of its own pixels only, but kernel B reads all of x after dL_dx is written
+    if (ranges_overlap(dL_dx, nx, x, nx) || ranges_overlap(dL_dx, nx, gt, (size_t)Cout * N * 4) ||
+        ranges_overlap(dL_dx, nx, weight, nw) || ranges_overlap(dL_dx, nx, bias, nb) ||
+        ranges_overlap(dL_dx, nx, dL_dweight, nw) || ranges_overlap(dL_dx, nx, dL_dbias, nb))
+        return fail(F3DGS_ERR_INVALID_ARGUMENT, "f3dgs_decoder_l1: dL_dx overlaps an input");
+    cudaError_t e = launch_decoder_l1(Cin, Cout, N, weight, bias, x, gt, grad_scale, loss_sum, dL_dx, dL_dweight,
+                                      dL_dbias, (cudaStream_t)cuda_stream);
+    if (e != cudaSuccess) return fail(F3DGS_ERR_CUDA, std::string("decoder_l1: ") + cudaGetErrorString(e));
+    return 0;
+}
+
 int f3dgs_mark_visible(int P, const float* means3D, const float* viewmatrix, const float* projmatrix,
                        uint8_t* present, void* cuda_stream) {
     (void)projmatrix;  // the reference's frustum side test is commented out (auxiliary.h:160)

@@ -8,7 +8,8 @@
 // the resize gradient with atomics into a zero-filled C*H*W tensor.  Here:
 //     resize_fwd   reads the C*H*W map once; with a target it writes  sign(interp - gt) * grad_scale  (the gradient of the
 //                  loss w.r.t. the resized map, ready for the backward) and accumulates sum |interp - gt|; without a
-//                  target it writes the resized map (decoder path: the 1x1 convolution in between stays a library GEMM).
+//                  target it writes the resized map (decoder path: feature_decoder.cu runs the 1x1 convolution and
+//                  its loss in between).
 //     resize_bwd   GATHERS: one thread per element of the C*H*W gradient sums the (few) target pixels whose bilinear
 //                  footprint covers it -- every element written exactly once, no atomics, no zero fill.
 // Sampling positions follow ATen's upsample_bilinear2d with align_corners=True: src = dst * (in - 1) / (out - 1),

@@ -76,4 +76,13 @@ bool image_loss_grid_ok(int planes, int H, int W);  // the launch grid fits CUDA
 cudaError_t launch_image_loss(int planes, int H, int W, const float* image, const float* gt, float w_l1, float w_ssim,
                               float* sums, float* dL_dimage, cudaStream_t s);
 
+// ---- feature_decoder.cu: 1x1-conv decoder y = W x + b, and its L1 loss with dL/dx (written), dL/dW and dL/db (added)
+constexpr int kDecoderMaxCin = 256, kDecoderMaxCout = 4096;
+bool decoder_grid_ok(int Cin, int Cout, int N);  // sizes in range and the launch grids fit CUDA's limits
+cudaError_t launch_decoder_forward(int Cin, int Cout, int N, const float* weight, const float* bias, const float* x,
+                                   float* y, cudaStream_t s);
+cudaError_t launch_decoder_l1(int Cin, int Cout, int N, const float* weight, const float* bias, const float* x,
+                              const float* gt, float grad_scale, float* loss_sum, float* dx, float* dW, float* db,
+                              cudaStream_t s);
+
 }  // namespace f3dgs

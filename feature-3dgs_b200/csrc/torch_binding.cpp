@@ -309,6 +309,81 @@ std::tuple<torch::Tensor, torch::Tensor> imageLoss(const torch::Tensor& image, c
     return std::make_tuple(sums, grad);
 }
 
+// ---- feature decoder (f3dgs_decoder_forward / f3dgs_decoder_l1): x [Cin,N] or [Cin,H,W], weight [Cout,Cin] or
+// [Cout,Cin,1,1], bias [Cout] or empty (no bias), gt [Cout, <x's spatial shape>]
+namespace {
+struct DecoderInputs {
+    torch::Tensor x, w, b;
+    int Cin, Cout, N;
+};
+
+DecoderInputs decoder_inputs(const torch::Tensor& x, const torch::Tensor& weight, const torch::Tensor& bias) {
+    TORCH_CHECK(x.is_cuda() && x.scalar_type() == torch::kFloat32 && x.dim() >= 2,
+                "x must be a float32 CUDA tensor [Cin,N] or [Cin,H,W]");
+    const auto dev = x.device();
+    TORCH_CHECK(weight.device() == dev && weight.scalar_type() == torch::kFloat32 &&
+                    (weight.dim() == 2 || (weight.dim() == 4 && weight.size(2) == 1 && weight.size(3) == 1)),
+                "weight must be a float32 tensor [Cout,Cin] or [Cout,Cin,1,1] on ", dev);
+    DecoderInputs d;
+    d.Cout = (int)weight.size(0);
+    d.Cin = (int)weight.size(1);
+    TORCH_CHECK(x.size(0) == d.Cin, "x has ", x.size(0), " channels, weight expects Cin = ", d.Cin);
+    const int64_t N = x.numel() / std::max<int64_t>(x.size(0), 1);
+    TORCH_CHECK(N >= 1 && N <= INT32_MAX, "x must have 1 <= N <= 2^31 - 1 pixels");
+    d.N = (int)N;
+    const bool has_b = bias.defined() && bias.numel() > 0;
+    if (has_b)
+        TORCH_CHECK(bias.device() == dev && bias.scalar_type() == torch::kFloat32 && bias.dim() == 1 &&
+                        bias.size(0) == d.Cout, "bias must be a float32 tensor [Cout] on ", dev, " (or empty)");
+    d.x = x.contiguous();
+    d.w = weight.contiguous();
+    d.b = has_b ? bias.contiguous() : torch::Tensor();
+    return d;
+}
+
+void check_accum(const torch::Tensor& t, const torch::Device& dev, int64_t numel, const char* name) {
+    TORCH_CHECK(t.defined() && t.device() == dev && t.scalar_type() == torch::kFloat32 && t.is_contiguous() &&
+                    t.numel() == numel, name, " must be a contiguous float32 tensor with ", numel, " elements on ", dev);
+}
+}  // namespace
+
+// -> y [Cout, <x's spatial shape>]
+torch::Tensor decoderForward(const torch::Tensor& x, const torch::Tensor& weight, const torch::Tensor& bias) {
+    auto d = decoder_inputs(x, weight, bias);
+    const c10::cuda::CUDAGuard guard(x.device());
+    auto shape = d.x.sizes().vec();
+    shape[0] = d.Cout;
+    torch::Tensor y = torch::empty(shape, d.x.options());
+    cudaStream_t stream = c10::cuda::getCurrentCUDAStream().stream();
+    check_rc(f3dgs_decoder_forward(d.Cin, d.Cout, d.N, fptr(d.w), fptr(d.b), fptr(d.x), y.data_ptr<float>(), (void*)stream),
+             "f3dgs_decoder_forward");
+    return y;
+}
+
+// -> (loss_sum [1] = sum |y - gt|, dL/dx shaped like x); dweight [Cout,Cin(,1,1)] and dbias [Cout] are ADDED into
+std::tuple<torch::Tensor, torch::Tensor> decoderL1(const torch::Tensor& x, const torch::Tensor& gt,
+                                                   const torch::Tensor& weight, const torch::Tensor& bias,
+                                                   double grad_scale, torch::Tensor dweight, torch::Tensor dbias) {
+    auto d = decoder_inputs(x, weight, bias);
+    const auto dev = x.device();
+    const c10::cuda::CUDAGuard guard(dev);
+    TORCH_CHECK(gt.device() == dev && gt.scalar_type() == torch::kFloat32 && gt.dim() == d.x.dim() && gt.size(0) == d.Cout &&
+                    gt.numel() == (int64_t)d.Cout * d.N && gt.sizes().slice(1) == d.x.sizes().slice(1),
+                "gt must be a float32 tensor [Cout, <x's spatial shape>] on ", dev);
+    auto g = gt.contiguous();
+    check_accum(dweight, dev, (int64_t)d.Cout * d.Cin, "dweight");
+    if (d.b.defined()) check_accum(dbias, dev, d.Cout, "dbias");
+    else TORCH_CHECK(!dbias.defined() || dbias.numel() == 0, "dbias must be empty without a bias");
+    torch::Tensor loss = torch::empty({1}, d.x.options());
+    torch::Tensor dx = torch::empty_like(d.x);
+    cudaStream_t stream = c10::cuda::getCurrentCUDAStream().stream();
+    check_rc(f3dgs_decoder_l1(d.Cin, d.Cout, d.N, fptr(d.w), fptr(d.b), fptr(d.x), fptr(g), (float)grad_scale,
+                              loss.data_ptr<float>(), dx.data_ptr<float>(), dweight.data_ptr<float>(),
+                              d.b.defined() ? dbias.data_ptr<float>() : nullptr, (void*)stream),
+             "f3dgs_decoder_l1");
+    return std::make_tuple(loss, dx);
+}
+
 // ---- activation prologue + fused optimizer step (f3dgs_activate / f3dgs_adam_step): in-place on the caller's tensors
 void activateParams(const torch::Tensor& raw_opacity, const torch::Tensor& raw_scaling, const torch::Tensor& raw_rotation,
                     const torch::Tensor& f_dc, const torch::Tensor& f_rest, torch::Tensor opacity, torch::Tensor scales,
@@ -371,6 +446,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     m.def("feature_resize_fwd", &featureResizeFwd);
     m.def("feature_resize_bwd", &featureResizeBwd);
     m.def("image_loss", &imageLoss);
+    m.def("decoder_forward", &decoderForward);
+    m.def("decoder_l1", &decoderL1);
     m.def("activate", &activateParams);
     m.def("adam_step", &adamStep);
     m.def("backward_scratch_bytes", [](int P) { return (unsigned long long)f3dgs_backward_scratch_bytes(P); });

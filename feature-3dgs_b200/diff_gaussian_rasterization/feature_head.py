@@ -6,6 +6,8 @@
 
 on two CUDA kernels of libf3dgs_b200 (csrc/feature_head.cu): a resize that, given the teacher map, directly emits the loss
 and dL/d(resized map), and a gather-style resize backward that writes every element of dL/dfeature_map exactly once.
+With --speedup the 1x1 decoder and its loss run in between on csrc/feature_decoder.cu (TF32 tensor cores, like cuDNN's
+default for the reference's nn.Conv2d): `decode`, `decoded_feature_l1_loss_and_grad`, `decoded_feature_l1_loss`.
 There is no CPU path (the extension raises on CPU tensors).
 """
 import torch
@@ -60,3 +62,65 @@ def resize_bilinear(feature_map: torch.Tensor, size) -> torch.Tensor:
     """`F.interpolate(feature_map[None], size, mode='bilinear', align_corners=True)[0]` with the gather backward; use
     it in front of the optional 1x1 decoder: `l1_loss(decoder(resize_bilinear(fm, gt.shape[1:])), gt)`."""
     return _Resize.apply(feature_map, int(size[0]), int(size[1]))
+
+
+def _empty(like: torch.Tensor) -> torch.Tensor:
+    return torch.empty(0, device=like.device, dtype=like.dtype)
+
+
+def decode(feature_map: torch.Tensor, weight: torch.Tensor, bias=None) -> torch.Tensor:
+    """The reference's `cnn_decoder(feature_map)` (nn.Conv2d(Cin, Cout, 1)) without a graph: feature_map [Cin,H,W],
+    weight [Cout,Cin,1,1] or [Cout,Cin], bias [Cout] or None -> [Cout,H,W]."""
+    with torch.no_grad():
+        return _C().decoder_forward(feature_map, weight, _empty(feature_map) if bias is None else bias)
+
+
+def decoded_feature_l1_loss_and_grad(feature_map: torch.Tensor, gt: torch.Tensor, weight: torch.Tensor, bias=None,
+                                     loss_weight: float = 1.0, dweight=None, dbias=None):
+    """-> (loss, dL/dfeature_map, dweight, dbias) for the --speedup feature loss
+
+        loss = loss_weight * l1_loss(cnn_decoder(F.interpolate(feature_map[None], gt.shape[1:], 'bilinear', True)[0]), gt)
+
+    with no autograd graph and no host sync: dL/dfeature_map is the `g_feature` a ViewBatch loop passes to `vb.backward`.
+    feature_map [Cin,H,W], gt [Cout,Hg,Wg], weight [Cout,Cin,1,1] or [Cout,Cin], bias [Cout] or None.  The gradients of
+    the decoder are ADDED into `dweight` / `dbias` (typically `conv.weight.grad` / `conv.bias.grad`, so the views of a step
+    accumulate); they are allocated zeroed when None, and dbias stays None without a bias.  Step the decoder with the
+    reference's `torch.optim.Adam(cnn_decoder.parameters())` on those tensors; with several ranks, all-reduce them (they
+    are small) before the step."""
+    Cout, Hg, Wg = gt.shape
+    with torch.no_grad():
+        resized, _ = _C().feature_resize_fwd(feature_map, _empty(feature_map), Hg, Wg, 0.0)
+        if dweight is None:
+            dweight = torch.zeros_like(weight, memory_format=torch.contiguous_format)
+        if dbias is None and bias is not None:
+            dbias = torch.zeros_like(bias, memory_format=torch.contiguous_format)
+        gs = float(loss_weight) / max(Cout * Hg * Wg, 1)
+        loss_sum, dres = _C().decoder_l1(resized, gt, weight, _empty(feature_map) if bias is None else bias, gs, dweight,
+                                         _empty(feature_map) if dbias is None else dbias)
+        grad = _C().feature_resize_bwd(dres, feature_map.shape[1], feature_map.shape[2])
+    return loss_sum[0] * gs, grad, dweight, dbias
+
+
+class _DecodedL1(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, feature_map, weight, bias, gt, loss_weight):
+        loss, g_fm, g_w, g_b = decoded_feature_l1_loss_and_grad(feature_map.detach(), gt.detach(), weight.detach(),
+                                                                None if bias is None else bias.detach(), loss_weight)
+        ctx.has_bias = bias is not None
+        ctx.save_for_backward(g_fm, g_w, *((g_b,) if bias is not None else ()))
+        return loss
+
+    @staticmethod
+    def backward(ctx, g):
+        saved = ctx.saved_tensors
+        g_b = saved[2] * g if ctx.has_bias else None
+        return saved[0] * g, saved[1] * g, g_b, None, None
+
+
+def decoded_feature_l1_loss(feature_map: torch.Tensor, gt: torch.Tensor, weight: torch.Tensor, bias=None,
+                            loss_weight: float = 1.0) -> torch.Tensor:
+    """Autograd-aware drop-in for the --speedup feature loss of train.py:
+    `decoded_feature_l1_loss(feature_map, gt_feature_map, cnn_decoder.conv.weight, cnn_decoder.conv.bias)` equals
+    `l1_loss(cnn_decoder(F.interpolate(feature_map[None], gt.shape[1:], 'bilinear', True)[0]), gt) * loss_weight`, with
+    gradients for feature_map, weight and bias (gt is the constant target)."""
+    return _DecodedL1.apply(feature_map, weight, bias, gt, float(loss_weight))

@@ -141,8 +141,8 @@ int f3dgs_backward_accum(int P, int D, int M, int R, int C,
  *   f3dgs_feature_resize_fwd  gt != NULL: out[C,Hg,Wg] = sign(resized - gt) * grad_scale  (dL/d resized for
  *                             L = grad_scale * sum |resized - gt|; pass weight / (C*Hg*Wg) for the weighted mean) and
  *                             *loss_sum += sum |resized - gt|  (device float, caller-zeroed, may be NULL);
- *                             gt == NULL: out = resized map (decoder path: the 1x1 convolution of
- *                             models/networks.py:107-119 runs between the two calls as a library GEMM).
+ *                             gt == NULL: out = resized map (decoder path: f3dgs_decoder_l1 below runs the
+ *                             1x1 convolution of models/networks.py:107-119 and its loss between the two calls).
  *   f3dgs_feature_resize_bwd  dL_dfeature_map[C,H,W] = resize^T(dout[C,Hg,Wg]); every element is written (gather, no
  *                             atomics, no zero fill needed).
  */
@@ -150,6 +150,23 @@ int f3dgs_feature_resize_fwd(int C, int H, int W, int Hg, int Wg, const float* f
                              float grad_scale, float* out, float* loss_sum, void* cuda_stream);
 int f3dgs_feature_resize_bwd(int C, int H, int W, int Hg, int Wg, const float* dout, float* dL_dfeature_map,
                              void* cuda_stream);
+
+/* ---- feature decoder (--speedup): models/networks.py:107-119 CNN_decoder, nn.Conv2d(Cin, Cout, kernel_size=1) -------
+ * x [Cin,N] (the resized map, N = Hg*Wg), weight [Cout,Cin] (the conv weight [Cout,Cin,1,1] as contiguous memory),
+ * bias [Cout] or NULL (a conv without bias), gt [Cout,N].  1 <= Cin <= 256, 1 <= Cout <= 4096, N >= 1.  TF32 tensor-core
+ * products (operands rounded to nearest, fp32 accumulate), the precision of cuDNN's default for the reference layer.
+ *   f3dgs_decoder_forward  y[Cout,N] = weight x + bias; y must not overlap an input.
+ *   f3dgs_decoder_l1       with s = sign(y - gt) (sign(0) = 0):  *loss_sum = sum |y - gt| (written);
+ *                          dL_dx[Cin,N] = grad_scale * weight^T s (every element written; must not overlap an input);
+ *                          dL_dweight[Cout,Cin] += grad_scale * s x^T;  dL_dbias[Cout] += grad_scale * sum_n s
+ *                          (added, so that the views of a step accumulate; dL_dbias may be NULL iff bias is NULL).
+ *                          l1_loss(decoder(x), gt) * w takes grad_scale = w / (Cout * N).
+ * y and s never reach memory as fp32; results are bitwise reproducible (no float atomics). */
+int f3dgs_decoder_forward(int Cin, int Cout, int N, const float* weight, const float* bias, const float* x, float* y,
+                          void* cuda_stream);
+int f3dgs_decoder_l1(int Cin, int Cout, int N, const float* weight, const float* bias, const float* x, const float* gt,
+                     float grad_scale, float* loss_sum, float* dL_dx, float* dL_dweight, float* dL_dbias,
+                     void* cuda_stream);
 
 /* ---- photometric loss: reference train.py (colour term), utils/loss_utils.py l1_loss + ssim(window_size=11) ---------
  * loss = (1 - lambda_dssim) * l1_loss(image, gt) + lambda_dssim * (1 - ssim(image, gt)).  image, gt [planes,H,W]; the
