@@ -603,6 +603,34 @@ int f3dgs_decoder_l1(int Cin, int Cout, int N, const float* weight, const float*
     return 0;
 }
 
+size_t f3dgs_knn_scratch_bytes(int P) {
+    t_error.clear();
+    size_t bytes = 0;
+    const cudaError_t e = knn_scratch_bytes(P, &bytes);
+    if (e != cudaSuccess) {
+        fail(F3DGS_ERR_CUDA, std::string("f3dgs_knn_scratch_bytes: ") + cudaGetErrorString(e));
+        return 0;
+    }
+    return bytes;
+}
+
+int f3dgs_knn_mean_dist(int P, const float* points, float* out, char* scratch, void* cuda_stream) {
+    t_error.clear();
+    if (P < 0) return fail(F3DGS_ERR_INVALID_ARGUMENT, "f3dgs_knn_mean_dist: P < 0");
+    if (P == 0) return 0;
+    if (!points || !out || !scratch) return fail(F3DGS_ERR_INVALID_ARGUMENT, "f3dgs_knn_mean_dist: NULL pointer");
+    const size_t no = (size_t)P * 4;
+    if (ranges_overlap(out, no, points, (size_t)P * 12) || ranges_overlap(out, no, scratch, knn_scratch_fixed_bytes(P)))
+        return fail(F3DGS_ERR_INVALID_ARGUMENT, "f3dgs_knn_mean_dist: out overlaps points or scratch");
+    size_t sb = 0;
+    CUDA_TRY(knn_scratch_bytes(P, &sb));  // the sort's share of the scratch is sized by CUB for the current device
+    if (ranges_overlap(out, no, scratch, sb))
+        return fail(F3DGS_ERR_INVALID_ARGUMENT, "f3dgs_knn_mean_dist: out overlaps points or scratch");
+    cudaError_t e = launch_knn_mean_dist(P, points, out, scratch, (cudaStream_t)cuda_stream);
+    if (e != cudaSuccess) return fail(F3DGS_ERR_CUDA, std::string("knn_mean_dist: ") + cudaGetErrorString(e));
+    return 0;
+}
+
 int f3dgs_mark_visible(int P, const float* means3D, const float* viewmatrix, const float* projmatrix,
                        uint8_t* present, void* cuda_stream) {
     (void)projmatrix;  // the reference's frustum side test is commented out (auxiliary.h:160)

@@ -85,4 +85,10 @@ cudaError_t launch_decoder_l1(int Cin, int Cout, int N, const float* weight, con
                               const float* gt, float grad_scale, float* loss_sum, float* dx, float* dW, float* db,
                               cudaStream_t s);
 
+// ---- knn.cu: exact mean squared distance to the 3 nearest other points (distCUDA2); scratch is knn_scratch_bytes(P)
+// bytes whose first knn_scratch_fixed_bytes(P) need no device query to size
+cudaError_t knn_scratch_bytes(int P, size_t* bytes);
+size_t knn_scratch_fixed_bytes(int P);
+cudaError_t launch_knn_mean_dist(int P, const float* points, float* out, char* scratch, cudaStream_t s);
+
 }  // namespace f3dgs

@@ -384,6 +384,27 @@ std::tuple<torch::Tensor, torch::Tensor> decoderL1(const torch::Tensor& x, const
     return std::make_tuple(loss, dx);
 }
 
+// ---- initial scales (f3dgs_knn_mean_dist, the reference's simple_knn distCUDA2): points [P,3] -> [P]
+torch::Tensor knnMeanDist(const torch::Tensor& points) {
+    TORCH_CHECK(points.is_cuda(), "points must be a CUDA tensor (this build has no CPU path)");
+    TORCH_CHECK(points.scalar_type() == torch::kFloat32 && points.dim() == 2 && points.size(1) == 3,
+                "points must be a float32 tensor [P,3]");
+    TORCH_CHECK(points.size(0) <= INT32_MAX, "points: P must be below 2^31");
+    const c10::cuda::CUDAGuard guard(points.device());
+    auto p = points.contiguous();
+    const int P = (int)p.size(0);
+    torch::Tensor out = torch::empty({P}, p.options());
+    if (P == 0) return out;
+    const size_t bytes = f3dgs_knn_scratch_bytes(P);
+    TORCH_CHECK(bytes > 0, "f3dgs_knn_scratch_bytes failed: ", f3dgs_last_error());
+    torch::Tensor scratch = torch::empty({(int64_t)bytes}, p.options().dtype(torch::kByte));
+    cudaStream_t stream = c10::cuda::getCurrentCUDAStream().stream();
+    check_rc(f3dgs_knn_mean_dist(P, fptr(p), out.data_ptr<float>(), reinterpret_cast<char*>(scratch.data_ptr()),
+                                 (void*)stream),
+             "f3dgs_knn_mean_dist");
+    return out;
+}
+
 // ---- activation prologue + fused optimizer step (f3dgs_activate / f3dgs_adam_step): in-place on the caller's tensors
 void activateParams(const torch::Tensor& raw_opacity, const torch::Tensor& raw_scaling, const torch::Tensor& raw_rotation,
                     const torch::Tensor& f_dc, const torch::Tensor& f_rest, torch::Tensor opacity, torch::Tensor scales,
@@ -448,6 +469,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     m.def("image_loss", &imageLoss);
     m.def("decoder_forward", &decoderForward);
     m.def("decoder_l1", &decoderL1);
+    m.def("knn_mean_dist", &knnMeanDist);
     m.def("activate", &activateParams);
     m.def("adam_step", &adamStep);
     m.def("backward_scratch_bytes", [](int P) { return (unsigned long long)f3dgs_backward_scratch_bytes(P); });

@@ -4,6 +4,8 @@
     one `vertex` element of float32 properties  x y z nx ny nz f_dc_* f_rest_* opacity scale_* rot_* semantic_*  in that
     order; f_dc / f_rest / semantic are stored channel-major (the reference transposes [P, K, 3] -> [P, 3, K] before
     flattening, :214-215, :220).
+  * points3D.ply of a COLMAP / synthetic scene (scene/dataset_readers.py fetchPly): x y z nx ny nz red green blue, the
+    input of GaussianState.from_point_cloud.
   * `<name>_fmap_CxHxW.pt` (render.py:179-180, scene/dataset_readers.py:110-112): the rendered / teacher feature map as a
     float16 tensor [C, H, W] saved with torch.save.
 Pure host-side I/O (numpy / torch.save): nothing here runs on the hot path.
@@ -106,6 +108,19 @@ def load_ply(path: str, max_sh_degree: int = 3) -> Dict[str, np.ndarray]:
     return dict(xyz=xyz, features_dc=np.ascontiguousarray(f_dc), features_rest=np.ascontiguousarray(f_rest),
                 opacity=np.asarray(v["opacity"], f32).reshape(P, 1), scaling=numbered("scale_"), rotation=numbered("rot_"),
                 semantic_feature=np.ascontiguousarray(sem.reshape(P, -1, 1).transpose(0, 2, 1)))
+
+
+def load_point_cloud(path: str):
+    """-> (points [P,3], colors [P,3], normals [P,3]) as the reference's fetchPly reads a points3D.ply
+    (scene/dataset_readers.py): x y z and nx ny nz as stored, red green blue (uchar) / 255.0 in float64."""
+    v = read_ply_vertices(path)
+    missing = [n for n in ("x", "y", "z", "nx", "ny", "nz", "red", "green", "blue") if n not in v]
+    if missing:
+        raise ValueError(f"{path}: vertex element lacks {', '.join(missing)}")
+    points = np.vstack([v["x"], v["y"], v["z"]]).T
+    colors = np.vstack([v["red"], v["green"], v["blue"]]).T / 255.0
+    normals = np.vstack([v["nx"], v["ny"], v["nz"]]).T
+    return points, colors, normals
 
 
 def fmap_filename(stem: str, C: int, H: int, W: int) -> str:

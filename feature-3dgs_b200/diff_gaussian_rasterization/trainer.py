@@ -4,6 +4,8 @@
 `GaussianState` keeps the RAW parameters the reference's GaussianModel optimises (`_xyz, _features_dc, _features_rest,
 _opacity, _scaling, _rotation, _semantic_feature`, :47-58) as plain CUDA tensors, and
 
+  from_point_cloud()    create_from_pcd (:133-160): a fresh state from a point cloud, initial scales from the native
+                        exact 3-NN distance (f3dgs_knn_mean_dist, the reference's simple_knn distCUDA2);
   activate()            raw -> the activated tensors the rasterizer consumes (:98-121) in ONE kernel (f3dgs_activate), once
                         per optimizer step instead of four elementwise kernels + a concat per view;
   batch()               a ViewBatch (parallel.py) over the activated tensors: forward / in-kernel accumulated backward of
@@ -18,6 +20,7 @@ _opacity, _scaling, _rotation, _semantic_feature`, :47-58) as plain CUDA tensors
 import math
 from typing import Dict, Optional
 
+import numpy as np
 import torch
 
 from .parallel import ViewBatch
@@ -56,6 +59,43 @@ class GaussianState:
                 raise RuntimeError(f"{k} must be a float32 CUDA tensor (this build has no CPU path)")
         self.betas, self.eps, self.percent_dense = betas, eps, percent_dense
         self._reset_derived()
+
+    @classmethod
+    def from_point_cloud(cls, points, colors, semantic_feature_size: int, speedup: bool = False, max_sh_degree: int = 3,
+                         device="cuda", **kwargs):
+        """scene/gaussian_model.py:133-160 (create_from_pcd): a fresh state from a point cloud.
+
+        points [P,3] and colors [P,3] (RGB in [0,1]) are arrays or tensors of any float dtype; both are converted to
+        float32 first, as the reference does.  The initial scale of each Gaussian is log(sqrt(mean squared distance to its
+        three nearest neighbours)), isotropic, from the native distCUDA2 (csrc/knn.cu).  Every other field is computed
+        with the reference's own tensor operations, so it is bitwise what create_from_pcd builds.  With `speedup` the
+        feature width is int(semantic_feature_size / 4), as there.  Raises ValueError on mismatched shapes or a
+        non-finite coordinate."""
+        from . import _C
+
+        def as_f32(a):
+            t = a if isinstance(a, torch.Tensor) else torch.as_tensor(np.asarray(a))
+            return t.float().to(device)
+
+        xyz, rgb = as_f32(points), as_f32(colors)
+        if xyz.dim() != 2 or xyz.shape[1] != 3 or rgb.shape != xyz.shape:
+            raise ValueError(f"points and colors must both be [P,3], got {tuple(xyz.shape)} and {tuple(rgb.shape)}")
+        if not bool(torch.isfinite(xyz).all()):
+            raise ValueError("points contain a non-finite coordinate")
+        P = xyz.shape[0]
+        fused_color = (rgb - 0.5) / 0.28209479177387814  # utils/sh_utils.py RGB2SH
+        features = torch.zeros((P, 3, (max_sh_degree + 1) ** 2), dtype=torch.float32, device=device)
+        features[:, :3, 0] = fused_color
+        if speedup:
+            semantic_feature_size = int(semantic_feature_size / 4)
+        semantic_feature = torch.zeros(P, semantic_feature_size, 1, dtype=torch.float32, device=device)
+        dist2 = torch.clamp_min(_C.knn_mean_dist(xyz), 0.0000001)
+        scales = torch.log(torch.sqrt(dist2))[..., None].repeat(1, 3)
+        rots = torch.zeros((P, 4), device=device)
+        rots[:, 0] = 1
+        opacities = inverse_sigmoid(0.1 * torch.ones((P, 1), dtype=torch.float, device=device))
+        return cls(xyz, features[:, :, 0:1].transpose(1, 2).contiguous(), features[:, :, 1:].transpose(1, 2).contiguous(),
+                   opacities, scales, rots, semantic_feature.transpose(1, 2).contiguous(), **kwargs)
 
     # ---------------------------------------------------------------------------------------------- buffers
     @property

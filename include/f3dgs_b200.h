@@ -201,6 +201,18 @@ int f3dgs_activate(int P, int M, const float* raw_opacity, const float* raw_scal
 int f3dgs_adam_step(int kind, size_t n, int M, float* param, const float* grad_activated, float* exp_avg,
                     float* exp_avg_sq, float lr, float beta1, float beta2, float eps, int step, void* cuda_stream);
 
+/* ---- initial scales: reference submodules/simple-knn distCUDA2, used by scene/gaussian_model.py:133-160 ------------
+ * out[i] = (d0 + d1 + d2) / 3 in fp32, where d0 <= d1 <= d2 are the three smallest squared distances from points[i] to
+ * the points j != i (exclusion by index: a coincident point counts as 0).  Missing neighbours (P < 4) keep FLT_MAX, as in
+ * the reference: +inf for P = 1, 2 and about FLT_MAX / 3 for P = 3.  The result is exact (not approximate), bitwise
+ * reproducible and independent of the order of the points.
+ *   points   [P,3] float32 device memory        out  [P] float32, must not overlap points or scratch
+ *   scratch  f3dgs_knn_scratch_bytes(P) bytes of device memory, 256-byte aligned
+ * Stream-ordered with no host sync.  P == 0 launches nothing.  f3dgs_knn_scratch_bytes returns 0 for P <= 0, and 0 with
+ * f3dgs_last_error() set if the size query of the device sort fails. */
+size_t f3dgs_knn_scratch_bytes(int P);
+int f3dgs_knn_mean_dist(int P, const float* points, float* out, char* scratch, void* cuda_stream);
+
 /* ---- markVisible: reference rasterizer_impl.cu:141-153 (checkFrustum :54-66) --------------
  * present[i] = (view-space z of means3D[i] > 0.2).  `present` is P bytes (0/1). */
 int f3dgs_mark_visible(int P, const float* means3D, const float* viewmatrix,
