@@ -12,6 +12,7 @@
 #include <cstring>
 #include <mutex>
 #include <string>
+#include <type_traits>
 #include <vector>
 
 #include "../../include/f3dgs_b200.h"
@@ -510,17 +511,51 @@ int f3dgs_backward_accum(int P, int D, int M, int R, int C, const float* backgro
     return 0;
 }
 
-int f3dgs_feature_resize_fwd(int C, int H, int W, int Hg, int Wg, const float* feature_map, const float* gt,
-                             float grad_scale, float* out, float* loss_sum, void* cuda_stream) {
+}  // extern "C"
+
+namespace {
+bool ranges_overlap(const void* a, size_t na, const void* b, size_t nb) {
+    if (!a || !b) return false;
+    const uintptr_t x = (uintptr_t)a, y = (uintptr_t)b;
+    return x < y + nb && y < x + na;
+}
+
+// The float16 entry points (_f16gt, _f16) validate and launch as their float32 twins do; `fn` is the twin's name without
+// the f3dgs_ prefix.  Half data is IEEE binary16 bits at the ABI (uint16_t) and __half in the kernels.
+template <typename GT>
+int feature_resize_fwd_impl(const char* fn, int C, int H, int W, int Hg, int Wg, const float* feature_map, const GT* gt,
+                            float grad_scale, float* out, float* loss_sum, void* cuda_stream) {
+    const std::string api = std::string("f3dgs_") + fn;
     t_error.clear();
-    if (C < 0 || H <= 0 || W <= 0 || Hg <= 0 || Wg <= 0)
-        return fail(F3DGS_ERR_INVALID_ARGUMENT, "f3dgs_feature_resize_fwd: bad sizes");
+    if (C < 0 || H <= 0 || W <= 0 || Hg <= 0 || Wg <= 0) return fail(F3DGS_ERR_INVALID_ARGUMENT, api + ": bad sizes");
     if (C == 0) return 0;
-    if (!feature_map || !out) return fail(F3DGS_ERR_INVALID_ARGUMENT, "f3dgs_feature_resize_fwd: NULL pointer");
+    if (!feature_map || !out) return fail(F3DGS_ERR_INVALID_ARGUMENT, api + ": NULL pointer");
+    if constexpr (std::is_same_v<GT, __half>) {
+        // no target is the float32 symbol's job; out's 4-byte elements cannot alias gt's 2-byte ones element for element
+        if (!gt) return fail(F3DGS_ERR_INVALID_ARGUMENT, api + ": NULL pointer (gt is required)");
+        const size_t n = (size_t)C * Hg * Wg;
+        if (ranges_overlap(out, n * 4, feature_map, (size_t)C * H * W * 4) || ranges_overlap(out, n * 4, gt, n * 2))
+            return fail(F3DGS_ERR_INVALID_ARGUMENT, api + ": out overlaps feature_map or gt");
+    }
     cudaError_t e = launch_feature_resize_fwd(C, H, W, Hg, Wg, feature_map, gt, grad_scale, out, loss_sum,
                                               (cudaStream_t)cuda_stream);
-    if (e != cudaSuccess) return fail(F3DGS_ERR_CUDA, std::string("feature_resize_fwd: ") + cudaGetErrorString(e));
+    if (e != cudaSuccess) return fail(F3DGS_ERR_CUDA, std::string(fn) + ": " + cudaGetErrorString(e));
     return 0;
+}
+}  // namespace
+
+extern "C" {
+
+int f3dgs_feature_resize_fwd(int C, int H, int W, int Hg, int Wg, const float* feature_map, const float* gt,
+                             float grad_scale, float* out, float* loss_sum, void* cuda_stream) {
+    return feature_resize_fwd_impl("feature_resize_fwd", C, H, W, Hg, Wg, feature_map, gt, grad_scale, out, loss_sum,
+                                   cuda_stream);
+}
+
+int f3dgs_feature_resize_fwd_f16gt(int C, int H, int W, int Hg, int Wg, const float* feature_map, const uint16_t* gt,
+                                   float grad_scale, float* out, float* loss_sum, void* cuda_stream) {
+    return feature_resize_fwd_impl("feature_resize_fwd_f16gt", C, H, W, Hg, Wg, feature_map,
+                                   reinterpret_cast<const __half*>(gt), grad_scale, out, loss_sum, cuda_stream);
 }
 
 int f3dgs_feature_resize_bwd(int C, int H, int W, int Hg, int Wg, const float* dout, float* dL_dfeature_map,
@@ -554,53 +589,80 @@ int f3dgs_image_loss(int planes, int H, int W, const float* image, const float* 
     return 0;
 }
 
+}  // extern "C"
+
 namespace {
-bool ranges_overlap(const void* a, size_t na, const void* b, size_t nb) {
-    if (!a || !b) return false;
-    const uintptr_t x = (uintptr_t)a, y = (uintptr_t)b;
-    return x < y + nb && y < x + na;
+template <typename Y>
+int decoder_forward_impl(const char* fn, int Cin, int Cout, int N, const float* weight, const float* bias, const float* x,
+                         Y* y, void* cuda_stream) {
+    const std::string api = std::string("f3dgs_") + fn;
+    t_error.clear();
+    if (Cin < 1 || Cin > kDecoderMaxCin || Cout < 1 || Cout > kDecoderMaxCout || N < 1)
+        return fail(F3DGS_ERR_INVALID_ARGUMENT, api + ": bad sizes (1 <= Cin <= 256, 1 <= Cout <= 4096, N >= 1)");
+    if (!decoder_grid_ok(Cin, Cout, N))
+        return fail(F3DGS_ERR_INVALID_ARGUMENT, api + ": sizes exceed the launch grid limits");
+    if (!weight || !x || !y) return fail(F3DGS_ERR_INVALID_ARGUMENT, api + ": NULL pointer");
+    const size_t ny = (size_t)Cout * N * sizeof(Y);
+    if (ranges_overlap(y, ny, weight, (size_t)Cout * Cin * 4) || ranges_overlap(y, ny, bias, (size_t)Cout * 4) ||
+        ranges_overlap(y, ny, x, (size_t)Cin * N * 4))
+        return fail(F3DGS_ERR_INVALID_ARGUMENT, api + ": y overlaps an input");
+    cudaError_t e = launch_decoder_forward(Cin, Cout, N, weight, bias, x, y, (cudaStream_t)cuda_stream);
+    if (e != cudaSuccess) return fail(F3DGS_ERR_CUDA, std::string(fn) + ": " + cudaGetErrorString(e));
+    return 0;
+}
+
+template <typename GT>
+int decoder_l1_impl(const char* fn, int Cin, int Cout, int N, const float* weight, const float* bias, const float* x,
+                    const GT* gt, float grad_scale, float* loss_sum, float* dL_dx, float* dL_dweight, float* dL_dbias,
+                    void* cuda_stream) {
+    const std::string api = std::string("f3dgs_") + fn;
+    t_error.clear();
+    if (Cin < 1 || Cin > kDecoderMaxCin || Cout < 1 || Cout > kDecoderMaxCout || N < 1)
+        return fail(F3DGS_ERR_INVALID_ARGUMENT, api + ": bad sizes (1 <= Cin <= 256, 1 <= Cout <= 4096, N >= 1)");
+    if (!decoder_grid_ok(Cin, Cout, N))
+        return fail(F3DGS_ERR_INVALID_ARGUMENT, api + ": sizes exceed the launch grid limits");
+    if (!weight || !x || !gt || !loss_sum || !dL_dx || !dL_dweight)
+        return fail(F3DGS_ERR_INVALID_ARGUMENT, api + ": NULL pointer");
+    if ((bias == nullptr) != (dL_dbias == nullptr))
+        return fail(F3DGS_ERR_INVALID_ARGUMENT, api + ": NULL pointer (dL_dbias goes with bias)");
+    const size_t nx = (size_t)Cin * N * 4, nw = (size_t)Cout * Cin * 4, nb = (size_t)Cout * 4;
+    // a warp reads x of its own pixels only, but kernel B reads all of x after dL_dx is written
+    if (ranges_overlap(dL_dx, nx, x, nx) || ranges_overlap(dL_dx, nx, gt, (size_t)Cout * N * sizeof(GT)) ||
+        ranges_overlap(dL_dx, nx, weight, nw) || ranges_overlap(dL_dx, nx, bias, nb) ||
+        ranges_overlap(dL_dx, nx, dL_dweight, nw) || ranges_overlap(dL_dx, nx, dL_dbias, nb))
+        return fail(F3DGS_ERR_INVALID_ARGUMENT, api + ": dL_dx overlaps an input");
+    cudaError_t e = launch_decoder_l1(Cin, Cout, N, weight, bias, x, gt, grad_scale, loss_sum, dL_dx, dL_dweight,
+                                      dL_dbias, (cudaStream_t)cuda_stream);
+    if (e != cudaSuccess) return fail(F3DGS_ERR_CUDA, std::string(fn) + ": " + cudaGetErrorString(e));
+    return 0;
 }
 }  // namespace
 
+extern "C" {
+
 int f3dgs_decoder_forward(int Cin, int Cout, int N, const float* weight, const float* bias, const float* x, float* y,
                           void* cuda_stream) {
-    t_error.clear();
-    if (Cin < 1 || Cin > kDecoderMaxCin || Cout < 1 || Cout > kDecoderMaxCout || N < 1)
-        return fail(F3DGS_ERR_INVALID_ARGUMENT, "f3dgs_decoder_forward: bad sizes (1 <= Cin <= 256, 1 <= Cout <= 4096, N >= 1)");
-    if (!decoder_grid_ok(Cin, Cout, N))
-        return fail(F3DGS_ERR_INVALID_ARGUMENT, "f3dgs_decoder_forward: sizes exceed the launch grid limits");
-    if (!weight || !x || !y) return fail(F3DGS_ERR_INVALID_ARGUMENT, "f3dgs_decoder_forward: NULL pointer");
-    const size_t ny = (size_t)Cout * N * 4;
-    if (ranges_overlap(y, ny, weight, (size_t)Cout * Cin * 4) || ranges_overlap(y, ny, bias, (size_t)Cout * 4) ||
-        ranges_overlap(y, ny, x, (size_t)Cin * N * 4))
-        return fail(F3DGS_ERR_INVALID_ARGUMENT, "f3dgs_decoder_forward: y overlaps an input");
-    cudaError_t e = launch_decoder_forward(Cin, Cout, N, weight, bias, x, y, (cudaStream_t)cuda_stream);
-    if (e != cudaSuccess) return fail(F3DGS_ERR_CUDA, std::string("decoder_forward: ") + cudaGetErrorString(e));
-    return 0;
+    return decoder_forward_impl("decoder_forward", Cin, Cout, N, weight, bias, x, y, cuda_stream);
+}
+
+int f3dgs_decoder_forward_f16(int Cin, int Cout, int N, const float* weight, const float* bias, const float* x,
+                              uint16_t* y, void* cuda_stream) {
+    return decoder_forward_impl("decoder_forward_f16", Cin, Cout, N, weight, bias, x, reinterpret_cast<__half*>(y),
+                                cuda_stream);
 }
 
 int f3dgs_decoder_l1(int Cin, int Cout, int N, const float* weight, const float* bias, const float* x, const float* gt,
                      float grad_scale, float* loss_sum, float* dL_dx, float* dL_dweight, float* dL_dbias,
                      void* cuda_stream) {
-    t_error.clear();
-    if (Cin < 1 || Cin > kDecoderMaxCin || Cout < 1 || Cout > kDecoderMaxCout || N < 1)
-        return fail(F3DGS_ERR_INVALID_ARGUMENT, "f3dgs_decoder_l1: bad sizes (1 <= Cin <= 256, 1 <= Cout <= 4096, N >= 1)");
-    if (!decoder_grid_ok(Cin, Cout, N))
-        return fail(F3DGS_ERR_INVALID_ARGUMENT, "f3dgs_decoder_l1: sizes exceed the launch grid limits");
-    if (!weight || !x || !gt || !loss_sum || !dL_dx || !dL_dweight)
-        return fail(F3DGS_ERR_INVALID_ARGUMENT, "f3dgs_decoder_l1: NULL pointer");
-    if ((bias == nullptr) != (dL_dbias == nullptr))
-        return fail(F3DGS_ERR_INVALID_ARGUMENT, "f3dgs_decoder_l1: NULL pointer (dL_dbias goes with bias)");
-    const size_t nx = (size_t)Cin * N * 4, nw = (size_t)Cout * Cin * 4, nb = (size_t)Cout * 4;
-    // a warp reads x of its own pixels only, but kernel B reads all of x after dL_dx is written
-    if (ranges_overlap(dL_dx, nx, x, nx) || ranges_overlap(dL_dx, nx, gt, (size_t)Cout * N * 4) ||
-        ranges_overlap(dL_dx, nx, weight, nw) || ranges_overlap(dL_dx, nx, bias, nb) ||
-        ranges_overlap(dL_dx, nx, dL_dweight, nw) || ranges_overlap(dL_dx, nx, dL_dbias, nb))
-        return fail(F3DGS_ERR_INVALID_ARGUMENT, "f3dgs_decoder_l1: dL_dx overlaps an input");
-    cudaError_t e = launch_decoder_l1(Cin, Cout, N, weight, bias, x, gt, grad_scale, loss_sum, dL_dx, dL_dweight,
-                                      dL_dbias, (cudaStream_t)cuda_stream);
-    if (e != cudaSuccess) return fail(F3DGS_ERR_CUDA, std::string("decoder_l1: ") + cudaGetErrorString(e));
-    return 0;
+    return decoder_l1_impl("decoder_l1", Cin, Cout, N, weight, bias, x, gt, grad_scale, loss_sum, dL_dx, dL_dweight,
+                           dL_dbias, cuda_stream);
+}
+
+int f3dgs_decoder_l1_f16gt(int Cin, int Cout, int N, const float* weight, const float* bias, const float* x,
+                           const uint16_t* gt, float grad_scale, float* loss_sum, float* dL_dx, float* dL_dweight,
+                           float* dL_dbias, void* cuda_stream) {
+    return decoder_l1_impl("decoder_l1_f16gt", Cin, Cout, N, weight, bias, x, reinterpret_cast<const __half*>(gt),
+                           grad_scale, loss_sum, dL_dx, dL_dweight, dL_dbias, cuda_stream);
 }
 
 size_t f3dgs_knn_scratch_bytes(int P) {

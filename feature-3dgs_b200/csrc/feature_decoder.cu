@@ -21,6 +21,9 @@
 //              per-CTA loss partials of kernel A in double.
 // No float atomics: every output element is written by one thread and every sum has a fixed order, so results are
 // bitwise reproducible.  Decode and loss mode run the same code for y, so decode(x) as gt gives exactly zero loss.
+// gt (loss) and y (decode) may also be float16, the data format's teacher maps: a float16 gt is upcast exactly at its load
+// (the result is the float32 one for gt.float()), a float16 y is rounded to nearest even at its store (y.half()).
+#include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
 
@@ -69,13 +72,19 @@ __device__ __forceinline__ uint32_t word_sign(uint32_t w, int i) {
     return (((w >> i) & 1u) * 0x3f800000u) | (((w >> (16 + i)) & 1u) << 31);
 }
 
+__device__ __forceinline__ float load_f32(const float* p) { return __ldg(p); }
+__device__ __forceinline__ float load_f32(const __half* p) { return __half2float(__ldg(p)); }
+__device__ __forceinline__ void store_f32(float* p, float v) { *p = v; }
+__device__ __forceinline__ void store_f32(__half* p, float v) { *p = __float2half_rn(v); }
+
+template <typename T>      // element type of gt and y: float or __half
 struct DecArgs {
     int Cin, Cout, N, N16;
     const float* wt;       // [Cout_pad, Cp] TF32, zero-padded
     const float* bias;     // [Cout_pad], zero-padded
     const float* x;        // [Cin, N]
-    const float* gt;       // [Cout, N]            (loss)
-    float* y;              // [Cout, N]            (decode)
+    const T* gt;           // [Cout, N]            (loss)
+    T* y;                  // [Cout, N]            (decode)
     float* dx;             // [Cin, N]             (loss)
     uint32_t* bits;        // [Cout, N16]          (loss)
     float* loss_part;      // [gridDim.x]          (loss)
@@ -93,8 +102,8 @@ struct DecSmem {
     static constexpr size_t bytes = (size_t)2 * step * SW * 4 + (x_in_regs ? 0 : (size_t)kWarpsA * KT * 32 * 16);
 };
 
-template <int KT, bool LOSS>
-__global__ void __launch_bounds__(kThreadsA, 1) decoder_kernel(DecArgs a) {
+template <int KT, bool LOSS, typename T>
+__global__ void __launch_bounds__(kThreadsA, 1) decoder_kernel(DecArgs<T> a) {
     using S = DecSmem<KT>;
     constexpr int Cp = S::Cp, SW = S::SW, kStep = S::step, kNT = kStep / 8;  // kNT n8 tiles of Y = k8 steps of dX
     extern __shared__ float4 smem4[];
@@ -159,10 +168,10 @@ __global__ void __launch_bounds__(kThreadsA, 1) decoder_kernel(DecArgs a) {
             for (int n = 0; n < kNT; n++) {
                 const int c = co + 8 * n + 2 * t;
                 const bool va = c < Cout, vb = c + 1 < Cout;
-                gv[n][0] = va && ina ? __ldg(a.gt + (size_t)c * N + pa) : 0.f;
-                gv[n][1] = vb && ina ? __ldg(a.gt + (size_t)(c + 1) * N + pa) : 0.f;
-                gv[n][2] = va && inb ? __ldg(a.gt + (size_t)c * N + pb) : 0.f;
-                gv[n][3] = vb && inb ? __ldg(a.gt + (size_t)(c + 1) * N + pb) : 0.f;
+                gv[n][0] = va && ina ? load_f32(a.gt + (size_t)c * N + pa) : 0.f;
+                gv[n][1] = vb && ina ? load_f32(a.gt + (size_t)(c + 1) * N + pa) : 0.f;
+                gv[n][2] = va && inb ? load_f32(a.gt + (size_t)c * N + pb) : 0.f;
+                gv[n][3] = vb && inb ? load_f32(a.gt + (size_t)(c + 1) * N + pb) : 0.f;
             }
         };
         if constexpr (LOSS && S::x_in_regs) load_gt();
@@ -198,12 +207,12 @@ __global__ void __launch_bounds__(kThreadsA, 1) decoder_kernel(DecArgs a) {
             for (int n = 0; n < kNT; n++) {
                 const int c = co + 8 * n + 2 * t;
                 if (c < Cout) {
-                    if (ina) a.y[(size_t)c * N + pa] = yv[n][0];
-                    if (inb) a.y[(size_t)c * N + pb] = yv[n][2];
+                    if (ina) store_f32(a.y + (size_t)c * N + pa, yv[n][0]);
+                    if (inb) store_f32(a.y + (size_t)c * N + pb, yv[n][2]);
                 }
                 if (c + 1 < Cout) {
-                    if (ina) a.y[(size_t)(c + 1) * N + pa] = yv[n][1];
-                    if (inb) a.y[(size_t)(c + 1) * N + pb] = yv[n][3];
+                    if (ina) store_f32(a.y + (size_t)(c + 1) * N + pa, yv[n][1]);
+                    if (inb) store_f32(a.y + (size_t)(c + 1) * N + pb, yv[n][3]);
                 }
             }
         } else {
@@ -416,17 +425,18 @@ Plan make_plan(int Cin, int Cout, int N) {
     return p;
 }
 
-template <int KT, bool LOSS>
-cudaError_t launch_a(const Plan& p, const DecArgs& a, cudaStream_t s) {
+template <int KT, bool LOSS, typename T>
+cudaError_t launch_a(const Plan& p, const DecArgs<T>& a, cudaStream_t s) {
     const size_t smem = DecSmem<KT>::bytes;
-    cudaError_t e = cudaFuncSetAttribute(decoder_kernel<KT, LOSS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    cudaError_t e =
+        cudaFuncSetAttribute(decoder_kernel<KT, LOSS, T>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return e;
-    decoder_kernel<KT, LOSS><<<p.gridA, kThreadsA, smem, s>>>(a);
+    decoder_kernel<KT, LOSS, T><<<p.gridA, kThreadsA, smem, s>>>(a);
     return cudaGetLastError();
 }
 
-template <bool LOSS>
-cudaError_t launch_a_kt(const Plan& p, const DecArgs& a, cudaStream_t s) {
+template <bool LOSS, typename T>
+cudaError_t launch_a_kt(const Plan& p, const DecArgs<T>& a, cudaStream_t s) {
     switch (p.KT) {
         case 4: return launch_a<4, LOSS>(p, a, s);
         case 8: return launch_a<8, LOSS>(p, a, s);
@@ -456,8 +466,9 @@ struct Scratch {
     }
 };
 
-cudaError_t decoder_run(int Cin, int Cout, int N, const float* weight, const float* bias, const float* x, const float* gt,
-                        float grad_scale, float* y, float* loss_sum, float* dx, float* dW, float* db, cudaStream_t s) {
+template <typename T>
+cudaError_t decoder_run(int Cin, int Cout, int N, const float* weight, const float* bias, const float* x, const T* gt,
+                        float grad_scale, T* y, float* loss_sum, float* dx, float* dW, float* db, cudaStream_t s) {
     if (!decoder_grid_ok(Cin, Cout, N)) return cudaErrorInvalidValue;
     const bool loss = gt != nullptr;
     const Plan p = make_plan(Cin, Cout, N);
@@ -465,7 +476,7 @@ cudaError_t decoder_run(int Cin, int Cout, int N, const float* weight, const flo
     char* ws = nullptr;
     cudaError_t e = cudaMallocAsync((void**)&ws, sc.bytes, s);
     if (e != cudaSuccess) return e;
-    DecArgs a;
+    DecArgs<T> a;
     a.Cin = Cin; a.Cout = Cout; a.N = N; a.N16 = p.N16;
     a.wt = reinterpret_cast<float*>(ws + sc.off_wt);
     a.bias = reinterpret_cast<float*>(ws + sc.off_bp);
@@ -509,13 +520,24 @@ bool decoder_grid_ok(int Cin, int Cout, int N) {
 
 cudaError_t launch_decoder_forward(int Cin, int Cout, int N, const float* weight, const float* bias, const float* x,
                                    float* y, cudaStream_t s) {
-    return decoder_run(Cin, Cout, N, weight, bias, x, nullptr, 0.f, y, nullptr, nullptr, nullptr, nullptr, s);
+    return decoder_run<float>(Cin, Cout, N, weight, bias, x, nullptr, 0.f, y, nullptr, nullptr, nullptr, nullptr, s);
+}
+
+cudaError_t launch_decoder_forward(int Cin, int Cout, int N, const float* weight, const float* bias, const float* x,
+                                   __half* y, cudaStream_t s) {
+    return decoder_run<__half>(Cin, Cout, N, weight, bias, x, nullptr, 0.f, y, nullptr, nullptr, nullptr, nullptr, s);
 }
 
 cudaError_t launch_decoder_l1(int Cin, int Cout, int N, const float* weight, const float* bias, const float* x,
                               const float* gt, float grad_scale, float* loss_sum, float* dx, float* dW, float* db,
                               cudaStream_t s) {
-    return decoder_run(Cin, Cout, N, weight, bias, x, gt, grad_scale, nullptr, loss_sum, dx, dW, db, s);
+    return decoder_run<float>(Cin, Cout, N, weight, bias, x, gt, grad_scale, nullptr, loss_sum, dx, dW, db, s);
+}
+
+cudaError_t launch_decoder_l1(int Cin, int Cout, int N, const float* weight, const float* bias, const float* x,
+                              const __half* gt, float grad_scale, float* loss_sum, float* dx, float* dW, float* db,
+                              cudaStream_t s) {
+    return decoder_run<__half>(Cin, Cout, N, weight, bias, x, gt, grad_scale, nullptr, loss_sum, dx, dW, db, s);
 }
 
 }  // namespace f3dgs

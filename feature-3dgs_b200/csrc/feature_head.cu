@@ -14,6 +14,9 @@
 //                  footprint covers it -- every element written exactly once, no atomics, no zero fill.
 // Sampling positions follow ATen's upsample_bilinear2d with align_corners=True: src = dst * (in - 1) / (out - 1),
 // i0 = (int)src, i1 = i0 + (i0 < in - 1), lambda1 = src - i0.
+// The target may be float32 or float16 (the data format's teacher maps); a float16 element is upcast exactly at its load,
+// so the result equals that of the float32 target gt.float().
+#include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
 
@@ -39,14 +42,18 @@ __device__ __forceinline__ void src_of(int o, float r, int in, int& i0, int& i1,
     l0 = 1.0f - l1;
 }
 
+__device__ __forceinline__ float load_f32(const float* p) { return __ldg(p); }
+__device__ __forceinline__ float load_f32(const __half* p) { return __half2float(__ldg(p)); }
+
 // One warp per output row (c, oy) at a time, lanes strided over ox: the row's channel plane and y taps are computed once per
 // row (no per-element division), a lane's loads are independent across its elements, and consecutive lanes read source
 // columns (in - 1) / (out - 1) apart -- neighbouring sectors.  A persistent grid, so that the loss needs one atomic per CTA
 // (200 K same-address atomics cost more than the whole resize).
 constexpr int kFwdThreads = 256;
 
+template <typename GT>  // float or __half
 __global__ void __launch_bounds__(kFwdThreads) resize_fwd_kernel(ResizeGeom g, const float* __restrict__ fm,
-                                                                 const float* __restrict__ gt, float grad_scale,
+                                                                 const GT* __restrict__ gt, float grad_scale,
                                                                  float* __restrict__ out, float* __restrict__ loss_sum) {
     const int lane = threadIdx.x & 31;
     const int warps = gridDim.x * (kFwdThreads / 32);
@@ -67,7 +74,7 @@ __global__ void __launch_bounds__(kFwdThreads) resize_fwd_kernel(ResizeGeom g, c
             src_of(ox, g.rx, g.W, x0, x1, lx0, lx1);
             const float v = ly0 * (lx0 * __ldg(p0 + x0) + lx1 * __ldg(p0 + x1)) + ly1 * (lx0 * __ldg(p1 + x0) + lx1 * __ldg(p1 + x1));
             if (gt != nullptr) {
-                const float d = v - __ldg(gt + obase + ox);
+                const float d = v - load_f32(gt + obase + ox);
                 ad += fabsf(d);
                 out[obase + ox] = d > 0.f ? grad_scale : (d < 0.f ? -grad_scale : 0.f);
             } else {
@@ -259,10 +266,9 @@ ResizeGeom make_geom(int C, int H, int W, int Hg, int Wg) {
     return g;
 }
 
-}  // namespace
-
-cudaError_t launch_feature_resize_fwd(int C, int H, int W, int Hg, int Wg, const float* fm, const float* gt,
-                                      float grad_scale, float* out, float* loss_sum, cudaStream_t s) {
+template <typename GT>
+cudaError_t resize_fwd(int C, int H, int W, int Hg, int Wg, const float* fm, const GT* gt, float grad_scale, float* out,
+                       float* loss_sum, cudaStream_t s) {
     const size_t n = (size_t)C * Hg * Wg;
     if (n == 0) return cudaSuccess;
     int dev = 0, sms = 132;
@@ -271,9 +277,21 @@ cudaError_t launch_feature_resize_fwd(int C, int H, int W, int Hg, int Wg, const
     const size_t rows = (size_t)C * Hg;
     if (rows > 0x7fffffffu) return cudaErrorInvalidValue;
     const unsigned grid = (unsigned)std::min<size_t>((rows + kFwdThreads / 32 - 1) / (kFwdThreads / 32), (size_t)sms * 8);
-    resize_fwd_kernel<<<grid, kFwdThreads, 0, s>>>(make_geom(C, H, W, Hg, Wg), fm, gt, grad_scale, out, loss_sum);
+    resize_fwd_kernel<GT><<<grid, kFwdThreads, 0, s>>>(make_geom(C, H, W, Hg, Wg), fm, gt, grad_scale, out, loss_sum);
     g_launches++;
     return cudaGetLastError();
+}
+
+}  // namespace
+
+cudaError_t launch_feature_resize_fwd(int C, int H, int W, int Hg, int Wg, const float* fm, const float* gt,
+                                      float grad_scale, float* out, float* loss_sum, cudaStream_t s) {
+    return resize_fwd(C, H, W, Hg, Wg, fm, gt, grad_scale, out, loss_sum, s);
+}
+
+cudaError_t launch_feature_resize_fwd(int C, int H, int W, int Hg, int Wg, const float* fm, const __half* gt,
+                                      float grad_scale, float* out, float* loss_sum, cudaStream_t s) {
+    return resize_fwd(C, H, W, Hg, Wg, fm, gt, grad_scale, out, loss_sum, s);
 }
 
 cudaError_t launch_feature_resize_bwd(int C, int H, int W, int Hg, int Wg, const float* dout, float* dfm, cudaStream_t s) {

@@ -1,5 +1,6 @@
 // Internal launch interface between the C-ABI orchestration (api.cu) and the kernel TUs.
 #pragma once
+#include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
 
@@ -66,8 +67,10 @@ cudaError_t launch_feature_bwd(const ViewParams& vp, const uint2* ranges, const 
                                const uint32_t* list_cnt, const float* dL_dfeat_pix, float* dL_dfeature,
                                int* work_counter, cudaStream_t s);
 
-// ---- feature_head.cu
+// ---- feature_head.cu (a float16 target gives the result of the float32 one upcast exactly)
 cudaError_t launch_feature_resize_fwd(int C, int H, int W, int Hg, int Wg, const float* fm, const float* gt,
+                                      float grad_scale, float* out, float* loss_sum, cudaStream_t s);
+cudaError_t launch_feature_resize_fwd(int C, int H, int W, int Hg, int Wg, const float* fm, const __half* gt,
                                       float grad_scale, float* out, float* loss_sum, cudaStream_t s);
 cudaError_t launch_feature_resize_bwd(int C, int H, int W, int Hg, int Wg, const float* dout, float* dfm, cudaStream_t s);
 
@@ -79,10 +82,16 @@ cudaError_t launch_image_loss(int planes, int H, int W, const float* image, cons
 // ---- feature_decoder.cu: 1x1-conv decoder y = W x + b, and its L1 loss with dL/dx (written), dL/dW and dL/db (added)
 constexpr int kDecoderMaxCin = 256, kDecoderMaxCout = 4096;
 bool decoder_grid_ok(int Cin, int Cout, int N);  // sizes in range and the launch grids fit CUDA's limits
+// y may be float16 (rounded to nearest even, as torch's .half()); a float16 gt is upcast exactly
 cudaError_t launch_decoder_forward(int Cin, int Cout, int N, const float* weight, const float* bias, const float* x,
                                    float* y, cudaStream_t s);
+cudaError_t launch_decoder_forward(int Cin, int Cout, int N, const float* weight, const float* bias, const float* x,
+                                   __half* y, cudaStream_t s);
 cudaError_t launch_decoder_l1(int Cin, int Cout, int N, const float* weight, const float* bias, const float* x,
                               const float* gt, float grad_scale, float* loss_sum, float* dx, float* dW, float* db,
+                              cudaStream_t s);
+cudaError_t launch_decoder_l1(int Cin, int Cout, int N, const float* weight, const float* bias, const float* x,
+                              const __half* gt, float grad_scale, float* loss_sum, float* dx, float* dW, float* db,
                               cudaStream_t s);
 
 // ---- knn.cu: exact mean squared distance to the 3 nearest other points (distCUDA2); scratch is knn_scratch_bytes(P)

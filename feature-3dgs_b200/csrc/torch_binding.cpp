@@ -249,6 +249,15 @@ torch::Tensor markVisible(torch::Tensor& means3D, torch::Tensor& viewmatrix, tor
 }
 
 // ---- post-raster feature head (include/f3dgs_b200.h: f3dgs_feature_resize_fwd / _bwd) ----------------------------
+namespace {
+// a teacher map may be float32 or float16 (the data format's dtype; the float16 symbols upcast it exactly in the kernel)
+bool is_target_dtype(const torch::Tensor& t) {
+    return t.scalar_type() == torch::kFloat32 || t.scalar_type() == torch::kFloat16;
+}
+
+const uint16_t* hptr(const torch::Tensor& t) { return reinterpret_cast<const uint16_t*>(t.data_ptr<at::Half>()); }
+}  // namespace
+
 // -> (out [C,Hg,Wg], loss_sum [1]); with gt: out = sign(resized - gt) * grad_scale and loss_sum = sum |resized - gt|
 std::tuple<torch::Tensor, torch::Tensor> featureResizeFwd(const torch::Tensor& feature_map, const torch::Tensor& gt,
                                                           int64_t Hg, int64_t Wg, double grad_scale) {
@@ -258,18 +267,24 @@ std::tuple<torch::Tensor, torch::Tensor> featureResizeFwd(const torch::Tensor& f
     auto fm = feature_map.contiguous();
     const int C = fm.size(0), H = fm.size(1), W = fm.size(2);
     const bool has_gt = gt.defined() && gt.numel() > 0;
+    const bool half_gt = has_gt && gt.scalar_type() == torch::kFloat16;
     torch::Tensor g;
     if (has_gt) {
-        TORCH_CHECK(gt.is_cuda() && gt.scalar_type() == torch::kFloat32 && gt.dim() == 3 && gt.size(0) == C &&
-                        gt.size(1) == Hg && gt.size(2) == Wg, "gt must be a float32 CUDA tensor [C,Hg,Wg]");
+        TORCH_CHECK(gt.is_cuda() && is_target_dtype(gt) && gt.dim() == 3 && gt.size(0) == C && gt.size(1) == Hg &&
+                        gt.size(2) == Wg, "gt must be a float32 or float16 CUDA tensor [C,Hg,Wg]");
         g = gt.contiguous();
     }
     torch::Tensor out = torch::empty({C, Hg, Wg}, fm.options());
     torch::Tensor loss = torch::zeros({1}, fm.options());
     cudaStream_t stream = c10::cuda::getCurrentCUDAStream().stream();
-    check_rc(f3dgs_feature_resize_fwd(C, H, W, (int)Hg, (int)Wg, fptr(fm), has_gt ? fptr(g) : nullptr, (float)grad_scale,
-                                      out.data_ptr<float>(), loss.data_ptr<float>(), (void*)stream),
-             "f3dgs_feature_resize_fwd");
+    if (half_gt)
+        check_rc(f3dgs_feature_resize_fwd_f16gt(C, H, W, (int)Hg, (int)Wg, fptr(fm), hptr(g), (float)grad_scale,
+                                                out.data_ptr<float>(), loss.data_ptr<float>(), (void*)stream),
+                 "f3dgs_feature_resize_fwd_f16gt");
+    else
+        check_rc(f3dgs_feature_resize_fwd(C, H, W, (int)Hg, (int)Wg, fptr(fm), has_gt ? fptr(g) : nullptr,
+                                          (float)grad_scale, out.data_ptr<float>(), loss.data_ptr<float>(), (void*)stream),
+                 "f3dgs_feature_resize_fwd");
     return std::make_tuple(out, loss);
 }
 
@@ -347,16 +362,24 @@ void check_accum(const torch::Tensor& t, const torch::Device& dev, int64_t numel
 }
 }  // namespace
 
-// -> y [Cout, <x's spatial shape>]
-torch::Tensor decoderForward(const torch::Tensor& x, const torch::Tensor& weight, const torch::Tensor& bias) {
+// -> y [Cout, <x's spatial shape>] of dtype float32, or float16 (rounded to nearest even, as y.half())
+torch::Tensor decoderForward(const torch::Tensor& x, const torch::Tensor& weight, const torch::Tensor& bias,
+                             torch::ScalarType dtype) {
+    TORCH_CHECK(dtype == torch::kFloat32 || dtype == torch::kFloat16, "decoder_forward: dtype must be float32 or float16");
     auto d = decoder_inputs(x, weight, bias);
     const c10::cuda::CUDAGuard guard(x.device());
     auto shape = d.x.sizes().vec();
     shape[0] = d.Cout;
-    torch::Tensor y = torch::empty(shape, d.x.options());
+    torch::Tensor y = torch::empty(shape, d.x.options().dtype(dtype));
     cudaStream_t stream = c10::cuda::getCurrentCUDAStream().stream();
-    check_rc(f3dgs_decoder_forward(d.Cin, d.Cout, d.N, fptr(d.w), fptr(d.b), fptr(d.x), y.data_ptr<float>(), (void*)stream),
-             "f3dgs_decoder_forward");
+    if (dtype == torch::kFloat16)
+        check_rc(f3dgs_decoder_forward_f16(d.Cin, d.Cout, d.N, fptr(d.w), fptr(d.b), fptr(d.x),
+                                           reinterpret_cast<uint16_t*>(y.data_ptr<at::Half>()), (void*)stream),
+                 "f3dgs_decoder_forward_f16");
+    else
+        check_rc(f3dgs_decoder_forward(d.Cin, d.Cout, d.N, fptr(d.w), fptr(d.b), fptr(d.x), y.data_ptr<float>(),
+                                       (void*)stream),
+                 "f3dgs_decoder_forward");
     return y;
 }
 
@@ -367,9 +390,9 @@ std::tuple<torch::Tensor, torch::Tensor> decoderL1(const torch::Tensor& x, const
     auto d = decoder_inputs(x, weight, bias);
     const auto dev = x.device();
     const c10::cuda::CUDAGuard guard(dev);
-    TORCH_CHECK(gt.device() == dev && gt.scalar_type() == torch::kFloat32 && gt.dim() == d.x.dim() && gt.size(0) == d.Cout &&
+    TORCH_CHECK(gt.device() == dev && is_target_dtype(gt) && gt.dim() == d.x.dim() && gt.size(0) == d.Cout &&
                     gt.numel() == (int64_t)d.Cout * d.N && gt.sizes().slice(1) == d.x.sizes().slice(1),
-                "gt must be a float32 tensor [Cout, <x's spatial shape>] on ", dev);
+                "gt must be a float32 or float16 tensor [Cout, <x's spatial shape>] on ", dev);
     auto g = gt.contiguous();
     check_accum(dweight, dev, (int64_t)d.Cout * d.Cin, "dweight");
     if (d.b.defined()) check_accum(dbias, dev, d.Cout, "dbias");
@@ -377,10 +400,17 @@ std::tuple<torch::Tensor, torch::Tensor> decoderL1(const torch::Tensor& x, const
     torch::Tensor loss = torch::empty({1}, d.x.options());
     torch::Tensor dx = torch::empty_like(d.x);
     cudaStream_t stream = c10::cuda::getCurrentCUDAStream().stream();
-    check_rc(f3dgs_decoder_l1(d.Cin, d.Cout, d.N, fptr(d.w), fptr(d.b), fptr(d.x), fptr(g), (float)grad_scale,
-                              loss.data_ptr<float>(), dx.data_ptr<float>(), dweight.data_ptr<float>(),
-                              d.b.defined() ? dbias.data_ptr<float>() : nullptr, (void*)stream),
-             "f3dgs_decoder_l1");
+    float* db = d.b.defined() ? dbias.data_ptr<float>() : nullptr;
+    if (g.scalar_type() == torch::kFloat16)
+        check_rc(f3dgs_decoder_l1_f16gt(d.Cin, d.Cout, d.N, fptr(d.w), fptr(d.b), fptr(d.x), hptr(g), (float)grad_scale,
+                                        loss.data_ptr<float>(), dx.data_ptr<float>(), dweight.data_ptr<float>(), db,
+                                        (void*)stream),
+                 "f3dgs_decoder_l1_f16gt");
+    else
+        check_rc(f3dgs_decoder_l1(d.Cin, d.Cout, d.N, fptr(d.w), fptr(d.b), fptr(d.x), fptr(g), (float)grad_scale,
+                                  loss.data_ptr<float>(), dx.data_ptr<float>(), dweight.data_ptr<float>(), db,
+                                  (void*)stream),
+                 "f3dgs_decoder_l1");
     return std::make_tuple(loss, dx);
 }
 
@@ -467,7 +497,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     m.def("feature_resize_fwd", &featureResizeFwd);
     m.def("feature_resize_bwd", &featureResizeBwd);
     m.def("image_loss", &imageLoss);
-    m.def("decoder_forward", &decoderForward);
+    m.def("decoder_forward", &decoderForward, pybind11::arg("x"), pybind11::arg("weight"), pybind11::arg("bias"),
+          pybind11::arg("dtype") = torch::kFloat32);
     m.def("decoder_l1", &decoderL1);
     m.def("knn_mean_dist", &knnMeanDist);
     m.def("activate", &activateParams);

@@ -9,6 +9,10 @@ and dL/d(resized map), and a gather-style resize backward that writes every elem
 With --speedup the 1x1 decoder and its loss run in between on csrc/feature_decoder.cu (TF32 tensor cores, like cuDNN's
 default for the reference's nn.Conv2d): `decode`, `decoded_feature_l1_loss_and_grad`, `decoded_feature_l1_loss`.
 There is no CPU path (the extension raises on CPU tensors).
+
+The teacher map `gt` may be float32 or float16, the dtype the data format stores it in (io.load_feature_map(path,
+dtype=None)).  A float16 map is read as it is and upcast exactly inside the kernels, so no float32 copy is made and every
+result equals the one for `gt.float()`; the loss and the gradients are float32, as PyTorch's `l1_loss(fp32, fp16)` gives.
 """
 import torch
 
@@ -68,11 +72,12 @@ def _empty(like: torch.Tensor) -> torch.Tensor:
     return torch.empty(0, device=like.device, dtype=like.dtype)
 
 
-def decode(feature_map: torch.Tensor, weight: torch.Tensor, bias=None) -> torch.Tensor:
+def decode(feature_map: torch.Tensor, weight: torch.Tensor, bias=None, dtype=torch.float32) -> torch.Tensor:
     """The reference's `cnn_decoder(feature_map)` (nn.Conv2d(Cin, Cout, 1)) without a graph: feature_map [Cin,H,W],
-    weight [Cout,Cin,1,1] or [Cout,Cin], bias [Cout] or None -> [Cout,H,W]."""
+    weight [Cout,Cin,1,1] or [Cout,Cin], bias [Cout] or None -> [Cout,H,W].  dtype=torch.float16 writes the map the way
+    render.py saves it, bitwise `decode(...).half()` without the float32 map or the cast pass."""
     with torch.no_grad():
-        return _C().decoder_forward(feature_map, weight, _empty(feature_map) if bias is None else bias)
+        return _C().decoder_forward(feature_map, weight, _empty(feature_map) if bias is None else bias, dtype)
 
 
 def decoded_feature_l1_loss_and_grad(feature_map: torch.Tensor, gt: torch.Tensor, weight: torch.Tensor, bias=None,

@@ -136,11 +136,13 @@ def save_feature_map(path: str, feature_map):
     torch.save(t.detach().to("cpu", torch.float16).contiguous(), path)
 
 
-def load_feature_map(path: str, device="cpu"):
-    """-> float32 [C,H,W] (scene/dataset_readers.py:110-112 loads the tensor and the trainer moves it to the GPU)."""
+def load_feature_map(path: str, device="cpu", dtype="float32"):
+    """-> [C,H,W] (scene/dataset_readers.py:110-112 loads the tensor and the trainer moves it to the GPU), float32 by
+    default; dtype=None keeps the stored dtype (float16 as save_feature_map writes it), which the feature losses of
+    feature_head take as it is, at half the memory.  (The default is spelt as a string because torch is imported lazily.)"""
     import torch
 
     t = torch.load(path, map_location="cpu")
     if t.dim() != 3:
         raise ValueError(f"{path}: expected a [C,H,W] tensor, got {tuple(t.shape)}")
-    return t.to(device=device, dtype=torch.float32)
+    return t.to(device=device, dtype=torch.float32 if dtype == "float32" else dtype)

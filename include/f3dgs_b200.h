@@ -19,7 +19,8 @@
  *   - errors are returned as negative codes with a message in f3dgs_last_error() instead of C++
  *     exceptions (reference: std::runtime_error from CHECK_CUDA, auxiliary.h:172-179).
  *
- * All float tensors are fp32, contiguous, device memory.  Matrices are the 16 floats of the
+ * All float tensors are fp32 (except where a symbol's _f16 / _f16gt suffix says float16), contiguous, device
+ * memory.  Matrices are the 16 floats of the
  * reference's row-major [4,4] torch tensors, i.e. column-major for the kernels
  * (auxiliary.h:58-77).  An absent optional input is a NULL pointer
  * (rasterize_points.cu: empty tensor -> nullptr).
@@ -150,6 +151,11 @@ int f3dgs_feature_resize_fwd(int C, int H, int W, int Hg, int Wg, const float* f
                              float grad_scale, float* out, float* loss_sum, void* cuda_stream);
 int f3dgs_feature_resize_bwd(int C, int H, int W, int Hg, int Wg, const float* dout, float* dL_dfeature_map,
                              void* cuda_stream);
+/* f3dgs_feature_resize_fwd with a float16 teacher map (the data format's <name>_fmap_CxHxW.pt): gt [C,Hg,Wg] holds IEEE
+ * binary16 bits and is required.  The result is that of f3dgs_feature_resize_fwd applied to the exactly upcast float32
+ * target.  It validates as its float32 twin does, and also rejects an `out` that overlaps feature_map or gt. */
+int f3dgs_feature_resize_fwd_f16gt(int C, int H, int W, int Hg, int Wg, const float* feature_map, const uint16_t* gt,
+                                   float grad_scale, float* out, float* loss_sum, void* cuda_stream);
 
 /* ---- feature decoder (--speedup): models/networks.py:107-119 CNN_decoder, nn.Conv2d(Cin, Cout, kernel_size=1) -------
  * x [Cin,N] (the resized map, N = Hg*Wg), weight [Cout,Cin] (the conv weight [Cout,Cin,1,1] as contiguous memory),
@@ -167,6 +173,16 @@ int f3dgs_decoder_forward(int Cin, int Cout, int N, const float* weight, const f
 int f3dgs_decoder_l1(int Cin, int Cout, int N, const float* weight, const float* bias, const float* x, const float* gt,
                      float grad_scale, float* loss_sum, float* dL_dx, float* dL_dweight, float* dL_dbias,
                      void* cuda_stream);
+/* float16 variants; half data is IEEE binary16 bits in uint16_t, and overlap checks use its 2-byte size.
+ *   f3dgs_decoder_l1_f16gt    gt [Cout,N] float16.  The result is that of f3dgs_decoder_l1 applied to the exactly upcast
+ *                             float32 target (bitwise, like the float32 call itself).  Validates as f3dgs_decoder_l1.
+ *   f3dgs_decoder_forward_f16 y [Cout,N] float16: the y of f3dgs_decoder_forward rounded to nearest even (torch's
+ *                             .half(): +-inf beyond 65504).  Validates as f3dgs_decoder_forward. */
+int f3dgs_decoder_l1_f16gt(int Cin, int Cout, int N, const float* weight, const float* bias, const float* x,
+                           const uint16_t* gt, float grad_scale, float* loss_sum, float* dL_dx, float* dL_dweight,
+                           float* dL_dbias, void* cuda_stream);
+int f3dgs_decoder_forward_f16(int Cin, int Cout, int N, const float* weight, const float* bias, const float* x,
+                              uint16_t* y, void* cuda_stream);
 
 /* ---- photometric loss: reference train.py (colour term), utils/loss_utils.py l1_loss + ssim(window_size=11) ---------
  * loss = (1 - lambda_dssim) * l1_loss(image, gt) + lambda_dssim * (1 - ssim(image, gt)).  image, gt [planes,H,W]; the
