@@ -693,6 +693,84 @@ int f3dgs_knn_mean_dist(int P, const float* points, float* out, char* scratch, v
     return 0;
 }
 
+size_t f3dgs_densify_scratch_bytes(int P) {
+    t_error.clear();
+    size_t bytes = 0;
+    const cudaError_t e = densify_scratch_bytes(P, &bytes);
+    if (e != cudaSuccess) {
+        fail(F3DGS_ERR_CUDA, std::string("f3dgs_densify_scratch_bytes: ") + cudaGetErrorString(e));
+        return 0;
+    }
+    return bytes;
+}
+
+int f3dgs_densify_plan(int P, const float* grad_accum, const float* denom, const float* raw_opacity,
+                       const float* raw_scaling, float max_grad, float dense_scale, float min_opacity,
+                       float max_world_scale, char* scratch, int32_t* counts, void* cuda_stream) {
+    t_error.clear();
+    if (P < 0 || 3 * (long long)P > INT_MAX)
+        return fail(F3DGS_ERR_INVALID_ARGUMENT, "f3dgs_densify_plan: bad sizes (0 <= 3 P <= INT_MAX)");
+    if (!counts || (P > 0 && (!grad_accum || !denom || !raw_opacity || !raw_scaling || !scratch)))
+        return fail(F3DGS_ERR_INVALID_ARGUMENT, "f3dgs_densify_plan: NULL pointer");
+    if (ranges_overlap(counts, 16, scratch, densify_scratch_fixed_bytes(P)))
+        return fail(F3DGS_ERR_INVALID_ARGUMENT, "f3dgs_densify_plan: counts overlaps scratch");
+    cudaError_t e = launch_densify_plan(P, grad_accum, denom, raw_opacity, raw_scaling, max_grad, dense_scale,
+                                        min_opacity, max_world_scale, scratch, counts, (cudaStream_t)cuda_stream);
+    if (e != cudaSuccess) return fail(F3DGS_ERR_CUDA, std::string("densify_plan: ") + cudaGetErrorString(e));
+    return 0;
+}
+
+int f3dgs_densify_apply(int P, int M, int C, const char* scratch, const int32_t counts[4], const float* normals,
+                        const f3dgs_gaussian_fields src[3], const f3dgs_gaussian_fields dst[3], void* cuda_stream) {
+    t_error.clear();
+    if (P < 0 || 3 * (long long)P > INT_MAX || M < 1 || C < 0 || C > F3DGS_MAX_FEATURE_DIM)
+        return fail(F3DGS_ERR_INVALID_ARGUMENT,
+                    "f3dgs_densify_apply: bad sizes (0 <= 3 P <= INT_MAX, M >= 1, 0 <= C <= F3DGS_MAX_FEATURE_DIM)");
+    if (!counts || !src || !dst) return fail(F3DGS_ERR_INVALID_ARGUMENT, "f3dgs_densify_apply: NULL pointer");
+    const long long A = counts[0], B = counts[1], Cc = counts[2], Ns = counts[3], Pn = A + B + 2 * Cc;
+    if (A < 0 || B < 0 || Cc < 0 || A > P || B > P || Cc > Ns || Ns > P || 3 * Pn > INT_MAX)
+        return fail(F3DGS_ERR_INVALID_ARGUMENT, "f3dgs_densify_apply: counts are not those of a plan over P Gaussians");
+    if (Ns > 0 && !normals) return fail(F3DGS_ERR_INVALID_ARGUMENT, "f3dgs_densify_apply: NULL pointer (normals)");
+    if (P > 0 && !scratch) return fail(F3DGS_ERR_INVALID_ARGUMENT, "f3dgs_densify_apply: NULL pointer (scratch)");
+    const size_t width[7] = {3, 3, 3 * (size_t)(M - 1), 1, 3, 4, (size_t)C};
+    const float* s[21];
+    float* d[21];
+    for (int g = 0; g < 3; g++) {
+        const f3dgs_gaussian_fields* f[2] = {&src[g], &dst[g]};
+        for (int k = 0; k < 2; k++) {
+            const float* p[7] = {f[k]->xyz, f[k]->f_dc, f[k]->f_rest, f[k]->opacity, f[k]->scaling, f[k]->rotation,
+                                 f[k]->semantic_feature};
+            for (int j = 0; j < 7; j++) {
+                if (width[j] && (k ? Pn : P) > 0 && !p[j])
+                    return fail(F3DGS_ERR_INVALID_ARGUMENT, "f3dgs_densify_apply: NULL pointer (a src or dst field)");
+                if (k) d[7 * g + j] = const_cast<float*>(p[j]);
+                else s[7 * g + j] = p[j];
+            }
+        }
+    }
+    for (int i = 0; i < 21; i++) {
+        const size_t nd = (size_t)Pn * width[i % 7] * 4;
+        bool bad = ranges_overlap(d[i], nd, scratch, densify_scratch_fixed_bytes(P)) ||
+                   ranges_overlap(d[i], nd, normals, (size_t)Ns * 24);
+        for (int j = 0; j < 21 && !bad; j++) bad = ranges_overlap(d[i], nd, s[j], (size_t)P * width[j % 7] * 4);
+        if (bad)
+            return fail(F3DGS_ERR_INVALID_ARGUMENT, "f3dgs_densify_apply: a dst field overlaps a src field, normals or scratch");
+    }
+    cudaError_t e = launch_densify_apply(P, M, C, scratch, counts, normals, s, d, (cudaStream_t)cuda_stream);
+    if (e != cudaSuccess) return fail(F3DGS_ERR_CUDA, std::string("densify_apply: ") + cudaGetErrorString(e));
+    return 0;
+}
+
+int f3dgs_reset_opacity(int P, float* raw_opacity, float* exp_avg, float* exp_avg_sq, float ceiling, void* cuda_stream) {
+    t_error.clear();
+    if (P < 0) return fail(F3DGS_ERR_INVALID_ARGUMENT, "f3dgs_reset_opacity: P < 0");
+    if (P == 0) return 0;
+    if (!raw_opacity || !exp_avg || !exp_avg_sq) return fail(F3DGS_ERR_INVALID_ARGUMENT, "f3dgs_reset_opacity: NULL pointer");
+    cudaError_t e = launch_reset_opacity(P, raw_opacity, exp_avg, exp_avg_sq, ceiling, (cudaStream_t)cuda_stream);
+    if (e != cudaSuccess) return fail(F3DGS_ERR_CUDA, std::string("reset_opacity: ") + cudaGetErrorString(e));
+    return 0;
+}
+
 int f3dgs_mark_visible(int P, const float* means3D, const float* viewmatrix, const float* projmatrix,
                        uint8_t* present, void* cuda_stream) {
     (void)projmatrix;  // the reference's frustum side test is commented out (auxiliary.h:160)

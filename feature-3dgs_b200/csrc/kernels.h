@@ -100,4 +100,17 @@ cudaError_t knn_scratch_bytes(int P, size_t* bytes);
 size_t knn_scratch_fixed_bytes(int P);
 cudaError_t launch_knn_mean_dist(int P, const float* points, float* out, char* scratch, cudaStream_t s);
 
+// ---- densify.cu: clone / split / prune (densify_and_prune) and reset_opacity.  scratch is densify_scratch_bytes(P)
+// bytes whose first densify_scratch_fixed_bytes(P) (the scanned per-Gaussian flags apply reads) need no device query;
+// src / dst are the 21 fields of f3dgs_gaussian_fields[3] in order
+cudaError_t densify_scratch_bytes(int P, size_t* bytes);
+size_t densify_scratch_fixed_bytes(int P);
+cudaError_t launch_densify_plan(int P, const float* grad_accum, const float* denom, const float* raw_opacity,
+                                const float* raw_scaling, float max_grad, float dense_scale, float min_opacity,
+                                float max_world_scale, char* scratch, int32_t* counts, cudaStream_t s);
+cudaError_t launch_densify_apply(int P, int M, int C, const char* scratch, const int32_t counts[4], const float* normals,
+                                 const float* const src[21], float* const dst[21], cudaStream_t s);
+cudaError_t launch_reset_opacity(int P, float* raw_opacity, float* exp_avg, float* exp_avg_sq, float ceiling,
+                                 cudaStream_t s);
+
 }  // namespace f3dgs

@@ -435,6 +435,91 @@ torch::Tensor knnMeanDist(const torch::Tensor& points) {
     return out;
 }
 
+// ---- densification (f3dgs_densify_plan / f3dgs_densify_apply / f3dgs_reset_opacity)
+void check_f32(const torch::Tensor& t, const torch::Device& dev, int64_t numel, const char* what) {
+    TORCH_CHECK(t.is_cuda() && t.device() == dev && t.scalar_type() == torch::kFloat32 && t.is_contiguous(), what,
+                " must be a contiguous float32 tensor on ", dev);
+    TORCH_CHECK(t.numel() == numel, what, ": expected ", numel, " elements, got ", t.numel());
+}
+
+// -> (scratch, counts): counts = device int32[4] {originals kept, clones kept, children kept per copy, split}
+std::tuple<torch::Tensor, torch::Tensor> densifyPlan(const torch::Tensor& grad_accum, const torch::Tensor& denom,
+                                                     const torch::Tensor& raw_opacity, const torch::Tensor& raw_scaling,
+                                                     double max_grad, double dense_scale, double min_opacity,
+                                                     double max_world_scale) {
+    TORCH_CHECK(raw_scaling.is_cuda(), "parameters must be CUDA tensors (this build has no CPU path)");
+    TORCH_CHECK(raw_scaling.dim() == 2 && raw_scaling.size(1) == 3, "raw_scaling must be [P,3]");
+    TORCH_CHECK(raw_scaling.size(0) <= INT32_MAX / 3, "densify: 3 P must be below 2^31");
+    const c10::cuda::CUDAGuard guard(raw_scaling.device());
+    const auto dev = raw_scaling.device();
+    const int P = (int)raw_scaling.size(0);
+    auto ga = grad_accum.contiguous(), dn = denom.contiguous();
+    check_f32(ga, dev, P, "grad_accum");
+    check_f32(dn, dev, P, "denom");
+    check_f32(raw_opacity, dev, P, "raw_opacity");
+    check_f32(raw_scaling, dev, 3 * (int64_t)P, "raw_scaling");
+    const size_t bytes = f3dgs_densify_scratch_bytes(P);
+    TORCH_CHECK(P == 0 || bytes > 0, "f3dgs_densify_scratch_bytes failed: ", f3dgs_last_error());
+    torch::Tensor scratch = torch::empty({(int64_t)bytes}, raw_scaling.options().dtype(torch::kByte));
+    torch::Tensor counts = torch::empty({4}, raw_scaling.options().dtype(torch::kInt32));
+    cudaStream_t stream = c10::cuda::getCurrentCUDAStream().stream();
+    check_rc(f3dgs_densify_plan(P, fptr(ga), fptr(dn), fptr(raw_opacity), fptr(raw_scaling), (float)max_grad,
+                                (float)dense_scale, (float)min_opacity, (float)max_world_scale,
+                                bytes ? reinterpret_cast<char*>(scratch.data_ptr()) : nullptr, counts.data_ptr<int32_t>(),
+                                (void*)stream),
+             "f3dgs_densify_plan");
+    return std::make_tuple(scratch, counts);
+}
+
+// src / dst: the 21 tensors raw (xyz, f_dc, f_rest, opacity, scaling, rotation, semantic_feature), exp_avg, exp_avg_sq;
+// counts: the host copy of densify_plan's counts; dst is written (P' = A + B + 2 Cc rows)
+void densifyApply(const torch::Tensor& scratch, const std::vector<int64_t>& counts, const torch::Tensor& normals,
+                  const std::vector<torch::Tensor>& src, const std::vector<torch::Tensor>& dst) {
+    TORCH_CHECK(src.size() == 21 && dst.size() == 21 && counts.size() == 4, "densify_apply: 21 src, 21 dst, 4 counts");
+    TORCH_CHECK(src[0].is_cuda(), "parameters must be CUDA tensors (this build has no CPU path)");
+    TORCH_CHECK(src[0].dim() == 2 && src[0].size(1) == 3 && src[0].size(0) <= INT32_MAX / 3, "xyz must be [P,3], 3 P < 2^31");
+    TORCH_CHECK(src[2].dim() == 3 && src[6].dim() >= 2, "f_rest must be [P,M-1,3], semantic_feature [P,1,C]");
+    const c10::cuda::CUDAGuard guard(src[0].device());
+    const auto dev = src[0].device();
+    const int64_t P = src[0].size(0), M = 1 + src[2].size(1), C = src[6].size(-1);
+    for (int64_t c : counts) TORCH_CHECK(c >= 0 && c <= INT32_MAX, "densify_apply: bad counts");
+    const int64_t Pn = counts[0] + counts[1] + 2 * counts[2];
+    const int64_t width[7] = {3, 3, 3 * (M - 1), 1, 3, 4, C};
+    static const char* names[7] = {"xyz", "f_dc", "f_rest", "opacity", "scaling", "rotation", "semantic_feature"};
+    f3dgs_gaussian_fields f[2][3];
+    for (int i = 0; i < 21; i++) {
+        check_f32(src[i], dev, P * width[i % 7], names[i % 7]);
+        check_f32(dst[i], dev, Pn * width[i % 7], names[i % 7]);
+        for (int k = 0; k < 2; k++) {
+            float* p = const_cast<float*>(fptr(k ? dst[i] : src[i]));
+            f3dgs_gaussian_fields& g = f[k][i / 7];
+            float** slot[7] = {&g.xyz, &g.f_dc, &g.f_rest, &g.opacity, &g.scaling, &g.rotation, &g.semantic_feature};
+            *slot[i % 7] = p;
+        }
+    }
+    check_f32(normals, dev, 6 * counts[3], "normals");
+    const int32_t c32[4] = {(int32_t)counts[0], (int32_t)counts[1], (int32_t)counts[2], (int32_t)counts[3]};
+    cudaStream_t stream = c10::cuda::getCurrentCUDAStream().stream();
+    check_rc(f3dgs_densify_apply((int)P, (int)M, (int)C,
+                                 scratch.numel() ? reinterpret_cast<const char*>(scratch.data_ptr()) : nullptr, c32,
+                                 fptr(normals), f[0], f[1], (void*)stream),
+             "f3dgs_densify_apply");
+}
+
+void resetOpacity(torch::Tensor raw_opacity, torch::Tensor exp_avg, torch::Tensor exp_avg_sq, double ceiling) {
+    TORCH_CHECK(raw_opacity.is_cuda(), "parameters must be CUDA tensors (this build has no CPU path)");
+    TORCH_CHECK(raw_opacity.numel() <= INT32_MAX, "reset_opacity: P must be below 2^31");
+    const c10::cuda::CUDAGuard guard(raw_opacity.device());
+    const int64_t P = raw_opacity.numel();
+    check_f32(raw_opacity, raw_opacity.device(), P, "raw_opacity");
+    check_f32(exp_avg, raw_opacity.device(), P, "exp_avg");
+    check_f32(exp_avg_sq, raw_opacity.device(), P, "exp_avg_sq");
+    cudaStream_t stream = c10::cuda::getCurrentCUDAStream().stream();
+    check_rc(f3dgs_reset_opacity((int)P, const_cast<float*>(fptr(raw_opacity)), const_cast<float*>(fptr(exp_avg)),
+                                 const_cast<float*>(fptr(exp_avg_sq)), (float)ceiling, (void*)stream),
+             "f3dgs_reset_opacity");
+}
+
 // ---- activation prologue + fused optimizer step (f3dgs_activate / f3dgs_adam_step): in-place on the caller's tensors
 void activateParams(const torch::Tensor& raw_opacity, const torch::Tensor& raw_scaling, const torch::Tensor& raw_rotation,
                     const torch::Tensor& f_dc, const torch::Tensor& f_rest, torch::Tensor opacity, torch::Tensor scales,
@@ -501,6 +586,10 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
           pybind11::arg("dtype") = torch::kFloat32);
     m.def("decoder_l1", &decoderL1);
     m.def("knn_mean_dist", &knnMeanDist);
+    m.def("densify_plan", &densifyPlan);
+    m.def("densify_apply", &densifyApply);
+    m.def("reset_opacity", &resetOpacity, pybind11::arg("raw_opacity"), pybind11::arg("exp_avg"),
+          pybind11::arg("exp_avg_sq"), pybind11::arg("ceiling") = 0.01);
     m.def("activate", &activateParams);
     m.def("adam_step", &adamStep);
     m.def("backward_scratch_bytes", [](int P) { return (unsigned long long)f3dgs_backward_scratch_bytes(P); });

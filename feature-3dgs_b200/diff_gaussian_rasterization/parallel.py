@@ -110,13 +110,16 @@ class ViewBatch:
         self.P = P
         sizes = [self.params[k].numel() for k in self.names]
         extra = 2 * P if densify_stats else 0
-        self.flat = torch.zeros(sum(sizes) + extra, device=dev, dtype=torch.float32)
-        self.grads, o = {}, 0
-        for k, n in zip(self.names, sizes):
-            self.grads[k] = self.flat[o:o + n].view_as(self.params[k])
-            o += n
+        # every view starts on a 16-byte boundary: the backward and the optimizer move the rotation gradient as float4,
+        # and P, which sets the offsets, is arbitrary once densification has run
+        offs, o = [], 0
+        for n in sizes:
+            offs.append(o)
+            o += -(-n // 4) * 4
+        self.flat = torch.zeros(o + extra, device=dev, dtype=torch.float32)
+        self.grads = {k: self.flat[s:s + n].view_as(self.params[k]) for k, s, n in zip(self.names, offs, sizes)}
         self.n_param = o
-        self.early = sum(self.params[k].numel() for k in self.names if k in ("semantic_feature", "opacities"))
+        self.early = next((s for k, s in zip(self.names, offs) if k not in ("semantic_feature", "opacities")), o)
         self.grad_accum = self.flat[o:o + P] if densify_stats else None
         self.denom = self.flat[o + P:o + 2 * P] if densify_stats else None
         self.scratch = torch.empty(int(_C.backward_scratch_bytes(P)), dtype=torch.uint8, device=dev)

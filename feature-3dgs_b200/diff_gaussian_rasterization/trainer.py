@@ -14,8 +14,9 @@ _opacity, _scaling, _rotation, _semantic_feature`, :47-58) as plain CUDA tensors
   step(lrs)             Adam (:163-190: lr per group, eps 1e-15) fused with the activations' Jacobians
                         (f3dgs_adam_step): consumes the all-reduced gradients w.r.t. the ACTIVATED tensors straight from the
                         flat buffer and updates the raw parameters in place -- no autograd graph anywhere;
-  densify_and_prune()   clone / split / prune (:350-434) with the optimizer state carried along, as in the reference
-                        (host-side tensor logic: the reference's is Python too).
+  densify_and_prune()   clone / split / prune (:350-434) with the optimizer state carried along, in two native calls
+                        (f3dgs_densify_plan / f3dgs_densify_apply) with one host read in between;
+  reset_opacity()       :231-234 in one kernel (f3dgs_reset_opacity).
 """
 import math
 from typing import Dict, Optional
@@ -32,17 +33,6 @@ GRAD_OF = dict(xyz="means3D", f_dc="shs", f_rest="shs", opacity="opacities", sca
 
 def inverse_sigmoid(x):
     return torch.log(x / (1 - x))
-
-
-def build_rotation(r):
-    """utils/general_utils.py:78-100: rotation matrices of (normalised) quaternions (w, x, y, z)."""
-    q = r / r.norm(dim=1, keepdim=True)
-    w, x, y, z = q[:, 0], q[:, 1], q[:, 2], q[:, 3]
-    R = torch.zeros((q.shape[0], 3, 3), device=r.device)
-    R[:, 0, 0] = 1 - 2 * (y * y + z * z); R[:, 0, 1] = 2 * (x * y - w * z); R[:, 0, 2] = 2 * (x * z + w * y)
-    R[:, 1, 0] = 2 * (x * y + w * z); R[:, 1, 1] = 1 - 2 * (x * x + z * z); R[:, 1, 2] = 2 * (y * z - w * x)
-    R[:, 2, 0] = 2 * (x * z - w * y); R[:, 2, 1] = 2 * (y * z + w * x); R[:, 2, 2] = 1 - 2 * (x * x + y * y)
-    return R
 
 
 class GaussianState:
@@ -106,11 +96,13 @@ class GaussianState:
     def M(self):
         return 1 + self.raw["f_rest"].shape[1]
 
-    def _reset_derived(self):
+    def _reset_derived(self, keep_optimizer_state=False):
         dev, P = self.raw["xyz"].device, self.P
-        self.exp_avg = {k: torch.zeros_like(v) for k, v in self.raw.items()}
-        self.exp_avg_sq = {k: torch.zeros_like(v) for k, v in self.raw.items()}
-        self.steps = {k: 0 for k in self.raw}
+        self.act = self._batch = None  # the old buffers are released before the new ones are allocated
+        if not keep_optimizer_state:
+            self.exp_avg = {k: torch.zeros_like(v) for k, v in self.raw.items()}
+            self.exp_avg_sq = {k: torch.zeros_like(v) for k, v in self.raw.items()}
+            self.steps = {k: 0 for k in self.raw}
         self.max_radii2D = torch.zeros(P, device=dev)
         self.act = dict(means3D=self.raw["xyz"], opacities=torch.empty(P, 1, device=dev), scales=torch.empty(P, 3, device=dev),
                         rotations=torch.empty(P, 4, device=dev), shs=torch.empty(P, self.M, 3, device=dev),
@@ -146,70 +138,60 @@ class GaussianState:
 
     # ---------------------------------------------------------------------------------------------- densification
     def update_max_radii(self, radii):
-        vis = radii > 0
-        self.max_radii2D[vis] = torch.max(self.max_radii2D[vis], radii[vis].float())  # train.py:131
-
-    def _select(self, mask):
-        for d in (self.raw, self.exp_avg, self.exp_avg_sq):
-            for k in d:
-                d[k] = d[k][mask].contiguous()
-
-    def _append(self, new: Dict[str, torch.Tensor]):
-        for k in self.raw:
-            self.raw[k] = torch.cat((self.raw[k], new[k]), dim=0).contiguous()
-            self.exp_avg[k] = torch.cat((self.exp_avg[k], torch.zeros_like(new[k])), dim=0).contiguous()
-            self.exp_avg_sq[k] = torch.cat((self.exp_avg_sq[k], torch.zeros_like(new[k])), dim=0).contiguous()
+        """train.py:131, without a host sync: max_radii2D = max(max_radii2D, radii) where radii > 0."""
+        self.max_radii2D = torch.where(radii > 0, torch.maximum(self.max_radii2D, radii.float()), self.max_radii2D)
 
     def densify_and_prune(self, max_grad, min_opacity, extent, max_screen_size, grad_accum=None, denom=None, generator=None):
-        """scene/gaussian_model.py:420-434 (clone :407-418, split :381-405, prune :316-330)."""
-        vb = self.batch()
-        grad_accum = vb.grad_accum if grad_accum is None else grad_accum
-        denom = vb.denom if denom is None else denom
-        grads = grad_accum / denom
-        grads[grads.isnan()] = 0.0
-        max_radii = self.max_radii2D
-        scaling = torch.exp(self.raw["scaling"])
-        # ---- clone small Gaussians with a large screen-space gradient
-        sel = (grads >= max_grad) & (scaling.max(dim=1).values <= self.percent_dense * extent)
-        n0 = self.P
-        self._append({k: v[sel] for k, v in self.raw.items()})
-        # ---- split large ones (the clones appended above take part with zero gradient, as in the reference :384-386)
-        padded = torch.zeros(self.P, device=grads.device)
-        padded[:n0] = grads
-        scaling = torch.exp(self.raw["scaling"])
-        sel = (padded >= max_grad) & (scaling.max(dim=1).values > self.percent_dense * extent)
-        N = 2
-        stds = scaling[sel].repeat(N, 1)
-        samples = torch.normal(mean=torch.zeros_like(stds), std=stds, generator=generator)
-        rots = build_rotation(self.raw["rotation"][sel]).repeat(N, 1, 1)
-        new = {k: v[sel].repeat(N, *([1] * (v.dim() - 1))) for k, v in self.raw.items()}
-        new["xyz"] = torch.bmm(rots, samples.unsqueeze(-1)).squeeze(-1) + self.raw["xyz"][sel].repeat(N, 1)
-        new["scaling"] = torch.log(scaling[sel].repeat(N, 1) / (0.8 * N))
-        n_before_split = self.P
-        self._append(new)
-        keep = torch.ones(self.P, dtype=torch.bool, device=grads.device)
-        keep[:n_before_split] = ~sel
-        # ---- prune: transparent, or too large on screen / in the world
-        opacity = torch.sigmoid(self.raw["opacity"]).squeeze(-1)
-        prune = opacity < min_opacity
-        if max_screen_size:
-            mr = torch.zeros(self.P, device=grads.device)  # densification_postfix resets max_radii2D (:376)
-            big_ws = torch.exp(self.raw["scaling"]).max(dim=1).values > 0.1 * extent
-            prune = prune | (mr > max_screen_size) | big_ws
-        del max_radii
-        self._select(keep & ~prune)
-        steps = dict(self.steps)
-        m, v = self.exp_avg, self.exp_avg_sq
-        self._reset_derived()
-        self.exp_avg, self.exp_avg_sq, self.steps = m, v, steps
+        """scene/gaussian_model.py:420-434 (clone :407-418, split :381-405, prune :316-330); returns the new P.
+
+        With g = grad_accum / denom (0 where that is NaN) and smax the largest of exp(scaling), a Gaussian is cloned when
+        g >= max_grad and smax <= percent_dense * extent, and split in two when g >= max_grad and smax is larger.  The
+        new rows are the order-preserving compaction of [originals | clones | split copy 0 | split copy 1] without the
+        split originals and without every row that is pruned: sigmoid(opacity) < min_opacity, or, when max_screen_size
+        is truthy, max(exp(scaling)) > 0.1 * extent on the row's own scaling.  As in the reference, max_radii2D is reset
+        before that test (densification_postfix), so its screen-size part never prunes anything.  The thresholds are
+        rounded to float32 once, as torch compares a float32 tensor with a Python scalar.
+
+        A split child copies its parent except scaling = log(exp(scaling) / 1.6) and xyz = R(rotation) (z * exp(scaling))
+        + xyz, with z = torch.randn((2 Ns, 3), generator=generator) over all Ns split Gaussians (rows [0, Ns) copy 0).
+        Kept rows keep their Adam moments, new rows start at zero; `steps` is unchanged.  Every output is bitwise what the
+        reference's tensor code computes, except the split children's xyz, which agree within float rounding (the
+        reference's torch.bmm has no defined summation order).
+
+        Two native calls (csrc/densify.cu) and ONE host sync, the read of the four output counts that size the new
+        tensors and the normal draw.  Deterministic: identical state, statistics and generator state give bitwise-
+        identical output, so data-parallel replicas that densify from the same all-reduced statistics with the same seed
+        stay identical."""
+        from . import _C
+
+        if grad_accum is None or denom is None:
+            vb = self.batch()
+            grad_accum = vb.grad_accum if grad_accum is None else grad_accum
+            denom = vb.denom if denom is None else denom
+            del vb
+        r = self.raw
+        scratch, counts = _C.densify_plan(grad_accum, denom, r["opacity"], r["scaling"], max_grad,
+                                          self.percent_dense * extent, min_opacity,
+                                          0.1 * extent if max_screen_size else math.inf)
+        del grad_accum, denom
+        A, B, Cc, Ns = counts.tolist()
+        normals = torch.randn((2 * Ns, 3), generator=generator, device=r["xyz"].device)
+        Pn = A + B + 2 * Cc
+        groups = (self.raw, self.exp_avg, self.exp_avg_sq)
+        new = [{k: torch.empty((Pn,) + r[k].shape[1:], device=r[k].device) for k in self.NAMES} for _ in groups]
+        _C.densify_apply(scratch, [A, B, Cc, Ns], normals, [g[k] for g in groups for k in self.NAMES],
+                         [g[k] for g in new for k in self.NAMES])
+        del r, groups, scratch, normals
+        self.raw, self.exp_avg, self.exp_avg_sq = new
+        del new
+        self._reset_derived(keep_optimizer_state=True)
         return self.P
 
     def reset_opacity(self):
-        """scene/gaussian_model.py:231-234: clamp opacity to <= 0.01 and clear its optimizer state."""
-        o = torch.sigmoid(self.raw["opacity"])
-        self.raw["opacity"] = inverse_sigmoid(torch.min(o, torch.ones_like(o) * 0.01)).contiguous()
-        self.exp_avg["opacity"].zero_()
-        self.exp_avg_sq["opacity"].zero_()
+        """scene/gaussian_model.py:231-234: clamp opacity to <= 0.01 and clear its optimizer state, in place."""
+        from . import _C
+
+        _C.reset_opacity(self.raw["opacity"], self.exp_avg["opacity"], self.exp_avg_sq["opacity"])
 
 
 def expon_lr(step, lr_init, lr_final, lr_delay_steps=0, lr_delay_mult=1.0, max_steps=1000000):

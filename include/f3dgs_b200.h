@@ -229,6 +229,45 @@ int f3dgs_adam_step(int kind, size_t n, int M, float* param, const float* grad_a
 size_t f3dgs_knn_scratch_bytes(int P);
 int f3dgs_knn_mean_dist(int P, const float* points, float* out, char* scratch, void* cuda_stream);
 
+/* ---- adaptive density control: reference scene/gaussian_model.py:350-434 (densify_and_prune: clone :407-418,
+ * split :381-405, prune :316-330) and :231-234 (reset_opacity) ----------------------------------------------------
+ * The seven raw parameter fields of P Gaussians (f_rest is NULL when M == 1, semantic_feature NULL when C == 0):
+ *   xyz [P,3]  f_dc [P,1,3]  f_rest [P,M-1,3]  opacity [P,1]  scaling [P,3] (log)  rotation [P,4]  semantic_feature [P,1,C]
+ * Densification is two calls with one host read in between:
+ *   f3dgs_densify_plan   classifies every Gaussian and writes counts = {A, B, Cc, Ns} (device int32[4]): A originals
+ *                        kept, B clones kept, Cc children kept per split copy, Ns Gaussians selected for split.  With
+ *                        g = grad_accum / denom (0 where NaN) and smax = max of expf(raw_scaling) over 3, in fp32:
+ *                          clone  g >= max_grad && smax <= dense_scale     (dense_scale = percent_dense * extent)
+ *                          split  g >= max_grad && smax >  dense_scale
+ *                          prune  sigmoid(opacity) < min_opacity || smax > max_world_scale (0.1 * extent; +inf
+ *                                 disables it), each row on its own scaling
+ *                        The thresholds are the caller's doubles rounded once to float, as torch compares.
+ *   f3dgs_densify_apply  writes the P' = A + B + 2 Cc output rows: the order-preserving compaction of
+ *                        [P originals | clones | split copy 0 | split copy 1] without the split originals and the
+ *                        pruned rows.  Every field of a clone or child is its parent's, except a child's
+ *                        scaling = logf(expf(s) * (1 / 1.6f)) and xyz = R(q) (z * expf(s)) + parent xyz, with
+ *                        R(q) of q = r / sqrt(sum r^2) and z = normals[Ns * copy + (split index), :].
+ *                        src[0] / dst[0] are the raw fields, [1] exp_avg, [2] exp_avg_sq: kept rows move their
+ *                        moments bitwise, clone and child rows get zeros.  counts is the HOST copy of what plan wrote
+ *                        (it sizes dst and normals [2 Ns, 3]); if it differs from the device counts nothing is
+ *                        written.  No dst field may overlap a src field, normals or the scratch.
+ *   scratch  f3dgs_densify_scratch_bytes(P) bytes of device memory, 256-byte aligned, unchanged between the calls
+ * Both calls are stream-ordered without host sync and bitwise deterministic.  3 P must not exceed INT_MAX.
+ * f3dgs_densify_scratch_bytes returns 0 for P <= 0, and 0 with f3dgs_last_error() set if the size query fails.
+ *
+ * f3dgs_reset_opacity: raw_opacity <- logf(x / (1 - x)) with x = min(sigmoid(raw_opacity), ceiling) (NaN propagates, as
+ * torch.minimum), in place; exp_avg and exp_avg_sq of the opacity [P] are zeroed.  The reference's ceiling is 0.01f. */
+typedef struct f3dgs_gaussian_fields {
+    float *xyz, *f_dc, *f_rest, *opacity, *scaling, *rotation, *semantic_feature;
+} f3dgs_gaussian_fields;
+size_t f3dgs_densify_scratch_bytes(int P);
+int f3dgs_densify_plan(int P, const float* grad_accum, const float* denom, const float* raw_opacity,
+                       const float* raw_scaling, float max_grad, float dense_scale, float min_opacity,
+                       float max_world_scale, char* scratch, int32_t* counts, void* cuda_stream);
+int f3dgs_densify_apply(int P, int M, int C, const char* scratch, const int32_t counts[4], const float* normals,
+                        const f3dgs_gaussian_fields src[3], const f3dgs_gaussian_fields dst[3], void* cuda_stream);
+int f3dgs_reset_opacity(int P, float* raw_opacity, float* exp_avg, float* exp_avg_sq, float ceiling, void* cuda_stream);
+
 /* ---- markVisible: reference rasterizer_impl.cu:141-153 (checkFrustum :54-66) --------------
  * present[i] = (view-space z of means3D[i] > 0.2).  `present` is P bytes (0/1). */
 int f3dgs_mark_visible(int P, const float* means3D, const float* viewmatrix,
