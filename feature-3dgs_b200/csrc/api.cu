@@ -8,6 +8,7 @@
 // minimal key width, range detection, composite.  Everything is enqueued on the caller's stream.
 #include <cub/cub.cuh>
 
+#include <cmath>
 #include <cstdio>
 #include <cstring>
 #include <mutex>
@@ -636,6 +637,43 @@ int decoder_l1_impl(const char* fn, int Cin, int Cout, int N, const float* weigh
     if (e != cudaSuccess) return fail(F3DGS_ERR_CUDA, std::string(fn) + ": " + cudaGetErrorString(e));
     return 0;
 }
+
+template <typename X>
+int feature_query_impl(const char* fn, int C, int D, int K, int N, const float* weight, const float* bias, const X* x,
+                       const float* text, float logit_scale, const uint8_t* positive, int64_t* labels, float* prob,
+                       float* logits, void* cuda_stream) {
+    const std::string api = std::string("f3dgs_") + fn;
+    t_error.clear();
+    if (K < 1 || K > kQueryMaxK || D < 1 || D > kQueryMaxD || C < 1 || N < 0 || (weight && C > kDecoderMaxCin))
+        return fail(F3DGS_ERR_INVALID_ARGUMENT,
+                    api + ": bad sizes (1 <= K <= 256, 1 <= D <= 4096, N >= 0, 1 <= C <= 256 with a decoder)");
+    if (!weight && D != C) return fail(F3DGS_ERR_INVALID_ARGUMENT, api + ": D != C needs a decoder weight");
+    if (bias && !weight) return fail(F3DGS_ERR_INVALID_ARGUMENT, api + ": bias without weight");
+    if (!x || !text) return fail(F3DGS_ERR_INVALID_ARGUMENT, api + ": NULL pointer (x and text are required)");
+    if (!labels && !prob && !logits) return fail(F3DGS_ERR_INVALID_ARGUMENT, api + ": no output requested");
+    if (prob && !positive) return fail(F3DGS_ERR_INVALID_ARGUMENT, api + ": prob needs a positive set");
+    if (!std::isfinite(logit_scale)) return fail(F3DGS_ERR_INVALID_ARGUMENT, api + ": logit_scale is not finite");
+    const size_t n = (size_t)N;
+    struct Range {
+        const void* p;
+        size_t bytes;
+    };
+    const Range in[] = {{weight, (size_t)D * C * 4}, {bias, (size_t)D * 4}, {x, (size_t)C * n * sizeof(X)},
+                        {text, (size_t)K * D * 4}, {positive, (size_t)K}};
+    const Range out[] = {{labels, n * 8}, {prob, n * 4}, {logits, (size_t)K * n * 4}};
+    for (int i = 0; i < 3; i++) {
+        for (const Range& r : in)
+            if (ranges_overlap(out[i].p, out[i].bytes, r.p, r.bytes))
+                return fail(F3DGS_ERR_INVALID_ARGUMENT, api + ": an output overlaps an input");
+        for (int j = 0; j < i; j++)
+            if (ranges_overlap(out[i].p, out[i].bytes, out[j].p, out[j].bytes))
+                return fail(F3DGS_ERR_INVALID_ARGUMENT, api + ": outputs overlap");
+    }
+    cudaError_t e = launch_feature_query(C, D, K, N, weight, bias, x, text, logit_scale, positive, labels, prob, logits,
+                                         (cudaStream_t)cuda_stream);
+    if (e != cudaSuccess) return fail(F3DGS_ERR_CUDA, std::string(fn) + ": " + cudaGetErrorString(e));
+    return 0;
+}
 }  // namespace
 
 extern "C" {
@@ -663,6 +701,20 @@ int f3dgs_decoder_l1_f16gt(int Cin, int Cout, int N, const float* weight, const 
                            float* dL_dbias, void* cuda_stream) {
     return decoder_l1_impl("decoder_l1_f16gt", Cin, Cout, N, weight, bias, x, reinterpret_cast<const __half*>(gt),
                            grad_scale, loss_sum, dL_dx, dL_dweight, dL_dbias, cuda_stream);
+}
+
+int f3dgs_feature_query(int C, int D, int K, int N, const float* weight, const float* bias, const float* x,
+                        const float* text, float logit_scale, const uint8_t* positive, int64_t* labels, float* prob,
+                        float* logits, void* cuda_stream) {
+    return feature_query_impl("feature_query", C, D, K, N, weight, bias, x, text, logit_scale, positive, labels, prob,
+                              logits, cuda_stream);
+}
+
+int f3dgs_feature_query_f16x(int C, int D, int K, int N, const float* weight, const float* bias, const uint16_t* x,
+                             const float* text, float logit_scale, const uint8_t* positive, int64_t* labels,
+                             float* prob, float* logits, void* cuda_stream) {
+    return feature_query_impl("feature_query_f16x", C, D, K, N, weight, bias, reinterpret_cast<const __half*>(x), text,
+                              logit_scale, positive, labels, prob, logits, cuda_stream);
 }
 
 size_t f3dgs_knn_scratch_bytes(int P) {

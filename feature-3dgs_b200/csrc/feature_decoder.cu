@@ -30,6 +30,7 @@
 #include <algorithm>
 
 #include "kernels.h"
+#include "tf32_mma.cuh"
 
 namespace f3dgs {
 namespace {
@@ -43,28 +44,6 @@ constexpr int kCoutAlign = kCoutB;             // Cout_pad: a whole number of ke
 constexpr int kTargetCtasB = 1024;             // split-K: about this many kernel B CTAs whatever the shape
 constexpr int kReduceThreads = 512;
 
-__device__ __forceinline__ uint32_t to_tf32(float x) {
-    uint32_t r;
-    asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(r) : "f"(x));
-    return r;
-}
-
-// d += a * b, m16n8k8 TF32, fp32 accumulate.  Fragments (PTX ISA, mma.m16n8k8 .tf32), g = lane >> 2, t = lane & 3:
-//   a0 (g, t)  a1 (g + 8, t)  a2 (g, t + 4)  a3 (g + 8, t + 4)      b0 (k = t, n = g)  b1 (k = t + 4, n = g)
-//   d0 (g, 2t) d1 (g, 2t + 1) d2 (g + 8, 2t) d3 (g + 8, 2t + 1)
-__device__ __forceinline__ void mma_tf32(float (&d)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
-    asm volatile(
-        "mma.sync.aligned.m16n8k8.row.col.f32.tf32.tf32.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
-        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
-        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
-}
-
-__device__ __forceinline__ void cp_async16(void* dst_smem, const void* src_gmem) {
-    asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(smem_u32(dst_smem)), "l"(src_gmem) : "memory");
-}
-__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
-__device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_group 0;" ::: "memory"); }
-
 // sign as a TF32 operand: +1, -1 or 0 (exact)
 __device__ __forceinline__ uint32_t sign_bits(float d) { return d > 0.f ? 0x3f800000u : (d < 0.f ? 0xbf800000u : 0u); }
 // the sign of pixel i (0..15) of a bit word
@@ -72,8 +51,6 @@ __device__ __forceinline__ uint32_t word_sign(uint32_t w, int i) {
     return (((w >> i) & 1u) * 0x3f800000u) | (((w >> (16 + i)) & 1u) << 31);
 }
 
-__device__ __forceinline__ float load_f32(const float* p) { return __ldg(p); }
-__device__ __forceinline__ float load_f32(const __half* p) { return __half2float(__ldg(p)); }
 __device__ __forceinline__ void store_f32(float* p, float v) { *p = v; }
 __device__ __forceinline__ void store_f32(__half* p, float v) { *p = __float2half_rn(v); }
 
@@ -484,11 +461,8 @@ cudaError_t decoder_run(int Cin, int Cout, int N, const float* weight, const flo
     a.bits = reinterpret_cast<uint32_t*>(ws + sc.off_bits);
     a.loss_part = reinterpret_cast<float*>(ws + sc.off_loss);
     a.grad_scale = grad_scale;
-    const size_t nprep = (size_t)p.Cout_pad * p.Cp;
-    decoder_prep_kernel<<<(unsigned)std::min<size_t>((nprep + 255) / 256, 1024), 256, 0, s>>>(
-        Cin, Cout, p.Cp, p.Cout_pad, weight, bias, const_cast<float*>(a.wt), const_cast<float*>(a.bias));
-    g_launches++;
-    e = cudaGetLastError();
+    e = launch_decoder_prep(Cin, Cout, p.Cp, p.Cout_pad, weight, bias, const_cast<float*>(a.wt),
+                            const_cast<float*>(a.bias), s);
     if (e == cudaSuccess) {
         e = loss ? launch_a_kt<true>(p, a, s) : launch_a_kt<false>(p, a, s);
         g_launches++;
@@ -510,6 +484,15 @@ cudaError_t decoder_run(int Cin, int Cout, int N, const float* weight, const flo
 }
 
 }  // namespace
+
+cudaError_t launch_decoder_prep(int Cin, int Cout, int Cp, int rows, const float* weight, const float* bias, float* wt,
+                                float* bp, cudaStream_t s) {
+    const size_t n = (size_t)rows * Cp;
+    decoder_prep_kernel<<<(unsigned)std::min<size_t>((n + 255) / 256, 1024), 256, 0, s>>>(Cin, Cout, Cp, rows, weight,
+                                                                                        bias, wt, bp);
+    g_launches++;
+    return cudaGetLastError();
+}
 
 bool decoder_grid_ok(int Cin, int Cout, int N) {
     if (Cin < 1 || Cin > kDecoderMaxCin || Cout < 1 || Cout > kDecoderMaxCout || N < 1) return false;

@@ -93,6 +93,19 @@ cudaError_t launch_decoder_l1(int Cin, int Cout, int N, const float* weight, con
 cudaError_t launch_decoder_l1(int Cin, int Cout, int N, const float* weight, const float* bias, const float* x,
                               const __half* gt, float grad_scale, float* loss_sum, float* dx, float* dW, float* db,
                               cudaStream_t s);
+// W [Cout,Cin] -> wt [rows, Cp] rounded to TF32 and zero-padded; b [Cout] or NULL -> bp [rows] zero-padded
+cudaError_t launch_decoder_prep(int Cin, int Cout, int Cp, int rows, const float* weight, const float* bias, float* wt,
+                                float* bp, cudaStream_t s);
+
+// ---- feature_query.cu: cosine similarity of (decoded) feature columns with text embeddings -> argmax label, softmax
+// probability of a positive prompt set, logits.  weight == NULL: no decoder (D == C).  x may be float16 (upcast exactly)
+constexpr int kQueryMaxK = 256, kQueryMaxD = 4096;
+cudaError_t launch_feature_query(int C, int D, int K, int N, const float* weight, const float* bias, const float* x,
+                                 const float* text, float logit_scale, const uint8_t* positive, int64_t* labels,
+                                 float* prob, float* logits, cudaStream_t s);
+cudaError_t launch_feature_query(int C, int D, int K, int N, const float* weight, const float* bias, const __half* x,
+                                 const float* text, float logit_scale, const uint8_t* positive, int64_t* labels,
+                                 float* prob, float* logits, cudaStream_t s);
 
 // ---- knn.cu: exact mean squared distance to the 3 nearest other points (distCUDA2); scratch is knn_scratch_bytes(P)
 // bytes whose first knn_scratch_fixed_bytes(P) need no device query to size

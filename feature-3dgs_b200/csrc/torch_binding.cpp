@@ -414,6 +414,74 @@ std::tuple<torch::Tensor, torch::Tensor> decoderL1(const torch::Tensor& x, const
     return std::make_tuple(loss, dx);
 }
 
+// ---- text query (f3dgs_feature_query / _f16x): x [C,N] or [C,H,W] float32 or float16, text [K,D], weight [D,C] or
+// [D,C,1,1] or empty (no decoder), bias [D] or empty, positive [K] uint8 / bool or empty
+// -> (labels int64, prob float32, logits float32 [K, ...]) shaped like x without its channel axis; an output that is not
+// wanted is an empty tensor
+std::tuple<torch::Tensor, torch::Tensor, torch::Tensor> featureQuery(const torch::Tensor& x, const torch::Tensor& text,
+                                                                     const torch::Tensor& weight,
+                                                                     const torch::Tensor& bias, double logit_scale,
+                                                                     const torch::Tensor& positive, bool want_labels,
+                                                                     bool want_prob, bool want_logits) {
+    TORCH_CHECK(x.is_cuda() && (x.scalar_type() == torch::kFloat32 || x.scalar_type() == torch::kFloat16) &&
+                    x.dim() >= 2, "feature_query: x must be a float32 or float16 CUDA tensor [C,N] or [C,H,W]");
+    const auto dev = x.device();
+    const c10::cuda::CUDAGuard guard(dev);
+    TORCH_CHECK(text.device() == dev && text.scalar_type() == torch::kFloat32 && text.dim() == 2,
+                "feature_query: text must be a float32 tensor [K,D] on ", dev);
+    const bool has_w = weight.defined() && weight.numel() > 0, has_b = bias.defined() && bias.numel() > 0;
+    const bool has_pos = positive.defined() && positive.numel() > 0;
+    const int64_t C = x.size(0), K = text.size(0), D = text.size(1);
+    if (has_w) {
+        TORCH_CHECK(weight.device() == dev && weight.scalar_type() == torch::kFloat32 &&
+                        (weight.dim() == 2 || (weight.dim() == 4 && weight.size(2) == 1 && weight.size(3) == 1)) &&
+                        weight.size(0) == D && weight.size(1) == C,
+                    "feature_query: weight must be a float32 tensor [D,C] or [D,C,1,1] on ", dev, " with D = ", D,
+                    " (text) and C = ", C, " (x)");
+    } else {
+        TORCH_CHECK(D == C, "feature_query: without a decoder text must have x's ", C, " channels (got ", D, ")");
+    }
+    if (has_b)
+        TORCH_CHECK(has_w && bias.device() == dev && bias.scalar_type() == torch::kFloat32 && bias.dim() == 1 &&
+                        bias.size(0) == D, "feature_query: bias must be a float32 tensor [D] on ", dev,
+                    ", and only with a weight");
+    if (has_pos)
+        TORCH_CHECK(positive.device() == dev &&
+                        (positive.scalar_type() == torch::kUInt8 || positive.scalar_type() == torch::kBool) &&
+                        positive.dim() == 1 && positive.size(0) == K,
+                    "feature_query: positive must be a uint8 or bool tensor [K] on ", dev);
+    TORCH_CHECK(!want_prob || has_pos, "feature_query: prob needs a positive set");
+    TORCH_CHECK(want_labels || want_prob || want_logits, "feature_query: no output requested");
+    const int64_t N = x.numel() / std::max<int64_t>(C, 1);
+    TORCH_CHECK(C >= 1 && K >= 1, "feature_query: x needs a channel and text a prompt");
+    TORCH_CHECK(N <= INT32_MAX && C <= INT32_MAX && K <= INT32_MAX && D <= INT32_MAX, "feature_query: sizes too large");
+    auto xc = x.contiguous(), tc = text.contiguous();
+    auto w = has_w ? weight.contiguous() : torch::Tensor(), b = has_b ? bias.contiguous() : torch::Tensor();
+    auto p = has_pos ? positive.contiguous() : torch::Tensor();
+    const auto spatial = xc.sizes().slice(1).vec();
+    auto lshape = spatial;
+    lshape.insert(lshape.begin(), K);
+    auto f32 = xc.options().dtype(torch::kFloat32);
+    torch::Tensor labels = torch::empty(want_labels ? spatial : std::vector<int64_t>{0}, f32.dtype(torch::kInt64));
+    torch::Tensor prob = torch::empty(want_prob ? spatial : std::vector<int64_t>{0}, f32);
+    torch::Tensor logits = torch::empty(want_logits ? lshape : std::vector<int64_t>{0}, f32);
+    if (N == 0) return std::make_tuple(labels, prob, logits);
+    const uint8_t* pp = has_pos ? reinterpret_cast<const uint8_t*>(p.data_ptr()) : nullptr;
+    int64_t* lp = want_labels ? labels.data_ptr<int64_t>() : nullptr;
+    float* pr = want_prob ? prob.data_ptr<float>() : nullptr;
+    float* lg = want_logits ? logits.data_ptr<float>() : nullptr;
+    cudaStream_t stream = c10::cuda::getCurrentCUDAStream().stream();
+    if (xc.scalar_type() == torch::kFloat16)
+        check_rc(f3dgs_feature_query_f16x((int)C, (int)D, (int)K, (int)N, fptr(w), fptr(b), hptr(xc), fptr(tc),
+                                          (float)logit_scale, pp, lp, pr, lg, (void*)stream),
+                 "f3dgs_feature_query_f16x");
+    else
+        check_rc(f3dgs_feature_query((int)C, (int)D, (int)K, (int)N, fptr(w), fptr(b), fptr(xc), fptr(tc),
+                                     (float)logit_scale, pp, lp, pr, lg, (void*)stream),
+                 "f3dgs_feature_query");
+    return std::make_tuple(labels, prob, logits);
+}
+
 // ---- initial scales (f3dgs_knn_mean_dist, the reference's simple_knn distCUDA2): points [P,3] -> [P]
 torch::Tensor knnMeanDist(const torch::Tensor& points) {
     TORCH_CHECK(points.is_cuda(), "points must be a CUDA tensor (this build has no CPU path)");
@@ -585,6 +653,9 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     m.def("decoder_forward", &decoderForward, pybind11::arg("x"), pybind11::arg("weight"), pybind11::arg("bias"),
           pybind11::arg("dtype") = torch::kFloat32);
     m.def("decoder_l1", &decoderL1);
+    m.def("feature_query", &featureQuery, pybind11::arg("x"), pybind11::arg("text"), pybind11::arg("weight"),
+          pybind11::arg("bias"), pybind11::arg("logit_scale"), pybind11::arg("positive"), pybind11::arg("want_labels"),
+          pybind11::arg("want_prob"), pybind11::arg("want_logits"));
     m.def("knn_mean_dist", &knnMeanDist);
     m.def("densify_plan", &densifyPlan);
     m.def("densify_apply", &densifyApply);

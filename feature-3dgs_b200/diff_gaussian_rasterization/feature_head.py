@@ -8,6 +8,8 @@ on two CUDA kernels of libf3dgs_b200 (csrc/feature_head.cu): a resize that, give
 and dL/d(resized map), and a gather-style resize backward that writes every element of dL/dfeature_map exactly once.
 With --speedup the 1x1 decoder and its loss run in between on csrc/feature_decoder.cu (TF32 tensor cores, like cuDNN's
 default for the reference's nn.Conv2d): `decode`, `decoded_feature_l1_loss_and_grad`, `decoded_feature_l1_loss`.
+`query` asks the trained field questions with text embeddings (csrc/feature_query.cu): LSeg's per-pixel labels and
+render_edit's per-Gaussian selection score, without materialising the decoded map.
 There is no CPU path (the extension raises on CPU tensors).
 
 The teacher map `gt` may be float32 or float16, the dtype the data format stores it in (io.load_feature_map(path,
@@ -104,6 +106,44 @@ def decoded_feature_l1_loss_and_grad(feature_map: torch.Tensor, gt: torch.Tensor
                                          _empty(feature_map) if dbias is None else dbias)
         grad = _C().feature_resize_bwd(dres, feature_map.shape[1], feature_map.shape[2])
     return loss_sum[0] * gs, grad, dweight, dbias
+
+
+def query(features: torch.Tensor, text: torch.Tensor, weight=None, bias=None, logit_scale: float = 1.0, positive=None,
+          logits: bool = False):
+    """Ask a feature field questions with text (csrc/feature_query.cu): -> (labels, prob or None, logits or None).
+
+    features [C,H,W] or [C,N], float32 or float16 (a saved map is read as float16, with the result of `.float()`);
+    text [K,D] embeddings (1 <= K <= 256); weight [D,C,1,1] or [D,C] and bias [D] the --speedup decoder, or None (then
+    D == C).  Per column, with y the decoded feature and l_k = logit_scale * cos(y, text_k):
+        labels  int64 argmax_k l_k                           (LSeg's segmentation head; first index on ties)
+        prob    sum over k in `positive` of softmax_k(l)     (with `positive`, a sequence of prompt indices)
+        logits  [K, ...] l                                   (with logits=True)
+    shaped like `features` without its channel axis.  Nothing of size D x N is allocated.  No autograd: this is an
+    inference path.
+
+    render_edit's selection score of Gaussians: `query(state.raw["semantic_feature"][:, 0, :].t().contiguous(), text,
+    w, b, positive=[0])`; the transposed [C,P] copy costs P x C x 4 bytes and one pass over the features.  Thresholding
+    and the edit (zeroing opacity, recolouring) are plain tensor ops on the returned score."""
+    K = text.shape[0]
+    idx = None
+    if positive is not None:
+        idx = [int(i) for i in positive]
+        bad = [i for i in idx if not 0 <= i < K]
+        if bad:
+            raise ValueError(f"query: positive indices {bad} out of range for {K} prompts")
+    for name, t in (("features", features), ("text", text), ("weight", weight), ("bias", bias)):
+        if t is not None and not t.is_cuda:
+            raise ValueError(f"query: {name} must be a CUDA tensor (there is no CPU path)")
+    with torch.no_grad():
+        mask = torch.empty(0, dtype=torch.uint8, device=text.device)
+        if idx is not None:
+            mask = torch.zeros(K, dtype=torch.uint8, device=text.device)
+            if idx:
+                mask[idx] = 1
+        lab, prob, lg = _C().feature_query(features, text, _empty(text) if weight is None else weight,
+                                           _empty(text) if bias is None else bias, float(logit_scale), mask, True,
+                                           idx is not None, bool(logits))
+    return lab, (prob if idx is not None else None), (lg if logits else None)
 
 
 class _DecodedL1(torch.autograd.Function):

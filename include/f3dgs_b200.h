@@ -184,6 +184,29 @@ int f3dgs_decoder_l1_f16gt(int Cin, int Cout, int N, const float* weight, const 
 int f3dgs_decoder_forward_f16(int Cin, int Cout, int N, const float* weight, const float* bias, const float* x,
                               uint16_t* y, void* cuda_stream);
 
+/* ---- text query: LSeg's segmentation head on a rendered or saved feature map; render_edit's CLIP-text selection of
+ * Gaussians (gaussian_renderer/__init__.py:58-170) -----------------------------------------------------------------
+ * x [C,N] (a map [C,H,W] as N = H*W columns, or per-Gaussian features transposed to [C,P]), weight [D,C] (the
+ * CNN_decoder conv weight as contiguous memory) or NULL (no decoder, D == C), bias [D] or NULL (only with weight),
+ * text [K,D] embeddings, positive [K] (nonzero = positive prompt) or NULL.  1 <= K <= 256, 1 <= D <= 4096, N >= 0
+ * (N == 0 launches nothing), 1 <= C <= 256 with a decoder.  For every column n:
+ *     y = weight x_n + bias (x_n without weight);  l_k = logit_scale * <y / max(||y||, 1e-12), t_k / max(||t_k||, 1e-12)>
+ *   f3dgs_feature_query  labels[N] int64 = argmax_k l_k (first maximal index, as torch.argmax; an all-NaN column
+ *                        gives 0); prob[N] = sum over positive k of softmax_k(l) (fp32, max-subtracted; exactly 1 when
+ *                        every prompt is positive; needs positive); logits[K,N] = l.  Each output may be NULL, but
+ *                        one is required; every element of a requested one is written; none may overlap an input or
+ *                        another output; logit_scale must be finite.
+ *   f3dgs_feature_query_f16x  x [C,N] float16 (a saved map): the result of f3dgs_feature_query for the exactly upcast
+ *                        x, bitwise.  Validates as f3dgs_feature_query, with x's 2-byte size in the overlap checks.
+ * Both products use TF32 operands (rounded to nearest) with fp32 accumulation, ||y||^2 is summed in fp32 before any
+ * rounding; nothing of size D*N is stored, and results are bitwise reproducible whichever outputs are requested. */
+int f3dgs_feature_query(int C, int D, int K, int N, const float* weight, const float* bias, const float* x,
+                        const float* text, float logit_scale, const uint8_t* positive, int64_t* labels, float* prob,
+                        float* logits, void* cuda_stream);
+int f3dgs_feature_query_f16x(int C, int D, int K, int N, const float* weight, const float* bias, const uint16_t* x,
+                             const float* text, float logit_scale, const uint8_t* positive, int64_t* labels,
+                             float* prob, float* logits, void* cuda_stream);
+
 /* ---- photometric loss: reference train.py (colour term), utils/loss_utils.py l1_loss + ssim(window_size=11) ---------
  * loss = (1 - lambda_dssim) * l1_loss(image, gt) + lambda_dssim * (1 - ssim(image, gt)).  image, gt [planes,H,W]; the
  * SSIM window is the 11-tap Gaussian (sigma 1.5) per plane with zero padding, C1 = 0.01^2, C2 = 0.03^2.
