@@ -299,83 +299,10 @@ def c3_scene():
 
 
 def _full_size_vs_reference(sc, with_grads, label):
-    """One full-size view, compared on the device; prints the worst violation ratio (|a-b| / tolerance, <= 1 passes) of
-    every float tensor so the margin is on record in the test log.
-
-    Against the unmodified reference build (oracle/_ref, where a reference checkout was there to build it): indices and
-    colour / depth / final_T bit-identical, feature map and gradients within the parity bar.  Without it, against the CPU
-    oracle (oracle/: the reference algorithm restated in C, pinned to the reference's outputs by test_oracle_golden.py)
-    with parity.compare's threshold-tie rule: libm's expf differs from CUDA's by <= 2 ulp, so up to max(2, 1e-4 * pixels)
-    pixels may differ in n_contrib; those are masked out of the images and widen the gradient bar 50x.  Every blend
-    weight then carries those ulps, so the feature map's relative bar applies to the sum of its terms' magnitudes
-    (the oracle's map of |features|) rather than to the possibly cancelled sum."""
-    import os
-
-    import torch
-    from oracle import ref_wrapper as rw
-
+    """One full-size view against the reference build where one exists, else the CPU oracle (parity.tie_aware_compare)."""
     cam = sc.cameras[0]
     grads = scenegen.upstream_grads(cam.image_height, cam.image_width, sc.C) if with_grads else None
-    ours = parity.run_ours(sc, cam, grads=grads)
-    vs_ref = rw.available(sc.C)
-    ref = parity.run_ref(sc, cam, grads=grads) if vs_ref else parity.run_oracle(sc, cam, grads=grads,
-                                                                                 threads=os.cpu_count())
-    for k in ("radii", "point_list", "ranges"):
-        assert np.array_equal(np.asarray(ours[k]).astype(np.int64), np.asarray(ref[k]).astype(np.int64)), k
-    assert int(ours["num_rendered"]) == int(ref["num_rendered"])
-    ties = np.asarray(ours["n_contrib"]).astype(np.int64) != np.asarray(ref["n_contrib"]).astype(np.int64)
-    n_ties = int(ties.sum())
-    if vs_ref:
-        assert n_ties == 0
-        for k in ("color", "depth", "final_T"):
-            assert np.array_equal(ours[k], ref[k]), k
-    else:
-        assert n_ties <= max(2, int(1e-4 * ties.size)), n_ties
-    keep = torch.from_numpy(~ties).cuda()
-    extra = []  # image pixels outside the bar with n_contrib unchanged (oracle only)
-
-    def viol(a, b, atol, widen=1.0, mask=None, mag=None):
-        a = torch.from_numpy(np.ascontiguousarray(a)).cuda().double()
-        b = torch.from_numpy(np.ascontiguousarray(b)).cuda().double()
-        if mask is not None:
-            a = torch.where(mask, a, b)
-        m = b.abs() if mag is None else torch.from_numpy(np.ascontiguousarray(mag)).cuda().double()
-        tol = widen * (parity.RTOL * m + atol * b.abs().max())
-        r = (a - b).abs() / tol
-        if not vs_ref and r.dim() >= 2 and r.shape[-2:] == keep.shape:
-            # a blend flipped at the threshold before the pixel's last contributor leaves n_contrib unchanged: such
-            # pixels count against the same tie budget and must stay within the 50x bar of a tie
-            px = r.reshape(-1, *r.shape[-2:]).amax(0)
-            extra.append(px > 1.0)
-            assert float(px.max()) <= 50.0, float(px.max())
-            r = torch.where(px > 1.0, 0.0, px)
-        return float(r.max())
-
-    worst = {}
-    if not vs_ref:
-        for k in ("color", "depth", "final_T"):
-            worst[k] = viol(ours[k], ref[k], parity.ATOL_REL, mask=keep)
-    if sc.C:
-        mag = None
-        if not vs_ref:
-            sc_abs = copy.copy(sc)
-            sc_abs.features = np.abs(sc.features)
-            mag = parity.run_oracle(sc_abs, cam, threads=os.cpu_count())["feature_map"]
-        worst["feature_map"] = viol(ours["feature_map"], ref["feature_map"], parity.ATOL_REL, mask=keep, mag=mag)
-    if with_grads:
-        for k in ("means3D", "means2D", "sh", "semantic_feature", "opacities", "scales", "rotations"):
-            if k in ours["grads"]:
-                worst["grad_" + k] = viol(ours["grads"][k], ref["grads"][k], parity.GRAD_ATOL_REL,
-                                          widen=50.0 if n_ties else 1.0)
-    if extra:
-        flipped = torch.stack(extra).any(0) & keep
-        n_ties += int(flipped.sum())
-        assert n_ties <= max(2, int(1e-4 * ties.size)), n_ties
-    print(f"[{label} vs {'reference build' if vs_ref else 'CPU oracle'}] V={int((ours['radii'] > 0).sum())} "
-          f"R={int(ours['num_rendered'])} n_contrib ties={n_ties} worst viol per tensor: "
-          + ", ".join(f"{k}={v:.3g}" for k, v in worst.items()))
-    for k, v in worst.items():
-        assert v <= 1.0, (k, v)
+    parity.tie_aware_compare(sc, cam, label, grads=grads)
 
 
 def test_c3_full_size_vs_reference(c3_scene):
@@ -397,30 +324,7 @@ def test_c3_structural_properties(c3_scene):
     """Size-independent properties at the full BASELINE size."""
     sc = c3_scene
     cam = sc.cameras[0]
-    ours = parity.run_ours(sc, cam)
-    R = int(ours["num_rendered"])
-    ranges, pl = ours["ranges"], ours["point_list"]
-    # ranges partition [0, R) in tile order; empty tiles are (0, 0)
-    nz = ranges[(ranges[:, 1] - ranges[:, 0]) > 0]
-    assert nz[0, 0] == 0 and nz[-1, 1] == R and np.array_equal(nz[1:, 0], nz[:-1, 1])
-    # within a tile the list is depth sorted (ties broken by index = stable sort)
-    depth = ours["rec"][:, 11]
-    d = depth[pl]
-    same_tile = np.ones(R - 1, bool)
-    same_tile[nz[:-1, 1] - 1] = False
-    assert (np.diff(d)[same_tile] >= 0).all()
-    ties = same_tile & (np.diff(d) == 0)
-    assert (np.diff(pl)[ties] > 0).all()
-    # every visible Gaussian appears exactly tiles_touched times
-    counts = np.bincount(pl, minlength=sc.P)
-    assert ((counts > 0) == (ours["radii"] > 0)).all()
-    # n_contrib never exceeds the tile's list length; T in (0, 1]
-    gx = (cam.image_width + 15) // 16
-    ty, tx = np.divmod(np.arange(cam.image_height * cam.image_width), cam.image_width)
-    tile = (ty // 16) * gx + (tx // 16)
-    lens = (ranges[:, 1] - ranges[:, 0])[tile].reshape(cam.image_height, cam.image_width)
-    assert (ours["n_contrib"] <= lens).all()
-    assert (ours["final_T"] > 0).all() and (ours["final_T"] <= 1).all()
+    parity.check_structure(parity.run_ours(sc, cam), cam, sc.P)
 
 
 def test_c3_feature_linearity_and_width_independence(c3_scene):
@@ -441,7 +345,30 @@ def test_c3_feature_linearity_and_width_independence(c3_scene):
 
 
 # ------------------------------------------------------------------------------------------- view batches
-@pytest.mark.parametrize("name", ["tiny", "small"])
+def _view_batch_case(name):
+    """-> (scene with 3 cameras, settings overrides).  Beyond tiny / small: the camera-inside-the-cloud scene of
+    test_gpu_regimes (visibility, and so `denom`, differs per view), C = 0 / 3 / 200, SH degree 0 and 3, odd P,
+    focal_x != focal_y and scale_modifier != 1."""
+    import test_gpu_regimes as regimes
+
+    if name in ("tiny", "small"):
+        return scenegen.make_config(name, views=3), {}
+    cases = {
+        "inside_C0_sh0": (dict(C=0, P=4001, sh_degree=0), 1.0, 1.0),
+        "inside_C3_sh3": (dict(C=3, P=4001, sh_degree=3), 1.0, 1.0),
+        "inside_C200_sh3": (dict(C=200, P=3001, sh_degree=3), 1.0, 1.0),
+        "inside_C16_fy_mod": (dict(C=16, P=4001, sh_degree=2), 1.15, 1.3),
+        "inside_wide_C16_fy_mod": (dict(C=16, P=6001, sh_degree=1, target_radius_px=40.0), 1 / 1.15, 0.7),
+    }
+    kw, factor, mod = cases[name]
+    sc = regimes.inside(views=3, **kw)
+    if factor != 1.0:
+        sc.cameras = [regimes.anisotropic(c, factor) for c in sc.cameras]
+    return sc, dict(scale_modifier=mod)
+
+
+@pytest.mark.parametrize("name", ["tiny", "small", "inside_C0_sh0", "inside_C3_sh3", "inside_C200_sh3",
+                                  "inside_C16_fy_mod", "inside_wide_C16_fy_mod"])
 def test_view_batch_accumulates_like_autograd(name):
     """ViewBatch (f3dgs_backward_accum: gradients ADDED in-kernel into one flat buffer, densification statistics folded
     in) against the sum over views of the per-view gradients from the reference-compatible autograd API."""
@@ -449,35 +376,39 @@ def test_view_batch_accumulates_like_autograd(name):
     from diff_gaussian_rasterization import GaussianRasterizationSettings, GaussianRasterizer
     from diff_gaussian_rasterization.parallel import ViewBatch
 
-    sc = scenegen.make_config(name, views=3)
+    sc, opts = _view_batch_case(name)
     dev = "cuda"
     t = scenegen.to_torch(sc, dev, requires_grad=True)
     cam0 = sc.cameras[0]
     ups = [[torch.from_numpy(g).to(dev) for g in scenegen.upstream_grads(cam0.image_height, cam0.image_width, sc.C, seed=50 + v)]
            for v in range(3)]
-    names = ("means3D", "scales", "rotations", "opacities", "shs", "semantic_feature")
+    names = ("means3D", "scales", "rotations", "opacities", "shs") + (("semantic_feature",) if sc.C else ())
     want = {k: torch.zeros_like(t[k]) for k in names}
     accum, denom = torch.zeros(sc.P, device=dev), torch.zeros(sc.P, device=dev)
-    outs = []
+    outs, vis_sets = [], []
     for v, cam in enumerate(sc.cameras):
-        rs = GaussianRasterizationSettings(**scenegen.settings_kwargs(sc, cam, dev))
+        rs = GaussianRasterizationSettings(**parity.settings(sc, cam, dev, **opts))
         m2 = torch.zeros_like(t["means3D"], requires_grad=True)
         color, feat, radii, depth = GaussianRasterizer(rs)(
             means3D=t["means3D"], means2D=m2, opacities=t["opacities"], shs=t["shs"],
-            semantic_feature=t["semantic_feature"], scales=t["scales"], rotations=t["rotations"])
-        torch.autograd.backward([color, depth, feat], [ups[v][0], ups[v][2], ups[v][1]])
+            semantic_feature=t["semantic_feature"] if sc.C else None, scales=t["scales"], rotations=t["rotations"])
+        torch.autograd.backward([color, depth] + ([feat] if sc.C else []),
+                                [ups[v][0], ups[v][2]] + ([ups[v][1]] if sc.C else []))
         for k in names:
             want[k] += t[k].grad
             t[k].grad = None
         vis = radii > 0
         accum[vis] += m2.grad[vis, :2].norm(dim=-1)   # scene/gaussian_model.py:436-438
         denom[vis] += 1
+        vis_sets.append(vis)
         outs.append((color.detach(), feat.detach(), depth.detach(), m2.grad.clone()))
+    if name not in ("tiny", "small"):  # visibility differs per view, so denom counts differ per Gaussian
+        assert not torch.equal(vis_sets[0], vis_sets[1]) and len(torch.unique(denom)) >= 3
 
     vb = ViewBatch({k: t[k].detach() for k in names})
     vb.zero_()
     for v, cam in enumerate(sc.cameras):
-        rs = GaussianRasterizationSettings(**scenegen.settings_kwargs(sc, cam, dev))
+        rs = GaussianRasterizationSettings(**parity.settings(sc, cam, dev, **opts))
         color, feat, radii, depth, ctx = vb.forward(rs)
         assert torch.equal(color, outs[v][0]) and torch.equal(depth, outs[v][2]) and torch.equal(feat, outs[v][1])
         m2 = torch.empty(sc.P, 3, device=dev)
