@@ -19,8 +19,8 @@ OBJ = os.path.join(PKG, "build")
 LIB = os.path.join(PKG, "libf3dgs_b200.so")
 EXT = os.path.join(PKG, "diff_gaussian_rasterization", "_C" + sysconfig.get_config_var("EXT_SUFFIX"))
 CU = ["api.cu", "preprocess.cu", "binning.cu", "composite_fwd.cu", "composite_bwd.cu", "feature_bwd.cu",
-      "feature_head.cu", "feature_decoder.cu", "feature_query.cu", "image_loss.cu", "optimizer.cu", "knn.cu",
-      "densify.cu"]
+      "feature_head.cu", "feature_decoder.cu", "feature_query.cu", "feature_pca.cu", "image_loss.cu", "optimizer.cu",
+      "knn.cu", "densify.cu"]
 HDRS = ["common.cuh", "kernels.h", "composite_common.cuh", "tf32_mma.cuh", os.path.join(ROOT, "include", "f3dgs_b200.h")]
 NVCC_FLAGS = ["-std=c++17", "-O3", "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo",
               "-Xcompiler", "-fPIC", "-Xptxas", "-v", "--expt-relaxed-constexpr"]

@@ -674,6 +674,71 @@ int feature_query_impl(const char* fn, int C, int D, int K, int N, const float* 
     if (e != cudaSuccess) return fail(F3DGS_ERR_CUDA, std::string(fn) + ": " + cudaGetErrorString(e));
     return 0;
 }
+
+// ---- feature PCA: shared validation of (C, N) and of output ranges against inputs
+bool pca_sizes_ok(int C, int N) { return C >= kPcaMinC && C <= kPcaMaxC && N >= 7; }  // n = ceil(N / 3) >= 3
+
+struct Range {
+    const void* p;
+    size_t bytes;
+};
+bool any_overlap(const Range& out, std::initializer_list<Range> in) {
+    for (const Range& r : in)
+        if (ranges_overlap(out.p, out.bytes, r.p, r.bytes)) return true;
+    return false;
+}
+
+template <typename X>
+int pca_moments_impl(const char* fn, int C, int N, const X* x, char* scratch, float* mean, double* cov,
+                     void* cuda_stream) {
+    const std::string api = std::string("f3dgs_") + fn;
+    t_error.clear();
+    if (!pca_sizes_ok(C, N)) return fail(F3DGS_ERR_INVALID_ARGUMENT, api + ": bad sizes (3 <= C <= 1024, N >= 7)");
+    if (!x || !scratch || !mean || !cov) return fail(F3DGS_ERR_INVALID_ARGUMENT, api + ": NULL pointer");
+    const Range rx{x, (size_t)C * N * sizeof(X)}, rs{scratch, pca_scratch_fixed_bytes(C, N)};
+    const Range rm{mean, (size_t)C * 4}, rc{cov, (size_t)C * C * 8};
+    if (any_overlap(rs, {rx}) || any_overlap(rm, {rx, rs}) || any_overlap(rc, {rx, rs, rm}))
+        return fail(F3DGS_ERR_INVALID_ARGUMENT, api + ": scratch, mean and cov must not overlap x or each other");
+    cudaError_t e = launch_pca_moments(C, N, x, scratch, mean, cov, (cudaStream_t)cuda_stream);
+    if (e != cudaSuccess) return fail(F3DGS_ERR_CUDA, std::string(fn) + ": " + cudaGetErrorString(e));
+    return 0;
+}
+
+template <typename X>
+int pca_range_impl(const char* fn, int C, int N, const X* x, const float* mean, const float* components, char* scratch,
+                   float* range, void* cuda_stream) {
+    const std::string api = std::string("f3dgs_") + fn;
+    t_error.clear();
+    if (!pca_sizes_ok(C, N)) return fail(F3DGS_ERR_INVALID_ARGUMENT, api + ": bad sizes (3 <= C <= 1024, N >= 7)");
+    if (!x || !mean || !components || !scratch || !range) return fail(F3DGS_ERR_INVALID_ARGUMENT, api + ": NULL pointer");
+    const Range rx{x, (size_t)C * N * sizeof(X)}, rm{mean, (size_t)C * 4}, rc{components, (size_t)3 * C * 4};
+    const Range rs{scratch, pca_scratch_fixed_bytes(C, N)}, rr{range, 8};
+    if (any_overlap(rs, {rx, rm, rc}) || any_overlap(rr, {rx, rm, rc, rs}))
+        return fail(F3DGS_ERR_INVALID_ARGUMENT, api + ": scratch or range overlaps an input");
+    size_t sb = 0;
+    CUDA_TRY(pca_scratch_bytes(C, N, &sb));  // the sort's share of the scratch is sized by CUB for the current device
+    if (any_overlap({scratch, sb}, {rx, rm, rc, rr}))
+        return fail(F3DGS_ERR_INVALID_ARGUMENT, api + ": scratch or range overlaps an input");
+    cudaError_t e = launch_pca_range(C, N, x, mean, components, scratch, range, (cudaStream_t)cuda_stream);
+    if (e != cudaSuccess) return fail(F3DGS_ERR_CUDA, std::string(fn) + ": " + cudaGetErrorString(e));
+    return 0;
+}
+
+template <typename X>
+int pca_image_impl(const char* fn, int C, int N, const X* x, const float* mean, const float* components,
+                   const float* range, float* image, void* cuda_stream) {
+    const std::string api = std::string("f3dgs_") + fn;
+    t_error.clear();
+    if (!pca_sizes_ok(C, N)) return fail(F3DGS_ERR_INVALID_ARGUMENT, api + ": bad sizes (3 <= C <= 1024, N >= 7)");
+    if (!x || !mean || !components || !range || !image) return fail(F3DGS_ERR_INVALID_ARGUMENT, api + ": NULL pointer");
+    const Range ri{image, (size_t)N * 3 * 4};
+    if (any_overlap(ri, {{x, (size_t)C * N * sizeof(X)}, {mean, (size_t)C * 4}, {components, (size_t)3 * C * 4},
+                         {range, 8}}))
+        return fail(F3DGS_ERR_INVALID_ARGUMENT, api + ": image overlaps an input");
+    cudaError_t e = launch_pca_image(C, N, x, mean, components, range, image, (cudaStream_t)cuda_stream);
+    if (e != cudaSuccess) return fail(F3DGS_ERR_CUDA, std::string(fn) + ": " + cudaGetErrorString(e));
+    return 0;
+}
 }  // namespace
 
 extern "C" {
@@ -715,6 +780,50 @@ int f3dgs_feature_query_f16x(int C, int D, int K, int N, const float* weight, co
                              float* prob, float* logits, void* cuda_stream) {
     return feature_query_impl("feature_query_f16x", C, D, K, N, weight, bias, reinterpret_cast<const __half*>(x), text,
                               logit_scale, positive, labels, prob, logits, cuda_stream);
+}
+
+size_t f3dgs_feature_pca_scratch_bytes(int C, int N) {
+    t_error.clear();
+    if (!pca_sizes_ok(C, N)) return 0;
+    size_t bytes = 0;
+    const cudaError_t e = pca_scratch_bytes(C, N, &bytes);
+    if (e != cudaSuccess) {
+        fail(F3DGS_ERR_CUDA, std::string("f3dgs_feature_pca_scratch_bytes: ") + cudaGetErrorString(e));
+        return 0;
+    }
+    return bytes;
+}
+
+int f3dgs_feature_pca_moments(int C, int N, const float* x, char* scratch, float* mean, double* cov, void* cuda_stream) {
+    return pca_moments_impl("feature_pca_moments", C, N, x, scratch, mean, cov, cuda_stream);
+}
+
+int f3dgs_feature_pca_moments_f16x(int C, int N, const uint16_t* x, char* scratch, float* mean, double* cov,
+                                   void* cuda_stream) {
+    return pca_moments_impl("feature_pca_moments_f16x", C, N, reinterpret_cast<const __half*>(x), scratch, mean, cov,
+                            cuda_stream);
+}
+
+int f3dgs_feature_pca_range(int C, int N, const float* x, const float* mean, const float* components, char* scratch,
+                            float* range, void* cuda_stream) {
+    return pca_range_impl("feature_pca_range", C, N, x, mean, components, scratch, range, cuda_stream);
+}
+
+int f3dgs_feature_pca_range_f16x(int C, int N, const uint16_t* x, const float* mean, const float* components,
+                                 char* scratch, float* range, void* cuda_stream) {
+    return pca_range_impl("feature_pca_range_f16x", C, N, reinterpret_cast<const __half*>(x), mean, components, scratch,
+                          range, cuda_stream);
+}
+
+int f3dgs_feature_pca_image(int C, int N, const float* x, const float* mean, const float* components,
+                            const float* range, float* image, void* cuda_stream) {
+    return pca_image_impl("feature_pca_image", C, N, x, mean, components, range, image, cuda_stream);
+}
+
+int f3dgs_feature_pca_image_f16x(int C, int N, const uint16_t* x, const float* mean, const float* components,
+                                 const float* range, float* image, void* cuda_stream) {
+    return pca_image_impl("feature_pca_image_f16x", C, N, reinterpret_cast<const __half*>(x), mean, components, range,
+                          image, cuda_stream);
 }
 
 size_t f3dgs_knn_scratch_bytes(int P) {

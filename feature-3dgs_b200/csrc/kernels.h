@@ -107,6 +107,22 @@ cudaError_t launch_feature_query(int C, int D, int K, int N, const float* weight
                                  const float* text, float logit_scale, const uint8_t* positive, int64_t* labels,
                                  float* prob, float* logits, cudaStream_t s);
 
+// ---- feature_pca.cu: PCA picture of a feature map x [C,N] (float16 x is upcast exactly).  scratch is
+// pca_scratch_bytes(C, N) bytes, whose first pca_scratch_fixed_bytes(C, N) need no device query to size
+constexpr int kPcaMinC = 3, kPcaMaxC = 1024;
+cudaError_t pca_scratch_bytes(int C, int N, size_t* bytes);
+size_t pca_scratch_fixed_bytes(int C, int N);
+cudaError_t launch_pca_moments(int C, int N, const float* x, char* scratch, float* mean, double* cov, cudaStream_t s);
+cudaError_t launch_pca_moments(int C, int N, const __half* x, char* scratch, float* mean, double* cov, cudaStream_t s);
+cudaError_t launch_pca_range(int C, int N, const float* x, const float* mean, const float* comp, char* scratch,
+                             float* range, cudaStream_t s);
+cudaError_t launch_pca_range(int C, int N, const __half* x, const float* mean, const float* comp, char* scratch,
+                             float* range, cudaStream_t s);
+cudaError_t launch_pca_image(int C, int N, const float* x, const float* mean, const float* comp, const float* range,
+                             float* image, cudaStream_t s);
+cudaError_t launch_pca_image(int C, int N, const __half* x, const float* mean, const float* comp, const float* range,
+                             float* image, cudaStream_t s);
+
 // ---- knn.cu: exact mean squared distance to the 3 nearest other points (distCUDA2); scratch is knn_scratch_bytes(P)
 // bytes whose first knn_scratch_fixed_bytes(P) need no device query to size
 cudaError_t knn_scratch_bytes(int P, size_t* bytes);

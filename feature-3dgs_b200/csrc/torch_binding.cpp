@@ -482,6 +482,100 @@ std::tuple<torch::Tensor, torch::Tensor, torch::Tensor> featureQuery(const torch
     return std::make_tuple(labels, prob, logits);
 }
 
+// ---- feature PCA (f3dgs_feature_pca_*): x [C,H,W] or [C,N], a contiguous float32 or float16 CUDA tensor, read in
+// place (never copied); mean [C] and components [3,C] contiguous float32, range [2] float32, all on x's device
+struct PcaX {
+    torch::Tensor x;
+    int C, N;
+    bool half;
+};
+
+PcaX pca_x(const torch::Tensor& x, const char* fn) {
+    TORCH_CHECK(x.is_cuda() && (x.scalar_type() == torch::kFloat32 || x.scalar_type() == torch::kFloat16) &&
+                    (x.dim() == 2 || x.dim() == 3) && x.is_contiguous(),
+                fn, ": x must be a contiguous float32 or float16 CUDA tensor [C,H,W] or [C,N]");
+    const int64_t C = x.size(0), N = x.numel() / std::max<int64_t>(C, 1);
+    TORCH_CHECK(C >= 3 && C <= 1024 && N >= 7 && N <= INT32_MAX, fn,
+                ": needs 3 <= C <= 1024 channels and N >= 7 pixels (at least 3 samples), got C = ", C, ", N = ", N);
+    return {x, (int)C, (int)N, x.scalar_type() == torch::kFloat16};
+}
+
+void pca_check_f32(const torch::Tensor& t, const PcaX& px, int64_t numel, const char* fn, const char* what) {
+    TORCH_CHECK(t.is_cuda() && t.device() == px.x.device() && t.scalar_type() == torch::kFloat32 && t.is_contiguous() &&
+                    t.numel() == numel,
+                fn, ": ", what, " must be a contiguous float32 tensor of ", numel, " elements on ", px.x.device());
+}
+
+torch::Tensor pca_scratch(const PcaX& px) {
+    const size_t bytes = f3dgs_feature_pca_scratch_bytes(px.C, px.N);
+    TORCH_CHECK(bytes > 0, "f3dgs_feature_pca_scratch_bytes failed: ", f3dgs_last_error());
+    return torch::empty({(int64_t)bytes}, px.x.options().dtype(torch::kByte));
+}
+
+// -> (mean [C] float32, cov [C,C] float64)
+std::tuple<torch::Tensor, torch::Tensor> featurePcaMoments(const torch::Tensor& x) {
+    const PcaX px = pca_x(x, "feature_pca_moments");
+    const c10::cuda::CUDAGuard guard(x.device());
+    torch::Tensor scratch = pca_scratch(px);
+    torch::Tensor mean = torch::empty({px.C}, x.options().dtype(torch::kFloat32));
+    torch::Tensor cov = torch::empty({px.C, px.C}, x.options().dtype(torch::kFloat64));
+    char* sp = reinterpret_cast<char*>(scratch.data_ptr());
+    void* stream = (void*)c10::cuda::getCurrentCUDAStream().stream();
+    if (px.half)
+        check_rc(f3dgs_feature_pca_moments_f16x(px.C, px.N, hptr(x), sp, mean.data_ptr<float>(),
+                                                cov.data_ptr<double>(), stream),
+                 "f3dgs_feature_pca_moments_f16x");
+    else
+        check_rc(f3dgs_feature_pca_moments(px.C, px.N, fptr(x), sp, mean.data_ptr<float>(), cov.data_ptr<double>(),
+                                           stream),
+                 "f3dgs_feature_pca_moments");
+    return std::make_tuple(mean, cov);
+}
+
+// -> range [2] float32 = (lo, hi)
+torch::Tensor featurePcaRange(const torch::Tensor& x, const torch::Tensor& mean, const torch::Tensor& components) {
+    const PcaX px = pca_x(x, "feature_pca_range");
+    pca_check_f32(mean, px, px.C, "feature_pca_range", "mean");
+    pca_check_f32(components, px, 3 * (int64_t)px.C, "feature_pca_range", "components");
+    const c10::cuda::CUDAGuard guard(x.device());
+    torch::Tensor scratch = pca_scratch(px);
+    torch::Tensor range = torch::empty({2}, x.options().dtype(torch::kFloat32));
+    char* sp = reinterpret_cast<char*>(scratch.data_ptr());
+    void* stream = (void*)c10::cuda::getCurrentCUDAStream().stream();
+    if (px.half)
+        check_rc(f3dgs_feature_pca_range_f16x(px.C, px.N, hptr(x), fptr(mean), fptr(components), sp,
+                                              range.data_ptr<float>(), stream),
+                 "f3dgs_feature_pca_range_f16x");
+    else
+        check_rc(f3dgs_feature_pca_range(px.C, px.N, fptr(x), fptr(mean), fptr(components), sp,
+                                         range.data_ptr<float>(), stream),
+                 "f3dgs_feature_pca_range");
+    return range;
+}
+
+// -> image [H,W,3] or [N,3] float32
+torch::Tensor featurePcaImage(const torch::Tensor& x, const torch::Tensor& mean, const torch::Tensor& components,
+                              const torch::Tensor& range) {
+    const PcaX px = pca_x(x, "feature_pca_image");
+    pca_check_f32(mean, px, px.C, "feature_pca_image", "mean");
+    pca_check_f32(components, px, 3 * (int64_t)px.C, "feature_pca_image", "components");
+    pca_check_f32(range, px, 2, "feature_pca_image", "range");
+    const c10::cuda::CUDAGuard guard(x.device());
+    auto shape = x.sizes().slice(1).vec();
+    shape.push_back(3);
+    torch::Tensor image = torch::empty(shape, x.options().dtype(torch::kFloat32));
+    void* stream = (void*)c10::cuda::getCurrentCUDAStream().stream();
+    if (px.half)
+        check_rc(f3dgs_feature_pca_image_f16x(px.C, px.N, hptr(x), fptr(mean), fptr(components), fptr(range),
+                                              image.data_ptr<float>(), stream),
+                 "f3dgs_feature_pca_image_f16x");
+    else
+        check_rc(f3dgs_feature_pca_image(px.C, px.N, fptr(x), fptr(mean), fptr(components), fptr(range),
+                                         image.data_ptr<float>(), stream),
+                 "f3dgs_feature_pca_image");
+    return image;
+}
+
 // ---- initial scales (f3dgs_knn_mean_dist, the reference's simple_knn distCUDA2): points [P,3] -> [P]
 torch::Tensor knnMeanDist(const torch::Tensor& points) {
     TORCH_CHECK(points.is_cuda(), "points must be a CUDA tensor (this build has no CPU path)");
@@ -656,6 +750,9 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     m.def("feature_query", &featureQuery, pybind11::arg("x"), pybind11::arg("text"), pybind11::arg("weight"),
           pybind11::arg("bias"), pybind11::arg("logit_scale"), pybind11::arg("positive"), pybind11::arg("want_labels"),
           pybind11::arg("want_prob"), pybind11::arg("want_logits"));
+    m.def("feature_pca_moments", &featurePcaMoments);
+    m.def("feature_pca_range", &featurePcaRange);
+    m.def("feature_pca_image", &featurePcaImage);
     m.def("knn_mean_dist", &knnMeanDist);
     m.def("densify_plan", &densifyPlan);
     m.def("densify_apply", &densifyApply);

@@ -9,13 +9,16 @@ and dL/d(resized map), and a gather-style resize backward that writes every elem
 With --speedup the 1x1 decoder and its loss run in between on csrc/feature_decoder.cu (TF32 tensor cores, like cuDNN's
 default for the reference's nn.Conv2d): `decode`, `decoded_feature_l1_loss_and_grad`, `decoded_feature_l1_loss`.
 `query` asks the trained field questions with text embeddings (csrc/feature_query.cu): LSeg's per-pixel labels and
-render_edit's per-Gaussian selection score, without materialising the decoded map.
+render_edit's per-Gaussian selection score, without materialising the decoded map.  `pca_fit` and `pca_image` make
+render.py's PCA picture of a feature map on the device (csrc/feature_pca.cu).
 There is no CPU path (the extension raises on CPU tensors).
 
 The teacher map `gt` may be float32 or float16, the dtype the data format stores it in (io.load_feature_map(path,
 dtype=None)).  A float16 map is read as it is and upcast exactly inside the kernels, so no float32 copy is made and every
 result equals the one for `gt.float()`; the loss and the gradients are float32, as PyTorch's `l1_loss(fp32, fp16)` gives.
 """
+from typing import NamedTuple, Optional
+
 import torch
 
 
@@ -144,6 +147,69 @@ def query(features: torch.Tensor, text: torch.Tensor, weight=None, bias=None, lo
                                            _empty(text) if bias is None else bias, float(logit_scale), mask, True,
                                            idx is not None, bool(logits))
     return lab, (prob if idx is not None else None), (lg if logits else None)
+
+
+class FeaturePCA(NamedTuple):
+    """A PCA colour basis of a feature map (device tensors): mean [C] and components [3,C] float32, and the percentile
+    range lo, hi (0-d float32) that maps the projections onto [0, 1]."""
+
+    mean: torch.Tensor
+    components: torch.Tensor
+    lo: torch.Tensor
+    hi: torch.Tensor
+
+
+def _pca_check(x: torch.Tensor, fn: str, fit: Optional[FeaturePCA] = None):
+    if not isinstance(x, torch.Tensor) or x.dim() not in (2, 3):
+        raise ValueError(f"{fn}: x must be a tensor [C,H,W] or [C,N], got {getattr(x, 'shape', type(x))}")
+    if x.dtype not in (torch.float32, torch.float16):
+        raise ValueError(f"{fn}: x must be float32 or float16, got {x.dtype}")
+    C = x.shape[0]
+    N = x.numel() // max(C, 1)
+    if not 3 <= C <= 1024:
+        raise ValueError(f"{fn}: needs 3 <= C <= 1024 channels, got {C}")
+    if (N + 2) // 3 < 3:
+        raise ValueError(f"{fn}: needs at least 3 samples (every 3rd pixel: N >= 7), got N = {N}")
+    if fit is not None and (tuple(fit.mean.shape) != (C,) or tuple(fit.components.shape) != (3, C)):
+        raise ValueError(f"{fn}: the fit has {fit.mean.shape[0]} channels, x has {C}")
+    if not x.is_cuda:
+        raise ValueError(f"{fn}: x must be a CUDA tensor (there is no CPU path)")
+    if not x.is_contiguous():
+        raise ValueError(f"{fn}: x must be contiguous (the map is read in place, never copied)")
+
+
+def pca_fit(x: torch.Tensor) -> FeaturePCA:
+    """Fit render.py's PCA colour basis to a feature map x [C,H,W] or [C,N] (float32, or float16 with bitwise the result
+    of `x.float()`, contiguous), on the device: the pixels are normalised (F.normalize, eps 1e-12), every 3rd pixel
+    (p = y W + x, p % 3 == 0) is a sample, and the fit is scikit-learn's PCA(3) of the samples (components signed so that
+    each one's largest |entry| is positive) with lo, hi = np.percentile(projections of the samples, [1, 99]).  x is read
+    in place; nothing of size C x n is allocated.  One host sync, in the float64 eigensolver of the C x C covariance
+    (torch.linalg.eigh on the device)."""
+    _pca_check(x, "pca_fit")
+    with torch.no_grad():
+        mean, cov = _C().feature_pca_moments(x)
+        # cuSOLVER on the device: at C = 512 it took 4.8 ms against 27-29 ms for LAPACK on the host, copy included
+        # (tools/time_feature_pca.py, H100 80GB HBM3 at 700 W).  Its result check is the fit's one host sync.
+        _, vec = torch.linalg.eigh(cov)
+        comps = vec.flip(1)[:, :3].t()  # the three largest eigenvalues, descending
+        first_max = comps.abs().argmax(dim=1, keepdim=True)  # first maximal |entry|
+        comps = comps * torch.sign(comps.gather(1, first_max))
+        comps = comps.float().contiguous()
+        rng = _C().feature_pca_range(x, mean, comps)
+    return FeaturePCA(mean, comps, rng[0], rng[1])
+
+
+def pca_image(x: torch.Tensor, fit: Optional[FeaturePCA] = None) -> torch.Tensor:
+    """PCA picture of a feature map x [C,H,W] or [C,N] -> [H,W,3] or [N,3] float32 on the device:
+    clamp((c_k . (normalize(x_p) - mean) - lo) / (hi - lo), 0, 1).  fit=None fits on x itself, which is the drop-in for
+    render.py's `feature_visualize_saving(x)` (== `pca_image(x).cpu()`); a fit from `pca_fit` on one frame gives the
+    frames of a video consistent colours.  One read of the map; no autograd."""
+    _pca_check(x, "pca_image", fit)
+    if fit is None:
+        fit = pca_fit(x)
+    with torch.no_grad():
+        rng = torch.stack((fit.lo, fit.hi)).to(device=x.device, dtype=torch.float32)
+        return _C().feature_pca_image(x, fit.mean.contiguous(), fit.components.contiguous(), rng)
 
 
 class _DecodedL1(torch.autograd.Function):

@@ -207,6 +207,39 @@ int f3dgs_feature_query_f16x(int C, int D, int K, int N, const float* weight, co
                              const float* text, float logit_scale, const uint8_t* positive, int64_t* labels,
                              float* prob, float* logits, void* cuda_stream);
 
+/* ---- PCA picture of a feature map: render.py's feature_visualize_saving (render.py:147-180) -----------------------
+ * x [C,N] (a map [C,H,W] as N = H*W pixels, p = y*W + x), 3 <= C <= 1024, N >= 7 (n = ceil(N/3) >= 3 samples: the
+ * pixels p = 3s).  With xh_p = x_p / max(||x_p||, 1e-12):
+ *   f3dgs_feature_pca_moments  mean[C] float32 = the mean of xh over the samples; cov[C,C] float64 =
+ *                              sum over samples of (xh - mean)(xh - mean)^T / (n - 1), symmetric.  Centred on load,
+ *                              fp32 FMA over blocks of 2048 samples, blocks and CTA partials added in fp64 in a fixed order.
+ *   (caller)                   the unit eigenvectors c_1..c_3 of cov for its three largest eigenvalues, descending, each
+ *                              signed so that its entry of largest |value| (the first such) is positive, as float32
+ *                              components[3,C].  This library has no eigensolver: LAPACK dsyevd (or cuSOLVER syevd) on
+ *                              cov is the intended one; cov is fp64 so that the solver sees the accumulated precision.
+ *   f3dgs_feature_pca_range    range[2] float32 = np.percentile(t, [1, 99]) (linear) of the 3n values
+ *                              t = c_k . (xh_s - mean), written on the device (no host sync).
+ *   f3dgs_feature_pca_image    image[N,3] float32: clamp((c_k . (xh_p - mean) - lo) / (hi - lo), 0, 1) for every pixel
+ *                              (lo, hi = range, read on the device; hi == lo gives the IEEE result, NaN stays NaN).
+ * scratch is f3dgs_feature_pca_scratch_bytes(C, N) bytes of device memory, 256-byte aligned, for the moments and range
+ * calls (the size does not depend on x's dtype; 0 for sizes out of range, and 0 with f3dgs_last_error() set if the size
+ * query of the device sort fails).  No output may overlap an input, the scratch or another output.  The _f16x variants
+ * take x as IEEE binary16 bits and give bitwise the result for the exactly upcast x; they validate as their float32
+ * twins, with x's 2-byte size in the overlap checks.  Every call is stream-ordered, launches only device work and is
+ * bitwise reproducible; a map is read once by the image call and about once per pass by the other two. */
+size_t f3dgs_feature_pca_scratch_bytes(int C, int N);
+int f3dgs_feature_pca_moments(int C, int N, const float* x, char* scratch, float* mean, double* cov, void* cuda_stream);
+int f3dgs_feature_pca_moments_f16x(int C, int N, const uint16_t* x, char* scratch, float* mean, double* cov,
+                                   void* cuda_stream);
+int f3dgs_feature_pca_range(int C, int N, const float* x, const float* mean, const float* components, char* scratch,
+                            float* range, void* cuda_stream);
+int f3dgs_feature_pca_range_f16x(int C, int N, const uint16_t* x, const float* mean, const float* components,
+                                 char* scratch, float* range, void* cuda_stream);
+int f3dgs_feature_pca_image(int C, int N, const float* x, const float* mean, const float* components,
+                            const float* range, float* image, void* cuda_stream);
+int f3dgs_feature_pca_image_f16x(int C, int N, const uint16_t* x, const float* mean, const float* components,
+                                 const float* range, float* image, void* cuda_stream);
+
 /* ---- photometric loss: reference train.py (colour term), utils/loss_utils.py l1_loss + ssim(window_size=11) ---------
  * loss = (1 - lambda_dssim) * l1_loss(image, gt) + lambda_dssim * (1 - ssim(image, gt)).  image, gt [planes,H,W]; the
  * SSIM window is the 11-tap Gaussian (sigma 1.5) per plane with zero padding, C1 = 0.01^2, C2 = 0.03^2.
