@@ -28,12 +28,38 @@ namespace {
 
 thread_local std::string t_error;
 
-int fail(int code, const std::string& msg) {
-    t_error = msg;
-    return -code;
-}
+// Every entry point that can fail opens an Api named after itself (__func__).  Opening it clears the calling thread's last
+// error; a failure records "f3dgs_<entry>: <message>" as the last error and returns the negated error code.
+struct Api {
+    const char* entry;
+    explicit Api(const char* name) : entry(name) { t_error.clear(); }
+    int fail(int code, const std::string& msg) const {
+        t_error = std::string(entry) + ": " + msg;
+        return -code;
+    }
+    int invalid(const std::string& msg) const { return fail(F3DGS_ERR_INVALID_ARGUMENT, msg); }
+    // 0 if a CUDA call or launch succeeded, else its failure, with `what` (if any) naming the step
+    int cuda(cudaError_t e, const char* what = nullptr) const {
+        if (e == cudaSuccess) return 0;
+        return fail(F3DGS_ERR_CUDA, what ? std::string(what) + ": " + cudaGetErrorString(e) : cudaGetErrorString(e));
+    }
+};
 
-inline size_t align_up(size_t x, size_t a = 256) { return (x + a - 1) / a * a; }
+// A byte range [p, p + bytes) of a caller's buffer; a NULL buffer is absent and overlaps nothing.
+struct Range {
+    const void* p;
+    size_t bytes;
+};
+
+// Does the output range `out` share a byte with any of the ranges `in`?
+template <size_t N>
+bool overlaps(const Range& out, const Range (&in)[N]) {
+    for (const Range& r : in) {
+        const uintptr_t x = (uintptr_t)out.p, y = (uintptr_t)r.p;
+        if (out.p && r.p && x < y + r.bytes && y < x + out.bytes) return true;
+    }
+    return false;
+}
 
 // ---- optional per-stage timing with CUDA events on the launch stream
 struct StageRec {
@@ -132,11 +158,10 @@ inline int bit_length(uint32_t n) {
     return b;
 }
 
+// both macros report through the entry point's `api`
 #define CUDA_TRY(expr)                                                                              \
     do {                                                                                            \
-        cudaError_t e_ = (expr);                                                                    \
-        if (e_ != cudaSuccess)                                                                      \
-            return fail(F3DGS_ERR_CUDA, std::string(#expr) + ": " + cudaGetErrorString(e_));        \
+        if (const int rc_ = api.cuda((expr), #expr)) return rc_;                                    \
     } while (0)
 
 // reference CHECK_CUDA (auxiliary.h:172-179): in debug mode synchronise and surface errors per stage
@@ -144,8 +169,7 @@ inline int bit_length(uint32_t n) {
     do {                                                                                            \
         cudaError_t e_ = cudaGetLastError();                                                        \
         if (e_ == cudaSuccess && debug) e_ = cudaStreamSynchronize(stream);                         \
-        if (e_ != cudaSuccess)                                                                      \
-            return fail(F3DGS_ERR_CUDA, std::string("stage ") + name + ": " + cudaGetErrorString(e_)); \
+        if (const int rc_ = api.cuda(e_, "stage " name)) return rc_;                                \
     } while (0)
 
 ViewParams make_view(int P, int D, int M, int C, int width, int height, float tan_fovx, float tan_fovy,
@@ -177,13 +201,14 @@ void f3dgs_profile_enable(int on) {
 }
 
 int f3dgs_profile_read(double* ms, unsigned long long* count) {
-    if (!ms || !count) return fail(F3DGS_ERR_INVALID_ARGUMENT, "f3dgs_profile_read: NULL output");
+    const Api api(__func__);
+    if (!ms || !count) return api.invalid("NULL output");
     std::lock_guard<std::mutex> lk(g_profile_mu);
     for (const StageRec& r : g_recs) {
         float t = 0.f;
         cudaError_t e = cudaEventSynchronize(r.e1);
         if (e == cudaSuccess) e = cudaEventElapsedTime(&t, r.e0, r.e1);
-        if (e != cudaSuccess) return fail(F3DGS_ERR_CUDA, std::string("profile_read: ") + cudaGetErrorString(e));
+        if (const int rc = api.cuda(e)) return rc;
         if (r.stage >= 0 && r.stage < F3DGS_N_STAGES) {
             ms[r.stage] += t;
             count[r.stage] += 1;
@@ -196,8 +221,8 @@ int f3dgs_profile_read(double* ms, unsigned long long* count) {
 }
 
 int f3dgs_get_layout(int P, int width, int height, int R, f3dgs_layout* out) {
-    if (!out || P < 0 || width <= 0 || height <= 0 || R < 0)
-        return fail(F3DGS_ERR_INVALID_ARGUMENT, "f3dgs_get_layout: bad argument");
+    const Api api(__func__);
+    if (!out || P < 0 || width <= 0 || height <= 0 || R < 0) return api.invalid("bad argument");
     const GeomLayout g((size_t)P);
     const size_t tiles = (size_t)((width + 15) / 16) * ((height + 15) / 16);
     const ImgLayout im((size_t)width * height, tiles);
@@ -219,25 +244,23 @@ int f3dgs_forward(f3dgs_alloc_fn geometry_alloc, void* geometry_ctx, f3dgs_alloc
                   const float* viewmatrix, const float* projmatrix, const float* cam_pos, float tan_fovx,
                   float tan_fovy, int prefiltered, float* out_color, float* out_feature_map, float* out_depth,
                   int* radii, int debug, void* cuda_stream) {
-    t_error.clear();
+    const Api api(__func__);
     cudaStream_t stream = (cudaStream_t)cuda_stream;
     if (P < 0 || width <= 0 || height <= 0 || C < 0 || C > F3DGS_MAX_FEATURE_DIM || D < 0 || D > 3)
-        return fail(F3DGS_ERR_INVALID_ARGUMENT, "f3dgs_forward: bad sizes (P, width, height, C or D)");
+        return api.invalid("bad sizes (P, width, height, C or D)");
     if (!geometry_alloc || !binning_alloc || !image_alloc)
-        return fail(F3DGS_ERR_INVALID_ARGUMENT, "f3dgs_forward: missing allocator");
+        return api.invalid("missing allocator");
     if (P == 0) return 0;
     if (!means3D || !opacities || !background || !viewmatrix || !projmatrix || !cam_pos || !out_color ||
         !out_depth)
-        return fail(F3DGS_ERR_INVALID_ARGUMENT, "f3dgs_forward: NULL required pointer");
+        return api.invalid("NULL required pointer");
     if ((shs == nullptr) == (colors_precomp == nullptr))
-        return fail(F3DGS_ERR_INVALID_ARGUMENT, "f3dgs_forward: provide exactly one of shs / colors_precomp");
+        return api.invalid("provide exactly one of shs / colors_precomp");
     if (((scales == nullptr) || (rotations == nullptr)) == (cov3D_precomp == nullptr))
-        return fail(F3DGS_ERR_INVALID_ARGUMENT,
-                    "f3dgs_forward: provide exactly one of (scales, rotations) / cov3D_precomp");
+        return api.invalid("provide exactly one of (scales, rotations) / cov3D_precomp");
     if (C > 0 && (!semantic_feature || !out_feature_map))
-        return fail(F3DGS_ERR_INVALID_ARGUMENT, "f3dgs_forward: C > 0 needs semantic_feature and out_feature_map");
-    if (shs && M < (D + 1) * (D + 1))
-        return fail(F3DGS_ERR_INVALID_ARGUMENT, "f3dgs_forward: M < (D+1)^2 SH coefficients");
+        return api.invalid("C > 0 needs semantic_feature and out_feature_map");
+    if (shs && M < (D + 1) * (D + 1)) return api.invalid("M < (D+1)^2 SH coefficients");
 
     const ViewParams vp = make_view(P, D, M, C, width, height, tan_fovx, tan_fovy, scale_modifier, viewmatrix,
                                     projmatrix, cam_pos);
@@ -248,7 +271,7 @@ int f3dgs_forward(f3dgs_alloc_fn geometry_alloc, void* geometry_ctx, f3dgs_alloc
     size_t scan_bytes = 0;
     CUDA_TRY(cub::DeviceScan::InclusiveSum(nullptr, scan_bytes, (uint32_t*)nullptr, (uint32_t*)nullptr, P, stream));
     char* geom = geometry_alloc(geometry_ctx, gl.fixed_bytes + align_up(scan_bytes));
-    if (!geom) return fail(F3DGS_ERR_ALLOC, "geometry allocator returned NULL");
+    if (!geom) return api.fail(F3DGS_ERR_ALLOC, "geometry allocator returned NULL");
     SplatRec* rec = reinterpret_cast<SplatRec*>(geom + gl.rec);
     float* cov3d = reinterpret_cast<float*>(geom + gl.cov3d);
     uint8_t* clamped = reinterpret_cast<uint8_t*>(geom + gl.clamped);
@@ -260,7 +283,7 @@ int f3dgs_forward(f3dgs_alloc_fn geometry_alloc, void* geometry_ctx, f3dgs_alloc
     // ---- image buffer
     const ImgLayout il((size_t)width * height, tiles);
     char* img = image_alloc(image_ctx, il.bytes);
-    if (!img) return fail(F3DGS_ERR_ALLOC, "image allocator returned NULL");
+    if (!img) return api.fail(F3DGS_ERR_ALLOC, "image allocator returned NULL");
     float* final_T = reinterpret_cast<float*>(img + il.final_T);
     uint32_t* n_contrib = reinterpret_cast<uint32_t*>(img + il.n_contrib);
     uint2* ranges = reinterpret_cast<uint2*>(img + il.ranges);
@@ -290,7 +313,7 @@ int f3dgs_forward(f3dgs_alloc_fn geometry_alloc, void* geometry_ctx, f3dgs_alloc
     CUDA_TRY(cudaMemcpyAsync(h_count, offsets + (P - 1), sizeof(int), cudaMemcpyDeviceToHost, stream));
     CUDA_TRY(cudaStreamSynchronize(stream));
     const int R = *h_count;
-    if (R < 0) return fail(F3DGS_ERR_CUDA, "num_rendered overflowed int32");
+    if (R < 0) return api.fail(F3DGS_ERR_CUDA, "num_rendered overflowed int32");
 
     // ---- binning buffer
     const BinLayout bl((size_t)R);
@@ -299,7 +322,7 @@ int f3dgs_forward(f3dgs_alloc_fn geometry_alloc, void* geometry_ctx, f3dgs_alloc
     CUDA_TRY(cub::DeviceRadixSort::SortPairs(nullptr, sort_bytes, (uint64_t*)nullptr, (uint64_t*)nullptr,
                                              (uint32_t*)nullptr, (uint32_t*)nullptr, R, 0, end_bit, stream));
     char* bin = binning_alloc(binning_ctx, bl.fixed_bytes + align_up(sort_bytes));
-    if (!bin) return fail(F3DGS_ERR_ALLOC, "binning allocator returned NULL");
+    if (!bin) return api.fail(F3DGS_ERR_ALLOC, "binning allocator returned NULL");
     uint32_t* point_list = reinterpret_cast<uint32_t*>(bin + bl.point_list);
     uint64_t* keys = reinterpret_cast<uint64_t*>(bin + bl.keys);
     uint32_t* point_list_unsorted = reinterpret_cast<uint32_t*>(bin + bl.point_list_unsorted);
@@ -333,7 +356,7 @@ int f3dgs_forward(f3dgs_alloc_fn geometry_alloc, void* geometry_ctx, f3dgs_alloc
         e = launch_composite_fwd(vp, ranges, point_list, rec, semantic_feature, background, final_T, n_contrib,
                                  out_color, out_feature_map, out_depth, counters, stream);
     }
-    if (e != cudaSuccess) return fail(F3DGS_ERR_CUDA, std::string("composite_fwd launch: ") + cudaGetErrorString(e));
+    if (const int rc = api.cuda(e, "composite_fwd launch")) return rc;
     STAGE_CHECK("composite_fwd");
     return R;
 }
@@ -357,7 +380,7 @@ struct ScratchLayout {  // per-view intermediates of the accumulating backward (
 
 // Shared body of f3dgs_backward (accumulate = false: the reference's assign-into-zeroed-buffers contract) and
 // f3dgs_backward_accum (accumulate = true: += into the caller's per-parameter gradient buffers).
-int backward_impl(const char* who, bool accumulate, int P, int D, int M, int R, int C, const float* background, int width,
+int backward_impl(const Api& api, bool accumulate, int P, int D, int M, int R, int C, const float* background, int width,
                   int height, const float* means3D, const float* shs, const float* scales, float scale_modifier,
                   const float* rotations, const float* cov3D_precomp, const float* viewmatrix, const float* projmatrix,
                   const float* cam_pos, float tan_fovx, float tan_fovy, const int* radii, char* geom_buffer,
@@ -366,20 +389,17 @@ int backward_impl(const char* who, bool accumulate, int P, int D, int M, int R, 
                   float* dL_dsemantic_feature, float* dL_dmean3D, float* dL_dcov3D, float* dL_dsh, float* dL_dscale,
                   float* dL_drot, float* dL_dz, float* grad_accum, float* denom, cudaEvent_t composite_done, int debug,
                   cudaStream_t stream) {
-    const std::string w(who);
     if (P < 0 || width <= 0 || height <= 0 || C < 0 || C > F3DGS_MAX_FEATURE_DIM || R < 0)
-        return fail(F3DGS_ERR_INVALID_ARGUMENT, w + ": bad sizes");
+        return api.invalid("bad sizes");
     if (P == 0) return 0;
-    if (!geom_buffer || !binning_buffer || !image_buffer)
-        return fail(F3DGS_ERR_INVALID_ARGUMENT, w + ": missing forward buffers");
+    if (!geom_buffer || !binning_buffer || !image_buffer) return api.invalid("missing forward buffers");
     if (!dL_dpix || !dL_depths || (C > 0 && (!dL_dfeaturepix || !dL_dsemantic_feature)) || !dL_dmean2D ||
         !dL_dconic || !dL_dopacity || !dL_dcolor || !dL_dmean3D || !dL_dcov3D || !dL_dz)
-        return fail(F3DGS_ERR_INVALID_ARGUMENT, w + ": NULL gradient pointer");
-    if (shs && !dL_dsh) return fail(F3DGS_ERR_INVALID_ARGUMENT, w + ": shs given but dL_dsh NULL");
+        return api.invalid("NULL gradient pointer");
+    if (shs && !dL_dsh) return api.invalid("shs given but dL_dsh NULL");
     if (scales && (!rotations || !dL_dscale || !dL_drot))
-        return fail(F3DGS_ERR_INVALID_ARGUMENT, w + ": scales given but rotations/dL_dscale/dL_drot NULL");
-    if ((grad_accum == nullptr) != (denom == nullptr))
-        return fail(F3DGS_ERR_INVALID_ARGUMENT, w + ": grad_accum and denom go together");
+        return api.invalid("scales given but rotations/dL_dscale/dL_drot NULL");
+    if ((grad_accum == nullptr) != (denom == nullptr)) return api.invalid("grad_accum and denom go together");
 
     const ViewParams vp = make_view(P, D, M, C, width, height, tan_fovx, tan_fovy, scale_modifier, viewmatrix,
                                     projmatrix, cam_pos);
@@ -420,9 +440,9 @@ int backward_impl(const char* who, bool accumulate, int P, int D, int M, int R, 
             });
             cudaError_t ea = cudaMallocAsync((void**)&lists, ll.bytes, stream);
             if (ea != cudaSuccess)
-                return fail(F3DGS_ERR_ALLOC, w + ": cudaMallocAsync of " + std::to_string(ll.bytes) +
-                                                 " bytes for the backward instance lists failed: " +
-                                                 cudaGetErrorString(ea));
+                return api.fail(F3DGS_ERR_ALLOC, "cudaMallocAsync of " + std::to_string(ll.bytes) +
+                                                     " bytes for the backward instance lists failed: " +
+                                                     cudaGetErrorString(ea));
         }
         e = launch_composite_bwd_geom(
             vp, ranges, point_list, rec, background, final_T, n_contrib, dL_dpix, dL_depths, dL_dmean2D, dL_dconic,
@@ -436,7 +456,7 @@ int backward_impl(const char* who, bool accumulate, int P, int D, int M, int R, 
                                    dL_dsemantic_feature, counters + 48, stream);
         if (lists) cudaFreeAsync(lists, stream);
     }
-    if (e != cudaSuccess) return fail(F3DGS_ERR_CUDA, std::string("composite_bwd launch: ") + cudaGetErrorString(e));
+    if (const int rc = api.cuda(e, "composite_bwd launch")) return rc;
     STAGE_CHECK("composite_bwd");
     if (composite_done) CUDA_TRY(cudaEventRecord(composite_done, stream));
     {
@@ -465,8 +485,7 @@ int f3dgs_backward(int P, int D, int M, int R, int C, const float* background, i
                    float* dL_dz, int debug, void* cuda_stream) {
     (void)semantic_feature;  // not needed: dL/dfeature depends only on the blend weights (SURVEY D.1/D.2)
     (void)colors_precomp;    // colours were copied into the per-Gaussian records by the forward
-    t_error.clear();
-    return backward_impl("f3dgs_backward", false, P, D, M, R, C, background, width, height, means3D, shs, scales,
+    return backward_impl(Api(__func__), false, P, D, M, R, C, background, width, height, means3D, shs, scales,
                          scale_modifier, rotations, cov3D_precomp, viewmatrix, projmatrix, cam_pos, tan_fovx, tan_fovy,
                          radii, geom_buffer, binning_buffer, image_buffer, dL_dpix, dL_dfeaturepix, dL_depths, dL_dmean2D,
                          dL_dconic, dL_dopacity, dL_dcolor, dL_dsemantic_feature, dL_dmean3D, dL_dcov3D, dL_dsh, dL_dscale,
@@ -485,14 +504,13 @@ int f3dgs_backward_accum(int P, int D, int M, int R, int C, const float* backgro
                          float* dL_dcov3D_precomp, float* dL_dsh, float* dL_dscale, float* dL_drot,
                          float* dL_dmean2D_out, float* grad_accum, float* denom, void* composite_done_event, int debug,
                          void* cuda_stream) {
-    t_error.clear();
+    const Api api(__func__);
     cudaStream_t stream = (cudaStream_t)cuda_stream;
-    if (P <= 0) return P == 0 ? 0 : fail(F3DGS_ERR_INVALID_ARGUMENT, "f3dgs_backward_accum: bad sizes");
-    if (!scratch) return fail(F3DGS_ERR_INVALID_ARGUMENT, "f3dgs_backward_accum: NULL scratch");
+    if (P <= 0) return P == 0 ? 0 : api.invalid("bad sizes");
+    if (!scratch) return api.invalid("NULL scratch");
     if ((colors_precomp != nullptr) != (dL_dcolors_precomp != nullptr) ||
         (cov3D_precomp != nullptr) != (dL_dcov3D_precomp != nullptr))
-        return fail(F3DGS_ERR_INVALID_ARGUMENT,
-                    "f3dgs_backward_accum: dL_dcolors_precomp / dL_dcov3D_precomp go with colors_precomp / cov3D_precomp");
+        return api.invalid("dL_dcolors_precomp / dL_dcov3D_precomp go with colors_precomp / cov3D_precomp");
     const ScratchLayout sl((size_t)P);
     CUDA_TRY(cudaMemsetAsync(scratch, 0, sl.bytes, stream));
     float* m2d = reinterpret_cast<float*>(scratch + sl.mean2D);
@@ -500,7 +518,7 @@ int f3dgs_backward_accum(int P, int D, int M, int R, int C, const float* backgro
     float* dcol = dL_dcolors_precomp ? dL_dcolors_precomp : reinterpret_cast<float*>(scratch + sl.color);
     float* dcov = dL_dcov3D_precomp ? dL_dcov3D_precomp : reinterpret_cast<float*>(scratch + sl.cov3D);
     const int rc = backward_impl(
-        "f3dgs_backward_accum", true, P, D, M, R, C, background, width, height, means3D, shs, scales, scale_modifier,
+        api, true, P, D, M, R, C, background, width, height, means3D, shs, scales, scale_modifier,
         rotations, cov3D_precomp, viewmatrix, projmatrix, cam_pos, tan_fovx, tan_fovy, radii, geom_buffer,
         binning_buffer, image_buffer, dL_dpix, dL_dfeaturepix, dL_depths, m2d,
         reinterpret_cast<float*>(scratch + sl.conic), dL_dopacity, dcol, dL_dsemantic_feature, dL_dmean3D, dcov, dL_dsh,
@@ -515,33 +533,24 @@ int f3dgs_backward_accum(int P, int D, int M, int R, int C, const float* backgro
 }  // extern "C"
 
 namespace {
-bool ranges_overlap(const void* a, size_t na, const void* b, size_t nb) {
-    if (!a || !b) return false;
-    const uintptr_t x = (uintptr_t)a, y = (uintptr_t)b;
-    return x < y + nb && y < x + na;
-}
-
-// The float16 entry points (_f16gt, _f16) validate and launch as their float32 twins do; `fn` is the twin's name without
-// the f3dgs_ prefix.  Half data is IEEE binary16 bits at the ABI (uint16_t) and __half in the kernels.
+// The float16 entry points (_f16gt, _f16, _f16x) validate and launch as their float32 twins do.  Half data is IEEE
+// binary16 bits at the ABI (uint16_t) and __half in the kernels.
 template <typename GT>
-int feature_resize_fwd_impl(const char* fn, int C, int H, int W, int Hg, int Wg, const float* feature_map, const GT* gt,
-                            float grad_scale, float* out, float* loss_sum, void* cuda_stream) {
-    const std::string api = std::string("f3dgs_") + fn;
-    t_error.clear();
-    if (C < 0 || H <= 0 || W <= 0 || Hg <= 0 || Wg <= 0) return fail(F3DGS_ERR_INVALID_ARGUMENT, api + ": bad sizes");
+int feature_resize_fwd_impl(const char* entry, int C, int H, int W, int Hg, int Wg, const float* feature_map,
+                            const GT* gt, float grad_scale, float* out, float* loss_sum, void* cuda_stream) {
+    const Api api(entry);
+    if (C < 0 || H <= 0 || W <= 0 || Hg <= 0 || Wg <= 0) return api.invalid("bad sizes");
     if (C == 0) return 0;
-    if (!feature_map || !out) return fail(F3DGS_ERR_INVALID_ARGUMENT, api + ": NULL pointer");
+    if (!feature_map || !out) return api.invalid("NULL pointer");
     if constexpr (std::is_same_v<GT, __half>) {
         // no target is the float32 symbol's job; out's 4-byte elements cannot alias gt's 2-byte ones element for element
-        if (!gt) return fail(F3DGS_ERR_INVALID_ARGUMENT, api + ": NULL pointer (gt is required)");
+        if (!gt) return api.invalid("NULL pointer (gt is required)");
         const size_t n = (size_t)C * Hg * Wg;
-        if (ranges_overlap(out, n * 4, feature_map, (size_t)C * H * W * 4) || ranges_overlap(out, n * 4, gt, n * 2))
-            return fail(F3DGS_ERR_INVALID_ARGUMENT, api + ": out overlaps feature_map or gt");
+        if (overlaps({out, n * 4}, {{feature_map, (size_t)C * H * W * 4}, {gt, n * 2}}))
+            return api.invalid("out overlaps feature_map or gt");
     }
-    cudaError_t e = launch_feature_resize_fwd(C, H, W, Hg, Wg, feature_map, gt, grad_scale, out, loss_sum,
-                                              (cudaStream_t)cuda_stream);
-    if (e != cudaSuccess) return fail(F3DGS_ERR_CUDA, std::string(fn) + ": " + cudaGetErrorString(e));
-    return 0;
+    return api.cuda(launch_feature_resize_fwd(C, H, W, Hg, Wg, feature_map, gt, grad_scale, out, loss_sum,
+                                              (cudaStream_t)cuda_stream));
 }
 }  // namespace
 
@@ -549,195 +558,149 @@ extern "C" {
 
 int f3dgs_feature_resize_fwd(int C, int H, int W, int Hg, int Wg, const float* feature_map, const float* gt,
                              float grad_scale, float* out, float* loss_sum, void* cuda_stream) {
-    return feature_resize_fwd_impl("feature_resize_fwd", C, H, W, Hg, Wg, feature_map, gt, grad_scale, out, loss_sum,
-                                   cuda_stream);
+    return feature_resize_fwd_impl(__func__, C, H, W, Hg, Wg, feature_map, gt, grad_scale, out, loss_sum, cuda_stream);
 }
 
 int f3dgs_feature_resize_fwd_f16gt(int C, int H, int W, int Hg, int Wg, const float* feature_map, const uint16_t* gt,
                                    float grad_scale, float* out, float* loss_sum, void* cuda_stream) {
-    return feature_resize_fwd_impl("feature_resize_fwd_f16gt", C, H, W, Hg, Wg, feature_map,
-                                   reinterpret_cast<const __half*>(gt), grad_scale, out, loss_sum, cuda_stream);
+    return feature_resize_fwd_impl(__func__, C, H, W, Hg, Wg, feature_map, reinterpret_cast<const __half*>(gt),
+                                   grad_scale, out, loss_sum, cuda_stream);
 }
 
 int f3dgs_feature_resize_bwd(int C, int H, int W, int Hg, int Wg, const float* dout, float* dL_dfeature_map,
                              void* cuda_stream) {
-    t_error.clear();
-    if (C < 0 || H <= 0 || W <= 0 || Hg <= 0 || Wg <= 0)
-        return fail(F3DGS_ERR_INVALID_ARGUMENT, "f3dgs_feature_resize_bwd: bad sizes");
+    const Api api(__func__);
+    if (C < 0 || H <= 0 || W <= 0 || Hg <= 0 || Wg <= 0) return api.invalid("bad sizes");
     if (C == 0) return 0;
-    if (!dout || !dL_dfeature_map) return fail(F3DGS_ERR_INVALID_ARGUMENT, "f3dgs_feature_resize_bwd: NULL pointer");
-    cudaError_t e = launch_feature_resize_bwd(C, H, W, Hg, Wg, dout, dL_dfeature_map, (cudaStream_t)cuda_stream);
-    if (e != cudaSuccess) return fail(F3DGS_ERR_CUDA, std::string("feature_resize_bwd: ") + cudaGetErrorString(e));
-    return 0;
+    if (!dout || !dL_dfeature_map) return api.invalid("NULL pointer");
+    return api.cuda(launch_feature_resize_bwd(C, H, W, Hg, Wg, dout, dL_dfeature_map, (cudaStream_t)cuda_stream));
 }
 
 int f3dgs_image_loss(int planes, int H, int W, const float* image, const float* gt, float w_l1, float w_ssim, float* sums,
                      float* dL_dimage, void* cuda_stream) {
-    t_error.clear();
-    if (planes < 0 || H <= 0 || W <= 0) return fail(F3DGS_ERR_INVALID_ARGUMENT, "f3dgs_image_loss: bad sizes");
+    const Api api(__func__);
+    if (planes < 0 || H <= 0 || W <= 0) return api.invalid("bad sizes");
     if (planes == 0) return 0;
-    if (!image_loss_grid_ok(planes, H, W))
-        return fail(F3DGS_ERR_INVALID_ARGUMENT, "f3dgs_image_loss: sizes exceed the launch grid limits");
-    if (!image || !gt || !sums) return fail(F3DGS_ERR_INVALID_ARGUMENT, "f3dgs_image_loss: NULL pointer");
-    if (dL_dimage) {  // a CTA reads its neighbours' pixels (the window halo), so the gradient cannot overwrite an input
-        const uintptr_t n = (uintptr_t)planes * H * W * sizeof(float), d = (uintptr_t)dL_dimage;
-        auto overlaps = [&](const float* p) { return d < (uintptr_t)p + n && (uintptr_t)p < d + n; };
-        if (overlaps(image) || overlaps(gt))
-            return fail(F3DGS_ERR_INVALID_ARGUMENT, "f3dgs_image_loss: dL_dimage overlaps image or gt");
-    }
-    cudaError_t e = launch_image_loss(planes, H, W, image, gt, w_l1, w_ssim, sums, dL_dimage, (cudaStream_t)cuda_stream);
-    if (e != cudaSuccess) return fail(F3DGS_ERR_CUDA, std::string("image_loss: ") + cudaGetErrorString(e));
-    return 0;
+    if (!image_loss_grid_ok(planes, H, W)) return api.invalid("sizes exceed the launch grid limits");
+    if (!image || !gt || !sums) return api.invalid("NULL pointer");
+    // a CTA reads its neighbours' pixels (the window halo), so the gradient cannot overwrite an input
+    const size_t n = (size_t)planes * H * W * sizeof(float);
+    if (overlaps({dL_dimage, n}, {{image, n}, {gt, n}})) return api.invalid("dL_dimage overlaps image or gt");
+    return api.cuda(launch_image_loss(planes, H, W, image, gt, w_l1, w_ssim, sums, dL_dimage, (cudaStream_t)cuda_stream));
 }
 
 }  // extern "C"
 
 namespace {
 template <typename Y>
-int decoder_forward_impl(const char* fn, int Cin, int Cout, int N, const float* weight, const float* bias, const float* x,
-                         Y* y, void* cuda_stream) {
-    const std::string api = std::string("f3dgs_") + fn;
-    t_error.clear();
+int decoder_forward_impl(const char* entry, int Cin, int Cout, int N, const float* weight, const float* bias,
+                         const float* x, Y* y, void* cuda_stream) {
+    const Api api(entry);
     if (Cin < 1 || Cin > kDecoderMaxCin || Cout < 1 || Cout > kDecoderMaxCout || N < 1)
-        return fail(F3DGS_ERR_INVALID_ARGUMENT, api + ": bad sizes (1 <= Cin <= 256, 1 <= Cout <= 4096, N >= 1)");
-    if (!decoder_grid_ok(Cin, Cout, N))
-        return fail(F3DGS_ERR_INVALID_ARGUMENT, api + ": sizes exceed the launch grid limits");
-    if (!weight || !x || !y) return fail(F3DGS_ERR_INVALID_ARGUMENT, api + ": NULL pointer");
-    const size_t ny = (size_t)Cout * N * sizeof(Y);
-    if (ranges_overlap(y, ny, weight, (size_t)Cout * Cin * 4) || ranges_overlap(y, ny, bias, (size_t)Cout * 4) ||
-        ranges_overlap(y, ny, x, (size_t)Cin * N * 4))
-        return fail(F3DGS_ERR_INVALID_ARGUMENT, api + ": y overlaps an input");
-    cudaError_t e = launch_decoder_forward(Cin, Cout, N, weight, bias, x, y, (cudaStream_t)cuda_stream);
-    if (e != cudaSuccess) return fail(F3DGS_ERR_CUDA, std::string(fn) + ": " + cudaGetErrorString(e));
-    return 0;
+        return api.invalid("bad sizes (1 <= Cin <= 256, 1 <= Cout <= 4096, N >= 1)");
+    if (!decoder_grid_ok(Cin, Cout, N)) return api.invalid("sizes exceed the launch grid limits");
+    if (!weight || !x || !y) return api.invalid("NULL pointer");
+    if (overlaps({y, (size_t)Cout * N * sizeof(Y)},
+                 {{weight, (size_t)Cout * Cin * 4}, {bias, (size_t)Cout * 4}, {x, (size_t)Cin * N * 4}}))
+        return api.invalid("y overlaps an input");
+    return api.cuda(launch_decoder_forward(Cin, Cout, N, weight, bias, x, y, (cudaStream_t)cuda_stream));
 }
 
 template <typename GT>
-int decoder_l1_impl(const char* fn, int Cin, int Cout, int N, const float* weight, const float* bias, const float* x,
+int decoder_l1_impl(const char* entry, int Cin, int Cout, int N, const float* weight, const float* bias, const float* x,
                     const GT* gt, float grad_scale, float* loss_sum, float* dL_dx, float* dL_dweight, float* dL_dbias,
                     void* cuda_stream) {
-    const std::string api = std::string("f3dgs_") + fn;
-    t_error.clear();
+    const Api api(entry);
     if (Cin < 1 || Cin > kDecoderMaxCin || Cout < 1 || Cout > kDecoderMaxCout || N < 1)
-        return fail(F3DGS_ERR_INVALID_ARGUMENT, api + ": bad sizes (1 <= Cin <= 256, 1 <= Cout <= 4096, N >= 1)");
-    if (!decoder_grid_ok(Cin, Cout, N))
-        return fail(F3DGS_ERR_INVALID_ARGUMENT, api + ": sizes exceed the launch grid limits");
-    if (!weight || !x || !gt || !loss_sum || !dL_dx || !dL_dweight)
-        return fail(F3DGS_ERR_INVALID_ARGUMENT, api + ": NULL pointer");
-    if ((bias == nullptr) != (dL_dbias == nullptr))
-        return fail(F3DGS_ERR_INVALID_ARGUMENT, api + ": NULL pointer (dL_dbias goes with bias)");
+        return api.invalid("bad sizes (1 <= Cin <= 256, 1 <= Cout <= 4096, N >= 1)");
+    if (!decoder_grid_ok(Cin, Cout, N)) return api.invalid("sizes exceed the launch grid limits");
+    if (!weight || !x || !gt || !loss_sum || !dL_dx || !dL_dweight) return api.invalid("NULL pointer");
+    if ((bias == nullptr) != (dL_dbias == nullptr)) return api.invalid("NULL pointer (dL_dbias goes with bias)");
     const size_t nx = (size_t)Cin * N * 4, nw = (size_t)Cout * Cin * 4, nb = (size_t)Cout * 4;
     // a warp reads x of its own pixels only, but kernel B reads all of x after dL_dx is written
-    if (ranges_overlap(dL_dx, nx, x, nx) || ranges_overlap(dL_dx, nx, gt, (size_t)Cout * N * sizeof(GT)) ||
-        ranges_overlap(dL_dx, nx, weight, nw) || ranges_overlap(dL_dx, nx, bias, nb) ||
-        ranges_overlap(dL_dx, nx, dL_dweight, nw) || ranges_overlap(dL_dx, nx, dL_dbias, nb))
-        return fail(F3DGS_ERR_INVALID_ARGUMENT, api + ": dL_dx overlaps an input");
-    cudaError_t e = launch_decoder_l1(Cin, Cout, N, weight, bias, x, gt, grad_scale, loss_sum, dL_dx, dL_dweight,
-                                      dL_dbias, (cudaStream_t)cuda_stream);
-    if (e != cudaSuccess) return fail(F3DGS_ERR_CUDA, std::string(fn) + ": " + cudaGetErrorString(e));
-    return 0;
+    if (overlaps({dL_dx, nx}, {{x, nx}, {gt, (size_t)Cout * N * sizeof(GT)}, {weight, nw}, {bias, nb},
+                               {dL_dweight, nw}, {dL_dbias, nb}}))
+        return api.invalid("dL_dx overlaps an input");
+    return api.cuda(launch_decoder_l1(Cin, Cout, N, weight, bias, x, gt, grad_scale, loss_sum, dL_dx, dL_dweight,
+                                      dL_dbias, (cudaStream_t)cuda_stream));
 }
 
 template <typename X>
-int feature_query_impl(const char* fn, int C, int D, int K, int N, const float* weight, const float* bias, const X* x,
+int feature_query_impl(const char* entry, int C, int D, int K, int N, const float* weight, const float* bias, const X* x,
                        const float* text, float logit_scale, const uint8_t* positive, int64_t* labels, float* prob,
                        float* logits, void* cuda_stream) {
-    const std::string api = std::string("f3dgs_") + fn;
-    t_error.clear();
+    const Api api(entry);
     if (K < 1 || K > kQueryMaxK || D < 1 || D > kQueryMaxD || C < 1 || N < 0 || (weight && C > kDecoderMaxCin))
-        return fail(F3DGS_ERR_INVALID_ARGUMENT,
-                    api + ": bad sizes (1 <= K <= 256, 1 <= D <= 4096, N >= 0, 1 <= C <= 256 with a decoder)");
-    if (!weight && D != C) return fail(F3DGS_ERR_INVALID_ARGUMENT, api + ": D != C needs a decoder weight");
-    if (bias && !weight) return fail(F3DGS_ERR_INVALID_ARGUMENT, api + ": bias without weight");
-    if (!x || !text) return fail(F3DGS_ERR_INVALID_ARGUMENT, api + ": NULL pointer (x and text are required)");
-    if (!labels && !prob && !logits) return fail(F3DGS_ERR_INVALID_ARGUMENT, api + ": no output requested");
-    if (prob && !positive) return fail(F3DGS_ERR_INVALID_ARGUMENT, api + ": prob needs a positive set");
-    if (!std::isfinite(logit_scale)) return fail(F3DGS_ERR_INVALID_ARGUMENT, api + ": logit_scale is not finite");
+        return api.invalid("bad sizes (1 <= K <= 256, 1 <= D <= 4096, N >= 0, 1 <= C <= 256 with a decoder)");
+    if (!weight && D != C) return api.invalid("D != C needs a decoder weight");
+    if (bias && !weight) return api.invalid("bias without weight");
+    if (!x || !text) return api.invalid("NULL pointer (x and text are required)");
+    if (!labels && !prob && !logits) return api.invalid("no output requested");
+    if (prob && !positive) return api.invalid("prob needs a positive set");
+    if (!std::isfinite(logit_scale)) return api.invalid("logit_scale is not finite");
     const size_t n = (size_t)N;
-    struct Range {
-        const void* p;
-        size_t bytes;
-    };
     const Range in[] = {{weight, (size_t)D * C * 4}, {bias, (size_t)D * 4}, {x, (size_t)C * n * sizeof(X)},
                         {text, (size_t)K * D * 4}, {positive, (size_t)K}};
     const Range out[] = {{labels, n * 8}, {prob, n * 4}, {logits, (size_t)K * n * 4}};
     for (int i = 0; i < 3; i++) {
-        for (const Range& r : in)
-            if (ranges_overlap(out[i].p, out[i].bytes, r.p, r.bytes))
-                return fail(F3DGS_ERR_INVALID_ARGUMENT, api + ": an output overlaps an input");
+        if (overlaps(out[i], in)) return api.invalid("an output overlaps an input");
         for (int j = 0; j < i; j++)
-            if (ranges_overlap(out[i].p, out[i].bytes, out[j].p, out[j].bytes))
-                return fail(F3DGS_ERR_INVALID_ARGUMENT, api + ": outputs overlap");
+            if (overlaps(out[i], {out[j]})) return api.invalid("outputs overlap");
     }
-    cudaError_t e = launch_feature_query(C, D, K, N, weight, bias, x, text, logit_scale, positive, labels, prob, logits,
-                                         (cudaStream_t)cuda_stream);
-    if (e != cudaSuccess) return fail(F3DGS_ERR_CUDA, std::string(fn) + ": " + cudaGetErrorString(e));
-    return 0;
+    return api.cuda(launch_feature_query(C, D, K, N, weight, bias, x, text, logit_scale, positive, labels, prob, logits,
+                                         (cudaStream_t)cuda_stream));
 }
 
-// ---- feature PCA: shared validation of (C, N) and of output ranges against inputs
+// ---- feature PCA: shared validation of (C, N)
 bool pca_sizes_ok(int C, int N) { return C >= kPcaMinC && C <= kPcaMaxC && N >= 7; }  // n = ceil(N / 3) >= 3
 
-struct Range {
-    const void* p;
-    size_t bytes;
-};
-bool any_overlap(const Range& out, std::initializer_list<Range> in) {
-    for (const Range& r : in)
-        if (ranges_overlap(out.p, out.bytes, r.p, r.bytes)) return true;
-    return false;
-}
-
 template <typename X>
-int pca_moments_impl(const char* fn, int C, int N, const X* x, char* scratch, float* mean, double* cov,
+int pca_moments_impl(const char* entry, int C, int N, const X* x, char* scratch, float* mean, double* cov,
                      void* cuda_stream) {
-    const std::string api = std::string("f3dgs_") + fn;
-    t_error.clear();
-    if (!pca_sizes_ok(C, N)) return fail(F3DGS_ERR_INVALID_ARGUMENT, api + ": bad sizes (3 <= C <= 1024, N >= 7)");
-    if (!x || !scratch || !mean || !cov) return fail(F3DGS_ERR_INVALID_ARGUMENT, api + ": NULL pointer");
+    const Api api(entry);
+    if (!pca_sizes_ok(C, N)) return api.invalid("bad sizes (3 <= C <= 1024, N >= 7)");
+    if (!x || !scratch || !mean || !cov) return api.invalid("NULL pointer");
     const Range rx{x, (size_t)C * N * sizeof(X)}, rs{scratch, pca_scratch_fixed_bytes(C, N)};
     const Range rm{mean, (size_t)C * 4}, rc{cov, (size_t)C * C * 8};
-    if (any_overlap(rs, {rx}) || any_overlap(rm, {rx, rs}) || any_overlap(rc, {rx, rs, rm}))
-        return fail(F3DGS_ERR_INVALID_ARGUMENT, api + ": scratch, mean and cov must not overlap x or each other");
-    cudaError_t e = launch_pca_moments(C, N, x, scratch, mean, cov, (cudaStream_t)cuda_stream);
-    if (e != cudaSuccess) return fail(F3DGS_ERR_CUDA, std::string(fn) + ": " + cudaGetErrorString(e));
-    return 0;
+    if (overlaps(rs, {rx}) || overlaps(rm, {rx, rs}) || overlaps(rc, {rx, rs, rm}))
+        return api.invalid("scratch, mean and cov must not overlap x or each other");
+    return api.cuda(launch_pca_moments(C, N, x, scratch, mean, cov, (cudaStream_t)cuda_stream));
 }
 
 template <typename X>
-int pca_range_impl(const char* fn, int C, int N, const X* x, const float* mean, const float* components, char* scratch,
+int pca_range_impl(const char* entry, int C, int N, const X* x, const float* mean, const float* components, char* scratch,
                    float* range, void* cuda_stream) {
-    const std::string api = std::string("f3dgs_") + fn;
-    t_error.clear();
-    if (!pca_sizes_ok(C, N)) return fail(F3DGS_ERR_INVALID_ARGUMENT, api + ": bad sizes (3 <= C <= 1024, N >= 7)");
-    if (!x || !mean || !components || !scratch || !range) return fail(F3DGS_ERR_INVALID_ARGUMENT, api + ": NULL pointer");
+    const Api api(entry);
+    if (!pca_sizes_ok(C, N)) return api.invalid("bad sizes (3 <= C <= 1024, N >= 7)");
+    if (!x || !mean || !components || !scratch || !range) return api.invalid("NULL pointer");
     const Range rx{x, (size_t)C * N * sizeof(X)}, rm{mean, (size_t)C * 4}, rc{components, (size_t)3 * C * 4};
     const Range rs{scratch, pca_scratch_fixed_bytes(C, N)}, rr{range, 8};
-    if (any_overlap(rs, {rx, rm, rc}) || any_overlap(rr, {rx, rm, rc, rs}))
-        return fail(F3DGS_ERR_INVALID_ARGUMENT, api + ": scratch or range overlaps an input");
+    if (overlaps(rs, {rx, rm, rc}) || overlaps(rr, {rx, rm, rc, rs}))
+        return api.invalid("scratch or range overlaps an input");
     size_t sb = 0;
     CUDA_TRY(pca_scratch_bytes(C, N, &sb));  // the sort's share of the scratch is sized by CUB for the current device
-    if (any_overlap({scratch, sb}, {rx, rm, rc, rr}))
-        return fail(F3DGS_ERR_INVALID_ARGUMENT, api + ": scratch or range overlaps an input");
-    cudaError_t e = launch_pca_range(C, N, x, mean, components, scratch, range, (cudaStream_t)cuda_stream);
-    if (e != cudaSuccess) return fail(F3DGS_ERR_CUDA, std::string(fn) + ": " + cudaGetErrorString(e));
-    return 0;
+    if (overlaps({scratch, sb}, {rx, rm, rc, rr})) return api.invalid("scratch or range overlaps an input");
+    return api.cuda(launch_pca_range(C, N, x, mean, components, scratch, range, (cudaStream_t)cuda_stream));
 }
 
 template <typename X>
-int pca_image_impl(const char* fn, int C, int N, const X* x, const float* mean, const float* components,
+int pca_image_impl(const char* entry, int C, int N, const X* x, const float* mean, const float* components,
                    const float* range, float* image, void* cuda_stream) {
-    const std::string api = std::string("f3dgs_") + fn;
-    t_error.clear();
-    if (!pca_sizes_ok(C, N)) return fail(F3DGS_ERR_INVALID_ARGUMENT, api + ": bad sizes (3 <= C <= 1024, N >= 7)");
-    if (!x || !mean || !components || !range || !image) return fail(F3DGS_ERR_INVALID_ARGUMENT, api + ": NULL pointer");
-    const Range ri{image, (size_t)N * 3 * 4};
-    if (any_overlap(ri, {{x, (size_t)C * N * sizeof(X)}, {mean, (size_t)C * 4}, {components, (size_t)3 * C * 4},
-                         {range, 8}}))
-        return fail(F3DGS_ERR_INVALID_ARGUMENT, api + ": image overlaps an input");
-    cudaError_t e = launch_pca_image(C, N, x, mean, components, range, image, (cudaStream_t)cuda_stream);
-    if (e != cudaSuccess) return fail(F3DGS_ERR_CUDA, std::string(fn) + ": " + cudaGetErrorString(e));
-    return 0;
+    const Api api(entry);
+    if (!pca_sizes_ok(C, N)) return api.invalid("bad sizes (3 <= C <= 1024, N >= 7)");
+    if (!x || !mean || !components || !range || !image) return api.invalid("NULL pointer");
+    if (overlaps({image, (size_t)N * 3 * 4}, {{x, (size_t)C * N * sizeof(X)}, {mean, (size_t)C * 4},
+                                              {components, (size_t)3 * C * 4}, {range, 8}}))
+        return api.invalid("image overlaps an input");
+    return api.cuda(launch_pca_image(C, N, x, mean, components, range, image, (cudaStream_t)cuda_stream));
+}
+
+// Body of the *_scratch_bytes entry points: `query` sizes the scratch; 0, with the last error set, if it fails.
+template <typename Query>
+size_t scratch_bytes(const char* entry, Query query) {
+    const Api api(entry);
+    size_t bytes = 0;
+    return api.cuda(query(&bytes)) == 0 ? bytes : 0;
 }
 }  // namespace
 
@@ -745,154 +708,124 @@ extern "C" {
 
 int f3dgs_decoder_forward(int Cin, int Cout, int N, const float* weight, const float* bias, const float* x, float* y,
                           void* cuda_stream) {
-    return decoder_forward_impl("decoder_forward", Cin, Cout, N, weight, bias, x, y, cuda_stream);
+    return decoder_forward_impl(__func__, Cin, Cout, N, weight, bias, x, y, cuda_stream);
 }
 
 int f3dgs_decoder_forward_f16(int Cin, int Cout, int N, const float* weight, const float* bias, const float* x,
                               uint16_t* y, void* cuda_stream) {
-    return decoder_forward_impl("decoder_forward_f16", Cin, Cout, N, weight, bias, x, reinterpret_cast<__half*>(y),
-                                cuda_stream);
+    return decoder_forward_impl(__func__, Cin, Cout, N, weight, bias, x, reinterpret_cast<__half*>(y), cuda_stream);
 }
 
 int f3dgs_decoder_l1(int Cin, int Cout, int N, const float* weight, const float* bias, const float* x, const float* gt,
                      float grad_scale, float* loss_sum, float* dL_dx, float* dL_dweight, float* dL_dbias,
                      void* cuda_stream) {
-    return decoder_l1_impl("decoder_l1", Cin, Cout, N, weight, bias, x, gt, grad_scale, loss_sum, dL_dx, dL_dweight,
+    return decoder_l1_impl(__func__, Cin, Cout, N, weight, bias, x, gt, grad_scale, loss_sum, dL_dx, dL_dweight,
                            dL_dbias, cuda_stream);
 }
 
 int f3dgs_decoder_l1_f16gt(int Cin, int Cout, int N, const float* weight, const float* bias, const float* x,
                            const uint16_t* gt, float grad_scale, float* loss_sum, float* dL_dx, float* dL_dweight,
                            float* dL_dbias, void* cuda_stream) {
-    return decoder_l1_impl("decoder_l1_f16gt", Cin, Cout, N, weight, bias, x, reinterpret_cast<const __half*>(gt),
-                           grad_scale, loss_sum, dL_dx, dL_dweight, dL_dbias, cuda_stream);
+    return decoder_l1_impl(__func__, Cin, Cout, N, weight, bias, x, reinterpret_cast<const __half*>(gt), grad_scale,
+                           loss_sum, dL_dx, dL_dweight, dL_dbias, cuda_stream);
 }
 
 int f3dgs_feature_query(int C, int D, int K, int N, const float* weight, const float* bias, const float* x,
                         const float* text, float logit_scale, const uint8_t* positive, int64_t* labels, float* prob,
                         float* logits, void* cuda_stream) {
-    return feature_query_impl("feature_query", C, D, K, N, weight, bias, x, text, logit_scale, positive, labels, prob,
-                              logits, cuda_stream);
+    return feature_query_impl(__func__, C, D, K, N, weight, bias, x, text, logit_scale, positive, labels, prob, logits,
+                              cuda_stream);
 }
 
 int f3dgs_feature_query_f16x(int C, int D, int K, int N, const float* weight, const float* bias, const uint16_t* x,
                              const float* text, float logit_scale, const uint8_t* positive, int64_t* labels,
                              float* prob, float* logits, void* cuda_stream) {
-    return feature_query_impl("feature_query_f16x", C, D, K, N, weight, bias, reinterpret_cast<const __half*>(x), text,
-                              logit_scale, positive, labels, prob, logits, cuda_stream);
+    return feature_query_impl(__func__, C, D, K, N, weight, bias, reinterpret_cast<const __half*>(x), text, logit_scale,
+                              positive, labels, prob, logits, cuda_stream);
 }
 
 size_t f3dgs_feature_pca_scratch_bytes(int C, int N) {
-    t_error.clear();
-    if (!pca_sizes_ok(C, N)) return 0;
-    size_t bytes = 0;
-    const cudaError_t e = pca_scratch_bytes(C, N, &bytes);
-    if (e != cudaSuccess) {
-        fail(F3DGS_ERR_CUDA, std::string("f3dgs_feature_pca_scratch_bytes: ") + cudaGetErrorString(e));
-        return 0;
-    }
-    return bytes;
+    return scratch_bytes(__func__,
+                         [=](size_t* b) { return pca_sizes_ok(C, N) ? pca_scratch_bytes(C, N, b) : cudaSuccess; });
 }
 
 int f3dgs_feature_pca_moments(int C, int N, const float* x, char* scratch, float* mean, double* cov, void* cuda_stream) {
-    return pca_moments_impl("feature_pca_moments", C, N, x, scratch, mean, cov, cuda_stream);
+    return pca_moments_impl(__func__, C, N, x, scratch, mean, cov, cuda_stream);
 }
 
 int f3dgs_feature_pca_moments_f16x(int C, int N, const uint16_t* x, char* scratch, float* mean, double* cov,
                                    void* cuda_stream) {
-    return pca_moments_impl("feature_pca_moments_f16x", C, N, reinterpret_cast<const __half*>(x), scratch, mean, cov,
-                            cuda_stream);
+    return pca_moments_impl(__func__, C, N, reinterpret_cast<const __half*>(x), scratch, mean, cov, cuda_stream);
 }
 
 int f3dgs_feature_pca_range(int C, int N, const float* x, const float* mean, const float* components, char* scratch,
                             float* range, void* cuda_stream) {
-    return pca_range_impl("feature_pca_range", C, N, x, mean, components, scratch, range, cuda_stream);
+    return pca_range_impl(__func__, C, N, x, mean, components, scratch, range, cuda_stream);
 }
 
 int f3dgs_feature_pca_range_f16x(int C, int N, const uint16_t* x, const float* mean, const float* components,
                                  char* scratch, float* range, void* cuda_stream) {
-    return pca_range_impl("feature_pca_range_f16x", C, N, reinterpret_cast<const __half*>(x), mean, components, scratch,
-                          range, cuda_stream);
+    return pca_range_impl(__func__, C, N, reinterpret_cast<const __half*>(x), mean, components, scratch, range,
+                          cuda_stream);
 }
 
 int f3dgs_feature_pca_image(int C, int N, const float* x, const float* mean, const float* components,
                             const float* range, float* image, void* cuda_stream) {
-    return pca_image_impl("feature_pca_image", C, N, x, mean, components, range, image, cuda_stream);
+    return pca_image_impl(__func__, C, N, x, mean, components, range, image, cuda_stream);
 }
 
 int f3dgs_feature_pca_image_f16x(int C, int N, const uint16_t* x, const float* mean, const float* components,
                                  const float* range, float* image, void* cuda_stream) {
-    return pca_image_impl("feature_pca_image_f16x", C, N, reinterpret_cast<const __half*>(x), mean, components, range,
-                          image, cuda_stream);
+    return pca_image_impl(__func__, C, N, reinterpret_cast<const __half*>(x), mean, components, range, image,
+                          cuda_stream);
 }
 
 size_t f3dgs_knn_scratch_bytes(int P) {
-    t_error.clear();
-    size_t bytes = 0;
-    const cudaError_t e = knn_scratch_bytes(P, &bytes);
-    if (e != cudaSuccess) {
-        fail(F3DGS_ERR_CUDA, std::string("f3dgs_knn_scratch_bytes: ") + cudaGetErrorString(e));
-        return 0;
-    }
-    return bytes;
+    return scratch_bytes(__func__, [=](size_t* b) { return knn_scratch_bytes(P, b); });
 }
 
 int f3dgs_knn_mean_dist(int P, const float* points, float* out, char* scratch, void* cuda_stream) {
-    t_error.clear();
-    if (P < 0) return fail(F3DGS_ERR_INVALID_ARGUMENT, "f3dgs_knn_mean_dist: P < 0");
+    const Api api(__func__);
+    if (P < 0) return api.invalid("P < 0");
     if (P == 0) return 0;
-    if (!points || !out || !scratch) return fail(F3DGS_ERR_INVALID_ARGUMENT, "f3dgs_knn_mean_dist: NULL pointer");
-    const size_t no = (size_t)P * 4;
-    if (ranges_overlap(out, no, points, (size_t)P * 12) || ranges_overlap(out, no, scratch, knn_scratch_fixed_bytes(P)))
-        return fail(F3DGS_ERR_INVALID_ARGUMENT, "f3dgs_knn_mean_dist: out overlaps points or scratch");
+    if (!points || !out || !scratch) return api.invalid("NULL pointer");
+    const Range ro{out, (size_t)P * 4};
+    if (overlaps(ro, {{points, (size_t)P * 12}, {scratch, knn_scratch_fixed_bytes(P)}}))
+        return api.invalid("out overlaps points or scratch");
     size_t sb = 0;
     CUDA_TRY(knn_scratch_bytes(P, &sb));  // the sort's share of the scratch is sized by CUB for the current device
-    if (ranges_overlap(out, no, scratch, sb))
-        return fail(F3DGS_ERR_INVALID_ARGUMENT, "f3dgs_knn_mean_dist: out overlaps points or scratch");
-    cudaError_t e = launch_knn_mean_dist(P, points, out, scratch, (cudaStream_t)cuda_stream);
-    if (e != cudaSuccess) return fail(F3DGS_ERR_CUDA, std::string("knn_mean_dist: ") + cudaGetErrorString(e));
-    return 0;
+    if (overlaps(ro, {{scratch, sb}})) return api.invalid("out overlaps points or scratch");
+    return api.cuda(launch_knn_mean_dist(P, points, out, scratch, (cudaStream_t)cuda_stream));
 }
 
 size_t f3dgs_densify_scratch_bytes(int P) {
-    t_error.clear();
-    size_t bytes = 0;
-    const cudaError_t e = densify_scratch_bytes(P, &bytes);
-    if (e != cudaSuccess) {
-        fail(F3DGS_ERR_CUDA, std::string("f3dgs_densify_scratch_bytes: ") + cudaGetErrorString(e));
-        return 0;
-    }
-    return bytes;
+    return scratch_bytes(__func__, [=](size_t* b) { return densify_scratch_bytes(P, b); });
 }
 
 int f3dgs_densify_plan(int P, const float* grad_accum, const float* denom, const float* raw_opacity,
                        const float* raw_scaling, float max_grad, float dense_scale, float min_opacity,
                        float max_world_scale, char* scratch, int32_t* counts, void* cuda_stream) {
-    t_error.clear();
-    if (P < 0 || 3 * (long long)P > INT_MAX)
-        return fail(F3DGS_ERR_INVALID_ARGUMENT, "f3dgs_densify_plan: bad sizes (0 <= 3 P <= INT_MAX)");
+    const Api api(__func__);
+    if (P < 0 || 3 * (long long)P > INT_MAX) return api.invalid("bad sizes (0 <= 3 P <= INT_MAX)");
     if (!counts || (P > 0 && (!grad_accum || !denom || !raw_opacity || !raw_scaling || !scratch)))
-        return fail(F3DGS_ERR_INVALID_ARGUMENT, "f3dgs_densify_plan: NULL pointer");
-    if (ranges_overlap(counts, 16, scratch, densify_scratch_fixed_bytes(P)))
-        return fail(F3DGS_ERR_INVALID_ARGUMENT, "f3dgs_densify_plan: counts overlaps scratch");
-    cudaError_t e = launch_densify_plan(P, grad_accum, denom, raw_opacity, raw_scaling, max_grad, dense_scale,
-                                        min_opacity, max_world_scale, scratch, counts, (cudaStream_t)cuda_stream);
-    if (e != cudaSuccess) return fail(F3DGS_ERR_CUDA, std::string("densify_plan: ") + cudaGetErrorString(e));
-    return 0;
+        return api.invalid("NULL pointer");
+    if (overlaps({counts, 16}, {{scratch, densify_scratch_fixed_bytes(P)}}))
+        return api.invalid("counts overlaps scratch");
+    return api.cuda(launch_densify_plan(P, grad_accum, denom, raw_opacity, raw_scaling, max_grad, dense_scale,
+                                        min_opacity, max_world_scale, scratch, counts, (cudaStream_t)cuda_stream));
 }
 
 int f3dgs_densify_apply(int P, int M, int C, const char* scratch, const int32_t counts[4], const float* normals,
                         const f3dgs_gaussian_fields src[3], const f3dgs_gaussian_fields dst[3], void* cuda_stream) {
-    t_error.clear();
+    const Api api(__func__);
     if (P < 0 || 3 * (long long)P > INT_MAX || M < 1 || C < 0 || C > F3DGS_MAX_FEATURE_DIM)
-        return fail(F3DGS_ERR_INVALID_ARGUMENT,
-                    "f3dgs_densify_apply: bad sizes (0 <= 3 P <= INT_MAX, M >= 1, 0 <= C <= F3DGS_MAX_FEATURE_DIM)");
-    if (!counts || !src || !dst) return fail(F3DGS_ERR_INVALID_ARGUMENT, "f3dgs_densify_apply: NULL pointer");
+        return api.invalid("bad sizes (0 <= 3 P <= INT_MAX, M >= 1, 0 <= C <= F3DGS_MAX_FEATURE_DIM)");
+    if (!counts || !src || !dst) return api.invalid("NULL pointer");
     const long long A = counts[0], B = counts[1], Cc = counts[2], Ns = counts[3], Pn = A + B + 2 * Cc;
     if (A < 0 || B < 0 || Cc < 0 || A > P || B > P || Cc > Ns || Ns > P || 3 * Pn > INT_MAX)
-        return fail(F3DGS_ERR_INVALID_ARGUMENT, "f3dgs_densify_apply: counts are not those of a plan over P Gaussians");
-    if (Ns > 0 && !normals) return fail(F3DGS_ERR_INVALID_ARGUMENT, "f3dgs_densify_apply: NULL pointer (normals)");
-    if (P > 0 && !scratch) return fail(F3DGS_ERR_INVALID_ARGUMENT, "f3dgs_densify_apply: NULL pointer (scratch)");
+        return api.invalid("counts are not those of a plan over P Gaussians");
+    if (Ns > 0 && !normals) return api.invalid("NULL pointer (normals)");
+    if (P > 0 && !scratch) return api.invalid("NULL pointer (scratch)");
     const size_t width[7] = {3, 3, 3 * (size_t)(M - 1), 1, 3, 4, (size_t)C};
     const float* s[21];
     float* d[21];
@@ -902,49 +835,65 @@ int f3dgs_densify_apply(int P, int M, int C, const char* scratch, const int32_t 
             const float* p[7] = {f[k]->xyz, f[k]->f_dc, f[k]->f_rest, f[k]->opacity, f[k]->scaling, f[k]->rotation,
                                  f[k]->semantic_feature};
             for (int j = 0; j < 7; j++) {
-                if (width[j] && (k ? Pn : P) > 0 && !p[j])
-                    return fail(F3DGS_ERR_INVALID_ARGUMENT, "f3dgs_densify_apply: NULL pointer (a src or dst field)");
+                if (width[j] && (k ? Pn : P) > 0 && !p[j]) return api.invalid("NULL pointer (a src or dst field)");
                 if (k) d[7 * g + j] = const_cast<float*>(p[j]);
                 else s[7 * g + j] = p[j];
             }
         }
     }
-    for (int i = 0; i < 21; i++) {
-        const size_t nd = (size_t)Pn * width[i % 7] * 4;
-        bool bad = ranges_overlap(d[i], nd, scratch, densify_scratch_fixed_bytes(P)) ||
-                   ranges_overlap(d[i], nd, normals, (size_t)Ns * 24);
-        for (int j = 0; j < 21 && !bad; j++) bad = ranges_overlap(d[i], nd, s[j], (size_t)P * width[j % 7] * 4);
-        if (bad)
-            return fail(F3DGS_ERR_INVALID_ARGUMENT, "f3dgs_densify_apply: a dst field overlaps a src field, normals or scratch");
-    }
-    cudaError_t e = launch_densify_apply(P, M, C, scratch, counts, normals, s, d, (cudaStream_t)cuda_stream);
-    if (e != cudaSuccess) return fail(F3DGS_ERR_CUDA, std::string("densify_apply: ") + cudaGetErrorString(e));
-    return 0;
+    Range in[23] = {{scratch, densify_scratch_fixed_bytes(P)}, {normals, (size_t)Ns * 24}};
+    for (int j = 0; j < 21; j++) in[2 + j] = {s[j], (size_t)P * width[j % 7] * 4};
+    for (int i = 0; i < 21; i++)
+        if (overlaps({d[i], (size_t)Pn * width[i % 7] * 4}, in))
+            return api.invalid("a dst field overlaps a src field, normals or scratch");
+    return api.cuda(launch_densify_apply(P, M, C, scratch, counts, normals, s, d, (cudaStream_t)cuda_stream));
 }
 
 int f3dgs_reset_opacity(int P, float* raw_opacity, float* exp_avg, float* exp_avg_sq, float ceiling, void* cuda_stream) {
-    t_error.clear();
-    if (P < 0) return fail(F3DGS_ERR_INVALID_ARGUMENT, "f3dgs_reset_opacity: P < 0");
+    const Api api(__func__);
+    if (P < 0) return api.invalid("P < 0");
     if (P == 0) return 0;
-    if (!raw_opacity || !exp_avg || !exp_avg_sq) return fail(F3DGS_ERR_INVALID_ARGUMENT, "f3dgs_reset_opacity: NULL pointer");
-    cudaError_t e = launch_reset_opacity(P, raw_opacity, exp_avg, exp_avg_sq, ceiling, (cudaStream_t)cuda_stream);
-    if (e != cudaSuccess) return fail(F3DGS_ERR_CUDA, std::string("reset_opacity: ") + cudaGetErrorString(e));
-    return 0;
+    if (!raw_opacity || !exp_avg || !exp_avg_sq) return api.invalid("NULL pointer");
+    return api.cuda(launch_reset_opacity(P, raw_opacity, exp_avg, exp_avg_sq, ceiling, (cudaStream_t)cuda_stream));
+}
+
+int f3dgs_activate(int P, int M, const float* raw_opacity, const float* raw_scaling, const float* raw_rotation,
+                   const float* features_dc, const float* features_rest, float* opacity, float* scales, float* rotations,
+                   float* shs, void* cuda_stream) {
+    const Api api(__func__);
+    if (P < 0 || M < 0) return api.invalid("bad sizes (P < 0 or M < 0)");
+    if (P == 0) return 0;
+    if ((raw_opacity && !opacity) || (raw_scaling && !scales) || (raw_rotation && !rotations) ||
+        (features_dc && (!shs || M < 1 || (M > 1 && !features_rest))))
+        return api.invalid("NULL pointer (an input without its output, or features_dc without shs, M >= 1 and, for "
+                           "M > 1, features_rest)");
+    return api.cuda(launch_activate(P, M, raw_opacity, raw_scaling, raw_rotation, features_dc, features_rest, opacity,
+                                    scales, rotations, shs, (cudaStream_t)cuda_stream));
+}
+
+int f3dgs_adam_step(int kind, size_t n, int M, float* param, const float* grad_activated, float* exp_avg, float* exp_avg_sq,
+                    float lr, float beta1, float beta2, float eps, int step, void* cuda_stream) {
+    const Api api(__func__);
+    if (kind < F3DGS_PARAM_IDENTITY || kind > F3DGS_PARAM_SH_REST) return api.invalid("unknown parameter kind");
+    if (step < 1) return api.invalid("step < 1");
+    if (!param || !grad_activated || !exp_avg || !exp_avg_sq) return api.invalid("NULL pointer");
+    if (kind == F3DGS_PARAM_NORMALIZE4 && (n % 4 != 0)) return api.invalid("n % 4 != 0 for F3DGS_PARAM_NORMALIZE4");
+    if ((kind == F3DGS_PARAM_SH_DC || kind == F3DGS_PARAM_SH_REST) && M < (kind == F3DGS_PARAM_SH_REST ? 2 : 1))
+        return api.invalid("M < 1 for F3DGS_PARAM_SH_DC or M < 2 for F3DGS_PARAM_SH_REST");
+    if (n == 0) return 0;
+    return api.cuda(launch_adam_step(kind, n, M, param, grad_activated, exp_avg, exp_avg_sq, lr, beta1, beta2, eps, step,
+                                     (cudaStream_t)cuda_stream));
 }
 
 int f3dgs_mark_visible(int P, const float* means3D, const float* viewmatrix, const float* projmatrix,
                        uint8_t* present, void* cuda_stream) {
     (void)projmatrix;  // the reference's frustum side test is commented out (auxiliary.h:160)
-    t_error.clear();
-    if (P < 0) return fail(F3DGS_ERR_INVALID_ARGUMENT, "f3dgs_mark_visible: P < 0");
+    const Api api(__func__);
+    if (P < 0) return api.invalid("P < 0");
     if (P == 0) return 0;
-    if (!means3D || !viewmatrix || !present)
-        return fail(F3DGS_ERR_INVALID_ARGUMENT, "f3dgs_mark_visible: NULL pointer");
-    cudaStream_t stream = (cudaStream_t)cuda_stream;
-    launch_mark_visible(P, means3D, viewmatrix, present, stream);
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return fail(F3DGS_ERR_CUDA, std::string("mark_visible: ") + cudaGetErrorString(e));
-    return 0;
+    if (!means3D || !viewmatrix || !present) return api.invalid("NULL pointer");
+    launch_mark_visible(P, means3D, viewmatrix, present, (cudaStream_t)cuda_stream);
+    return api.cuda(cudaGetLastError());
 }
 
 }  // extern "C"

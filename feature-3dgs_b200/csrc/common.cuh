@@ -19,6 +19,12 @@
 
 namespace f3dgs {
 
+// ---------------------------------------------------------------- host launch arithmetic
+// scratch buffers are carved into sub-buffers that start on 256-byte boundaries
+inline size_t align_up(size_t x, size_t a = 256) { return (x + a - 1) / a * a; }
+// CTAs of 256 threads for one thread per work item
+inline unsigned blocks_for(long long threads) { return (unsigned)((threads + 255) / 256); }
+
 // ---------------------------------------------------------------- exact fp32 building blocks
 __device__ __forceinline__ float mulr(float a, float b) { return __fmul_rn(a, b); }
 __device__ __forceinline__ float addr(float a, float b) { return __fadd_rn(a, b); }

@@ -30,8 +30,6 @@ namespace f3dgs {
 
 namespace {
 
-inline size_t align_up(size_t x) { return (x + 255) / 256 * 256; }
-
 struct Add4 {
     __device__ __forceinline__ int4 operator()(const int4& a, const int4& b) const {
         return make_int4(a.x + b.x, a.y + b.y, a.z + b.z, a.w + b.w);
@@ -185,8 +183,6 @@ __global__ void __launch_bounds__(256) reset_opacity_kernel(int P, float* __rest
     m[i] = 0.0f;
     v[i] = 0.0f;
 }
-
-inline unsigned blocks_for(long long threads) { return (unsigned)((threads + 255) / 256); }
 
 }  // namespace
 

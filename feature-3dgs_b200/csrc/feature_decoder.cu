@@ -380,7 +380,6 @@ __global__ void __launch_bounds__(kReduceThreads) decoder_loss_reduce_kernel(con
 }
 
 int kt_of(int Cin) { return Cin <= 32 ? 4 : Cin <= 64 ? 8 : Cin <= 128 ? 16 : 32; }
-size_t round_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
 
 struct Plan {
     int KT, Cp, Cout_pad, N16, gridA, cin_tiles, splits, blk_per_split;
@@ -390,7 +389,7 @@ Plan make_plan(int Cin, int Cout, int N) {
     Plan p;
     p.KT = kt_of(Cin);
     p.Cp = 8 * p.KT;
-    p.Cout_pad = (int)round_up(Cout, kCoutAlign);
+    p.Cout_pad = (int)align_up(Cout, kCoutAlign);
     p.N16 = (N + kPixWarp - 1) / kPixWarp;
     const int pix_a = kPixWarp * kWarpsA / (p.KT <= 16 ? DecSmem<16>::share : DecSmem<32>::share);
     p.gridA = (N + pix_a - 1) / pix_a;
@@ -426,16 +425,16 @@ cudaError_t launch_a_kt(const Plan& p, const DecArgs<T>& a, cudaStream_t s) {
 struct Scratch {
     size_t off_wt = 0, off_bp, off_bits, off_loss, off_pw, off_pb, bytes;
     Scratch(const Plan& p, int Cout, bool loss) {
-        size_t o = round_up((size_t)p.Cout_pad * p.Cp * 4, 256);
+        size_t o = align_up((size_t)p.Cout_pad * p.Cp * 4, 256);
         off_bp = o;
-        o = round_up(o + (size_t)p.Cout_pad * 4, 256);
+        o = align_up(o + (size_t)p.Cout_pad * 4, 256);
         off_bits = off_loss = off_pw = off_pb = o;
         if (loss) {
-            o = round_up(o + (size_t)Cout * p.N16 * 4, 256);
+            o = align_up(o + (size_t)Cout * p.N16 * 4, 256);
             off_loss = o;
-            o = round_up(o + (size_t)p.gridA * 4, 256);
+            o = align_up(o + (size_t)p.gridA * 4, 256);
             off_pw = o;
-            o = round_up(o + (size_t)p.splits * p.Cout_pad * p.Cp * 4, 256);
+            o = align_up(o + (size_t)p.splits * p.Cout_pad * p.Cp * 4, 256);
             off_pb = o;
             o += (size_t)p.splits * p.Cout_pad * 4;
         }
@@ -501,26 +500,23 @@ bool decoder_grid_ok(int Cin, int Cout, int N) {
            (size_t)Cout * Cin + Cout <= (size_t)0x7fffffff * 256;
 }
 
-cudaError_t launch_decoder_forward(int Cin, int Cout, int N, const float* weight, const float* bias, const float* x,
-                                   float* y, cudaStream_t s) {
-    return decoder_run<float>(Cin, Cout, N, weight, bias, x, nullptr, 0.f, y, nullptr, nullptr, nullptr, nullptr, s);
+template <typename Y>
+cudaError_t launch_decoder_forward(int Cin, int Cout, int N, const float* weight, const float* bias, const float* x, Y* y,
+                                   cudaStream_t s) {
+    return decoder_run<Y>(Cin, Cout, N, weight, bias, x, nullptr, 0.f, y, nullptr, nullptr, nullptr, nullptr, s);
 }
+template cudaError_t launch_decoder_forward(int, int, int, const float*, const float*, const float*, float*, cudaStream_t);
+template cudaError_t launch_decoder_forward(int, int, int, const float*, const float*, const float*, __half*, cudaStream_t);
 
-cudaError_t launch_decoder_forward(int Cin, int Cout, int N, const float* weight, const float* bias, const float* x,
-                                   __half* y, cudaStream_t s) {
-    return decoder_run<__half>(Cin, Cout, N, weight, bias, x, nullptr, 0.f, y, nullptr, nullptr, nullptr, nullptr, s);
-}
-
+template <typename GT>
 cudaError_t launch_decoder_l1(int Cin, int Cout, int N, const float* weight, const float* bias, const float* x,
-                              const float* gt, float grad_scale, float* loss_sum, float* dx, float* dW, float* db,
+                              const GT* gt, float grad_scale, float* loss_sum, float* dx, float* dW, float* db,
                               cudaStream_t s) {
-    return decoder_run<float>(Cin, Cout, N, weight, bias, x, gt, grad_scale, nullptr, loss_sum, dx, dW, db, s);
+    return decoder_run<GT>(Cin, Cout, N, weight, bias, x, gt, grad_scale, nullptr, loss_sum, dx, dW, db, s);
 }
-
-cudaError_t launch_decoder_l1(int Cin, int Cout, int N, const float* weight, const float* bias, const float* x,
-                              const __half* gt, float grad_scale, float* loss_sum, float* dx, float* dW, float* db,
-                              cudaStream_t s) {
-    return decoder_run<__half>(Cin, Cout, N, weight, bias, x, gt, grad_scale, nullptr, loss_sum, dx, dW, db, s);
-}
+template cudaError_t launch_decoder_l1(int, int, int, const float*, const float*, const float*, const float*, float, float*,
+                                       float*, float*, float*, cudaStream_t);
+template cudaError_t launch_decoder_l1(int, int, int, const float*, const float*, const float*, const __half*, float,
+                                       float*, float*, float*, float*, cudaStream_t);
 
 }  // namespace f3dgs

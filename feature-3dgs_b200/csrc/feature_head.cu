@@ -25,6 +25,7 @@
 
 #include "../../include/f3dgs_b200.h"
 #include "kernels.h"
+#include "tf32_mma.cuh"
 
 namespace f3dgs {
 namespace {
@@ -41,9 +42,6 @@ __device__ __forceinline__ void src_of(int o, float r, int in, int& i0, int& i1,
     l1 = s - (float)i0;
     l0 = 1.0f - l1;
 }
-
-__device__ __forceinline__ float load_f32(const float* p) { return __ldg(p); }
-__device__ __forceinline__ float load_f32(const __half* p) { return __half2float(__ldg(p)); }
 
 // One warp per output row (c, oy) at a time, lanes strided over ox: the row's channel plane and y taps are computed once per
 // row (no per-element division), a lane's loads are independent across its elements, and consecutive lanes read source
@@ -266,9 +264,11 @@ ResizeGeom make_geom(int C, int H, int W, int Hg, int Wg) {
     return g;
 }
 
+}  // namespace
+
 template <typename GT>
-cudaError_t resize_fwd(int C, int H, int W, int Hg, int Wg, const float* fm, const GT* gt, float grad_scale, float* out,
-                       float* loss_sum, cudaStream_t s) {
+cudaError_t launch_feature_resize_fwd(int C, int H, int W, int Hg, int Wg, const float* fm, const GT* gt, float grad_scale,
+                                      float* out, float* loss_sum, cudaStream_t s) {
     const size_t n = (size_t)C * Hg * Wg;
     if (n == 0) return cudaSuccess;
     int dev = 0, sms = 132;
@@ -281,18 +281,10 @@ cudaError_t resize_fwd(int C, int H, int W, int Hg, int Wg, const float* fm, con
     g_launches++;
     return cudaGetLastError();
 }
-
-}  // namespace
-
-cudaError_t launch_feature_resize_fwd(int C, int H, int W, int Hg, int Wg, const float* fm, const float* gt,
-                                      float grad_scale, float* out, float* loss_sum, cudaStream_t s) {
-    return resize_fwd(C, H, W, Hg, Wg, fm, gt, grad_scale, out, loss_sum, s);
-}
-
-cudaError_t launch_feature_resize_fwd(int C, int H, int W, int Hg, int Wg, const float* fm, const __half* gt,
-                                      float grad_scale, float* out, float* loss_sum, cudaStream_t s) {
-    return resize_fwd(C, H, W, Hg, Wg, fm, gt, grad_scale, out, loss_sum, s);
-}
+template cudaError_t launch_feature_resize_fwd(int, int, int, int, int, const float*, const float*, float, float*, float*,
+                                               cudaStream_t);
+template cudaError_t launch_feature_resize_fwd(int, int, int, int, int, const float*, const __half*, float, float*,
+                                               float*, cudaStream_t);
 
 cudaError_t launch_feature_resize_bwd(int C, int H, int W, int Hg, int Wg, const float* dout, float* dfm, cudaStream_t s) {
     const size_t n = (size_t)C * H * W;

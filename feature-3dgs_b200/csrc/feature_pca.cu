@@ -41,8 +41,6 @@ constexpr int kGS = kGT + 4;         // Gram smem row stride: at most 2-way conf
 constexpr int kGramBlock = 2048;     // samples per fp32 accumulation block
 constexpr int kSms = 132;            // H100 SXM; the Gram kernel runs one CTA per SM (255 registers)
 
-size_t up(size_t v, size_t a = 256) { return (v + a - 1) / a * a; }
-
 int gram_tiles(int C) {
     const int nt = (C + kGT - 1) / kGT;
     return nt * (nt + 1) / 2;
@@ -66,11 +64,11 @@ struct PcaLayout {  // scratch of the moments and range calls; every size is a f
     PcaLayout(int C, int N) {
         const size_t n = ((size_t)N + 2) / 3;
         size_t o = 0;
-        inv = o;     o = up(o + n * 4);
-        mpart = o;   o = up(o + (size_t)moment_ctas((int)n) * C * 8);
-        gpart = o;   o = up(o + (size_t)gram_splits(C, (int)n) * gram_tiles(C) * kGT * kGT * 8);
-        keys = o;    o = up(o + 3 * n * 4);
-        sorted = o;  o = up(o + 3 * n * 4);
+        inv = o;     o = align_up(o + n * 4);
+        mpart = o;   o = align_up(o + (size_t)moment_ctas((int)n) * C * 8);
+        gpart = o;   o = align_up(o + (size_t)gram_splits(C, (int)n) * gram_tiles(C) * kGT * kGT * 8);
+        keys = o;    o = align_up(o + 3 * n * 4);
+        sorted = o;  o = align_up(o + 3 * n * 4);
         sort_tmp = o;
     }
 };
@@ -307,8 +305,21 @@ cudaError_t launch_tile(const TileArgs<T>& a, unsigned grid, cudaStream_t s) {
     return cudaGetLastError();
 }
 
+}  // namespace
+
+size_t pca_scratch_fixed_bytes(int C, int N) { return PcaLayout(C, N).sort_tmp; }
+
+cudaError_t pca_scratch_bytes(int C, int N, size_t* bytes) {
+    *bytes = 0;
+    size_t sb = 0;
+    const cudaError_t e = sort_bytes(3 * ((N + 2) / 3), &sb);
+    if (e != cudaSuccess) return e;
+    *bytes = PcaLayout(C, N).sort_tmp + align_up(sb);
+    return cudaSuccess;
+}
+
 template <typename T>
-cudaError_t moments_run(int C, int N, const T* x, char* scratch, float* mean, double* cov, cudaStream_t s) {
+cudaError_t launch_pca_moments(int C, int N, const T* x, char* scratch, float* mean, double* cov, cudaStream_t s) {
     const PcaLayout ly(C, N);
     const int n = (N + 2) / 3, parts = moment_ctas(n);
     float* inv = reinterpret_cast<float*>(scratch + ly.inv);
@@ -338,8 +349,8 @@ cudaError_t moments_run(int C, int N, const T* x, char* scratch, float* mean, do
 }
 
 template <typename T>
-cudaError_t range_run(int C, int N, const T* x, const float* mean, const float* comp, char* scratch, float* range,
-                      cudaStream_t s) {
+cudaError_t launch_pca_range(int C, int N, const T* x, const float* mean, const float* comp, char* scratch, float* range,
+                             cudaStream_t s) {
     const PcaLayout ly(C, N);
     const int n = (N + 2) / 3, m = 3 * n;
     float* keys = reinterpret_cast<float*>(scratch + ly.keys);
@@ -359,48 +370,18 @@ cudaError_t range_run(int C, int N, const T* x, const float* mean, const float* 
 }
 
 template <typename T>
-cudaError_t image_run(int C, int N, const T* x, const float* mean, const float* comp, const float* range, float* image,
-                      cudaStream_t s) {
+cudaError_t launch_pca_image(int C, int N, const T* x, const float* mean, const float* comp, const float* range,
+                             float* image, cudaStream_t s) {
     TileArgs<T> ta{};
     ta.C = C; ta.N = N; ta.stride = 1; ta.count = N;
     ta.x = x; ta.mean = mean; ta.comp = comp; ta.range = range; ta.out = image;
     return launch_tile<kImage>(ta, (unsigned)((N + 31) / 32), s);
 }
-
-}  // namespace
-
-size_t pca_scratch_fixed_bytes(int C, int N) { return PcaLayout(C, N).sort_tmp; }
-
-cudaError_t pca_scratch_bytes(int C, int N, size_t* bytes) {
-    *bytes = 0;
-    size_t sb = 0;
-    const cudaError_t e = sort_bytes(3 * ((N + 2) / 3), &sb);
-    if (e != cudaSuccess) return e;
-    *bytes = PcaLayout(C, N).sort_tmp + up(sb);
-    return cudaSuccess;
-}
-
-cudaError_t launch_pca_moments(int C, int N, const float* x, char* scratch, float* mean, double* cov, cudaStream_t s) {
-    return moments_run(C, N, x, scratch, mean, cov, s);
-}
-cudaError_t launch_pca_moments(int C, int N, const __half* x, char* scratch, float* mean, double* cov, cudaStream_t s) {
-    return moments_run(C, N, x, scratch, mean, cov, s);
-}
-cudaError_t launch_pca_range(int C, int N, const float* x, const float* mean, const float* comp, char* scratch,
-                             float* range, cudaStream_t s) {
-    return range_run(C, N, x, mean, comp, scratch, range, s);
-}
-cudaError_t launch_pca_range(int C, int N, const __half* x, const float* mean, const float* comp, char* scratch,
-                             float* range, cudaStream_t s) {
-    return range_run(C, N, x, mean, comp, scratch, range, s);
-}
-cudaError_t launch_pca_image(int C, int N, const float* x, const float* mean, const float* comp, const float* range,
-                             float* image, cudaStream_t s) {
-    return image_run(C, N, x, mean, comp, range, image, s);
-}
-cudaError_t launch_pca_image(int C, int N, const __half* x, const float* mean, const float* comp, const float* range,
-                             float* image, cudaStream_t s) {
-    return image_run(C, N, x, mean, comp, range, image, s);
-}
+template cudaError_t launch_pca_moments(int, int, const float*, char*, float*, double*, cudaStream_t);
+template cudaError_t launch_pca_moments(int, int, const __half*, char*, float*, double*, cudaStream_t);
+template cudaError_t launch_pca_range(int, int, const float*, const float*, const float*, char*, float*, cudaStream_t);
+template cudaError_t launch_pca_range(int, int, const __half*, const float*, const float*, char*, float*, cudaStream_t);
+template cudaError_t launch_pca_image(int, int, const float*, const float*, const float*, const float*, float*, cudaStream_t);
+template cudaError_t launch_pca_image(int, int, const __half*, const float*, const float*, const float*, float*, cudaStream_t);
 
 }  // namespace f3dgs

@@ -321,7 +321,6 @@ __global__ void query_text_prep_kernel(int K, int D, int Dp, const float* __rest
 }
 
 int kt_of(int C) { return C <= 32 ? 4 : C <= 64 ? 8 : C <= 128 ? 16 : 32; }
-size_t round_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
 
 template <int KT, typename T>
 cudaError_t launch_query(const QArgs<T>& a, cudaStream_t s) {
@@ -334,23 +333,25 @@ cudaError_t launch_query(const QArgs<T>& a, cudaStream_t s) {
     return cudaGetLastError();
 }
 
-template <typename T>
-cudaError_t query_run(int C, int D, int K, int N, const float* weight, const float* bias, const T* x, const float* text,
-                      float scale, const uint8_t* positive, int64_t* labels, float* prob, float* logits,
-                      cudaStream_t s) {
+}  // namespace
+
+template <typename X>
+cudaError_t launch_feature_query(int C, int D, int K, int N, const float* weight, const float* bias, const X* x,
+                                 const float* text, float scale, const uint8_t* positive, int64_t* labels, float* prob,
+                                 float* logits, cudaStream_t s) {
     if (N == 0) return cudaSuccess;
     const int KT = weight != nullptr ? kt_of(C) : 0, Cp = 8 * KT;
-    QArgs<T> a;
+    QArgs<X> a;
     a.C = C; a.D = D; a.K = K; a.N = N;
-    a.Dp = (int)round_up(D, kDAlign);
+    a.Dp = (int)align_up(D, kDAlign);
     a.tiles = (K + 7) / 8;
     a.chunks = (a.tiles + kMaxTiles - 1) / kMaxTiles;
     a.chunk_tiles = (a.tiles + a.chunks - 1) / a.chunks;  // equal chunks: K = 150 runs 2 x 80 prompts, not 128 + 128
     const int Kp = 8 * a.tiles;
     // stream-ordered scratch: W [Dp, Cp] and b [Dp] (decoder), text [Kp, Dp], mask [Kp]
-    const size_t off_b = round_up((size_t)a.Dp * Cp * 4, 256);
-    const size_t off_t = round_up(off_b + (weight != nullptr ? (size_t)a.Dp * 4 : 0), 256);
-    const size_t off_m = round_up(off_t + (size_t)Kp * a.Dp * 4, 256);
+    const size_t off_b = align_up((size_t)a.Dp * Cp * 4, 256);
+    const size_t off_t = align_up(off_b + (weight != nullptr ? (size_t)a.Dp * 4 : 0), 256);
+    const size_t off_m = align_up(off_t + (size_t)Kp * a.Dp * 4, 256);
     char* ws = nullptr;
     cudaError_t e = cudaMallocAsync((void**)&ws, off_m + Kp, s);
     if (e != cudaSuccess) return e;
@@ -381,19 +382,9 @@ cudaError_t query_run(int C, int D, int K, int N, const float* weight, const flo
     cudaFreeAsync(ws, s);
     return e;
 }
-
-}  // namespace
-
-cudaError_t launch_feature_query(int C, int D, int K, int N, const float* weight, const float* bias, const float* x,
-                                 const float* text, float logit_scale, const uint8_t* positive, int64_t* labels,
-                                 float* prob, float* logits, cudaStream_t s) {
-    return query_run<float>(C, D, K, N, weight, bias, x, text, logit_scale, positive, labels, prob, logits, s);
-}
-
-cudaError_t launch_feature_query(int C, int D, int K, int N, const float* weight, const float* bias, const __half* x,
-                                 const float* text, float logit_scale, const uint8_t* positive, int64_t* labels,
-                                 float* prob, float* logits, cudaStream_t s) {
-    return query_run<__half>(C, D, K, N, weight, bias, x, text, logit_scale, positive, labels, prob, logits, s);
-}
+template cudaError_t launch_feature_query(int, int, int, int, const float*, const float*, const float*, const float*, float,
+                                          const uint8_t*, int64_t*, float*, float*, cudaStream_t);
+template cudaError_t launch_feature_query(int, int, int, int, const float*, const float*, const __half*, const float*, float,
+                                          const uint8_t*, int64_t*, float*, float*, cudaStream_t);
 
 }  // namespace f3dgs

@@ -1,4 +1,5 @@
-// Internal launch interface between the C-ABI orchestration (api.cu) and the kernel TUs.
+// Internal launch interface between the C-ABI orchestration (api.cu) and the kernel TUs.  A launcher templated on the
+// element type of its data is instantiated for float and __half in its .cu.
 #pragma once
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
@@ -68,10 +69,9 @@ cudaError_t launch_feature_bwd(const ViewParams& vp, const uint2* ranges, const 
                                int* work_counter, cudaStream_t s);
 
 // ---- feature_head.cu (a float16 target gives the result of the float32 one upcast exactly)
-cudaError_t launch_feature_resize_fwd(int C, int H, int W, int Hg, int Wg, const float* fm, const float* gt,
-                                      float grad_scale, float* out, float* loss_sum, cudaStream_t s);
-cudaError_t launch_feature_resize_fwd(int C, int H, int W, int Hg, int Wg, const float* fm, const __half* gt,
-                                      float grad_scale, float* out, float* loss_sum, cudaStream_t s);
+template <typename GT>
+cudaError_t launch_feature_resize_fwd(int C, int H, int W, int Hg, int Wg, const float* fm, const GT* gt, float grad_scale,
+                                      float* out, float* loss_sum, cudaStream_t s);
 cudaError_t launch_feature_resize_bwd(int C, int H, int W, int Hg, int Wg, const float* dout, float* dfm, cudaStream_t s);
 
 // ---- image_loss.cu: fused L1 + SSIM sums and, with dL_dimage != nullptr, the gradient w.r.t. image
@@ -83,15 +83,12 @@ cudaError_t launch_image_loss(int planes, int H, int W, const float* image, cons
 constexpr int kDecoderMaxCin = 256, kDecoderMaxCout = 4096;
 bool decoder_grid_ok(int Cin, int Cout, int N);  // sizes in range and the launch grids fit CUDA's limits
 // y may be float16 (rounded to nearest even, as torch's .half()); a float16 gt is upcast exactly
-cudaError_t launch_decoder_forward(int Cin, int Cout, int N, const float* weight, const float* bias, const float* x,
-                                   float* y, cudaStream_t s);
-cudaError_t launch_decoder_forward(int Cin, int Cout, int N, const float* weight, const float* bias, const float* x,
-                                   __half* y, cudaStream_t s);
+template <typename Y>
+cudaError_t launch_decoder_forward(int Cin, int Cout, int N, const float* weight, const float* bias, const float* x, Y* y,
+                                   cudaStream_t s);
+template <typename GT>
 cudaError_t launch_decoder_l1(int Cin, int Cout, int N, const float* weight, const float* bias, const float* x,
-                              const float* gt, float grad_scale, float* loss_sum, float* dx, float* dW, float* db,
-                              cudaStream_t s);
-cudaError_t launch_decoder_l1(int Cin, int Cout, int N, const float* weight, const float* bias, const float* x,
-                              const __half* gt, float grad_scale, float* loss_sum, float* dx, float* dW, float* db,
+                              const GT* gt, float grad_scale, float* loss_sum, float* dx, float* dW, float* db,
                               cudaStream_t s);
 // W [Cout,Cin] -> wt [rows, Cp] rounded to TF32 and zero-padded; b [Cout] or NULL -> bp [rows] zero-padded
 cudaError_t launch_decoder_prep(int Cin, int Cout, int Cp, int rows, const float* weight, const float* bias, float* wt,
@@ -100,10 +97,8 @@ cudaError_t launch_decoder_prep(int Cin, int Cout, int Cp, int rows, const float
 // ---- feature_query.cu: cosine similarity of (decoded) feature columns with text embeddings -> argmax label, softmax
 // probability of a positive prompt set, logits.  weight == NULL: no decoder (D == C).  x may be float16 (upcast exactly)
 constexpr int kQueryMaxK = 256, kQueryMaxD = 4096;
-cudaError_t launch_feature_query(int C, int D, int K, int N, const float* weight, const float* bias, const float* x,
-                                 const float* text, float logit_scale, const uint8_t* positive, int64_t* labels,
-                                 float* prob, float* logits, cudaStream_t s);
-cudaError_t launch_feature_query(int C, int D, int K, int N, const float* weight, const float* bias, const __half* x,
+template <typename X>
+cudaError_t launch_feature_query(int C, int D, int K, int N, const float* weight, const float* bias, const X* x,
                                  const float* text, float logit_scale, const uint8_t* positive, int64_t* labels,
                                  float* prob, float* logits, cudaStream_t s);
 
@@ -112,15 +107,13 @@ cudaError_t launch_feature_query(int C, int D, int K, int N, const float* weight
 constexpr int kPcaMinC = 3, kPcaMaxC = 1024;
 cudaError_t pca_scratch_bytes(int C, int N, size_t* bytes);
 size_t pca_scratch_fixed_bytes(int C, int N);
-cudaError_t launch_pca_moments(int C, int N, const float* x, char* scratch, float* mean, double* cov, cudaStream_t s);
-cudaError_t launch_pca_moments(int C, int N, const __half* x, char* scratch, float* mean, double* cov, cudaStream_t s);
-cudaError_t launch_pca_range(int C, int N, const float* x, const float* mean, const float* comp, char* scratch,
-                             float* range, cudaStream_t s);
-cudaError_t launch_pca_range(int C, int N, const __half* x, const float* mean, const float* comp, char* scratch,
-                             float* range, cudaStream_t s);
-cudaError_t launch_pca_image(int C, int N, const float* x, const float* mean, const float* comp, const float* range,
-                             float* image, cudaStream_t s);
-cudaError_t launch_pca_image(int C, int N, const __half* x, const float* mean, const float* comp, const float* range,
+template <typename X>
+cudaError_t launch_pca_moments(int C, int N, const X* x, char* scratch, float* mean, double* cov, cudaStream_t s);
+template <typename X>
+cudaError_t launch_pca_range(int C, int N, const X* x, const float* mean, const float* comp, char* scratch, float* range,
+                             cudaStream_t s);
+template <typename X>
+cudaError_t launch_pca_image(int C, int N, const X* x, const float* mean, const float* comp, const float* range,
                              float* image, cudaStream_t s);
 
 // ---- knn.cu: exact mean squared distance to the 3 nearest other points (distCUDA2); scratch is knn_scratch_bytes(P)
@@ -141,5 +134,12 @@ cudaError_t launch_densify_apply(int P, int M, int C, const char* scratch, const
                                  const float* const src[21], float* const dst[21], cudaStream_t s);
 cudaError_t launch_reset_opacity(int P, float* raw_opacity, float* exp_avg, float* exp_avg_sq, float ceiling,
                                  cudaStream_t s);
+
+// ---- optimizer.cu: activation prologue and fused Adam step (include/f3dgs_b200.h: f3dgs_activate / f3dgs_adam_step)
+cudaError_t launch_activate(int P, int M, const float* raw_opacity, const float* raw_scaling, const float* raw_rotation,
+                            const float* features_dc, const float* features_rest, float* opacity, float* scales,
+                            float* rotations, float* shs, cudaStream_t s);
+cudaError_t launch_adam_step(int kind, size_t n, int M, float* param, const float* grad_activated, float* exp_avg,
+                             float* exp_avg_sq, float lr, float beta1, float beta2, float eps, int step, cudaStream_t s);
 
 }  // namespace f3dgs

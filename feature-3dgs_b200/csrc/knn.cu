@@ -58,8 +58,6 @@ KnnLevels knn_levels(int P) {
     return L;
 }
 
-inline size_t align_up(size_t x) { return (x + 255) / 256 * 256; }
-
 struct KnnLayout {
     KnnLevels lv;
     size_t bbox, keys_in, keys_out, idx_in, idx_out, pts, box_lo, box_hi, sort_tmp, fixed_bytes;
@@ -297,8 +295,6 @@ __global__ void __launch_bounds__(256) query_kernel(int P, int top, long long to
     }
     if (active) out[order[self]] = __fdiv_rn(__fadd_rn(__fadd_rn(d0, d1), d2), 3.f);
 }
-
-inline unsigned blocks_for(long long threads) { return (unsigned)((threads + 255) / 256); }
 
 }  // namespace
 

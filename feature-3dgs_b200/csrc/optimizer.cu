@@ -115,36 +115,19 @@ __global__ void __launch_bounds__(256) adam_step_kernel(AdamArgs a) {
 }
 
 }  // namespace
-}  // namespace f3dgs
 
-using namespace f3dgs;
-
-extern "C" {
-
-int f3dgs_activate(int P, int M, const float* raw_opacity, const float* raw_scaling, const float* raw_rotation,
-                   const float* features_dc, const float* features_rest, float* opacity, float* scales, float* rotations,
-                   float* shs, void* cuda_stream) {
-    if (P < 0 || M < 0) return -F3DGS_ERR_INVALID_ARGUMENT;
-    if (P == 0) return 0;
-    if ((raw_opacity && !opacity) || (raw_scaling && !scales) || (raw_rotation && !rotations) ||
-        (features_dc && (!shs || M < 1 || (M > 1 && !features_rest))))
-        return -F3DGS_ERR_INVALID_ARGUMENT;
+cudaError_t launch_activate(int P, int M, const float* raw_opacity, const float* raw_scaling, const float* raw_rotation,
+                            const float* features_dc, const float* features_rest, float* opacity, float* scales,
+                            float* rotations, float* shs, cudaStream_t s) {
     const size_t n = 5 * (size_t)P + 3 * (size_t)M * P;
-    activate_kernel<<<(unsigned)((n + 255) / 256), 256, 0, (cudaStream_t)cuda_stream>>>(
-        P, M, raw_opacity, raw_scaling, raw_rotation, features_dc, features_rest, opacity, scales, rotations, shs);
+    activate_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(P, M, raw_opacity, raw_scaling, raw_rotation, features_dc,
+                                                                features_rest, opacity, scales, rotations, shs);
     g_launches++;
-    return cudaGetLastError() == cudaSuccess ? 0 : -F3DGS_ERR_CUDA;
+    return cudaGetLastError();
 }
 
-int f3dgs_adam_step(int kind, size_t n, int M, float* param, const float* grad_activated, float* exp_avg, float* exp_avg_sq,
-                    float lr, float beta1, float beta2, float eps, int step, void* cuda_stream) {
-    if (kind < F3DGS_PARAM_IDENTITY || kind > F3DGS_PARAM_SH_REST || step < 1 || !param || !grad_activated || !exp_avg ||
-        !exp_avg_sq)
-        return -F3DGS_ERR_INVALID_ARGUMENT;
-    if (kind == F3DGS_PARAM_NORMALIZE4 && (n % 4 != 0)) return -F3DGS_ERR_INVALID_ARGUMENT;
-    if ((kind == F3DGS_PARAM_SH_DC || kind == F3DGS_PARAM_SH_REST) && M < (kind == F3DGS_PARAM_SH_REST ? 2 : 1))
-        return -F3DGS_ERR_INVALID_ARGUMENT;
-    if (n == 0) return 0;
+cudaError_t launch_adam_step(int kind, size_t n, int M, float* param, const float* grad_activated, float* exp_avg,
+                             float* exp_avg_sq, float lr, float beta1, float beta2, float eps, int step, cudaStream_t s) {
     AdamArgs a;
     a.param = param; a.grad = grad_activated; a.m = exp_avg; a.v = exp_avg_sq; a.n = n; a.kind = kind; a.M = M;
     const double bc1 = 1.0 - pow((double)beta1, (double)step), bc2 = 1.0 - pow((double)beta2, (double)step);
@@ -152,9 +135,9 @@ int f3dgs_adam_step(int kind, size_t n, int M, float* param, const float* grad_a
     a.inv_sqrt_bc2 = (float)(1.0 / sqrt(bc2));
     a.b1 = beta1; a.b2 = beta2; a.eps = eps;
     const size_t threads = kind == F3DGS_PARAM_NORMALIZE4 ? n / 4 : n;
-    adam_step_kernel<<<(unsigned)((threads + 255) / 256), 256, 0, (cudaStream_t)cuda_stream>>>(a);
+    adam_step_kernel<<<(unsigned)((threads + 255) / 256), 256, 0, s>>>(a);
     g_launches++;
-    return cudaGetLastError() == cudaSuccess ? 0 : -F3DGS_ERR_CUDA;
+    return cudaGetLastError();
 }
 
-}  // extern "C"
+}  // namespace f3dgs

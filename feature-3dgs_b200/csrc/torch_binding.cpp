@@ -35,15 +35,43 @@ const float* fptr(const torch::Tensor& t) {  // empty tensor -> nullptr, as in t
     return t.data_ptr<float>();
 }
 
-torch::Tensor prep(const torch::Tensor& t, const torch::Device& dev, const char* name) {
+// The two tensor checks.  An undefined or empty tensor is an absent argument for both.
+// A float32 input on `dev` that is only read: made contiguous (a copy if it is not).
+torch::Tensor input(const torch::Tensor& t, const torch::Device& dev, const char* name) {
     if (!t.defined() || t.numel() == 0) return t;
     TORCH_CHECK(t.scalar_type() == torch::kFloat32, name, " must be float32");
     TORCH_CHECK(t.device() == dev, name, " must be on ", dev, " (got ", t.device(), ")");
     return t.contiguous();
 }
+// A float32 tensor of `numel` elements on `dev` that the call reads or writes in place, so it must be contiguous already
+// -> its data, or nullptr if absent.
+float* in_place(const torch::Tensor& t, const torch::Device& dev, int64_t numel, const char* name) {
+    if (!t.defined() || t.numel() == 0) return nullptr;
+    TORCH_CHECK(t.is_cuda() && t.device() == dev && t.scalar_type() == torch::kFloat32 && t.is_contiguous() &&
+                    t.numel() == numel,
+                name, " must be a contiguous float32 tensor of ", numel, " elements on ", dev, " (got ", t.numel(),
+                " elements of ", t.scalar_type(), " on ", t.device(), ")");
+    return t.data_ptr<float>();
+}
 
 void check_rc(int rc, const char* what) {
     TORCH_CHECK(rc >= 0, what, " failed (code ", -rc, "): ", f3dgs_last_error());
+}
+
+// Calls the float16 twin of a C-ABI function with t's IEEE binary16 bits if t is float16, else the float32 one with t's
+// float data; `call(fn, ptr)` writes the argument list once for both.
+template <typename F32, typename F16, typename Call>
+void call_f32_or_f16(const torch::Tensor& t, F32 f32, const char* name32, F16 f16, const char* name16, Call call) {
+    if (t.defined() && t.scalar_type() == torch::kFloat16)
+        check_rc(call(f16, reinterpret_cast<uint16_t*>(t.data_ptr<at::Half>())), name16);
+    else
+        check_rc(call(f32, const_cast<float*>(fptr(t))), name32);
+}
+
+// A scratch tensor of the size a f3dgs_*_scratch_bytes function returned: 0 is a failure when it set the last error
+torch::Tensor scratch_tensor(size_t bytes, const char* fn, const torch::Tensor& like) {
+    TORCH_CHECK(bytes > 0 || f3dgs_last_error()[0] == '\0', fn, " failed: ", f3dgs_last_error());
+    return torch::empty({(int64_t)bytes}, like.options().dtype(torch::kByte));
 }
 
 }  // namespace
@@ -87,12 +115,12 @@ RasterizeGaussiansCUDA(const torch::Tensor& background, const torch::Tensor& mea
     if (P != 0) {
         int M = 0;
         if (sh.defined() && sh.numel() != 0) M = sh.size(1);
-        auto bg = prep(background, dev, "bg"), m3 = prep(means3D, dev, "means3D");
-        auto col = prep(colors, dev, "colors_precomp"), sf = prep(semantic_feature, dev, "semantic_feature");
-        auto op = prep(opacity, dev, "opacities"), sc = prep(scales, dev, "scales");
-        auto rot = prep(rotations, dev, "rotations"), cov = prep(cov3D_precomp, dev, "cov3D_precomp");
-        auto vm = prep(viewmatrix, dev, "viewmatrix"), pm = prep(projmatrix, dev, "projmatrix");
-        auto shc = prep(sh, dev, "shs"), cp = prep(campos, dev, "campos");
+        auto bg = input(background, dev, "bg"), m3 = input(means3D, dev, "means3D");
+        auto col = input(colors, dev, "colors_precomp"), sf = input(semantic_feature, dev, "semantic_feature");
+        auto op = input(opacity, dev, "opacities"), sc = input(scales, dev, "scales");
+        auto rot = input(rotations, dev, "rotations"), cov = input(cov3D_precomp, dev, "cov3D_precomp");
+        auto vm = input(viewmatrix, dev, "viewmatrix"), pm = input(projmatrix, dev, "projmatrix");
+        auto shc = input(sh, dev, "shs"), cp = input(campos, dev, "campos");
         cudaStream_t stream = c10::cuda::getCurrentCUDAStream().stream();
         rendered = f3dgs_forward(resize_tensor, &geomBuffer, resize_tensor, &binningBuffer, resize_tensor, &imgBuffer,
                                  P, degree, M, C, fptr(bg), W, H, fptr(m3), fptr(shc), fptr(col), fptr(sf), fptr(op),
@@ -143,15 +171,15 @@ RasterizeGaussiansBackwardCUDA(const torch::Tensor& background, const torch::Ten
     torch::Tensor dL_dz = torch::zeros({P, 1}, o);
 
     if (P != 0) {
-        auto bg = prep(background, dev, "bg"), m3 = prep(means3D, dev, "means3D");
-        auto col = prep(colors, dev, "colors_precomp"), sf = prep(semantic_feature, dev, "semantic_feature");
-        auto sc = prep(scales, dev, "scales"), rot = prep(rotations, dev, "rotations");
-        auto cov = prep(cov3D_precomp, dev, "cov3D_precomp");
-        auto vm = prep(viewmatrix, dev, "viewmatrix"), pm = prep(projmatrix, dev, "projmatrix");
-        auto shc = prep(sh, dev, "shs"), cp = prep(campos, dev, "campos");
-        auto gc = prep(dL_dout_color, dev, "grad_out_color");
-        auto gd = prep(dL_dout_depth, dev, "grad_out_depth");
-        torch::Tensor gf = C ? prep(dL_dout_feature, dev, "grad_out_feature") : dL_dout_feature;
+        auto bg = input(background, dev, "bg"), m3 = input(means3D, dev, "means3D");
+        auto col = input(colors, dev, "colors_precomp"), sf = input(semantic_feature, dev, "semantic_feature");
+        auto sc = input(scales, dev, "scales"), rot = input(rotations, dev, "rotations");
+        auto cov = input(cov3D_precomp, dev, "cov3D_precomp");
+        auto vm = input(viewmatrix, dev, "viewmatrix"), pm = input(projmatrix, dev, "projmatrix");
+        auto shc = input(sh, dev, "shs"), cp = input(campos, dev, "campos");
+        auto gc = input(dL_dout_color, dev, "grad_out_color");
+        auto gd = input(dL_dout_depth, dev, "grad_out_depth");
+        torch::Tensor gf = C ? input(dL_dout_feature, dev, "grad_out_feature") : dL_dout_feature;
         TORCH_CHECK(radii.scalar_type() == torch::kInt32 && radii.is_cuda(), "radii must be int32 CUDA");
         auto rad = radii.contiguous();
         auto gb = geomBuffer.contiguous(), bb = binningBuffer.contiguous(), ib = imageBuffer.contiguous();
@@ -195,20 +223,14 @@ void RasterizeGaussiansBackwardAccumCUDA(
     int M = 0;
     if (sh.defined() && sh.numel() != 0) M = sh.size(1);
     const int C = (dL_dout_feature.defined() && dL_dout_feature.dim() == 3) ? (int)dL_dout_feature.size(0) : 0;
-    auto gcheck = [&](const torch::Tensor& t, int64_t numel, const char* name) -> float* {
-        if (!t.defined() || t.numel() == 0) return nullptr;
-        TORCH_CHECK(t.is_cuda() && t.device() == dev && t.scalar_type() == torch::kFloat32 && t.is_contiguous() &&
-                        t.numel() == numel, name, " must be a contiguous float32 CUDA tensor with ", numel, " elements");
-        return t.data_ptr<float>();
-    };
-    auto bg = prep(background, dev, "bg"), m3 = prep(means3D, dev, "means3D");
-    auto col = prep(colors, dev, "colors_precomp");
-    auto sc = prep(scales, dev, "scales"), rot = prep(rotations, dev, "rotations");
-    auto cov = prep(cov3D_precomp, dev, "cov3D_precomp");
-    auto vm = prep(viewmatrix, dev, "viewmatrix"), pm = prep(projmatrix, dev, "projmatrix");
-    auto shc = prep(sh, dev, "shs"), cp = prep(campos, dev, "campos");
-    auto gc = prep(dL_dout_color, dev, "grad_out_color"), gd = prep(dL_dout_depth, dev, "grad_out_depth");
-    torch::Tensor gf = C ? prep(dL_dout_feature, dev, "grad_out_feature") : dL_dout_feature;
+    auto bg = input(background, dev, "bg"), m3 = input(means3D, dev, "means3D");
+    auto col = input(colors, dev, "colors_precomp");
+    auto sc = input(scales, dev, "scales"), rot = input(rotations, dev, "rotations");
+    auto cov = input(cov3D_precomp, dev, "cov3D_precomp");
+    auto vm = input(viewmatrix, dev, "viewmatrix"), pm = input(projmatrix, dev, "projmatrix");
+    auto shc = input(sh, dev, "shs"), cp = input(campos, dev, "campos");
+    auto gc = input(dL_dout_color, dev, "grad_out_color"), gd = input(dL_dout_depth, dev, "grad_out_depth");
+    torch::Tensor gf = C ? input(dL_dout_feature, dev, "grad_out_feature") : dL_dout_feature;
     TORCH_CHECK(radii.scalar_type() == torch::kInt32 && radii.is_cuda(), "radii must be int32 CUDA");
     auto rad = radii.contiguous();
     const size_t need = f3dgs_backward_scratch_bytes(P);
@@ -221,12 +243,14 @@ void RasterizeGaussiansBackwardAccumCUDA(
         fptr(vm), fptr(pm), fptr(cp), tan_fovx, tan_fovy, rad.data_ptr<int>(),
         reinterpret_cast<char*>(geomBuffer.data_ptr()), reinterpret_cast<char*>(binningBuffer.data_ptr()),
         reinterpret_cast<char*>(imageBuffer.data_ptr()), fptr(gc), C ? fptr(gf) : nullptr, fptr(gd),
-        reinterpret_cast<char*>(scratch.data_ptr()), gcheck(g_opacities, P, "g_opacities"),
-        gcheck(g_colors, (int64_t)P * 3, "g_colors_precomp"), gcheck(g_semantic_feature, (int64_t)P * C, "g_semantic_feature"),
-        gcheck(g_means3D, (int64_t)P * 3, "g_means3D"), gcheck(g_cov3D, (int64_t)P * 6, "g_cov3D_precomp"),
-        gcheck(g_sh, (int64_t)P * M * 3, "g_sh"), gcheck(g_scales, (int64_t)P * 3, "g_scales"),
-        gcheck(g_rotations, (int64_t)P * 4, "g_rotations"), gcheck(g_means2D_out, (int64_t)P * 3, "g_means2D_out"),
-        gcheck(grad_accum, P, "grad_accum"), gcheck(denom, P, "denom"),
+        reinterpret_cast<char*>(scratch.data_ptr()), in_place(g_opacities, dev, P, "g_opacities"),
+        in_place(g_colors, dev, (int64_t)P * 3, "g_colors_precomp"),
+        in_place(g_semantic_feature, dev, (int64_t)P * C, "g_semantic_feature"),
+        in_place(g_means3D, dev, (int64_t)P * 3, "g_means3D"), in_place(g_cov3D, dev, (int64_t)P * 6, "g_cov3D_precomp"),
+        in_place(g_sh, dev, (int64_t)P * M * 3, "g_sh"), in_place(g_scales, dev, (int64_t)P * 3, "g_scales"),
+        in_place(g_rotations, dev, (int64_t)P * 4, "g_rotations"),
+        in_place(g_means2D_out, dev, (int64_t)P * 3, "g_means2D_out"), in_place(grad_accum, dev, P, "grad_accum"),
+        in_place(denom, dev, P, "denom"),
         reinterpret_cast<void*>(static_cast<intptr_t>(composite_done_event)), debug ? 1 : 0, (void*)stream);
     check_rc(rc, "f3dgs_backward_accum");
 }
@@ -238,8 +262,8 @@ torch::Tensor markVisible(torch::Tensor& means3D, torch::Tensor& viewmatrix, tor
     const int P = means3D.size(0);
     torch::Tensor present = torch::full({P}, false, means3D.options().dtype(at::kBool));
     if (P != 0) {
-        auto m3 = prep(means3D, dev, "means3D"), vm = prep(viewmatrix, dev, "viewmatrix"),
-             pm = prep(projmatrix, dev, "projmatrix");
+        auto m3 = input(means3D, dev, "means3D"), vm = input(viewmatrix, dev, "viewmatrix"),
+             pm = input(projmatrix, dev, "projmatrix");
         cudaStream_t stream = c10::cuda::getCurrentCUDAStream().stream();
         int rc = f3dgs_mark_visible(P, fptr(m3), fptr(vm), fptr(pm), reinterpret_cast<uint8_t*>(present.data_ptr<bool>()),
                                     (void*)stream);
@@ -254,8 +278,6 @@ namespace {
 bool is_target_dtype(const torch::Tensor& t) {
     return t.scalar_type() == torch::kFloat32 || t.scalar_type() == torch::kFloat16;
 }
-
-const uint16_t* hptr(const torch::Tensor& t) { return reinterpret_cast<const uint16_t*>(t.data_ptr<at::Half>()); }
 }  // namespace
 
 // -> (out [C,Hg,Wg], loss_sum [1]); with gt: out = sign(resized - gt) * grad_scale and loss_sum = sum |resized - gt|
@@ -267,7 +289,6 @@ std::tuple<torch::Tensor, torch::Tensor> featureResizeFwd(const torch::Tensor& f
     auto fm = feature_map.contiguous();
     const int C = fm.size(0), H = fm.size(1), W = fm.size(2);
     const bool has_gt = gt.defined() && gt.numel() > 0;
-    const bool half_gt = has_gt && gt.scalar_type() == torch::kFloat16;
     torch::Tensor g;
     if (has_gt) {
         TORCH_CHECK(gt.is_cuda() && is_target_dtype(gt) && gt.dim() == 3 && gt.size(0) == C && gt.size(1) == Hg &&
@@ -277,14 +298,11 @@ std::tuple<torch::Tensor, torch::Tensor> featureResizeFwd(const torch::Tensor& f
     torch::Tensor out = torch::empty({C, Hg, Wg}, fm.options());
     torch::Tensor loss = torch::zeros({1}, fm.options());
     cudaStream_t stream = c10::cuda::getCurrentCUDAStream().stream();
-    if (half_gt)
-        check_rc(f3dgs_feature_resize_fwd_f16gt(C, H, W, (int)Hg, (int)Wg, fptr(fm), hptr(g), (float)grad_scale,
-                                                out.data_ptr<float>(), loss.data_ptr<float>(), (void*)stream),
-                 "f3dgs_feature_resize_fwd_f16gt");
-    else
-        check_rc(f3dgs_feature_resize_fwd(C, H, W, (int)Hg, (int)Wg, fptr(fm), has_gt ? fptr(g) : nullptr,
-                                          (float)grad_scale, out.data_ptr<float>(), loss.data_ptr<float>(), (void*)stream),
-                 "f3dgs_feature_resize_fwd");
+    call_f32_or_f16(g, f3dgs_feature_resize_fwd, "f3dgs_feature_resize_fwd", f3dgs_feature_resize_fwd_f16gt,
+                    "f3dgs_feature_resize_fwd_f16gt", [&](auto fn, auto gp) {
+                        return fn(C, H, W, (int)Hg, (int)Wg, fptr(fm), gp, (float)grad_scale, out.data_ptr<float>(),
+                                  loss.data_ptr<float>(), (void*)stream);
+                    });
     return std::make_tuple(out, loss);
 }
 
@@ -355,11 +373,6 @@ DecoderInputs decoder_inputs(const torch::Tensor& x, const torch::Tensor& weight
     d.b = has_b ? bias.contiguous() : torch::Tensor();
     return d;
 }
-
-void check_accum(const torch::Tensor& t, const torch::Device& dev, int64_t numel, const char* name) {
-    TORCH_CHECK(t.defined() && t.device() == dev && t.scalar_type() == torch::kFloat32 && t.is_contiguous() &&
-                    t.numel() == numel, name, " must be a contiguous float32 tensor with ", numel, " elements on ", dev);
-}
 }  // namespace
 
 // -> y [Cout, <x's spatial shape>] of dtype float32, or float16 (rounded to nearest even, as y.half())
@@ -372,14 +385,10 @@ torch::Tensor decoderForward(const torch::Tensor& x, const torch::Tensor& weight
     shape[0] = d.Cout;
     torch::Tensor y = torch::empty(shape, d.x.options().dtype(dtype));
     cudaStream_t stream = c10::cuda::getCurrentCUDAStream().stream();
-    if (dtype == torch::kFloat16)
-        check_rc(f3dgs_decoder_forward_f16(d.Cin, d.Cout, d.N, fptr(d.w), fptr(d.b), fptr(d.x),
-                                           reinterpret_cast<uint16_t*>(y.data_ptr<at::Half>()), (void*)stream),
-                 "f3dgs_decoder_forward_f16");
-    else
-        check_rc(f3dgs_decoder_forward(d.Cin, d.Cout, d.N, fptr(d.w), fptr(d.b), fptr(d.x), y.data_ptr<float>(),
-                                       (void*)stream),
-                 "f3dgs_decoder_forward");
+    call_f32_or_f16(y, f3dgs_decoder_forward, "f3dgs_decoder_forward", f3dgs_decoder_forward_f16,
+                    "f3dgs_decoder_forward_f16", [&](auto fn, auto yp) {
+                        return fn(d.Cin, d.Cout, d.N, fptr(d.w), fptr(d.b), fptr(d.x), yp, (void*)stream);
+                    });
     return y;
 }
 
@@ -394,23 +403,16 @@ std::tuple<torch::Tensor, torch::Tensor> decoderL1(const torch::Tensor& x, const
                     gt.numel() == (int64_t)d.Cout * d.N && gt.sizes().slice(1) == d.x.sizes().slice(1),
                 "gt must be a float32 or float16 tensor [Cout, <x's spatial shape>] on ", dev);
     auto g = gt.contiguous();
-    check_accum(dweight, dev, (int64_t)d.Cout * d.Cin, "dweight");
-    if (d.b.defined()) check_accum(dbias, dev, d.Cout, "dbias");
-    else TORCH_CHECK(!dbias.defined() || dbias.numel() == 0, "dbias must be empty without a bias");
+    float* dw = in_place(dweight, dev, (int64_t)d.Cout * d.Cin, "dweight");
+    float* db = in_place(dbias, dev, d.b.defined() ? d.Cout : 0, "dbias");
     torch::Tensor loss = torch::empty({1}, d.x.options());
     torch::Tensor dx = torch::empty_like(d.x);
     cudaStream_t stream = c10::cuda::getCurrentCUDAStream().stream();
-    float* db = d.b.defined() ? dbias.data_ptr<float>() : nullptr;
-    if (g.scalar_type() == torch::kFloat16)
-        check_rc(f3dgs_decoder_l1_f16gt(d.Cin, d.Cout, d.N, fptr(d.w), fptr(d.b), fptr(d.x), hptr(g), (float)grad_scale,
-                                        loss.data_ptr<float>(), dx.data_ptr<float>(), dweight.data_ptr<float>(), db,
-                                        (void*)stream),
-                 "f3dgs_decoder_l1_f16gt");
-    else
-        check_rc(f3dgs_decoder_l1(d.Cin, d.Cout, d.N, fptr(d.w), fptr(d.b), fptr(d.x), fptr(g), (float)grad_scale,
-                                  loss.data_ptr<float>(), dx.data_ptr<float>(), dweight.data_ptr<float>(), db,
-                                  (void*)stream),
-                 "f3dgs_decoder_l1");
+    call_f32_or_f16(g, f3dgs_decoder_l1, "f3dgs_decoder_l1", f3dgs_decoder_l1_f16gt, "f3dgs_decoder_l1_f16gt",
+                    [&](auto fn, auto gp) {
+                        return fn(d.Cin, d.Cout, d.N, fptr(d.w), fptr(d.b), fptr(d.x), gp, (float)grad_scale,
+                                  loss.data_ptr<float>(), dx.data_ptr<float>(), dw, db, (void*)stream);
+                    });
     return std::make_tuple(loss, dx);
 }
 
@@ -471,14 +473,11 @@ std::tuple<torch::Tensor, torch::Tensor, torch::Tensor> featureQuery(const torch
     float* pr = want_prob ? prob.data_ptr<float>() : nullptr;
     float* lg = want_logits ? logits.data_ptr<float>() : nullptr;
     cudaStream_t stream = c10::cuda::getCurrentCUDAStream().stream();
-    if (xc.scalar_type() == torch::kFloat16)
-        check_rc(f3dgs_feature_query_f16x((int)C, (int)D, (int)K, (int)N, fptr(w), fptr(b), hptr(xc), fptr(tc),
-                                          (float)logit_scale, pp, lp, pr, lg, (void*)stream),
-                 "f3dgs_feature_query_f16x");
-    else
-        check_rc(f3dgs_feature_query((int)C, (int)D, (int)K, (int)N, fptr(w), fptr(b), fptr(xc), fptr(tc),
-                                     (float)logit_scale, pp, lp, pr, lg, (void*)stream),
-                 "f3dgs_feature_query");
+    call_f32_or_f16(xc, f3dgs_feature_query, "f3dgs_feature_query", f3dgs_feature_query_f16x, "f3dgs_feature_query_f16x",
+                    [&](auto fn, auto xp) {
+                        return fn((int)C, (int)D, (int)K, (int)N, fptr(w), fptr(b), xp, fptr(tc), (float)logit_scale, pp,
+                                  lp, pr, lg, (void*)stream);
+                    });
     return std::make_tuple(labels, prob, logits);
 }
 
@@ -487,7 +486,6 @@ std::tuple<torch::Tensor, torch::Tensor, torch::Tensor> featureQuery(const torch
 struct PcaX {
     torch::Tensor x;
     int C, N;
-    bool half;
 };
 
 PcaX pca_x(const torch::Tensor& x, const char* fn) {
@@ -497,19 +495,11 @@ PcaX pca_x(const torch::Tensor& x, const char* fn) {
     const int64_t C = x.size(0), N = x.numel() / std::max<int64_t>(C, 1);
     TORCH_CHECK(C >= 3 && C <= 1024 && N >= 7 && N <= INT32_MAX, fn,
                 ": needs 3 <= C <= 1024 channels and N >= 7 pixels (at least 3 samples), got C = ", C, ", N = ", N);
-    return {x, (int)C, (int)N, x.scalar_type() == torch::kFloat16};
-}
-
-void pca_check_f32(const torch::Tensor& t, const PcaX& px, int64_t numel, const char* fn, const char* what) {
-    TORCH_CHECK(t.is_cuda() && t.device() == px.x.device() && t.scalar_type() == torch::kFloat32 && t.is_contiguous() &&
-                    t.numel() == numel,
-                fn, ": ", what, " must be a contiguous float32 tensor of ", numel, " elements on ", px.x.device());
+    return {x, (int)C, (int)N};
 }
 
 torch::Tensor pca_scratch(const PcaX& px) {
-    const size_t bytes = f3dgs_feature_pca_scratch_bytes(px.C, px.N);
-    TORCH_CHECK(bytes > 0, "f3dgs_feature_pca_scratch_bytes failed: ", f3dgs_last_error());
-    return torch::empty({(int64_t)bytes}, px.x.options().dtype(torch::kByte));
+    return scratch_tensor(f3dgs_feature_pca_scratch_bytes(px.C, px.N), "f3dgs_feature_pca_scratch_bytes", px.x);
 }
 
 // -> (mean [C] float32, cov [C,C] float64)
@@ -521,35 +511,27 @@ std::tuple<torch::Tensor, torch::Tensor> featurePcaMoments(const torch::Tensor& 
     torch::Tensor cov = torch::empty({px.C, px.C}, x.options().dtype(torch::kFloat64));
     char* sp = reinterpret_cast<char*>(scratch.data_ptr());
     void* stream = (void*)c10::cuda::getCurrentCUDAStream().stream();
-    if (px.half)
-        check_rc(f3dgs_feature_pca_moments_f16x(px.C, px.N, hptr(x), sp, mean.data_ptr<float>(),
-                                                cov.data_ptr<double>(), stream),
-                 "f3dgs_feature_pca_moments_f16x");
-    else
-        check_rc(f3dgs_feature_pca_moments(px.C, px.N, fptr(x), sp, mean.data_ptr<float>(), cov.data_ptr<double>(),
-                                           stream),
-                 "f3dgs_feature_pca_moments");
+    call_f32_or_f16(x, f3dgs_feature_pca_moments, "f3dgs_feature_pca_moments", f3dgs_feature_pca_moments_f16x,
+                    "f3dgs_feature_pca_moments_f16x", [&](auto fn, auto xp) {
+                        return fn(px.C, px.N, xp, sp, mean.data_ptr<float>(), cov.data_ptr<double>(), stream);
+                    });
     return std::make_tuple(mean, cov);
 }
 
 // -> range [2] float32 = (lo, hi)
 torch::Tensor featurePcaRange(const torch::Tensor& x, const torch::Tensor& mean, const torch::Tensor& components) {
     const PcaX px = pca_x(x, "feature_pca_range");
-    pca_check_f32(mean, px, px.C, "feature_pca_range", "mean");
-    pca_check_f32(components, px, 3 * (int64_t)px.C, "feature_pca_range", "components");
+    const float* mp = in_place(mean, x.device(), px.C, "feature_pca_range: mean");
+    const float* cp = in_place(components, x.device(), 3 * (int64_t)px.C, "feature_pca_range: components");
     const c10::cuda::CUDAGuard guard(x.device());
     torch::Tensor scratch = pca_scratch(px);
     torch::Tensor range = torch::empty({2}, x.options().dtype(torch::kFloat32));
     char* sp = reinterpret_cast<char*>(scratch.data_ptr());
     void* stream = (void*)c10::cuda::getCurrentCUDAStream().stream();
-    if (px.half)
-        check_rc(f3dgs_feature_pca_range_f16x(px.C, px.N, hptr(x), fptr(mean), fptr(components), sp,
-                                              range.data_ptr<float>(), stream),
-                 "f3dgs_feature_pca_range_f16x");
-    else
-        check_rc(f3dgs_feature_pca_range(px.C, px.N, fptr(x), fptr(mean), fptr(components), sp,
-                                         range.data_ptr<float>(), stream),
-                 "f3dgs_feature_pca_range");
+    call_f32_or_f16(x, f3dgs_feature_pca_range, "f3dgs_feature_pca_range", f3dgs_feature_pca_range_f16x,
+                    "f3dgs_feature_pca_range_f16x", [&](auto fn, auto xp) {
+                        return fn(px.C, px.N, xp, mp, cp, sp, range.data_ptr<float>(), stream);
+                    });
     return range;
 }
 
@@ -557,22 +539,18 @@ torch::Tensor featurePcaRange(const torch::Tensor& x, const torch::Tensor& mean,
 torch::Tensor featurePcaImage(const torch::Tensor& x, const torch::Tensor& mean, const torch::Tensor& components,
                               const torch::Tensor& range) {
     const PcaX px = pca_x(x, "feature_pca_image");
-    pca_check_f32(mean, px, px.C, "feature_pca_image", "mean");
-    pca_check_f32(components, px, 3 * (int64_t)px.C, "feature_pca_image", "components");
-    pca_check_f32(range, px, 2, "feature_pca_image", "range");
+    const float* mp = in_place(mean, x.device(), px.C, "feature_pca_image: mean");
+    const float* cp = in_place(components, x.device(), 3 * (int64_t)px.C, "feature_pca_image: components");
+    const float* rp = in_place(range, x.device(), 2, "feature_pca_image: range");
     const c10::cuda::CUDAGuard guard(x.device());
     auto shape = x.sizes().slice(1).vec();
     shape.push_back(3);
     torch::Tensor image = torch::empty(shape, x.options().dtype(torch::kFloat32));
     void* stream = (void*)c10::cuda::getCurrentCUDAStream().stream();
-    if (px.half)
-        check_rc(f3dgs_feature_pca_image_f16x(px.C, px.N, hptr(x), fptr(mean), fptr(components), fptr(range),
-                                              image.data_ptr<float>(), stream),
-                 "f3dgs_feature_pca_image_f16x");
-    else
-        check_rc(f3dgs_feature_pca_image(px.C, px.N, fptr(x), fptr(mean), fptr(components), fptr(range),
-                                         image.data_ptr<float>(), stream),
-                 "f3dgs_feature_pca_image");
+    call_f32_or_f16(x, f3dgs_feature_pca_image, "f3dgs_feature_pca_image", f3dgs_feature_pca_image_f16x,
+                    "f3dgs_feature_pca_image_f16x", [&](auto fn, auto xp) {
+                        return fn(px.C, px.N, xp, mp, cp, rp, image.data_ptr<float>(), stream);
+                    });
     return image;
 }
 
@@ -587,9 +565,7 @@ torch::Tensor knnMeanDist(const torch::Tensor& points) {
     const int P = (int)p.size(0);
     torch::Tensor out = torch::empty({P}, p.options());
     if (P == 0) return out;
-    const size_t bytes = f3dgs_knn_scratch_bytes(P);
-    TORCH_CHECK(bytes > 0, "f3dgs_knn_scratch_bytes failed: ", f3dgs_last_error());
-    torch::Tensor scratch = torch::empty({(int64_t)bytes}, p.options().dtype(torch::kByte));
+    torch::Tensor scratch = scratch_tensor(f3dgs_knn_scratch_bytes(P), "f3dgs_knn_scratch_bytes", p);
     cudaStream_t stream = c10::cuda::getCurrentCUDAStream().stream();
     check_rc(f3dgs_knn_mean_dist(P, fptr(p), out.data_ptr<float>(), reinterpret_cast<char*>(scratch.data_ptr()),
                                  (void*)stream),
@@ -598,11 +574,6 @@ torch::Tensor knnMeanDist(const torch::Tensor& points) {
 }
 
 // ---- densification (f3dgs_densify_plan / f3dgs_densify_apply / f3dgs_reset_opacity)
-void check_f32(const torch::Tensor& t, const torch::Device& dev, int64_t numel, const char* what) {
-    TORCH_CHECK(t.is_cuda() && t.device() == dev && t.scalar_type() == torch::kFloat32 && t.is_contiguous(), what,
-                " must be a contiguous float32 tensor on ", dev);
-    TORCH_CHECK(t.numel() == numel, what, ": expected ", numel, " elements, got ", t.numel());
-}
 
 // -> (scratch, counts): counts = device int32[4] {originals kept, clones kept, children kept per copy, split}
 std::tuple<torch::Tensor, torch::Tensor> densifyPlan(const torch::Tensor& grad_accum, const torch::Tensor& denom,
@@ -616,19 +587,17 @@ std::tuple<torch::Tensor, torch::Tensor> densifyPlan(const torch::Tensor& grad_a
     const auto dev = raw_scaling.device();
     const int P = (int)raw_scaling.size(0);
     auto ga = grad_accum.contiguous(), dn = denom.contiguous();
-    check_f32(ga, dev, P, "grad_accum");
-    check_f32(dn, dev, P, "denom");
-    check_f32(raw_opacity, dev, P, "raw_opacity");
-    check_f32(raw_scaling, dev, 3 * (int64_t)P, "raw_scaling");
-    const size_t bytes = f3dgs_densify_scratch_bytes(P);
-    TORCH_CHECK(P == 0 || bytes > 0, "f3dgs_densify_scratch_bytes failed: ", f3dgs_last_error());
-    torch::Tensor scratch = torch::empty({(int64_t)bytes}, raw_scaling.options().dtype(torch::kByte));
+    const float* gp = in_place(ga, dev, P, "grad_accum");
+    const float* dp = in_place(dn, dev, P, "denom");
+    const float* op = in_place(raw_opacity, dev, P, "raw_opacity");
+    const float* sp = in_place(raw_scaling, dev, 3 * (int64_t)P, "raw_scaling");
+    torch::Tensor scratch = scratch_tensor(f3dgs_densify_scratch_bytes(P), "f3dgs_densify_scratch_bytes", raw_scaling);
     torch::Tensor counts = torch::empty({4}, raw_scaling.options().dtype(torch::kInt32));
     cudaStream_t stream = c10::cuda::getCurrentCUDAStream().stream();
-    check_rc(f3dgs_densify_plan(P, fptr(ga), fptr(dn), fptr(raw_opacity), fptr(raw_scaling), (float)max_grad,
-                                (float)dense_scale, (float)min_opacity, (float)max_world_scale,
-                                bytes ? reinterpret_cast<char*>(scratch.data_ptr()) : nullptr, counts.data_ptr<int32_t>(),
-                                (void*)stream),
+    check_rc(f3dgs_densify_plan(P, gp, dp, op, sp, (float)max_grad, (float)dense_scale, (float)min_opacity,
+                                (float)max_world_scale,
+                                scratch.numel() ? reinterpret_cast<char*>(scratch.data_ptr()) : nullptr,
+                                counts.data_ptr<int32_t>(), (void*)stream),
              "f3dgs_densify_plan");
     return std::make_tuple(scratch, counts);
 }
@@ -650,35 +619,30 @@ void densifyApply(const torch::Tensor& scratch, const std::vector<int64_t>& coun
     static const char* names[7] = {"xyz", "f_dc", "f_rest", "opacity", "scaling", "rotation", "semantic_feature"};
     f3dgs_gaussian_fields f[2][3];
     for (int i = 0; i < 21; i++) {
-        check_f32(src[i], dev, P * width[i % 7], names[i % 7]);
-        check_f32(dst[i], dev, Pn * width[i % 7], names[i % 7]);
         for (int k = 0; k < 2; k++) {
-            float* p = const_cast<float*>(fptr(k ? dst[i] : src[i]));
             f3dgs_gaussian_fields& g = f[k][i / 7];
             float** slot[7] = {&g.xyz, &g.f_dc, &g.f_rest, &g.opacity, &g.scaling, &g.rotation, &g.semantic_feature};
-            *slot[i % 7] = p;
+            *slot[i % 7] = in_place(k ? dst[i] : src[i], dev, (k ? Pn : P) * width[i % 7], names[i % 7]);
         }
     }
-    check_f32(normals, dev, 6 * counts[3], "normals");
+    const float* np = in_place(normals, dev, 6 * counts[3], "normals");
     const int32_t c32[4] = {(int32_t)counts[0], (int32_t)counts[1], (int32_t)counts[2], (int32_t)counts[3]};
     cudaStream_t stream = c10::cuda::getCurrentCUDAStream().stream();
     check_rc(f3dgs_densify_apply((int)P, (int)M, (int)C,
                                  scratch.numel() ? reinterpret_cast<const char*>(scratch.data_ptr()) : nullptr, c32,
-                                 fptr(normals), f[0], f[1], (void*)stream),
+                                 np, f[0], f[1], (void*)stream),
              "f3dgs_densify_apply");
 }
 
 void resetOpacity(torch::Tensor raw_opacity, torch::Tensor exp_avg, torch::Tensor exp_avg_sq, double ceiling) {
     TORCH_CHECK(raw_opacity.is_cuda(), "parameters must be CUDA tensors (this build has no CPU path)");
     TORCH_CHECK(raw_opacity.numel() <= INT32_MAX, "reset_opacity: P must be below 2^31");
-    const c10::cuda::CUDAGuard guard(raw_opacity.device());
+    const auto dev = raw_opacity.device();
+    const c10::cuda::CUDAGuard guard(dev);
     const int64_t P = raw_opacity.numel();
-    check_f32(raw_opacity, raw_opacity.device(), P, "raw_opacity");
-    check_f32(exp_avg, raw_opacity.device(), P, "exp_avg");
-    check_f32(exp_avg_sq, raw_opacity.device(), P, "exp_avg_sq");
     cudaStream_t stream = c10::cuda::getCurrentCUDAStream().stream();
-    check_rc(f3dgs_reset_opacity((int)P, const_cast<float*>(fptr(raw_opacity)), const_cast<float*>(fptr(exp_avg)),
-                                 const_cast<float*>(fptr(exp_avg_sq)), (float)ceiling, (void*)stream),
+    check_rc(f3dgs_reset_opacity((int)P, in_place(raw_opacity, dev, P, "raw_opacity"), in_place(exp_avg, dev, P, "exp_avg"),
+                                 in_place(exp_avg_sq, dev, P, "exp_avg_sq"), (float)ceiling, (void*)stream),
              "f3dgs_reset_opacity");
 }
 
@@ -687,31 +651,31 @@ void activateParams(const torch::Tensor& raw_opacity, const torch::Tensor& raw_s
                     const torch::Tensor& f_dc, const torch::Tensor& f_rest, torch::Tensor opacity, torch::Tensor scales,
                     torch::Tensor rotations, torch::Tensor shs) {
     TORCH_CHECK(raw_opacity.is_cuda(), "parameters must be CUDA tensors (this build has no CPU path)");
-    const c10::cuda::CUDAGuard guard(raw_opacity.device());
-    const int P = raw_opacity.size(0);
+    const auto dev = raw_opacity.device();
+    const c10::cuda::CUDAGuard guard(dev);
+    const int64_t P = raw_opacity.size(0);
     const int M = shs.defined() && shs.numel() ? (int)shs.size(1) : 0;
-    for (const torch::Tensor* t : std::initializer_list<const torch::Tensor*>{&raw_opacity, &raw_scaling, &raw_rotation, &f_dc, &f_rest, &opacity, &scales, &rotations, &shs})
-        TORCH_CHECK(!t->defined() || t->numel() == 0 || (t->is_cuda() && t->is_contiguous() && t->scalar_type() == torch::kFloat32),
-                    "activate: tensors must be contiguous float32 CUDA tensors");
+    auto ro = input(raw_opacity, dev, "raw_opacity"), rs = input(raw_scaling, dev, "raw_scaling");
+    auto rr = input(raw_rotation, dev, "raw_rotation"), dc = input(f_dc, dev, "f_dc"), rest = input(f_rest, dev, "f_rest");
     cudaStream_t stream = c10::cuda::getCurrentCUDAStream().stream();
-    check_rc(f3dgs_activate(P, M, fptr(raw_opacity), fptr(raw_scaling), fptr(raw_rotation), fptr(f_dc), fptr(f_rest),
-                            const_cast<float*>(fptr(opacity)), const_cast<float*>(fptr(scales)),
-                            const_cast<float*>(fptr(rotations)), const_cast<float*>(fptr(shs)), (void*)stream),
+    check_rc(f3dgs_activate((int)P, M, fptr(ro), fptr(rs), fptr(rr), fptr(dc), fptr(rest),
+                            in_place(opacity, dev, P, "opacity"), in_place(scales, dev, 3 * P, "scales"),
+                            in_place(rotations, dev, 4 * P, "rotations"), in_place(shs, dev, 3 * M * P, "shs"),
+                            (void*)stream),
              "f3dgs_activate");
 }
 
 void adamStep(int64_t kind, torch::Tensor param, const torch::Tensor& grad_activated, torch::Tensor exp_avg,
               torch::Tensor exp_avg_sq, int64_t M, double lr, double beta1, double beta2, double eps, int64_t step) {
     TORCH_CHECK(param.is_cuda(), "parameters must be CUDA tensors (this build has no CPU path)");
-    const c10::cuda::CUDAGuard guard(param.device());
-    for (const torch::Tensor* t : std::initializer_list<const torch::Tensor*>{&param, &grad_activated, &exp_avg, &exp_avg_sq})
-        TORCH_CHECK(t->is_cuda() && t->is_contiguous() && t->scalar_type() == torch::kFloat32,
-                    "adam_step: tensors must be contiguous float32 CUDA tensors");
-    TORCH_CHECK(exp_avg.numel() == param.numel() && exp_avg_sq.numel() == param.numel(), "adam_step: state shape mismatch");
+    const auto dev = param.device();
+    const c10::cuda::CUDAGuard guard(dev);
+    const int64_t n = param.numel();
+    auto g = input(grad_activated, dev, "grad_activated");
     cudaStream_t stream = c10::cuda::getCurrentCUDAStream().stream();
-    check_rc(f3dgs_adam_step((int)kind, (size_t)param.numel(), (int)M, param.data_ptr<float>(), fptr(grad_activated),
-                             exp_avg.data_ptr<float>(), exp_avg_sq.data_ptr<float>(), (float)lr, (float)beta1, (float)beta2,
-                             (float)eps, (int)step, (void*)stream),
+    check_rc(f3dgs_adam_step((int)kind, (size_t)n, (int)M, in_place(param, dev, n, "param"), fptr(g),
+                             in_place(exp_avg, dev, n, "exp_avg"), in_place(exp_avg_sq, dev, n, "exp_avg_sq"), (float)lr,
+                             (float)beta1, (float)beta2, (float)eps, (int)step, (void*)stream),
              "f3dgs_adam_step");
 }
 

@@ -100,3 +100,24 @@ def test_mark_visible_and_backward_validate(lib):
     args = [5, 3, 16, 0, 4, null, 64, 64] + [null] * 4 + [null, ctypes.c_float(1.0), null, null, null, null, null,
             ctypes.c_float(0.5), ctypes.c_float(0.5), null, null, null, null] + [null] * 14 + [0, null]
     assert lib.f3dgs_backward(*args) == -1
+
+
+def test_every_entry_point_reports_its_own_error(lib):
+    """A rejected call names itself in the last error, also after another entry point failed."""
+    lib.f3dgs_last_error.restype = ctypes.c_char_p
+    null = ctypes.c_void_p(0)
+    one = ctypes.c_float(1.0)
+    calls = {
+        b"f3dgs_adam_step": lambda: lib.f3dgs_adam_step(99, ctypes.c_size_t(4), 1, null, null, null, null, one, one,
+                                                        one, one, 1, null),
+        b"f3dgs_activate": lambda: lib.f3dgs_activate(-1, 1, null, null, null, null, null, null, null, null, null, null),
+        b"f3dgs_knn_mean_dist": lambda: lib.f3dgs_knn_mean_dist(-1, null, null, null, null),
+    }
+    for name, call in calls.items():
+        for other, fail_first in calls.items():
+            if other != name:
+                assert fail_first() == -1
+                assert call() == -1
+                assert lib.f3dgs_last_error().startswith(name + b": "), (name, lib.f3dgs_last_error())
+    lib.f3dgs_launch_count.restype = ctypes.c_ulonglong
+    assert lib.f3dgs_launch_count() == 0
