@@ -157,7 +157,9 @@ __device__ __forceinline__ void ring_init(RING& ring, int n_stage_consumers, int
         mbar_fence_init();
     }
     if (CH > 0) {
-        // rows shorter than CH (last channel chunk) rely on zero padding
+        // Zero the rings once per CTA.  A row shorter than CH (C < CH, or the last channel chunk) fills only the head of
+        // its stage row; the tail keeps channels of an earlier work item, which the feature warps accumulate too.  Those
+        // accumulators never reach memory: the epilogue stores channel ch only if ch < C.
         float4* p = reinterpret_cast<float4*>(&ring.stage[0]);
         const int n16 = (int)(sizeof(Stage<CH>) * kStages / 16);
         for (int i = threadIdx.x; i < n16; i += blockDim.x) p[i] = make_float4(0.f, 0.f, 0.f, 0.f);

@@ -84,7 +84,8 @@ def test_forward_rejects_bad_arguments_before_touching_cuda(lib):
                                  ctypes.c_float(0.5), 0, null, null, null, null, 0, null)
 
     assert call(P=-1) == -1 and b"bad sizes" in lib.f3dgs_last_error()
-    assert call(C=5000) == -1
+    assert call(C=4097) == -1 and b"bad sizes" in lib.f3dgs_last_error()  # F3DGS_MAX_FEATURE_DIM + 1
+    assert call(C=4096) == -1 and b"NULL required pointer" in lib.f3dgs_last_error()  # the limit itself passes
     assert call(W=0) == -1
     assert call(D=4) == -1
     assert call(allocs=False) == -1 and b"allocator" in lib.f3dgs_last_error()

@@ -218,7 +218,7 @@ def classes(st, ga, dn):
 # ---------------------------------------------------------------------------------------------------- GPU tests
 @pytest.mark.gpu
 @pytest.mark.parametrize("M", [1, 16])
-@pytest.mark.parametrize("C", [0, 3, 32, 128])
+@pytest.mark.parametrize("C", [0, 3, 32, 128, 257, 512])
 @pytest.mark.parametrize("P", [0, 1, 1000, 200_000])
 def test_densify_matches_restatement(P, C, M):
     st, ga, dn = make_state(P, C, M, seed=P + 7 * C + M)

@@ -84,18 +84,25 @@ def test_golden_fixtures_match_gpu():
 
 
 # ------------------------------------------------------------------------------------------- feature widths
-@pytest.mark.parametrize("C", [0, 1, 3, 4, 5, 8, 16, 31, 32, 33, 64, 100, 128, 129, 160, 256, 300])
+@pytest.mark.parametrize("C", [0, 1, 3, 4, 5, 8, 16, 31, 32, 33, 64, 100, 128, 129, 160, 256, 300,
+                               384, 511, 512, 513, 516, 1000, 1024, 2048, 4096])
 def test_feature_widths(C):
     """Run-time feature width incl. widths that are not a multiple of 4 (no bulk-copy path), padding inside a
-    128-channel chunk and multi-chunk widths (> 128)."""
+    128-channel chunk and multi-chunk widths (> 128) up to F3DGS_MAX_FEATURE_DIM = 4096 (32 chunks).  513 leaves a
+    one-channel last chunk with no bulk copies, 516 a 16-byte bulk row after four full chunks."""
     sc = scenegen.make_scene(P=1500, W=96, H=64, C=C, sh_degree=1, seed=100 + C)
     _check(sc, sc.cameras[0])
 
 
 # ------------------------------------------------------------------------------------------- image shapes
-@pytest.mark.parametrize("W,H", [(83, 61), (100, 40), (16, 16), (17, 33), (250, 10), (8, 8)])
-def test_image_shapes_not_multiple_of_tile_or_vector(W, H):
-    sc = scenegen.make_scene(P=800, W=W, H=H, C=8, sh_degree=2, seed=W * 1000 + H, target_radius_px=4.0)
+SHAPES = [(83, 61, 8), (100, 40, 8), (16, 16, 8), (17, 33, 8), (250, 10, 8), (8, 8, 8), (83, 61, 513), (83, 61, 4096)]
+
+
+@pytest.mark.parametrize("W,H,C", SHAPES, ids=[f"{w}-{h}" + (f"-C{c}" if c != 8 else "") for w, h, c in SHAPES])
+def test_image_shapes_not_multiple_of_tile_or_vector(W, H, C):
+    """Partial tiles, and widths with W % 4 != 0 (scalar feature stores and image-row loads); 83x61 also with 5 and 32
+    channel chunks (C = 513, 4096)."""
+    sc = scenegen.make_scene(P=800, W=W, H=H, C=C, sh_degree=2, seed=W * 1000 + H, target_radius_px=4.0)
     _check(sc, sc.cameras[0])
 
 
@@ -347,7 +354,7 @@ def test_c3_feature_linearity_and_width_independence(c3_scene):
 # ------------------------------------------------------------------------------------------- view batches
 def _view_batch_case(name):
     """-> (scene with 3 cameras, settings overrides).  Beyond tiny / small: the camera-inside-the-cloud scene of
-    test_gpu_regimes (visibility, and so `denom`, differs per view), C = 0 / 3 / 200, SH degree 0 and 3, odd P,
+    test_gpu_regimes (visibility, and so `denom`, differs per view), C = 0 / 3 / 200 / 512, SH degree 0 and 3, odd P,
     focal_x != focal_y and scale_modifier != 1."""
     import test_gpu_regimes as regimes
 
@@ -357,6 +364,7 @@ def _view_batch_case(name):
         "inside_C0_sh0": (dict(C=0, P=4001, sh_degree=0), 1.0, 1.0),
         "inside_C3_sh3": (dict(C=3, P=4001, sh_degree=3), 1.0, 1.0),
         "inside_C200_sh3": (dict(C=200, P=3001, sh_degree=3), 1.0, 1.0),
+        "inside_C512_sh3": (dict(C=512, P=3001, sh_degree=3), 1.0, 1.0),
         "inside_C16_fy_mod": (dict(C=16, P=4001, sh_degree=2), 1.15, 1.3),
         "inside_wide_C16_fy_mod": (dict(C=16, P=6001, sh_degree=1, target_radius_px=40.0), 1 / 1.15, 0.7),
     }
@@ -368,7 +376,7 @@ def _view_batch_case(name):
 
 
 @pytest.mark.parametrize("name", ["tiny", "small", "inside_C0_sh0", "inside_C3_sh3", "inside_C200_sh3",
-                                  "inside_C16_fy_mod", "inside_wide_C16_fy_mod"])
+                                  "inside_C512_sh3", "inside_C16_fy_mod", "inside_wide_C16_fy_mod"])
 def test_view_batch_accumulates_like_autograd(name):
     """ViewBatch (f3dgs_backward_accum: gradients ADDED in-kernel into one flat buffer, densification statistics folded
     in) against the sum over views of the per-view gradients from the reference-compatible autograd API."""

@@ -142,10 +142,10 @@ def _check_all(sc, cam, label, **opts):
 
 
 # ------------------------------------------------------------------------------------------- regimes x feature widths
-CASES = [("inside", 0), ("inside", 16), ("inside", 200), ("inside_wide", 3), ("inside_wide", 128),
+CASES = [("inside", 0), ("inside", 16), ("inside", 200), ("inside", 512), ("inside_wide", 3), ("inside_wide", 128),
          ("needles", 3), ("needles", 128),
          ("needles_inside", 0), ("needles_inside", 3), ("needles_inside", 16), ("needles_inside", 128),
-         ("needles_inside", 200), ("plane", 3), ("plane", 16), ("plane", 128)]
+         ("needles_inside", 200), ("needles_inside", 512), ("plane", 3), ("plane", 16), ("plane", 128), ("plane", 512)]
 
 
 @pytest.mark.parametrize("name,C", CASES)
@@ -223,7 +223,7 @@ def _offset_copy(x):
     return y
 
 
-@pytest.mark.parametrize("C", [4, 16, 128, 256])
+@pytest.mark.parametrize("C", [4, 16, 128, 256, 512, 4096])
 def test_misaligned_features_and_feature_gradients(C):
     """semantic_feature and dL/dfeature_map given as contiguous views at a 1-float storage offset with C % 4 == 0:
     the forward composite (use_bulk, composite_fwd.cu) and the feature backward (vec, feature_bwd.cu) test the

@@ -19,9 +19,9 @@ from oracle.next_rows import resize_bilinear_ac, resize_bilinear_ac_bwd
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 DECODE_REL = 1.2e-3  # the TF32 decode bar of test_feature_decoder.py
-# test_next_rows.py SHAPES plus the LSeg --speedup sizes (map 1080x1920, teacher 480x853)
+# test_next_rows.py SHAPES plus the LSeg --speedup sizes (map 1080x1920, teacher 480x853) and LSeg's full width (C = 512)
 RESIZE_SHAPES = [((5, 37, 53), (21, 30)), ((3, 16, 16), (16, 16)), ((4, 20, 31), (45, 64)), ((2, 9, 7), (1, 1)),
-                 ((6, 54, 96), (24, 43)), ((128, 1080, 1920), (480, 853))]
+                 ((6, 54, 96), (24, 43)), ((128, 1080, 1920), (480, 853)), ((512, 270, 480), (120, 160))]
 DECODER_SHAPES = [(1, 1, 1), (5, 7, 1000), (16, 64, 4099), (128, 512, 409440), (256, 33, 777)]  # test_feature_decoder.py
 
 

@@ -128,7 +128,8 @@ def test_one_tap_gather_rule_holds_for_every_size():
 
 # =================================================================================================== GPU
 @pytest.mark.gpu
-@pytest.mark.parametrize("shape,size", SHAPES + [((128, 270, 480), (120, 160)), ((3, 45, 2101), (20, 900))])
+@pytest.mark.parametrize("shape,size", SHAPES + [((128, 270, 480), (120, 160)), ((3, 45, 2101), (20, 900)),
+                                                 ((512, 270, 480), (120, 160)), ((512, 40, 60), (90, 120))])
 def test_feature_head_kernels_match_pytorch_gpu(shape, size):
     from diff_gaussian_rasterization import feature_head as fh
 
