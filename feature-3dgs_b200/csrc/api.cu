@@ -236,15 +236,21 @@ int f3dgs_get_layout(int P, int width, int height, int R, f3dgs_layout* out) {
     return 0;
 }
 
-int f3dgs_forward(f3dgs_alloc_fn geometry_alloc, void* geometry_ctx, f3dgs_alloc_fn binning_alloc,
-                  void* binning_ctx, f3dgs_alloc_fn image_alloc, void* image_ctx, int P, int D, int M, int C,
-                  const float* background, int width, int height, const float* means3D, const float* shs,
-                  const float* colors_precomp, const float* semantic_feature, const float* opacities,
-                  const float* scales, float scale_modifier, const float* rotations, const float* cov3D_precomp,
-                  const float* viewmatrix, const float* projmatrix, const float* cam_pos, float tan_fovx,
-                  float tan_fovy, int prefiltered, float* out_color, float* out_feature_map, float* out_depth,
-                  int* radii, int debug, void* cuda_stream) {
-    const Api api(__func__);
+}  // extern "C"
+
+namespace {
+
+// Shared body of f3dgs_forward (TF = float) and f3dgs_forward_f16 (TF = __half): TF is the element type of
+// semantic_feature and out_feature_map only.
+template <typename TF>
+int forward_impl(const char* entry, f3dgs_alloc_fn geometry_alloc, void* geometry_ctx, f3dgs_alloc_fn binning_alloc,
+                 void* binning_ctx, f3dgs_alloc_fn image_alloc, void* image_ctx, int P, int D, int M, int C,
+                 const float* background, int width, int height, const float* means3D, const float* shs,
+                 const float* colors_precomp, const TF* semantic_feature, const float* opacities, const float* scales,
+                 float scale_modifier, const float* rotations, const float* cov3D_precomp, const float* viewmatrix,
+                 const float* projmatrix, const float* cam_pos, float tan_fovx, float tan_fovy, int prefiltered,
+                 float* out_color, TF* out_feature_map, float* out_depth, int* radii, int debug, void* cuda_stream) {
+    const Api api(entry);
     cudaStream_t stream = (cudaStream_t)cuda_stream;
     if (P < 0 || width <= 0 || height <= 0 || C < 0 || C > F3DGS_MAX_FEATURE_DIM || D < 0 || D > 3)
         return api.invalid("bad sizes (P, width, height, C or D)");
@@ -359,6 +365,39 @@ int f3dgs_forward(f3dgs_alloc_fn geometry_alloc, void* geometry_ctx, f3dgs_alloc
     if (const int rc = api.cuda(e, "composite_fwd launch")) return rc;
     STAGE_CHECK("composite_fwd");
     return R;
+}
+
+}  // namespace
+
+extern "C" {
+
+int f3dgs_forward(f3dgs_alloc_fn geometry_alloc, void* geometry_ctx, f3dgs_alloc_fn binning_alloc,
+                  void* binning_ctx, f3dgs_alloc_fn image_alloc, void* image_ctx, int P, int D, int M, int C,
+                  const float* background, int width, int height, const float* means3D, const float* shs,
+                  const float* colors_precomp, const float* semantic_feature, const float* opacities,
+                  const float* scales, float scale_modifier, const float* rotations, const float* cov3D_precomp,
+                  const float* viewmatrix, const float* projmatrix, const float* cam_pos, float tan_fovx,
+                  float tan_fovy, int prefiltered, float* out_color, float* out_feature_map, float* out_depth,
+                  int* radii, int debug, void* cuda_stream) {
+    return forward_impl(__func__, geometry_alloc, geometry_ctx, binning_alloc, binning_ctx, image_alloc, image_ctx, P,
+                        D, M, C, background, width, height, means3D, shs, colors_precomp, semantic_feature, opacities,
+                        scales, scale_modifier, rotations, cov3D_precomp, viewmatrix, projmatrix, cam_pos, tan_fovx,
+                        tan_fovy, prefiltered, out_color, out_feature_map, out_depth, radii, debug, cuda_stream);
+}
+
+int f3dgs_forward_f16(f3dgs_alloc_fn geometry_alloc, void* geometry_ctx, f3dgs_alloc_fn binning_alloc,
+                      void* binning_ctx, f3dgs_alloc_fn image_alloc, void* image_ctx, int P, int D, int M, int C,
+                      const float* background, int width, int height, const float* means3D, const float* shs,
+                      const float* colors_precomp, const uint16_t* semantic_feature, const float* opacities,
+                      const float* scales, float scale_modifier, const float* rotations, const float* cov3D_precomp,
+                      const float* viewmatrix, const float* projmatrix, const float* cam_pos, float tan_fovx,
+                      float tan_fovy, int prefiltered, float* out_color, uint16_t* out_feature_map, float* out_depth,
+                      int* radii, int debug, void* cuda_stream) {
+    return forward_impl(__func__, geometry_alloc, geometry_ctx, binning_alloc, binning_ctx, image_alloc, image_ctx, P,
+                        D, M, C, background, width, height, means3D, shs, colors_precomp,
+                        reinterpret_cast<const __half*>(semantic_feature), opacities, scales, scale_modifier, rotations,
+                        cov3D_precomp, viewmatrix, projmatrix, cam_pos, tan_fovx, tan_fovy, prefiltered, out_color,
+                        reinterpret_cast<__half*>(out_feature_map), out_depth, radii, debug, cuda_stream);
 }
 
 }  // extern "C"

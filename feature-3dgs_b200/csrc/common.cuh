@@ -141,6 +141,15 @@ __device__ __forceinline__ void st_na_f8(float* p, float4 a, float4 b) {
     st_na_f4(p, a);
     st_na_f4(p + 4, b);
 }
+// the same store of packed 16-bit data (float16 maps): 16 bytes to a 16-byte aligned p, 8 bytes to an 8-byte aligned p
+__device__ __forceinline__ void st_na_b128(void* p, uint4 v) {
+    asm volatile("st.global.L1::no_allocate.v4.b32 [%0], {%1,%2,%3,%4};" ::"l"(p), "r"(v.x), "r"(v.y), "r"(v.z),
+                 "r"(v.w)
+                 : "memory");
+}
+__device__ __forceinline__ void st_na_b64(void* p, uint2 v) {
+    asm volatile("st.global.L1::no_allocate.v2.b32 [%0], {%1,%2};" ::"l"(p), "r"(v.x), "r"(v.y) : "memory");
+}
 __device__ __forceinline__ float4 ld_nc_f4(const float* p) {
     float4 v;
     asm volatile("ld.global.nc.L1::no_allocate.v4.f32 {%0,%1,%2,%3}, [%4];"

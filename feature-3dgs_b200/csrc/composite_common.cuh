@@ -8,8 +8,8 @@
 //                         instances whose alpha >= 1/255 footprint cannot reach the tile, and fills
 //                         a ring of stages with 48-byte splat records via 128-bit loads.  When there
 //                         are features, warp 1 (the copy warp) fetches the stage's C-wide feature
-//                         rows with 1-D TMA bulk copies (cp.async.bulk -> UBLKCP) that complete on
-//                         the stage's `full` mbarrier.  The producer runs ahead across tile
+//                         rows (float32 or float16: the ring's element type TF) with 1-D TMA bulk
+//                         copies (cp.async.bulk -> UBLKCP) that complete on the stage's `full` mbarrier.  The producer runs ahead across tile
 //                         boundaries, so the next tile's first stage is already resident when the
 //                         consumers get there (no per-tile start-up bubble).  Warps 2 and 3 retire.
 //   alpha warps (8)       warp a owns the 8x4 pixel block a of the tile, one pixel per lane: alpha,
@@ -41,9 +41,10 @@ constexpr int kDoneSlots = 8;       // > kStages: the producer is never further 
                                     // CTA's own work sequence number, NOT by the work id: ids come from a global
                                     // atomic counter, so two items in flight in one CTA can be congruent mod 8.
 
-template <int CH>
+// TF: element type of the staged feature rows, float or __half (a float16 row is half the bytes)
+template <int CH, typename TF = float>
 struct alignas(128) Stage {
-    float feat[CH > 0 ? kStageEntries : 1][CH > 0 ? CH : 4];  // CH == 0: 16 B dummy, never touched
+    TF feat[CH > 0 ? kStageEntries : 1][CH > 0 ? CH : 4];  // CH == 0: dummy, never touched
     float4 rec0[kStageEntries];                   // x, y, ex, ey
     float4 rec1[kStageEntries];                   // conic a, b, c, opacity
     float4 rec2[kStageEntries];                   // r, g, b, depth
@@ -65,10 +66,11 @@ struct alignas(128) WSlot {
     int32_t work;
 };
 
-template <int CH>
+template <int CH, typename TF = float>
 struct alignas(128) RingV2 {
+    using Feat = TF;
     static constexpr int kWB = kBlocksPerTile, kWJ = kWSlots;  // dimensions of the weight-slot ring
-    Stage<CH> stage[kStages];
+    Stage<CH, TF> stage[kStages];
     WSlot ws[kBlocksPerTile][kWSlots];
     uint64_t full[kStages];
     uint64_t empty[kStages];
@@ -82,6 +84,7 @@ struct alignas(128) RingV2 {
 // 14 KB instead of 83 KB of shared memory, so that two CTAs fit on an SM.  The one-element `ws` / `wfull` / `wempty` are
 // not used; ring_init<> initialises the two barriers.
 struct alignas(128) RingSlim {
+    using Feat = float;
     static constexpr int kWB = 1, kWJ = 1;
     Stage<0> stage[kStages];
     WSlot ws[1][1];
@@ -161,7 +164,7 @@ __device__ __forceinline__ void ring_init(RING& ring, int n_stage_consumers, int
         // its stage row; the tail keeps channels of an earlier work item, which the feature warps accumulate too.  Those
         // accumulators never reach memory: the epilogue stores channel ch only if ch < C.
         float4* p = reinterpret_cast<float4*>(&ring.stage[0]);
-        const int n16 = (int)(sizeof(Stage<CH>) * kStages / 16);
+        const int n16 = (int)(sizeof(ring.stage) / 16);
         for (int i = threadIdx.x; i < n16; i += blockDim.x) p[i] = make_float4(0.f, 0.f, 0.f, 0.f);
         // order these generic-proxy stores before the async-proxy (bulk copy) writes to the same rows
         asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
@@ -173,7 +176,7 @@ struct ProducerArgs {
     const uint2* ranges;
     const uint32_t* point_list;
     const SplatRec* rec;
-    const float* features;      // nullptr: no feature rows (backward, or C == 0)
+    const void* features;       // [P, C] of the ring's element type; nullptr: no feature rows (backward, or C == 0)
     const uint32_t* n_contrib;  // backward only: bounds the reverse walk
     int* work_counter;          // zeroed by the launcher; tiles are handed out with atomicAdd
     int W, H, C;
@@ -189,6 +192,7 @@ struct ProducerArgs {
 // producer is on the pipeline's critical path.
 template <int CH, bool REVERSE, typename RING = RingV2<CH>>
 __device__ __forceinline__ void producer_loop(RING& ring, const ProducerArgs& pa) {
+    using TF = typename RING::Feat;
     constexpr bool COPYWARP = CH > 0;
     const int lane = threadIdx.x & 31;
     int s = 0;
@@ -199,7 +203,7 @@ __device__ __forceinline__ void producer_loop(RING& ring, const ProducerArgs& pa
     auto publish = [&](uint32_t n, uint32_t last, uint32_t first, int work) {
         __syncwarp();
         if (lane == 0) {
-            Stage<CH>& st = ring.stage[s];
+            Stage<CH, TF>& st = ring.stage[s];
             st.done_slot = seq % kDoneSlots;
             st.n = n;
             st.last = last;
@@ -257,15 +261,15 @@ __device__ __forceinline__ void producer_loop(RING& ring, const ProducerArgs& pa
             return REVERSE ? (range_begin + walk_count - 1 - i) : (range_begin + i);
         };
         auto store_entry = [&](uint32_t slot, uint32_t gid, uint32_t lpos, float4 r0, float4 r1, float4 r2) {
-            Stage<CH>& st = ring.stage[s];
+            Stage<CH, TF>& st = ring.stage[s];
             st.rec0[slot] = r0;
             st.rec1[slot] = r1;
             st.rec2[slot] = r2;
             st.listpos[slot] = lpos;
             st.gid[slot] = gid;
             if (CH > 0 && row_floats > 0) {
-                const float* src = pa.features + (size_t)gid * pa.C + chunk_off;
-                if (!pa.use_bulk)  // unaligned rows or C % 4 != 0: no bulk copies, the producer loads the row
+                const TF* src = static_cast<const TF*>(pa.features) + (size_t)gid * pa.C + chunk_off;
+                if (!pa.use_bulk)  // unaligned rows or rows not a multiple of 16 bytes: the producer loads the row
                     for (int c = 0; c < row_floats; c++) st.feat[slot][c] = __ldg(src + c);
             }
         };
@@ -325,14 +329,14 @@ __device__ __forceinline__ void producer_loop(RING& ring, const ProducerArgs& pa
 }
 
 // Second warp of the producer group (forward with features): fetches the feature rows of each listed stage.
-template <int CH>
-__device__ __forceinline__ void copy_loop(RingV2<CH>& ring, const ProducerArgs& pa) {
+template <int CH, typename TF>
+__device__ __forceinline__ void copy_loop(RingV2<CH, TF>& ring, const ProducerArgs& pa) {
     const int lane = threadIdx.x & 31;
     int s = 0;
     uint32_t parity = 0;
     for (;;) {
         mbar_wait(&ring.listed[s], parity);
-        Stage<CH>& st = ring.stage[s];
+        Stage<CH, TF>& st = ring.stage[s];
         const uint32_t n = st.n;
         const int work = st.work;
         if (work < 0) {
@@ -340,12 +344,13 @@ __device__ __forceinline__ void copy_loop(RingV2<CH>& ring, const ProducerArgs& 
             break;
         }
         const int chunk_off = (work % pa.chunks) * CH;
-        const uint32_t row_bytes = (uint32_t)min(CH, pa.C - chunk_off) * 4u;
+        const uint32_t row_bytes = (uint32_t)min(CH, pa.C - chunk_off) * (uint32_t)sizeof(TF);
         if (pa.use_bulk && n > 0) {
             if (lane == 0) mbar_arrive_expect_tx(&ring.full[s], n * row_bytes);
             __syncwarp();
             if (lane < n)
-                bulk_g2s(&st.feat[lane][0], pa.features + (size_t)st.gid[lane] * pa.C + chunk_off, row_bytes,
+                bulk_g2s(&st.feat[lane][0],
+                         static_cast<const TF*>(pa.features) + (size_t)st.gid[lane] * pa.C + chunk_off, row_bytes,
                          &ring.full[s]);
         } else {
             if (lane == 0) mbar_arrive(&ring.full[s]);

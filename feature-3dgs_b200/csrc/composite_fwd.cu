@@ -19,8 +19,16 @@
 // Channel counts above 128 are split into chunks of 128 (extra work items); chunk 0 also writes
 // colour, depth, final_T and n_contrib.
 //
+// Feature element type TF (float or __half): the per-Gaussian features and the feature map share it.  A float16 ring
+// stages half the bytes per row; the feature warps upcast each channel exactly as they load it, accumulate in float32
+// exactly as for float32 features, and the epilogue rounds each accumulator once to nearest even.  So a float16 render
+// is bitwise the float32 render of the upcast features followed by .half(), and everything else is bitwise the float32
+// render's (the alpha warps never read features).
+//
 // Registers: the 20 warps are launched at 96 registers per thread (61440 in the CTA pool); setmaxnreg then gives the
 // producer group 40, the alpha warps 64 and the feature warps 152 (4x32x40 + 8x32x64 + 8x32x152 = 60416).
+#include <type_traits>
+
 #include "composite_common.cuh"
 
 namespace f3dgs {
@@ -29,22 +37,38 @@ constexpr int kFwdThreads = (kFeatWarp0 + kBlocksPerTile) * 32;
 constexpr int kRegsAlpha = 64;
 constexpr int kRegsFeature = 152;
 
+template <typename TF>
 struct FwdArgs {
     ProducerArgs pa;
     const float* bg;
     float* final_T;
     uint32_t* n_contrib;
     float* out_color;
-    float* out_feature;
+    TF* out_feature;
     float* out_depth;
     int vec_store;
 };
 
-template <int CH>
+// A lane's 4 channels of a staged feature row as loaded (float4, or 8 bytes of float16) and as float32 (exact).
+template <typename TF>
+using Feat4 = std::conditional_t<std::is_same_v<TF, float>, float4, uint2>;
+__device__ __forceinline__ float4 feat_f32(float4 v) { return v; }
+__device__ __forceinline__ float4 feat_f32(uint2 v) {
+    const float2 a = __half22float2(*reinterpret_cast<const __half2*>(&v.x));
+    const float2 b = __half22float2(*reinterpret_cast<const __half2*>(&v.y));
+    return make_float4(a.x, a.y, b.x, b.y);
+}
+// two accumulators rounded to float16 (nearest even, as torch's .half()), packed low = a
+__device__ __forceinline__ uint32_t pack_half2(float a, float b) {
+    const __half2 h = __floats2half2_rn(a, b);
+    return *reinterpret_cast<const uint32_t*>(&h);
+}
+
+template <int CH, typename TF>
 __global__ void __launch_bounds__(kFwdThreads, 1)
-composite_fwd_kernel(const FwdArgs args) {
+composite_fwd_kernel(const FwdArgs<TF> args) {
     extern __shared__ __align__(128) unsigned char smem_raw[];
-    using RING = RingV2<CH>;
+    using RING = RingV2<CH, TF>;
     RING& ring = *reinterpret_cast<RING*>(smem_raw);
     // The warp index goes through a shuffle so that ptxas knows it is warp-uniform: role branches, ring/slot addresses
     // and everything loaded from them (instance masks, work ids) then live in uniform registers, the per-quad branches
@@ -63,7 +87,7 @@ composite_fwd_kernel(const FwdArgs args) {
         if (warp == kProducerWarp) {
             producer_loop<CH, false>(ring, args.pa);
         } else if constexpr (CH > 0) {
-            if (warp == kProducerWarp + 1) copy_loop<CH>(ring, args.pa);
+            if (warp == kProducerWarp + 1) copy_loop<CH, TF>(ring, args.pa);
         }
         return;
     }
@@ -80,7 +104,7 @@ composite_fwd_kernel(const FwdArgs args) {
         bool done = true, inside = false, blk_done = true;
         for (;;) {
             mbar_wait(&ring.full[s], parity);
-            Stage<CH>& st = ring.stage[s];
+            Stage<CH, TF>& st = ring.stage[s];
             const uint32_t n = st.n, last = st.last, first = st.first;
             const int work = st.work;
             if (work < 0) break;
@@ -237,20 +261,20 @@ composite_fwd_kernel(const FwdArgs args) {
             uint32_t km = ws.km;
             const uint32_t last = ws.last;
             mbar_wait(&ring.full[s], parity);  // feature rows landed
-            const Stage<CH>& st = ring.stage[s];
+            const Stage<CH, TF>& st = ring.stage[s];
             // the next instance's pixel mask and feature float4 are requested before this instance's FMAs, so their
             // LDS latency hides behind the FMA stream instead of heading every instance
             int kn = km ? __ffs(km) - 1 : 0;
             uint32_t pm_n = ws.pm[kn];
-            float4 f_n = *reinterpret_cast<const float4*>(&st.feat[kn][cl * 4]);
+            Feat4<TF> f_n = *reinterpret_cast<const Feat4<TF>*>(&st.feat[kn][cl * 4]);
             while (km) {
                 const int k = kn;
                 const uint32_t pm = pm_n;
-                const float4 f = f_n;
+                const float4 f = feat_f32(f_n);
                 km &= km - 1;
                 kn = km ? __ffs(km) - 1 : k;
                 pm_n = ws.pm[kn];
-                f_n = *reinterpret_cast<const float4*>(&st.feat[kn][cl * 4]);
+                f_n = *reinterpret_cast<const Feat4<TF>*>(&st.feat[kn][cl * 4]);
 #pragma unroll
                 for (int qi = 0; qi < NQ; qi++) {
                     const int q = qi * G + grp;
@@ -277,45 +301,91 @@ composite_fwd_kernel(const FwdArgs args) {
                 for (int c = 0; c < 4; c++) {
                     const int ch = chunk * CH + cl * 4 + c;
                     if (ch < C) {
-                        float* plane = args.out_feature + (size_t)ch * HW;
-                        if (G == 1 && (args.vec_store & 2) && bx0 + 8 <= W) {
-                            // lane holds all 8 quads: a full 32-byte sector per 8-pixel row
+                        if constexpr (std::is_same_v<TF, float>) {
+                            float* plane = args.out_feature + (size_t)ch * HW;
+                            if (G == 1 && (args.vec_store & 2) && bx0 + 8 <= W) {
+                                // lane holds all 8 quads: a full 32-byte sector per 8-pixel row
 #pragma unroll
-                            for (int y = 0; y < 4; y++) {
-                                const int yy = by0 + y;
-                                if (yy >= H) continue;
-                                const int qa = (y >> 1) * 4, i0 = (y & 1) * 2;
-                                st_na_f8(plane + (size_t)yy * W + bx0,
-                                         make_float4(ACC(qa % NQ, i0, c), ACC(qa % NQ, i0 + 1, c),
-                                                     ACC((qa + 1) % NQ, i0, c), ACC((qa + 1) % NQ, i0 + 1, c)),
-                                         make_float4(ACC((qa + 2) % NQ, i0, c), ACC((qa + 2) % NQ, i0 + 1, c),
-                                                     ACC((qa + 3) % NQ, i0, c), ACC((qa + 3) % NQ, i0 + 1, c)));
-                            }
-                        } else if (G == 1 && (args.vec_store & 1)) {
-                            // rows of 8 pixels -> two 128-bit stores per row
+                                for (int y = 0; y < 4; y++) {
+                                    const int yy = by0 + y;
+                                    if (yy >= H) continue;
+                                    const int qa = (y >> 1) * 4, i0 = (y & 1) * 2;
+                                    st_na_f8(plane + (size_t)yy * W + bx0,
+                                             make_float4(ACC(qa % NQ, i0, c), ACC(qa % NQ, i0 + 1, c),
+                                                         ACC((qa + 1) % NQ, i0, c), ACC((qa + 1) % NQ, i0 + 1, c)),
+                                             make_float4(ACC((qa + 2) % NQ, i0, c), ACC((qa + 2) % NQ, i0 + 1, c),
+                                                         ACC((qa + 3) % NQ, i0, c), ACC((qa + 3) % NQ, i0 + 1, c)));
+                                }
+                            } else if (G == 1 && (args.vec_store & 1)) {
+                                // rows of 8 pixels -> two 128-bit stores per row
 #pragma unroll
-                            for (int y = 0; y < 4; y++) {
-                                const int yy = by0 + y;
-                                if (yy >= H) continue;
+                                for (int y = 0; y < 4; y++) {
+                                    const int yy = by0 + y;
+                                    if (yy >= H) continue;
 #pragma unroll
-                                for (int half = 0; half < 2; half++) {
-                                    const int xx = bx0 + half * 4;
-                                    if (xx >= W) continue;
-                                    const int qa = (y >> 1) * 4 + half * 2, i0 = (y & 1) * 2;
-                                    const float4 v =
-                                        make_float4(ACC(qa % NQ, i0, c), ACC(qa % NQ, i0 + 1, c),
-                                                    ACC((qa + 1) % NQ, i0, c), ACC((qa + 1) % NQ, i0 + 1, c));
-                                    st_na_f4(plane + (size_t)yy * W + xx, v);
+                                    for (int half = 0; half < 2; half++) {
+                                        const int xx = bx0 + half * 4;
+                                        if (xx >= W) continue;
+                                        const int qa = (y >> 1) * 4 + half * 2, i0 = (y & 1) * 2;
+                                        const float4 v =
+                                            make_float4(ACC(qa % NQ, i0, c), ACC(qa % NQ, i0 + 1, c),
+                                                        ACC((qa + 1) % NQ, i0, c), ACC((qa + 1) % NQ, i0 + 1, c));
+                                        st_na_f4(plane + (size_t)yy * W + xx, v);
+                                    }
+                                }
+                            } else {
+#pragma unroll
+                                for (int qi = 0; qi < NQ; qi++) {
+                                    const int q = qi * G + grp;
+#pragma unroll
+                                    for (int i = 0; i < 4; i++) {
+                                        const int xx = bx0 + (q & 3) * 2 + (i & 1), yy = by0 + (q >> 2) * 2 + (i >> 1);
+                                        if (xx < W && yy < H) plane[(size_t)yy * W + xx] = ACC(qi, i, c);
+                                    }
                                 }
                             }
                         } else {
+                            __half* plane = args.out_feature + (size_t)ch * HW;
+                            if (G == 1 && (args.vec_store & 2) && bx0 + 8 <= W) {
+                                // lane holds all 8 quads: one 16-byte store per 8-pixel row
 #pragma unroll
-                            for (int qi = 0; qi < NQ; qi++) {
-                                const int q = qi * G + grp;
+                                for (int y = 0; y < 4; y++) {
+                                    const int yy = by0 + y;
+                                    if (yy >= H) continue;
+                                    const int qa = (y >> 1) * 4, i0 = (y & 1) * 2;
+                                    uint32_t h[4];
 #pragma unroll
-                                for (int i = 0; i < 4; i++) {
-                                    const int xx = bx0 + (q & 3) * 2 + (i & 1), yy = by0 + (q >> 2) * 2 + (i >> 1);
-                                    if (xx < W && yy < H) plane[(size_t)yy * W + xx] = ACC(qi, i, c);
+                                    for (int k = 0; k < 4; k++)
+                                        h[k] = pack_half2(ACC((qa + k) % NQ, i0, c), ACC((qa + k) % NQ, i0 + 1, c));
+                                    st_na_b128(plane + (size_t)yy * W + bx0, make_uint4(h[0], h[1], h[2], h[3]));
+                                }
+                            } else if (G == 1 && (args.vec_store & 1)) {
+                                // rows of 8 pixels -> two 8-byte stores per row
+#pragma unroll
+                                for (int y = 0; y < 4; y++) {
+                                    const int yy = by0 + y;
+                                    if (yy >= H) continue;
+#pragma unroll
+                                    for (int half = 0; half < 2; half++) {
+                                        const int xx = bx0 + half * 4;
+                                        if (xx >= W) continue;
+                                        const int qa = (y >> 1) * 4 + half * 2, i0 = (y & 1) * 2;
+                                        const uint32_t h0 = pack_half2(ACC(qa % NQ, i0, c), ACC(qa % NQ, i0 + 1, c));
+                                        const uint32_t h1 =
+                                            pack_half2(ACC((qa + 1) % NQ, i0, c), ACC((qa + 1) % NQ, i0 + 1, c));
+                                        st_na_b64(plane + (size_t)yy * W + xx, make_uint2(h0, h1));
+                                    }
+                                }
+                            } else {
+#pragma unroll
+                                for (int qi = 0; qi < NQ; qi++) {
+                                    const int q = qi * G + grp;
+#pragma unroll
+                                    for (int i = 0; i < 4; i++) {
+                                        const int xx = bx0 + (q & 3) * 2 + (i & 1), yy = by0 + (q >> 2) * 2 + (i >> 1);
+                                        if (xx < W && yy < H)
+                                            plane[(size_t)yy * W + xx] = __float2half_rn(ACC(qi, i, c));
+                                    }
                                 }
                             }
                         }
@@ -336,12 +406,12 @@ composite_fwd_kernel(const FwdArgs args) {
 #undef ACC
 }
 
-template <int CH>
+template <int CH, typename TF>
 static cudaError_t launch_fwd_t(const ViewParams& vp, const uint2* ranges, const uint32_t* point_list,
-                                const SplatRec* rec, const float* features, const float* bg, float* final_T,
-                                uint32_t* n_contrib, float* out_color, float* out_feature, float* out_depth,
+                                const SplatRec* rec, const TF* features, const float* bg, float* final_T,
+                                uint32_t* n_contrib, float* out_color, TF* out_feature, float* out_depth,
                                 int* work_counter, cudaStream_t s) {
-    const size_t smem = sizeof(RingV2<CH>);
+    const size_t smem = sizeof(RingV2<CH, TF>);
     // the opt-in to > 48 KB of dynamic shared memory is per device (context): remember it per device ordinal, so that one
     // process driving several GPUs works too
     static std::atomic<int> sms_of_device[64];  // zero-initialised; set once per device (idempotent)
@@ -349,15 +419,15 @@ static cudaError_t launch_fwd_t(const ViewParams& vp, const uint2* ranges, const
     cudaGetDevice(&dev);
     if (dev < 0 || dev >= 64) return cudaErrorInvalidDevice;
     if (sms_of_device[dev].load() == 0) {
-        cudaError_t e = cudaFuncSetAttribute(composite_fwd_kernel<CH>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                             (int)smem);
+        cudaError_t e = cudaFuncSetAttribute(composite_fwd_kernel<CH, TF>,
+                                             cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
         if (e != cudaSuccess) return e;
         int n = 0;
         cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
         sms_of_device[dev].store(n > 0 ? n : 132);
     }
     const int num_sms = sms_of_device[dev].load();
-    FwdArgs a;
+    FwdArgs<TF> a;
     a.pa.ranges = ranges; a.pa.point_list = point_list; a.pa.rec = rec;
     a.pa.features = CH > 0 ? features : nullptr;
     a.pa.n_contrib = nullptr;
@@ -366,27 +436,42 @@ static cudaError_t launch_fwd_t(const ViewParams& vp, const uint2* ranges, const
     a.pa.tiles_x = (int)vp.grid_x;
     a.pa.num_tiles = (int)(vp.grid_x * vp.grid_y);
     a.pa.chunks = CH > 0 ? (vp.C + CH - 1) / CH : 1;
-    a.pa.use_bulk = (CH > 0 && vp.C % 4 == 0 && (reinterpret_cast<uintptr_t>(features) & 15) == 0) ? 1 : 0;
+    // bulk copies move rows of a multiple of 16 bytes from 16-byte aligned addresses: C % 4 == 0 (float), C % 8 == 0
+    // (half)
+    constexpr int kPer16 = 16 / (int)sizeof(TF);
+    a.pa.use_bulk = (CH > 0 && vp.C % kPer16 == 0 && (reinterpret_cast<uintptr_t>(features) & 15) == 0) ? 1 : 0;
     a.bg = bg; a.final_T = final_T; a.n_contrib = n_contrib;
     a.out_color = out_color; a.out_feature = out_feature; a.out_depth = out_depth;
-    a.vec_store = (vp.W % 4 == 0 && (reinterpret_cast<uintptr_t>(out_feature) & 15) == 0) ? 1 : 0;
-    if (vp.W % 8 == 0 && (reinterpret_cast<uintptr_t>(out_feature) & 31) == 0) a.vec_store |= 2;
+    // 1: 4-pixel stores (16 B of float, 8 B of half); 2: 8-pixel rows (32 B of float, 16 B of half)
+    const uintptr_t out_addr = reinterpret_cast<uintptr_t>(out_feature);
+    a.vec_store = (vp.W % 4 == 0 && (out_addr & (4 * sizeof(TF) - 1)) == 0) ? 1 : 0;
+    if (vp.W % 8 == 0 && (out_addr & (8 * sizeof(TF) - 1)) == 0) a.vec_store |= 2;
     cudaError_t e = cudaMemsetAsync(work_counter, 0, sizeof(int), s);
     if (e != cudaSuccess) return e;
     const int grid = min(a.pa.num_tiles * a.pa.chunks, num_sms);
-    composite_fwd_kernel<CH><<<grid, kFwdThreads, smem, s>>>(a);
+    composite_fwd_kernel<CH, TF><<<grid, kFwdThreads, smem, s>>>(a);
     g_launches++;
     return cudaGetLastError();
 }
 
+template <typename TF>
 cudaError_t launch_composite_fwd(const ViewParams& vp, const uint2* ranges, const uint32_t* point_list,
-                                 const SplatRec* rec, const float* features, const float* bg,
+                                 const SplatRec* rec, const TF* features, const float* bg,
                                  float* final_T, uint32_t* n_contrib, float* out_color,
-                                 float* out_feature, float* out_depth, int* work_counter, cudaStream_t s) {
-    const auto launch = vp.C == 0 ? launch_fwd_t<0> : vp.C <= 32 ? launch_fwd_t<32> : vp.C <= 64 ? launch_fwd_t<64>
-                                                                                                  : launch_fwd_t<128>;
+                                 TF* out_feature, float* out_depth, int* work_counter, cudaStream_t s) {
+    if (vp.C == 0)  // no feature rows or map: one kernel for both element types
+        return launch_fwd_t<0, float>(vp, ranges, point_list, rec, nullptr, bg, final_T, n_contrib, out_color, nullptr,
+                                      out_depth, work_counter, s);
+    const auto launch = vp.C <= 32 ? launch_fwd_t<32, TF> : vp.C <= 64 ? launch_fwd_t<64, TF> : launch_fwd_t<128, TF>;
     return launch(vp, ranges, point_list, rec, features, bg, final_T, n_contrib, out_color, out_feature, out_depth,
                   work_counter, s);
 }
+
+template cudaError_t launch_composite_fwd<float>(const ViewParams&, const uint2*, const uint32_t*, const SplatRec*,
+                                                 const float*, const float*, float*, uint32_t*, float*, float*, float*,
+                                                 int*, cudaStream_t);
+template cudaError_t launch_composite_fwd<__half>(const ViewParams&, const uint2*, const uint32_t*, const SplatRec*,
+                                                  const __half*, const float*, float*, uint32_t*, float*, __half*,
+                                                  float*, int*, cudaStream_t);
 
 }  // namespace f3dgs

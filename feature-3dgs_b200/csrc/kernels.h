@@ -48,11 +48,13 @@ void launch_duplicate_keys(int P, const SplatRec* rec, const uint32_t* offsets, 
 void launch_tile_ranges(int R, const uint64_t* sorted_keys, uint2* ranges, cudaStream_t s);
 
 // ---- composite_fwd.cu
-// returns cudaSuccess or the launch error
+// returns cudaSuccess or the launch error.  TF (float or __half) is the element type of features and out_feature: the
+// float16 map is bitwise the float32 map of the exactly upcast features rounded to nearest even
+template <typename TF>
 cudaError_t launch_composite_fwd(const ViewParams& vp, const uint2* ranges, const uint32_t* point_list,
-                                 const SplatRec* rec, const float* features, const float* bg,
+                                 const SplatRec* rec, const TF* features, const float* bg,
                                  float* final_T, uint32_t* n_contrib, float* out_color,
-                                 float* out_feature, float* out_depth, int* work_counter, cudaStream_t s);
+                                 TF* out_feature, float* out_depth, int* work_counter, cudaStream_t s);
 
 // ---- composite_bwd.cu: geometric-gradient kernel of the two-kernel backward, two CTAs per SM; with list pointers it
 // also emits the per-(tile, block) blend weights for launch_feature_bwd

@@ -9,8 +9,10 @@
 //   mark_visible(means3D, viewmatrix, projmatrix) -> bool[P]
 // Differences (all permissive): the feature width is read from semantic_feature.size(-1) at run
 // time (reference: compile-time NUM_SEMANTIC_CHANNELS, config.h:16); an empty / undefined
-// semantic_feature means C = 0; inputs are checked for device/dtype and errors from the C ABI
-// are raised as RuntimeError.  This file contains no CUDA code and there is no CPU fallback.
+// semantic_feature means C = 0; semantic_feature may be float32 or float16, and the feature map
+// has its dtype (f3dgs_forward / f3dgs_forward_f16); inputs are checked for device/dtype and errors
+// from the C ABI are raised as RuntimeError.  This file contains no CUDA code and there is no CPU
+// fallback.
 #include <c10/cuda/CUDAGuard.h>
 #include <c10/cuda/CUDAStream.h>
 #include <torch/extension.h>
@@ -52,6 +54,15 @@ float* in_place(const torch::Tensor& t, const torch::Device& dev, int64_t numel,
                 name, " must be a contiguous float32 tensor of ", numel, " elements on ", dev, " (got ", t.numel(),
                 " elements of ", t.scalar_type(), " on ", t.device(), ")");
     return t.data_ptr<float>();
+}
+
+// semantic_feature of the rasterizer calls: float32 or float16 on `dev` (the feature map takes its dtype); undefined or
+// empty is absent, as for input()
+void check_features(const torch::Tensor& t, const torch::Device& dev) {
+    if (!t.defined() || t.numel() == 0) return;
+    TORCH_CHECK(t.scalar_type() == torch::kFloat32 || t.scalar_type() == torch::kFloat16,
+                "semantic_feature must be float32 or float16 (got ", t.scalar_type(), ")");
+    TORCH_CHECK(t.device() == dev, "semantic_feature must be on ", dev, " (got ", t.device(), ")");
 }
 
 void check_rc(int rc, const char* what) {
@@ -99,11 +110,13 @@ RasterizeGaussiansCUDA(const torch::Tensor& background, const torch::Tensor& mea
                 "semantic_feature must be [P, 1, C]");
 
     auto float_opts = means3D.options().dtype(torch::kFloat32);
+    const bool half = semantic_feature.defined() && semantic_feature.scalar_type() == torch::kFloat16;
+    auto feat_opts = means3D.options().dtype(half ? torch::kFloat16 : torch::kFloat32);
     // every element of the outputs is written by the composite kernel, so no zero-fill pass
     // (reference: torch::full 0, rasterize_points.cu:67-73); P == 0 keeps the reference's zeros
     torch::Tensor out_color = P ? torch::empty({3, H, W}, float_opts) : torch::zeros({3, H, W}, float_opts);
     torch::Tensor out_depth = P ? torch::empty({1, H, W}, float_opts) : torch::zeros({1, H, W}, float_opts);
-    torch::Tensor out_feature = P ? torch::empty({C, H, W}, float_opts) : torch::zeros({C, H, W}, float_opts);
+    torch::Tensor out_feature = P ? torch::empty({C, H, W}, feat_opts) : torch::zeros({C, H, W}, feat_opts);
     torch::Tensor radii = torch::empty({P}, means3D.options().dtype(torch::kInt32));
 
     auto byte_opts = torch::TensorOptions().dtype(torch::kByte).device(dev);
@@ -115,20 +128,27 @@ RasterizeGaussiansCUDA(const torch::Tensor& background, const torch::Tensor& mea
     if (P != 0) {
         int M = 0;
         if (sh.defined() && sh.numel() != 0) M = sh.size(1);
+        check_features(semantic_feature, dev);
         auto bg = input(background, dev, "bg"), m3 = input(means3D, dev, "means3D");
-        auto col = input(colors, dev, "colors_precomp"), sf = input(semantic_feature, dev, "semantic_feature");
+        auto col = input(colors, dev, "colors_precomp");
+        const bool has_sf = semantic_feature.defined() && semantic_feature.numel();
+        auto sf = has_sf ? semantic_feature.contiguous() : semantic_feature;
         auto op = input(opacity, dev, "opacities"), sc = input(scales, dev, "scales");
         auto rot = input(rotations, dev, "rotations"), cov = input(cov3D_precomp, dev, "cov3D_precomp");
         auto vm = input(viewmatrix, dev, "viewmatrix"), pm = input(projmatrix, dev, "projmatrix");
         auto shc = input(sh, dev, "shs"), cp = input(campos, dev, "campos");
         cudaStream_t stream = c10::cuda::getCurrentCUDAStream().stream();
-        rendered = f3dgs_forward(resize_tensor, &geomBuffer, resize_tensor, &binningBuffer, resize_tensor, &imgBuffer,
-                                 P, degree, M, C, fptr(bg), W, H, fptr(m3), fptr(shc), fptr(col), fptr(sf), fptr(op),
-                                 fptr(sc), scale_modifier, fptr(rot), fptr(cov), fptr(vm), fptr(pm), fptr(cp),
-                                 tan_fovx, tan_fovy, prefiltered ? 1 : 0, out_color.data_ptr<float>(),
-                                 C ? out_feature.data_ptr<float>() : nullptr, out_depth.data_ptr<float>(),
-                                 radii.data_ptr<int>(), debug ? 1 : 0, (void*)stream);
-        check_rc(rendered, "f3dgs_forward");
+        call_f32_or_f16(sf, f3dgs_forward, "f3dgs_forward", f3dgs_forward_f16, "f3dgs_forward_f16",
+                        [&](auto fn, auto sp) {  // sp: float* or uint16_t*, and the feature map is of the same type
+                            auto* fm = C ? static_cast<decltype(sp)>(out_feature.data_ptr()) : nullptr;
+                            return rendered = fn(resize_tensor, &geomBuffer, resize_tensor, &binningBuffer,
+                                                 resize_tensor, &imgBuffer, P, degree, M, C, fptr(bg), W, H, fptr(m3),
+                                                 fptr(shc), fptr(col), sp, fptr(op), fptr(sc), scale_modifier,
+                                                 fptr(rot), fptr(cov), fptr(vm), fptr(pm), fptr(cp), tan_fovx,
+                                                 tan_fovy, prefiltered ? 1 : 0, out_color.data_ptr<float>(), fm,
+                                                 out_depth.data_ptr<float>(), radii.data_ptr<int>(), debug ? 1 : 0,
+                                                 (void*)stream);
+                        });
     }
     return std::make_tuple(rendered, out_color, out_feature, out_depth, radii, geomBuffer, binningBuffer, imgBuffer);
 }
@@ -171,8 +191,11 @@ RasterizeGaussiansBackwardCUDA(const torch::Tensor& background, const torch::Ten
     torch::Tensor dL_dz = torch::zeros({P, 1}, o);
 
     if (P != 0) {
+        // only semantic_feature's shape is used: dL/dfeature depends on the blend weights alone (f3dgs_backward does
+        // not read the features), so a float16 one needs no float32 copy
+        check_features(semantic_feature, dev);
         auto bg = input(background, dev, "bg"), m3 = input(means3D, dev, "means3D");
-        auto col = input(colors, dev, "colors_precomp"), sf = input(semantic_feature, dev, "semantic_feature");
+        auto col = input(colors, dev, "colors_precomp");
         auto sc = input(scales, dev, "scales"), rot = input(rotations, dev, "rotations");
         auto cov = input(cov3D_precomp, dev, "cov3D_precomp");
         auto vm = input(viewmatrix, dev, "viewmatrix"), pm = input(projmatrix, dev, "projmatrix");
@@ -185,7 +208,7 @@ RasterizeGaussiansBackwardCUDA(const torch::Tensor& background, const torch::Ten
         auto gb = geomBuffer.contiguous(), bb = binningBuffer.contiguous(), ib = imageBuffer.contiguous();
         cudaStream_t stream = c10::cuda::getCurrentCUDAStream().stream();
         int rc = f3dgs_backward(
-            P, degree, M, R, C, fptr(bg), W, H, fptr(m3), fptr(shc), fptr(col), fptr(sf), fptr(sc), scale_modifier,
+            P, degree, M, R, C, fptr(bg), W, H, fptr(m3), fptr(shc), fptr(col), nullptr, fptr(sc), scale_modifier,
             fptr(rot), fptr(cov), fptr(vm), fptr(pm), fptr(cp), tan_fovx, tan_fovy, rad.data_ptr<int>(),
             reinterpret_cast<char*>(gb.data_ptr()), reinterpret_cast<char*>(bb.data_ptr()),
             reinterpret_cast<char*>(ib.data_ptr()), fptr(gc), C ? fptr(gf) : nullptr, fptr(gd),

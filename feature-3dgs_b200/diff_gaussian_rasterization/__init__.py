@@ -16,6 +16,11 @@ returns `(color[3,H,W], feature_map[C,H,W], radii[P] int32, depth[1,H,W])`.
 Behavioural notes
   * feature width C is taken from `semantic_feature.shape[-1]` at run time (the reference needs a
     rebuild per width, config.h:16); `semantic_feature=None` renders RGB + depth only (C = 0).
+  * the feature map has the dtype of `semantic_feature`: float32 or float16 (the reference is float32 only).  A float16
+    map is bitwise the float32 map of `semantic_feature.float()` rounded by `.half()`, without a float32 map ever
+    being made; colour, depth and radii are bitwise the float32 render's.  The backward stays float32: a float16 map's
+    gradient is upcast exactly and dL/dsemantic_feature is returned in `semantic_feature`'s dtype.  Float16 is for
+    rendering a trained field (render.py); GaussianState / ViewBatch training is float32.
   * `debug=True` keeps the reference semantics: arguments are snapshotted to CPU first and dumped
     to snapshot_fw.dump / snapshot_bw.dump if the native call raises (reference :89-97,:147-155);
     natively it synchronises and checks after every stage.
@@ -109,6 +114,8 @@ class _RasterizeGaussians(torch.autograd.Function):
         if grad_out_feature is None:
             C = semantic_feature.shape[-1] if semantic_feature.numel() else 0
             grad_out_feature = torch.zeros(C, rs.image_height, rs.image_width, device=means3D.device)
+        elif grad_out_feature.dtype == torch.float16:
+            grad_out_feature = grad_out_feature.float()  # exact; the native backward is float32
         args = (rs.bg, means3D, radii, colors_precomp, semantic_feature, scales, rotations, rs.scale_modifier,
                 cov3Ds_precomp, rs.viewmatrix, rs.projmatrix, rs.tanfovx, rs.tanfovy, grad_out_color,
                 grad_out_feature, grad_depth, sh, rs.sh_degree, rs.campos, geomBuffer, ctx.num_rendered,
@@ -118,6 +125,8 @@ class _RasterizeGaussians(torch.autograd.Function):
             _C.rasterize_gaussians_backward, args, rs.debug, "snapshot_bw.dump", "backward")
         if not ctx.needs_input_grad[4]:
             grad_semantic_feature = None
+        else:
+            grad_semantic_feature = grad_semantic_feature.to(semantic_feature.dtype)
         return (grad_means3D, grad_means2D, grad_sh, grad_colors_precomp, grad_semantic_feature, grad_opacities,
                 grad_scales, grad_rotations, grad_cov3Ds_precomp, None)
 

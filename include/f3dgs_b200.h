@@ -78,6 +78,24 @@ int f3dgs_forward(f3dgs_alloc_fn geometry_alloc, void* geometry_ctx,
                   float tan_fovx, float tan_fovy, int prefiltered,
                   float* out_color, float* out_feature_map, float* out_depth, int* radii,
                   int debug, void* cuda_stream);
+/* f3dgs_forward with float16 features (rendering a trained field): semantic_feature [P,C] and out_feature_map [C,H,W]
+ * hold IEEE binary16 bits; every other argument is as above.  The feature map is bitwise that of f3dgs_forward for the
+ * exactly upcast features, rounded once to nearest even (torch's .half()); colour, depth, radii, num_rendered and the
+ * three buffers are bitwise those of f3dgs_forward, so f3dgs_backward takes them as they are (it does not read the
+ * features).  Validates as f3dgs_forward. */
+int f3dgs_forward_f16(f3dgs_alloc_fn geometry_alloc, void* geometry_ctx,
+                      f3dgs_alloc_fn binning_alloc, void* binning_ctx,
+                      f3dgs_alloc_fn image_alloc, void* image_ctx,
+                      int P, int D, int M, int C,
+                      const float* background, int width, int height,
+                      const float* means3D, const float* shs, const float* colors_precomp,
+                      const uint16_t* semantic_feature, const float* opacities,
+                      const float* scales, float scale_modifier, const float* rotations,
+                      const float* cov3D_precomp,
+                      const float* viewmatrix, const float* projmatrix, const float* cam_pos,
+                      float tan_fovx, float tan_fovy, int prefiltered,
+                      float* out_color, uint16_t* out_feature_map, float* out_depth, int* radii,
+                      int debug, void* cuda_stream);
 
 /* ---- backward: reference Rasterizer::backward, rasterizer_impl.cu:347-461 -----------------
  * R is the num_rendered returned by the matching forward; the three buffers are the ones the
