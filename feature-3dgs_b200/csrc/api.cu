@@ -417,17 +417,20 @@ struct ScratchLayout {  // per-view intermediates of the accumulating backward (
     }
 };
 
-// Shared body of f3dgs_backward (accumulate = false: the reference's assign-into-zeroed-buffers contract) and
-// f3dgs_backward_accum (accumulate = true: += into the caller's per-parameter gradient buffers).
+// Shared body of f3dgs_backward (accumulate = false: the reference's assign-into-zeroed-buffers contract),
+// f3dgs_backward_accum (accumulate = true: += into the caller's per-parameter gradient buffers) and their _f16 twins.
+// TG (float or __half) is the element type of dL_dfeaturepix; a __half map stands for dL/dO = scale * float(h).
+// `zero` (accumulate only): the caller's scratch, zeroed once the arguments are validated.
+template <typename TG>
 int backward_impl(const Api& api, bool accumulate, int P, int D, int M, int R, int C, const float* background, int width,
                   int height, const float* means3D, const float* shs, const float* scales, float scale_modifier,
                   const float* rotations, const float* cov3D_precomp, const float* viewmatrix, const float* projmatrix,
                   const float* cam_pos, float tan_fovx, float tan_fovy, const int* radii, char* geom_buffer,
-                  char* binning_buffer, char* image_buffer, const float* dL_dpix, const float* dL_dfeaturepix,
-                  const float* dL_depths, float* dL_dmean2D, float* dL_dconic, float* dL_dopacity, float* dL_dcolor,
-                  float* dL_dsemantic_feature, float* dL_dmean3D, float* dL_dcov3D, float* dL_dsh, float* dL_dscale,
-                  float* dL_drot, float* dL_dz, float* grad_accum, float* denom, cudaEvent_t composite_done, int debug,
-                  cudaStream_t stream) {
+                  char* binning_buffer, char* image_buffer, const float* dL_dpix, const TG* dL_dfeaturepix,
+                  float dL_dfeaturepix_scale, const float* dL_depths, float* dL_dmean2D, float* dL_dconic,
+                  float* dL_dopacity, float* dL_dcolor, float* dL_dsemantic_feature, float* dL_dmean3D, float* dL_dcov3D,
+                  float* dL_dsh, float* dL_dscale, float* dL_drot, float* dL_dz, float* grad_accum, float* denom,
+                  cudaEvent_t composite_done, int debug, cudaStream_t stream, const Range& zero = {nullptr, 0}) {
     if (P < 0 || width <= 0 || height <= 0 || C < 0 || C > F3DGS_MAX_FEATURE_DIM || R < 0)
         return api.invalid("bad sizes");
     if (P == 0) return 0;
@@ -439,6 +442,14 @@ int backward_impl(const Api& api, bool accumulate, int P, int D, int M, int R, i
     if (scales && (!rotations || !dL_dscale || !dL_drot))
         return api.invalid("scales given but rotations/dL_dscale/dL_drot NULL");
     if ((grad_accum == nullptr) != (denom == nullptr)) return api.invalid("grad_accum and denom go together");
+    if constexpr (std::is_same_v<TG, __half>) {
+        if (!std::isfinite(dL_dfeaturepix_scale) || dL_dfeaturepix_scale == 0.f)
+            return api.invalid("dL_dfeaturepix_scale must be finite and nonzero");
+        // the feature kernel reduces into dL_dsemantic_feature while other warps still read the map
+        if (overlaps({dL_dsemantic_feature, (size_t)P * C * 4}, {{dL_dfeaturepix, (size_t)C * width * height * 2}}))
+            return api.invalid("dL_dsemantic_feature overlaps dL_dfeaturepix");
+    }
+    if (zero.p) CUDA_TRY(cudaMemsetAsync(const_cast<void*>(zero.p), 0, zero.bytes, stream));
 
     const ViewParams vp = make_view(P, D, M, C, width, height, tan_fovx, tan_fovy, scale_modifier, viewmatrix,
                                     projmatrix, cam_pos);
@@ -492,7 +503,7 @@ int backward_impl(const Api& api, bool accumulate, int P, int D, int M, int R, i
             e = launch_feature_bwd(vp, ranges, reinterpret_cast<const float*>(lists + ll.w),
                                    reinterpret_cast<const uint2*>(lists + ll.meta),
                                    reinterpret_cast<const uint32_t*>(lists + ll.cnt), dL_dfeaturepix,
-                                   dL_dsemantic_feature, counters + 48, stream);
+                                   dL_dfeaturepix_scale, dL_dsemantic_feature, counters + 48, stream);
         if (lists) cudaFreeAsync(lists, stream);
     }
     if (const int rc = api.cuda(e, "composite_bwd launch")) return rc;
@@ -526,12 +537,75 @@ int f3dgs_backward(int P, int D, int M, int R, int C, const float* background, i
     (void)colors_precomp;    // colours were copied into the per-Gaussian records by the forward
     return backward_impl(Api(__func__), false, P, D, M, R, C, background, width, height, means3D, shs, scales,
                          scale_modifier, rotations, cov3D_precomp, viewmatrix, projmatrix, cam_pos, tan_fovx, tan_fovy,
-                         radii, geom_buffer, binning_buffer, image_buffer, dL_dpix, dL_dfeaturepix, dL_depths, dL_dmean2D,
+                         radii, geom_buffer, binning_buffer, image_buffer, dL_dpix, dL_dfeaturepix, 1.f, dL_depths,
+                         dL_dmean2D, dL_dconic, dL_dopacity, dL_dcolor, dL_dsemantic_feature, dL_dmean3D, dL_dcov3D, dL_dsh,
+                         dL_dscale, dL_drot, dL_dz, nullptr, nullptr, nullptr, debug, (cudaStream_t)cuda_stream);
+}
+
+int f3dgs_backward_f16(int P, int D, int M, int R, int C, const float* background, int width, int height,
+                       const float* means3D, const float* shs, const float* colors_precomp,
+                       const float* semantic_feature, const float* scales, float scale_modifier,
+                       const float* rotations, const float* cov3D_precomp, const float* viewmatrix,
+                       const float* projmatrix, const float* cam_pos, float tan_fovx, float tan_fovy,
+                       const int* radii, char* geom_buffer, char* binning_buffer, char* image_buffer,
+                       const float* dL_dpix, const uint16_t* dL_dfeaturepix, float dL_dfeaturepix_scale,
+                       const float* dL_depths, float* dL_dmean2D, float* dL_dconic, float* dL_dopacity,
+                       float* dL_dcolor, float* dL_dsemantic_feature, float* dL_dmean3D, float* dL_dcov3D,
+                       float* dL_dsh, float* dL_dscale, float* dL_drot, float* dL_dz, int debug, void* cuda_stream) {
+    (void)semantic_feature;
+    (void)colors_precomp;
+    return backward_impl(Api(__func__), false, P, D, M, R, C, background, width, height, means3D, shs, scales,
+                         scale_modifier, rotations, cov3D_precomp, viewmatrix, projmatrix, cam_pos, tan_fovx, tan_fovy,
+                         radii, geom_buffer, binning_buffer, image_buffer, dL_dpix,
+                         reinterpret_cast<const __half*>(dL_dfeaturepix), dL_dfeaturepix_scale, dL_depths, dL_dmean2D,
                          dL_dconic, dL_dopacity, dL_dcolor, dL_dsemantic_feature, dL_dmean3D, dL_dcov3D, dL_dsh, dL_dscale,
                          dL_drot, dL_dz, nullptr, nullptr, nullptr, debug, (cudaStream_t)cuda_stream);
 }
 
 size_t f3dgs_backward_scratch_bytes(int P) { return P > 0 ? ScratchLayout((size_t)P).bytes : 0; }
+
+}  // extern "C"
+
+namespace {
+// Shared body of f3dgs_backward_accum and f3dgs_backward_accum_f16 (TG as in backward_impl)
+template <typename TG>
+int backward_accum_impl(const char* entry, int P, int D, int M, int R, int C, const float* background, int width,
+                        int height, const float* means3D, const float* shs, const float* colors_precomp,
+                        const float* scales, float scale_modifier, const float* rotations, const float* cov3D_precomp,
+                        const float* viewmatrix, const float* projmatrix, const float* cam_pos, float tan_fovx,
+                        float tan_fovy, const int* radii, char* geom_buffer, char* binning_buffer, char* image_buffer,
+                        const float* dL_dpix, const TG* dL_dfeaturepix, float dL_dfeaturepix_scale,
+                        const float* dL_depths, char* scratch, float* dL_dopacity, float* dL_dcolors_precomp,
+                        float* dL_dsemantic_feature, float* dL_dmean3D, float* dL_dcov3D_precomp, float* dL_dsh,
+                        float* dL_dscale, float* dL_drot, float* dL_dmean2D_out, float* grad_accum, float* denom,
+                        void* composite_done_event, int debug, void* cuda_stream) {
+    const Api api(entry);
+    cudaStream_t stream = (cudaStream_t)cuda_stream;
+    if (P <= 0) return P == 0 ? 0 : api.invalid("bad sizes");
+    if (!scratch) return api.invalid("NULL scratch");
+    if ((colors_precomp != nullptr) != (dL_dcolors_precomp != nullptr) ||
+        (cov3D_precomp != nullptr) != (dL_dcov3D_precomp != nullptr))
+        return api.invalid("dL_dcolors_precomp / dL_dcov3D_precomp go with colors_precomp / cov3D_precomp");
+    const ScratchLayout sl((size_t)P);
+    float* m2d = reinterpret_cast<float*>(scratch + sl.mean2D);
+    // colours / cov3D are intermediates unless they are inputs of the caller (then their gradients accumulate)
+    float* dcol = dL_dcolors_precomp ? dL_dcolors_precomp : reinterpret_cast<float*>(scratch + sl.color);
+    float* dcov = dL_dcov3D_precomp ? dL_dcov3D_precomp : reinterpret_cast<float*>(scratch + sl.cov3D);
+    const int rc = backward_impl(
+        api, true, P, D, M, R, C, background, width, height, means3D, shs, scales, scale_modifier,
+        rotations, cov3D_precomp, viewmatrix, projmatrix, cam_pos, tan_fovx, tan_fovy, radii, geom_buffer,
+        binning_buffer, image_buffer, dL_dpix, dL_dfeaturepix, dL_dfeaturepix_scale, dL_depths, m2d,
+        reinterpret_cast<float*>(scratch + sl.conic), dL_dopacity, dcol, dL_dsemantic_feature, dL_dmean3D, dcov, dL_dsh,
+        dL_dscale, dL_drot, reinterpret_cast<float*>(scratch + sl.dz), grad_accum, denom,
+        (cudaEvent_t)composite_done_event, debug, stream, {scratch, sl.bytes});
+    if (rc < 0) return rc;
+    if (dL_dmean2D_out)
+        CUDA_TRY(cudaMemcpyAsync(dL_dmean2D_out, m2d, (size_t)P * 3 * sizeof(float), cudaMemcpyDeviceToDevice, stream));
+    return 0;
+}
+}  // namespace
+
+extern "C" {
 
 int f3dgs_backward_accum(int P, int D, int M, int R, int C, const float* background, int width, int height,
                          const float* means3D, const float* shs, const float* colors_precomp, const float* scales,
@@ -543,30 +617,32 @@ int f3dgs_backward_accum(int P, int D, int M, int R, int C, const float* backgro
                          float* dL_dcov3D_precomp, float* dL_dsh, float* dL_dscale, float* dL_drot,
                          float* dL_dmean2D_out, float* grad_accum, float* denom, void* composite_done_event, int debug,
                          void* cuda_stream) {
-    const Api api(__func__);
-    cudaStream_t stream = (cudaStream_t)cuda_stream;
-    if (P <= 0) return P == 0 ? 0 : api.invalid("bad sizes");
-    if (!scratch) return api.invalid("NULL scratch");
-    if ((colors_precomp != nullptr) != (dL_dcolors_precomp != nullptr) ||
-        (cov3D_precomp != nullptr) != (dL_dcov3D_precomp != nullptr))
-        return api.invalid("dL_dcolors_precomp / dL_dcov3D_precomp go with colors_precomp / cov3D_precomp");
-    const ScratchLayout sl((size_t)P);
-    CUDA_TRY(cudaMemsetAsync(scratch, 0, sl.bytes, stream));
-    float* m2d = reinterpret_cast<float*>(scratch + sl.mean2D);
-    // colours / cov3D are intermediates unless they are inputs of the caller (then their gradients accumulate)
-    float* dcol = dL_dcolors_precomp ? dL_dcolors_precomp : reinterpret_cast<float*>(scratch + sl.color);
-    float* dcov = dL_dcov3D_precomp ? dL_dcov3D_precomp : reinterpret_cast<float*>(scratch + sl.cov3D);
-    const int rc = backward_impl(
-        api, true, P, D, M, R, C, background, width, height, means3D, shs, scales, scale_modifier,
-        rotations, cov3D_precomp, viewmatrix, projmatrix, cam_pos, tan_fovx, tan_fovy, radii, geom_buffer,
-        binning_buffer, image_buffer, dL_dpix, dL_dfeaturepix, dL_depths, m2d,
-        reinterpret_cast<float*>(scratch + sl.conic), dL_dopacity, dcol, dL_dsemantic_feature, dL_dmean3D, dcov, dL_dsh,
-        dL_dscale, dL_drot, reinterpret_cast<float*>(scratch + sl.dz), grad_accum, denom,
-        (cudaEvent_t)composite_done_event, debug, stream);
-    if (rc < 0) return rc;
-    if (dL_dmean2D_out)
-        CUDA_TRY(cudaMemcpyAsync(dL_dmean2D_out, m2d, (size_t)P * 3 * sizeof(float), cudaMemcpyDeviceToDevice, stream));
-    return 0;
+    return backward_accum_impl(__func__, P, D, M, R, C, background, width, height, means3D, shs, colors_precomp, scales,
+                               scale_modifier, rotations, cov3D_precomp, viewmatrix, projmatrix, cam_pos, tan_fovx,
+                               tan_fovy, radii, geom_buffer, binning_buffer, image_buffer, dL_dpix, dL_dfeaturepix, 1.f,
+                               dL_depths, scratch, dL_dopacity, dL_dcolors_precomp, dL_dsemantic_feature, dL_dmean3D,
+                               dL_dcov3D_precomp, dL_dsh, dL_dscale, dL_drot, dL_dmean2D_out, grad_accum, denom,
+                               composite_done_event, debug, cuda_stream);
+}
+
+int f3dgs_backward_accum_f16(int P, int D, int M, int R, int C, const float* background, int width, int height,
+                             const float* means3D, const float* shs, const float* colors_precomp, const float* scales,
+                             float scale_modifier, const float* rotations, const float* cov3D_precomp,
+                             const float* viewmatrix, const float* projmatrix, const float* cam_pos, float tan_fovx,
+                             float tan_fovy, const int* radii, char* geom_buffer, char* binning_buffer,
+                             char* image_buffer, const float* dL_dpix, const uint16_t* dL_dfeaturepix,
+                             float dL_dfeaturepix_scale, const float* dL_depths, char* scratch, float* dL_dopacity,
+                             float* dL_dcolors_precomp, float* dL_dsemantic_feature, float* dL_dmean3D,
+                             float* dL_dcov3D_precomp, float* dL_dsh, float* dL_dscale, float* dL_drot,
+                             float* dL_dmean2D_out, float* grad_accum, float* denom, void* composite_done_event,
+                             int debug, void* cuda_stream) {
+    return backward_accum_impl(__func__, P, D, M, R, C, background, width, height, means3D, shs, colors_precomp, scales,
+                               scale_modifier, rotations, cov3D_precomp, viewmatrix, projmatrix, cam_pos, tan_fovx,
+                               tan_fovy, radii, geom_buffer, binning_buffer, image_buffer, dL_dpix,
+                               reinterpret_cast<const __half*>(dL_dfeaturepix), dL_dfeaturepix_scale, dL_depths, scratch,
+                               dL_dopacity, dL_dcolors_precomp, dL_dsemantic_feature, dL_dmean3D, dL_dcov3D_precomp,
+                               dL_dsh, dL_dscale, dL_drot, dL_dmean2D_out, grad_accum, denom, composite_done_event, debug,
+                               cuda_stream);
 }
 
 }  // extern "C"
@@ -574,18 +650,19 @@ int f3dgs_backward_accum(int P, int D, int M, int R, int C, const float* backgro
 namespace {
 // The float16 entry points (_f16gt, _f16, _f16x) validate and launch as their float32 twins do.  Half data is IEEE
 // binary16 bits at the ABI (uint16_t) and __half in the kernels.
-template <typename GT>
-int feature_resize_fwd_impl(const char* entry, int C, int H, int W, int Hg, int Wg, const float* feature_map,
+template <typename FM, typename GT>
+int feature_resize_fwd_impl(const char* entry, int C, int H, int W, int Hg, int Wg, const FM* feature_map,
                             const GT* gt, float grad_scale, float* out, float* loss_sum, void* cuda_stream) {
     const Api api(entry);
     if (C < 0 || H <= 0 || W <= 0 || Hg <= 0 || Wg <= 0) return api.invalid("bad sizes");
     if (C == 0) return 0;
     if (!feature_map || !out) return api.invalid("NULL pointer");
-    if constexpr (std::is_same_v<GT, __half>) {
-        // no target is the float32 symbol's job; out's 4-byte elements cannot alias gt's 2-byte ones element for element
-        if (!gt) return api.invalid("NULL pointer (gt is required)");
+    if constexpr (std::is_same_v<GT, __half> || std::is_same_v<FM, __half>) {
+        // a float16 target is required (no target is the _f16 symbol's job for a float16 map, the float32 one's
+        // otherwise); out's 4-byte elements cannot alias 2-byte ones element for element
+        if (std::is_same_v<GT, __half> && !gt) return api.invalid("NULL pointer (gt is required)");
         const size_t n = (size_t)C * Hg * Wg;
-        if (overlaps({out, n * 4}, {{feature_map, (size_t)C * H * W * 4}, {gt, n * 2}}))
+        if (overlaps({out, n * 4}, {{feature_map, (size_t)C * H * W * sizeof(FM)}, {gt, n * sizeof(GT)}}))
             return api.invalid("out overlaps feature_map or gt");
     }
     return api.cuda(launch_feature_resize_fwd(C, H, W, Hg, Wg, feature_map, gt, grad_scale, out, loss_sum,
@@ -606,13 +683,41 @@ int f3dgs_feature_resize_fwd_f16gt(int C, int H, int W, int Hg, int Wg, const fl
                                    grad_scale, out, loss_sum, cuda_stream);
 }
 
+int f3dgs_feature_resize_fwd_f16(int C, int H, int W, int Hg, int Wg, const uint16_t* feature_map, const float* gt,
+                                 float grad_scale, float* out, float* loss_sum, void* cuda_stream) {
+    return feature_resize_fwd_impl(__func__, C, H, W, Hg, Wg, reinterpret_cast<const __half*>(feature_map), gt,
+                                   grad_scale, out, loss_sum, cuda_stream);
+}
+
+int f3dgs_feature_resize_fwd_f16_f16gt(int C, int H, int W, int Hg, int Wg, const uint16_t* feature_map,
+                                       const uint16_t* gt, float grad_scale, float* out, float* loss_sum,
+                                       void* cuda_stream) {
+    return feature_resize_fwd_impl(__func__, C, H, W, Hg, Wg, reinterpret_cast<const __half*>(feature_map),
+                                   reinterpret_cast<const __half*>(gt), grad_scale, out, loss_sum, cuda_stream);
+}
+
 int f3dgs_feature_resize_bwd(int C, int H, int W, int Hg, int Wg, const float* dout, float* dL_dfeature_map,
                              void* cuda_stream) {
     const Api api(__func__);
     if (C < 0 || H <= 0 || W <= 0 || Hg <= 0 || Wg <= 0) return api.invalid("bad sizes");
     if (C == 0) return 0;
     if (!dout || !dL_dfeature_map) return api.invalid("NULL pointer");
-    return api.cuda(launch_feature_resize_bwd(C, H, W, Hg, Wg, dout, dL_dfeature_map, (cudaStream_t)cuda_stream));
+    return api.cuda(
+        launch_feature_resize_bwd(C, H, W, Hg, Wg, dout, dL_dfeature_map, 1.f, (cudaStream_t)cuda_stream));
+}
+
+int f3dgs_feature_resize_bwd_f16(int C, int H, int W, int Hg, int Wg, const float* dout, float out_scale,
+                                 uint16_t* dL_dfeature_map, void* cuda_stream) {
+    const Api api(__func__);
+    if (C < 0 || H <= 0 || W <= 0 || Hg <= 0 || Wg <= 0) return api.invalid("bad sizes");
+    if (C == 0) return 0;
+    if (!dout || !dL_dfeature_map) return api.invalid("NULL pointer");
+    if (!std::isfinite(out_scale) || out_scale == 0.f) return api.invalid("out_scale must be finite and nonzero");
+    // the gather reads dout around every element it writes
+    if (overlaps({dL_dfeature_map, (size_t)C * H * W * 2}, {{dout, (size_t)C * Hg * Wg * 4}}))
+        return api.invalid("dL_dfeature_map overlaps dout");
+    return api.cuda(launch_feature_resize_bwd(C, H, W, Hg, Wg, dout, reinterpret_cast<__half*>(dL_dfeature_map),
+                                              out_scale, (cudaStream_t)cuda_stream));
 }
 
 int f3dgs_image_loss(int planes, int H, int W, const float* image, const float* gt, float w_l1, float w_ssim, float* sums,
@@ -922,6 +1027,20 @@ int f3dgs_adam_step(int kind, size_t n, int M, float* param, const float* grad_a
     if (n == 0) return 0;
     return api.cuda(launch_adam_step(kind, n, M, param, grad_activated, exp_avg, exp_avg_sq, lr, beta1, beta2, eps, step,
                                      (cudaStream_t)cuda_stream));
+}
+
+int f3dgs_adam_step_f16out(int kind, size_t n, int M, float* param, const float* grad_activated, float* exp_avg,
+                           float* exp_avg_sq, uint16_t* param_f16, float lr, float beta1, float beta2, float eps,
+                           int step, void* cuda_stream) {
+    const Api api(__func__);
+    if (kind != F3DGS_PARAM_IDENTITY) return api.invalid("kind must be F3DGS_PARAM_IDENTITY");
+    if (step < 1) return api.invalid("step < 1");
+    if (!param || !grad_activated || !exp_avg || !exp_avg_sq || !param_f16) return api.invalid("NULL pointer");
+    if (overlaps({param_f16, n * 2}, {{param, n * 4}, {grad_activated, n * 4}, {exp_avg, n * 4}, {exp_avg_sq, n * 4}}))
+        return api.invalid("param_f16 overlaps param, grad_activated, exp_avg or exp_avg_sq");
+    if (n == 0) return 0;
+    return api.cuda(launch_adam_step(kind, n, M, param, grad_activated, exp_avg, exp_avg_sq, lr, beta1, beta2, eps, step,
+                                     (cudaStream_t)cuda_stream, reinterpret_cast<__half*>(param_f16)));
 }
 
 int f3dgs_mark_visible(int P, const float* means3D, const float* viewmatrix, const float* projmatrix,

@@ -12,6 +12,8 @@
 // dL/df[g] += sum_pixels w * dL/dO with paired FMAs (fma2_rn) over the 2x2-pixel quads that blended, one red.global.add.v4
 // per lane and entry.  No inter-warp synchronisation at all; 12 warps per SM.  Channel counts above 128 reuse the same
 // lists for every 128-channel chunk (the alpha evaluation is not repeated per chunk).
+// The upstream gradient may be a float16 map h with a float32 scale s (training float16 feature fields): it is upcast and
+// multiplied by s once, where the block's gradient is loaded, and everything after that is the float32 kernel.
 // Reference semantics: backward.cu:565-575 (feature gradient; the feature loss does not feed dL/dalpha, :575 disabled).
 #include <cstdio>
 #include <cstdlib>
@@ -36,7 +38,10 @@ struct FeatArgs {
     float* dL_dfeature;         // backward: [P, C]
     int* work_counter;
     int W, H, C, tiles_x, num_tiles, chunks;
-    int vec;  // bit0: gradient rows are 16-byte aligned and C % 4 == 0; bit1: 128-bit image rows
+    int vec;  // bit0: gradient rows are 16-byte aligned and C % 4 == 0; bit1: 4-pixel vector loads of image rows
+    // a float16 upstream gradient instead of dL_dfeat_pix: dL/dO = scale * float(map), one fp32 multiply rounded to nearest
+    const __half* dL_dfeat_pix_h;
+    float scale;
 };
 
 __device__ __forceinline__ void cp_async16(void* dst_smem, const void* src_gmem) {
@@ -65,8 +70,21 @@ __device__ __forceinline__ ItemPos decode_item(int item, const FeatArgs& a) {
     return p;
 }
 
+// Loads of the upstream gradient: 4 consecutive pixels (16 bytes of float / 8 bytes of __half, aligned) or one.  A __half
+// element is upcast exactly and multiplied by the map's float32 scale once, rounded to nearest.
+__device__ __forceinline__ float4 ld_dO4(const float* p, float) { return ld_nc_f4(p); }
+__device__ __forceinline__ float4 ld_dO4(const __half* p, float s) {
+    uint32_t u0, u1;
+    asm volatile("ld.global.nc.L1::no_allocate.v2.u32 {%0,%1}, [%2];" : "=r"(u0), "=r"(u1) : "l"(p));
+    const float2 a = __half22float2(*reinterpret_cast<const __half2*>(&u0));
+    const float2 b = __half22float2(*reinterpret_cast<const __half2*>(&u1));
+    return make_float4(__fmul_rn(a.x, s), __fmul_rn(a.y, s), __fmul_rn(b.x, s), __fmul_rn(b.y, s));
+}
+__device__ __forceinline__ float ld_dO1(const float* p, float) { return __ldg(p); }
+__device__ __forceinline__ float ld_dO1(const __half* p, float s) { return __fmul_rn(__half2float(__ldg(p)), s); }
+
 // ------------------------------------------------------------------------------------------------ backward
-template <int CH>
+template <int CH, typename TG>  // TG: element type of the upstream gradient map, float or __half
 __global__ void __launch_bounds__(kFeatWarps * 32, 3) feature_bwd_kernel(const FeatArgs a) {
     extern __shared__ __align__(128) unsigned char smem_raw[];
     const int warp = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0), lane = threadIdx.x & 31;
@@ -122,7 +140,11 @@ __global__ void __launch_bounds__(kFeatWarps * 32, 3) feature_bwd_kernel(const F
         for (int c = 0; c < 4; c++) {
             const int ch = ch0 + c;
             if (ch >= C) continue;
-            const float* plane = a.dL_dfeat_pix + (size_t)ch * HW;
+            const TG* plane;
+            if constexpr (std::is_same_v<TG, float>)
+                plane = a.dL_dfeat_pix + (size_t)ch * HW;
+            else
+                plane = a.dL_dfeat_pix_h + (size_t)ch * HW;
             if (G == 1 && (a.vec & 2)) {
 #pragma unroll
                 for (int y = 0; y < 4; y++) {
@@ -133,7 +155,7 @@ __global__ void __launch_bounds__(kFeatWarps * 32, 3) feature_bwd_kernel(const F
                         const int xx = ip.bx0 + half * 4;
                         if (xx >= W) continue;
                         const int qa = (y >> 1) * 4 + half * 2, i0 = (y & 1) * 2;
-                        const float4 v = ld_nc_f4(plane + (size_t)yy * W + xx);
+                        const float4 v = ld_dO4(plane + (size_t)yy * W + xx, a.scale);
                         DOB(qa % NQ, i0, c) = v.x;
                         DOB(qa % NQ, i0 + 1, c) = v.y;
                         DOB((qa + 1) % NQ, i0, c) = v.z;
@@ -147,7 +169,7 @@ __global__ void __launch_bounds__(kFeatWarps * 32, 3) feature_bwd_kernel(const F
 #pragma unroll
                     for (int i = 0; i < 4; i++) {
                         const int xx = ip.bx0 + (q & 3) * 2 + (i & 1), yy = ip.by0 + (q >> 2) * 2 + (i >> 1);
-                        if (xx < W && yy < H) DOB(qi, i, c) = __ldg(plane + (size_t)yy * W + xx);
+                        if (xx < W && yy < H) DOB(qi, i, c) = ld_dO1(plane + (size_t)yy * W + xx, a.scale);
                     }
                 }
             }
@@ -223,36 +245,46 @@ static int workers_grid() {
     return sms_of_device[dev].load() * 3;  // __launch_bounds__(128, 3): three CTAs of four workers per SM
 }
 
-template <int CH>
+template <int CH, typename TG>
 static cudaError_t launch_feat_bwd_t(const FeatArgs& a, cudaStream_t s) {
     const size_t smem = kFeatWarps * sizeof(FeatSmem);
     const int items = a.num_tiles * a.chunks * kBlocksPerTile;
     const int grid = min((items + kFeatWarps - 1) / kFeatWarps, workers_grid());
-    feature_bwd_kernel<CH><<<grid, kFeatWarps * 32, smem, s>>>(a);
+    feature_bwd_kernel<CH, TG><<<grid, kFeatWarps * 32, smem, s>>>(a);
     g_launches++;
     return cudaGetLastError();
 }
 
 static int feat_ch(int C) { return C <= 32 ? 32 : (C <= 64 ? 64 : 128); }
 
+template <typename TG>
 cudaError_t launch_feature_bwd(const ViewParams& vp, const uint2* ranges, const float* list_w, const uint2* list_meta,
-                               const uint32_t* list_cnt, const float* dL_dfeat_pix, float* dL_dfeature,
-                               int* work_counter, cudaStream_t s) {
+                               const uint32_t* list_cnt, const TG* dL_dfeat_pix, float dL_dfeat_pix_scale,
+                               float* dL_dfeature, int* work_counter, cudaStream_t s) {
     FeatArgs a;
     a.ranges = ranges; a.list_w = list_w; a.list_meta = list_meta; a.list_cnt = list_cnt;
-    a.dL_dfeat_pix = dL_dfeat_pix; a.dL_dfeature = dL_dfeature;
+    if constexpr (std::is_same_v<TG, float>) {
+        a.dL_dfeat_pix = dL_dfeat_pix; a.dL_dfeat_pix_h = nullptr;
+    } else {
+        a.dL_dfeat_pix = nullptr; a.dL_dfeat_pix_h = dL_dfeat_pix;
+    }
+    a.dL_dfeature = dL_dfeature; a.scale = dL_dfeat_pix_scale;
     a.work_counter = work_counter;
     a.W = vp.W; a.H = vp.H; a.C = vp.C; a.tiles_x = (int)vp.grid_x; a.num_tiles = (int)(vp.grid_x * vp.grid_y);
     const int CH = feat_ch(vp.C);
     a.chunks = (vp.C + CH - 1) / CH;
     a.vec = 0;
     if (vp.C % 4 == 0 && (reinterpret_cast<uintptr_t>(dL_dfeature) & 15) == 0) a.vec |= 1;
-    if (vp.W % 4 == 0 && (reinterpret_cast<uintptr_t>(dL_dfeat_pix) & 15) == 0) a.vec |= 2;
+    if (vp.W % 4 == 0 && (reinterpret_cast<uintptr_t>(dL_dfeat_pix) & (4 * sizeof(TG) - 1)) == 0) a.vec |= 2;
     cudaError_t e = cudaMemsetAsync(work_counter, 0, sizeof(int), s);
     if (e != cudaSuccess) return e;
-    if (CH == 32) return launch_feat_bwd_t<32>(a, s);
-    if (CH == 64) return launch_feat_bwd_t<64>(a, s);
-    return launch_feat_bwd_t<128>(a, s);
+    if (CH == 32) return launch_feat_bwd_t<32, TG>(a, s);
+    if (CH == 64) return launch_feat_bwd_t<64, TG>(a, s);
+    return launch_feat_bwd_t<128, TG>(a, s);
 }
+template cudaError_t launch_feature_bwd(const ViewParams&, const uint2*, const float*, const uint2*, const uint32_t*,
+                                       const float*, float, float*, int*, cudaStream_t);
+template cudaError_t launch_feature_bwd(const ViewParams&, const uint2*, const float*, const uint2*, const uint32_t*,
+                                       const __half*, float, float*, int*, cudaStream_t);
 
 }  // namespace f3dgs

@@ -14,14 +14,16 @@
 //                  footprint covers it -- every element written exactly once, no atomics, no zero fill.
 // Sampling positions follow ATen's upsample_bilinear2d with align_corners=True: src = dst * (in - 1) / (out - 1),
 // i0 = (int)src, i1 = i0 + (i0 < in - 1), lambda1 = src - i0.
-// The target may be float32 or float16 (the data format's teacher maps); a float16 element is upcast exactly at its load,
-// so the result equals that of the float32 target gt.float().
+// The target may be float32 or float16 (the data format's teacher maps), and so may the rendered map; a float16 element
+// is upcast exactly at its load, so the result equals that of the float32 inputs .float().  resize_bwd can also write a
+// float16 gradient, half_rn(out_scale * the float32 element), for training float16 feature fields.
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
 
 #include <algorithm>
 #include <cmath>
+#include <type_traits>
 
 #include "../../include/f3dgs_b200.h"
 #include "kernels.h"
@@ -49,8 +51,8 @@ __device__ __forceinline__ void src_of(int o, float r, int in, int& i0, int& i1,
 // (200 K same-address atomics cost more than the whole resize).
 constexpr int kFwdThreads = 256;
 
-template <typename GT>  // float or __half
-__global__ void __launch_bounds__(kFwdThreads) resize_fwd_kernel(ResizeGeom g, const float* __restrict__ fm,
+template <typename FM, typename GT>  // each float or __half
+__global__ void __launch_bounds__(kFwdThreads) resize_fwd_kernel(ResizeGeom g, const FM* __restrict__ fm,
                                                                  const GT* __restrict__ gt, float grad_scale,
                                                                  float* __restrict__ out, float* __restrict__ loss_sum) {
     const int lane = threadIdx.x & 31;
@@ -62,15 +64,24 @@ __global__ void __launch_bounds__(kFwdThreads) resize_fwd_kernel(ResizeGeom g, c
         int y0, y1;
         float ly0, ly1;
         src_of(oy, g.ry, g.H, y0, y1, ly0, ly1);
-        const float* p0 = fm + ((size_t)c * g.H + y0) * g.W;
-        const float* p1 = fm + ((size_t)c * g.H + y1) * g.W;
+        const FM* p0 = fm + ((size_t)c * g.H + y0) * g.W;
+        const FM* p1 = fm + ((size_t)c * g.H + y1) * g.W;
         const size_t obase = (size_t)row * g.Wg;
 #pragma unroll 2
         for (int ox = lane; ox < g.Wg; ox += 32) {
             int x0, x1;
             float lx0, lx1;
             src_of(ox, g.rx, g.W, x0, x1, lx0, lx1);
-            const float v = ly0 * (lx0 * __ldg(p0 + x0) + lx1 * __ldg(p0 + x1)) + ly1 * (lx0 * __ldg(p1 + x0) + lx1 * __ldg(p1 + x1));
+            float v;
+            if constexpr (std::is_same_v<FM, float>) {
+                v = ly0 * (lx0 * __ldg(p0 + x0) + lx1 * __ldg(p0 + x1)) + ly1 * (lx0 * __ldg(p1 + x0) + lx1 * __ldg(p1 + x1));
+            } else {
+                // the FMAs the compiler forms for the float map above, spelled out: the contraction is chosen per
+                // instantiation, and the float16 map must give bitwise the float32 result of its upcast
+                const float a = load_f32(p0 + x0), b = load_f32(p0 + x1), c = load_f32(p1 + x0), d = load_f32(p1 + x1);
+                const float r0 = __fmaf_rn(lx1, b, __fmul_rn(lx0, a)), r1 = __fmaf_rn(lx0, c, __fmul_rn(lx1, d));
+                v = __fmaf_rn(ly0, r0, __fmul_rn(ly1, r1));
+            }
             if (gt != nullptr) {
                 const float d = v - load_f32(gt + obase + ox);
                 ad += fabsf(d);
@@ -139,8 +150,15 @@ struct GatherTables {
 constexpr int kRowsPerBlock = 8;   // at least; more when C * H / 8 would exceed the 65535 limit of gridDim.y
 constexpr int kMaxKx = 6;   // x-table entries kept in registers; wider tables (strong up-sampling) take the generic loop
 
+// The gradient's element: the float32 sum itself, or half_rn(out_scale * sum) for a float16 gradient
+__device__ __forceinline__ float out_elem(float acc, float, float*) { return acc; }
+__device__ __forceinline__ __half out_elem(float acc, float out_scale, __half*) {
+    return __float2half_rn(__fmul_rn(out_scale, acc));
+}
+
+template <typename OUT>  // float or __half
 __global__ void __launch_bounds__(256) resize_bwd_kernel(ResizeGeom g, GatherTables t, const float* __restrict__ dout,
-                                                         float* __restrict__ dfm, int rows_per_block) {
+                                                         OUT* __restrict__ dfm, int rows_per_block, float out_scale) {
     const int x0 = (blockIdx.x * 256 + threadIdx.x) * 4;
     if (x0 >= g.W) return;
     const int rows = g.C * g.H;
@@ -186,13 +204,19 @@ __global__ void __launch_bounds__(256) resize_bwd_kernel(ResizeGeom g, GatherTab
                 acc[j] += wy * s;
             }
         }
-        float* o = dfm + (size_t)row * g.W + x0;
-        if (x0 + 3 < g.W && ((reinterpret_cast<uintptr_t>(o) & 15) == 0)) {
-            *reinterpret_cast<float4*>(o) = make_float4(acc[0], acc[1], acc[2], acc[3]);
+        OUT* o = dfm + (size_t)row * g.W + x0;
+        if (x0 + 3 < g.W && ((reinterpret_cast<uintptr_t>(o) & (4 * sizeof(OUT) - 1)) == 0)) {
+            if constexpr (std::is_same_v<OUT, float>) {
+                *reinterpret_cast<float4*>(o) = make_float4(acc[0], acc[1], acc[2], acc[3]);
+            } else {
+                __half2 h[2] = {__halves2half2(out_elem(acc[0], out_scale, o), out_elem(acc[1], out_scale, o)),
+                                __halves2half2(out_elem(acc[2], out_scale, o), out_elem(acc[3], out_scale, o))};
+                *reinterpret_cast<uint2*>(o) = *reinterpret_cast<const uint2*>(h);
+            }
         } else {
 #pragma unroll
             for (int j = 0; j < 4; j++)
-                if (x0 + j < g.W) o[j] = acc[j];
+                if (x0 + j < g.W) o[j] = out_elem(acc[j], out_scale, o);
         }
     }
 }
@@ -204,8 +228,9 @@ __global__ void __launch_bounds__(256) resize_bwd_kernel(ResizeGeom g, GatherTab
 // alignment is, and the four rows of a trip are independent loads in flight.
 constexpr int kOneMaxRows = 32;
 
+template <typename OUT>  // float or __half
 __global__ void __launch_bounds__(512) resize_bwd_one_kernel(ResizeGeom g, GatherTables t, const float* __restrict__ dout,
-                                                             float* __restrict__ dfm, int rows_per_block) {
+                                                             OUT* __restrict__ dfm, int rows_per_block, float out_scale) {
     __shared__ size_t s_off[kOneMaxRows];
     __shared__ float s_wy[kOneMaxRows];
     const int rows = g.C * g.H, row0 = blockIdx.y * rows_per_block, T = blockDim.x;
@@ -248,10 +273,10 @@ __global__ void __launch_bounds__(512) resize_bwd_one_kernel(ResizeGeom g, Gathe
 #pragma unroll
         for (int u = 0; u < 4; u++) {
             if (r + u >= nrow) break;
-            float* o = dfm + (size_t)(row0 + r + u) * g.W + (size_t)blockIdx.x * 4 * T + threadIdx.x;
+            OUT* o = dfm + (size_t)(row0 + r + u) * g.W + (size_t)blockIdx.x * 4 * T + threadIdx.x;
 #pragma unroll
             for (int j = 0; j < 4; j++)
-                if (in[j]) o[j * T] = v[u][j];
+                if (in[j]) o[j * T] = out_elem(v[u][j], out_scale, o);
         }
     }
 }
@@ -266,8 +291,8 @@ ResizeGeom make_geom(int C, int H, int W, int Hg, int Wg) {
 
 }  // namespace
 
-template <typename GT>
-cudaError_t launch_feature_resize_fwd(int C, int H, int W, int Hg, int Wg, const float* fm, const GT* gt, float grad_scale,
+template <typename FM, typename GT>
+cudaError_t launch_feature_resize_fwd(int C, int H, int W, int Hg, int Wg, const FM* fm, const GT* gt, float grad_scale,
                                       float* out, float* loss_sum, cudaStream_t s) {
     const size_t n = (size_t)C * Hg * Wg;
     if (n == 0) return cudaSuccess;
@@ -277,7 +302,7 @@ cudaError_t launch_feature_resize_fwd(int C, int H, int W, int Hg, int Wg, const
     const size_t rows = (size_t)C * Hg;
     if (rows > 0x7fffffffu) return cudaErrorInvalidValue;
     const unsigned grid = (unsigned)std::min<size_t>((rows + kFwdThreads / 32 - 1) / (kFwdThreads / 32), (size_t)sms * 8);
-    resize_fwd_kernel<GT><<<grid, kFwdThreads, 0, s>>>(make_geom(C, H, W, Hg, Wg), fm, gt, grad_scale, out, loss_sum);
+    resize_fwd_kernel<FM, GT><<<grid, kFwdThreads, 0, s>>>(make_geom(C, H, W, Hg, Wg), fm, gt, grad_scale, out, loss_sum);
     g_launches++;
     return cudaGetLastError();
 }
@@ -285,8 +310,14 @@ template cudaError_t launch_feature_resize_fwd(int, int, int, int, int, const fl
                                                cudaStream_t);
 template cudaError_t launch_feature_resize_fwd(int, int, int, int, int, const float*, const __half*, float, float*,
                                                float*, cudaStream_t);
+template cudaError_t launch_feature_resize_fwd(int, int, int, int, int, const __half*, const float*, float, float*,
+                                               float*, cudaStream_t);
+template cudaError_t launch_feature_resize_fwd(int, int, int, int, int, const __half*, const __half*, float, float*,
+                                               float*, cudaStream_t);
 
-cudaError_t launch_feature_resize_bwd(int C, int H, int W, int Hg, int Wg, const float* dout, float* dfm, cudaStream_t s) {
+template <typename OUT>
+cudaError_t launch_feature_resize_bwd(int C, int H, int W, int Hg, int Wg, const float* dout, OUT* dfm, float out_scale,
+                                      cudaStream_t s) {
     const size_t n = (size_t)C * H * W;
     if (n == 0) return cudaSuccess;
     const ResizeGeom g = make_geom(C, H, W, Hg, Wg);
@@ -310,15 +341,18 @@ cudaError_t launch_feature_resize_bwd(int C, int H, int W, int Hg, int Wg, const
     if (g.ry >= 2.001f && g.rx >= 2.001f && (rows + kOneMaxRows - 1) / kOneMaxRows <= 65535) {
         const int T = std::min(512, ((W + 3) / 4 + 31) / 32 * 32);
         const int rpb = std::max(16, std::min(kOneMaxRows, (rows + 65534) / 65535));
-        resize_bwd_one_kernel<<<dim3((W + 4 * T - 1) / (4 * T), (rows + rpb - 1) / rpb), T, 0, s>>>(g, t, dout, dfm, rpb);
+        resize_bwd_one_kernel<<<dim3((W + 4 * T - 1) / (4 * T), (rows + rpb - 1) / rpb), T, 0, s>>>(g, t, dout, dfm, rpb,
+                                                                                                     out_scale);
     } else {
         const int rpb = std::max(kRowsPerBlock, (rows + 65534) / 65535);
-        resize_bwd_kernel<<<dim3((W + 1023) / 1024, (rows + rpb - 1) / rpb), 256, 0, s>>>(g, t, dout, dfm, rpb);
+        resize_bwd_kernel<<<dim3((W + 1023) / 1024, (rows + rpb - 1) / rpb), 256, 0, s>>>(g, t, dout, dfm, rpb, out_scale);
     }
     g_launches += 3;
     e = cudaGetLastError();
     cudaFreeAsync(ws, s);
     return e;
 }
+template cudaError_t launch_feature_resize_bwd(int, int, int, int, int, const float*, float*, float, cudaStream_t);
+template cudaError_t launch_feature_resize_bwd(int, int, int, int, int, const float*, __half*, float, cudaStream_t);
 
 }  // namespace f3dgs

@@ -65,16 +65,22 @@ cudaError_t launch_composite_bwd_geom(const ViewParams& vp, const uint2* ranges,
                                       float* dL_dz, int* work_counter, cudaStream_t s, float* list_w = nullptr,
                                       uint2* list_meta = nullptr, uint32_t* list_cnt = nullptr);
 
-// ---- feature_bwd.cu: feature gradient from the instance lists (second kernel of the two-kernel backward)
+// ---- feature_bwd.cu: feature gradient from the instance lists (second kernel of the two-kernel backward).  TG (float or
+// __half) is the element type of the upstream gradient map; a __half map stands for dL/dO = scale * float(h) (the scale is
+// not read for a float map)
+template <typename TG>
 cudaError_t launch_feature_bwd(const ViewParams& vp, const uint2* ranges, const float* list_w, const uint2* list_meta,
-                               const uint32_t* list_cnt, const float* dL_dfeat_pix, float* dL_dfeature,
-                               int* work_counter, cudaStream_t s);
+                               const uint32_t* list_cnt, const TG* dL_dfeat_pix, float dL_dfeat_pix_scale,
+                               float* dL_dfeature, int* work_counter, cudaStream_t s);
 
-// ---- feature_head.cu (a float16 target gives the result of the float32 one upcast exactly)
-template <typename GT>
-cudaError_t launch_feature_resize_fwd(int C, int H, int W, int Hg, int Wg, const float* fm, const GT* gt, float grad_scale,
+// ---- feature_head.cu (a float16 map or target gives the result of the float32 one upcast exactly; a float16 gradient
+// is half_rn(out_scale * the float32 one), out_scale not read for a float gradient)
+template <typename FM, typename GT>
+cudaError_t launch_feature_resize_fwd(int C, int H, int W, int Hg, int Wg, const FM* fm, const GT* gt, float grad_scale,
                                       float* out, float* loss_sum, cudaStream_t s);
-cudaError_t launch_feature_resize_bwd(int C, int H, int W, int Hg, int Wg, const float* dout, float* dfm, cudaStream_t s);
+template <typename OUT>
+cudaError_t launch_feature_resize_bwd(int C, int H, int W, int Hg, int Wg, const float* dout, OUT* dfm, float out_scale,
+                                      cudaStream_t s);
 
 // ---- image_loss.cu: fused L1 + SSIM sums and, with dL_dimage != nullptr, the gradient w.r.t. image
 bool image_loss_grid_ok(int planes, int H, int W);  // the launch grid fits CUDA's limits
@@ -141,7 +147,9 @@ cudaError_t launch_reset_opacity(int P, float* raw_opacity, float* exp_avg, floa
 cudaError_t launch_activate(int P, int M, const float* raw_opacity, const float* raw_scaling, const float* raw_rotation,
                             const float* features_dc, const float* features_rest, float* opacity, float* scales,
                             float* rotations, float* shs, cudaStream_t s);
+// param_f16 (IDENTITY only, may be NULL): also written, half_rn of the updated param
 cudaError_t launch_adam_step(int kind, size_t n, int M, float* param, const float* grad_activated, float* exp_avg,
-                             float* exp_avg_sq, float lr, float beta1, float beta2, float eps, int step, cudaStream_t s);
+                             float* exp_avg_sq, float lr, float beta1, float beta2, float eps, int step, cudaStream_t s,
+                             __half* param_f16 = nullptr);
 
 }  // namespace f3dgs

@@ -13,6 +13,9 @@
 //                     (sigmoid / exp / normalize / the dc-rest split of the SH tensor) and the Adam update in place.
 //                     Formulas follow torch.optim.Adam's single-tensor path: m <- lerp(m, g, 1 - b1),
 //                     v <- b2 v + (1 - b2) g^2, p <- p - (lr / (1 - b1^t)) m / (sqrt(v) / sqrt(1 - b2^t) + eps).
+//                     With kHalfOut (IDENTITY groups: float16 feature fields) the same pass also writes the float16
+//                     working copy half_rn(p) of the float32 master, instead of a separate cast pass after the step.
+#include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
 
@@ -69,7 +72,8 @@ __device__ __forceinline__ void adam_update(float& p, float& m, float& v, float 
     p = p - a.lr_over_bc1 * (m / denom);
 }
 
-__global__ void __launch_bounds__(256) adam_step_kernel(AdamArgs a) {
+template <bool kHalfOut>
+__global__ void __launch_bounds__(256) adam_step_kernel(AdamArgs a, __half* __restrict__ param_f16) {
     const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (a.kind == F3DGS_PARAM_NORMALIZE4) {
         if (i >= a.n / 4) return;
@@ -112,6 +116,7 @@ __global__ void __launch_bounds__(256) adam_step_kernel(AdamArgs a) {
     a.param[i] = p;
     a.m[i] = m;
     a.v[i] = v;
+    if constexpr (kHalfOut) param_f16[i] = __float2half_rn(p);
 }
 
 }  // namespace
@@ -127,7 +132,8 @@ cudaError_t launch_activate(int P, int M, const float* raw_opacity, const float*
 }
 
 cudaError_t launch_adam_step(int kind, size_t n, int M, float* param, const float* grad_activated, float* exp_avg,
-                             float* exp_avg_sq, float lr, float beta1, float beta2, float eps, int step, cudaStream_t s) {
+                             float* exp_avg_sq, float lr, float beta1, float beta2, float eps, int step, cudaStream_t s,
+                             __half* param_f16) {
     AdamArgs a;
     a.param = param; a.grad = grad_activated; a.m = exp_avg; a.v = exp_avg_sq; a.n = n; a.kind = kind; a.M = M;
     const double bc1 = 1.0 - pow((double)beta1, (double)step), bc2 = 1.0 - pow((double)beta2, (double)step);
@@ -135,7 +141,11 @@ cudaError_t launch_adam_step(int kind, size_t n, int M, float* param, const floa
     a.inv_sqrt_bc2 = (float)(1.0 / sqrt(bc2));
     a.b1 = beta1; a.b2 = beta2; a.eps = eps;
     const size_t threads = kind == F3DGS_PARAM_NORMALIZE4 ? n / 4 : n;
-    adam_step_kernel<<<(unsigned)((threads + 255) / 256), 256, 0, s>>>(a);
+    const unsigned grid = (unsigned)((threads + 255) / 256);
+    if (param_f16)
+        adam_step_kernel<true><<<grid, 256, 0, s>>>(a, param_f16);
+    else
+        adam_step_kernel<false><<<grid, 256, 0, s>>>(a, nullptr);
     g_launches++;
     return cudaGetLastError();
 }

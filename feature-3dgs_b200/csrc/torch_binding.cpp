@@ -10,7 +10,8 @@
 // Differences (all permissive): the feature width is read from semantic_feature.size(-1) at run
 // time (reference: compile-time NUM_SEMANTIC_CHANNELS, config.h:16); an empty / undefined
 // semantic_feature means C = 0; semantic_feature may be float32 or float16, and the feature map
-// has its dtype (f3dgs_forward / f3dgs_forward_f16); inputs are checked for device/dtype and errors
+// has its dtype (f3dgs_forward / f3dgs_forward_f16); the backward calls take a float32 or float16 feature-map
+// gradient (f3dgs_backward_f16 / f3dgs_backward_accum_f16); inputs are checked for device/dtype and errors
 // from the C ABI are raised as RuntimeError.  This file contains no CUDA code and there is no CPU
 // fallback.
 #include <c10/cuda/CUDAGuard.h>
@@ -63,6 +64,15 @@ void check_features(const torch::Tensor& t, const torch::Device& dev) {
     TORCH_CHECK(t.scalar_type() == torch::kFloat32 || t.scalar_type() == torch::kFloat16,
                 "semantic_feature must be float32 or float16 (got ", t.scalar_type(), ")");
     TORCH_CHECK(t.device() == dev, "semantic_feature must be on ", dev, " (got ", t.device(), ")");
+}
+
+// dL/dfeature_map of the backward calls: float32 or float16 [C,H,W] on `dev`, made contiguous; undefined or empty is absent
+torch::Tensor feature_grad(const torch::Tensor& t, const torch::Device& dev) {
+    if (!t.defined() || t.numel() == 0) return t;
+    TORCH_CHECK(t.scalar_type() == torch::kFloat32 || t.scalar_type() == torch::kFloat16,
+                "grad_out_feature must be float32 or float16 (got ", t.scalar_type(), ")");
+    TORCH_CHECK(t.device() == dev, "grad_out_feature must be on ", dev, " (got ", t.device(), ")");
+    return t.contiguous();
 }
 
 void check_rc(int rc, const char* what) {
@@ -202,22 +212,30 @@ RasterizeGaussiansBackwardCUDA(const torch::Tensor& background, const torch::Ten
         auto shc = input(sh, dev, "shs"), cp = input(campos, dev, "campos");
         auto gc = input(dL_dout_color, dev, "grad_out_color");
         auto gd = input(dL_dout_depth, dev, "grad_out_depth");
-        torch::Tensor gf = C ? input(dL_dout_feature, dev, "grad_out_feature") : dL_dout_feature;
+        // a float16 map gradient goes to f3dgs_backward_f16 as it is (scale 1), without a float32 copy
+        torch::Tensor gf = C ? feature_grad(dL_dout_feature, dev) : torch::Tensor();
         TORCH_CHECK(radii.scalar_type() == torch::kInt32 && radii.is_cuda(), "radii must be int32 CUDA");
         auto rad = radii.contiguous();
         auto gb = geomBuffer.contiguous(), bb = binningBuffer.contiguous(), ib = imageBuffer.contiguous();
         cudaStream_t stream = c10::cuda::getCurrentCUDAStream().stream();
-        int rc = f3dgs_backward(
-            P, degree, M, R, C, fptr(bg), W, H, fptr(m3), fptr(shc), fptr(col), nullptr, fptr(sc), scale_modifier,
-            fptr(rot), fptr(cov), fptr(vm), fptr(pm), fptr(cp), tan_fovx, tan_fovy, rad.data_ptr<int>(),
-            reinterpret_cast<char*>(gb.data_ptr()), reinterpret_cast<char*>(bb.data_ptr()),
-            reinterpret_cast<char*>(ib.data_ptr()), fptr(gc), C ? fptr(gf) : nullptr, fptr(gd),
-            dL_dmeans2D.data_ptr<float>(), dL_dconic.data_ptr<float>(), dL_dopacity.data_ptr<float>(),
-            dL_dcolors.data_ptr<float>(), C ? dL_dsemantic_feature.data_ptr<float>() : nullptr,
-            dL_dmeans3D.data_ptr<float>(), dL_dcov3D.data_ptr<float>(), M ? dL_dsh.data_ptr<float>() : nullptr,
-            dL_dscales.data_ptr<float>(), dL_drotations.data_ptr<float>(), dL_dz.data_ptr<float>(), debug ? 1 : 0,
-            (void*)stream);
-        check_rc(rc, "f3dgs_backward");
+        // gs: the float16 symbol's scale after the map, nothing for the float32 one
+        auto run = [&](auto fn, auto gp, auto... gs) {
+            return fn(P, degree, M, R, C, fptr(bg), W, H, fptr(m3), fptr(shc), fptr(col), nullptr, fptr(sc),
+                      scale_modifier, fptr(rot), fptr(cov), fptr(vm), fptr(pm), fptr(cp), tan_fovx, tan_fovy,
+                      rad.data_ptr<int>(), reinterpret_cast<char*>(gb.data_ptr()),
+                      reinterpret_cast<char*>(bb.data_ptr()), reinterpret_cast<char*>(ib.data_ptr()), fptr(gc), gp,
+                      gs..., fptr(gd), dL_dmeans2D.data_ptr<float>(), dL_dconic.data_ptr<float>(),
+                      dL_dopacity.data_ptr<float>(), dL_dcolors.data_ptr<float>(),
+                      C ? dL_dsemantic_feature.data_ptr<float>() : nullptr, dL_dmeans3D.data_ptr<float>(),
+                      dL_dcov3D.data_ptr<float>(), M ? dL_dsh.data_ptr<float>() : nullptr,
+                      dL_dscales.data_ptr<float>(), dL_drotations.data_ptr<float>(), dL_dz.data_ptr<float>(),
+                      debug ? 1 : 0, (void*)stream);
+        };
+        call_f32_or_f16(gf, f3dgs_backward, "f3dgs_backward", f3dgs_backward_f16, "f3dgs_backward_f16",
+                        [&](auto fn, auto gp) {
+                            if constexpr (std::is_same_v<decltype(gp), uint16_t*>) return run(fn, gp, 1.0f);
+                            else return run(fn, gp);
+                        });
     }
     return std::make_tuple(dL_dmeans2D, dL_dcolors, dL_dsemantic_feature, dL_dopacity, dL_dmeans3D, dL_dcov3D, dL_dsh,
                            dL_dscales, dL_drotations);
@@ -236,7 +254,7 @@ void RasterizeGaussiansBackwardAccumCUDA(
     torch::Tensor scratch, torch::Tensor g_means3D, torch::Tensor g_sh, torch::Tensor g_colors,
     torch::Tensor g_semantic_feature, torch::Tensor g_opacities, torch::Tensor g_scales, torch::Tensor g_rotations,
     torch::Tensor g_cov3D, torch::Tensor g_means2D_out, torch::Tensor grad_accum, torch::Tensor denom,
-    const int64_t composite_done_event, const bool debug) {
+    const int64_t composite_done_event, const bool debug, const double feature_grad_scale) {
     TORCH_CHECK(means3D.is_cuda(), "means3D must be a CUDA tensor (this build has no CPU path)");
     const c10::cuda::CUDAGuard guard(means3D.device());
     const auto dev = means3D.device();
@@ -253,7 +271,12 @@ void RasterizeGaussiansBackwardAccumCUDA(
     auto vm = input(viewmatrix, dev, "viewmatrix"), pm = input(projmatrix, dev, "projmatrix");
     auto shc = input(sh, dev, "shs"), cp = input(campos, dev, "campos");
     auto gc = input(dL_dout_color, dev, "grad_out_color"), gd = input(dL_dout_depth, dev, "grad_out_depth");
-    torch::Tensor gf = C ? input(dL_dout_feature, dev, "grad_out_feature") : dL_dout_feature;
+    // a float16 map gradient stands for feature_grad_scale * grad (f3dgs_backward_accum_f16); a float32 one is the
+    // gradient itself, so its scale must be 1
+    torch::Tensor gf = C ? feature_grad(dL_dout_feature, dev) : torch::Tensor();
+    TORCH_CHECK(feature_grad_scale == 1.0 || (gf.defined() && gf.scalar_type() == torch::kFloat16),
+                "feature_grad_scale != 1 needs a float16 grad_out_feature (got ",
+                gf.defined() ? c10::toString(gf.scalar_type()) : "none", ")");
     TORCH_CHECK(radii.scalar_type() == torch::kInt32 && radii.is_cuda(), "radii must be int32 CUDA");
     auto rad = radii.contiguous();
     const size_t need = f3dgs_backward_scratch_bytes(P);
@@ -261,21 +284,29 @@ void RasterizeGaussiansBackwardAccumCUDA(
                     scratch.is_contiguous() && (size_t)scratch.numel() >= need,
                 "scratch must be a contiguous uint8 CUDA tensor of at least ", need, " bytes");
     cudaStream_t stream = c10::cuda::getCurrentCUDAStream().stream();
-    int rc = f3dgs_backward_accum(
-        P, degree, M, R, C, fptr(bg), W, H, fptr(m3), fptr(shc), fptr(col), fptr(sc), scale_modifier, fptr(rot), fptr(cov),
-        fptr(vm), fptr(pm), fptr(cp), tan_fovx, tan_fovy, rad.data_ptr<int>(),
-        reinterpret_cast<char*>(geomBuffer.data_ptr()), reinterpret_cast<char*>(binningBuffer.data_ptr()),
-        reinterpret_cast<char*>(imageBuffer.data_ptr()), fptr(gc), C ? fptr(gf) : nullptr, fptr(gd),
-        reinterpret_cast<char*>(scratch.data_ptr()), in_place(g_opacities, dev, P, "g_opacities"),
-        in_place(g_colors, dev, (int64_t)P * 3, "g_colors_precomp"),
-        in_place(g_semantic_feature, dev, (int64_t)P * C, "g_semantic_feature"),
-        in_place(g_means3D, dev, (int64_t)P * 3, "g_means3D"), in_place(g_cov3D, dev, (int64_t)P * 6, "g_cov3D_precomp"),
-        in_place(g_sh, dev, (int64_t)P * M * 3, "g_sh"), in_place(g_scales, dev, (int64_t)P * 3, "g_scales"),
-        in_place(g_rotations, dev, (int64_t)P * 4, "g_rotations"),
-        in_place(g_means2D_out, dev, (int64_t)P * 3, "g_means2D_out"), in_place(grad_accum, dev, P, "grad_accum"),
-        in_place(denom, dev, P, "denom"),
-        reinterpret_cast<void*>(static_cast<intptr_t>(composite_done_event)), debug ? 1 : 0, (void*)stream);
-    check_rc(rc, "f3dgs_backward_accum");
+    auto run = [&](auto fn, auto gp, auto... gs) {  // gs: the float16 symbol's scale after the map
+        return fn(P, degree, M, R, C, fptr(bg), W, H, fptr(m3), fptr(shc), fptr(col), fptr(sc), scale_modifier, fptr(rot),
+                  fptr(cov), fptr(vm), fptr(pm), fptr(cp), tan_fovx, tan_fovy, rad.data_ptr<int>(),
+                  reinterpret_cast<char*>(geomBuffer.data_ptr()), reinterpret_cast<char*>(binningBuffer.data_ptr()),
+                  reinterpret_cast<char*>(imageBuffer.data_ptr()), fptr(gc), gp, gs..., fptr(gd),
+                  reinterpret_cast<char*>(scratch.data_ptr()), in_place(g_opacities, dev, P, "g_opacities"),
+                  in_place(g_colors, dev, (int64_t)P * 3, "g_colors_precomp"),
+                  in_place(g_semantic_feature, dev, (int64_t)P * C, "g_semantic_feature"),
+                  in_place(g_means3D, dev, (int64_t)P * 3, "g_means3D"),
+                  in_place(g_cov3D, dev, (int64_t)P * 6, "g_cov3D_precomp"),
+                  in_place(g_sh, dev, (int64_t)P * M * 3, "g_sh"), in_place(g_scales, dev, (int64_t)P * 3, "g_scales"),
+                  in_place(g_rotations, dev, (int64_t)P * 4, "g_rotations"),
+                  in_place(g_means2D_out, dev, (int64_t)P * 3, "g_means2D_out"),
+                  in_place(grad_accum, dev, P, "grad_accum"), in_place(denom, dev, P, "denom"),
+                  reinterpret_cast<void*>(static_cast<intptr_t>(composite_done_event)), debug ? 1 : 0, (void*)stream);
+    };
+    call_f32_or_f16(gf, f3dgs_backward_accum, "f3dgs_backward_accum", f3dgs_backward_accum_f16,
+                    "f3dgs_backward_accum_f16", [&](auto fn, auto gp) {
+                        if constexpr (std::is_same_v<decltype(gp), uint16_t*>)
+                            return run(fn, gp, (float)feature_grad_scale);
+                        else
+                            return run(fn, gp);
+                    });
 }
 
 torch::Tensor markVisible(torch::Tensor& means3D, torch::Tensor& viewmatrix, torch::Tensor& projmatrix) {
@@ -303,11 +334,12 @@ bool is_target_dtype(const torch::Tensor& t) {
 }
 }  // namespace
 
-// -> (out [C,Hg,Wg], loss_sum [1]); with gt: out = sign(resized - gt) * grad_scale and loss_sum = sum |resized - gt|
+// -> (out [C,Hg,Wg], loss_sum [1]), float32; with gt: out = sign(resized - gt) * grad_scale and loss_sum =
+// sum |resized - gt|.  feature_map and gt may each be float32 or float16 (upcast exactly in the kernel)
 std::tuple<torch::Tensor, torch::Tensor> featureResizeFwd(const torch::Tensor& feature_map, const torch::Tensor& gt,
                                                           int64_t Hg, int64_t Wg, double grad_scale) {
-    TORCH_CHECK(feature_map.is_cuda() && feature_map.dim() == 3 && feature_map.scalar_type() == torch::kFloat32,
-                "feature_map must be a float32 CUDA tensor [C,H,W]");
+    TORCH_CHECK(feature_map.is_cuda() && feature_map.dim() == 3 && is_target_dtype(feature_map),
+                "feature_map must be a float32 or float16 CUDA tensor [C,H,W]");
     const c10::cuda::CUDAGuard guard(feature_map.device());
     auto fm = feature_map.contiguous();
     const int C = fm.size(0), H = fm.size(1), W = fm.size(2);
@@ -318,27 +350,45 @@ std::tuple<torch::Tensor, torch::Tensor> featureResizeFwd(const torch::Tensor& f
                         gt.size(2) == Wg, "gt must be a float32 or float16 CUDA tensor [C,Hg,Wg]");
         g = gt.contiguous();
     }
-    torch::Tensor out = torch::empty({C, Hg, Wg}, fm.options());
-    torch::Tensor loss = torch::zeros({1}, fm.options());
+    auto f32 = fm.options().dtype(torch::kFloat32);
+    torch::Tensor out = torch::empty({C, Hg, Wg}, f32);
+    torch::Tensor loss = torch::zeros({1}, f32);
     cudaStream_t stream = c10::cuda::getCurrentCUDAStream().stream();
-    call_f32_or_f16(g, f3dgs_feature_resize_fwd, "f3dgs_feature_resize_fwd", f3dgs_feature_resize_fwd_f16gt,
-                    "f3dgs_feature_resize_fwd_f16gt", [&](auto fn, auto gp) {
-                        return fn(C, H, W, (int)Hg, (int)Wg, fptr(fm), gp, (float)grad_scale, out.data_ptr<float>(),
-                                  loss.data_ptr<float>(), (void*)stream);
-                    });
+    auto run = [&](auto fn, auto fp, auto gp) {
+        return fn(C, H, W, (int)Hg, (int)Wg, fp, gp, (float)grad_scale, out.data_ptr<float>(), loss.data_ptr<float>(),
+                  (void*)stream);
+    };
+    if (fm.scalar_type() == torch::kFloat16) {
+        const uint16_t* fp = reinterpret_cast<const uint16_t*>(fm.data_ptr<at::Half>());
+        call_f32_or_f16(g, f3dgs_feature_resize_fwd_f16, "f3dgs_feature_resize_fwd_f16",
+                        f3dgs_feature_resize_fwd_f16_f16gt, "f3dgs_feature_resize_fwd_f16_f16gt",
+                        [&](auto fn, auto gp) { return run(fn, fp, gp); });
+    } else {
+        call_f32_or_f16(g, f3dgs_feature_resize_fwd, "f3dgs_feature_resize_fwd", f3dgs_feature_resize_fwd_f16gt,
+                        "f3dgs_feature_resize_fwd_f16gt", [&](auto fn, auto gp) { return run(fn, fptr(fm), gp); });
+    }
     return std::make_tuple(out, loss);
 }
 
-torch::Tensor featureResizeBwd(const torch::Tensor& dout, int64_t H, int64_t W) {
+// -> dL/dfeature_map [C,H,W] of `dtype`: float32, or float16 holding half_rn(out_scale * the float32 gradient)
+torch::Tensor featureResizeBwd(const torch::Tensor& dout, int64_t H, int64_t W, torch::ScalarType dtype,
+                               double out_scale) {
     TORCH_CHECK(dout.is_cuda() && dout.dim() == 3 && dout.scalar_type() == torch::kFloat32,
                 "dout must be a float32 CUDA tensor [C,Hg,Wg]");
+    TORCH_CHECK(dtype == torch::kFloat32 || dtype == torch::kFloat16, "feature_resize_bwd: dtype must be float32 or float16");
+    TORCH_CHECK(dtype == torch::kFloat16 || out_scale == 1.0, "feature_resize_bwd: out_scale != 1 needs dtype float16");
     const c10::cuda::CUDAGuard guard(dout.device());
     auto d = dout.contiguous();
     const int C = d.size(0), Hg = d.size(1), Wg = d.size(2);
-    torch::Tensor dfm = torch::empty({C, H, W}, d.options());
+    torch::Tensor dfm = torch::empty({C, H, W}, d.options().dtype(dtype));
     cudaStream_t stream = c10::cuda::getCurrentCUDAStream().stream();
-    check_rc(f3dgs_feature_resize_bwd(C, (int)H, (int)W, Hg, Wg, fptr(d), dfm.data_ptr<float>(), (void*)stream),
-             "f3dgs_feature_resize_bwd");
+    call_f32_or_f16(dfm, f3dgs_feature_resize_bwd, "f3dgs_feature_resize_bwd", f3dgs_feature_resize_bwd_f16,
+                    "f3dgs_feature_resize_bwd_f16", [&](auto fn, auto op) {
+                        if constexpr (std::is_same_v<decltype(op), uint16_t*>)
+                            return fn(C, (int)H, (int)W, Hg, Wg, fptr(d), (float)out_scale, op, (void*)stream);
+                        else
+                            return fn(C, (int)H, (int)W, Hg, Wg, fptr(d), op, (void*)stream);
+                    });
     return dfm;
 }
 
@@ -688,17 +738,32 @@ void activateParams(const torch::Tensor& raw_opacity, const torch::Tensor& raw_s
              "f3dgs_activate");
 }
 
+// param_f16 (optional, IDENTITY groups): a contiguous float16 tensor of param's size, written with param.half() after
+// the step (f3dgs_adam_step_f16out)
 void adamStep(int64_t kind, torch::Tensor param, const torch::Tensor& grad_activated, torch::Tensor exp_avg,
-              torch::Tensor exp_avg_sq, int64_t M, double lr, double beta1, double beta2, double eps, int64_t step) {
+              torch::Tensor exp_avg_sq, int64_t M, double lr, double beta1, double beta2, double eps, int64_t step,
+              const c10::optional<torch::Tensor>& param_f16) {
     TORCH_CHECK(param.is_cuda(), "parameters must be CUDA tensors (this build has no CPU path)");
     const auto dev = param.device();
     const c10::cuda::CUDAGuard guard(dev);
     const int64_t n = param.numel();
     auto g = input(grad_activated, dev, "grad_activated");
     cudaStream_t stream = c10::cuda::getCurrentCUDAStream().stream();
-    check_rc(f3dgs_adam_step((int)kind, (size_t)n, (int)M, in_place(param, dev, n, "param"), fptr(g),
-                             in_place(exp_avg, dev, n, "exp_avg"), in_place(exp_avg_sq, dev, n, "exp_avg_sq"), (float)lr,
-                             (float)beta1, (float)beta2, (float)eps, (int)step, (void*)stream),
+    float* p = in_place(param, dev, n, "param");
+    float *m = in_place(exp_avg, dev, n, "exp_avg"), *v = in_place(exp_avg_sq, dev, n, "exp_avg_sq");
+    if (param_f16.has_value() && param_f16->defined()) {
+        const torch::Tensor& h = *param_f16;
+        TORCH_CHECK(h.is_cuda() && h.device() == dev && h.scalar_type() == torch::kFloat16 && h.is_contiguous() &&
+                        h.numel() == n,
+                    "param_f16 must be a contiguous float16 tensor of ", n, " elements on ", dev);
+        check_rc(f3dgs_adam_step_f16out((int)kind, (size_t)n, (int)M, p, fptr(g), m, v,
+                                        reinterpret_cast<uint16_t*>(h.data_ptr<at::Half>()), (float)lr, (float)beta1,
+                                        (float)beta2, (float)eps, (int)step, (void*)stream),
+                 "f3dgs_adam_step_f16out");
+        return;
+    }
+    check_rc(f3dgs_adam_step((int)kind, (size_t)n, (int)M, p, fptr(g), m, v, (float)lr, (float)beta1, (float)beta2,
+                             (float)eps, (int)step, (void*)stream),
              "f3dgs_adam_step");
 }
 
@@ -727,9 +792,22 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     m.def("rasterize_gaussians", &RasterizeGaussiansCUDA);
     m.def("rasterize_gaussians_backward", &RasterizeGaussiansBackwardCUDA);
     m.def("mark_visible", &markVisible);
-    m.def("rasterize_gaussians_backward_accum", &RasterizeGaussiansBackwardAccumCUDA);
+    {
+        namespace py = pybind11;
+        m.def("rasterize_gaussians_backward_accum", &RasterizeGaussiansBackwardAccumCUDA, py::arg("background"),
+              py::arg("means3D"), py::arg("radii"), py::arg("colors"), py::arg("scales"), py::arg("rotations"),
+              py::arg("scale_modifier"), py::arg("cov3D_precomp"), py::arg("viewmatrix"), py::arg("projmatrix"),
+              py::arg("tan_fovx"), py::arg("tan_fovy"), py::arg("dL_dout_color"), py::arg("dL_dout_feature"),
+              py::arg("dL_dout_depth"), py::arg("sh"), py::arg("degree"), py::arg("campos"), py::arg("geomBuffer"),
+              py::arg("R"), py::arg("binningBuffer"), py::arg("imageBuffer"), py::arg("scratch"), py::arg("g_means3D"),
+              py::arg("g_sh"), py::arg("g_colors"), py::arg("g_semantic_feature"), py::arg("g_opacities"),
+              py::arg("g_scales"), py::arg("g_rotations"), py::arg("g_cov3D"), py::arg("g_means2D_out"),
+              py::arg("grad_accum"), py::arg("denom"), py::arg("composite_done_event"), py::arg("debug"),
+              py::arg("feature_grad_scale") = 1.0);
+    }
     m.def("feature_resize_fwd", &featureResizeFwd);
-    m.def("feature_resize_bwd", &featureResizeBwd);
+    m.def("feature_resize_bwd", &featureResizeBwd, pybind11::arg("dout"), pybind11::arg("H"), pybind11::arg("W"),
+          pybind11::arg("dtype") = torch::kFloat32, pybind11::arg("out_scale") = 1.0);
     m.def("image_loss", &imageLoss);
     m.def("decoder_forward", &decoderForward, pybind11::arg("x"), pybind11::arg("weight"), pybind11::arg("bias"),
           pybind11::arg("dtype") = torch::kFloat32);
@@ -746,7 +824,10 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     m.def("reset_opacity", &resetOpacity, pybind11::arg("raw_opacity"), pybind11::arg("exp_avg"),
           pybind11::arg("exp_avg_sq"), pybind11::arg("ceiling") = 0.01);
     m.def("activate", &activateParams);
-    m.def("adam_step", &adamStep);
+    m.def("adam_step", &adamStep, pybind11::arg("kind"), pybind11::arg("param"), pybind11::arg("grad_activated"),
+          pybind11::arg("exp_avg"), pybind11::arg("exp_avg_sq"), pybind11::arg("M"), pybind11::arg("lr"),
+          pybind11::arg("beta1"), pybind11::arg("beta2"), pybind11::arg("eps"), pybind11::arg("step"),
+          pybind11::arg("param_f16") = pybind11::none());
     m.def("backward_scratch_bytes", [](int P) { return (unsigned long long)f3dgs_backward_scratch_bytes(P); });
     m.def("debug_views", &debugViews);
     m.def("launch_count", []() { return (unsigned long long)f3dgs_launch_count(); });

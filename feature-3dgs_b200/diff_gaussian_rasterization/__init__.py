@@ -18,9 +18,11 @@ Behavioural notes
     rebuild per width, config.h:16); `semantic_feature=None` renders RGB + depth only (C = 0).
   * the feature map has the dtype of `semantic_feature`: float32 or float16 (the reference is float32 only).  A float16
     map is bitwise the float32 map of `semantic_feature.float()` rounded by `.half()`, without a float32 map ever
-    being made; colour, depth and radii are bitwise the float32 render's.  The backward stays float32: a float16 map's
-    gradient is upcast exactly and dL/dsemantic_feature is returned in `semantic_feature`'s dtype.  Float16 is for
-    rendering a trained field (render.py); GaussianState / ViewBatch training is float32.
+    being made; colour, depth and radii are bitwise the float32 render's.  A float16 map's gradient goes to the native
+    backward as it is (upcast exactly as it is loaded, no float32 copy); dL/dsemantic_feature is accumulated in float32
+    and returned in `semantic_feature`'s dtype.  To train a float16 feature field use GaussianState(feature_dtype=
+    torch.float16) with ViewBatch and feature_head's `*_and_grad(..., grad_dtype=torch.float16)`: their ScaledGrad
+    carries the float32 scale that keeps the L1 gradient (~1e-8) from underflowing in float16, which autograd cannot.
   * `debug=True` keeps the reference semantics: arguments are snapshotted to CPU first and dumped
     to snapshot_fw.dump / snapshot_bw.dump if the native call raises (reference :89-97,:147-155);
     natively it synchronises and checks after every stage.
@@ -114,8 +116,6 @@ class _RasterizeGaussians(torch.autograd.Function):
         if grad_out_feature is None:
             C = semantic_feature.shape[-1] if semantic_feature.numel() else 0
             grad_out_feature = torch.zeros(C, rs.image_height, rs.image_width, device=means3D.device)
-        elif grad_out_feature.dtype == torch.float16:
-            grad_out_feature = grad_out_feature.float()  # exact; the native backward is float32
         args = (rs.bg, means3D, radii, colors_precomp, semantic_feature, scales, rotations, rs.scale_modifier,
                 cov3Ds_precomp, rs.viewmatrix, rs.projmatrix, rs.tanfovx, rs.tanfovy, grad_out_color,
                 grad_out_feature, grad_depth, sh, rs.sh_degree, rs.campos, geomBuffer, ctx.num_rendered,

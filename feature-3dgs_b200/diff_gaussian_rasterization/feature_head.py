@@ -16,6 +16,13 @@ There is no CPU path (the extension raises on CPU tensors).
 The teacher map `gt` may be float32 or float16, the dtype the data format stores it in (io.load_feature_map(path,
 dtype=None)).  A float16 map is read as it is and upcast exactly inside the kernels, so no float32 copy is made and every
 result equals the one for `gt.float()`; the loss and the gradients are float32, as PyTorch's `l1_loss(fp32, fp16)` gives.
+
+Training a float16 feature field (GaussianState(feature_dtype=torch.float16), ViewBatch): the two `_and_grad` functions
+also read a float16 rendered map exactly, and with grad_dtype=torch.float16 return dL/dfeature_map as a `ScaledGrad`, a
+float16 map plus a float32 scale, for `ViewBatch.backward`.  The scale is needed: the L1 gradient is
+sign * weight / (C*Hg*Wg), about 1.9e-8 at C = 128 and a 853x480 teacher, below float16's smallest subnormal (5.96e-8),
+so a plain float16 cast of it is all zeros.  The autograd wrappers stay float32: autograd would cast the gradient to
+float16 without a scale.
 """
 from typing import NamedTuple, Optional
 
@@ -28,18 +35,54 @@ def _C():
     return ext
 
 
-def feature_l1_loss_and_grad(feature_map: torch.Tensor, gt: torch.Tensor, weight: float = 1.0):
-    """-> (loss, dL/dfeature_map) for loss = weight * mean|resize(feature_map) - gt|, no autograd graph (ViewBatch loops)."""
+class ScaledGrad(NamedTuple):
+    """A float16 gradient map that stands for `scale * grad.float()`: grad [C,H,W] float16 holds dL/dO / scale, so that
+    a gradient far below float16's range keeps its digits (ViewBatch.backward applies the scale in float32)."""
+
+    grad: torch.Tensor
+    scale: float
+
+
+def _grad_half(grad_dtype) -> bool:
+    if grad_dtype is None or grad_dtype == torch.float32:
+        return False
+    if grad_dtype == torch.float16:
+        return True
+    raise ValueError(f"grad_dtype must be None, torch.float32 or torch.float16, got {grad_dtype}")
+
+
+def _reject_half(feature_map: torch.Tensor, fn: str):
+    if feature_map.dtype == torch.float16:
+        raise RuntimeError(
+            f"{fn}: feature_map must be float32; train a float16 map without autograd: the ViewBatch path, "
+            f"{fn}_and_grad(..., grad_dtype=torch.float16) -> ViewBatch.backward (autograd would cast the gradient to "
+            "float16 without a scale, and it would underflow)")
+
+
+def feature_l1_loss_and_grad(feature_map: torch.Tensor, gt: torch.Tensor, weight: float = 1.0, grad_dtype=None):
+    """-> (loss, dL/dfeature_map) for loss = weight * mean|resize(feature_map) - gt|, no autograd graph (ViewBatch loops).
+
+    feature_map may be float32 or float16 (read exactly).  grad_dtype=torch.float16 returns the gradient as a
+    ScaledGrad: the float16 map resize^T(sign(resized - gt)) with scale = weight / (C*Hg*Wg), so no [C,H,W] float32
+    tensor is made.  With the default arguments the results are the float32 ones."""
     C, Hg, Wg = gt.shape
     n = max(C * Hg * Wg, 1)
-    sign, loss_sum = _C().feature_resize_fwd(feature_map, gt, Hg, Wg, weight / n)
-    grad = _C().feature_resize_bwd(sign, feature_map.shape[1], feature_map.shape[2])
-    return loss_sum[0] * (weight / n), grad
+    H, W = feature_map.shape[1], feature_map.shape[2]
+    if not _grad_half(grad_dtype):
+        sign, loss_sum = _C().feature_resize_fwd(feature_map, gt, Hg, Wg, weight / n)
+        grad = _C().feature_resize_bwd(sign, H, W)
+        return loss_sum[0] * (weight / n), grad
+    # exact signs (grad_scale 1) and the whole factor weight / n in the float32 scale; a zero weight gives zero signs
+    scale = weight / n
+    sign, loss_sum = _C().feature_resize_fwd(feature_map, gt, Hg, Wg, 1.0 if scale != 0 else 0.0)
+    grad = _C().feature_resize_bwd(sign, H, W, torch.float16, 1.0)
+    return loss_sum[0] * scale, ScaledGrad(grad, scale if scale != 0 else 1.0)
 
 
 class _FeatureL1(torch.autograd.Function):
     @staticmethod
     def forward(ctx, feature_map, gt, weight):
+        _reject_half(feature_map, "feature_l1_loss")
         loss, grad = feature_l1_loss_and_grad(feature_map, gt, weight)
         ctx.save_for_backward(grad)
         return loss
@@ -58,6 +101,9 @@ def feature_l1_loss(feature_map: torch.Tensor, gt: torch.Tensor, weight: float =
 class _Resize(torch.autograd.Function):
     @staticmethod
     def forward(ctx, feature_map, Hg, Wg):
+        if feature_map.dtype != torch.float32:
+            raise RuntimeError("resize_bilinear: feature_map must be float32 (autograd would cast its gradient to "
+                               "float16 without a scale)")
         ctx.hw = (feature_map.shape[1], feature_map.shape[2])
         out, _ = _C().feature_resize_fwd(feature_map, torch.empty(0, device=feature_map.device), Hg, Wg, 0.0)
         return out
@@ -86,7 +132,7 @@ def decode(feature_map: torch.Tensor, weight: torch.Tensor, bias=None, dtype=tor
 
 
 def decoded_feature_l1_loss_and_grad(feature_map: torch.Tensor, gt: torch.Tensor, weight: torch.Tensor, bias=None,
-                                     loss_weight: float = 1.0, dweight=None, dbias=None):
+                                     loss_weight: float = 1.0, dweight=None, dbias=None, grad_dtype=None):
     """-> (loss, dL/dfeature_map, dweight, dbias) for the --speedup feature loss
 
         loss = loss_weight * l1_loss(cnn_decoder(F.interpolate(feature_map[None], gt.shape[1:], 'bilinear', True)[0]), gt)
@@ -96,7 +142,11 @@ def decoded_feature_l1_loss_and_grad(feature_map: torch.Tensor, gt: torch.Tensor
     the decoder are ADDED into `dweight` / `dbias` (typically `conv.weight.grad` / `conv.bias.grad`, so the views of a step
     accumulate); they are allocated zeroed when None, and dbias stays None without a bias.  Step the decoder with the
     reference's `torch.optim.Adam(cnn_decoder.parameters())` on those tensors; with several ranks, all-reduce them (they
-    are small) before the step."""
+    are small) before the step.
+
+    feature_map may be float32 or float16 (read exactly).  grad_dtype=torch.float16 returns dL/dfeature_map as a
+    ScaledGrad with scale = loss_weight / (Cout*Hg*Wg): the decoder's gradients use the true scale, and the float16 map
+    is resize^T(dL/d resized) / scale."""
     Cout, Hg, Wg = gt.shape
     with torch.no_grad():
         resized, _ = _C().feature_resize_fwd(feature_map, _empty(feature_map), Hg, Wg, 0.0)
@@ -105,9 +155,14 @@ def decoded_feature_l1_loss_and_grad(feature_map: torch.Tensor, gt: torch.Tensor
         if dbias is None and bias is not None:
             dbias = torch.zeros_like(bias, memory_format=torch.contiguous_format)
         gs = float(loss_weight) / max(Cout * Hg * Wg, 1)
-        loss_sum, dres = _C().decoder_l1(resized, gt, weight, _empty(feature_map) if bias is None else bias, gs, dweight,
-                                         _empty(feature_map) if dbias is None else dbias)
-        grad = _C().feature_resize_bwd(dres, feature_map.shape[1], feature_map.shape[2])
+        loss_sum, dres = _C().decoder_l1(resized, gt, weight, _empty(resized) if bias is None else bias, gs, dweight,
+                                         _empty(resized) if dbias is None else dbias)
+        H, W = feature_map.shape[1], feature_map.shape[2]
+        if _grad_half(grad_dtype):
+            s = gs if gs != 0 else 1.0  # gs == 0: dres is zero
+            grad = ScaledGrad(_C().feature_resize_bwd(dres, H, W, torch.float16, 1.0 / s), s)
+        else:
+            grad = _C().feature_resize_bwd(dres, H, W)
     return loss_sum[0] * gs, grad, dweight, dbias
 
 
@@ -215,6 +270,7 @@ def pca_image(x: torch.Tensor, fit: Optional[FeaturePCA] = None) -> torch.Tensor
 class _DecodedL1(torch.autograd.Function):
     @staticmethod
     def forward(ctx, feature_map, weight, bias, gt, loss_weight):
+        _reject_half(feature_map, "decoded_feature_l1_loss")
         loss, g_fm, g_w, g_b = decoded_feature_l1_loss_and_grad(feature_map.detach(), gt.detach(), weight.detach(),
                                                                 None if bias is None else bias.detach(), loss_weight)
         ctx.has_bias = bias is not None

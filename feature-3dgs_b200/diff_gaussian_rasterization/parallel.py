@@ -95,6 +95,9 @@ class ViewBatch:
 
     Parameter order inside the flat buffer: the feature and opacity gradients come first -- they are complete as soon as
     the last view's backward composite has run, so their bucket of the all-reduce overlaps the last backward preprocess.
+
+    `semantic_feature` may be float16 (a float16 feature field): the forward then renders a float16 map, and the
+    feature gradient still accumulates in float32, in a slot of the same shape.
     """
 
     ORDER = ("semantic_feature", "opacities", "means3D", "shs", "scales", "rotations")
@@ -150,9 +153,13 @@ class ViewBatch:
 
     def backward(self, ctx, g_color, g_feature, g_depth, means2D_out=None, last: bool = False):
         """Add this view's parameter gradients into the flat buffer.  `last=True` on the rank's last view of the step
-        lets all_reduce() start the feature/opacity bucket early."""
+        lets all_reduce() start the feature/opacity bucket early.  g_feature: dL/dfeature_map as a float32 or float16
+        [C,H,W] tensor, a feature_head.ScaledGrad (a float16 map and its float32 scale), or None."""
         rs, p, g, e = ctx.rs, self.params, self.grads, torch.Tensor([])
         none = self._empty
+        scale = 1.0
+        if isinstance(g_feature, tuple):  # ScaledGrad (not imported: this module loads without the package)
+            g_feature, scale = g_feature
         self._C.rasterize_gaussians_backward_accum(
             rs.bg, p["means3D"], ctx.radii, e, p["scales"], p["rotations"], rs.scale_modifier, e, rs.viewmatrix,
             rs.projmatrix, rs.tanfovx, rs.tanfovy, g_color, g_feature if g_feature is not None else none, g_depth,
@@ -160,7 +167,7 @@ class ViewBatch:
             g["means3D"], g["shs"], none, g.get("semantic_feature", none), g["opacities"], g["scales"], g["rotations"],
             none, means2D_out if means2D_out is not None else none,
             self.grad_accum if self.grad_accum is not None else none, self.denom if self.denom is not None else none,
-            int(self._ev.cuda_event) if (last and self._ev is not None) else 0, rs.debug)
+            int(self._ev.cuda_event) if (last and self._ev is not None) else 0, rs.debug, float(scale))
         self._early_pending = bool(last and self._ev is not None)
 
     def all_reduce(self, group: Optional[dist.ProcessGroup] = None):

@@ -17,6 +17,12 @@ _opacity, _scaling, _rotation, _semantic_feature`, :47-58) as plain CUDA tensors
   densify_and_prune()   clone / split / prune (:350-434) with the optimizer state carried along, in two native calls
                         (f3dgs_densify_plan / f3dgs_densify_apply) with one host read in between;
   reset_opacity()       :231-234 in one kernel (f3dgs_reset_opacity).
+
+Float16 feature fields: with feature_dtype=torch.float16 the rasterizer reads a float16 working copy
+act["semantic_feature"] of the float32 master raw["semantic_feature"], so every view renders a float16 map and the feature
+loss hands back a float16 gradient (feature_head `*_and_grad(..., grad_dtype=torch.float16)`).  The master, its Adam
+moments and the accumulated gradient stay float32; the copy is made by one cast at construction and after
+densify_and_prune, and step() refreshes it in the Adam pass itself (f3dgs_adam_step_f16out).
 """
 import math
 from typing import Dict, Optional
@@ -39,7 +45,7 @@ class GaussianState:
     NAMES = ("xyz", "f_dc", "f_rest", "opacity", "scaling", "rotation", "semantic_feature")
 
     def __init__(self, xyz, features_dc, features_rest, opacity, scaling, rotation, semantic_feature,
-                 betas=(0.9, 0.999), eps=1e-15, percent_dense=0.01):
+                 betas=(0.9, 0.999), eps=1e-15, percent_dense=0.01, feature_dtype=torch.float32):
         self.raw: Dict[str, torch.Tensor] = dict(
             xyz=xyz.contiguous(), f_dc=features_dc.contiguous(), f_rest=features_rest.contiguous(),
             opacity=opacity.contiguous(), scaling=scaling.contiguous(), rotation=rotation.contiguous(),
@@ -47,7 +53,10 @@ class GaussianState:
         for k, v in self.raw.items():
             if not v.is_cuda or v.dtype != torch.float32:
                 raise RuntimeError(f"{k} must be a float32 CUDA tensor (this build has no CPU path)")
+        if feature_dtype not in (torch.float32, torch.float16):
+            raise ValueError(f"feature_dtype must be torch.float32 or torch.float16, got {feature_dtype}")
         self.betas, self.eps, self.percent_dense = betas, eps, percent_dense
+        self.feature_dtype = feature_dtype
         self._reset_derived()
 
     @classmethod
@@ -60,7 +69,7 @@ class GaussianState:
         three nearest neighbours)), isotropic, from the native distCUDA2 (csrc/knn.cu).  Every other field is computed
         with the reference's own tensor operations, so it is bitwise what create_from_pcd builds.  With `speedup` the
         feature width is int(semantic_feature_size / 4), as there.  Raises ValueError on mismatched shapes or a
-        non-finite coordinate."""
+        non-finite coordinate.  kwargs (feature_dtype among them) go to the constructor."""
         from . import _C
 
         def as_f32(a):
@@ -104,9 +113,10 @@ class GaussianState:
             self.exp_avg_sq = {k: torch.zeros_like(v) for k, v in self.raw.items()}
             self.steps = {k: 0 for k in self.raw}
         self.max_radii2D = torch.zeros(P, device=dev)
+        sf = self.raw["semantic_feature"]
         self.act = dict(means3D=self.raw["xyz"], opacities=torch.empty(P, 1, device=dev), scales=torch.empty(P, 3, device=dev),
                         rotations=torch.empty(P, 4, device=dev), shs=torch.empty(P, self.M, 3, device=dev),
-                        semantic_feature=self.raw["semantic_feature"])
+                        semantic_feature=sf if self.feature_dtype == torch.float32 else sf.to(self.feature_dtype))
         self._batch: Optional[ViewBatch] = None
 
     def activate(self):
@@ -133,8 +143,11 @@ class GaussianState:
             if p.numel() == 0:
                 continue
             self.steps[name] += 1
+            # a float16 working copy of the features is rewritten in the same pass
+            half = name == "semantic_feature" and self.feature_dtype == torch.float16
+            copy = self.act["semantic_feature"] if half else None
             _C.adam_step(KIND[name], p, g[GRAD_OF[name]], self.exp_avg[name], self.exp_avg_sq[name], self.M, lrs[name],
-                         self.betas[0], self.betas[1], self.eps, self.steps[name])
+                         self.betas[0], self.betas[1], self.eps, self.steps[name], copy)
 
     # ---------------------------------------------------------------------------------------------- densification
     def update_max_radii(self, radii):

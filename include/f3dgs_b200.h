@@ -118,6 +118,28 @@ int f3dgs_backward(int P, int D, int M, int R, int C,
                    float* dL_dsemantic_feature, float* dL_dmean3D, float* dL_dcov3D,
                    float* dL_dsh, float* dL_dscale, float* dL_drot, float* dL_dz,
                    int debug, void* cuda_stream);
+/* f3dgs_backward with a float16 feature-map gradient (training float16 feature fields): dL_dfeaturepix [C,H,W] holds
+ * IEEE binary16 bits h standing for the gradient dL_dfeaturepix_scale * float(h) (finite, nonzero).  The scale lets a
+ * gradient far below float16's range (an L1 feature loss's weight / (C*Hg*Wg) is ~1e-8) be stored without underflow;
+ * it is applied in float32 (one multiply, rounded to nearest) as the map is loaded, and no float32 [C,H,W] buffer is
+ * made.  Every output equals that of f3dgs_backward called with the float32 map scale * float(h), up to the order of
+ * the float reductions f3dgs_backward already has; dL_dsemantic_feature stays float32 (the master gradient) and must
+ * not overlap dL_dfeaturepix.  Validates as f3dgs_backward. */
+int f3dgs_backward_f16(int P, int D, int M, int R, int C,
+                       const float* background, int width, int height,
+                       const float* means3D, const float* shs, const float* colors_precomp,
+                       const float* semantic_feature,
+                       const float* scales, float scale_modifier, const float* rotations,
+                       const float* cov3D_precomp,
+                       const float* viewmatrix, const float* projmatrix, const float* cam_pos,
+                       float tan_fovx, float tan_fovy, const int* radii,
+                       char* geom_buffer, char* binning_buffer, char* image_buffer,
+                       const float* dL_dpix, const uint16_t* dL_dfeaturepix, float dL_dfeaturepix_scale,
+                       const float* dL_depths,
+                       float* dL_dmean2D, float* dL_dconic, float* dL_dopacity, float* dL_dcolor,
+                       float* dL_dsemantic_feature, float* dL_dmean3D, float* dL_dcov3D,
+                       float* dL_dsh, float* dL_dscale, float* dL_drot, float* dL_dz,
+                       int debug, void* cuda_stream);
 
 /* ---- accumulating backward for view batches (additive: the reference ASSIGNS per-view gradients into freshly
  * zero-filled tensors, rasterize_points.cu:163-173, backward.cu:273, and leaves the sum over views to autograd) ----
@@ -151,6 +173,22 @@ int f3dgs_backward_accum(int P, int D, int M, int R, int C,
                          float* dL_dmean3D, float* dL_dcov3D_precomp, float* dL_dsh, float* dL_dscale,
                          float* dL_drot, float* dL_dmean2D_out, float* grad_accum, float* denom,
                          void* composite_done_event, int debug, void* cuda_stream);
+/* f3dgs_backward_accum with a float16 feature-map gradient, scaled as for f3dgs_backward_f16.  Arguments are validated
+ * before the scratch is zeroed. */
+int f3dgs_backward_accum_f16(int P, int D, int M, int R, int C,
+                             const float* background, int width, int height,
+                             const float* means3D, const float* shs, const float* colors_precomp,
+                             const float* scales, float scale_modifier, const float* rotations,
+                             const float* cov3D_precomp,
+                             const float* viewmatrix, const float* projmatrix, const float* cam_pos,
+                             float tan_fovx, float tan_fovy, const int* radii,
+                             char* geom_buffer, char* binning_buffer, char* image_buffer,
+                             const float* dL_dpix, const uint16_t* dL_dfeaturepix, float dL_dfeaturepix_scale,
+                             const float* dL_depths, char* scratch,
+                             float* dL_dopacity, float* dL_dcolors_precomp, float* dL_dsemantic_feature,
+                             float* dL_dmean3D, float* dL_dcov3D_precomp, float* dL_dsh, float* dL_dscale,
+                             float* dL_drot, float* dL_dmean2D_out, float* grad_accum, float* denom,
+                             void* composite_done_event, int debug, void* cuda_stream);
 
 /* ==== callers either side of the rasterizer (SURVEY.md section 8 f): additive entry points ======================= */
 
@@ -174,6 +212,22 @@ int f3dgs_feature_resize_bwd(int C, int H, int W, int Hg, int Wg, const float* d
  * target.  It validates as its float32 twin does, and also rejects an `out` that overlaps feature_map or gt. */
 int f3dgs_feature_resize_fwd_f16gt(int C, int H, int W, int Hg, int Wg, const float* feature_map, const uint16_t* gt,
                                    float grad_scale, float* out, float* loss_sum, void* cuda_stream);
+/* Training float16 feature fields.
+ *   f3dgs_feature_resize_fwd_f16        feature_map [C,H,W] float16; gt float32 or NULL.
+ *   f3dgs_feature_resize_fwd_f16_f16gt  feature_map and gt float16 (gt required).
+ *       The result (out and loss_sum, float32) is that of f3dgs_feature_resize_fwd applied to the exactly upcast inputs.
+ *   f3dgs_feature_resize_bwd_f16        dL_dfeature_map [C,H,W] float16 = half_rn(out_scale * f3dgs_feature_resize_bwd
+ *       (dout)) elementwise (+-inf beyond 65504, as torch's .half()); out_scale finite and nonzero.  An L1 loss passes
+ *       grad_scale = 1 to the forward (exact signs), out_scale = 1, and hands the map to f3dgs_backward_f16 with the
+ *       scale weight / (C*Hg*Wg), which float16 alone cannot hold.
+ * They validate as their float32 twins, and also reject an output that overlaps an input (2-byte sizes for float16). */
+int f3dgs_feature_resize_fwd_f16(int C, int H, int W, int Hg, int Wg, const uint16_t* feature_map, const float* gt,
+                                 float grad_scale, float* out, float* loss_sum, void* cuda_stream);
+int f3dgs_feature_resize_fwd_f16_f16gt(int C, int H, int W, int Hg, int Wg, const uint16_t* feature_map,
+                                       const uint16_t* gt, float grad_scale, float* out, float* loss_sum,
+                                       void* cuda_stream);
+int f3dgs_feature_resize_bwd_f16(int C, int H, int W, int Hg, int Wg, const float* dout, float out_scale,
+                                 uint16_t* dL_dfeature_map, void* cuda_stream);
 
 /* ---- feature decoder (--speedup): models/networks.py:107-119 CNN_decoder, nn.Conv2d(Cin, Cout, kernel_size=1) -------
  * x [Cin,N] (the resized map, N = Hg*Wg), weight [Cout,Cin] (the conv weight [Cout,Cin,1,1] as contiguous memory),
@@ -290,6 +344,13 @@ int f3dgs_activate(int P, int M, const float* raw_opacity, const float* raw_scal
 #define F3DGS_PARAM_SH_REST 5
 int f3dgs_adam_step(int kind, size_t n, int M, float* param, const float* grad_activated, float* exp_avg,
                     float* exp_avg_sq, float lr, float beta1, float beta2, float eps, int step, void* cuda_stream);
+/* f3dgs_adam_step of an IDENTITY group (kind must be F3DGS_PARAM_IDENTITY) that also keeps a float16 working copy: in the
+ * same pass, param_f16[n] (IEEE binary16 bits) = the updated param rounded to nearest even (torch's .half()).  param,
+ * exp_avg and exp_avg_sq are bitwise those of f3dgs_adam_step and stay float32 (the master weights); param_f16 must not
+ * overlap the other buffers.  For float16 feature fields: the rasterizer reads the copy, the optimizer the master. */
+int f3dgs_adam_step_f16out(int kind, size_t n, int M, float* param, const float* grad_activated, float* exp_avg,
+                           float* exp_avg_sq, uint16_t* param_f16, float lr, float beta1, float beta2, float eps,
+                           int step, void* cuda_stream);
 
 /* ---- initial scales: reference submodules/simple-knn distCUDA2, used by scene/gaussian_model.py:133-160 ------------
  * out[i] = (d0 + d1 + d2) / 3 in fp32, where d0 <= d1 <= d2 are the three smallest squared distances from points[i] to
