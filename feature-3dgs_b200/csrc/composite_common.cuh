@@ -24,6 +24,8 @@
 // The forward launches all 20 warps (composite_fwd.cu); the backward geometry kernel launches the
 // producer group and the alpha warps only (composite_bwd.cu).
 #pragma once
+#include <initializer_list>
+
 #include "kernels.h"
 
 namespace f3dgs {
@@ -66,35 +68,144 @@ struct alignas(128) WSlot {
     int32_t work;
 };
 
-template <int CH, typename TF = float>
+// WB x WJ: dimensions of the weight-slot ring (pixel blocks x slots per block)
+template <int CH, typename TF = float, int WB = kBlocksPerTile, int WJ = kWSlots>
 struct alignas(128) RingV2 {
     using Feat = TF;
-    static constexpr int kWB = kBlocksPerTile, kWJ = kWSlots;  // dimensions of the weight-slot ring
+    static constexpr int kWB = WB, kWJ = WJ;
     Stage<CH, TF> stage[kStages];
-    WSlot ws[kBlocksPerTile][kWSlots];
+    WSlot ws[WB][WJ];
     uint64_t full[kStages];
     uint64_t empty[kStages];
     uint64_t listed[kStages];  // records + ids of the stage are written: the copy warp may fetch its feature rows
-    uint64_t wfull[kBlocksPerTile][kWSlots];
-    uint64_t wempty[kBlocksPerTile][kWSlots];
+    uint64_t wfull[WB][WJ];
+    uint64_t wempty[WB][WJ];
     uint32_t done_mask[kDoneSlots];  // bit b set: pixel block b of that work item needs no more instances
 };
 
-// The same ring without feature rows or weight slots, for the backward geometry kernel, which has no feature warps:
-// 14 KB instead of 83 KB of shared memory, so that two CTAs fit on an SM.  The one-element `ws` / `wfull` / `wempty` are
-// not used; ring_init<> initialises the two barriers.
-struct alignas(128) RingSlim {
-    using Feat = float;
-    static constexpr int kWB = 1, kWJ = 1;
-    Stage<0> stage[kStages];
-    WSlot ws[1][1];
-    uint64_t full[kStages];
-    uint64_t empty[kStages];
-    uint64_t listed[kStages];
-    uint64_t wfull[1][1];
-    uint64_t wempty[1][1];
-    uint32_t done_mask[kDoneSlots];
+// The ring without feature rows and with a single weight slot, for the backward geometry kernel, which has no feature
+// warps: 14 KB instead of 83 KB of shared memory, so that two CTAs fit on an SM.  The one-element `ws` / `wfull` /
+// `wempty` are not used; ring_init<> initialises the two barriers.
+using RingSlim = RingV2<0, float, 1, 1>;
+
+static_assert(sizeof(RingV2<0>) == 81664 && sizeof(RingSlim) == 16128, "ring layout changed");
+static_assert(sizeof(RingV2<32>) == 106240 && sizeof(RingV2<64>) == 130816 && sizeof(RingV2<128>) == 179968,
+              "ring layout changed");
+static_assert(sizeof(RingV2<32, __half>) == 93952 && sizeof(RingV2<64, __half>) == 106240 &&
+                  sizeof(RingV2<128, __half>) == 130816,
+              "ring layout changed");
+
+// ---------------------------------------------------------------- pixel-block layout
+// A 16x16 tile is 8 blocks of 8x4 pixels, 2 across and 4 down.  Slot p of a block (an alpha warp's lane, a column of
+// the weight tiles and of the emitted list_w rows) is pixel i = p & 3 of the 2x2 quad q = p >> 2; the quads lie 4
+// across, so bits 4q..4q+3 of a pixel mask are quad q.
+// Origin (bx0, by0) of block b of the tile at (tile_x, tile_y); tile = tile_y * tiles_x + tile_x.
+__device__ __forceinline__ int block_x0(int tile_x, int b) { return tile_x * 16 + (b & 1) * 8; }
+__device__ __forceinline__ int block_y0(int tile_y, int b) { return tile_y * 16 + (b >> 1) * 4; }
+// offset of slot p from the block origin
+__device__ __forceinline__ int slot_px(int p) { return ((p >> 2) & 3) * 2 + (p & 1); }
+__device__ __forceinline__ int slot_py(int p) { return (p >> 4) * 2 + ((p >> 1) & 1); }
+
+// Register tile of a feature lane: float2 t[NQ][2][4] = [quad][quad row][channel], the two pixels of a quad row in .x
+// and .y (one paired FMA covers both).  With CH / 4 lanes per feature row, G = 32 / (CH / 4) lane groups share the
+// block's 8 quads: group grp holds quads qi * G + grp, qi < NQ = 8 / G.
+template <int NQ>
+__device__ __forceinline__ float& tile_px(float2 (&t)[NQ][2][4], int qi, int i, int c) {
+    return (i & 1) ? t[qi][i >> 1][c].y : t[qi][i >> 1][c].x;
+}
+// Pixel k of the run of pixels 4 * half .. 4 * half + 3 in row y of the block, for a lane that holds all 8 quads
+// (G == 1).  (% NQ only keeps the indices in range in the instantiations with G > 1, which never get here.)
+template <int NQ>
+__device__ __forceinline__ float& tile_run_px(float2 (&t)[NQ][2][4], int y, int half, int k, int c) {
+    return tile_px(t, ((y >> 1) * 4 + half * 2 + (k >> 1)) % NQ, (y & 1) * 2 + (k & 1), c);
+}
+template <int NQ>
+__device__ __forceinline__ float4 tile_run(float2 (&t)[NQ][2][4], int y, int half, int c) {
+    return make_float4(tile_run_px(t, y, half, 0, c), tile_run_px(t, y, half, 1, c), tile_run_px(t, y, half, 2, c),
+                       tile_run_px(t, y, half, 3, c));
+}
+template <int NQ>
+__device__ __forceinline__ void set_tile_run(float2 (&t)[NQ][2][4], int y, int half, int c, float4 v) {
+    tile_run_px(t, y, half, 0, c) = v.x;
+    tile_run_px(t, y, half, 1, c) = v.y;
+    tile_run_px(t, y, half, 2, c) = v.z;
+    tile_run_px(t, y, half, 3, c) = v.w;
+}
+
+// Visits one channel plane of a register tile over the block's pixels inside the W x H image, in the widest access the
+// plane allows, and hands each access its address in `plane`:
+//   row(p, y)           8-pixel row y: G == 1, `rows` (8-pixel alignment of the plane) and the row inside the image
+//   run(p, y, half)     4-pixel run: G == 1 and `runs` (4-pixel alignment)
+//   px(p, qi, i)        otherwise pixel i of the lane's quad qi, one at a time
+template <int G, int NQ, typename T, class Row, class Run, class Px>
+__device__ __forceinline__ void for_tile_pixels(T* plane, int bx0, int by0, int W, int H, int grp, bool rows, bool runs,
+                                                Row row, Run run, Px px) {
+    if (G == 1 && rows && bx0 + 8 <= W) {
+#pragma unroll
+        for (int y = 0; y < 4; y++) {
+            const int yy = by0 + y;
+            if (yy >= H) continue;
+            row(plane + (size_t)yy * W + bx0, y);
+        }
+    } else if (G == 1 && runs) {
+#pragma unroll
+        for (int y = 0; y < 4; y++) {
+            const int yy = by0 + y;
+            if (yy >= H) continue;
+#pragma unroll
+            for (int half = 0; half < 2; half++) {
+                const int xx = bx0 + half * 4;
+                if (xx >= W) continue;
+                run(plane + (size_t)yy * W + xx, y, half);
+            }
+        }
+    } else {
+#pragma unroll
+        for (int qi = 0; qi < NQ; qi++) {
+            const int q = qi * G + grp;
+#pragma unroll
+            for (int i = 0; i < 4; i++) {
+                // slot_px / slot_py of slot 4 * q + i, spelled per quad: q is a runtime value when G > 1, and the compiler
+                // does not fold slot_px(4 * q + i) back to this form (280-460 more SASS instructions in each CH = 32 / 64
+                // forward kernel)
+                const int xx = bx0 + (q & 3) * 2 + (i & 1), yy = by0 + (q >> 2) * 2 + (i >> 1);
+                if (xx < W && yy < H) px(plane + (size_t)yy * W + xx, qi, i);
+            }
+        }
+    }
+}
+
+// Four float16 values (8 bytes, low half first) as float32, exactly
+__device__ __forceinline__ float4 to_float4(float4 v) { return v; }
+__device__ __forceinline__ float4 to_float4(uint2 v) {
+    const float2 a = __half22float2(*reinterpret_cast<const __half2*>(&v.x));
+    const float2 b = __half22float2(*reinterpret_cast<const __half2*>(&v.y));
+    return make_float4(a.x, a.y, b.x, b.y);
+}
+
+// The backward's per-(tile, block) instance lists need no counting pass: block b of a tile owns entries
+// [list_begin(range.x, range.y, b), ... + len), len = range.y - range.x, because an instance of the tile's list appears at most once
+// per block.
+__device__ __forceinline__ size_t list_begin(uint32_t begin, uint32_t end, int b) {
+    return kBlocksPerTile * (size_t)begin + (size_t)b * (end - begin);
+}
+
+// Splat alpha at pixel (pxf, pyf), with the reference's expression trees (forward.cu:340-351, backward.cu:525-535): plain
+// fp32, no _rn intrinsics (see common.cuh).  alpha is 0 where the reference skips the pair (power > 0 or alpha < 1/255)
+// and where !valid.
+struct SplatAlpha {
+    float dx, dy, G, alpha;
 };
+__device__ __forceinline__ SplatAlpha splat_alpha(const float4 r0, const float4 r1, float pxf, float pyf, bool valid) {
+    SplatAlpha s;
+    s.dx = r0.x - pxf;
+    s.dy = r0.y - pyf;
+    const float power = -0.5f * (r1.x * s.dx * s.dx + r1.z * s.dy * s.dy) - r1.y * s.dx * s.dy;
+    s.G = expf(power);
+    const float av = fminf(0.99f, r1.w * s.G);
+    s.alpha = (valid && !(power > 0.0f) && !(av < 1.0f / 255.0f)) ? av : 0.f;
+    return s;
+}
 
 // Can the region where alpha >= 1/255 reach the pixel rectangle [x0,x1] x [y0,y1] (pixel-centre coordinates)?
 // r0 = {x, y, ex, ey}, r1 = {conic a, b, c, opacity} of the splat record.  Conservative in both steps: a pair this returns
@@ -128,10 +239,6 @@ __device__ __forceinline__ bool footprint_hits_rect(const float4 r0, const float
     }
     return q <= tau;
 }
-
-// pixel <-> lane mapping inside a block: 2x2 quads, quad q = lane>>2 laid out 4 across
-__device__ __forceinline__ int lane_px(int lane) { return ((lane >> 2) & 3) * 2 + (lane & 1); }
-__device__ __forceinline__ int lane_py(int lane) { return (lane >> 4) * 2 + ((lane >> 1) & 1); }
 
 template <int N>
 __device__ __forceinline__ void reg_dec() {
@@ -183,6 +290,40 @@ struct ProducerArgs {
     int tiles_x, num_tiles, chunks;
     int use_bulk;
 };
+
+// The producer's view of vp without feature rows (C = 0, one chunk, no bulk copies); the forward adds its feature fields.
+inline ProducerArgs producer_args(const ViewParams& vp, const uint2* ranges, const uint32_t* point_list,
+                                  const SplatRec* rec, const uint32_t* n_contrib, int* work_counter) {
+    return ProducerArgs{ranges, point_list, rec, nullptr, n_contrib, work_counter, vp.W, vp.H, 0, (int)vp.grid_x,
+                        (int)(vp.grid_x * vp.grid_y), 1, 0};
+}
+
+// Channels per work item of the kernels that keep a block's 32 pixels x 4 channels per lane: one of the instantiated
+// 32 / 64 / 128; wider features are split into chunks of 128.
+inline int channel_chunk(int C) { return C <= 32 ? 32 : (C <= 64 ? 64 : 128); }
+
+// SM count of the current device.  The first call for a device ordinal also opts the kernels K in to `smem` bytes of
+// dynamic shared memory: the opt-in is per device (context), so the count is remembered per ordinal and one process
+// driving several GPUs works too.  A failed opt-in is returned and retried on the next call; an ordinal of 64 or more
+// returns cudaErrorInvalidDevice and leaves `sms` as it is.
+template <auto... K>
+cudaError_t device_sms(int& sms, size_t smem) {
+    static std::atomic<int> sms_of_device[64];  // zero-initialised; set once per device (idempotent)
+    int dev = 0;
+    cudaGetDevice(&dev);
+    if (dev < 0 || dev >= 64) return cudaErrorInvalidDevice;
+    if (sms_of_device[dev].load() == 0) {
+        for (const void* k : std::initializer_list<const void*>{reinterpret_cast<const void*>(K)...}) {
+            const cudaError_t e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+            if (e != cudaSuccess) return e;
+        }
+        int n = 0;
+        cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
+        sms_of_device[dev].store(n > 0 ? n : 132);
+    }
+    sms = sms_of_device[dev].load();
+    return cudaSuccess;
+}
 
 // Producer warp: persistent over work items.  REVERSE: walk each list back to front (backward pass).
 // With features (CH > 0) the producer only walks, culls and compacts; it hands each stage's id list to copy_loop() (a

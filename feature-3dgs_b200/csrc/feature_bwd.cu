@@ -2,9 +2,7 @@
 //
 // The geometric-gradient kernel (composite_bwd.cu, alpha-only layout at two CTAs per SM) appends, per (tile, 8x4 block), one
 // list entry per instance that blended at least one pixel of the block: {Gaussian id, pixel mask} + the 32 blend weights
-// w = alpha * T (136 bytes per entry, ~6.0 M entries = 0.8 GB per view at config 3, back to front).  Lists need no counting
-// pass: block b of tile t owns entries [8*range.x + b*len, ... + len), len = range.y - range.x (an instance of the tile
-// list appears at most once per block).
+// w = alpha * T (136 bytes per entry, ~6.0 M entries = 0.8 GB per view at config 3, back to front), laid out by list_begin.
 //
 // feature_bwd_kernel<CH> (here): every warp is an independent worker that pulls (tile, channel chunk, block) items from an
 // atomic counter, keeps the block's upstream gradient dL/dfeature_map (32 pixels x 4 channels per lane) in registers,
@@ -29,18 +27,18 @@ struct alignas(128) FeatSmem {  // per warp
     float w[2][kListChunk][32];
 };
 
+template <typename TG>  // TG: element type of the upstream gradient map, float or __half
 struct FeatArgs {
     const uint2* ranges;
     const float* list_w;
     const uint2* list_meta;
     const uint32_t* list_cnt;
-    const float* dL_dfeat_pix;  // backward: [C, H, W]
-    float* dL_dfeature;         // backward: [P, C]
+    const TG* dL_dfeat_pix;  // backward: [C, H, W]
+    float* dL_dfeature;      // backward: [P, C]
     int* work_counter;
     int W, H, C, tiles_x, num_tiles, chunks;
     int vec;  // bit0: gradient rows are 16-byte aligned and C % 4 == 0; bit1: 4-pixel vector loads of image rows
-    // a float16 upstream gradient instead of dL_dfeat_pix: dL/dO = scale * float(map), one fp32 multiply rounded to nearest
-    const __half* dL_dfeat_pix_h;
+    // a float16 map stands for dL/dO = scale * float(map), one fp32 multiply rounded to nearest; not read for float
     float scale;
 };
 
@@ -58,15 +56,16 @@ __device__ __forceinline__ void cp_async_wait() {
 struct ItemPos {
     int tile, chunk, b, bx0, by0;
 };
-__device__ __forceinline__ ItemPos decode_item(int item, const FeatArgs& a) {
+template <typename TG>
+__device__ __forceinline__ ItemPos decode_item(int item, const FeatArgs<TG>& a) {
     ItemPos p;
     p.b = item & (kBlocksPerTile - 1);
     const int tc = item / kBlocksPerTile;
     p.chunk = tc % a.chunks;
     p.tile = tc / a.chunks;
     const int tile_x = p.tile % a.tiles_x, tile_y = p.tile / a.tiles_x;
-    p.bx0 = tile_x * 16 + (p.b & 1) * 8;
-    p.by0 = tile_y * 16 + (p.b >> 1) * 4;
+    p.bx0 = block_x0(tile_x, p.b);
+    p.by0 = block_y0(tile_y, p.b);
     return p;
 }
 
@@ -76,16 +75,15 @@ __device__ __forceinline__ float4 ld_dO4(const float* p, float) { return ld_nc_f
 __device__ __forceinline__ float4 ld_dO4(const __half* p, float s) {
     uint32_t u0, u1;
     asm volatile("ld.global.nc.L1::no_allocate.v2.u32 {%0,%1}, [%2];" : "=r"(u0), "=r"(u1) : "l"(p));
-    const float2 a = __half22float2(*reinterpret_cast<const __half2*>(&u0));
-    const float2 b = __half22float2(*reinterpret_cast<const __half2*>(&u1));
-    return make_float4(__fmul_rn(a.x, s), __fmul_rn(a.y, s), __fmul_rn(b.x, s), __fmul_rn(b.y, s));
+    const float4 v = to_float4(make_uint2(u0, u1));
+    return make_float4(__fmul_rn(v.x, s), __fmul_rn(v.y, s), __fmul_rn(v.z, s), __fmul_rn(v.w, s));
 }
 __device__ __forceinline__ float ld_dO1(const float* p, float) { return __ldg(p); }
 __device__ __forceinline__ float ld_dO1(const __half* p, float s) { return __fmul_rn(__half2float(__ldg(p)), s); }
 
 // ------------------------------------------------------------------------------------------------ backward
-template <int CH, typename TG>  // TG: element type of the upstream gradient map, float or __half
-__global__ void __launch_bounds__(kFeatWarps * 32, 3) feature_bwd_kernel(const FeatArgs a) {
+template <int CH, typename TG>
+__global__ void __launch_bounds__(kFeatWarps * 32, 3) feature_bwd_kernel(const FeatArgs<TG> a) {
     extern __shared__ __align__(128) unsigned char smem_raw[];
     const int warp = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0), lane = threadIdx.x & 31;
     FeatSmem& sm = reinterpret_cast<FeatSmem*>(smem_raw)[warp];
@@ -107,7 +105,7 @@ __global__ void __launch_bounds__(kFeatWarps * 32, 3) feature_bwd_kernel(const F
         // trip counts and branches: no reconvergence pairs around the quad tests)
         const uint32_t rx = __shfl_sync(0xffffffffu, a.ranges[ip.tile].x, 0);
         const uint32_t ry = __shfl_sync(0xffffffffu, a.ranges[ip.tile].y, 0);
-        const size_t base = 8 * (size_t)rx + (size_t)ip.b * (ry - rx);
+        const size_t base = list_begin(rx, ry, ip.b);
         const uint32_t n = __shfl_sync(0xffffffffu, a.list_cnt[(size_t)ip.tile * kBlocksPerTile + ip.b], 0);
         if (n == 0) continue;
         const int ch0 = ip.chunk * CH + cl * 4;
@@ -129,7 +127,6 @@ __global__ void __launch_bounds__(kFeatWarps * 32, 3) feature_bwd_kernel(const F
         // upstream gradient of the block's 32 pixels x 4 channels: [quad][pixel pair][channel]: the two pixels of a
         // quad row share a 64-bit register pair, as do their weights in the LDS.128
         float2 dO2[NQ][2][4];
-#define DOB(q, i, c) (((i) & 1) ? dO2[q][(i) >> 1][c].y : dO2[q][(i) >> 1][c].x)
 #pragma unroll
         for (int q = 0; q < NQ; q++)
 #pragma unroll
@@ -140,41 +137,11 @@ __global__ void __launch_bounds__(kFeatWarps * 32, 3) feature_bwd_kernel(const F
         for (int c = 0; c < 4; c++) {
             const int ch = ch0 + c;
             if (ch >= C) continue;
-            const TG* plane;
-            if constexpr (std::is_same_v<TG, float>)
-                plane = a.dL_dfeat_pix + (size_t)ch * HW;
-            else
-                plane = a.dL_dfeat_pix_h + (size_t)ch * HW;
-            if (G == 1 && (a.vec & 2)) {
-#pragma unroll
-                for (int y = 0; y < 4; y++) {
-                    const int yy = ip.by0 + y;
-                    if (yy >= H) continue;
-#pragma unroll
-                    for (int half = 0; half < 2; half++) {
-                        const int xx = ip.bx0 + half * 4;
-                        if (xx >= W) continue;
-                        const int qa = (y >> 1) * 4 + half * 2, i0 = (y & 1) * 2;
-                        const float4 v = ld_dO4(plane + (size_t)yy * W + xx, a.scale);
-                        DOB(qa % NQ, i0, c) = v.x;
-                        DOB(qa % NQ, i0 + 1, c) = v.y;
-                        DOB((qa + 1) % NQ, i0, c) = v.z;
-                        DOB((qa + 1) % NQ, i0 + 1, c) = v.w;
-                    }
-                }
-            } else {
-#pragma unroll
-                for (int qi = 0; qi < NQ; qi++) {
-                    const int q = qi * G + grp;
-#pragma unroll
-                    for (int i = 0; i < 4; i++) {
-                        const int xx = ip.bx0 + (q & 3) * 2 + (i & 1), yy = ip.by0 + (q >> 2) * 2 + (i >> 1);
-                        if (xx < W && yy < H) DOB(qi, i, c) = ld_dO1(plane + (size_t)yy * W + xx, a.scale);
-                    }
-                }
-            }
+            for_tile_pixels<G, NQ>(
+                a.dL_dfeat_pix + (size_t)ch * HW, ip.bx0, ip.by0, W, H, grp, false, a.vec & 2, [](const TG*, int) {},
+                [&](const TG* p, int y, int half) { set_tile_run(dO2, y, half, c, ld_dO4(p, a.scale)); },
+                [&](const TG* p, int qi, int i) { tile_px(dO2, qi, i, c) = ld_dO1(p, a.scale); });
         }
-#undef DOB
 
         for (uint32_t c = 0; c < nch; c++) {
             const int buf = c & 1;
@@ -232,46 +199,30 @@ __global__ void __launch_bounds__(kFeatWarps * 32, 3) feature_bwd_kernel(const F
 }
 
 // ------------------------------------------------------------------------------------------------ launchers
-static int workers_grid() {
-    static std::atomic<int> sms_of_device[64];  // zero-initialised; set once per device (idempotent)
-    int dev = 0;
-    cudaGetDevice(&dev);
-    if (dev < 0 || dev >= 64) return 132 * 3;
-    if (sms_of_device[dev].load() == 0) {
-        int n = 0;
-        cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-        sms_of_device[dev].store(n > 0 ? n : 132);
-    }
-    return sms_of_device[dev].load() * 3;  // __launch_bounds__(128, 3): three CTAs of four workers per SM
-}
-
 template <int CH, typename TG>
-static cudaError_t launch_feat_bwd_t(const FeatArgs& a, cudaStream_t s) {
-    const size_t smem = kFeatWarps * sizeof(FeatSmem);
+static cudaError_t launch_feat_bwd_t(const FeatArgs<TG>& a, cudaStream_t s) {
+    const size_t smem = kFeatWarps * sizeof(FeatSmem);  // under 48 KB: no opt-in
+    int sms = 132;  // kept for a device ordinal device_sms does not cover
+    device_sms<>(sms, smem);
     const int items = a.num_tiles * a.chunks * kBlocksPerTile;
-    const int grid = min((items + kFeatWarps - 1) / kFeatWarps, workers_grid());
+    // __launch_bounds__(128, 3): three CTAs of four workers per SM
+    const int grid = min((items + kFeatWarps - 1) / kFeatWarps, sms * 3);
     feature_bwd_kernel<CH, TG><<<grid, kFeatWarps * 32, smem, s>>>(a);
     g_launches++;
     return cudaGetLastError();
 }
 
-static int feat_ch(int C) { return C <= 32 ? 32 : (C <= 64 ? 64 : 128); }
-
 template <typename TG>
 cudaError_t launch_feature_bwd(const ViewParams& vp, const uint2* ranges, const float* list_w, const uint2* list_meta,
                                const uint32_t* list_cnt, const TG* dL_dfeat_pix, float dL_dfeat_pix_scale,
                                float* dL_dfeature, int* work_counter, cudaStream_t s) {
-    FeatArgs a;
+    FeatArgs<TG> a;
     a.ranges = ranges; a.list_w = list_w; a.list_meta = list_meta; a.list_cnt = list_cnt;
-    if constexpr (std::is_same_v<TG, float>) {
-        a.dL_dfeat_pix = dL_dfeat_pix; a.dL_dfeat_pix_h = nullptr;
-    } else {
-        a.dL_dfeat_pix = nullptr; a.dL_dfeat_pix_h = dL_dfeat_pix;
-    }
+    a.dL_dfeat_pix = dL_dfeat_pix;
     a.dL_dfeature = dL_dfeature; a.scale = dL_dfeat_pix_scale;
     a.work_counter = work_counter;
     a.W = vp.W; a.H = vp.H; a.C = vp.C; a.tiles_x = (int)vp.grid_x; a.num_tiles = (int)(vp.grid_x * vp.grid_y);
-    const int CH = feat_ch(vp.C);
+    const int CH = channel_chunk(vp.C);
     a.chunks = (vp.C + CH - 1) / CH;
     a.vec = 0;
     if (vp.C % 4 == 0 && (reinterpret_cast<uintptr_t>(dL_dfeature) & 15) == 0) a.vec |= 1;
