@@ -16,13 +16,16 @@
 //                         the T recurrence, RGB/depth (and in the backward every geometric gradient
 //                         term).  In the forward they publish the blend weights w = alpha*T as a
 //                         [instance][pixel] tile plus a per-instance pixel mask in a small per-block
-//                         ring (`wfull`/`wempty`).
-//   feature warps (8)     forward only: warp b consumes block b's weight tiles with one float4 of
-//                         channels per lane; all 32 pixels x 4 channels of the block stay in
+//                         ring (`wfull`/`wempty`), and per 8x2 half of the block a mask of the
+//                         instances that blended a pixel there.
+//   feature warps (16)    forward only: a pair per block.  Warp h of block b's pair owns rows 2h and
+//                         2h+1 of the block (quads 4h..4h+3, pixel-mask bits 16h..16h+15) and consumes
+//                         the entries of block b's weight tiles that blended a pixel of that half, with
+//                         one float4 of channels per lane; the half's 16 pixels x 4 channels stay in
 //                         registers, and the weights arrive as broadcast LDS.128 per 2x2 pixel quad.
 //
-// The forward launches all 20 warps (composite_fwd.cu); the backward geometry kernel launches the
-// producer group and the alpha warps only (composite_bwd.cu).
+// The forward with features launches all 28 warps (composite_fwd.cu; without features, 20 warps with no feature warp
+// doing any work); the backward geometry kernel launches the producer group and the alpha warps only (composite_bwd.cu).
 #pragma once
 #include <initializer_list>
 
@@ -34,7 +37,7 @@ constexpr int kBlocksPerTile = 8;   // 8x4-pixel blocks in a 16x16 tile
 constexpr int kProducerWarp = 0;    // warps 0..3: producer warpgroup
 constexpr int kAlphaWarp0 = 4;      // then one alpha warp per pixel block
 constexpr int kAlphaWarps = kBlocksPerTile;
-constexpr int kFeatWarp0 = kAlphaWarp0 + kAlphaWarps;  // then one feature warp per pixel block (forward)
+constexpr int kFeatWarp0 = kAlphaWarp0 + kAlphaWarps;  // then two feature warps per pixel block (forward)
 constexpr int kRegsProducer = 40;   // setmaxnreg of the producer group
 constexpr int kStageEntries = 32;
 constexpr int kStages = 6;
@@ -62,11 +65,12 @@ struct alignas(128) Stage {
 struct alignas(128) WSlot {
     float w[kStageEntries][32];    // blend weights [instance][pixel of the block]
     uint32_t pm[kStageEntries];    // per instance: which pixels blended
-    uint32_t km;                   // which instances have pm != 0
+    uint32_t km[2];                // km[h]: which instances blended a pixel of rows 2h, 2h+1 (pm bits 16h..16h+15)
     uint32_t last;
     uint32_t first;
     int32_t work;
 };
+static_assert(sizeof(WSlot) == 4352, "weight slot layout changed");  // 4244 bytes of fields, padded to 128
 
 // WB x WJ: dimensions of the weight-slot ring (pixel blocks x slots per block)
 template <int CH, typename TF = float, int WB = kBlocksPerTile, int WJ = kWSlots>
@@ -108,12 +112,12 @@ __device__ __forceinline__ int slot_py(int p) { return (p >> 4) * 2 + ((p >> 1) 
 
 // Register tile of a feature lane: float2 t[NQ][2][4] = [quad][quad row][channel], the two pixels of a quad row in .x
 // and .y (one paired FMA covers both).  With CH / 4 lanes per feature row, G = 32 / (CH / 4) lane groups share the
-// block's 8 quads: group grp holds quads qi * G + grp, qi < NQ = 8 / G.
+// tile's quads (8 for a whole block, 4 for an 8x2 half): group grp holds quads qi * G + grp, qi < NQ = 8 / G (or 4 / G).
 template <int NQ>
 __device__ __forceinline__ float& tile_px(float2 (&t)[NQ][2][4], int qi, int i, int c) {
     return (i & 1) ? t[qi][i >> 1][c].y : t[qi][i >> 1][c].x;
 }
-// Pixel k of the run of pixels 4 * half .. 4 * half + 3 in row y of the block, for a lane that holds all 8 quads
+// Pixel k of the run of pixels 4 * half .. 4 * half + 3 in row y of the register tile, for a lane that holds all its quads
 // (G == 1).  (% NQ only keeps the indices in range in the instantiations with G > 1, which never get here.)
 template <int NQ>
 __device__ __forceinline__ float& tile_run_px(float2 (&t)[NQ][2][4], int y, int half, int k, int c) {
@@ -137,19 +141,22 @@ __device__ __forceinline__ void set_tile_run(float2 (&t)[NQ][2][4], int y, int h
 //   row(p, y)           8-pixel row y: G == 1, `rows` (8-pixel alignment of the plane) and the row inside the image
 //   run(p, y, half)     4-pixel run: G == 1 and `runs` (4-pixel alignment)
 //   px(p, qi, i)        otherwise pixel i of the lane's quad qi, one at a time
-template <int G, int NQ, typename T, class Row, class Run, class Px>
+// NY: rows of the register tile, image rows by0 .. by0 + NY - 1.  NY = 2 is one 8x2 half of a block (quads 0..3 of the
+// register tile, NQ * G = 4), with by0 the half's first row.
+template <int G, int NQ, int NY = 4, typename T, class Row, class Run, class Px>
 __device__ __forceinline__ void for_tile_pixels(T* plane, int bx0, int by0, int W, int H, int grp, bool rows, bool runs,
                                                 Row row, Run run, Px px) {
+    static_assert(NQ * G * 2 == NY * 4, "a register tile of NQ quads per lane group covers NY rows of 8 pixels");
     if (G == 1 && rows && bx0 + 8 <= W) {
 #pragma unroll
-        for (int y = 0; y < 4; y++) {
+        for (int y = 0; y < NY; y++) {
             const int yy = by0 + y;
             if (yy >= H) continue;
             row(plane + (size_t)yy * W + bx0, y);
         }
     } else if (G == 1 && runs) {
 #pragma unroll
-        for (int y = 0; y < 4; y++) {
+        for (int y = 0; y < NY; y++) {
             const int yy = by0 + y;
             if (yy >= H) continue;
 #pragma unroll
@@ -250,7 +257,8 @@ __device__ __forceinline__ void reg_inc() {
 }
 
 template <int CH, typename RING>
-__device__ __forceinline__ void ring_init(RING& ring, int n_stage_consumers, int n_full_arrivals = 1) {
+__device__ __forceinline__ void ring_init(RING& ring, int n_stage_consumers, int n_full_arrivals = 1,
+                                          int n_wslot_consumers = 1) {
     // called by all threads before the role split; followed by __syncthreads()
     if (threadIdx.x == 0) {
         for (int s = 0; s < kStages; s++) {
@@ -261,7 +269,7 @@ __device__ __forceinline__ void ring_init(RING& ring, int n_stage_consumers, int
         for (int b = 0; b < RING::kWB; b++)
             for (int j = 0; j < RING::kWJ; j++) {
                 mbar_init(&ring.wfull[b][j], 1);
-                mbar_init(&ring.wempty[b][j], 1);
+                mbar_init(&ring.wempty[b][j], n_wslot_consumers);
             }
         for (int i = 0; i < kDoneSlots; i++) ring.done_mask[i] = 0;
         mbar_fence_init();

@@ -10,12 +10,20 @@
 // Roles (composite_common.cuh): producer + copy warp -> alpha warps -> feature warps, persistent over tiles.
 //   alpha warp b   lane = pixel of block b.  For every staged instance whose footprint reaches
 //                  the block: alpha, T update, RGB/depth accumulate; publishes w = alpha*T as a
-//                  [instance][pixel] tile + a 32-bit "which pixels blended" mask per instance.
-//   feature warp b lane = float4 of channels.  acc[pixel][4] += w[pixel] * f[4] for the pixels in
-//                  the mask, one 2x2-pixel quad at a time: one broadcast LDS.128 of the quad's weights
-//                  feeds paired FMAs on the quad rows that blended; the next instance's mask and feature
-//                  float4 are loaded during this one's FMAs.  All 32 pixels x 4 channels (= 128
-//                  accumulators per lane at CH = 128) live in registers.
+//                  [instance][pixel] tile + a 32-bit "which pixels blended" mask per instance, and
+//                  two instance masks: which instances blended a pixel of rows 0-1 / rows 2-3.
+//   feature warps  a pair per block: warp (b, h) owns the 8x2 half of block b made of rows 2h and
+//   (b, h)         2h+1 (quads 4h..4h+3, mask bits 16h..16h+15); lane = float4 of channels.  It walks
+//                  the instances of its half's mask and does acc[pixel][4] += w[pixel] * f[4] for the
+//                  pixels of its half that blended, one 2x2-pixel quad at a time: one broadcast LDS.128
+//                  of the quad's weights feeds the FMAs of the quad rows that blended; the next
+//                  instance's mask and feature float4 are loaded during this one's FMAs.  The half's 16
+//                  pixels x 4 channels (= 64 accumulators per lane at CH = 128) live in registers.
+//                  Every accumulator sees the same FMAs in the same order as with one warp per block
+//                  (an instance a warp skips adds nothing to its pixels), so the map is bitwise the
+//                  same.  Hopper has no paired FP32 FMA (fma2_rn is two FFMAs): with one warp per block
+//                  the feature FMAs cost 0.50 ms of 2.67 ms at config 3; with the pair, issued on two
+//                  sub-partitions and skipping the other half's entries, 0.15 ms of 2.32 ms (README).
 // Channel counts above 128 are split into chunks of 128 (extra work items); chunk 0 also writes
 // colour, depth, final_T and n_contrib.
 //
@@ -25,17 +33,23 @@
 // is bitwise the float32 render of the upcast features followed by .half(), and everything else is bitwise the float32
 // render's (the alpha warps never read features).
 //
-// Registers: the 20 warps are launched at 96 registers per thread (61440 in the CTA pool); setmaxnreg then gives the
-// producer group 40, the alpha warps 64 and the feature warps 152 (4x32x40 + 8x32x64 + 8x32x152 = 60416).
+// Registers: with features the 28 warps are launched at 72 registers per thread (64512 in the CTA pool); setmaxnreg
+// then gives the producer group 40, the alpha warps 56 and the feature warps 88 (4x32x40 + 8x32x56 + 16x32x88 =
+// 64512).  (setmaxnreg acts per warpgroup of 4 consecutive warps, so the producer group is one unit.)  Without
+// features the 20 warps are launched at 96, and the producer group gets 40 and the alpha warps 64.
 #include <type_traits>
 
 #include "composite_common.cuh"
 
 namespace f3dgs {
 
-constexpr int kFwdThreads = (kFeatWarp0 + kBlocksPerTile) * 32;
-constexpr int kRegsAlpha = 64;
-constexpr int kRegsFeature = 152;
+// With features: the producer group, 8 alpha warps and 16 feature warps.  Without features the kernel keeps its
+// 20-warp launch (the 8 warps after the alpha warps return at once).
+template <int CH>
+constexpr int kFwdThreads = (kFeatWarp0 + (CH > 0 ? 2 : 1) * kBlocksPerTile) * 32;
+template <int CH>
+constexpr int kRegsAlpha = CH > 0 ? 56 : 64;
+constexpr int kRegsFeature = 88;
 
 template <typename TF>
 struct FwdArgs {
@@ -71,7 +85,7 @@ __device__ __forceinline__ void st_px(float* p, float v) { *p = v; }
 __device__ __forceinline__ void st_px(__half* p, float v) { *p = __float2half_rn(v); }
 
 template <int CH, typename TF>
-__global__ void __launch_bounds__(kFwdThreads, 1)
+__global__ void __launch_bounds__(kFwdThreads<CH>, 1)
 composite_fwd_kernel(const FwdArgs<TF> args) {
     extern __shared__ __align__(128) unsigned char smem_raw[];
     using RING = RingV2<CH, TF>;
@@ -84,7 +98,7 @@ composite_fwd_kernel(const FwdArgs<TF> args) {
     const int W = args.pa.W, H = args.pa.H, C = args.pa.C;
     const size_t HW = (size_t)H * W;
 
-    ring_init<CH>(ring, CH > 0 ? kAlphaWarps + kBlocksPerTile : kAlphaWarps, CH > 0 ? 2 : 1);
+    ring_init<CH>(ring, CH > 0 ? kAlphaWarps + 2 * kBlocksPerTile : kAlphaWarps, CH > 0 ? 2 : 1, CH > 0 ? 2 : 1);
     __syncthreads();
 
     // ======================================================================== producer group
@@ -100,7 +114,7 @@ composite_fwd_kernel(const FwdArgs<TF> args) {
 
     // ======================================================================== alpha warps
     if (warp < kFeatWarp0) {
-        reg_dec<kRegsAlpha>();
+        reg_dec<kRegsAlpha<CH>>();
         const int b = warp - kAlphaWarp0;  // owns pixel block b
         int s = 0, j = 0;
         uint32_t parity = 0, wparity = 1;  // wempty: fresh barrier falls through on parity 1
@@ -132,7 +146,7 @@ composite_fwd_kernel(const FwdArgs<TF> args) {
             }
             WSlot* ws = &ring.ws[b][j];
             if (CH > 0) mbar_wait(&ring.wempty[b][j], wparity);
-            uint32_t km = 0;
+            uint32_t km0 = 0, km1 = 0;  // instances that blended a pixel of rows 0-1 / rows 2-3
             if (!blk_done && n > 0) {
                 bool hit = false;
                 if (lane < n) hit = footprint_hits_rect(st.rec0[lane], st.rec1[lane], fbx0, fbx0 + 7.f, fby0, fby0 + 3.f);
@@ -178,7 +192,8 @@ composite_fwd_kernel(const FwdArgs<TF> args) {
                         if (CH > 0) {
                             ws->w[kk[u]][lane] = wgt;
                             if (lane == 0) ws->pm[kk[u]] = pm;
-                            km |= (pm ? 1u : 0u) << kk[u];
+                            km0 |= ((pm & 0xFFFFu) ? 1u : 0u) << kk[u];
+                            km1 |= ((pm >> 16) ? 1u : 0u) << kk[u];
                         }
                     }
                 }
@@ -190,7 +205,8 @@ composite_fwd_kernel(const FwdArgs<TF> args) {
             if (CH > 0) {
                 __syncwarp();
                 if (lane == 0) {
-                    ws->km = km;
+                    ws->km[0] = km0;
+                    ws->km[1] = km1;
                     ws->last = last;
                     ws->first = first;
                     ws->work = work;
@@ -211,11 +227,11 @@ composite_fwd_kernel(const FwdArgs<TF> args) {
             if (++s == kStages) { s = 0; parity ^= 1; }
             if (CH > 0 && ++j == kWSlots) { j = 0; wparity ^= 1; }
         }
-        if (CH > 0) {  // tell the feature warp of this block that the work is over
+        if (CH > 0) {  // tell the feature warps of this block that the work is over
             mbar_wait(&ring.wempty[b][j], wparity);
             if (lane == 0) {
                 ring.ws[b][j].work = -1;
-                ring.ws[b][j].km = 0;
+                ring.ws[b][j].km[0] = ring.ws[b][j].km[1] = 0;
                 mbar_arrive(&ring.wfull[b][j]);
             }
         }
@@ -227,9 +243,13 @@ composite_fwd_kernel(const FwdArgs<TF> args) {
     reg_inc<kRegsFeature>();
     {  // own scope: ending the accumulators' lifetime here keeps the instruction schedule the kernel was tuned with
         constexpr int LPR = CH > 0 ? CH / 4 : 32;  // lanes per feature row
-        constexpr int G = 32 / LPR;                // lane groups sharing the 32 pixels
-        constexpr int NQ = 8 / G;                  // 2x2 quads per lane
-        const int b = warp - kFeatWarp0;
+        constexpr int G = 32 / LPR;                // lane groups sharing the half's 16 pixels
+        constexpr int NQ = 4 / G;                  // 2x2 quads of the warp's 8x2 half per lane
+        // Warps kFeatWarp0 + 2b and + 2b + 1 are block b's pair.  Warp w runs on sub-partition w % 4, so each
+        // sub-partition holds four feature warps: the upper halves (h = 0) of the even blocks on sub-partition 0, the
+        // lower halves of the even blocks on 1, and the odd blocks' halves on 2 and 3.  The two halves of a block run on
+        // different sub-partitions.
+        const int b = (warp - kFeatWarp0) >> 1, h = (warp - kFeatWarp0) & 1;
         const int grp = lane / LPR, cl = lane % LPR;
         // Accumulators [quad][pixel pair (row of the 2x2 quad)][channel]: the two pixels of a quad row share a 64-bit register
         // pair and one paired FMA (fma2_rn: feature channel broadcast x weight pair + accumulator pair) covers both; each half
@@ -255,7 +275,7 @@ composite_fwd_kernel(const FwdArgs<TF> args) {
             const WSlot& ws = ring.ws[b][j];
             const int work = ws.work;
             if (work < 0) break;
-            uint32_t km = ws.km;
+            uint32_t km = ws.km[h];
             const uint32_t last = ws.last;
             mbar_wait(&ring.full[s], parity);  // feature rows landed
             const Stage<CH, TF>& st = ring.stage[s];
@@ -266,7 +286,7 @@ composite_fwd_kernel(const FwdArgs<TF> args) {
             Feat4<TF> f_n = *reinterpret_cast<const Feat4<TF>*>(&st.feat[kn][cl * 4]);
             while (km) {
                 const int k = kn;
-                const uint32_t pm = pm_n;
+                const uint32_t pm = pm_n >> (16 * h);  // the half's pixels: quad q of the half in bits 4q..4q+3
                 const float4 f = to_float4(f_n);
                 km &= km - 1;
                 kn = km ? __ffs(km) - 1 : k;
@@ -276,7 +296,7 @@ composite_fwd_kernel(const FwdArgs<TF> args) {
                 for (int qi = 0; qi < NQ; qi++) {
                     const int q = qi * G + grp;
                     if ((pm >> (4 * q)) & 0xFu) {
-                        const float4 w4 = *reinterpret_cast<const float4*>(&ws.w[k][4 * q]);
+                        const float4 w4 = *reinterpret_cast<const float4*>(&ws.w[k][16 * h + 4 * q]);
                         // a pixel that did not blend has w = 0 and adds +0: skipping its FMAs leaves every accumulator
                         // bit-identical (fma(f, +0, acc) == acc for finite f; acc is never -0 because it starts at +0)
                         if ((pm >> (4 * q)) & 0x3u) FEAT_ROW_FMA(qi, 0, make_float2(w4.x, w4.y));
@@ -290,15 +310,15 @@ composite_fwd_kernel(const FwdArgs<TF> args) {
                 mbar_arrive(&ring.empty[s]);
             }
             if (last) {
-                // ---- epilogue of this work item: write the block's 32 pixels x CH channels, reset
+                // ---- epilogue of this work item: write the half's 16 pixels x CH channels, reset
                 const int tile = work / args.pa.chunks, chunk = work - tile * args.pa.chunks;
                 const int tile_x = tile % args.pa.tiles_x, tile_y = tile / args.pa.tiles_x;
-                const int bx0 = block_x0(tile_x, b), by0 = block_y0(tile_y, b);
+                const int bx0 = block_x0(tile_x, b), by0 = block_y0(tile_y, b) + 2 * h;
 #pragma unroll
                 for (int c = 0; c < 4; c++) {
                     const int ch = chunk * CH + cl * 4 + c;
                     if (ch < C)
-                        for_tile_pixels<G, NQ>(
+                        for_tile_pixels<G, NQ, 2>(
                             args.out_feature + (size_t)ch * HW, bx0, by0, W, H, grp, args.vec_store & 2,
                             args.vec_store & 1,
                             [&](TF* p, int y) { st_row(p, tile_run(acc2, y, 0, c), tile_run(acc2, y, 1, c)); },
@@ -346,7 +366,7 @@ static cudaError_t launch_fwd_t(const ViewParams& vp, const uint2* ranges, const
     e = cudaMemsetAsync(work_counter, 0, sizeof(int), s);
     if (e != cudaSuccess) return e;
     const int grid = min(a.pa.num_tiles * a.pa.chunks, num_sms);
-    composite_fwd_kernel<CH, TF><<<grid, kFwdThreads, smem, s>>>(a);
+    composite_fwd_kernel<CH, TF><<<grid, kFwdThreads<CH>, smem, s>>>(a);
     g_launches++;
     return cudaGetLastError();
 }
