@@ -149,6 +149,27 @@ struct ListLayout {
     }
 };
 
+// Stream-ordered scratch for the instance lists (the reference's backward allocates its scratch too,
+// rasterizer_impl.cu:402-430); the default pool keeps freed blocks, so steady-state calls do not reach the driver.
+// The caller releases them with cudaFreeAsync on the same stream.
+int alloc_lists(const Api& api, const ListLayout& ll, char** lists, cudaStream_t stream) {
+    static std::once_flag once;
+    std::call_once(once, [] {
+        int dev = 0;
+        cudaGetDevice(&dev);
+        cudaMemPool_t pool;
+        if (cudaDeviceGetDefaultMemPool(&pool, dev) == cudaSuccess) {
+            unsigned long long keep = ~0ull;
+            cudaMemPoolSetAttribute(pool, cudaMemPoolAttrReleaseThreshold, &keep);
+        }
+    });
+    const cudaError_t ea = cudaMallocAsync((void**)lists, ll.bytes, stream);
+    if (ea != cudaSuccess)
+        return api.fail(F3DGS_ERR_ALLOC, "cudaMallocAsync of " + std::to_string(ll.bytes) +
+                                             " bytes for the instance lists failed: " + cudaGetErrorString(ea));
+    return 0;
+}
+
 inline int bit_length(uint32_t n) {
     int b = 0;
     while (n) {
@@ -476,23 +497,7 @@ int backward_impl(const Api& api, bool accumulate, int P, int D, int M, int R, i
         char* lists = nullptr;
         const ListLayout ll((size_t)R, tiles);
         if (C > 0 && R > 0) {
-            // stream-ordered scratch (the reference's backward allocates its scratch too, rasterizer_impl.cu:402-430);
-            // the default pool keeps freed blocks, so steady-state calls do not reach the driver
-            static std::once_flag once;
-            std::call_once(once, [] {
-                int dev = 0;
-                cudaGetDevice(&dev);
-                cudaMemPool_t pool;
-                if (cudaDeviceGetDefaultMemPool(&pool, dev) == cudaSuccess) {
-                    unsigned long long keep = ~0ull;
-                    cudaMemPoolSetAttribute(pool, cudaMemPoolAttrReleaseThreshold, &keep);
-                }
-            });
-            cudaError_t ea = cudaMallocAsync((void**)&lists, ll.bytes, stream);
-            if (ea != cudaSuccess)
-                return api.fail(F3DGS_ERR_ALLOC, "cudaMallocAsync of " + std::to_string(ll.bytes) +
-                                                     " bytes for the backward instance lists failed: " +
-                                                     cudaGetErrorString(ea));
+            if (const int rc = alloc_lists(api, ll, &lists, stream)) return rc;
         }
         e = launch_composite_bwd_geom(
             vp, ranges, point_list, rec, background, final_T, n_contrib, dL_dpix, dL_depths, dL_dmean2D, dL_dconic,
@@ -643,6 +648,69 @@ int f3dgs_backward_accum_f16(int P, int D, int M, int R, int C, const float* bac
                                dL_dopacity, dL_dcolors_precomp, dL_dsemantic_feature, dL_dmean3D, dL_dcov3D_precomp,
                                dL_dsh, dL_dscale, dL_drot, dL_dmean2D_out, grad_accum, denom, composite_done_event, debug,
                                cuda_stream);
+}
+
+}  // extern "C"
+
+namespace {
+// Shared body of f3dgs_lift_features_accum (TF = float) and f3dgs_lift_features_accum_f16 (TF = __half, the map only).
+// The geometry kernel's LIFT mode emits the backward's per-(tile, block) lists and adds the blend weights into
+// weight_sum; the backward's feature kernel then adds sum_p w * map[:, p] into feature_sum (scale 1: exact for a map).
+template <typename TF>
+int lift_impl(const char* entry, int P, int R, int C, int width, int height, char* geom_buffer, char* binning_buffer,
+              char* image_buffer, const TF* feature_map, float* feature_sum, float* weight_sum, void* cuda_stream) {
+    const Api api(entry);
+    cudaStream_t stream = (cudaStream_t)cuda_stream;
+    if (P < 0 || R < 0 || width <= 0 || height <= 0 || C < 1 || C > F3DGS_MAX_FEATURE_DIM)
+        return api.invalid("bad sizes (P >= 0, R >= 0, width, height >= 1, 1 <= C <= F3DGS_MAX_FEATURE_DIM)");
+    if (P == 0 || R == 0) return 0;  // nothing is blended (a forward with R == 0 may leave an empty binning buffer)
+    if (!geom_buffer || !binning_buffer || !image_buffer) return api.invalid("missing forward buffers");
+    if (!feature_map || !feature_sum || !weight_sum) return api.invalid("NULL pointer (feature_map, feature_sum or weight_sum)");
+    // both kernels reduce into the outputs while other warps still read the map
+    const Range rmap{feature_map, (size_t)C * width * height * sizeof(TF)}, rws{weight_sum, (size_t)P * 4};
+    if (overlaps({feature_sum, (size_t)P * C * 4}, {rmap, rws}) || overlaps(rws, {rmap}))
+        return api.invalid("feature_sum, weight_sum and feature_map must not overlap");
+
+    const ViewParams vp = make_view(P, 0, 0, C, width, height, 0.f, 0.f, 1.f, nullptr, nullptr, nullptr);
+    const size_t tiles = (size_t)vp.grid_x * vp.grid_y;
+    const GeomLayout gl((size_t)P);
+    const ImgLayout il((size_t)width * height, tiles);
+    const BinLayout bl((size_t)R);
+    const ListLayout ll((size_t)R, tiles);
+    char* lists = nullptr;
+    if (const int rc = alloc_lists(api, ll, &lists, stream)) return rc;
+    int* counters = reinterpret_cast<int*>(image_buffer + il.counters);
+    const uint2* ranges = reinterpret_cast<const uint2*>(image_buffer + il.ranges);
+    float* list_w = reinterpret_cast<float*>(lists + ll.w);
+    uint2* list_meta = reinterpret_cast<uint2*>(lists + ll.meta);
+    uint32_t* list_cnt = reinterpret_cast<uint32_t*>(lists + ll.cnt);
+    cudaError_t e = launch_composite_bwd_lift(
+        vp, ranges, reinterpret_cast<const uint32_t*>(binning_buffer + bl.point_list),
+        reinterpret_cast<const SplatRec*>(geom_buffer + gl.rec), reinterpret_cast<const float*>(image_buffer + il.final_T),
+        reinterpret_cast<const uint32_t*>(image_buffer + il.n_contrib), weight_sum, counters + 16, stream, list_w,
+        list_meta, list_cnt);
+    if (e == cudaSuccess)
+        e = launch_feature_bwd(vp, ranges, list_w, list_meta, list_cnt, feature_map, 1.f, feature_sum, counters + 48,
+                               stream);
+    cudaFreeAsync(lists, stream);
+    return api.cuda(e, "lift launch");
+}
+}  // namespace
+
+extern "C" {
+
+int f3dgs_lift_features_accum(int P, int R, int C, int width, int height, char* geom_buffer, char* binning_buffer,
+                              char* image_buffer, const float* feature_map, float* feature_sum, float* weight_sum,
+                              void* cuda_stream) {
+    return lift_impl(__func__, P, R, C, width, height, geom_buffer, binning_buffer, image_buffer, feature_map,
+                     feature_sum, weight_sum, cuda_stream);
+}
+
+int f3dgs_lift_features_accum_f16(int P, int R, int C, int width, int height, char* geom_buffer, char* binning_buffer,
+                                  char* image_buffer, const uint16_t* feature_map, float* feature_sum, float* weight_sum,
+                                  void* cuda_stream) {
+    return lift_impl(__func__, P, R, C, width, height, geom_buffer, binning_buffer, image_buffer,
+                     reinterpret_cast<const __half*>(feature_map), feature_sum, weight_sum, cuda_stream);
 }
 
 }  // extern "C"

@@ -12,6 +12,9 @@
 //       inside the warp.
 //   EMIT           with features, the alpha warps also append one list entry per (tile, block, instance that blended in
 //       the block): {Gaussian id, pixel mask} + the 32 blend weights w = alpha*T, for feature_bwd.cu.
+//   LIFT           feature lifting: the EMIT lists, and instead of the 10 gradient terms the one value w = alpha*T per pair,
+//       reduced into weight_sum[P] through the same tile; no upstream gradient or background is read.  feature_bwd.cu
+//       then forms sum_p w * map[:, p] over the lists with the teacher map in place of dL/dfeature_map.
 // 12 warps and a ring without weight slots (RingSlim, 106 KB of shared memory with the reduction tiles): two CTAs per SM,
 // and the alpha warps keep the launch register count (80).
 // As in the reference, the feature loss does not feed dL/dalpha (backward.cu:575 is disabled).
@@ -50,7 +53,17 @@ struct BwdArgs {
     float* list_w;        // [8R][32] blend weights w = alpha * T (the backward's unwound T), entry list_begin(range.x, range.y, b) + i
     uint2* list_meta;     // [8R]     {Gaussian id, pixel mask}
     uint32_t* list_cnt;   // [8T]     entries written per (tile, block)
+    float* weight_sum;    // LIFT: [P] += sum over the view's pixels of w
 };
+
+// GEOM: geometric gradients; EMIT: and the feature lists; LIFT: the feature lists and the per-Gaussian weight sums
+enum class BwdMode { GEOM, EMIT, LIFT };
+// Namespace-scope constants: as constexpr locals of the kernel they changed the register allocation of the EMIT
+// instantiation, which is meant to stay instruction-for-instruction what it was before lifting existed.
+template <BwdMode M>
+constexpr bool kLift = M == BwdMode::LIFT;
+template <BwdMode M>
+constexpr int kVals = kLift<M> ? 1 : kRedVals;  // values reduced per pair
 
 // destination of reduced value v (0..9) of Gaussian gid: reference backward.cu:560-610 (atomicAdd targets)
 __device__ __forceinline__ float* geom_dst(const BwdArgs& args, int v, uint32_t gid) {
@@ -66,9 +79,10 @@ __device__ __forceinline__ float* geom_dst(const BwdArgs& args, int v, uint32_t 
     }
 }
 
-template <bool EMIT>
+template <BwdMode MODE>
 __global__ void __launch_bounds__(kBwdThreads, kSlimCtas)
 composite_bwd_kernel(const BwdArgs args) {
+    constexpr bool EMIT = MODE != BwdMode::GEOM;
     extern __shared__ __align__(128) unsigned char smem_raw[];
     BwdSmem& sm = *reinterpret_cast<BwdSmem*>(smem_raw);
     RingSlim& ring = sm.ring;
@@ -110,7 +124,7 @@ composite_bwd_kernel(const BwdArgs args) {
 
     auto flush = [&]() {
         __syncwarp();
-        for (int r = lane; r < kRedRows; r += 32) {
+        for (int r = lane; r < kVals<MODE> * kRedSlots; r += 32) {
             const int slot = r % kRedSlots, v = r / kRedSlots;
             if (slot < (int)nslots) {
                 float s0 = 0.f, s1 = 0.f, s2 = 0.f, s3 = 0.f;
@@ -123,7 +137,10 @@ composite_bwd_kernel(const BwdArgs args) {
                     s2 += q.z;
                     s3 += q.w;
                 }
-                red_add_f1(geom_dst(args, v, red_gid[slot]), (s0 + s1) + (s2 + s3));
+                if constexpr (kLift<MODE>)
+                    red_add_f1(args.weight_sum + red_gid[slot], (s0 + s1) + (s2 + s3));
+                else
+                    red_add_f1(geom_dst(args, v, red_gid[slot]), (s0 + s1) + (s2 + s3));
             }
         }
         __syncwarp();
@@ -154,13 +171,15 @@ composite_bwd_kernel(const BwdArgs args) {
             p.T = p.T_final;
             p.last_contrib = p.inside ? args.n_contrib[pix] : 0u;
             p.dLp0 = p.dLp1 = p.dLp2 = p.dLd = 0.f;
-            if (p.inside) {
-                p.dLp0 = args.dL_dpix[pix];
-                p.dLp1 = args.dL_dpix[HW + pix];
-                p.dLp2 = args.dL_dpix[2 * HW + pix];
-                p.dLd = args.dL_ddepth[pix];
+            if constexpr (!kLift<MODE>) {
+                if (p.inside) {
+                    p.dLp0 = args.dL_dpix[pix];
+                    p.dLp1 = args.dL_dpix[HW + pix];
+                    p.dLp2 = args.dL_dpix[2 * HW + pix];
+                    p.dLd = args.dL_ddepth[pix];
+                }
+                p.bg_dot = args.bg[0] * p.dLp0 + args.bg[1] * p.dLp1 + args.bg[2] * p.dLp2;
             }
-            p.bg_dot = args.bg[0] * p.dLp0 + args.bg[1] * p.dLp1 + args.bg[2] * p.dLp2;
             p.ar0 = p.ar1 = p.ar2 = p.lc0 = p.lc1 = p.lc2 = 0.f;
             p.last_alpha = p.accum_depth = p.last_depth = 0.f;
             uint32_t wm = p.last_contrib;
@@ -197,7 +216,13 @@ composite_bwd_kernel(const BwdArgs args) {
                     float v[kRedVals];
 #pragma unroll
                     for (int i = 0; i < kRedVals; i++) v[i] = 0.f;
-                    if (contrib) {
+                    if constexpr (kLift<MODE>) {
+                        if (contrib) {  // the T unwind below, without the gradient terms
+                            p.T = p.T * rcp_approx(1.f - alpha);
+                            wgt = alpha * p.T;
+                            v[0] = wgt;
+                        }
+                    } else if (contrib) {
                         const float4 r1 = st.rec1[k];
                         const float4 r2 = st.rec2[k];
                         // 1/(1-alpha), 1-alpha in [0.01, 1]: one MUFU.RCP (<= 1 ulp) serves both the T unwind and
@@ -240,7 +265,7 @@ composite_bwd_kernel(const BwdArgs args) {
                             ecount++;
                         }
 #pragma unroll
-                        for (int i = 0; i < kRedVals; i++) red[i * kRedSlots + nslots][lane] = v[i];
+                        for (int i = 0; i < kVals<MODE>; i++) red[i * kRedSlots + nslots][lane] = v[i];
                         if (lane == 0) red_gid[nslots] = st.gid[k];
                         nslots++;
                         if (nslots == kRedSlots) flush();
@@ -256,29 +281,53 @@ composite_bwd_kernel(const BwdArgs args) {
     }
 }
 
+// Every instantiation is opted in to the shared memory it needs on the first launch of any of them on a device
+static cudaError_t bwd_device_sms(int& num_sms) {
+    return device_sms<composite_bwd_kernel<BwdMode::GEOM>, composite_bwd_kernel<BwdMode::EMIT>,
+                      composite_bwd_kernel<BwdMode::LIFT>>(num_sms, sizeof(BwdSmem));
+}
+
+static cudaError_t launch_bwd(void (*kernel)(BwdArgs), const BwdArgs& a, int num_sms, cudaStream_t s) {
+    const cudaError_t e = cudaMemsetAsync(a.pa.work_counter, 0, sizeof(int), s);
+    if (e != cudaSuccess) return e;
+    const int grid = min(a.pa.num_tiles, kSlimCtas * num_sms);
+    kernel<<<grid, kBwdThreads, sizeof(BwdSmem), s>>>(a);
+    g_launches++;
+    return cudaGetLastError();
+}
+
 cudaError_t launch_composite_bwd_geom(const ViewParams& vp, const uint2* ranges, const uint32_t* point_list,
                                       const SplatRec* rec, const float* bg, const float* final_T,
                                       const uint32_t* n_contrib, const float* dL_dpix, const float* dL_ddepth,
                                       float* dL_dmean2D, float* dL_dconic, float* dL_dopacity, float* dL_dcolor,
                                       float* dL_dz, int* work_counter, cudaStream_t s, float* list_w,
                                       uint2* list_meta, uint32_t* list_cnt) {
-    const size_t smem = sizeof(BwdSmem);
     int num_sms = 0;
-    cudaError_t e = device_sms<composite_bwd_kernel<false>, composite_bwd_kernel<true>>(num_sms, smem);
+    cudaError_t e = bwd_device_sms(num_sms);
     if (e != cudaSuccess) return e;
-    BwdArgs a;
+    BwdArgs a{};
     a.pa = producer_args(vp, ranges, point_list, rec, n_contrib, work_counter);
     a.bg = bg; a.final_T = final_T; a.n_contrib = n_contrib; a.dL_dpix = dL_dpix; a.dL_ddepth = dL_ddepth;
     a.dL_dmean2D = dL_dmean2D; a.dL_dconic = dL_dconic; a.dL_dopacity = dL_dopacity; a.dL_dcolor = dL_dcolor;
     a.dL_dz = dL_dz;
     a.list_w = list_w; a.list_meta = list_meta; a.list_cnt = list_cnt;
-    e = cudaMemsetAsync(work_counter, 0, sizeof(int), s);
+    return launch_bwd(list_w != nullptr ? composite_bwd_kernel<BwdMode::EMIT> : composite_bwd_kernel<BwdMode::GEOM>, a,
+                      num_sms, s);
+}
+
+cudaError_t launch_composite_bwd_lift(const ViewParams& vp, const uint2* ranges, const uint32_t* point_list,
+                                      const SplatRec* rec, const float* final_T, const uint32_t* n_contrib,
+                                      float* weight_sum, int* work_counter, cudaStream_t s, float* list_w,
+                                      uint2* list_meta, uint32_t* list_cnt) {
+    int num_sms = 0;
+    cudaError_t e = bwd_device_sms(num_sms);
     if (e != cudaSuccess) return e;
-    const int grid = min(a.pa.num_tiles, kSlimCtas * num_sms);
-    const auto kernel = list_w != nullptr ? composite_bwd_kernel<true> : composite_bwd_kernel<false>;
-    kernel<<<grid, kBwdThreads, smem, s>>>(a);
-    g_launches++;
-    return cudaGetLastError();
+    BwdArgs a{};
+    a.pa = producer_args(vp, ranges, point_list, rec, n_contrib, work_counter);
+    a.final_T = final_T; a.n_contrib = n_contrib;
+    a.list_w = list_w; a.list_meta = list_meta; a.list_cnt = list_cnt;
+    a.weight_sum = weight_sum;
+    return launch_bwd(composite_bwd_kernel<BwdMode::LIFT>, a, num_sms, s);
 }
 
 }  // namespace f3dgs

@@ -64,6 +64,12 @@ cudaError_t launch_composite_bwd_geom(const ViewParams& vp, const uint2* ranges,
                                       float* dL_dmean2D, float* dL_dconic, float* dL_dopacity, float* dL_dcolor,
                                       float* dL_dz, int* work_counter, cudaStream_t s, float* list_w = nullptr,
                                       uint2* list_meta = nullptr, uint32_t* list_cnt = nullptr);
+// Feature lifting: the lists of the backward's EMIT mode (every pointer required) and weight_sum[P] += the blend weights
+// w = alpha*T of each Gaussian over the view; launch_feature_bwd with the teacher map then adds sum_p w * map[:, p]
+cudaError_t launch_composite_bwd_lift(const ViewParams& vp, const uint2* ranges, const uint32_t* point_list,
+                                      const SplatRec* rec, const float* final_T, const uint32_t* n_contrib,
+                                      float* weight_sum, int* work_counter, cudaStream_t s, float* list_w,
+                                      uint2* list_meta, uint32_t* list_cnt);
 
 // ---- feature_bwd.cu: feature gradient from the instance lists (second kernel of the two-kernel backward).  TG (float or
 // __half) is the element type of the upstream gradient map; a __half map stands for dL/dO = scale * float(h) (the scale is

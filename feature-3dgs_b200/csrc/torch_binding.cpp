@@ -309,6 +309,36 @@ void RasterizeGaussiansBackwardAccumCUDA(
                     });
 }
 
+// Feature lifting (f3dgs_lift_features_accum / _f16): the buffers and R of a forward of this view; feature_map [C,H,W]
+// float32 or float16 at the forward's resolution; feature_sum [P,...,C] and weight_sum [P] contiguous float32, ADDED into
+void liftFeaturesAccum(const torch::Tensor& geomBuffer, const int R, const torch::Tensor& binningBuffer,
+                       const torch::Tensor& imageBuffer, const torch::Tensor& feature_map, torch::Tensor feature_sum,
+                       torch::Tensor weight_sum) {
+    TORCH_CHECK(feature_map.is_cuda() && feature_map.dim() == 3 &&
+                    (feature_map.scalar_type() == torch::kFloat32 || feature_map.scalar_type() == torch::kFloat16),
+                "lift_features_accum: feature_map must be a float32 or float16 CUDA tensor [C,H,W]");
+    const auto dev = feature_map.device();
+    const c10::cuda::CUDAGuard guard(dev);
+    const int64_t C = feature_map.size(0), H = feature_map.size(1), W = feature_map.size(2);
+    TORCH_CHECK(C <= INT32_MAX && H <= INT32_MAX && W <= INT32_MAX && weight_sum.numel() <= INT32_MAX,
+                "lift_features_accum: sizes too large");
+    const int64_t P = weight_sum.numel();
+    float* ws = in_place(weight_sum, dev, P, "lift_features_accum: weight_sum");
+    float* fs = in_place(feature_sum, dev, P * C, "lift_features_accum: feature_sum");
+    for (const torch::Tensor* b : {&geomBuffer, &binningBuffer, &imageBuffer})
+        TORCH_CHECK(b->device() == dev && b->scalar_type() == torch::kByte && b->is_contiguous(),
+                    "lift_features_accum: the forward buffers must be contiguous uint8 tensors on ", dev);
+    if (P == 0) return;
+    auto fm = feature_map.contiguous();
+    cudaStream_t stream = c10::cuda::getCurrentCUDAStream().stream();
+    call_f32_or_f16(fm, f3dgs_lift_features_accum, "f3dgs_lift_features_accum", f3dgs_lift_features_accum_f16,
+                    "f3dgs_lift_features_accum_f16", [&](auto fn, auto mp) {
+                        return fn((int)P, R, (int)C, (int)W, (int)H, reinterpret_cast<char*>(geomBuffer.data_ptr()),
+                                  reinterpret_cast<char*>(binningBuffer.data_ptr()),
+                                  reinterpret_cast<char*>(imageBuffer.data_ptr()), mp, fs, ws, (void*)stream);
+                    });
+}
+
 torch::Tensor markVisible(torch::Tensor& means3D, torch::Tensor& viewmatrix, torch::Tensor& projmatrix) {
     TORCH_CHECK(means3D.is_cuda(), "means3D must be a CUDA tensor (this build has no CPU path)");
     const c10::cuda::CUDAGuard guard(means3D.device());
@@ -805,6 +835,9 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
               py::arg("grad_accum"), py::arg("denom"), py::arg("composite_done_event"), py::arg("debug"),
               py::arg("feature_grad_scale") = 1.0);
     }
+    m.def("lift_features_accum", &liftFeaturesAccum, pybind11::arg("geomBuffer"), pybind11::arg("R"),
+          pybind11::arg("binningBuffer"), pybind11::arg("imageBuffer"), pybind11::arg("feature_map"),
+          pybind11::arg("feature_sum"), pybind11::arg("weight_sum"));
     m.def("feature_resize_fwd", &featureResizeFwd);
     m.def("feature_resize_bwd", &featureResizeBwd, pybind11::arg("dout"), pybind11::arg("H"), pybind11::arg("W"),
           pybind11::arg("dtype") = torch::kFloat32, pybind11::arg("out_scale") = 1.0);

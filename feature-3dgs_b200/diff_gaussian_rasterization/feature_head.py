@@ -10,7 +10,9 @@ With --speedup the 1x1 decoder and its loss run in between on csrc/feature_decod
 default for the reference's nn.Conv2d): `decode`, `decoded_feature_l1_loss_and_grad`, `decoded_feature_l1_loss`.
 `query` asks the trained field questions with text embeddings (csrc/feature_query.cu): LSeg's per-pixel labels and
 render_edit's per-Gaussian selection score, without materialising the decoded map.  `pca_fit` and `pca_image` make
-render.py's PCA picture of a feature map on the device (csrc/feature_pca.cu).
+render.py's PCA picture of a feature map on the device (csrc/feature_pca.cu).  `FeatureLift` makes a feature field
+without training: every Gaussian gets the blend-weighted mean of the teacher features of the pixels it is blended into
+(the backward composite's lift mode, csrc/composite_bwd.cu, and feature_bwd.cu).
 There is no CPU path (the extension raises on CPU tensors).
 
 The teacher map `gt` may be float32 or float16, the dtype the data format stores it in (io.load_feature_map(path,
@@ -291,3 +293,90 @@ def decoded_feature_l1_loss(feature_map: torch.Tensor, gt: torch.Tensor, weight:
     `l1_loss(cnn_decoder(F.interpolate(feature_map[None], gt.shape[1:], 'bilinear', True)[0]), gt) * loss_weight`, with
     gradients for feature_map, weight and bias (gt is the constant target)."""
     return _DecodedL1.apply(feature_map, weight, bias, gt, float(loss_weight))
+
+
+class FeatureLift:
+    """Lift 2-D feature maps onto Gaussians without training (blend-weighted back-projection over views):
+
+        f_i = sum_{v,p} w_ivp F_v[:, p] / sum_{v,p} w_ivp,     w_ivp = alpha * T, Gaussian i's blend weight at pixel p of view v
+
+        lift = FeatureLift(means3D, opacities, scales, rotations, C)     # or cov3D_precomp=...;  FeatureLift.from_state(state)
+        for rs, fmap in views:        # fmap [C,Hg,Wg] float32 or float16; (rs.image_height, rs.image_width) == (Hg, Wg)
+            lift.add(rs, fmap)
+        feats, weight = lift.result(min_weight=0.0, dtype=torch.float32)     # [P,1,C] (semantic_feature layout), [P]
+
+    Any trained 3DGS scene (a plain PLY from io.load_ply included) becomes a feature field in one pass over the views;
+    the result can also initialise distillation.  Each `add` is a forward at C = 0 with zero colors_precomp (no SH
+    work) and one native lift call (f3dgs_lift_features_accum), which accumulates into `feature_sum` and `weight_sum`:
+    the two slices of the single float32 buffer `flat` ([P*C] then [P]), so a data-parallel caller that lifts a share
+    of the views on each rank all-reduces `flat` once before `result`.
+
+    Resolution: the map's pixels are the rasterizer's pixels of `rs`.  To lift at a teacher's resolution pass
+    `rs._replace(image_height=Hg, image_width=Wg)`: pixel centres then follow the rasterizer's own projection at that
+    resolution (pixel x covers [x, x+1) of Wg, the same field of view).  That is deliberately not the relation of the
+    training loss, which resizes the W x H render to Hg x Wg with align_corners=True (corner pixel centres on corner
+    pixel centres); the two differ by up to half a teacher pixel at the image borders.  There is no autograd."""
+
+    def __init__(self, means3D, opacities, scales=None, rotations=None, C: int = None, cov3D_precomp=None):
+        if C is None or int(C) < 1 or int(C) > 4096:
+            raise ValueError(f"FeatureLift: C must be 1..4096, got {C}")
+        if (scales is None or rotations is None) == (cov3D_precomp is None):
+            raise ValueError("FeatureLift: provide exactly one of (scales, rotations) / cov3D_precomp")
+        if not means3D.is_cuda:
+            raise ValueError("FeatureLift: means3D must be a CUDA tensor (there is no CPU path)")
+        dev = means3D.device
+        self.C, self.P = int(C), int(means3D.shape[0])
+        e = torch.empty(0, device=dev)
+        self._geom = dict(means3D=means3D.detach(), opacities=opacities.detach(),
+                          scales=e if scales is None else scales.detach(),
+                          rotations=e if rotations is None else rotations.detach(),
+                          cov3D=e if cov3D_precomp is None else cov3D_precomp.detach())
+        self._colors = torch.zeros(self.P, 3, device=dev)
+        self._empty = e
+        self.flat = torch.zeros(self.P * (self.C + 1), device=dev)
+        self.feature_sum = self.flat[: self.P * self.C].view(self.P, 1, self.C)
+        self.weight_sum = self.flat[self.P * self.C:]
+
+    @classmethod
+    def from_state(cls, state, C: int = None):
+        """A lift over the Gaussians of a trainer.GaussianState (its activated geometry); C defaults to the state's
+        feature width."""
+        act = state.activate()
+        C = state.raw["semantic_feature"].shape[-1] if C is None else C
+        return cls(act["means3D"], act["opacities"], act["scales"], act["rotations"], C)
+
+    def add(self, raster_settings, feature_map: torch.Tensor):
+        """Accumulate one view: feature_map [C,H,W] (float32, or float16 read exactly) with (H, W) ==
+        (raster_settings.image_height, raster_settings.image_width)."""
+        rs = raster_settings
+        if not isinstance(feature_map, torch.Tensor) or feature_map.dim() != 3:
+            raise ValueError(f"FeatureLift.add: feature_map must be a tensor [C,H,W], got "
+                             f"{getattr(feature_map, 'shape', type(feature_map))}")
+        if feature_map.dtype not in (torch.float32, torch.float16):
+            raise ValueError(f"FeatureLift.add: feature_map must be float32 or float16, got {feature_map.dtype}")
+        C, H, W = feature_map.shape
+        if C != self.C:
+            raise ValueError(f"FeatureLift.add: the lift has C = {self.C} channels, feature_map has {C}")
+        if (H, W) != (rs.image_height, rs.image_width):
+            raise ValueError(f"FeatureLift.add: feature_map is {H}x{W} (HxW) but the settings render "
+                             f"{rs.image_height}x{rs.image_width}; pass rs._replace(image_height={H}, image_width={W})")
+        if feature_map.device != self.flat.device:
+            raise ValueError(f"FeatureLift.add: feature_map must be on {self.flat.device}, got {feature_map.device}")
+        if self.P == 0:
+            return
+        g, e = self._geom, self._empty
+        with torch.no_grad():
+            R, _, _, _, _, geom, binning, img = _C().rasterize_gaussians(
+                rs.bg, g["means3D"], self._colors, e, g["opacities"], g["scales"], g["rotations"], rs.scale_modifier,
+                g["cov3D"], rs.viewmatrix, rs.projmatrix, rs.tanfovx, rs.tanfovy, H, W, e, rs.sh_degree, rs.campos,
+                rs.prefiltered, rs.debug)
+            _C().lift_features_accum(geom, R, binning, img, feature_map, self.feature_sum, self.weight_sum)
+
+    def result(self, min_weight: float = 0.0, dtype=torch.float32):
+        """-> (features [P,1,C] of `dtype`, weight_sum [P] float32): feature_sum / weight_sum where weight_sum >
+        min_weight, 0 elsewhere (Gaussians no view blended, radii == 0 ones among them)."""
+        with torch.no_grad():
+            w = self.weight_sum
+            keep = w > min_weight
+            f = torch.where(keep[:, None, None], self.feature_sum / torch.where(keep, w, 1.0)[:, None, None], 0.0)
+            return f.to(dtype), w.clone()

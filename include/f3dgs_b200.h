@@ -190,6 +190,26 @@ int f3dgs_backward_accum_f16(int P, int D, int M, int R, int C,
                              float* dL_drot, float* dL_dmean2D_out, float* grad_accum, float* denom,
                              void* composite_done_event, int debug, void* cuda_stream);
 
+/* ---- feature lifting (no reference counterpart): training-free back-projection of 2-D feature maps onto Gaussians ----
+ * The buffers and R are those of an f3dgs_forward / f3dgs_forward_f16 of this view at width x height (any C of that
+ * forward, 0 included); feature_map [C,H,W] is a map at that resolution, 1 <= C <= F3DGS_MAX_FEATURE_DIM.
+ * ACCUMULATES:  feature_sum[P,C] += sum_p w_ip * feature_map[:,p];   weight_sum[P] += sum_p w_ip,
+ * w_ip = the blend weight alpha*T of Gaussian i at pixel p (the backward's unwound T: equal to the forward's blend weight
+ * to a few ulp).  Over views, feature_sum / weight_sum is the blend-weighted mean of the maps per Gaussian.  The result
+ * equals f3dgs_backward's dL_dsemantic_feature and dL_dcolor[:,0] for dL_dfeaturepix = feature_map, dL_dpix = the planes
+ * (1, 0, 0) and dL_depths = 0, up to the order of the float reductions, without the geometric gradients.
+ * The outputs must not overlap the map or each other.  P == 0 or R == 0 launches nothing.  The instance lists (136
+ * bytes per (instance, 8x4 block) of capacity) are stream-ordered scratch of the device's default memory pool.
+ *   f3dgs_lift_features_accum_f16: feature_map holds IEEE binary16 bits (a saved *_fmap_CxHxW.pt as loaded), upcast
+ *   exactly; the result is that of the float32 call on the upcast map.  Validates as the float32 call, with the map's
+ *   2-byte size in the overlap checks. */
+int f3dgs_lift_features_accum(int P, int R, int C, int width, int height, char* geom_buffer, char* binning_buffer,
+                              char* image_buffer, const float* feature_map, float* feature_sum, float* weight_sum,
+                              void* cuda_stream);
+int f3dgs_lift_features_accum_f16(int P, int R, int C, int width, int height, char* geom_buffer, char* binning_buffer,
+                                  char* image_buffer, const uint16_t* feature_map, float* feature_sum,
+                                  float* weight_sum, void* cuda_stream);
+
 /* ==== callers either side of the rasterizer (SURVEY.md section 8 f): additive entry points ======================= */
 
 /* ---- post-raster feature head: reference train.py:98-104 ---------------------------------------------------------
