@@ -18,6 +18,8 @@
 // 12 warps and a ring without weight slots (RingSlim, 106 KB of shared memory with the reduction tiles): two CTAs per SM,
 // and the alpha warps keep the launch register count (80).
 // As in the reference, the feature loss does not feed dL/dalpha (backward.cu:575 is disabled).
+#include <mutex>
+
 #include "composite_common.cuh"
 
 namespace f3dgs {
@@ -49,10 +51,7 @@ struct BwdArgs {
     float* dL_dopacity;  // [P]
     float* dL_dcolor;    // [P,3]
     float* dL_dz;        // [P]
-    // EMIT: per (tile, 8x4 block) lists of the instances that blended in the block
-    float* list_w;        // [8R][32] blend weights w = alpha * T (the backward's unwound T), entry list_begin(range.x, range.y, b) + i
-    uint2* list_meta;     // [8R]     {Gaussian id, pixel mask}
-    uint32_t* list_cnt;   // [8T]     entries written per (tile, block)
+    InstanceLists lists;  // EMIT and LIFT; w = alpha * T with the backward's unwound T
     float* weight_sum;    // LIFT: [P] += sum over the view's pixels of w
 };
 
@@ -260,8 +259,8 @@ composite_bwd_kernel(const BwdArgs args) {
                     if (pm) {
                         if (EMIT) {  // one 128-byte row of weights + {id, mask} per blended (block, instance)
                             const size_t e = ebase + ecount;
-                            args.list_w[e * 32 + lane] = wgt;
-                            if (lane == 0) args.list_meta[e] = make_uint2(st.gid[k], pm);
+                            args.lists.w[e * 32 + lane] = wgt;
+                            if (lane == 0) args.lists.meta[e] = make_uint2(st.gid[k], pm);
                             ecount++;
                         }
 #pragma unroll
@@ -275,59 +274,93 @@ composite_bwd_kernel(const BwdArgs args) {
         }
         __syncwarp();
         if (lane == 0) mbar_arrive(&ring.empty[s]);
-        if (EMIT && last && lane == 0) args.list_cnt[(size_t)etile * kBlocksPerTile + a] = ecount;
+        if (EMIT && last && lane == 0) args.lists.cnt[(size_t)etile * kBlocksPerTile + a] = ecount;
         if (last && nslots > 0) flush();
         if (++s == kStages) { s = 0; parity ^= 1; }
     }
 }
 
-// Every instantiation is opted in to the shared memory it needs on the first launch of any of them on a device
-static cudaError_t bwd_device_sms(int& num_sms) {
-    return device_sms<composite_bwd_kernel<BwdMode::GEOM>, composite_bwd_kernel<BwdMode::EMIT>,
-                      composite_bwd_kernel<BwdMode::LIFT>>(num_sms, sizeof(BwdSmem));
+// Stream-ordered scratch for the instance lists (the reference's backward allocates its scratch too,
+// rasterizer_impl.cu:402-430); the default pool keeps freed blocks, so steady-state calls do not reach the driver.
+// The caller releases *mem with cudaFreeAsync on the same stream.
+static cudaError_t alloc_lists(size_t R, size_t tiles, char** mem, InstanceLists& lists, cudaStream_t s) {
+    static std::once_flag once;
+    std::call_once(once, [] {
+        int dev = 0;
+        cudaGetDevice(&dev);
+        cudaMemPool_t pool;
+        if (cudaDeviceGetDefaultMemPool(&pool, dev) == cudaSuccess) {
+            unsigned long long keep = ~0ull;
+            cudaMemPoolSetAttribute(pool, cudaMemPoolAttrReleaseThreshold, &keep);
+        }
+    });
+    const ListLayout ll(R, tiles);
+    const cudaError_t e = cudaMallocAsync((void**)mem, ll.bytes, s);
+    if (e == cudaSuccess)
+        lists = {reinterpret_cast<float*>(*mem + ll.w), reinterpret_cast<uint2*>(*mem + ll.meta),
+                 reinterpret_cast<uint32_t*>(*mem + ll.cnt)};
+    return e;
 }
 
-static cudaError_t launch_bwd(void (*kernel)(BwdArgs), const BwdArgs& a, int num_sms, cudaStream_t s) {
-    const cudaError_t e = cudaMemsetAsync(a.pa.work_counter, 0, sizeof(int), s);
-    if (e != cudaSuccess) return e;
-    const int grid = min(a.pa.num_tiles, kSlimCtas * num_sms);
-    kernel<<<grid, kBwdThreads, sizeof(BwdSmem), s>>>(a);
-    g_launches++;
-    return cudaGetLastError();
-}
-
-cudaError_t launch_composite_bwd_geom(const ViewParams& vp, const uint2* ranges, const uint32_t* point_list,
-                                      const SplatRec* rec, const float* bg, const float* final_T,
-                                      const uint32_t* n_contrib, const float* dL_dpix, const float* dL_ddepth,
-                                      float* dL_dmean2D, float* dL_dconic, float* dL_dopacity, float* dL_dcolor,
-                                      float* dL_dz, int* work_counter, cudaStream_t s, float* list_w,
-                                      uint2* list_meta, uint32_t* list_cnt) {
+// The geometry kernel in mode MODE over the view's forward buffers; for EMIT and LIFT also the instance lists and then
+// feature_bwd over them, reducing sum_p w * scale * map[:, p] into dst.  `a` brings the mode's outputs.
+template <BwdMode MODE, typename TG>
+static cudaError_t run_bwd(BwdArgs a, const ViewParams& vp, const ForwardBuffers& fb, const TG* map, float scale,
+                           float* dst, cudaStream_t s) {
+    a.pa = producer_args(vp, fb.ranges, fb.point_list, fb.rec, fb.n_contrib, fb.counters + kCounterBwdGeom);
+    a.final_T = fb.final_T; a.n_contrib = fb.n_contrib;
+    char* mem = nullptr;
+    if (MODE != BwdMode::GEOM) {
+        const cudaError_t e = alloc_lists((size_t)fb.R, (size_t)a.pa.num_tiles, &mem, a.lists, s);
+        if (e != cudaSuccess) return e;
+    }
+    // every instantiation is opted in to the shared memory it needs on the first launch of any of them on a device
     int num_sms = 0;
-    cudaError_t e = bwd_device_sms(num_sms);
-    if (e != cudaSuccess) return e;
+    cudaError_t e = device_sms<composite_bwd_kernel<BwdMode::GEOM>, composite_bwd_kernel<BwdMode::EMIT>,
+                               composite_bwd_kernel<BwdMode::LIFT>>(num_sms, sizeof(BwdSmem));
+    if (e == cudaSuccess) e = cudaMemsetAsync(a.pa.work_counter, 0, sizeof(int), s);
+    if (e == cudaSuccess) {
+        composite_bwd_kernel<MODE><<<min(a.pa.num_tiles, kSlimCtas * num_sms), kBwdThreads, sizeof(BwdSmem), s>>>(a);
+        g_launches++;
+        e = cudaGetLastError();
+    }
+    if (MODE != BwdMode::GEOM) {
+        if (e == cudaSuccess) e = launch_feature_bwd(vp, fb.ranges, a.lists, map, scale, dst, fb.counters, s);
+        cudaFreeAsync(mem, s);
+    }
+    return e;
+}
+
+template <typename TG>
+cudaError_t launch_composite_bwd(const ViewParams& vp, const ForwardBuffers& fb, const float* bg, const float* dL_dpix,
+                                 const float* dL_ddepth, const TG* dL_dfeat_pix, float dL_dfeat_pix_scale,
+                                 float* dL_dmean2D, float* dL_dconic, float* dL_dopacity, float* dL_dcolor, float* dL_dz,
+                                 float* dL_dfeature, cudaStream_t s) {
     BwdArgs a{};
-    a.pa = producer_args(vp, ranges, point_list, rec, n_contrib, work_counter);
-    a.bg = bg; a.final_T = final_T; a.n_contrib = n_contrib; a.dL_dpix = dL_dpix; a.dL_ddepth = dL_ddepth;
+    a.bg = bg; a.dL_dpix = dL_dpix; a.dL_ddepth = dL_ddepth;
     a.dL_dmean2D = dL_dmean2D; a.dL_dconic = dL_dconic; a.dL_dopacity = dL_dopacity; a.dL_dcolor = dL_dcolor;
     a.dL_dz = dL_dz;
-    a.list_w = list_w; a.list_meta = list_meta; a.list_cnt = list_cnt;
-    return launch_bwd(list_w != nullptr ? composite_bwd_kernel<BwdMode::EMIT> : composite_bwd_kernel<BwdMode::GEOM>, a,
-                      num_sms, s);
+    const auto run = vp.C > 0 && fb.R > 0 ? run_bwd<BwdMode::EMIT, TG> : run_bwd<BwdMode::GEOM, TG>;
+    return run(a, vp, fb, dL_dfeat_pix, dL_dfeat_pix_scale, dL_dfeature, s);
 }
 
-cudaError_t launch_composite_bwd_lift(const ViewParams& vp, const uint2* ranges, const uint32_t* point_list,
-                                      const SplatRec* rec, const float* final_T, const uint32_t* n_contrib,
-                                      float* weight_sum, int* work_counter, cudaStream_t s, float* list_w,
-                                      uint2* list_meta, uint32_t* list_cnt) {
-    int num_sms = 0;
-    cudaError_t e = bwd_device_sms(num_sms);
-    if (e != cudaSuccess) return e;
+template <typename TF>
+cudaError_t launch_feature_lift(const ViewParams& vp, const ForwardBuffers& fb, const TF* map, float* feature_sum,
+                                float* weight_sum, cudaStream_t s) {
     BwdArgs a{};
-    a.pa = producer_args(vp, ranges, point_list, rec, n_contrib, work_counter);
-    a.final_T = final_T; a.n_contrib = n_contrib;
-    a.list_w = list_w; a.list_meta = list_meta; a.list_cnt = list_cnt;
     a.weight_sum = weight_sum;
-    return launch_bwd(composite_bwd_kernel<BwdMode::LIFT>, a, num_sms, s);
+    return run_bwd<BwdMode::LIFT>(a, vp, fb, map, 1.f, feature_sum, s);
 }
+
+template cudaError_t launch_composite_bwd(const ViewParams&, const ForwardBuffers&, const float*, const float*,
+                                          const float*, const float*, float, float*, float*, float*, float*, float*,
+                                          float*, cudaStream_t);
+template cudaError_t launch_composite_bwd(const ViewParams&, const ForwardBuffers&, const float*, const float*,
+                                          const float*, const __half*, float, float*, float*, float*, float*, float*,
+                                          float*, cudaStream_t);
+template cudaError_t launch_feature_lift(const ViewParams&, const ForwardBuffers&, const float*, float*, float*,
+                                         cudaStream_t);
+template cudaError_t launch_feature_lift(const ViewParams&, const ForwardBuffers&, const __half*, float*, float*,
+                                         cudaStream_t);
 
 }  // namespace f3dgs

@@ -190,12 +190,47 @@ __device__ __forceinline__ float4 to_float4(uint2 v) {
     return make_float4(a.x, a.y, b.x, b.y);
 }
 
-// The backward's per-(tile, block) instance lists need no counting pass: block b of a tile owns entries
-// [list_begin(range.x, range.y, b), ... + len), len = range.y - range.x, because an instance of the tile's list appears at most once
-// per block.
+// ---------------------------------------------------------------- the backward's per-(tile, block) instance lists
+// The geometry kernel (composite_bwd.cu, EMIT and LIFT) writes one entry per instance that blended in an 8x4 block, back
+// to front; feature_bwd.cu reads them.  An entry is the 32 blend weights w = alpha * T of the block's pixel slots plus
+// {Gaussian id, pixel mask}: 136 bytes.
+struct InstanceLists {
+    float* w;       // [8R][32] blend weights, entry e at w[e * 32 + slot]
+    uint2* meta;    // [8R]     {Gaussian id, pixel mask}
+    uint32_t* cnt;  // [8 tiles] entries written per (tile, block)
+};
+
+// The lists need no counting pass: block b of a tile owns entries [list_begin(range.x, range.y, b), ... + len),
+// len = range.y - range.x, because an instance of the tile's list appears at most once per block.  The tiles' ranges
+// partition [0, R), so block b's entries end at 8 range.x + (b + 1) len <= 8 range.y <= 8R: a capacity of 8R entries
+// (ListLayout) holds every block of every tile.
 __device__ __forceinline__ size_t list_begin(uint32_t begin, uint32_t end, int b) {
     return kBlocksPerTile * (size_t)begin + (size_t)b * (end - begin);
 }
+
+// Byte offsets of the three lists in one allocation of `bytes`, for R instances over `tiles` tiles
+struct ListLayout {
+    size_t w, meta, cnt, bytes;
+    ListLayout(size_t R, size_t tiles) {
+        size_t o = 0;
+        w = o;     o = align_up(o + kBlocksPerTile * R * 32 * sizeof(float));
+        meta = o;  o = align_up(o + kBlocksPerTile * R * sizeof(uint2));
+        cnt = o;   o = align_up(o + kBlocksPerTile * tiles * sizeof(uint32_t));
+        bytes = o;
+    }
+};
+
+// Work counters of the persistent composite kernels: int slots of the 256-byte counter region of the image buffer, for
+// composite_fwd.cu, composite_bwd.cu and feature_bwd.cu.  Each launcher takes the region's base and zeroes its own slot.
+constexpr int kCounterFwd = 0, kCounterBwdGeom = 16, kCounterFeatureBwd = 48;
+
+// ---- feature_bwd.cu: dL/dfeature[g] += sum over the pixels of each list entry of w * dL/dfeature_map, over the lists of
+// the view.  TG (float or __half) is the element type of the map; a __half map stands for dL/dO = scale * float(h) (the
+// scale is not read for a float map).  Feature lifting passes the teacher map at scale 1.
+template <typename TG>
+cudaError_t launch_feature_bwd(const ViewParams& vp, const uint2* ranges, const InstanceLists& lists,
+                               const TG* dL_dfeat_pix, float dL_dfeat_pix_scale, float* dL_dfeature, int* counters,
+                               cudaStream_t s);
 
 // Splat alpha at pixel (pxf, pyf), with the reference's expression trees (forward.cu:340-351, backward.cu:525-535): plain
 // fp32, no _rn intrinsics (see common.cuh).  alpha is 0 where the reference skips the pair (power > 0 or alpha < 1/255)

@@ -375,7 +375,8 @@ template <typename TF>
 cudaError_t launch_composite_fwd(const ViewParams& vp, const uint2* ranges, const uint32_t* point_list,
                                  const SplatRec* rec, const TF* features, const float* bg,
                                  float* final_T, uint32_t* n_contrib, float* out_color,
-                                 TF* out_feature, float* out_depth, int* work_counter, cudaStream_t s) {
+                                 TF* out_feature, float* out_depth, int* counters, cudaStream_t s) {
+    int* const work_counter = counters + kCounterFwd;
     if (vp.C == 0)  // no feature rows or map: one kernel for both element types
         return launch_fwd_t<0, float>(vp, ranges, point_list, rec, nullptr, bg, final_T, n_contrib, out_color, nullptr,
                                       out_depth, work_counter, s);

@@ -30,9 +30,7 @@ struct alignas(128) FeatSmem {  // per warp
 template <typename TG>  // TG: element type of the upstream gradient map, float or __half
 struct FeatArgs {
     const uint2* ranges;
-    const float* list_w;
-    const uint2* list_meta;
-    const uint32_t* list_cnt;
+    InstanceLists lists;
     const TG* dL_dfeat_pix;  // backward: [C, H, W]
     float* dL_dfeature;      // backward: [P, C]
     int* work_counter;
@@ -106,18 +104,18 @@ __global__ void __launch_bounds__(kFeatWarps * 32, 3) feature_bwd_kernel(const F
         const uint32_t rx = __shfl_sync(0xffffffffu, a.ranges[ip.tile].x, 0);
         const uint32_t ry = __shfl_sync(0xffffffffu, a.ranges[ip.tile].y, 0);
         const size_t base = list_begin(rx, ry, ip.b);
-        const uint32_t n = __shfl_sync(0xffffffffu, a.list_cnt[(size_t)ip.tile * kBlocksPerTile + ip.b], 0);
+        const uint32_t n = __shfl_sync(0xffffffffu, a.lists.cnt[(size_t)ip.tile * kBlocksPerTile + ip.b], 0);
         if (n == 0) continue;
         const int ch0 = ip.chunk * CH + cl * 4;
         const uint32_t nch = (n + kListChunk - 1) / kListChunk;
 
         auto load_meta = [&](uint32_t c) -> uint2 {
             const uint32_t e = c * kListChunk + lane;
-            return (lane < kListChunk && e < n) ? __ldg(&a.list_meta[base + e]) : make_uint2(0u, 0u);
+            return (lane < kListChunk && e < n) ? __ldg(&a.lists.meta[base + e]) : make_uint2(0u, 0u);
         };
         auto issue = [&](uint32_t c, int buf) {
             const uint32_t cnt = min((uint32_t)kListChunk, n - c * kListChunk);
-            const float* wsrc = a.list_w + (base + (size_t)c * kListChunk) * 32;
+            const float* wsrc = a.lists.w + (base + (size_t)c * kListChunk) * 32;
             for (uint32_t j = lane; j < cnt * 8; j += 32) cp_async16(&sm.w[buf][0][0] + j * 4, wsrc + j * 4);
             cp_async_commit();
         };
@@ -213,29 +211,29 @@ static cudaError_t launch_feat_bwd_t(const FeatArgs<TG>& a, cudaStream_t s) {
 }
 
 template <typename TG>
-cudaError_t launch_feature_bwd(const ViewParams& vp, const uint2* ranges, const float* list_w, const uint2* list_meta,
-                               const uint32_t* list_cnt, const TG* dL_dfeat_pix, float dL_dfeat_pix_scale,
-                               float* dL_dfeature, int* work_counter, cudaStream_t s) {
+cudaError_t launch_feature_bwd(const ViewParams& vp, const uint2* ranges, const InstanceLists& lists,
+                               const TG* dL_dfeat_pix, float dL_dfeat_pix_scale, float* dL_dfeature, int* counters,
+                               cudaStream_t s) {
     FeatArgs<TG> a;
-    a.ranges = ranges; a.list_w = list_w; a.list_meta = list_meta; a.list_cnt = list_cnt;
+    a.ranges = ranges; a.lists = lists;
     a.dL_dfeat_pix = dL_dfeat_pix;
     a.dL_dfeature = dL_dfeature; a.scale = dL_dfeat_pix_scale;
-    a.work_counter = work_counter;
+    a.work_counter = counters + kCounterFeatureBwd;
     a.W = vp.W; a.H = vp.H; a.C = vp.C; a.tiles_x = (int)vp.grid_x; a.num_tiles = (int)(vp.grid_x * vp.grid_y);
     const int CH = channel_chunk(vp.C);
     a.chunks = (vp.C + CH - 1) / CH;
     a.vec = 0;
     if (vp.C % 4 == 0 && (reinterpret_cast<uintptr_t>(dL_dfeature) & 15) == 0) a.vec |= 1;
     if (vp.W % 4 == 0 && (reinterpret_cast<uintptr_t>(dL_dfeat_pix) & (4 * sizeof(TG) - 1)) == 0) a.vec |= 2;
-    cudaError_t e = cudaMemsetAsync(work_counter, 0, sizeof(int), s);
+    cudaError_t e = cudaMemsetAsync(a.work_counter, 0, sizeof(int), s);
     if (e != cudaSuccess) return e;
     if (CH == 32) return launch_feat_bwd_t<32, TG>(a, s);
     if (CH == 64) return launch_feat_bwd_t<64, TG>(a, s);
     return launch_feat_bwd_t<128, TG>(a, s);
 }
-template cudaError_t launch_feature_bwd(const ViewParams&, const uint2*, const float*, const uint2*, const uint32_t*,
-                                       const float*, float, float*, int*, cudaStream_t);
-template cudaError_t launch_feature_bwd(const ViewParams&, const uint2*, const float*, const uint2*, const uint32_t*,
-                                       const __half*, float, float*, int*, cudaStream_t);
+template cudaError_t launch_feature_bwd(const ViewParams&, const uint2*, const InstanceLists&, const float*, float,
+                                       float*, int*, cudaStream_t);
+template cudaError_t launch_feature_bwd(const ViewParams&, const uint2*, const InstanceLists&, const __half*, float,
+                                       float*, int*, cudaStream_t);
 
 }  // namespace f3dgs

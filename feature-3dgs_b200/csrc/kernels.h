@@ -54,30 +54,32 @@ template <typename TF>
 cudaError_t launch_composite_fwd(const ViewParams& vp, const uint2* ranges, const uint32_t* point_list,
                                  const SplatRec* rec, const TF* features, const float* bg,
                                  float* final_T, uint32_t* n_contrib, float* out_color,
-                                 TF* out_feature, float* out_depth, int* work_counter, cudaStream_t s);
+                                 TF* out_feature, float* out_depth, int* counters, cudaStream_t s);
 
-// ---- composite_bwd.cu: geometric-gradient kernel of the two-kernel backward, two CTAs per SM; with list pointers it
-// also emits the per-(tile, block) blend weights for launch_feature_bwd
-cudaError_t launch_composite_bwd_geom(const ViewParams& vp, const uint2* ranges, const uint32_t* point_list,
-                                      const SplatRec* rec, const float* bg, const float* final_T,
-                                      const uint32_t* n_contrib, const float* dL_dpix, const float* dL_ddepth,
-                                      float* dL_dmean2D, float* dL_dconic, float* dL_dopacity, float* dL_dcolor,
-                                      float* dL_dz, int* work_counter, cudaStream_t s, float* list_w = nullptr,
-                                      uint2* list_meta = nullptr, uint32_t* list_cnt = nullptr);
-// Feature lifting: the lists of the backward's EMIT mode (every pointer required) and weight_sum[P] += the blend weights
-// w = alpha*T of each Gaussian over the view; launch_feature_bwd with the teacher map then adds sum_p w * map[:, p]
-cudaError_t launch_composite_bwd_lift(const ViewParams& vp, const uint2* ranges, const uint32_t* point_list,
-                                      const SplatRec* rec, const float* final_T, const uint32_t* n_contrib,
-                                      float* weight_sum, int* work_counter, cudaStream_t s, float* list_w,
-                                      uint2* list_meta, uint32_t* list_cnt);
-
-// ---- feature_bwd.cu: feature gradient from the instance lists (second kernel of the two-kernel backward).  TG (float or
-// __half) is the element type of the upstream gradient map; a __half map stands for dL/dO = scale * float(h) (the scale is
-// not read for a float map)
+// ---- composite_bwd.cu + feature_bwd.cu: the composite backward of a view, from that view's forward buffers
+struct ForwardBuffers {
+    const uint2* ranges;
+    const uint32_t* point_list;
+    const SplatRec* rec;
+    const float* final_T;
+    const uint32_t* n_contrib;
+    int* counters;  // the image buffer's work-counter region
+    int R;
+};
+// Geometric gradients from a kernel at two CTAs per SM.  With C > 0 and R > 0 that kernel also emits per-(tile, block)
+// instance lists (scratch of the device's default pool, freed on the stream before return), and a second kernel forms
+// dL_dfeature from them.  TG (float or __half) is the element type of dL_dfeat_pix; a __half map stands for
+// dL/dO = scale * float(h) (the scale is not read for a float map)
 template <typename TG>
-cudaError_t launch_feature_bwd(const ViewParams& vp, const uint2* ranges, const float* list_w, const uint2* list_meta,
-                               const uint32_t* list_cnt, const TG* dL_dfeat_pix, float dL_dfeat_pix_scale,
-                               float* dL_dfeature, int* work_counter, cudaStream_t s);
+cudaError_t launch_composite_bwd(const ViewParams& vp, const ForwardBuffers& fb, const float* bg, const float* dL_dpix,
+                                 const float* dL_ddepth, const TG* dL_dfeat_pix, float dL_dfeat_pix_scale,
+                                 float* dL_dmean2D, float* dL_dconic, float* dL_dopacity, float* dL_dcolor, float* dL_dz,
+                                 float* dL_dfeature, cudaStream_t s);
+// Feature lifting, R > 0: weight_sum[P] += the blend weights w = alpha*T of each Gaussian over the view and
+// feature_sum[P, C] += sum_p w * map[:, p], through the same lists.  TF (float or __half) is the element type of map
+template <typename TF>
+cudaError_t launch_feature_lift(const ViewParams& vp, const ForwardBuffers& fb, const TF* map, float* feature_sum,
+                                float* weight_sum, cudaStream_t s);
 
 // ---- feature_head.cu (a float16 map or target gives the result of the float32 one upcast exactly; a float16 gradient
 // is half_rn(out_scale * the float32 one), out_scale not read for a float gradient)
