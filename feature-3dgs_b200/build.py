@@ -5,6 +5,9 @@
   feature-3dgs_b200/diff_gaussian_rasterization/_C*.so   torch/pybind11 binding over the C ABI; g++ only
 
 Usage: python feature-3dgs_b200/build.py [--force]
+
+build_all(out=DIR, defines=[...]) builds a variant (extra -D switches) with the same layout under DIR instead, for tools
+that measure an instrumented library next to the normal one.
 """
 import os
 import subprocess
@@ -15,9 +18,15 @@ from concurrent.futures import ThreadPoolExecutor
 PKG = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(PKG)
 CSRC = os.path.join(PKG, "csrc")
-OBJ = os.path.join(PKG, "build")
-LIB = os.path.join(PKG, "libf3dgs_b200.so")
-EXT = os.path.join(PKG, "diff_gaussian_rasterization", "_C" + sysconfig.get_config_var("EXT_SUFFIX"))
+
+
+def _paths(out):
+    """(object directory, library, torch extension) of a build under `out`"""
+    return (os.path.join(out, "build"), os.path.join(out, "libf3dgs_b200.so"),
+            os.path.join(out, "diff_gaussian_rasterization", "_C" + sysconfig.get_config_var("EXT_SUFFIX")))
+
+
+OBJ, LIB, EXT = _paths(PKG)
 CU = ["api.cu", "preprocess.cu", "binning.cu", "composite_fwd.cu", "composite_bwd.cu", "feature_bwd.cu",
       "feature_head.cu", "feature_decoder.cu", "feature_query.cu", "feature_pca.cu", "image_loss.cu", "optimizer.cu",
       "knn.cu", "densify.cu"]
@@ -44,12 +53,12 @@ def _newer(target, deps):
     return any(os.path.getmtime(d) > t for d in deps)
 
 
-def _flags_changed():
+def _flags_changed(obj_dir, flags):
     """Objects are only reusable for the flags they were built with."""
     import hashlib
 
-    h = hashlib.sha256(" ".join(NVCC_FLAGS).encode()).hexdigest()
-    stamp = os.path.join(OBJ, "flags.sha256")
+    h = hashlib.sha256(" ".join(flags).encode()).hexdigest()
+    stamp = os.path.join(obj_dir, "flags.sha256")
     old = open(stamp).read().strip() if os.path.exists(stamp) else None
     if old != h:
         with open(stamp, "w") as f:
@@ -58,46 +67,50 @@ def _flags_changed():
     return False
 
 
-def build_lib(force=False):
-    os.makedirs(OBJ, exist_ok=True)
-    force = _flags_changed() or force
+def build_lib(force=False, out=PKG, defines=()):
+    obj_dir, lib, _ = _paths(out)
+    flags = NVCC_FLAGS + ["-D" + d for d in defines]
+    os.makedirs(obj_dir, exist_ok=True)
+    force = _flags_changed(obj_dir, flags) or force
     hdrs = [h if os.path.isabs(h) else os.path.join(CSRC, h) for h in HDRS]
     jobs, objs = [], []
     for cu in CU:
-        src, obj = os.path.join(CSRC, cu), os.path.join(OBJ, cu + ".o")
+        src, obj = os.path.join(CSRC, cu), os.path.join(obj_dir, cu + ".o")
         objs.append(obj)
         if force or _newer(obj, [src] + hdrs):
-            jobs.append((["nvcc", "-c", src, "-o", obj] + NVCC_FLAGS, os.path.join(OBJ, cu + ".log")))
+            jobs.append((["nvcc", "-c", src, "-o", obj] + flags, os.path.join(obj_dir, cu + ".log")))
     with ThreadPoolExecutor(max(1, min(len(jobs), os.cpu_count() or 1))) as ex:
         list(ex.map(lambda j: _run(*j), jobs))
-    if force or jobs or not os.path.exists(LIB):
-        _run(["nvcc", "-shared", "-o", LIB] + objs + ["-gencode", "arch=compute_90a,code=sm_90a", "-cudart", "static"])
-    return LIB
+    if force or jobs or not os.path.exists(lib):
+        _run(["nvcc", "-shared", "-o", lib] + objs + ["-gencode", "arch=compute_90a,code=sm_90a", "-cudart", "static"])
+    return lib
 
 
-def build_ext(force=False):
+def build_ext(force=False, out=PKG):
     import torch
     from torch.utils import cpp_extension as ce
 
+    _, lib, ext = _paths(out)
     src = os.path.join(CSRC, "torch_binding.cpp")
-    if not (force or _newer(EXT, [src, os.path.join(ROOT, "include", "f3dgs_b200.h"), LIB])):
-        return EXT
+    if not (force or _newer(ext, [src, os.path.join(ROOT, "include", "f3dgs_b200.h"), lib])):
+        return ext
+    os.makedirs(os.path.dirname(ext), exist_ok=True)
     inc = []
     for p in ce.include_paths() + [sysconfig.get_paths()["include"], "/usr/local/cuda/include"]:
         inc += ["-I", p]
     libs = []
     for p in ce.library_paths():
         libs += ["-L", p, f"-Wl,-rpath,{p}"]
-    _run(["g++", "-shared", "-fPIC", "-O2", "-std=c++17", src, "-o", EXT,
+    _run(["g++", "-shared", "-fPIC", "-O2", "-std=c++17", src, "-o", ext,
           "-DTORCH_EXTENSION_NAME=_C", "-DTORCH_API_INCLUDE_EXTENSION_H",
           f"-D_GLIBCXX_USE_CXX11_ABI={int(torch._C._GLIBCXX_USE_CXX11_ABI)}"] + inc + libs +
-         ["-L", PKG, "-lf3dgs_b200", "-Wl,-rpath,$ORIGIN/..",
+         ["-L", out, "-lf3dgs_b200", "-Wl,-rpath,$ORIGIN/..",
           "-lc10", "-lc10_cuda", "-ltorch_cpu", "-ltorch_cuda", "-ltorch", "-ltorch_python"])
-    return EXT
+    return ext
 
 
-def build_all(force=False):
-    return build_lib(force), build_ext(force)
+def build_all(force=False, out=PKG, defines=()):
+    return build_lib(force, out, defines), build_ext(force, out)
 
 
 if __name__ == "__main__":

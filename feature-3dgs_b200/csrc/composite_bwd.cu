@@ -15,7 +15,7 @@
 //   LIFT           feature lifting: the EMIT lists, and instead of the 10 gradient terms the one value w = alpha*T per pair,
 //       reduced into weight_sum[P] through the same tile; no upstream gradient or background is read.  feature_bwd.cu
 //       then forms sum_p w * map[:, p] over the lists with the teacher map in place of dL/dfeature_map.
-// 12 warps and a ring without weight slots (RingSlim, 106 KB of shared memory with the reduction tiles): two CTAs per SM,
+// 12 warps and a ring without weight slots (RingSlim, 113 KB of shared memory with the reduction tiles): two CTAs per SM,
 // and the alpha warps keep the launch register count (80).
 // As in the reference, the feature loss does not feed dL/dalpha (backward.cu:575 is disabled).
 #include <mutex>
@@ -37,7 +37,7 @@ struct alignas(128) BwdSmem {
     float red[kBlocksPerTile][kRedRows][kRedStride];
     uint32_t red_gid[kBlocksPerTile][kRedSlots];
 };
-static_assert(sizeof(BwdSmem) == 108544, "shared-memory layout changed");
+static_assert(sizeof(BwdSmem) == 115200, "shared-memory layout changed");
 
 struct BwdArgs {
     ProducerArgs pa;
@@ -146,8 +146,9 @@ composite_bwd_kernel(const BwdArgs args) {
         nslots = 0;
     };
 
+    ROLE_CLK(uint32_t clk_full = 0; const uint32_t clk_0 = (uint32_t)clock64();)
     for (;;) {
-        mbar_wait(&ring.full[s], parity);
+        ROLE_CLK_WAIT(clk_full, mbar_wait(&ring.full[s], parity));
         Stage<0>& st = ring.stage[s];
         const uint32_t n = st.n, last = st.last, first = st.first;
         const int work = st.work;
@@ -278,6 +279,10 @@ composite_bwd_kernel(const BwdArgs args) {
         if (last && nslots > 0) flush();
         if (++s == kStages) { s = 0; parity ^= 1; }
     }
+    ROLE_CLK(if (lane == 0) {
+        ROLE_CLK_ADD(kClkAlphaFull, clk_full);
+        ROLE_CLK_ADD(kClkAlphaLoop, (uint32_t)clock64() - clk_0);
+    })
 }
 
 // Stream-ordered scratch for the instance lists (the reference's backward allocates its scratch too,
@@ -317,7 +322,7 @@ static cudaError_t run_bwd(BwdArgs a, const ViewParams& vp, const ForwardBuffers
     // every instantiation is opted in to the shared memory it needs on the first launch of any of them on a device
     int num_sms = 0;
     cudaError_t e = device_sms<composite_bwd_kernel<BwdMode::GEOM>, composite_bwd_kernel<BwdMode::EMIT>,
-                               composite_bwd_kernel<BwdMode::LIFT>>(num_sms, sizeof(BwdSmem));
+                               composite_bwd_kernel<BwdMode::LIFT>>(num_sms, sizeof(BwdSmem), kBwdThreads, kSlimCtas);
     if (e == cudaSuccess) e = cudaMemsetAsync(a.pa.work_counter, 0, sizeof(int), s);
     if (e == cudaSuccess) {
         composite_bwd_kernel<MODE><<<min(a.pa.num_tiles, kSlimCtas * num_sms), kBwdThreads, sizeof(BwdSmem), s>>>(a);
@@ -364,3 +369,7 @@ template cudaError_t launch_feature_lift(const ViewParams&, const ForwardBuffers
                                          cudaStream_t);
 
 }  // namespace f3dgs
+
+#ifdef F3DGS_ROLE_CLOCKS
+ROLE_CLK_EXPORT(f3dgs_role_clocks_bwd)
+#endif

@@ -6,7 +6,9 @@
 //
 //   producer group (4)    warp 0 walks the tile's slice of the depth-sorted instance list, drops the
 //                         instances whose alpha >= 1/255 footprint cannot reach the tile, and fills
-//                         a ring of stages with 48-byte splat records via 128-bit loads.  When there
+//                         a ring of stages with 48-byte splat records.  The records reach it through a
+//                         small shared-memory queue (RecQueue) that cp.async fills kPrefetch chunks of 32
+//                         ahead of the cull, across the boundary to the next tile.  When there
 //                         are features, warp 1 (the copy warp) fetches the stage's C-wide feature
 //                         rows (float32 or float16: the ring's element type TF) with 1-D TMA bulk
 //                         copies (cp.async.bulk -> UBLKCP) that complete on the stage's `full` mbarrier.  The producer runs ahead across tile
@@ -72,6 +74,14 @@ struct alignas(128) WSlot {
 };
 static_assert(sizeof(WSlot) == 4352, "weight slot layout changed");  // 4244 bytes of fields, padded to 128
 
+// The producer's record queue: splat records on their way from global memory to the producer warp, kPrefetch chunks of
+// 32 records, filled by cp.async (in-flight copies hold no registers) and read back by the lane that issued the copy.
+constexpr int kPrefetch = 4;
+struct alignas(16) RecQueue {
+    float4 q[kPrefetch][3][32];  // [slot][16-byte third of the 48-byte record][lane]
+    uint32_t id[kPrefetch][32];  // Gaussian index
+};
+
 // WB x WJ: dimensions of the weight-slot ring (pixel blocks x slots per block)
 template <int CH, typename TF = float, int WB = kBlocksPerTile, int WJ = kWSlots>
 struct alignas(128) RingV2 {
@@ -85,18 +95,20 @@ struct alignas(128) RingV2 {
     uint64_t wfull[WB][WJ];
     uint64_t wempty[WB][WJ];
     uint32_t done_mask[kDoneSlots];  // bit b set: pixel block b of that work item needs no more instances
+    RecQueue rq;                     // private to the producer warp: no barrier guards it
 };
 
 // The ring without feature rows and with a single weight slot, for the backward geometry kernel, which has no feature
-// warps: 14 KB instead of 83 KB of shared memory, so that two CTAs fit on an SM.  The one-element `ws` / `wfull` /
+// warps: 22 KB instead of 86 KB of shared memory, so that two CTAs fit on an SM.  The one-element `ws` / `wfull` /
 // `wempty` are not used; ring_init<> initialises the two barriers.
 using RingSlim = RingV2<0, float, 1, 1>;
 
-static_assert(sizeof(RingV2<0>) == 81664 && sizeof(RingSlim) == 16128, "ring layout changed");
-static_assert(sizeof(RingV2<32>) == 106240 && sizeof(RingV2<64>) == 130816 && sizeof(RingV2<128>) == 179968,
+static_assert(sizeof(RecQueue) == 6656, "record queue layout changed");
+static_assert(sizeof(RingV2<0>) == 88320 && sizeof(RingSlim) == 22784, "ring layout changed");
+static_assert(sizeof(RingV2<32>) == 112896 && sizeof(RingV2<64>) == 137472 && sizeof(RingV2<128>) == 186624,
               "ring layout changed");
-static_assert(sizeof(RingV2<32, __half>) == 93952 && sizeof(RingV2<64, __half>) == 106240 &&
-                  sizeof(RingV2<128, __half>) == 130816,
+static_assert(sizeof(RingV2<32, __half>) == 100608 && sizeof(RingV2<64, __half>) == 112896 &&
+                  sizeof(RingV2<128, __half>) == 137472,
               "ring layout changed");
 
 // ---------------------------------------------------------------- pixel-block layout
@@ -282,6 +294,59 @@ __device__ __forceinline__ bool footprint_hits_rect(const float4 r0, const float
     return q <= tau;
 }
 
+// ---------------------------------------------------------------- role clocks
+// Who waits for whom: compiled with -DF3DGS_ROLE_CLOCKS (tools/time_composite_roles.py; off in the normal build, whose
+// SASS is what it is without these lines) every warp of composite_fwd.cu / composite_bwd.cu adds the cycles it spent
+// in each mbarrier wait of its role, and in its whole loop, to g_role_clocks of its translation unit.
+enum RoleClock {
+    kClkProdEmpty, kClkProdLoop,                    // producer: wait for a free stage; whole loop
+    kClkAlphaFull, kClkAlphaWempty, kClkAlphaLoop,  // alpha warps: wait for a stage, for a weight slot; whole loop
+    kClkFeatWfull, kClkFeatFull, kClkFeatLoop,      // feature warps: wait for a weight slot, for the feature rows
+    kRoleClocks
+};
+#ifdef F3DGS_ROLE_CLOCKS
+static __device__ unsigned long long g_role_clocks[kRoleClocks];
+// 32-bit cycle counts (a kernel runs far less than 2^32 cycles): the producer has 40 registers
+#define ROLE_CLK(...) __VA_ARGS__
+#define ROLE_CLK_WAIT(acc, wait)                      \
+    do {                                              \
+        const uint32_t clk_t_ = (uint32_t)clock64();  \
+        wait;                                         \
+        acc += (uint32_t)clock64() - clk_t_;          \
+    } while (0)
+#define ROLE_CLK_ADD(slot, cycles) atomicAdd(&g_role_clocks[slot], (unsigned long long)(cycles))
+// g_role_clocks of this translation unit -> out[kRoleClocks]; reset != 0 zeroes them afterwards
+#define ROLE_CLK_EXPORT(name)                                                                              \
+    extern "C" int name(unsigned long long* out, int reset) {                                              \
+        cudaError_t e = cudaMemcpyFromSymbol(out, f3dgs::g_role_clocks, sizeof(f3dgs::g_role_clocks));     \
+        const unsigned long long zero[f3dgs::kRoleClocks] = {};                                            \
+        if (e == cudaSuccess && reset) e = cudaMemcpyToSymbol(f3dgs::g_role_clocks, zero, sizeof(zero));   \
+        return (int)e;                                                                                     \
+    }
+#else
+#define ROLE_CLK(...)
+#define ROLE_CLK_WAIT(acc, wait) wait
+#endif
+
+// ---------------------------------------------------------------- cp.async (16 bytes per copy, commit groups)
+__device__ __forceinline__ void cp_async16(void* dst_smem, const void* src_gmem) {
+    asm volatile("cp.async.ca.shared.global [%0], [%1], 16;" ::"r"(smem_u32(dst_smem)), "l"(src_gmem) : "memory");
+}
+__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
+// wait until at most the N newest commit groups of this thread are pending
+template <int N>
+__device__ __forceinline__ void cp_async_wait() {
+    asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory");
+}
+// the same for a warp-uniform run-time count n; n >= kPrefetch - 1 waits for all but the kPrefetch - 1 newest
+__device__ __forceinline__ void cp_async_wait_pending(uint32_t n) {
+    static_assert(kPrefetch <= 4, "one case per count below kPrefetch - 1");
+    if (n >= (uint32_t)kPrefetch - 1u) cp_async_wait<kPrefetch - 1>();
+    else if (n == 2) cp_async_wait<2>();
+    else if (n == 1) cp_async_wait<1>();
+    else cp_async_wait<0>();
+}
+
 template <int N>
 __device__ __forceinline__ void reg_dec() {
     asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N));
@@ -348,9 +413,11 @@ inline int channel_chunk(int C) { return C <= 32 ? 32 : (C <= 64 ? 64 : 128); }
 // SM count of the current device.  The first call for a device ordinal also opts the kernels K in to `smem` bytes of
 // dynamic shared memory: the opt-in is per device (context), so the count is remembered per ordinal and one process
 // driving several GPUs works too.  A failed opt-in is returned and retried on the next call; an ordinal of 64 or more
-// returns cudaErrorInvalidDevice and leaves `sms` as it is.
+// returns cudaErrorInvalidDevice and leaves `sms` as it is.  With min_ctas > 0 the first call also checks that min_ctas CTAs
+// of `threads` threads of every K are resident per SM with that shared memory, and fails with
+// cudaErrorLaunchOutOfResources if not: a kernel planned for two CTAs per SM must not silently run at one.
 template <auto... K>
-cudaError_t device_sms(int& sms, size_t smem) {
+cudaError_t device_sms(int& sms, size_t smem, int threads = 0, int min_ctas = 0) {
     static std::atomic<int> sms_of_device[64];  // zero-initialised; set once per device (idempotent)
     int dev = 0;
     cudaGetDevice(&dev);
@@ -359,6 +426,12 @@ cudaError_t device_sms(int& sms, size_t smem) {
         for (const void* k : std::initializer_list<const void*>{reinterpret_cast<const void*>(K)...}) {
             const cudaError_t e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
             if (e != cudaSuccess) return e;
+            int ctas = min_ctas;
+            if (min_ctas > 0) {
+                const cudaError_t eo = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ctas, k, threads, smem);
+                if (eo != cudaSuccess) return eo;
+            }
+            if (ctas < min_ctas) return cudaErrorLaunchOutOfResources;
         }
         int n = 0;
         cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
@@ -381,7 +454,8 @@ __device__ __forceinline__ void producer_loop(RING& ring, const ProducerArgs& pa
     const int lane = threadIdx.x & 31;
     int s = 0;
     uint32_t empty_parity = 1;  // fresh barrier: waiting on parity 1 falls through
-    mbar_wait(&ring.empty[0], empty_parity);
+    ROLE_CLK(uint32_t clk_empty = 0; const uint32_t clk_0 = (uint32_t)clock64();)
+    ROLE_CLK_WAIT(clk_empty, mbar_wait(&ring.empty[0], empty_parity));
 
     uint32_t seq = 0;  // work items this CTA has started
     auto publish = [&](uint32_t n, uint32_t last, uint32_t first, int work) {
@@ -404,35 +478,108 @@ __device__ __forceinline__ void producer_loop(RING& ring, const ProducerArgs& pa
             s = 0;
             empty_parity ^= 1;
         }
-        mbar_wait_sleep(&ring.empty[s], empty_parity, 64);  // the producer runs stages ahead: sleep, do not spin
+        // the producer runs stages ahead: sleep, do not spin
+        ROLE_CLK_WAIT(clk_empty, mbar_wait_sleep(&ring.empty[s], empty_parity, 64));
     };
 
+    // ---- the prefetch stream: the record chunks of this CTA's work items, in walk order, copied into ring.rq ahead of
+    // their use.  `issued` and `taken` count chunks over the whole kernel; chunk number g lives in slot g % kPrefetch.
     const int num_work = pa.num_tiles * pa.chunks;
-    int pending = 0;  // lane 0: the next work item, requested one item ahead so the atomic's round trip is hidden
-    if (lane == 0) pending = atomicAdd(pa.work_counter, 1);
+    struct Walk {
+        int work;               // >= num_work: no more work
+        uint32_t begin, count;  // first instance of the tile's list; instances to visit
+    };
+    auto load_walk = [&](int work) {
+        Walk w{work, 0u, 0u};
+        if (work < num_work) {
+            const int tile = work / pa.chunks;
+            const uint2 range = pa.ranges[tile];
+            w.begin = range.x;
+            w.count = range.y - range.x;
+            if (REVERSE) {
+                // nothing behind the deepest last-contributor of the tile is ever used
+                const int tile_x = tile % pa.tiles_x, tile_y = tile / pa.tiles_x;
+                uint32_t tmax = 0;
+                const int yy = tile_y * 16 + (lane >> 1), xb = tile_x * 16 + (lane & 1) * 8;
+                if (yy < pa.H)
+                    for (int i = 0; i < 8; i++)
+                        if (xb + i < pa.W) tmax = max(tmax, pa.n_contrib[(size_t)yy * pa.W + xb + i]);
+#pragma unroll
+                for (int o = 16; o > 0; o >>= 1) tmax = max(tmax, __shfl_xor_sync(0xffffffffu, tmax, o));
+                w.count = min(w.count, tmax);
+            }
+        }
+        return w;
+    };
+    // i-th visited element of a walk -> index into point_list
+    auto list_index = [&](uint32_t begin, uint32_t count, uint32_t i) -> uint32_t {
+        return REVERSE ? (begin + count - 1 - i) : (begin + i);
+    };
+
+    // Work ids are requested two items ahead (lane 0): `cur` is walked, `nxt` is the item whose first chunks are
+    // prefetched while cur's last ones are consumed, and `pending` hides the atomic's round trip.
+    int pending = 0;
+    Walk cur, nxt;
+    {
+        int w0 = 0, w1 = 0;
+        if (lane == 0) {
+            w0 = atomicAdd(pa.work_counter, 1);
+            w1 = atomicAdd(pa.work_counter, 1);
+            pending = atomicAdd(pa.work_counter, 1);
+        }
+        cur = load_walk(__shfl_sync(0xffffffffu, w0, 0));
+        nxt = load_walk(__shfl_sync(0xffffffffu, w1, 0));
+    }
+    // Issue cursor: chunk `ic` of the walk (ibegin, icount), which is cur's or, once every chunk of cur is issued, nxt's
+    // (in_nxt); id_iss is this lane's Gaussian id of that chunk, loaded one issue ahead of its record copy.  The cursor
+    // is exhausted (ic * 32 >= icount) only in nxt: there is no look-ahead beyond the next work item.
+    RecQueue& rq = ring.rq;
+    uint32_t issued = 0, taken = 0;
+    uint32_t ibegin = cur.begin, icount = cur.count, ic = 0, id_iss = 0;
+    bool in_nxt = false;
+    auto load_id = [&]() -> uint32_t {
+        const uint32_t i = ic * 32 + lane;
+        return i < icount ? pa.point_list[list_index(ibegin, icount, i)] : 0u;
+    };
+    auto cursor_cross = [&]() -> bool {  // past cur's last chunk: on to nxt
+        if (in_nxt || ic * 32 < icount) return false;
+        in_nxt = true;
+        ibegin = nxt.begin;
+        icount = nxt.count;
+        ic = 0;
+        return true;
+    };
+    // Copies the cursor's chunk into slot issued % kPrefetch, one commit group per chunk.  That slot held chunk
+    // issued - kPrefetch: wait_group kPrefetch - 1 completes that group before the slot is rewritten, whether the chunk
+    // was consumed or dropped by an early exit, so a dropped copy can never land on top of a newer one.
+    auto issue = [&]() {
+        cp_async_wait<kPrefetch - 1>();
+        const uint32_t slot = issued % kPrefetch;
+        if (ic * 32 + lane < icount) {
+            const float4* r = reinterpret_cast<const float4*>(pa.rec + id_iss);
+            cp_async16(&rq.q[slot][0][lane], r);
+            cp_async16(&rq.q[slot][1][lane], r + 1);
+            cp_async16(&rq.q[slot][2][lane], r + 2);
+            rq.id[slot][lane] = id_iss;
+        }
+        cp_async_commit();
+        issued++;
+        ic++;
+        cursor_cross();
+        id_iss = load_id();
+    };
+    cursor_cross();
+    id_iss = load_id();
+
     for (;;) {
-        const int work = __shfl_sync(0xffffffffu, pending, 0);
-        if (lane == 0 && work < num_work) pending = atomicAdd(pa.work_counter, 1);
+        const int work = cur.work;
         if (work >= num_work) {
             publish(0, 1, 1, -1);
             break;
         }
         const int tile = work / pa.chunks, chunk = work - tile * pa.chunks;
         const int tile_x = tile % pa.tiles_x, tile_y = tile / pa.tiles_x;
-        const uint2 range = pa.ranges[tile];
-        const uint32_t range_begin = range.x;
-        uint32_t walk_count = range.y - range.x;
-        if (REVERSE) {
-            // nothing behind the deepest last-contributor of the tile is ever used
-            uint32_t tmax = 0;
-            const int yy = tile_y * 16 + (lane >> 1), xb = tile_x * 16 + (lane & 1) * 8;
-            if (yy < pa.H)
-                for (int i = 0; i < 8; i++)
-                    if (xb + i < pa.W) tmax = max(tmax, pa.n_contrib[(size_t)yy * pa.W + xb + i]);
-#pragma unroll
-            for (int o = 16; o > 0; o >>= 1) tmax = max(tmax, __shfl_xor_sync(0xffffffffu, tmax, o));
-            walk_count = min(walk_count, tmax);
-        }
+        const uint32_t range_begin = cur.begin, walk_count = cur.count;
         const float tx0 = (float)(tile_x * 16), ty0 = (float)(tile_y * 16), tx1 = tx0 + 15.f, ty1 = ty0 + 15.f;
         const int chunk_off = chunk * CH;
         const int row_floats = (CH > 0 && pa.features != nullptr) ? min(CH, pa.C - chunk_off) : 0;
@@ -441,9 +588,6 @@ __device__ __forceinline__ void producer_loop(RING& ring, const ProducerArgs& pa
         if (lane == 0) *reinterpret_cast<volatile uint32_t*>(done) = 0;
         __syncwarp();
 
-        auto list_index = [&](uint32_t i) -> uint32_t {  // i-th visited element -> index into point_list
-            return REVERSE ? (range_begin + walk_count - 1 - i) : (range_begin + i);
-        };
         auto store_entry = [&](uint32_t slot, uint32_t gid, uint32_t lpos, float4 r0, float4 r1, float4 r2) {
             Stage<CH, TF>& st = ring.stage[s];
             st.rec0[slot] = r0;
@@ -459,30 +603,29 @@ __device__ __forceinline__ void producer_loop(RING& ring, const ProducerArgs& pa
         };
 
         uint32_t fill = 0, first = 1;
-        // two-deep software pipeline on the dependent loads (list index -> id -> record)
         const uint32_t nchunks = (walk_count + 31) / 32;
-        uint32_t id_cur = 0, id_nxt = 0;
-        float4 a0, a1, a2;
-        a0 = a1 = a2 = make_float4(0.f, 0.f, 0.f, 0.f);
-        if (nchunks > 0) {
-            if (lane < walk_count) id_cur = pa.point_list[list_index(lane)];
-            if (32 + lane < walk_count) id_nxt = pa.point_list[list_index(32 + lane)];
-            if (lane < walk_count) {
-                const float4* r = reinterpret_cast<const float4*>(pa.rec + id_cur);
-                a0 = __ldg(r); a1 = __ldg(r + 1); a2 = __ldg(r + 2);
-            }
-        }
         for (uint32_t c = 0; c < nchunks; c++) {
-            if (*reinterpret_cast<volatile uint32_t*>(done) == (1u << kBlocksPerTile) - 1u) break;
-            float4 b0, b1, b2;
-            b0 = b1 = b2 = make_float4(0.f, 0.f, 0.f, 0.f);
-            const uint32_t i1 = (c + 1) * 32 + lane, i2 = (c + 2) * 32 + lane;
-            uint32_t id_nn = 0;
-            if (i1 < walk_count) {
-                const float4* r = reinterpret_cast<const float4*>(pa.rec + id_nxt);
-                b0 = __ldg(r); b1 = __ldg(r + 1); b2 = __ldg(r + 2);
+            if (*reinterpret_cast<volatile uint32_t*>(done) == (1u << kBlocksPerTile) - 1u) {
+                // Early exit: the issued chunks of this walk are dropped by stepping `taken` over them, and the cursor
+                // moves on to nxt.  Their copies may still be in flight; the slot sequence keeps running, and issue()
+                // waits for a slot's previous group before it rewrites the slot.
+                taken += (in_nxt ? nchunks : ic) - c;
+                if (!in_nxt) {
+                    ic = nchunks;
+                    cursor_cross();
+                    id_iss = load_id();
+                }
+                break;
             }
-            if (i2 < walk_count) id_nn = pa.point_list[list_index(i2)];
+            // this chunk and kPrefetch - 1 chunks behind it in flight, across the boundary to the next work item
+            while (issued - taken < (uint32_t)kPrefetch && ic * 32 < icount) issue();
+            cp_async_wait_pending(issued - taken - 1);  // groups newer than this chunk's may still be in flight
+            __syncwarp();
+            const uint32_t qs = taken % kPrefetch;
+            taken++;
+            // every lane reads back what it copied itself: conflict-free LDS.128
+            const float4 a0 = rq.q[qs][0][lane], a1 = rq.q[qs][1][lane], a2 = rq.q[qs][2][lane];
+            const uint32_t id_cur = rq.id[qs][lane];
 
             const uint32_t i0 = c * 32 + lane;
             const bool valid = i0 < walk_count;
@@ -491,7 +634,7 @@ __device__ __forceinline__ void producer_loop(RING& ring, const ProducerArgs& pa
             const uint32_t m = __ballot_sync(0xffffffffu, keep);
             const uint32_t cnt = __popc(m);
             const uint32_t rank = __popc(m & ((1u << lane) - 1u));
-            const uint32_t lpos = list_index(i0) - range_begin + 1;
+            const uint32_t lpos = list_index(range_begin, walk_count, i0) - range_begin + 1;
             const uint32_t room = kStageEntries - fill;
             if (keep && rank < room) store_entry(fill + rank, id_cur, lpos, a0, a1, a2);
             if (cnt >= room) {
@@ -503,13 +646,23 @@ __device__ __forceinline__ void producer_loop(RING& ring, const ProducerArgs& pa
             } else {
                 fill += cnt;
             }
-            a0 = b0; a1 = b1; a2 = b2;
-            id_cur = id_nxt;
-            id_nxt = id_nn;
         }
         publish(fill, 1, first, work);
         advance();
+
+        // next work item.  Every chunk of cur was issued or stepped over, so the cursor is in nxt.
+        const int new_work = __shfl_sync(0xffffffffu, pending, 0);
+        if (lane == 0 && new_work < num_work) pending = atomicAdd(pa.work_counter, 1);
+        cur = nxt;
+        nxt = load_walk(new_work);
+        in_nxt = false;
+        if (cursor_cross()) id_iss = load_id();
     }
+    cp_async_wait<0>();  // dropped copies land before the warp retires
+    ROLE_CLK(if (lane == 0) {
+        ROLE_CLK_ADD(kClkProdEmpty, clk_empty);
+        ROLE_CLK_ADD(kClkProdLoop, (uint32_t)clock64() - clk_0);
+    })
 }
 
 // Second warp of the producer group (forward with features): fetches the feature rows of each listed stage.

@@ -122,8 +122,9 @@ composite_fwd_kernel(const FwdArgs<TF> args) {
         uint32_t last_contrib = 0;
         int px = 0, py = 0, chunk = 0;
         bool done = true, inside = false, blk_done = true;
+        ROLE_CLK(uint32_t clk_full = 0, clk_wempty = 0; const uint32_t clk_0 = (uint32_t)clock64();)
         for (;;) {
-            mbar_wait(&ring.full[s], parity);
+            ROLE_CLK_WAIT(clk_full, mbar_wait(&ring.full[s], parity));
             Stage<CH, TF>& st = ring.stage[s];
             const uint32_t n = st.n, last = st.last, first = st.first;
             const int work = st.work;
@@ -145,7 +146,7 @@ composite_fwd_kernel(const FwdArgs<TF> args) {
                 if (blk_done && lane == 0) atomicOr(&ring.done_mask[st.done_slot], 1u << b);
             }
             WSlot* ws = &ring.ws[b][j];
-            if (CH > 0) mbar_wait(&ring.wempty[b][j], wparity);
+            if (CH > 0) ROLE_CLK_WAIT(clk_wempty, mbar_wait(&ring.wempty[b][j], wparity));
             uint32_t km0 = 0, km1 = 0;  // instances that blended a pixel of rows 0-1 / rows 2-3
             if (!blk_done && n > 0) {
                 bool hit = false;
@@ -227,6 +228,11 @@ composite_fwd_kernel(const FwdArgs<TF> args) {
             if (++s == kStages) { s = 0; parity ^= 1; }
             if (CH > 0 && ++j == kWSlots) { j = 0; wparity ^= 1; }
         }
+        ROLE_CLK(if (lane == 0) {
+            ROLE_CLK_ADD(kClkAlphaFull, clk_full);
+            ROLE_CLK_ADD(kClkAlphaWempty, clk_wempty);
+            ROLE_CLK_ADD(kClkAlphaLoop, (uint32_t)clock64() - clk_0);
+        })
         if (CH > 0) {  // tell the feature warps of this block that the work is over
             mbar_wait(&ring.wempty[b][j], wparity);
             if (lane == 0) {
@@ -270,14 +276,15 @@ composite_fwd_kernel(const FwdArgs<TF> args) {
         } while (0)
         int s = 0, j = 0;
         uint32_t parity = 0, wparity = 0;
+        ROLE_CLK(uint32_t clk_wfull = 0, clk_full = 0; const uint32_t clk_0 = (uint32_t)clock64();)
         for (;;) {
-            mbar_wait(&ring.wfull[b][j], wparity);
+            ROLE_CLK_WAIT(clk_wfull, mbar_wait(&ring.wfull[b][j], wparity));
             const WSlot& ws = ring.ws[b][j];
             const int work = ws.work;
             if (work < 0) break;
             uint32_t km = ws.km[h];
             const uint32_t last = ws.last;
-            mbar_wait(&ring.full[s], parity);  // feature rows landed
+            ROLE_CLK_WAIT(clk_full, mbar_wait(&ring.full[s], parity));  // feature rows landed
             const Stage<CH, TF>& st = ring.stage[s];
             // the next instance's pixel mask and feature float4 are requested before this instance's FMAs, so their
             // LDS latency hides behind the FMA stream instead of heading every instance
@@ -335,6 +342,11 @@ composite_fwd_kernel(const FwdArgs<TF> args) {
             if (++s == kStages) { s = 0; parity ^= 1; }
             if (++j == kWSlots) { j = 0; wparity ^= 1; }
         }
+        ROLE_CLK(if (lane == 0) {
+            ROLE_CLK_ADD(kClkFeatWfull, clk_wfull);
+            ROLE_CLK_ADD(kClkFeatFull, clk_full);
+            ROLE_CLK_ADD(kClkFeatLoop, (uint32_t)clock64() - clk_0);
+        })
     }
 #undef FEAT_ROW_FMA
 }
@@ -394,3 +406,7 @@ template cudaError_t launch_composite_fwd<__half>(const ViewParams&, const uint2
                                                   float*, int*, cudaStream_t);
 
 }  // namespace f3dgs
+
+#ifdef F3DGS_ROLE_CLOCKS
+ROLE_CLK_EXPORT(f3dgs_role_clocks_fwd)
+#endif

@@ -40,15 +40,6 @@ struct FeatArgs {
     float scale;
 };
 
-__device__ __forceinline__ void cp_async16(void* dst_smem, const void* src_gmem) {
-    asm volatile("cp.async.ca.shared.global [%0], [%1], 16;" ::"r"(smem_u32(dst_smem)), "l"(src_gmem) : "memory");
-}
-__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
-template <int N>
-__device__ __forceinline__ void cp_async_wait() {
-    asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory");
-}
-
 // Decode a work item.  Blocks of one tile are neighbours in the item order, so the workers that run at the same time
 // mostly share their instances' feature rows in L2.
 struct ItemPos {
