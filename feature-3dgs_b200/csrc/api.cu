@@ -439,7 +439,8 @@ int backward_impl(const Api& api, bool accumulate, int P, int D, int M, int R, i
                   float dL_dfeaturepix_scale, const float* dL_depths, float* dL_dmean2D, float* dL_dconic,
                   float* dL_dopacity, float* dL_dcolor, float* dL_dsemantic_feature, float* dL_dmean3D, float* dL_dcov3D,
                   float* dL_dsh, float* dL_dscale, float* dL_drot, float* dL_dz, float* grad_accum, float* denom,
-                  cudaEvent_t composite_done, int debug, cudaStream_t stream, const Range& zero = {nullptr, 0}) {
+                  float* dL_dcamera, cudaEvent_t composite_done, int debug, cudaStream_t stream,
+                  const Range& zero = {nullptr, 0}) {
     if (P < 0 || width <= 0 || height <= 0 || C < 0 || C > F3DGS_MAX_FEATURE_DIM || R < 0)
         return api.invalid("bad sizes");
     if (P == 0) return 0;
@@ -457,6 +458,15 @@ int backward_impl(const Api& api, bool accumulate, int P, int D, int M, int R, i
         // the feature kernel reduces into dL_dsemantic_feature while other warps still read the map
         if (overlaps({dL_dsemantic_feature, (size_t)P * C * 4}, {{dL_dfeaturepix, (size_t)C * width * height * 2}}))
             return api.invalid("dL_dsemantic_feature overlaps dL_dfeaturepix");
+    }
+    if (dL_dcamera) {
+        const size_t p4 = (size_t)P * 4;
+        const Range outs[] = {{dL_dmean2D, 3 * p4}, {dL_dconic, 4 * p4}, {dL_dopacity, p4}, {dL_dcolor, 3 * p4},
+                              {dL_dsemantic_feature, (size_t)C * p4}, {dL_dmean3D, 3 * p4}, {dL_dcov3D, 6 * p4},
+                              {dL_dsh, (size_t)M * 3 * p4}, {dL_dscale, 3 * p4}, {dL_drot, 4 * p4}, {dL_dz, p4},
+                              {grad_accum, p4}, {denom, p4}, zero};
+        if (overlaps({dL_dcamera, F3DGS_CAMERA_GRAD_FLOATS * sizeof(float)}, outs))
+            return api.invalid("dL_dcamera overlaps another output");
     }
     if (zero.p) CUDA_TRY(cudaMemsetAsync(const_cast<void*>(zero.p), 0, zero.bytes, stream));
 
@@ -479,10 +489,14 @@ int backward_impl(const Api& api, bool accumulate, int P, int D, int M, int R, i
     if (composite_done) CUDA_TRY(cudaEventRecord(composite_done, stream));
     {
         StageTimer t(F3DGS_STAGE_PREPROCESS_BWD, stream);
-        launch_preprocess_bwd(vp, means3D, radii, shs, clamped, scales, rotations, cov3d, dL_dmean2D, dL_dconic,
-                              dL_dmean3D, dL_dcolor, dL_dcov3D, dL_dsh, dL_dscale, dL_drot, dL_dz, stream, accumulate,
-                              grad_accum, denom);
+        e = launch_preprocess_bwd(vp, means3D, radii, shs, clamped, scales, rotations, cov3d, dL_dmean2D, dL_dconic,
+                                  dL_dmean3D, dL_dcolor, dL_dcov3D, dL_dsh, dL_dscale, dL_drot, dL_dz, stream,
+                                  accumulate, grad_accum, denom, dL_dcamera);
     }
+    if (e == cudaErrorMemoryAllocation)
+        return api.fail(F3DGS_ERR_ALLOC, std::string("cudaMallocAsync for the camera-gradient partials failed: ") +
+                                             cudaGetErrorString(e));
+    CUDA_TRY(e);
     STAGE_CHECK("preprocess_bwd");
     return 0;
 }
@@ -507,7 +521,7 @@ int f3dgs_backward(int P, int D, int M, int R, int C, const float* background, i
                          scale_modifier, rotations, cov3D_precomp, viewmatrix, projmatrix, cam_pos, tan_fovx, tan_fovy,
                          radii, geom_buffer, binning_buffer, image_buffer, dL_dpix, dL_dfeaturepix, 1.f, dL_depths,
                          dL_dmean2D, dL_dconic, dL_dopacity, dL_dcolor, dL_dsemantic_feature, dL_dmean3D, dL_dcov3D, dL_dsh,
-                         dL_dscale, dL_drot, dL_dz, nullptr, nullptr, nullptr, debug, (cudaStream_t)cuda_stream);
+                         dL_dscale, dL_drot, dL_dz, nullptr, nullptr, nullptr, nullptr, debug, (cudaStream_t)cuda_stream);
 }
 
 int f3dgs_backward_f16(int P, int D, int M, int R, int C, const float* background, int width, int height,
@@ -527,7 +541,53 @@ int f3dgs_backward_f16(int P, int D, int M, int R, int C, const float* backgroun
                          radii, geom_buffer, binning_buffer, image_buffer, dL_dpix,
                          reinterpret_cast<const __half*>(dL_dfeaturepix), dL_dfeaturepix_scale, dL_depths, dL_dmean2D,
                          dL_dconic, dL_dopacity, dL_dcolor, dL_dsemantic_feature, dL_dmean3D, dL_dcov3D, dL_dsh, dL_dscale,
-                         dL_drot, dL_dz, nullptr, nullptr, nullptr, debug, (cudaStream_t)cuda_stream);
+                         dL_drot, dL_dz, nullptr, nullptr, nullptr, nullptr, debug, (cudaStream_t)cuda_stream);
+}
+
+int f3dgs_backward_cam(int P, int D, int M, int R, int C, const float* background, int width, int height,
+                       const float* means3D, const float* shs, const float* colors_precomp,
+                       const float* semantic_feature, const float* scales, float scale_modifier,
+                       const float* rotations, const float* cov3D_precomp, const float* viewmatrix,
+                       const float* projmatrix, const float* cam_pos, float tan_fovx, float tan_fovy,
+                       const int* radii, char* geom_buffer, char* binning_buffer, char* image_buffer,
+                       const float* dL_dpix, const float* dL_dfeaturepix, const float* dL_depths, float* dL_dmean2D,
+                       float* dL_dconic, float* dL_dopacity, float* dL_dcolor, float* dL_dsemantic_feature,
+                       float* dL_dmean3D, float* dL_dcov3D, float* dL_dsh, float* dL_dscale, float* dL_drot,
+                       float* dL_dz, int debug, void* cuda_stream, float* dL_dcamera) {
+    (void)semantic_feature;
+    (void)colors_precomp;
+    const Api api(__func__);
+    if (!dL_dcamera) return api.invalid("NULL dL_dcamera");
+    return backward_impl(api, false, P, D, M, R, C, background, width, height, means3D, shs, scales, scale_modifier,
+                         rotations, cov3D_precomp, viewmatrix, projmatrix, cam_pos, tan_fovx, tan_fovy, radii,
+                         geom_buffer, binning_buffer, image_buffer, dL_dpix, dL_dfeaturepix, 1.f, dL_depths, dL_dmean2D,
+                         dL_dconic, dL_dopacity, dL_dcolor, dL_dsemantic_feature, dL_dmean3D, dL_dcov3D, dL_dsh,
+                         dL_dscale, dL_drot, dL_dz, nullptr, nullptr, dL_dcamera, nullptr, debug,
+                         (cudaStream_t)cuda_stream);
+}
+
+int f3dgs_backward_cam_f16(int P, int D, int M, int R, int C, const float* background, int width, int height,
+                           const float* means3D, const float* shs, const float* colors_precomp,
+                           const float* semantic_feature, const float* scales, float scale_modifier,
+                           const float* rotations, const float* cov3D_precomp, const float* viewmatrix,
+                           const float* projmatrix, const float* cam_pos, float tan_fovx, float tan_fovy,
+                           const int* radii, char* geom_buffer, char* binning_buffer, char* image_buffer,
+                           const float* dL_dpix, const uint16_t* dL_dfeaturepix, float dL_dfeaturepix_scale,
+                           const float* dL_depths, float* dL_dmean2D, float* dL_dconic, float* dL_dopacity,
+                           float* dL_dcolor, float* dL_dsemantic_feature, float* dL_dmean3D, float* dL_dcov3D,
+                           float* dL_dsh, float* dL_dscale, float* dL_drot, float* dL_dz, int debug,
+                           void* cuda_stream, float* dL_dcamera) {
+    (void)semantic_feature;
+    (void)colors_precomp;
+    const Api api(__func__);
+    if (!dL_dcamera) return api.invalid("NULL dL_dcamera");
+    return backward_impl(api, false, P, D, M, R, C, background, width, height, means3D, shs, scales, scale_modifier,
+                         rotations, cov3D_precomp, viewmatrix, projmatrix, cam_pos, tan_fovx, tan_fovy, radii,
+                         geom_buffer, binning_buffer, image_buffer, dL_dpix,
+                         reinterpret_cast<const __half*>(dL_dfeaturepix), dL_dfeaturepix_scale, dL_depths, dL_dmean2D,
+                         dL_dconic, dL_dopacity, dL_dcolor, dL_dsemantic_feature, dL_dmean3D, dL_dcov3D, dL_dsh,
+                         dL_dscale, dL_drot, dL_dz, nullptr, nullptr, dL_dcamera, nullptr, debug,
+                         (cudaStream_t)cuda_stream);
 }
 
 size_t f3dgs_backward_scratch_bytes(int P) { return P > 0 ? ScratchLayout((size_t)P).bytes : 0; }
@@ -546,11 +606,15 @@ int backward_accum_impl(const char* entry, int P, int D, int M, int R, int C, co
                         const float* dL_depths, char* scratch, float* dL_dopacity, float* dL_dcolors_precomp,
                         float* dL_dsemantic_feature, float* dL_dmean3D, float* dL_dcov3D_precomp, float* dL_dsh,
                         float* dL_dscale, float* dL_drot, float* dL_dmean2D_out, float* grad_accum, float* denom,
-                        void* composite_done_event, int debug, void* cuda_stream) {
+                        void* composite_done_event, int debug, void* cuda_stream, bool camera = false,
+                        float* dL_dcamera = nullptr) {
     const Api api(entry);
     cudaStream_t stream = (cudaStream_t)cuda_stream;
+    if (camera && !dL_dcamera) return api.invalid("NULL dL_dcamera");
     if (P <= 0) return P == 0 ? 0 : api.invalid("bad sizes");
     if (!scratch) return api.invalid("NULL scratch");
+    if (overlaps({dL_dcamera, F3DGS_CAMERA_GRAD_FLOATS * sizeof(float)}, {{dL_dmean2D_out, (size_t)P * 3 * 4}}))
+        return api.invalid("dL_dcamera overlaps another output");
     if ((colors_precomp != nullptr) != (dL_dcolors_precomp != nullptr) ||
         (cov3D_precomp != nullptr) != (dL_dcov3D_precomp != nullptr))
         return api.invalid("dL_dcolors_precomp / dL_dcov3D_precomp go with colors_precomp / cov3D_precomp");
@@ -564,7 +628,7 @@ int backward_accum_impl(const char* entry, int P, int D, int M, int R, int C, co
         rotations, cov3D_precomp, viewmatrix, projmatrix, cam_pos, tan_fovx, tan_fovy, radii, geom_buffer,
         binning_buffer, image_buffer, dL_dpix, dL_dfeaturepix, dL_dfeaturepix_scale, dL_depths, m2d,
         reinterpret_cast<float*>(scratch + sl.conic), dL_dopacity, dcol, dL_dsemantic_feature, dL_dmean3D, dcov, dL_dsh,
-        dL_dscale, dL_drot, reinterpret_cast<float*>(scratch + sl.dz), grad_accum, denom,
+        dL_dscale, dL_drot, reinterpret_cast<float*>(scratch + sl.dz), grad_accum, denom, dL_dcamera,
         (cudaEvent_t)composite_done_event, debug, stream, {scratch, sl.bytes});
     if (rc < 0) return rc;
     if (dL_dmean2D_out)
@@ -611,6 +675,45 @@ int f3dgs_backward_accum_f16(int P, int D, int M, int R, int C, const float* bac
                                dL_dopacity, dL_dcolors_precomp, dL_dsemantic_feature, dL_dmean3D, dL_dcov3D_precomp,
                                dL_dsh, dL_dscale, dL_drot, dL_dmean2D_out, grad_accum, denom, composite_done_event, debug,
                                cuda_stream);
+}
+
+int f3dgs_backward_accum_cam(int P, int D, int M, int R, int C, const float* background, int width, int height,
+                             const float* means3D, const float* shs, const float* colors_precomp, const float* scales,
+                             float scale_modifier, const float* rotations, const float* cov3D_precomp,
+                             const float* viewmatrix, const float* projmatrix, const float* cam_pos, float tan_fovx,
+                             float tan_fovy, const int* radii, char* geom_buffer, char* binning_buffer,
+                             char* image_buffer, const float* dL_dpix, const float* dL_dfeaturepix,
+                             const float* dL_depths, char* scratch, float* dL_dopacity, float* dL_dcolors_precomp,
+                             float* dL_dsemantic_feature, float* dL_dmean3D, float* dL_dcov3D_precomp, float* dL_dsh,
+                             float* dL_dscale, float* dL_drot, float* dL_dmean2D_out, float* grad_accum, float* denom,
+                             void* composite_done_event, int debug, void* cuda_stream, float* dL_dcamera) {
+    return backward_accum_impl(__func__, P, D, M, R, C, background, width, height, means3D, shs, colors_precomp, scales,
+                               scale_modifier, rotations, cov3D_precomp, viewmatrix, projmatrix, cam_pos, tan_fovx,
+                               tan_fovy, radii, geom_buffer, binning_buffer, image_buffer, dL_dpix, dL_dfeaturepix, 1.f,
+                               dL_depths, scratch, dL_dopacity, dL_dcolors_precomp, dL_dsemantic_feature, dL_dmean3D,
+                               dL_dcov3D_precomp, dL_dsh, dL_dscale, dL_drot, dL_dmean2D_out, grad_accum, denom,
+                               composite_done_event, debug, cuda_stream, true, dL_dcamera);
+}
+
+int f3dgs_backward_accum_cam_f16(int P, int D, int M, int R, int C, const float* background, int width, int height,
+                                 const float* means3D, const float* shs, const float* colors_precomp,
+                                 const float* scales, float scale_modifier, const float* rotations,
+                                 const float* cov3D_precomp, const float* viewmatrix, const float* projmatrix,
+                                 const float* cam_pos, float tan_fovx, float tan_fovy, const int* radii,
+                                 char* geom_buffer, char* binning_buffer, char* image_buffer, const float* dL_dpix,
+                                 const uint16_t* dL_dfeaturepix, float dL_dfeaturepix_scale, const float* dL_depths,
+                                 char* scratch, float* dL_dopacity, float* dL_dcolors_precomp,
+                                 float* dL_dsemantic_feature, float* dL_dmean3D, float* dL_dcov3D_precomp,
+                                 float* dL_dsh, float* dL_dscale, float* dL_drot, float* dL_dmean2D_out,
+                                 float* grad_accum, float* denom, void* composite_done_event, int debug,
+                                 void* cuda_stream, float* dL_dcamera) {
+    return backward_accum_impl(__func__, P, D, M, R, C, background, width, height, means3D, shs, colors_precomp, scales,
+                               scale_modifier, rotations, cov3D_precomp, viewmatrix, projmatrix, cam_pos, tan_fovx,
+                               tan_fovy, radii, geom_buffer, binning_buffer, image_buffer, dL_dpix,
+                               reinterpret_cast<const __half*>(dL_dfeaturepix), dL_dfeaturepix_scale, dL_depths, scratch,
+                               dL_dopacity, dL_dcolors_precomp, dL_dsemantic_feature, dL_dmean3D, dL_dcov3D_precomp,
+                               dL_dsh, dL_dscale, dL_drot, dL_dmean2D_out, grad_accum, denom, composite_done_event, debug,
+                               cuda_stream, true, dL_dcamera);
 }
 
 }  // extern "C"

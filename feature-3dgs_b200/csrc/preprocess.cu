@@ -317,7 +317,18 @@ __device__ __forceinline__ void put(float* __restrict__ dst, float v) {
 // shared memory: rows come in and go out with coalesced 128-bit accesses, each thread works on its own (padded,
 // conflict-free) row in between.
 
-template <bool ACCUM>
+// Camera gradient (CAM = true).  Each visible Gaussian contributes kCamTerms floats, slot j:
+//   j = 3k + r       (k = 0..3, r = 0..2)      dL/dviewmatrix[4k + r]   view-space mean, depth and W of T = W J
+//   j = 12 + 3k + i  (k = 0..3, r = 0, 1, 3)  dL/dprojmatrix[4k + r]   screen-space mean
+//   j = 24 + k       (k = 0..2)                dL/dcampos[k]            SH view direction
+// The other 8 matrix entries (vm[3,7,11,15], pm[2,6,10,14]) are never read by the forward: their gradient is 0.
+constexpr int kCamTerms = 27;
+__host__ __device__ constexpr int cam_slot(int j) {  // slot -> index in the 35-float camera gradient
+    return j < 12 ? 4 * (j / 3) + j % 3
+                  : j < 24 ? 16 + 4 * ((j - 12) / 3) + ((j - 12) % 3 == 2 ? 3 : (j - 12) % 3) : 32 + (j - 24);
+}
+
+template <bool ACCUM, bool CAM>
 __global__ void __launch_bounds__(kBwdBlock)
 preprocess_bwd_kernel(ViewParams vp, const float* __restrict__ means3D, const int* __restrict__ radii,
                       const float* __restrict__ shs, const uint8_t* __restrict__ clamped,
@@ -326,7 +337,8 @@ preprocess_bwd_kernel(ViewParams vp, const float* __restrict__ means3D, const in
                       const float* __restrict__ dL_dconic, float* __restrict__ dL_dmean3D,
                       const float* __restrict__ dL_dcolor, float* __restrict__ dL_dcov3D,
                       float* __restrict__ dL_dsh, float* __restrict__ dL_dscale, float* __restrict__ dL_drot,
-                      const float* __restrict__ dL_dz, float* __restrict__ grad_accum, float* __restrict__ vis_count) {
+                      const float* __restrict__ dL_dz, float* __restrict__ grad_accum, float* __restrict__ vis_count,
+                      double* __restrict__ cam_part) {
     extern __shared__ float bwd_smem[];
     const int idx = blockIdx.x * blockDim.x + threadIdx.x;
     const int row_floats = vp.M * 3, stride = bwd_row_stride(row_floats);
@@ -353,6 +365,11 @@ preprocess_bwd_kernel(ViewParams vp, const float* __restrict__ means3D, const in
         // gradient rows start as zeros: degrees above the active one are not written by the owner thread
         for (int i = threadIdx.x; i < kBwdBlock * stride; i += kBwdBlock) dsh_rows[i] = 0.f;
         __syncthreads();
+    }
+    float cg[kCamTerms];  // CAM: this Gaussian's camera terms (slots above), 0 for a culled one
+    if constexpr (CAM) {
+#pragma unroll
+        for (int j = 0; j < kCamTerms; j++) cg[j] = 0.f;
     }
     if (visible) {
     if (ACCUM && grad_accum != nullptr) {
@@ -426,6 +443,24 @@ preprocess_bwd_kernel(ViewParams vp, const float* __restrict__ means3D, const in
     float gx = vm[0] * dL_dtx + vm[1] * dL_dty + vm[2] * dL_dtz;
     float gy = vm[4] * dL_dtx + vm[5] * dL_dty + vm[6] * dL_dtz;
     float gz = vm[8] * dL_dtx + vm[9] * dL_dty + vm[10] * dL_dtz;
+    if constexpr (CAM) {
+        // t_r = xf(vm, r, p) gives dL/dvm[4k + r] = dL/dt_r p_k; T.c[a][k] = sum_r vm[4k + r] J.c[a][r] gives the W term
+        // (J.c[0] = (fx/tz, 0, -fx tx/tz^2), J.c[1] = (0, fy/tz, -fy ty/tz^2), J.c[2] = 0)
+        const float p[4] = {mx, my, mz, 1.f};
+        const float dT0[3] = {dL_dT00, dL_dT01, dL_dT02}, dT1[3] = {dL_dT10, dL_dT11, dL_dT12};
+        const float J00 = h_x * tz, J11 = h_y * tz, J02 = -h_x * c2.tx * tz2, J12 = -h_y * c2.ty * tz2;
+#pragma unroll
+        for (int k = 0; k < 4; k++) {
+            cg[3 * k] = dL_dtx * p[k];
+            cg[3 * k + 1] = dL_dty * p[k];
+            cg[3 * k + 2] = dL_dtz * p[k];
+            if (k < 3) {
+                cg[3 * k] += dT0[k] * J00;
+                cg[3 * k + 1] += dT1[k] * J11;
+                cg[3 * k + 2] += dT0[k] * J02 + dT1[k] * J12;
+            }
+        }
+    }
 
     // ---- screen-space mean and depth (reference backward.cu:372-395)
     {
@@ -442,6 +477,18 @@ preprocess_bwd_kernel(ViewParams vp, const float* __restrict__ means3D, const in
         ay += dldz * vm[6];
         az += dldz * vm[10];
         gx += ax; gy += ay; gz += az;
+        if constexpr (CAM) {
+            // proj = (h_0, h_1) m_w with h_r = xf(pm, r, p): dL/dh_0 = m_w d2x, dL/dh_1 = m_w d2y,
+            // dL/dh_3 = -(mul1 d2x + mul2 d2y); depth = xf(vm, 2, p)
+            const float p[4] = {mx, my, mz, 1.f};
+            const float gh[3] = {m_w * d2x, m_w * d2y, -(mul1 * d2x + mul2 * d2y)};
+#pragma unroll
+            for (int k = 0; k < 4; k++) {
+                cg[3 * k + 2] += dldz * p[k];
+#pragma unroll
+                for (int i = 0; i < 3; i++) cg[12 + 3 * k + i] = gh[i] * p[k];
+            }
+        }
     }
 
     // ---- SH backward (reference backward.cu:20-139)
@@ -528,6 +575,15 @@ preprocess_bwd_kernel(ViewParams vp, const float* __restrict__ means3D, const in
 #undef WR
         const F3 dm = dnormvdv3(dir_orig, F3{ddx, ddy, ddz});
         gx += dm.x; gy += dm.y; gz += dm.z;
+        if constexpr (CAM) {
+            // dir_orig = p - campos: dL/dcampos = -dm.  dm is recomputed from opaque copies of its inputs rather than
+            // read: a second use of dm's products would change how the compiler contracts `gx += dm.x` into FMAs, and
+            // so the bits of dL_dmean3D, which must equal those of the CAM = false kernel.
+            F3 v = dir_orig, dv = F3{ddx, ddy, ddz};
+            asm("" : "+f"(v.x), "+f"(v.y), "+f"(v.z), "+f"(dv.x), "+f"(dv.y), "+f"(dv.z));
+            const F3 dmc = dnormvdv3(v, dv);
+            cg[24] = -dmc.x; cg[25] = -dmc.y; cg[26] = -dmc.z;
+        }
     }
     put<ACCUM>(dL_dmean3D + 3 * idx, gx);
     put<ACCUM>(dL_dmean3D + 3 * idx + 1, gy);
@@ -615,6 +671,44 @@ preprocess_bwd_kernel(ViewParams vp, const float* __restrict__ means3D, const in
             }
         }
     }
+    if constexpr (CAM) {
+        // fixed-order block reduction: float32 warp shuffles, then the four warp sums in float64 -> cam_part[block][27]
+        __shared__ float cam_warp[kBwdBlock / 32][kCamTerms];
+        const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+#pragma unroll
+        for (int j = 0; j < kCamTerms; j++) {
+            float v = cg[j];
+#pragma unroll
+            for (int o = 16; o > 0; o >>= 1) v += __shfl_down_sync(0xffffffffu, v, o);
+            if (lane == 0) cam_warp[warp][j] = v;
+        }
+        __syncthreads();
+        if (threadIdx.x < kCamTerms) {
+            double s = 0.0;
+#pragma unroll
+            for (int w = 0; w < kBwdBlock / 32; w++) s += (double)cam_warp[w][threadIdx.x];
+            cam_part[(size_t)blockIdx.x * kCamTerms + threadIdx.x] = s;
+        }
+    }
+}
+
+// dL_dcamera[cam_slot(j)] += the float64 sum of the blocks' partials of slot j (one CTA per slot; each thread sums a
+// fixed stride of blocks in index order, then a fixed tree), rounded once to float32
+constexpr int kCamSumThreads = 256;
+__global__ void __launch_bounds__(kCamSumThreads)
+camera_grad_sum_kernel(int blocks, const double* __restrict__ cam_part, float* __restrict__ dL_dcamera) {
+    __shared__ double s[kCamSumThreads];
+    const int j = blockIdx.x;
+    double a = 0.0;
+    for (int b = threadIdx.x; b < blocks; b += kCamSumThreads) a += cam_part[(size_t)b * kCamTerms + j];
+    s[threadIdx.x] = a;
+    __syncthreads();
+#pragma unroll
+    for (int w = kCamSumThreads / 2; w > 0; w >>= 1) {
+        if (threadIdx.x < w) s[threadIdx.x] += s[threadIdx.x + w];
+        __syncthreads();
+    }
+    if (threadIdx.x == 0) dL_dcamera[cam_slot(j)] += (float)s[0];
 }
 
 // -------------------------------------------------------------------------------- launchers
@@ -632,32 +726,52 @@ void launch_preprocess_fwd(const ViewParams& vp, const float* means3D, const flo
     g_launches++;
 }
 
-void launch_preprocess_bwd(const ViewParams& vp, const float* means3D, const int* radii, const float* shs,
-                           const uint8_t* clamped, const float* scales, const float* rotations,
-                           const float* cov3D, const float* dL_dmean2D, const float* dL_dconic,
-                           float* dL_dmean3D, const float* dL_dcolor, float* dL_dcov3D, float* dL_dsh,
-                           float* dL_dscale, float* dL_drot, const float* dL_dz, cudaStream_t s, bool accumulate,
-                           float* grad_accum, float* denom) {
-    if (vp.P <= 0) return;
+cudaError_t launch_preprocess_bwd(const ViewParams& vp, const float* means3D, const int* radii, const float* shs,
+                                  const uint8_t* clamped, const float* scales, const float* rotations,
+                                  const float* cov3D, const float* dL_dmean2D, const float* dL_dconic,
+                                  float* dL_dmean3D, const float* dL_dcolor, float* dL_dcov3D, float* dL_dsh,
+                                  float* dL_dscale, float* dL_drot, const float* dL_dz, cudaStream_t s, bool accumulate,
+                                  float* grad_accum, float* denom, float* dL_dcamera) {
+    if (vp.P <= 0) return cudaSuccess;
     const size_t smem = shs ? (size_t)2 * kBwdBlock * bwd_row_stride(vp.M * 3) * sizeof(float) + kBwdBlock : 0;
     static std::atomic<int> attr_set{0};
     int dev = 0;
     cudaGetDevice(&dev);
     if (smem > 48 * 1024 && !((attr_set.load() >> (dev & 31)) & 1)) {  // once per device; harmless if repeated
-        cudaFuncSetAttribute(preprocess_bwd_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024);
-        cudaFuncSetAttribute(preprocess_bwd_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024);
+        cudaFuncSetAttribute(preprocess_bwd_kernel<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024);
+        cudaFuncSetAttribute(preprocess_bwd_kernel<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024);
+        cudaFuncSetAttribute(preprocess_bwd_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024);
+        cudaFuncSetAttribute(preprocess_bwd_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024);
         attr_set.fetch_or(1 << (dev & 31));
     }
     const int grid = (vp.P + kBwdBlock - 1) / kBwdBlock;
+    if (dL_dcamera == nullptr) {
+        if (accumulate)
+            preprocess_bwd_kernel<true, false><<<grid, kBwdBlock, smem, s>>>(
+                vp, means3D, radii, shs, clamped, scales, rotations, cov3D, dL_dmean2D, dL_dconic, dL_dmean3D,
+                dL_dcolor, dL_dcov3D, dL_dsh, dL_dscale, dL_drot, dL_dz, grad_accum, denom, nullptr);
+        else
+            preprocess_bwd_kernel<false, false><<<grid, kBwdBlock, smem, s>>>(
+                vp, means3D, radii, shs, clamped, scales, rotations, cov3D, dL_dmean2D, dL_dconic, dL_dmean3D,
+                dL_dcolor, dL_dcov3D, dL_dsh, dL_dscale, dL_drot, dL_dz, nullptr, nullptr, nullptr);
+        g_launches++;
+        return cudaSuccess;  // a launch error is left for the caller's cudaGetLastError
+    }
+    // the block partials come from the device's default memory pool, stream-ordered like the launches
+    double* part = nullptr;
+    cudaError_t e = cudaMallocAsync((void**)&part, (size_t)grid * kCamTerms * sizeof(double), s);
+    if (e != cudaSuccess) return e;
     if (accumulate)
-        preprocess_bwd_kernel<true><<<grid, kBwdBlock, smem, s>>>(
+        preprocess_bwd_kernel<true, true><<<grid, kBwdBlock, smem, s>>>(
             vp, means3D, radii, shs, clamped, scales, rotations, cov3D, dL_dmean2D, dL_dconic, dL_dmean3D, dL_dcolor,
-            dL_dcov3D, dL_dsh, dL_dscale, dL_drot, dL_dz, grad_accum, denom);
+            dL_dcov3D, dL_dsh, dL_dscale, dL_drot, dL_dz, grad_accum, denom, part);
     else
-        preprocess_bwd_kernel<false><<<grid, kBwdBlock, smem, s>>>(
+        preprocess_bwd_kernel<false, true><<<grid, kBwdBlock, smem, s>>>(
             vp, means3D, radii, shs, clamped, scales, rotations, cov3D, dL_dmean2D, dL_dconic, dL_dmean3D, dL_dcolor,
-            dL_dcov3D, dL_dsh, dL_dscale, dL_drot, dL_dz, nullptr, nullptr);
-    g_launches++;
+            dL_dcov3D, dL_dsh, dL_dscale, dL_drot, dL_dz, nullptr, nullptr, part);
+    camera_grad_sum_kernel<<<kCamTerms, kCamSumThreads, 0, s>>>(grid, part, dL_dcamera);
+    g_launches += 2;
+    return cudaFreeAsync(part, s);
 }
 
 void launch_mark_visible(int P, const float* means3D, const float* viewmatrix, uint8_t* present,

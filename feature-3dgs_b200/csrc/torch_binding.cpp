@@ -7,6 +7,8 @@
 //   rasterize_gaussians_backward(...) -> (dL_dmeans2D, dL_dcolors, dL_dsemantic_feature, dL_dopacity,
 //                                         dL_dmeans3D, dL_dcov3D, dL_dsh, dL_dscales, dL_drotations)
 //   mark_visible(means3D, viewmatrix, projmatrix) -> bool[P]
+// plus rasterize_gaussians_backward_camera(same arguments as rasterize_gaussians_backward) -> its 9 gradients +
+// (dL_dviewmatrix [4,4], dL_dprojmatrix [4,4], dL_dcampos [3]) for pose refinement (f3dgs_backward_cam).
 // Differences (all permissive): the feature width is read from semantic_feature.size(-1) at run
 // time (reference: compile-time NUM_SEMANTIC_CHANNELS, config.h:16); an empty / undefined
 // semantic_feature means C = 0; semantic_feature may be float32 or float16, and the feature map
@@ -163,9 +165,12 @@ RasterizeGaussiansCUDA(const torch::Tensor& background, const torch::Tensor& mea
     return std::make_tuple(rendered, out_color, out_feature, out_depth, radii, geomBuffer, binningBuffer, imgBuffer);
 }
 
-std::tuple<torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor,
-           torch::Tensor, torch::Tensor>
-RasterizeGaussiansBackwardCUDA(const torch::Tensor& background, const torch::Tensor& means3D,
+using BackwardGrads = std::tuple<torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor,
+                                 torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor>;
+
+// Body of rasterize_gaussians_backward and rasterize_gaussians_backward_camera: with a non-NULL camera (35 floats on the
+// device), the _cam entries, which add the camera gradient to it
+static BackwardGrads backward_grads(const torch::Tensor& background, const torch::Tensor& means3D,
                                const torch::Tensor& radii, const torch::Tensor& colors,
                                const torch::Tensor& semantic_feature, const torch::Tensor& scales,
                                const torch::Tensor& rotations, const float scale_modifier,
@@ -175,7 +180,7 @@ RasterizeGaussiansBackwardCUDA(const torch::Tensor& background, const torch::Ten
                                const torch::Tensor& dL_dout_depth, const torch::Tensor& sh, const int degree,
                                const torch::Tensor& campos, const torch::Tensor& geomBuffer, const int R,
                                const torch::Tensor& binningBuffer, const torch::Tensor& imageBuffer,
-                               const bool debug) {
+                               const bool debug, float* camera) {
     TORCH_CHECK(means3D.is_cuda(), "means3D must be a CUDA tensor (this build has no CPU path)");
     const c10::cuda::CUDAGuard guard(means3D.device());
     const auto dev = means3D.device();
@@ -218,28 +223,70 @@ RasterizeGaussiansBackwardCUDA(const torch::Tensor& background, const torch::Ten
         auto rad = radii.contiguous();
         auto gb = geomBuffer.contiguous(), bb = binningBuffer.contiguous(), ib = imageBuffer.contiguous();
         cudaStream_t stream = c10::cuda::getCurrentCUDAStream().stream();
-        // gs: the float16 symbol's scale after the map, nothing for the float32 one
-        auto run = [&](auto fn, auto gp, auto... gs) {
-            return fn(P, degree, M, R, C, fptr(bg), W, H, fptr(m3), fptr(shc), fptr(col), nullptr, fptr(sc),
-                      scale_modifier, fptr(rot), fptr(cov), fptr(vm), fptr(pm), fptr(cp), tan_fovx, tan_fovy,
-                      rad.data_ptr<int>(), reinterpret_cast<char*>(gb.data_ptr()),
-                      reinterpret_cast<char*>(bb.data_ptr()), reinterpret_cast<char*>(ib.data_ptr()), fptr(gc), gp,
-                      gs..., fptr(gd), dL_dmeans2D.data_ptr<float>(), dL_dconic.data_ptr<float>(),
-                      dL_dopacity.data_ptr<float>(), dL_dcolors.data_ptr<float>(),
-                      C ? dL_dsemantic_feature.data_ptr<float>() : nullptr, dL_dmeans3D.data_ptr<float>(),
-                      dL_dcov3D.data_ptr<float>(), M ? dL_dsh.data_ptr<float>() : nullptr,
-                      dL_dscales.data_ptr<float>(), dL_drotations.data_ptr<float>(), dL_dz.data_ptr<float>(),
-                      debug ? 1 : 0, (void*)stream);
+        // scale: the float16 symbol's scale after the map, () for the float32 one; tail: (dL_dcamera) or ()
+        auto run = [&](auto fn, auto gp, auto scale, auto tail) {
+            return std::apply(
+                fn, std::tuple_cat(
+                        std::make_tuple(P, degree, M, R, C, fptr(bg), W, H, fptr(m3), fptr(shc), fptr(col), nullptr,
+                                        fptr(sc), scale_modifier, fptr(rot), fptr(cov), fptr(vm), fptr(pm), fptr(cp),
+                                        tan_fovx, tan_fovy, rad.data_ptr<int>(), reinterpret_cast<char*>(gb.data_ptr()),
+                                        reinterpret_cast<char*>(bb.data_ptr()), reinterpret_cast<char*>(ib.data_ptr()),
+                                        fptr(gc), gp),
+                        scale,
+                        std::make_tuple(fptr(gd), dL_dmeans2D.data_ptr<float>(), dL_dconic.data_ptr<float>(),
+                                        dL_dopacity.data_ptr<float>(), dL_dcolors.data_ptr<float>(),
+                                        C ? dL_dsemantic_feature.data_ptr<float>() : nullptr,
+                                        dL_dmeans3D.data_ptr<float>(), dL_dcov3D.data_ptr<float>(),
+                                        M ? dL_dsh.data_ptr<float>() : nullptr, dL_dscales.data_ptr<float>(),
+                                        dL_drotations.data_ptr<float>(), dL_dz.data_ptr<float>(), debug ? 1 : 0,
+                                        (void*)stream),
+                        tail));
         };
-        call_f32_or_f16(gf, f3dgs_backward, "f3dgs_backward", f3dgs_backward_f16, "f3dgs_backward_f16",
-                        [&](auto fn, auto gp) {
-                            if constexpr (std::is_same_v<decltype(gp), uint16_t*>) return run(fn, gp, 1.0f);
-                            else return run(fn, gp);
-                        });
+        auto dispatch = [&](auto tail) {
+            return [&, tail](auto fn, auto gp) {
+                if constexpr (std::is_same_v<decltype(gp), uint16_t*>) return run(fn, gp, std::make_tuple(1.0f), tail);
+                else return run(fn, gp, std::tuple<>(), tail);
+            };
+        };
+        if (camera)
+            call_f32_or_f16(gf, f3dgs_backward_cam, "f3dgs_backward_cam", f3dgs_backward_cam_f16,
+                            "f3dgs_backward_cam_f16", dispatch(std::make_tuple(camera)));
+        else
+            call_f32_or_f16(gf, f3dgs_backward, "f3dgs_backward", f3dgs_backward_f16, "f3dgs_backward_f16",
+                            dispatch(std::tuple<>()));
     }
     return std::make_tuple(dL_dmeans2D, dL_dcolors, dL_dsemantic_feature, dL_dopacity, dL_dmeans3D, dL_dcov3D, dL_dsh,
                            dL_dscales, dL_drotations);
 }
+
+#define BACKWARD_PARAMS                                                                                                \
+    const torch::Tensor &background, const torch::Tensor &means3D, const torch::Tensor &radii,                        \
+        const torch::Tensor &colors, const torch::Tensor &semantic_feature, const torch::Tensor &scales,              \
+        const torch::Tensor &rotations, const float scale_modifier, const torch::Tensor &cov3D_precomp,               \
+        const torch::Tensor &viewmatrix, const torch::Tensor &projmatrix, const float tan_fovx, const float tan_fovy, \
+        const torch::Tensor &dL_dout_color, const torch::Tensor &dL_dout_feature, const torch::Tensor &dL_dout_depth, \
+        const torch::Tensor &sh, const int degree, const torch::Tensor &campos, const torch::Tensor &geomBuffer,       \
+        const int R, const torch::Tensor &binningBuffer, const torch::Tensor &imageBuffer, const bool debug
+#define BACKWARD_ARGS                                                                                                  \
+    background, means3D, radii, colors, semantic_feature, scales, rotations, scale_modifier, cov3D_precomp,           \
+        viewmatrix, projmatrix, tan_fovx, tan_fovy, dL_dout_color, dL_dout_feature, dL_dout_depth, sh, degree, campos, \
+        geomBuffer, R, binningBuffer, imageBuffer, debug
+
+BackwardGrads RasterizeGaussiansBackwardCUDA(BACKWARD_PARAMS) { return backward_grads(BACKWARD_ARGS, nullptr); }
+
+// rasterize_gaussians_backward's 9 gradients + (dL_dviewmatrix [4,4], dL_dprojmatrix [4,4], dL_dcampos [3]), each in the
+// layout of its input (f3dgs_backward_cam / _cam_f16)
+decltype(std::tuple_cat(BackwardGrads(), std::tuple<torch::Tensor, torch::Tensor, torch::Tensor>()))
+RasterizeGaussiansBackwardCameraCUDA(BACKWARD_PARAMS) {
+    TORCH_CHECK(means3D.is_cuda(), "means3D must be a CUDA tensor (this build has no CPU path)");
+    const c10::cuda::CUDAGuard guard(means3D.device());
+    torch::Tensor cam = torch::zeros({F3DGS_CAMERA_GRAD_FLOATS}, means3D.options().dtype(torch::kFloat32));
+    return std::tuple_cat(backward_grads(BACKWARD_ARGS, cam.data_ptr<float>()),
+                          std::make_tuple(cam.narrow(0, 0, 16).view({4, 4}), cam.narrow(0, 16, 16).view({4, 4}),
+                                          cam.narrow(0, 32, 3)));
+}
+#undef BACKWARD_PARAMS
+#undef BACKWARD_ARGS
 
 // Accumulating backward for view batches (additive to the reference module): gradients are ADDED into the tensors the
 // caller passes (typically views of one flat gradient buffer, see diff_gaussian_rasterization/parallel.py); nothing is
@@ -254,7 +301,8 @@ void RasterizeGaussiansBackwardAccumCUDA(
     torch::Tensor scratch, torch::Tensor g_means3D, torch::Tensor g_sh, torch::Tensor g_colors,
     torch::Tensor g_semantic_feature, torch::Tensor g_opacities, torch::Tensor g_scales, torch::Tensor g_rotations,
     torch::Tensor g_cov3D, torch::Tensor g_means2D_out, torch::Tensor grad_accum, torch::Tensor denom,
-    const int64_t composite_done_event, const bool debug, const double feature_grad_scale) {
+    const int64_t composite_done_event, const bool debug, const double feature_grad_scale,
+    const std::optional<torch::Tensor>& camera_grad) {
     TORCH_CHECK(means3D.is_cuda(), "means3D must be a CUDA tensor (this build has no CPU path)");
     const c10::cuda::CUDAGuard guard(means3D.device());
     const auto dev = means3D.device();
@@ -283,30 +331,53 @@ void RasterizeGaussiansBackwardAccumCUDA(
     TORCH_CHECK(scratch.defined() && scratch.is_cuda() && scratch.scalar_type() == torch::kByte &&
                     scratch.is_contiguous() && (size_t)scratch.numel() >= need,
                 "scratch must be a contiguous uint8 CUDA tensor of at least ", need, " bytes");
+    // camera_grad (optional): 35 contiguous float32 on the device, ADDED to by the _accum_cam entries
+    float* cam = nullptr;
+    if (camera_grad.has_value() && camera_grad->defined()) {
+        TORCH_CHECK(camera_grad->numel() == F3DGS_CAMERA_GRAD_FLOATS, "camera_grad must have ",
+                    F3DGS_CAMERA_GRAD_FLOATS, " elements (got ", camera_grad->numel(), ")");
+        cam = in_place(*camera_grad, dev, F3DGS_CAMERA_GRAD_FLOATS, "camera_grad");
+    }
     cudaStream_t stream = c10::cuda::getCurrentCUDAStream().stream();
-    auto run = [&](auto fn, auto gp, auto... gs) {  // gs: the float16 symbol's scale after the map
-        return fn(P, degree, M, R, C, fptr(bg), W, H, fptr(m3), fptr(shc), fptr(col), fptr(sc), scale_modifier, fptr(rot),
-                  fptr(cov), fptr(vm), fptr(pm), fptr(cp), tan_fovx, tan_fovy, rad.data_ptr<int>(),
-                  reinterpret_cast<char*>(geomBuffer.data_ptr()), reinterpret_cast<char*>(binningBuffer.data_ptr()),
-                  reinterpret_cast<char*>(imageBuffer.data_ptr()), fptr(gc), gp, gs..., fptr(gd),
-                  reinterpret_cast<char*>(scratch.data_ptr()), in_place(g_opacities, dev, P, "g_opacities"),
-                  in_place(g_colors, dev, (int64_t)P * 3, "g_colors_precomp"),
-                  in_place(g_semantic_feature, dev, (int64_t)P * C, "g_semantic_feature"),
-                  in_place(g_means3D, dev, (int64_t)P * 3, "g_means3D"),
-                  in_place(g_cov3D, dev, (int64_t)P * 6, "g_cov3D_precomp"),
-                  in_place(g_sh, dev, (int64_t)P * M * 3, "g_sh"), in_place(g_scales, dev, (int64_t)P * 3, "g_scales"),
-                  in_place(g_rotations, dev, (int64_t)P * 4, "g_rotations"),
-                  in_place(g_means2D_out, dev, (int64_t)P * 3, "g_means2D_out"),
-                  in_place(grad_accum, dev, P, "grad_accum"), in_place(denom, dev, P, "denom"),
-                  reinterpret_cast<void*>(static_cast<intptr_t>(composite_done_event)), debug ? 1 : 0, (void*)stream);
+    // scale: the float16 symbol's scale after the map, () for the float32 one; tail: (dL_dcamera) or ()
+    auto run = [&](auto fn, auto gp, auto scale, auto tail) {
+        return std::apply(
+            fn, std::tuple_cat(
+                    std::make_tuple(P, degree, M, R, C, fptr(bg), W, H, fptr(m3), fptr(shc), fptr(col), fptr(sc),
+                                    scale_modifier, fptr(rot), fptr(cov), fptr(vm), fptr(pm), fptr(cp), tan_fovx,
+                                    tan_fovy, rad.data_ptr<int>(), reinterpret_cast<char*>(geomBuffer.data_ptr()),
+                                    reinterpret_cast<char*>(binningBuffer.data_ptr()),
+                                    reinterpret_cast<char*>(imageBuffer.data_ptr()), fptr(gc), gp),
+                    scale,
+                    std::make_tuple(fptr(gd), reinterpret_cast<char*>(scratch.data_ptr()),
+                                    in_place(g_opacities, dev, P, "g_opacities"),
+                                    in_place(g_colors, dev, (int64_t)P * 3, "g_colors_precomp"),
+                                    in_place(g_semantic_feature, dev, (int64_t)P * C, "g_semantic_feature"),
+                                    in_place(g_means3D, dev, (int64_t)P * 3, "g_means3D"),
+                                    in_place(g_cov3D, dev, (int64_t)P * 6, "g_cov3D_precomp"),
+                                    in_place(g_sh, dev, (int64_t)P * M * 3, "g_sh"),
+                                    in_place(g_scales, dev, (int64_t)P * 3, "g_scales"),
+                                    in_place(g_rotations, dev, (int64_t)P * 4, "g_rotations"),
+                                    in_place(g_means2D_out, dev, (int64_t)P * 3, "g_means2D_out"),
+                                    in_place(grad_accum, dev, P, "grad_accum"), in_place(denom, dev, P, "denom"),
+                                    reinterpret_cast<void*>(static_cast<intptr_t>(composite_done_event)),
+                                    debug ? 1 : 0, (void*)stream),
+                    tail));
     };
-    call_f32_or_f16(gf, f3dgs_backward_accum, "f3dgs_backward_accum", f3dgs_backward_accum_f16,
-                    "f3dgs_backward_accum_f16", [&](auto fn, auto gp) {
-                        if constexpr (std::is_same_v<decltype(gp), uint16_t*>)
-                            return run(fn, gp, (float)feature_grad_scale);
-                        else
-                            return run(fn, gp);
-                    });
+    auto dispatch = [&](auto tail) {
+        return [&, tail](auto fn, auto gp) {
+            if constexpr (std::is_same_v<decltype(gp), uint16_t*>)
+                return run(fn, gp, std::make_tuple((float)feature_grad_scale), tail);
+            else
+                return run(fn, gp, std::tuple<>(), tail);
+        };
+    };
+    if (cam)
+        call_f32_or_f16(gf, f3dgs_backward_accum_cam, "f3dgs_backward_accum_cam", f3dgs_backward_accum_cam_f16,
+                        "f3dgs_backward_accum_cam_f16", dispatch(std::make_tuple(cam)));
+    else
+        call_f32_or_f16(gf, f3dgs_backward_accum, "f3dgs_backward_accum", f3dgs_backward_accum_f16,
+                        "f3dgs_backward_accum_f16", dispatch(std::tuple<>()));
 }
 
 // Feature lifting (f3dgs_lift_features_accum / _f16): the buffers and R of a forward of this view; feature_map [C,H,W]
@@ -833,8 +904,9 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
               py::arg("g_sh"), py::arg("g_colors"), py::arg("g_semantic_feature"), py::arg("g_opacities"),
               py::arg("g_scales"), py::arg("g_rotations"), py::arg("g_cov3D"), py::arg("g_means2D_out"),
               py::arg("grad_accum"), py::arg("denom"), py::arg("composite_done_event"), py::arg("debug"),
-              py::arg("feature_grad_scale") = 1.0);
+              py::arg("feature_grad_scale") = 1.0, py::arg("camera_grad") = py::none());
     }
+    m.def("rasterize_gaussians_backward_camera", &RasterizeGaussiansBackwardCameraCUDA);
     m.def("lift_features_accum", &liftFeaturesAccum, pybind11::arg("geomBuffer"), pybind11::arg("R"),
           pybind11::arg("binningBuffer"), pybind11::arg("imageBuffer"), pybind11::arg("feature_map"),
           pybind11::arg("feature_sum"), pybind11::arg("weight_sum"));

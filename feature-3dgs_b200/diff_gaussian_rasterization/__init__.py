@@ -23,6 +23,10 @@ Behavioural notes
     and returned in `semantic_feature`'s dtype.  To train a float16 feature field use GaussianState(feature_dtype=
     torch.float16) with ViewBatch and feature_head's `*_and_grad(..., grad_dtype=torch.float16)`: their ScaledGrad
     carries the float32 scale that keeps the L1 gradient (~1e-8) from underflowing in float16, which autograd cannot.
+  * camera gradients (pose refinement, localisation, tracking): when grad mode is on and `raster_settings.viewmatrix`,
+    `.projmatrix` or `.campos` requires grad, `rasterize_gaussians` goes through `_RasterizeGaussiansCamera`, which
+    also returns dL/dviewmatrix, dL/dprojmatrix and dL/dcampos (f3dgs_backward_cam); otherwise the call and its graph
+    are `_RasterizeGaussians`'s.  `camera.settings_from_w2c` builds differentiable settings from a world-to-camera pose.
   * `debug=True` keeps the reference semantics: arguments are snapshotted to CPU first and dumped
     to snapshot_fw.dump / snapshot_bw.dump if the native call raises (reference :89-97,:147-155);
     natively it synchronises and checks after every stage.
@@ -105,34 +109,72 @@ class _RasterizeGaussians(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, grad_out_color, grad_out_feature, _grad_radii, grad_depth):
-        rs = ctx.raster_settings
-        (colors_precomp, semantic_feature, means3D, scales, rotations, cov3Ds_precomp, radii, sh, geomBuffer,
-         binningBuffer, imgBuffer) = ctx.saved_tensors
-        # autograd hands None/undefined for outputs that did not take part in the loss
-        if grad_out_color is None:
-            grad_out_color = torch.zeros(3, rs.image_height, rs.image_width, device=means3D.device)
-        if grad_depth is None:
-            grad_depth = torch.zeros(1, rs.image_height, rs.image_width, device=means3D.device)
-        if grad_out_feature is None:
-            C = semantic_feature.shape[-1] if semantic_feature.numel() else 0
-            grad_out_feature = torch.zeros(C, rs.image_height, rs.image_width, device=means3D.device)
-        args = (rs.bg, means3D, radii, colors_precomp, semantic_feature, scales, rotations, rs.scale_modifier,
-                cov3Ds_precomp, rs.viewmatrix, rs.projmatrix, rs.tanfovx, rs.tanfovy, grad_out_color,
-                grad_out_feature, grad_depth, sh, rs.sh_degree, rs.campos, geomBuffer, ctx.num_rendered,
-                binningBuffer, imgBuffer, rs.debug)
-        (grad_means2D, grad_colors_precomp, grad_semantic_feature, grad_opacities, grad_means3D,
-         grad_cov3Ds_precomp, grad_sh, grad_scales, grad_rotations) = _call_native(
-            _C.rasterize_gaussians_backward, args, rs.debug, "snapshot_bw.dump", "backward")
-        if not ctx.needs_input_grad[4]:
-            grad_semantic_feature = None
-        else:
-            grad_semantic_feature = grad_semantic_feature.to(semantic_feature.dtype)
-        return (grad_means3D, grad_means2D, grad_sh, grad_colors_precomp, grad_semantic_feature, grad_opacities,
-                grad_scales, grad_rotations, grad_cov3Ds_precomp, None)
+        grads = _native_backward(ctx, _C.rasterize_gaussians_backward, grad_out_color, grad_out_feature, grad_depth)
+        return grads[:9] + (None,)
+
+
+def _native_backward(ctx, fn, grad_out_color, grad_out_feature, grad_depth):
+    """The native backward `fn` of a forward saved by _RasterizeGaussians.forward -> the autograd gradients of
+    (means3D, means2D, sh, colors_precomp, semantic_feature, opacities, scales, rotations, cov3Ds_precomp), followed by
+    whatever else `fn` returns."""
+    rs = ctx.raster_settings
+    (colors_precomp, semantic_feature, means3D, scales, rotations, cov3Ds_precomp, radii, sh, geomBuffer,
+     binningBuffer, imgBuffer) = ctx.saved_tensors
+    # autograd hands None/undefined for outputs that did not take part in the loss
+    if grad_out_color is None:
+        grad_out_color = torch.zeros(3, rs.image_height, rs.image_width, device=means3D.device)
+    if grad_depth is None:
+        grad_depth = torch.zeros(1, rs.image_height, rs.image_width, device=means3D.device)
+    if grad_out_feature is None:
+        C = semantic_feature.shape[-1] if semantic_feature.numel() else 0
+        grad_out_feature = torch.zeros(C, rs.image_height, rs.image_width, device=means3D.device)
+    args = (rs.bg, means3D, radii, colors_precomp, semantic_feature, scales, rotations, rs.scale_modifier,
+            cov3Ds_precomp, rs.viewmatrix, rs.projmatrix, rs.tanfovx, rs.tanfovy, grad_out_color,
+            grad_out_feature, grad_depth, sh, rs.sh_degree, rs.campos, geomBuffer, ctx.num_rendered,
+            binningBuffer, imgBuffer, rs.debug)
+    (grad_means2D, grad_colors_precomp, grad_semantic_feature, grad_opacities, grad_means3D,
+     grad_cov3Ds_precomp, grad_sh, grad_scales, grad_rotations, *rest) = _call_native(
+        fn, args, rs.debug, "snapshot_bw.dump", "backward")
+    if not ctx.needs_input_grad[4]:
+        grad_semantic_feature = None
+    else:
+        grad_semantic_feature = grad_semantic_feature.to(semantic_feature.dtype)
+    return (grad_means3D, grad_means2D, grad_sh, grad_colors_precomp, grad_semantic_feature, grad_opacities,
+            grad_scales, grad_rotations, grad_cov3Ds_precomp, *rest)
+
+
+class _RasterizeGaussiansCamera(torch.autograd.Function):
+    """_RasterizeGaussians with the camera as autograd inputs: viewmatrix, projmatrix and campos (the tensors of
+    raster_settings, passed explicitly) also get gradients, from the native backward (f3dgs_backward_cam).  Intrinsics
+    (tanfovx/y) are floats and get none."""
+
+    @staticmethod
+    def forward(ctx, means3D, means2D, sh, colors_precomp, semantic_feature, opacities, scales, rotations,
+                cov3Ds_precomp, viewmatrix, projmatrix, campos, raster_settings):
+        rs = raster_settings._replace(viewmatrix=viewmatrix, projmatrix=projmatrix, campos=campos)
+        ctx.camera_shapes = (viewmatrix.shape, projmatrix.shape, campos.shape)
+        return _RasterizeGaussians.forward(ctx, means3D, means2D, sh, colors_precomp, semantic_feature, opacities,
+                                           scales, rotations, cov3Ds_precomp, rs)
+
+    @staticmethod
+    def backward(ctx, grad_out_color, grad_out_feature, _grad_radii, grad_depth):
+        grads = _native_backward(ctx, _C.rasterize_gaussians_backward_camera, grad_out_color, grad_out_feature,
+                                 grad_depth)
+        cam = tuple(g.reshape(shape) for g, shape in zip(grads[9:], ctx.camera_shapes))
+        return grads[:9] + cam + (None,)
+
+
+def _camera_requires_grad(rs):
+    return any(isinstance(t, torch.Tensor) and t.requires_grad for t in (rs.viewmatrix, rs.projmatrix, rs.campos))
 
 
 def rasterize_gaussians(means3D, means2D, sh, colors_precomp, semantic_feature, opacities, scales, rotations,
                         cov3Ds_precomp, raster_settings):
+    rs = raster_settings
+    if torch.is_grad_enabled() and _camera_requires_grad(rs):
+        return _RasterizeGaussiansCamera.apply(means3D, means2D, sh, colors_precomp, semantic_feature, opacities,
+                                               scales, rotations, cov3Ds_precomp, rs.viewmatrix, rs.projmatrix,
+                                               rs.campos, rs)
     return _RasterizeGaussians.apply(means3D, means2D, sh, colors_precomp, semantic_feature, opacities, scales,
                                      rotations, cov3Ds_precomp, raster_settings)
 

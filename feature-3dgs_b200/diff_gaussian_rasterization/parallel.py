@@ -19,7 +19,7 @@ additions, densification statistics folded in.  The step's collective is issued 
 opacity slice, final after the last view's composite kernel, is reduced on a side stream while the last view's backward
 preprocess still runs.
 """
-from typing import Iterable, List, Optional, Sequence
+from typing import Iterable, List, NamedTuple, Optional, Sequence
 
 import torch
 import torch.distributed as dist
@@ -76,6 +76,14 @@ class FlatGradBuffer:
         return self.flat
 
 
+
+
+class CameraGrad(NamedTuple):
+    """One view's camera gradient (ViewBatch.backward(..., camera=True)): views of one 35-float buffer, each in the
+    layout of the settings tensor it belongs to."""
+    viewmatrix: torch.Tensor  # [4, 4]
+    projmatrix: torch.Tensor  # [4, 4]
+    campos: torch.Tensor  # [3]
 
 
 class _ViewCtx:
@@ -151,15 +159,20 @@ class ViewBatch:
         ctx.num_rendered, color, feat, depth, ctx.radii, ctx.geom, ctx.binning, ctx.img = out
         return color, feat, ctx.radii, depth, ctx
 
-    def backward(self, ctx, g_color, g_feature, g_depth, means2D_out=None, last: bool = False):
+    def backward(self, ctx, g_color, g_feature, g_depth, means2D_out=None, last: bool = False, camera: bool = False):
         """Add this view's parameter gradients into the flat buffer.  `last=True` on the rank's last view of the step
         lets all_reduce() start the feature/opacity bucket early.  g_feature: dL/dfeature_map as a float32 or float16
-        [C,H,W] tensor, a feature_head.ScaledGrad (a float16 map and its float32 scale), or None."""
+        [C,H,W] tensor, a feature_head.ScaledGrad (a float16 map and its float32 scale), or None.
+
+        camera=True also returns this view's CameraGrad (dL/dviewmatrix, dL/dprojmatrix, dL/dcampos of its settings,
+        f3dgs_backward_accum_cam); the flat buffer and the densification statistics are bitwise those of camera=False.
+        A camera gradient belongs to its view and stays on the rank that rendered it: all_reduce() does not touch it."""
         rs, p, g, e = ctx.rs, self.params, self.grads, torch.Tensor([])
         none = self._empty
         scale = 1.0
         if isinstance(g_feature, tuple):  # ScaledGrad (not imported: this module loads without the package)
             g_feature, scale = g_feature
+        cam = torch.zeros(35, device=self.flat.device, dtype=torch.float32) if camera else None
         self._C.rasterize_gaussians_backward_accum(
             rs.bg, p["means3D"], ctx.radii, e, p["scales"], p["rotations"], rs.scale_modifier, e, rs.viewmatrix,
             rs.projmatrix, rs.tanfovx, rs.tanfovy, g_color, g_feature if g_feature is not None else none, g_depth,
@@ -167,8 +180,11 @@ class ViewBatch:
             g["means3D"], g["shs"], none, g.get("semantic_feature", none), g["opacities"], g["scales"], g["rotations"],
             none, means2D_out if means2D_out is not None else none,
             self.grad_accum if self.grad_accum is not None else none, self.denom if self.denom is not None else none,
-            int(self._ev.cuda_event) if (last and self._ev is not None) else 0, rs.debug, float(scale))
+            int(self._ev.cuda_event) if (last and self._ev is not None) else 0, rs.debug, float(scale), cam)
         self._early_pending = bool(last and self._ev is not None)
+        if cam is not None:
+            return CameraGrad(cam[:16].view(4, 4), cam[16:32].view(4, 4), cam[32:35])
+        return None
 
     def all_reduce(self, group: Optional[dist.ProcessGroup] = None):
         """The step's collective (sum over ranks).  After backward(..., last=True): two buckets, the feature/opacity one

@@ -38,6 +38,7 @@ extern "C" {
 #define F3DGS_ABI_VERSION 2
 #define F3DGS_MAX_FEATURE_DIM 4096
 #define F3DGS_TILE 16 /* BLOCK_X == BLOCK_Y == 16, reference config.h:18-19 */
+#define F3DGS_CAMERA_GRAD_FLOATS 35 /* dL_dcamera of the _cam backward entries */
 
 /* error codes (returned negated) */
 #define F3DGS_OK 0
@@ -189,6 +190,77 @@ int f3dgs_backward_accum_f16(int P, int D, int M, int R, int C,
                              float* dL_dmean3D, float* dL_dcov3D_precomp, float* dL_dsh, float* dL_dscale,
                              float* dL_drot, float* dL_dmean2D_out, float* grad_accum, float* denom,
                              void* composite_done_event, int debug, void* cuda_stream);
+
+/* ---- camera gradients (pose refinement, localisation, tracking): the _cam twins of the four backward entries ----
+ * Each takes its twin's arguments plus a final dL_dcamera of F3DGS_CAMERA_GRAD_FLOATS (35) floats of device memory and
+ * ADDS (+=) this view's camera gradient to it; every other output is bitwise its twin's.  Layout:
+ *   [0, 16)   dL/dviewmatrix, [16, 32) dL/dprojmatrix: in the 16-float layout of the input matrices;
+ *   [32, 35)  dL/dcampos.
+ * The entries the forward never reads (viewmatrix[3,7,11,15], projmatrix[2,6,10,14]) get 0, and dL/dcampos gets only
+ * the SH view-direction term (0 with colors_precomp).  A clamped view-space coordinate of the EWA Jacobian passes no
+ * gradient, as for dL_dmean3D.  The feature map does not feed the geometry (SURVEY D.1): a loss on features alone gives
+ * a zero camera gradient, as it gives a zero dL_dmean3D.
+ * The sum over Gaussians is free of floating-point atomics: float32 per-Gaussian terms, float64 block partials (taken
+ * from the device's default memory pool; F3DGS_ERR_ALLOC if that fails) reduced in a fixed order, then rounded once and
+ * added, so equal inputs give bitwise-equal results.  A NULL dL_dcamera, or one that overlaps another output (or the
+ * scratch of the accumulating entries), is F3DGS_ERR_INVALID_ARGUMENT; P == 0 leaves it untouched. */
+int f3dgs_backward_cam(int P, int D, int M, int R, int C,
+                       const float* background, int width, int height,
+                       const float* means3D, const float* shs, const float* colors_precomp,
+                       const float* semantic_feature,
+                       const float* scales, float scale_modifier, const float* rotations,
+                       const float* cov3D_precomp,
+                       const float* viewmatrix, const float* projmatrix, const float* cam_pos,
+                       float tan_fovx, float tan_fovy, const int* radii,
+                       char* geom_buffer, char* binning_buffer, char* image_buffer,
+                       const float* dL_dpix, const float* dL_dfeaturepix, const float* dL_depths,
+                       float* dL_dmean2D, float* dL_dconic, float* dL_dopacity, float* dL_dcolor,
+                       float* dL_dsemantic_feature, float* dL_dmean3D, float* dL_dcov3D,
+                       float* dL_dsh, float* dL_dscale, float* dL_drot, float* dL_dz,
+                       int debug, void* cuda_stream, float* dL_dcamera);
+int f3dgs_backward_cam_f16(int P, int D, int M, int R, int C,
+                           const float* background, int width, int height,
+                           const float* means3D, const float* shs, const float* colors_precomp,
+                           const float* semantic_feature,
+                           const float* scales, float scale_modifier, const float* rotations,
+                           const float* cov3D_precomp,
+                           const float* viewmatrix, const float* projmatrix, const float* cam_pos,
+                           float tan_fovx, float tan_fovy, const int* radii,
+                           char* geom_buffer, char* binning_buffer, char* image_buffer,
+                           const float* dL_dpix, const uint16_t* dL_dfeaturepix, float dL_dfeaturepix_scale,
+                           const float* dL_depths,
+                           float* dL_dmean2D, float* dL_dconic, float* dL_dopacity, float* dL_dcolor,
+                           float* dL_dsemantic_feature, float* dL_dmean3D, float* dL_dcov3D,
+                           float* dL_dsh, float* dL_dscale, float* dL_drot, float* dL_dz,
+                           int debug, void* cuda_stream, float* dL_dcamera);
+int f3dgs_backward_accum_cam(int P, int D, int M, int R, int C,
+                             const float* background, int width, int height,
+                             const float* means3D, const float* shs, const float* colors_precomp,
+                             const float* scales, float scale_modifier, const float* rotations,
+                             const float* cov3D_precomp,
+                             const float* viewmatrix, const float* projmatrix, const float* cam_pos,
+                             float tan_fovx, float tan_fovy, const int* radii,
+                             char* geom_buffer, char* binning_buffer, char* image_buffer,
+                             const float* dL_dpix, const float* dL_dfeaturepix, const float* dL_depths,
+                             char* scratch,
+                             float* dL_dopacity, float* dL_dcolors_precomp, float* dL_dsemantic_feature,
+                             float* dL_dmean3D, float* dL_dcov3D_precomp, float* dL_dsh, float* dL_dscale,
+                             float* dL_drot, float* dL_dmean2D_out, float* grad_accum, float* denom,
+                             void* composite_done_event, int debug, void* cuda_stream, float* dL_dcamera);
+int f3dgs_backward_accum_cam_f16(int P, int D, int M, int R, int C,
+                                 const float* background, int width, int height,
+                                 const float* means3D, const float* shs, const float* colors_precomp,
+                                 const float* scales, float scale_modifier, const float* rotations,
+                                 const float* cov3D_precomp,
+                                 const float* viewmatrix, const float* projmatrix, const float* cam_pos,
+                                 float tan_fovx, float tan_fovy, const int* radii,
+                                 char* geom_buffer, char* binning_buffer, char* image_buffer,
+                                 const float* dL_dpix, const uint16_t* dL_dfeaturepix, float dL_dfeaturepix_scale,
+                                 const float* dL_depths, char* scratch,
+                                 float* dL_dopacity, float* dL_dcolors_precomp, float* dL_dsemantic_feature,
+                                 float* dL_dmean3D, float* dL_dcov3D_precomp, float* dL_dsh, float* dL_dscale,
+                                 float* dL_drot, float* dL_dmean2D_out, float* grad_accum, float* denom,
+                                 void* composite_done_event, int debug, void* cuda_stream, float* dL_dcamera);
 
 /* ---- feature lifting (no reference counterpart): training-free back-projection of 2-D feature maps onto Gaussians ----
  * The buffers and R are those of an f3dgs_forward / f3dgs_forward_f16 of this view at width x height (any C of that
