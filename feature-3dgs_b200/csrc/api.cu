@@ -429,7 +429,8 @@ struct ScratchLayout {  // per-view intermediates of the accumulating backward (
 // Shared body of f3dgs_backward (accumulate = false: the reference's assign-into-zeroed-buffers contract),
 // f3dgs_backward_accum (accumulate = true: += into the caller's per-parameter gradient buffers) and their _f16 twins.
 // TG (float or __half) is the element type of dL_dfeaturepix; a __half map stands for dL/dO = scale * float(h).
-// `zero` (accumulate only): the caller's scratch, zeroed once the arguments are validated.
+// `zero` (accumulate only): the caller's scratch, zeroed once the arguments are validated.  feat.rows (the _feature_geometry
+// entries only; NULL on every other path): the Gaussians' features, for the feature term of dL/dalpha.
 template <typename TG>
 int backward_impl(const Api& api, bool accumulate, int P, int D, int M, int R, int C, const float* background, int width,
                   int height, const float* means3D, const float* shs, const float* scales, float scale_modifier,
@@ -440,7 +441,7 @@ int backward_impl(const Api& api, bool accumulate, int P, int D, int M, int R, i
                   float* dL_dopacity, float* dL_dcolor, float* dL_dsemantic_feature, float* dL_dmean3D, float* dL_dcov3D,
                   float* dL_dsh, float* dL_dscale, float* dL_drot, float* dL_dz, float* grad_accum, float* denom,
                   float* dL_dcamera, cudaEvent_t composite_done, int debug, cudaStream_t stream,
-                  const Range& zero = {nullptr, 0}) {
+                  const Range& zero = {nullptr, 0}, const FeatureRows& feat = {}) {
     if (P < 0 || width <= 0 || height <= 0 || C < 0 || C > F3DGS_MAX_FEATURE_DIM || R < 0)
         return api.invalid("bad sizes");
     if (P == 0) return 0;
@@ -468,6 +469,16 @@ int backward_impl(const Api& api, bool accumulate, int P, int D, int M, int R, i
         if (overlaps({dL_dcamera, F3DGS_CAMERA_GRAD_FLOATS * sizeof(float)}, outs))
             return api.invalid("dL_dcamera overlaps another output");
     }
+    if (feat.rows) {
+        const size_t p4 = (size_t)P * 4;
+        const Range outs[] = {{dL_dmean2D, 3 * p4}, {dL_dconic, 4 * p4}, {dL_dopacity, p4}, {dL_dcolor, 3 * p4},
+                              {dL_dsemantic_feature, (size_t)C * p4}, {dL_dmean3D, 3 * p4}, {dL_dcov3D, 6 * p4},
+                              {dL_dsh, (size_t)M * 3 * p4}, {dL_dscale, 3 * p4}, {dL_drot, 4 * p4}, {dL_dz, p4},
+                              {grad_accum, p4}, {denom, p4}, {dL_dcamera, F3DGS_CAMERA_GRAD_FLOATS * sizeof(float)},
+                              zero};
+        if (overlaps({feat.rows, (size_t)P * C * (feat.f16 ? 2 : 4)}, outs))
+            return api.invalid("semantic_feature overlaps an output");
+    }
     if (zero.p) CUDA_TRY(cudaMemsetAsync(const_cast<void*>(zero.p), 0, zero.bytes, stream));
 
     const ViewParams vp = make_view(P, D, M, C, width, height, tan_fovx, tan_fovy, scale_modifier, viewmatrix,
@@ -482,7 +493,7 @@ int backward_impl(const Api& api, bool accumulate, int P, int D, int M, int R, i
         StageTimer t(F3DGS_STAGE_COMPOSITE_BWD, stream);
         e = launch_composite_bwd(vp, forward_buffers(vp, R, geom_buffer, binning_buffer, image_buffer), background,
                                  dL_dpix, dL_depths, dL_dfeaturepix, dL_dfeaturepix_scale, dL_dmean2D, dL_dconic,
-                                 dL_dopacity, dL_dcolor, dL_dz, dL_dsemantic_feature, stream);
+                                 dL_dopacity, dL_dcolor, dL_dz, dL_dsemantic_feature, stream, feat);
     }
     if (const int rc = composite_bwd_result(api, e, "composite_bwd launch")) return rc;
     STAGE_CHECK("composite_bwd");
@@ -607,7 +618,7 @@ int backward_accum_impl(const char* entry, int P, int D, int M, int R, int C, co
                         float* dL_dsemantic_feature, float* dL_dmean3D, float* dL_dcov3D_precomp, float* dL_dsh,
                         float* dL_dscale, float* dL_drot, float* dL_dmean2D_out, float* grad_accum, float* denom,
                         void* composite_done_event, int debug, void* cuda_stream, bool camera = false,
-                        float* dL_dcamera = nullptr) {
+                        float* dL_dcamera = nullptr, const FeatureRows& feat = {}) {
     const Api api(entry);
     cudaStream_t stream = (cudaStream_t)cuda_stream;
     if (camera && !dL_dcamera) return api.invalid("NULL dL_dcamera");
@@ -615,6 +626,8 @@ int backward_accum_impl(const char* entry, int P, int D, int M, int R, int C, co
     if (!scratch) return api.invalid("NULL scratch");
     if (overlaps({dL_dcamera, F3DGS_CAMERA_GRAD_FLOATS * sizeof(float)}, {{dL_dmean2D_out, (size_t)P * 3 * 4}}))
         return api.invalid("dL_dcamera overlaps another output");
+    if (overlaps({feat.rows, (size_t)P * C * (feat.f16 ? 2 : 4)}, {{dL_dmean2D_out, (size_t)P * 3 * 4}}))
+        return api.invalid("semantic_feature overlaps an output");
     if ((colors_precomp != nullptr) != (dL_dcolors_precomp != nullptr) ||
         (cov3D_precomp != nullptr) != (dL_dcov3D_precomp != nullptr))
         return api.invalid("dL_dcolors_precomp / dL_dcov3D_precomp go with colors_precomp / cov3D_precomp");
@@ -629,7 +642,7 @@ int backward_accum_impl(const char* entry, int P, int D, int M, int R, int C, co
         binning_buffer, image_buffer, dL_dpix, dL_dfeaturepix, dL_dfeaturepix_scale, dL_depths, m2d,
         reinterpret_cast<float*>(scratch + sl.conic), dL_dopacity, dcol, dL_dsemantic_feature, dL_dmean3D, dcov, dL_dsh,
         dL_dscale, dL_drot, reinterpret_cast<float*>(scratch + sl.dz), grad_accum, denom, dL_dcamera,
-        (cudaEvent_t)composite_done_event, debug, stream, {scratch, sl.bytes});
+        (cudaEvent_t)composite_done_event, debug, stream, {scratch, sl.bytes}, feat);
     if (rc < 0) return rc;
     if (dL_dmean2D_out)
         CUDA_TRY(cudaMemcpyAsync(dL_dmean2D_out, m2d, (size_t)P * 3 * sizeof(float), cudaMemcpyDeviceToDevice, stream));
@@ -714,6 +727,81 @@ int f3dgs_backward_accum_cam_f16(int P, int D, int M, int R, int C, const float*
                                dL_dopacity, dL_dcolors_precomp, dL_dsemantic_feature, dL_dmean3D, dL_dcov3D_precomp,
                                dL_dsh, dL_dscale, dL_drot, dL_dmean2D_out, grad_accum, denom, composite_done_event, debug,
                                cuda_stream, true, dL_dcamera);
+}
+
+}  // extern "C"
+
+namespace {
+// The Gaussians' features of a _feature_geometry entry, after the checks every such entry makes before any launch
+int feature_rows(const Api& api, int C, const void* semantic_feature, int semantic_feature_dtype,
+                 int dL_dfeaturepix_dtype, FeatureRows& feat) {
+    const auto known = [](int t) { return t == F3DGS_F32 || t == F3DGS_F16; };
+    if (!known(semantic_feature_dtype) || !known(dL_dfeaturepix_dtype)) return api.invalid("unknown dtype code");
+    if (C > 0 && !semantic_feature) return api.invalid("NULL semantic_feature");
+    feat = {C > 0 ? semantic_feature : nullptr, semantic_feature_dtype == F3DGS_F16};
+    return 0;
+}
+}  // namespace
+
+extern "C" {
+
+int f3dgs_backward_feature_geometry(int P, int D, int M, int R, int C, const float* background, int width, int height,
+                                    const float* means3D, const float* shs, const float* colors_precomp,
+                                    const void* semantic_feature, int semantic_feature_dtype, const float* scales,
+                                    float scale_modifier, const float* rotations, const float* cov3D_precomp,
+                                    const float* viewmatrix, const float* projmatrix, const float* cam_pos,
+                                    float tan_fovx, float tan_fovy, const int* radii, char* geom_buffer,
+                                    char* binning_buffer, char* image_buffer, const float* dL_dpix,
+                                    const void* dL_dfeaturepix, int dL_dfeaturepix_dtype, float dL_dfeaturepix_scale,
+                                    const float* dL_depths, float* dL_dmean2D, float* dL_dconic, float* dL_dopacity,
+                                    float* dL_dcolor, float* dL_dsemantic_feature, float* dL_dmean3D,
+                                    float* dL_dcov3D, float* dL_dsh, float* dL_dscale, float* dL_drot, float* dL_dz,
+                                    int debug, void* cuda_stream, float* dL_dcamera) {
+    (void)colors_precomp;
+    const Api api(__func__);
+    FeatureRows feat;
+    if (const int rc = feature_rows(api, C, semantic_feature, semantic_feature_dtype, dL_dfeaturepix_dtype, feat))
+        return rc;
+    const auto run = [&](auto map, float scale) {
+        return backward_impl(api, false, P, D, M, R, C, background, width, height, means3D, shs, scales,
+                             scale_modifier, rotations, cov3D_precomp, viewmatrix, projmatrix, cam_pos, tan_fovx,
+                             tan_fovy, radii, geom_buffer, binning_buffer, image_buffer, dL_dpix, map, scale, dL_depths,
+                             dL_dmean2D, dL_dconic, dL_dopacity, dL_dcolor, dL_dsemantic_feature, dL_dmean3D, dL_dcov3D,
+                             dL_dsh, dL_dscale, dL_drot, dL_dz, nullptr, nullptr, dL_dcamera, nullptr, debug,
+                             (cudaStream_t)cuda_stream, {nullptr, 0}, feat);
+    };
+    if (dL_dfeaturepix_dtype == F3DGS_F16)
+        return run(static_cast<const __half*>(dL_dfeaturepix), dL_dfeaturepix_scale);
+    return run(static_cast<const float*>(dL_dfeaturepix), 1.f);
+}
+
+int f3dgs_backward_accum_feature_geometry(
+    int P, int D, int M, int R, int C, const float* background, int width, int height, const float* means3D,
+    const float* shs, const float* colors_precomp, const void* semantic_feature, int semantic_feature_dtype,
+    const float* scales, float scale_modifier, const float* rotations, const float* cov3D_precomp,
+    const float* viewmatrix, const float* projmatrix, const float* cam_pos, float tan_fovx, float tan_fovy,
+    const int* radii, char* geom_buffer, char* binning_buffer, char* image_buffer, const float* dL_dpix,
+    const void* dL_dfeaturepix, int dL_dfeaturepix_dtype, float dL_dfeaturepix_scale, const float* dL_depths,
+    char* scratch, float* dL_dopacity, float* dL_dcolors_precomp, float* dL_dsemantic_feature, float* dL_dmean3D,
+    float* dL_dcov3D_precomp, float* dL_dsh, float* dL_dscale, float* dL_drot, float* dL_dmean2D_out,
+    float* grad_accum, float* denom, void* composite_done_event, int debug, void* cuda_stream, float* dL_dcamera) {
+    const char* entry = __func__;
+    FeatureRows feat;
+    if (const int rc = feature_rows(Api(entry), C, semantic_feature, semantic_feature_dtype, dL_dfeaturepix_dtype,
+                                    feat))
+        return rc;
+    const auto run = [&](auto map, float scale) {
+        return backward_accum_impl(entry, P, D, M, R, C, background, width, height, means3D, shs, colors_precomp,
+                                   scales, scale_modifier, rotations, cov3D_precomp, viewmatrix, projmatrix, cam_pos,
+                                   tan_fovx, tan_fovy, radii, geom_buffer, binning_buffer, image_buffer, dL_dpix, map,
+                                   scale, dL_depths, scratch, dL_dopacity, dL_dcolors_precomp, dL_dsemantic_feature,
+                                   dL_dmean3D, dL_dcov3D_precomp, dL_dsh, dL_dscale, dL_drot, dL_dmean2D_out,
+                                   grad_accum, denom, composite_done_event, debug, cuda_stream, false, dL_dcamera,
+                                   feat);
+    };
+    if (dL_dfeaturepix_dtype == F3DGS_F16)
+        return run(static_cast<const __half*>(dL_dfeaturepix), dL_dfeaturepix_scale);
+    return run(static_cast<const float*>(dL_dfeaturepix), 1.f);
 }
 
 }  // extern "C"

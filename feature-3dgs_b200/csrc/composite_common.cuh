@@ -243,6 +243,12 @@ template <typename TG>
 cudaError_t launch_feature_bwd(const ViewParams& vp, const uint2* ranges, const InstanceLists& lists,
                                const TG* dL_dfeat_pix, float dL_dfeat_pix_scale, float* dL_dfeature, int* counters,
                                cudaStream_t s);
+// ---- feature_bwd.cu: overwrites each list entry's weight row with the pair dot products d_ip = f_i . dL/dfeature_map[:, p]
+// over the C channels (TG and scale as above), for the FEAT walk of composite_bwd.cu
+template <typename TG>
+cudaError_t launch_feature_dot(const ViewParams& vp, const uint2* ranges, const InstanceLists& lists,
+                               const FeatureRows& feat, const TG* dL_dfeat_pix, float dL_dfeat_pix_scale, int* counters,
+                               cudaStream_t s);
 
 // Splat alpha at pixel (pxf, pyf), with the reference's expression trees (forward.cu:340-351, backward.cu:525-535): plain
 // fp32, no _rn intrinsics (see common.cuh).  alpha is 0 where the reference skips the pair (power > 0 or alpha < 1/255)

@@ -13,6 +13,14 @@
 // The upstream gradient may be a float16 map h with a float32 scale s (training float16 feature fields): it is upcast and
 // multiplied by s once, where the block's gradient is loaded, and everything after that is the float32 kernel.
 // Reference semantics: backward.cu:565-575 (feature gradient; the feature loss does not feed dL/dalpha, :575 disabled).
+//
+// feature_dot_kernel<CH> (here, opt-in): the pair dot products d_ip = f_i . dL/dfeature_map[:, p] for the feature term
+// of dL/dalpha (composite_bwd.cu, FEAT).  One warp per (tile, block) item walks the block's list once per CH-channel
+// chunk, with the block's gradient chunk in registers exactly as above, gathers each entry's feature-row chunk (4
+// channels per lane) and forms its partial dot product at each of the lane's pixels; a reduce-scatter over the CH / 4
+// lanes that share those pixels leaves each lane with the chunk's whole dot product at one pixel.  The first chunk
+// stores it into the entry's weight row, which feature_bwd is done with, and later chunks add to it: the warp owns the
+// rows of its item, so there are no atomics and the result is deterministic.
 #include <cstdio>
 #include <cstdlib>
 
@@ -187,6 +195,150 @@ __global__ void __launch_bounds__(kFeatWarps * 32, 3) feature_bwd_kernel(const F
     }
 }
 
+// ------------------------------------------------------------------------------------------------ pair dot products
+template <typename TF, typename TG>
+struct DotArgs {
+    FeatArgs<TG> f;      // bit0 of f.vec: feature rows are 4-channel aligned (C % 4 == 0 and an aligned base)
+    const TF* features;  // [P, C]
+};
+
+// Four channels of a feature row, a float16 row upcast exactly as the forward reads it
+__device__ __forceinline__ float4 ld_feat4(const float* p) { return ld_nc_f4(p); }
+__device__ __forceinline__ float4 ld_feat4(const __half* p) {
+    uint32_t u0, u1;
+    asm volatile("ld.global.nc.v2.u32 {%0,%1}, [%2];" : "=r"(u0), "=r"(u1) : "l"(p));
+    return to_float4(make_uint2(u0, u1));
+}
+__device__ __forceinline__ float ld_feat1(const float* p) { return __ldg(p); }
+__device__ __forceinline__ float ld_feat1(const __half* p) { return __half2float(__ldg(p)); }
+
+// c ? x : y as one SELP: spelled as a select, the compiler turns the reduce-scatter's selects into a dynamically indexed
+// array in local memory
+__device__ __forceinline__ float sel(uint32_t c, float x, float y) {
+    float r;
+    asm("{.reg .pred p; setp.ne.u32 p, %3, 0; selp.f32 %0, %1, %2, p;}" : "=f"(r) : "f"(x), "f"(y), "r"(c));
+    return r;
+}
+
+template <int CH, typename TF, typename TG>
+__global__ void __launch_bounds__(kFeatWarps * 32, 3) feature_dot_kernel(const DotArgs<TF, TG> d) {
+    const FeatArgs<TG>& a = d.f;
+    const int lane = threadIdx.x & 31;
+    constexpr int LPR = CH / 4;  // lanes per feature row = pixels per lane
+    constexpr int G = 32 / LPR;
+    constexpr int NQ = 8 / G;
+    const int grp = lane / LPR, cl = lane % LPR;
+    // after the reduce-scatter lane (grp, cl) holds the lane group's pixel cl: pixel cl & 3 of its quad cl >> 2
+    const int slot = 4 * ((cl >> 2) * G + grp) + (cl & 3);
+    const int W = a.W, H = a.H, C = a.C;
+    const size_t HW = (size_t)H * W;
+
+    const int items = a.num_tiles * kBlocksPerTile;
+    for (;;) {
+        int item = 0;
+        if (lane == 0) item = atomicAdd(a.work_counter, 1);
+        item = __shfl_sync(0xffffffffu, item, 0);
+        if (item >= items) break;
+        const int tile = item / kBlocksPerTile, b = item % kBlocksPerTile;
+        const int bx0 = block_x0(tile % a.tiles_x, b), by0 = block_y0(tile / a.tiles_x, b);
+        const uint32_t rx = __shfl_sync(0xffffffffu, a.ranges[tile].x, 0);
+        const uint32_t ry = __shfl_sync(0xffffffffu, a.ranges[tile].y, 0);
+        const size_t base = list_begin(rx, ry, b);
+        const uint32_t n = __shfl_sync(0xffffffffu, a.lists.cnt[(size_t)tile * kBlocksPerTile + b], 0);
+        if (n == 0) continue;
+
+        for (int chunk = 0; chunk < a.chunks; chunk++) {
+            const int ch0 = chunk * CH + cl * 4;
+            float2 dO2[NQ][2][4];  // as in feature_bwd_kernel
+#pragma unroll
+            for (int q = 0; q < NQ; q++)
+#pragma unroll
+                for (int r = 0; r < 2; r++)
+#pragma unroll
+                    for (int c = 0; c < 4; c++) dO2[q][r][c] = make_float2(0.f, 0.f);
+#pragma unroll
+            for (int c = 0; c < 4; c++) {
+                const int ch = ch0 + c;
+                if (ch >= C) continue;
+                for_tile_pixels<G, NQ>(
+                    a.dL_dfeat_pix + (size_t)ch * HW, bx0, by0, W, H, grp, false, a.vec & 2, [](const TG*, int) {},
+                    [&](const TG* p, int y, int half) { set_tile_run(dO2, y, half, c, ld_dO4(p, a.scale)); },
+                    [&](const TG* p, int qi, int i) { tile_px(dO2, qi, i, c) = ld_dO1(p, a.scale); });
+            }
+
+            for (uint32_t c0 = 0; c0 < n; c0 += 32) {
+                const uint2 m = c0 + lane < n ? __ldg(&a.lists.meta[base + c0 + lane]) : make_uint2(0u, 0u);
+                const uint32_t cnt = min(32u, n - c0);
+                // the entry's feature-row chunk, loaded one entry ahead of its use
+                auto load_row = [&](uint32_t gid) {
+                    float4 f = make_float4(0.f, 0.f, 0.f, 0.f);
+                    const TF* src = d.features + (size_t)gid * C + ch0;
+                    if (ch0 < C) {
+                        if (a.vec & 1) {
+                            f = ld_feat4(src);
+                        } else {
+                            f.x = ld_feat1(src);
+                            if (ch0 + 1 < C) f.y = ld_feat1(src + 1);
+                            if (ch0 + 2 < C) f.z = ld_feat1(src + 2);
+                            if (ch0 + 3 < C) f.w = ld_feat1(src + 3);
+                        }
+                    }
+                    return f;
+                };
+                float4 f_nxt = load_row(__shfl_sync(0xffffffffu, m.x, 0));
+#pragma unroll 1
+                for (uint32_t i = 0; i < cnt; i++) {
+                    const uint32_t pm = __shfl_sync(0xffffffffu, m.y, i);
+                    const float4 f = f_nxt;
+                    const uint32_t gid_nxt = __shfl_sync(0xffffffffu, m.x, (i + 1) & 31);
+                    if (i + 1 < cnt) f_nxt = load_row(gid_nxt);
+                    // partial dot product at each of the lane's pixels, pixel i of its quad qi at index 4 qi + i (0 where
+                    // the quad did not blend: the FEAT walk reads only the blended pixels), then a reduce-scatter over the
+                    // LPR lanes of the group: at offset o the lane keeps the half of its values selected by bit o of cl and
+                    // adds its partner's copy of that half.  The first step (o = LPR / 2: quads qi and qi + NQ / 2) is
+                    // taken as the values are formed, so that only half of them are ever live.
+                    auto dot = [&](int qi, int r) {
+                        float2 acc = make_float2(0.f, 0.f);
+                        if ((pm >> (4 * (qi * G + grp))) & 0xFu) {
+                            acc = fma2_rn(make_float2(f.x, f.x), dO2[qi][r][0], acc);
+                            acc = fma2_rn(make_float2(f.y, f.y), dO2[qi][r][1], acc);
+                            acc = fma2_rn(make_float2(f.z, f.z), dO2[qi][r][2], acc);
+                            acc = fma2_rn(make_float2(f.w, f.w), dO2[qi][r][3], acc);
+                        }
+                        return acc;
+                    };
+                    constexpr int H2 = LPR / 2;
+                    float v[H2];
+                    {
+                        const uint32_t up = cl & H2;
+#pragma unroll
+                        for (int qi = 0; qi < NQ / 2; qi++)
+#pragma unroll
+                            for (int r = 0; r < 2; r++) {
+                                const float2 lo = dot(qi, r), hi = dot(qi + NQ / 2, r);
+                                v[4 * qi + 2 * r] = sel(up, hi.x, lo.x) + __shfl_xor_sync(0xffffffffu, sel(up, lo.x, hi.x), H2);
+                                v[4 * qi + 2 * r + 1] =
+                                    sel(up, hi.y, lo.y) + __shfl_xor_sync(0xffffffffu, sel(up, lo.y, hi.y), H2);
+                            }
+                    }
+#pragma unroll
+                    for (int o = H2 / 2; o > 0; o >>= 1) {
+                        const uint32_t up = cl & o;
+#pragma unroll
+                        for (int j = 0; j < o; j++) {
+                            const float send = sel(up, v[j], v[j + o]);
+                            const float keep = sel(up, v[j + o], v[j]);
+                            v[j] = keep + __shfl_xor_sync(0xffffffffu, send, o);
+                        }
+                    }
+                    float* dst = a.lists.w + (base + c0 + i) * 32 + slot;
+                    *dst = chunk == 0 ? v[0] : *dst + v[0];
+                }
+            }
+        }
+    }
+}
+
 // ------------------------------------------------------------------------------------------------ launchers
 template <int CH, typename TG>
 static cudaError_t launch_feat_bwd_t(const FeatArgs<TG>& a, cudaStream_t s) {
@@ -226,5 +378,49 @@ template cudaError_t launch_feature_bwd(const ViewParams&, const uint2*, const I
                                        float*, int*, cudaStream_t);
 template cudaError_t launch_feature_bwd(const ViewParams&, const uint2*, const InstanceLists&, const __half*, float,
                                        float*, int*, cudaStream_t);
+
+template <int CH, typename TF, typename TG>
+static cudaError_t launch_feat_dot_t(const DotArgs<TF, TG>& d, cudaStream_t s) {
+    int sms = 132;  // kept for a device ordinal device_sms does not cover
+    device_sms<>(sms, 0);
+    const int items = d.f.num_tiles * kBlocksPerTile;
+    const int grid = min((items + kFeatWarps - 1) / kFeatWarps, sms * 3);
+    feature_dot_kernel<CH, TF, TG><<<grid, kFeatWarps * 32, 0, s>>>(d);
+    g_launches++;
+    return cudaGetLastError();
+}
+
+template <typename TF, typename TG>
+static cudaError_t launch_feat_dot_tf(const DotArgs<TF, TG>& d, cudaStream_t s) {
+    const int CH = channel_chunk(d.f.C);
+    if (CH == 32) return launch_feat_dot_t<32>(d, s);
+    if (CH == 64) return launch_feat_dot_t<64>(d, s);
+    return launch_feat_dot_t<128>(d, s);
+}
+
+template <typename TG>
+cudaError_t launch_feature_dot(const ViewParams& vp, const uint2* ranges, const InstanceLists& lists,
+                               const FeatureRows& feat, const TG* dL_dfeat_pix, float dL_dfeat_pix_scale, int* counters,
+                               cudaStream_t s) {
+    FeatArgs<TG> a;
+    a.ranges = ranges; a.lists = lists;
+    a.dL_dfeat_pix = dL_dfeat_pix; a.scale = dL_dfeat_pix_scale;
+    a.dL_dfeature = nullptr;
+    a.work_counter = counters + kCounterFeatureBwd;
+    a.W = vp.W; a.H = vp.H; a.C = vp.C; a.tiles_x = (int)vp.grid_x; a.num_tiles = (int)(vp.grid_x * vp.grid_y);
+    a.chunks = (vp.C + channel_chunk(vp.C) - 1) / channel_chunk(vp.C);
+    a.vec = 0;
+    const size_t fsz = feat.f16 ? sizeof(__half) : sizeof(float);
+    if (vp.C % 4 == 0 && (reinterpret_cast<uintptr_t>(feat.rows) & (4 * fsz - 1)) == 0) a.vec |= 1;
+    if (vp.W % 4 == 0 && (reinterpret_cast<uintptr_t>(dL_dfeat_pix) & (4 * sizeof(TG) - 1)) == 0) a.vec |= 2;
+    const cudaError_t e = cudaMemsetAsync(a.work_counter, 0, sizeof(int), s);
+    if (e != cudaSuccess) return e;
+    if (feat.f16) return launch_feat_dot_tf(DotArgs<__half, TG>{a, static_cast<const __half*>(feat.rows)}, s);
+    return launch_feat_dot_tf(DotArgs<float, TG>{a, static_cast<const float*>(feat.rows)}, s);
+}
+template cudaError_t launch_feature_dot(const ViewParams&, const uint2*, const InstanceLists&, const FeatureRows&,
+                                       const float*, float, int*, cudaStream_t);
+template cudaError_t launch_feature_dot(const ViewParams&, const uint2*, const InstanceLists&, const FeatureRows&,
+                                       const __half*, float, int*, cudaStream_t);
 
 }  // namespace f3dgs

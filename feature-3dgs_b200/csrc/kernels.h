@@ -69,15 +69,22 @@ struct ForwardBuffers {
     int* counters;  // the image buffer's work-counter region
     int R;
 };
+// The Gaussians' feature rows [P, C], float32 or float16 (upcast exactly, as the forward reads them); rows == nullptr:
+// none given
+struct FeatureRows {
+    const void* rows = nullptr;
+    bool f16 = false;
+};
 // Geometric gradients from a kernel at two CTAs per SM.  With C > 0 and R > 0 that kernel also emits per-(tile, block)
 // instance lists (scratch of the device's default pool, freed on the stream before return), and a second kernel forms
 // dL_dfeature from them.  TG (float or __half) is the element type of dL_dfeat_pix; a __half map stands for
-// dL/dO = scale * float(h) (the scale is not read for a float map)
+// dL/dO = scale * float(h) (the scale is not read for a float map).  With feat.rows (and C > 0, R > 0) the feature term
+// of dL/dalpha is added to dL_dmean2D, dL_dconic and dL_dopacity by two more kernels over the same lists.
 template <typename TG>
 cudaError_t launch_composite_bwd(const ViewParams& vp, const ForwardBuffers& fb, const float* bg, const float* dL_dpix,
                                  const float* dL_ddepth, const TG* dL_dfeat_pix, float dL_dfeat_pix_scale,
                                  float* dL_dmean2D, float* dL_dconic, float* dL_dopacity, float* dL_dcolor, float* dL_dz,
-                                 float* dL_dfeature, cudaStream_t s);
+                                 float* dL_dfeature, cudaStream_t s, const FeatureRows& feat = {});
 // Feature lifting, R > 0: weight_sum[P] += the blend weights w = alpha*T of each Gaussian over the view and
 // feature_sum[P, C] += sum_p w * map[:, p], through the same lists.  TF (float or __half) is the element type of map
 template <typename TF>

@@ -8,7 +8,9 @@
 //                                         dL_dmeans3D, dL_dcov3D, dL_dsh, dL_dscales, dL_drotations)
 //   mark_visible(means3D, viewmatrix, projmatrix) -> bool[P]
 // plus rasterize_gaussians_backward_camera(same arguments as rasterize_gaussians_backward) -> its 9 gradients +
-// (dL_dviewmatrix [4,4], dL_dprojmatrix [4,4], dL_dcampos [3]) for pose refinement (f3dgs_backward_cam).
+// (dL_dviewmatrix [4,4], dL_dprojmatrix [4,4], dL_dcampos [3]) for pose refinement (f3dgs_backward_cam), and
+// rasterize_gaussians_backward_feature_geometry(same arguments, camera) -> the same 12 (the camera three None unless
+// `camera`) with the feature term of dL/dalpha (f3dgs_backward_feature_geometry).
 // Differences (all permissive): the feature width is read from semantic_feature.size(-1) at run
 // time (reference: compile-time NUM_SEMANTIC_CHANNELS, config.h:16); an empty / undefined
 // semantic_feature means C = 0; semantic_feature may be float32 or float16, and the feature map
@@ -75,6 +77,11 @@ torch::Tensor feature_grad(const torch::Tensor& t, const torch::Device& dev) {
                 "grad_out_feature must be float32 or float16 (got ", t.scalar_type(), ")");
     TORCH_CHECK(t.device() == dev, "grad_out_feature must be on ", dev, " (got ", t.device(), ")");
     return t.contiguous();
+}
+
+// C-ABI element-type code of a float32 or float16 tensor (absent: float32)
+int dtype_code(const torch::Tensor& t) {
+    return t.defined() && t.scalar_type() == torch::kFloat16 ? F3DGS_F16 : F3DGS_F32;
 }
 
 void check_rc(int rc, const char* what) {
@@ -168,8 +175,9 @@ RasterizeGaussiansCUDA(const torch::Tensor& background, const torch::Tensor& mea
 using BackwardGrads = std::tuple<torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor,
                                  torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor>;
 
-// Body of rasterize_gaussians_backward and rasterize_gaussians_backward_camera: with a non-NULL camera (35 floats on the
-// device), the _cam entries, which add the camera gradient to it
+// Body of rasterize_gaussians_backward, _camera and _feature_geometry: with a non-NULL camera (35 floats on the device),
+// the _cam entries, which add the camera gradient to it; with feature_geometry, f3dgs_backward_feature_geometry, which
+// reads semantic_feature and takes the camera gradient as an optional argument
 static BackwardGrads backward_grads(const torch::Tensor& background, const torch::Tensor& means3D,
                                const torch::Tensor& radii, const torch::Tensor& colors,
                                const torch::Tensor& semantic_feature, const torch::Tensor& scales,
@@ -180,7 +188,7 @@ static BackwardGrads backward_grads(const torch::Tensor& background, const torch
                                const torch::Tensor& dL_dout_depth, const torch::Tensor& sh, const int degree,
                                const torch::Tensor& campos, const torch::Tensor& geomBuffer, const int R,
                                const torch::Tensor& binningBuffer, const torch::Tensor& imageBuffer,
-                               const bool debug, float* camera) {
+                               const bool debug, float* camera, bool feature_geometry = false) {
     TORCH_CHECK(means3D.is_cuda(), "means3D must be a CUDA tensor (this build has no CPU path)");
     const c10::cuda::CUDAGuard guard(means3D.device());
     const auto dev = means3D.device();
@@ -248,7 +256,24 @@ static BackwardGrads backward_grads(const torch::Tensor& background, const torch
                 else return run(fn, gp, std::tuple<>(), tail);
             };
         };
-        if (camera)
+        if (feature_geometry) {
+            // this entry reads the features themselves, not only their shape
+            TORCH_CHECK(!C || semantic_feature.numel() == (int64_t)P * C, "semantic_feature must have P * C = ",
+                        (int64_t)P * C, " elements (got ", semantic_feature.numel(), ")");
+            auto sf = C ? semantic_feature.contiguous() : semantic_feature;
+            check_rc(f3dgs_backward_feature_geometry(
+                         P, degree, M, R, C, fptr(bg), W, H, fptr(m3), fptr(shc), fptr(col), C ? sf.data_ptr() : nullptr,
+                         dtype_code(sf), fptr(sc), scale_modifier, fptr(rot), fptr(cov), fptr(vm), fptr(pm), fptr(cp),
+                         tan_fovx, tan_fovy, rad.data_ptr<int>(), reinterpret_cast<char*>(gb.data_ptr()),
+                         reinterpret_cast<char*>(bb.data_ptr()), reinterpret_cast<char*>(ib.data_ptr()), fptr(gc),
+                         gf.defined() ? gf.data_ptr() : nullptr, dtype_code(gf), 1.0f, fptr(gd),
+                         dL_dmeans2D.data_ptr<float>(), dL_dconic.data_ptr<float>(), dL_dopacity.data_ptr<float>(),
+                         dL_dcolors.data_ptr<float>(), C ? dL_dsemantic_feature.data_ptr<float>() : nullptr,
+                         dL_dmeans3D.data_ptr<float>(), dL_dcov3D.data_ptr<float>(),
+                         M ? dL_dsh.data_ptr<float>() : nullptr, dL_dscales.data_ptr<float>(),
+                         dL_drotations.data_ptr<float>(), dL_dz.data_ptr<float>(), debug ? 1 : 0, (void*)stream, camera),
+                     "f3dgs_backward_feature_geometry");
+        } else if (camera)
             call_f32_or_f16(gf, f3dgs_backward_cam, "f3dgs_backward_cam", f3dgs_backward_cam_f16,
                             "f3dgs_backward_cam_f16", dispatch(std::make_tuple(camera)));
         else
@@ -285,12 +310,29 @@ RasterizeGaussiansBackwardCameraCUDA(BACKWARD_PARAMS) {
                           std::make_tuple(cam.narrow(0, 0, 16).view({4, 4}), cam.narrow(0, 16, 16).view({4, 4}),
                                           cam.narrow(0, 32, 3)));
 }
+
+// rasterize_gaussians_backward_camera's 12 results, with the feature term of dL/dalpha in the geometric gradients
+// (f3dgs_backward_feature_geometry); without `camera` the three camera gradients are None and none is computed
+decltype(std::tuple_cat(BackwardGrads(), std::tuple<torch::Tensor, torch::Tensor, torch::Tensor>()))
+RasterizeGaussiansBackwardFeatureGeometryCUDA(BACKWARD_PARAMS, const bool camera) {
+    TORCH_CHECK(means3D.is_cuda(), "means3D must be a CUDA tensor (this build has no CPU path)");
+    const c10::cuda::CUDAGuard guard(means3D.device());
+    if (!camera)
+        return std::tuple_cat(backward_grads(BACKWARD_ARGS, nullptr, true),
+                              std::make_tuple(torch::Tensor(), torch::Tensor(), torch::Tensor()));
+    torch::Tensor cam = torch::zeros({F3DGS_CAMERA_GRAD_FLOATS}, means3D.options().dtype(torch::kFloat32));
+    return std::tuple_cat(backward_grads(BACKWARD_ARGS, cam.data_ptr<float>(), true),
+                          std::make_tuple(cam.narrow(0, 0, 16).view({4, 4}), cam.narrow(0, 16, 16).view({4, 4}),
+                                          cam.narrow(0, 32, 3)));
+}
 #undef BACKWARD_PARAMS
 #undef BACKWARD_ARGS
 
 // Accumulating backward for view batches (additive to the reference module): gradients are ADDED into the tensors the
 // caller passes (typically views of one flat gradient buffer, see diff_gaussian_rasterization/parallel.py); nothing is
 // allocated besides one cached scratch tensor per device.  Undefined / empty tensors stand for "not an input".
+// semantic_feature (optional, [P,...,C] float32 or float16): f3dgs_backward_accum_feature_geometry, the feature term of
+// dL/dalpha in the geometric gradients.
 void RasterizeGaussiansBackwardAccumCUDA(
     const torch::Tensor& background, const torch::Tensor& means3D, const torch::Tensor& radii,
     const torch::Tensor& colors, const torch::Tensor& scales, const torch::Tensor& rotations, const float scale_modifier,
@@ -302,7 +344,7 @@ void RasterizeGaussiansBackwardAccumCUDA(
     torch::Tensor g_semantic_feature, torch::Tensor g_opacities, torch::Tensor g_scales, torch::Tensor g_rotations,
     torch::Tensor g_cov3D, torch::Tensor g_means2D_out, torch::Tensor grad_accum, torch::Tensor denom,
     const int64_t composite_done_event, const bool debug, const double feature_grad_scale,
-    const std::optional<torch::Tensor>& camera_grad) {
+    const std::optional<torch::Tensor>& camera_grad, const std::optional<torch::Tensor>& semantic_feature) {
     TORCH_CHECK(means3D.is_cuda(), "means3D must be a CUDA tensor (this build has no CPU path)");
     const c10::cuda::CUDAGuard guard(means3D.device());
     const auto dev = means3D.device();
@@ -339,6 +381,32 @@ void RasterizeGaussiansBackwardAccumCUDA(
         cam = in_place(*camera_grad, dev, F3DGS_CAMERA_GRAD_FLOATS, "camera_grad");
     }
     cudaStream_t stream = c10::cuda::getCurrentCUDAStream().stream();
+    if (semantic_feature.has_value() && semantic_feature->defined()) {
+        check_features(*semantic_feature, dev);
+        TORCH_CHECK(semantic_feature->numel() == (int64_t)P * C, "semantic_feature must have P * C = ", (int64_t)P * C,
+                    " elements (got ", semantic_feature->numel(), ")");
+        auto sf = semantic_feature->contiguous();
+        check_rc(f3dgs_backward_accum_feature_geometry(
+                     P, degree, M, R, C, fptr(bg), W, H, fptr(m3), fptr(shc), fptr(col), C ? sf.data_ptr() : nullptr,
+                     dtype_code(sf), fptr(sc), scale_modifier, fptr(rot), fptr(cov), fptr(vm), fptr(pm), fptr(cp),
+                     tan_fovx, tan_fovy, rad.data_ptr<int>(), reinterpret_cast<char*>(geomBuffer.data_ptr()),
+                     reinterpret_cast<char*>(binningBuffer.data_ptr()),
+                     reinterpret_cast<char*>(imageBuffer.data_ptr()), fptr(gc), gf.defined() ? gf.data_ptr() : nullptr,
+                     dtype_code(gf), (float)feature_grad_scale, fptr(gd), reinterpret_cast<char*>(scratch.data_ptr()),
+                     in_place(g_opacities, dev, P, "g_opacities"),
+                     in_place(g_colors, dev, (int64_t)P * 3, "g_colors_precomp"),
+                     in_place(g_semantic_feature, dev, (int64_t)P * C, "g_semantic_feature"),
+                     in_place(g_means3D, dev, (int64_t)P * 3, "g_means3D"),
+                     in_place(g_cov3D, dev, (int64_t)P * 6, "g_cov3D_precomp"),
+                     in_place(g_sh, dev, (int64_t)P * M * 3, "g_sh"), in_place(g_scales, dev, (int64_t)P * 3, "g_scales"),
+                     in_place(g_rotations, dev, (int64_t)P * 4, "g_rotations"),
+                     in_place(g_means2D_out, dev, (int64_t)P * 3, "g_means2D_out"),
+                     in_place(grad_accum, dev, P, "grad_accum"), in_place(denom, dev, P, "denom"),
+                     reinterpret_cast<void*>(static_cast<intptr_t>(composite_done_event)), debug ? 1 : 0,
+                     (void*)stream, cam),
+                 "f3dgs_backward_accum_feature_geometry");
+        return;
+    }
     // scale: the float16 symbol's scale after the map, () for the float32 one; tail: (dL_dcamera) or ()
     auto run = [&](auto fn, auto gp, auto scale, auto tail) {
         return std::apply(
@@ -904,9 +972,11 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
               py::arg("g_sh"), py::arg("g_colors"), py::arg("g_semantic_feature"), py::arg("g_opacities"),
               py::arg("g_scales"), py::arg("g_rotations"), py::arg("g_cov3D"), py::arg("g_means2D_out"),
               py::arg("grad_accum"), py::arg("denom"), py::arg("composite_done_event"), py::arg("debug"),
-              py::arg("feature_grad_scale") = 1.0, py::arg("camera_grad") = py::none());
+              py::arg("feature_grad_scale") = 1.0, py::arg("camera_grad") = py::none(),
+              py::arg("semantic_feature") = py::none());
     }
     m.def("rasterize_gaussians_backward_camera", &RasterizeGaussiansBackwardCameraCUDA);
+    m.def("rasterize_gaussians_backward_feature_geometry", &RasterizeGaussiansBackwardFeatureGeometryCUDA);
     m.def("lift_features_accum", &liftFeaturesAccum, pybind11::arg("geomBuffer"), pybind11::arg("R"),
           pybind11::arg("binningBuffer"), pybind11::arg("imageBuffer"), pybind11::arg("feature_map"),
           pybind11::arg("feature_sum"), pybind11::arg("weight_sum"));

@@ -27,6 +27,10 @@ Behavioural notes
     `.projmatrix` or `.campos` requires grad, `rasterize_gaussians` goes through `_RasterizeGaussiansCamera`, which
     also returns dL/dviewmatrix, dL/dprojmatrix and dL/dcampos (f3dgs_backward_cam); otherwise the call and its graph
     are `_RasterizeGaussians`'s.  `camera.settings_from_w2c` builds differentiable settings from a world-to-camera pose.
+  * feature gradients into geometry (opt-in): `GaussianRasterizer(raster_settings, feature_geometry=True)`, or
+    `rasterize_gaussians_feature_geometry` with `rasterize_gaussians`'s arguments, lets a loss on the feature map move
+    opacities, means, scales, rotations and the camera too (f3dgs_backward_feature_geometry).  By default the feature
+    map feeds dL/dsemantic_feature only, as in the reference (SURVEY D.1).
   * `debug=True` keeps the reference semantics: arguments are snapshotted to CPU first and dumped
     to snapshot_fw.dump / snapshot_bw.dump if the native call raises (reference :89-97,:147-155);
     natively it synchronises and checks after every stage.
@@ -51,6 +55,7 @@ __all__ = [
     "GaussianRasterizationSettings",
     "GaussianRasterizer",
     "rasterize_gaussians",
+    "rasterize_gaussians_feature_geometry",
 ]
 
 
@@ -164,25 +169,69 @@ class _RasterizeGaussiansCamera(torch.autograd.Function):
         return grads[:9] + cam + (None,)
 
 
+def _feature_geometry_backward(camera):
+    """rasterize_gaussians_backward_feature_geometry with the reference backward's positional arguments"""
+    return lambda *args: _C.rasterize_gaussians_backward_feature_geometry(*args, camera)
+
+
+class _RasterizeGaussiansFeatureGeometry(_RasterizeGaussians):
+    """_RasterizeGaussians whose backward also carries the feature map's gradient into the geometry: the feature term
+    of dL/dalpha (f3dgs_backward_feature_geometry), which reads semantic_feature."""
+
+    @staticmethod
+    def backward(ctx, grad_out_color, grad_out_feature, _grad_radii, grad_depth):
+        grads = _native_backward(ctx, _feature_geometry_backward(False), grad_out_color, grad_out_feature, grad_depth)
+        return grads[:9] + (None,)
+
+
+class _RasterizeGaussiansCameraFeatureGeometry(_RasterizeGaussiansCamera):
+    """_RasterizeGaussiansCamera with the feature term of dL/dalpha, so that the camera gets it too."""
+
+    @staticmethod
+    def backward(ctx, grad_out_color, grad_out_feature, _grad_radii, grad_depth):
+        grads = _native_backward(ctx, _feature_geometry_backward(True), grad_out_color, grad_out_feature, grad_depth)
+        cam = tuple(g.reshape(shape) for g, shape in zip(grads[9:], ctx.camera_shapes))
+        return grads[:9] + cam + (None,)
+
+
 def _camera_requires_grad(rs):
     return any(isinstance(t, torch.Tensor) and t.requires_grad for t in (rs.viewmatrix, rs.projmatrix, rs.campos))
 
 
+def _rasterize(means3D, means2D, sh, colors_precomp, semantic_feature, opacities, scales, rotations, cov3Ds_precomp,
+               rs, feature_geometry):
+    if torch.is_grad_enabled() and _camera_requires_grad(rs):
+        fn = _RasterizeGaussiansCameraFeatureGeometry if feature_geometry else _RasterizeGaussiansCamera
+        return fn.apply(means3D, means2D, sh, colors_precomp, semantic_feature, opacities, scales, rotations,
+                        cov3Ds_precomp, rs.viewmatrix, rs.projmatrix, rs.campos, rs)
+    fn = _RasterizeGaussiansFeatureGeometry if feature_geometry else _RasterizeGaussians
+    return fn.apply(means3D, means2D, sh, colors_precomp, semantic_feature, opacities, scales, rotations,
+                    cov3Ds_precomp, rs)
+
+
 def rasterize_gaussians(means3D, means2D, sh, colors_precomp, semantic_feature, opacities, scales, rotations,
                         cov3Ds_precomp, raster_settings):
-    rs = raster_settings
-    if torch.is_grad_enabled() and _camera_requires_grad(rs):
-        return _RasterizeGaussiansCamera.apply(means3D, means2D, sh, colors_precomp, semantic_feature, opacities,
-                                               scales, rotations, cov3Ds_precomp, rs.viewmatrix, rs.projmatrix,
-                                               rs.campos, rs)
-    return _RasterizeGaussians.apply(means3D, means2D, sh, colors_precomp, semantic_feature, opacities, scales,
-                                     rotations, cov3Ds_precomp, raster_settings)
+    return _rasterize(means3D, means2D, sh, colors_precomp, semantic_feature, opacities, scales, rotations,
+                      cov3Ds_precomp, raster_settings, False)
+
+
+def rasterize_gaussians_feature_geometry(means3D, means2D, sh, colors_precomp, semantic_feature, opacities, scales,
+                                         rotations, cov3Ds_precomp, raster_settings):
+    """rasterize_gaussians whose backward also feeds the feature map's gradient into dL/dalpha, and so into the
+    opacities, means, scales, rotations (or cov3Ds_precomp) and a camera that requires grad.  The render and every
+    other gradient are rasterize_gaussians'."""
+    return _rasterize(means3D, means2D, sh, colors_precomp, semantic_feature, opacities, scales, rotations,
+                      cov3Ds_precomp, raster_settings, True)
 
 
 class GaussianRasterizer(nn.Module):
-    def __init__(self, raster_settings):
+    """The reference's rasterizer module.  feature_geometry=True: the backward also feeds the feature map's gradient
+    into the geometry (rasterize_gaussians_feature_geometry)."""
+
+    def __init__(self, raster_settings, feature_geometry=False):
         super().__init__()
         self.raster_settings = raster_settings
+        self.feature_geometry = feature_geometry
 
     def markVisible(self, positions):
         """Boolean mask of points in front of the near plane (reference :193-202)."""
@@ -209,5 +258,5 @@ class GaussianRasterizer(nn.Module):
             rotations = empty
         if cov3D_precomp is None:
             cov3D_precomp = empty
-        return rasterize_gaussians(means3D, means2D, shs, colors_precomp, semantic_feature, opacities, scales,
-                                   rotations, cov3D_precomp, rs)
+        return _rasterize(means3D, means2D, shs, colors_precomp, semantic_feature, opacities, scales, rotations,
+                          cov3D_precomp, rs, self.feature_geometry)

@@ -159,14 +159,19 @@ class ViewBatch:
         ctx.num_rendered, color, feat, depth, ctx.radii, ctx.geom, ctx.binning, ctx.img = out
         return color, feat, ctx.radii, depth, ctx
 
-    def backward(self, ctx, g_color, g_feature, g_depth, means2D_out=None, last: bool = False, camera: bool = False):
+    def backward(self, ctx, g_color, g_feature, g_depth, means2D_out=None, last: bool = False, camera: bool = False,
+                 feature_geometry: bool = False):
         """Add this view's parameter gradients into the flat buffer.  `last=True` on the rank's last view of the step
         lets all_reduce() start the feature/opacity bucket early.  g_feature: dL/dfeature_map as a float32 or float16
         [C,H,W] tensor, a feature_head.ScaledGrad (a float16 map and its float32 scale), or None.
 
         camera=True also returns this view's CameraGrad (dL/dviewmatrix, dL/dprojmatrix, dL/dcampos of its settings,
         f3dgs_backward_accum_cam); the flat buffer and the densification statistics are bitwise those of camera=False.
-        A camera gradient belongs to its view and stays on the rank that rendered it: all_reduce() does not touch it."""
+        A camera gradient belongs to its view and stays on the rank that rendered it: all_reduce() does not touch it.
+
+        feature_geometry=True also feeds g_feature into dL/dalpha, so that the feature loss reaches the opacities, means,
+        scales, rotations, the densification statistics and the camera gradient (f3dgs_backward_accum_feature_geometry,
+        which reads the batch's semantic_feature)."""
         rs, p, g, e = ctx.rs, self.params, self.grads, torch.Tensor([])
         none = self._empty
         scale = 1.0
@@ -180,7 +185,8 @@ class ViewBatch:
             g["means3D"], g["shs"], none, g.get("semantic_feature", none), g["opacities"], g["scales"], g["rotations"],
             none, means2D_out if means2D_out is not None else none,
             self.grad_accum if self.grad_accum is not None else none, self.denom if self.denom is not None else none,
-            int(self._ev.cuda_event) if (last and self._ev is not None) else 0, rs.debug, float(scale), cam)
+            int(self._ev.cuda_event) if (last and self._ev is not None) else 0, rs.debug, float(scale), cam,
+            p.get("semantic_feature") if feature_geometry else None)
         self._early_pending = bool(last and self._ev is not None)
         if cam is not None:
             return CameraGrad(cam[:16].view(4, 4), cam[16:32].view(4, 4), cam[32:35])

@@ -39,6 +39,9 @@ extern "C" {
 #define F3DGS_MAX_FEATURE_DIM 4096
 #define F3DGS_TILE 16 /* BLOCK_X == BLOCK_Y == 16, reference config.h:18-19 */
 #define F3DGS_CAMERA_GRAD_FLOATS 35 /* dL_dcamera of the _cam backward entries */
+/* element-type codes of the _feature_geometry backward entries */
+#define F3DGS_F32 0 /* IEEE binary32 */
+#define F3DGS_F16 1 /* IEEE binary16 */
 
 /* error codes (returned negated) */
 #define F3DGS_OK 0
@@ -199,7 +202,7 @@ int f3dgs_backward_accum_f16(int P, int D, int M, int R, int C,
  * The entries the forward never reads (viewmatrix[3,7,11,15], projmatrix[2,6,10,14]) get 0, and dL/dcampos gets only
  * the SH view-direction term (0 with colors_precomp).  A clamped view-space coordinate of the EWA Jacobian passes no
  * gradient, as for dL_dmean3D.  The feature map does not feed the geometry (SURVEY D.1): a loss on features alone gives
- * a zero camera gradient, as it gives a zero dL_dmean3D.
+ * a zero camera gradient, as it gives a zero dL_dmean3D (the _feature_geometry entries below lift that).
  * The sum over Gaussians is free of floating-point atomics: float32 per-Gaussian terms, float64 block partials (taken
  * from the device's default memory pool; F3DGS_ERR_ALLOC if that fails) reduced in a fixed order, then rounded once and
  * added, so equal inputs give bitwise-equal results.  A NULL dL_dcamera, or one that overlaps another output (or the
@@ -261,6 +264,57 @@ int f3dgs_backward_accum_cam_f16(int P, int D, int M, int R, int C,
                                  float* dL_dmean3D, float* dL_dcov3D_precomp, float* dL_dsh, float* dL_dscale,
                                  float* dL_drot, float* dL_dmean2D_out, float* grad_accum, float* denom,
                                  void* composite_done_event, int debug, void* cuda_stream, float* dL_dcamera);
+
+/* ---- feature gradients into geometry (opt-in; no reference counterpart: the reference disables the line,
+ * backward.cu:575, and every other backward entry here keeps that, SURVEY D.1) ----
+ * f3dgs_backward_feature_geometry takes f3dgs_backward's arguments and f3dgs_backward_accum_feature_geometry those of
+ * f3dgs_backward_accum, with contracts unchanged, except that:
+ *   - semantic_feature [P,C] (the forward's features) is read, of element type semantic_feature_dtype (F3DGS_F32, or
+ *     F3DGS_F16 upcast exactly, as the forward reads it);
+ *   - dL_dfeaturepix [C,H,W] has element type dL_dfeaturepix_dtype: F3DGS_F32, or F3DGS_F16 standing for
+ *     dL_dfeaturepix_scale * float(h) as in f3dgs_backward_f16 (the scale is not read for F3DGS_F32);
+ *   - dL_dcamera (optional, NULL: none) is the _cam entries' 35-float camera gradient, added to;
+ *   - the feature map's gradient also feeds dL/dalpha, so that it reaches dL_dopacity, the screen-space mean and conic
+ *     and, through them, dL_dmean3D, dL_dscale, dL_drot, dL_dcov3D and dL_dcamera.  For pixel p with blend weights
+ *     w_i = alpha_i T_i (front to back) and d_ip = f_i . dL_dfeaturepix[:,p] (a C-wide dot product), the term added is
+ *         dL/dalpha_i += T_i (d_ip - A_i),   A_i = alpha_{i+1} d_{i+1,p} + (1 - alpha_{i+1}) A_{i+1},   A_last = 0,
+ *     the colour channels' recurrence with one channel d and a zero feature background (the feature map has none).
+ * dL_dsemantic_feature, dL_dcolor and dL_dz are bitwise those of the counterpart; with a zero dL_dfeaturepix every output
+ * is.  The densification statistics (grad_accum += ||dL_dmean2D.xy||) and dL_dmean2D_out include the feature term.  The
+ * term costs two more kernels over the backward's per-block instance lists.  With C == 0 these entries are their
+ * counterparts.  F3DGS_ERR_INVALID_ARGUMENT, before any launch, for a NULL semantic_feature with C > 0, an unknown dtype
+ * code, a float16 map's scale that is not finite and nonzero, semantic_feature overlapping an output, and whatever the
+ * counterpart (or, with dL_dcamera, its _cam twin) rejects. */
+int f3dgs_backward_feature_geometry(int P, int D, int M, int R, int C,
+                                    const float* background, int width, int height,
+                                    const float* means3D, const float* shs, const float* colors_precomp,
+                                    const void* semantic_feature, int semantic_feature_dtype,
+                                    const float* scales, float scale_modifier, const float* rotations,
+                                    const float* cov3D_precomp,
+                                    const float* viewmatrix, const float* projmatrix, const float* cam_pos,
+                                    float tan_fovx, float tan_fovy, const int* radii,
+                                    char* geom_buffer, char* binning_buffer, char* image_buffer,
+                                    const float* dL_dpix, const void* dL_dfeaturepix, int dL_dfeaturepix_dtype,
+                                    float dL_dfeaturepix_scale, const float* dL_depths,
+                                    float* dL_dmean2D, float* dL_dconic, float* dL_dopacity, float* dL_dcolor,
+                                    float* dL_dsemantic_feature, float* dL_dmean3D, float* dL_dcov3D,
+                                    float* dL_dsh, float* dL_dscale, float* dL_drot, float* dL_dz,
+                                    int debug, void* cuda_stream, float* dL_dcamera);
+int f3dgs_backward_accum_feature_geometry(int P, int D, int M, int R, int C,
+                                          const float* background, int width, int height,
+                                          const float* means3D, const float* shs, const float* colors_precomp,
+                                          const void* semantic_feature, int semantic_feature_dtype,
+                                          const float* scales, float scale_modifier, const float* rotations,
+                                          const float* cov3D_precomp,
+                                          const float* viewmatrix, const float* projmatrix, const float* cam_pos,
+                                          float tan_fovx, float tan_fovy, const int* radii,
+                                          char* geom_buffer, char* binning_buffer, char* image_buffer,
+                                          const float* dL_dpix, const void* dL_dfeaturepix, int dL_dfeaturepix_dtype,
+                                          float dL_dfeaturepix_scale, const float* dL_depths, char* scratch,
+                                          float* dL_dopacity, float* dL_dcolors_precomp, float* dL_dsemantic_feature,
+                                          float* dL_dmean3D, float* dL_dcov3D_precomp, float* dL_dsh, float* dL_dscale,
+                                          float* dL_drot, float* dL_dmean2D_out, float* grad_accum, float* denom,
+                                          void* composite_done_event, int debug, void* cuda_stream, float* dL_dcamera);
 
 /* ---- feature lifting (no reference counterpart): training-free back-projection of 2-D feature maps onto Gaussians ----
  * The buffers and R are those of an f3dgs_forward / f3dgs_forward_f16 of this view at width x height (any C of that
