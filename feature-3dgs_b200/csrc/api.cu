@@ -249,8 +249,8 @@ int f3dgs_get_layout(int P, int width, int height, int R, f3dgs_layout* out) {
 
 namespace {
 
-// Shared body of f3dgs_forward (TF = float) and f3dgs_forward_f16 (TF = __half): TF is the element type of
-// semantic_feature and out_feature_map only.
+// Shared body of f3dgs_forward (TF = float), f3dgs_forward_f16 (TF = __half) and f3dgs_forward_antialiased: TF is the
+// element type of semantic_feature and out_feature_map only.  antialiasing: op_eff = opacity * rho in the records.
 template <typename TF>
 int forward_impl(const char* entry, f3dgs_alloc_fn geometry_alloc, void* geometry_ctx, f3dgs_alloc_fn binning_alloc,
                  void* binning_ctx, f3dgs_alloc_fn image_alloc, void* image_ctx, int P, int D, int M, int C,
@@ -258,7 +258,8 @@ int forward_impl(const char* entry, f3dgs_alloc_fn geometry_alloc, void* geometr
                  const float* colors_precomp, const TF* semantic_feature, const float* opacities, const float* scales,
                  float scale_modifier, const float* rotations, const float* cov3D_precomp, const float* viewmatrix,
                  const float* projmatrix, const float* cam_pos, float tan_fovx, float tan_fovy, int prefiltered,
-                 float* out_color, TF* out_feature_map, float* out_depth, int* radii, int debug, void* cuda_stream) {
+                 float* out_color, TF* out_feature_map, float* out_depth, int* radii, int debug, void* cuda_stream,
+                 bool antialiasing = false) {
     const Api api(entry);
     cudaStream_t stream = (cudaStream_t)cuda_stream;
     if (P < 0 || width <= 0 || height <= 0 || C < 0 || C > F3DGS_MAX_FEATURE_DIM || D < 0 || D > 3)
@@ -306,7 +307,7 @@ int forward_impl(const char* entry, f3dgs_alloc_fn geometry_alloc, void* geometr
     {
         StageTimer t(F3DGS_STAGE_PREPROCESS_FWD, stream);
         launch_preprocess_fwd(vp, means3D, scales, rotations, opacities, shs, cov3D_precomp, colors_precomp,
-                              prefiltered != 0, radii, rec, cov3d, clamped, tiles_touched, stream);
+                              prefiltered != 0, radii, rec, cov3d, clamped, tiles_touched, stream, antialiasing);
     }
     STAGE_CHECK("preprocess");
     {
@@ -409,6 +410,29 @@ int f3dgs_forward_f16(f3dgs_alloc_fn geometry_alloc, void* geometry_ctx, f3dgs_a
                         reinterpret_cast<__half*>(out_feature_map), out_depth, radii, debug, cuda_stream);
 }
 
+int f3dgs_forward_antialiased(f3dgs_alloc_fn geometry_alloc, void* geometry_ctx, f3dgs_alloc_fn binning_alloc,
+                              void* binning_ctx, f3dgs_alloc_fn image_alloc, void* image_ctx, int P, int D, int M,
+                              int C, const float* background, int width, int height, const float* means3D,
+                              const float* shs, const float* colors_precomp, const void* semantic_feature,
+                              int semantic_feature_dtype, const float* opacities, const float* scales,
+                              float scale_modifier, const float* rotations, const float* cov3D_precomp,
+                              const float* viewmatrix, const float* projmatrix, const float* cam_pos, float tan_fovx,
+                              float tan_fovy, int prefiltered, float* out_color, void* out_feature_map,
+                              float* out_depth, int* radii, int debug, void* cuda_stream) {
+    const char* entry = __func__;
+    const auto run = [&](auto* features) {
+        using TF = std::remove_const_t<std::remove_pointer_t<decltype(features)>>;
+        return forward_impl(entry, geometry_alloc, geometry_ctx, binning_alloc, binning_ctx, image_alloc, image_ctx,
+                            P, D, M, C, background, width, height, means3D, shs, colors_precomp, features, opacities,
+                            scales, scale_modifier, rotations, cov3D_precomp, viewmatrix, projmatrix, cam_pos, tan_fovx,
+                            tan_fovy, prefiltered, out_color, static_cast<TF*>(out_feature_map), out_depth, radii,
+                            debug, cuda_stream, true);
+    };
+    if (semantic_feature_dtype == F3DGS_F32) return run(static_cast<const float*>(semantic_feature));
+    if (semantic_feature_dtype == F3DGS_F16) return run(static_cast<const __half*>(semantic_feature));
+    return Api(__func__).invalid("unknown dtype code");
+}
+
 }  // extern "C"
 
 namespace {
@@ -430,7 +454,11 @@ struct ScratchLayout {  // per-view intermediates of the accumulating backward (
 // f3dgs_backward_accum (accumulate = true: += into the caller's per-parameter gradient buffers) and their _f16 twins.
 // TG (float or __half) is the element type of dL_dfeaturepix; a __half map stands for dL/dO = scale * float(h).
 // `zero` (accumulate only): the caller's scratch, zeroed once the arguments are validated.  feat.rows (the _feature_geometry
-// entries only; NULL on every other path): the Gaussians' features, for the feature term of dL/dalpha.
+// entries only; NULL on every other path): the Gaussians' features, for the feature term of dL/dalpha.  antialiasing
+// (the _antialiased entries): the forward's records hold op_eff = opacity * rho, so the composite's opacity gradient is
+// dL/dop_eff and the preprocess backward turns it into dL/dopacity (and rho's geometric terms).  The assigning backward
+// lets the composite write into dL_dopacity and rescales it in place; the accumulating one needs dL/dop_eff of this view
+// alone, so the composite writes into P zeroed floats of the device's default memory pool.
 template <typename TG>
 int backward_impl(const Api& api, bool accumulate, int P, int D, int M, int R, int C, const float* background, int width,
                   int height, const float* means3D, const float* shs, const float* scales, float scale_modifier,
@@ -441,7 +469,7 @@ int backward_impl(const Api& api, bool accumulate, int P, int D, int M, int R, i
                   float* dL_dopacity, float* dL_dcolor, float* dL_dsemantic_feature, float* dL_dmean3D, float* dL_dcov3D,
                   float* dL_dsh, float* dL_dscale, float* dL_drot, float* dL_dz, float* grad_accum, float* denom,
                   float* dL_dcamera, cudaEvent_t composite_done, int debug, cudaStream_t stream,
-                  const Range& zero = {nullptr, 0}, const FeatureRows& feat = {}) {
+                  const Range& zero = {nullptr, 0}, const FeatureRows& feat = {}, bool antialiasing = false) {
     if (P < 0 || width <= 0 || height <= 0 || C < 0 || C > F3DGS_MAX_FEATURE_DIM || R < 0)
         return api.invalid("bad sizes");
     if (P == 0) return 0;
@@ -479,6 +507,15 @@ int backward_impl(const Api& api, bool accumulate, int P, int D, int M, int R, i
         if (overlaps({feat.rows, (size_t)P * C * (feat.f16 ? 2 : 4)}, outs))
             return api.invalid("semantic_feature overlaps an output");
     }
+    if (antialiasing) {  // the preprocess backward writes dL_dopacity while it writes the others
+        const size_t p4 = (size_t)P * 4;
+        const Range outs[] = {{dL_dmean2D, 3 * p4}, {dL_dconic, 4 * p4}, {dL_dcolor, 3 * p4},
+                              {dL_dsemantic_feature, (size_t)C * p4}, {dL_dmean3D, 3 * p4}, {dL_dcov3D, 6 * p4},
+                              {dL_dsh, (size_t)M * 3 * p4}, {dL_dscale, 3 * p4}, {dL_drot, 4 * p4}, {dL_dz, p4},
+                              {grad_accum, p4}, {denom, p4}, {dL_dcamera, F3DGS_CAMERA_GRAD_FLOATS * sizeof(float)},
+                              zero};
+        if (overlaps({dL_dopacity, p4}, outs)) return api.invalid("dL_dopacity overlaps another output");
+    }
     if (zero.p) CUDA_TRY(cudaMemsetAsync(const_cast<void*>(zero.p), 0, zero.bytes, stream));
 
     const ViewParams vp = make_view(P, D, M, C, width, height, tan_fovx, tan_fovy, scale_modifier, viewmatrix,
@@ -489,26 +526,46 @@ int backward_impl(const Api& api, bool accumulate, int P, int D, int M, int R, i
     if (radii == nullptr) radii = reinterpret_cast<const int*>(geom_buffer + gl.radii);
 
     cudaError_t e;
+    // where the composite puts the opacity gradient: dL/dop_eff under antialiasing (see above)
+    struct PoolFloats {  // returned to the pool on every exit
+        float* p = nullptr;
+        cudaStream_t s;
+        ~PoolFloats() {
+            if (p) cudaFreeAsync(p, s);
+        }
+    } op_eff_grad{nullptr, stream};
+    float* dL_dop_eff = dL_dopacity;
+    if (antialiasing && accumulate) {
+        e = cudaMallocAsync((void**)&op_eff_grad.p, (size_t)P * sizeof(float), stream);
+        if (e != cudaSuccess)
+            return api.fail(F3DGS_ERR_ALLOC, std::string("cudaMallocAsync for dL/dop_eff failed: ") +
+                                                 cudaGetErrorString(e));
+        CUDA_TRY(cudaMemsetAsync(op_eff_grad.p, 0, (size_t)P * sizeof(float), stream));
+        dL_dop_eff = op_eff_grad.p;
+    }
     {
         StageTimer t(F3DGS_STAGE_COMPOSITE_BWD, stream);
         e = launch_composite_bwd(vp, forward_buffers(vp, R, geom_buffer, binning_buffer, image_buffer), background,
                                  dL_dpix, dL_depths, dL_dfeaturepix, dL_dfeaturepix_scale, dL_dmean2D, dL_dconic,
-                                 dL_dopacity, dL_dcolor, dL_dz, dL_dsemantic_feature, stream, feat);
+                                 dL_dop_eff, dL_dcolor, dL_dz, dL_dsemantic_feature, stream, feat);
     }
     if (const int rc = composite_bwd_result(api, e, "composite_bwd launch")) return rc;
     STAGE_CHECK("composite_bwd");
-    if (composite_done) CUDA_TRY(cudaEventRecord(composite_done, stream));
+    // dL_dopacity is final after the composite, or under antialiasing after the preprocess backward
+    if (composite_done && !antialiasing) CUDA_TRY(cudaEventRecord(composite_done, stream));
     {
         StageTimer t(F3DGS_STAGE_PREPROCESS_BWD, stream);
         e = launch_preprocess_bwd(vp, means3D, radii, shs, clamped, scales, rotations, cov3d, dL_dmean2D, dL_dconic,
                                   dL_dmean3D, dL_dcolor, dL_dcov3D, dL_dsh, dL_dscale, dL_drot, dL_dz, stream,
-                                  accumulate, grad_accum, denom, dL_dcamera);
+                                  accumulate, grad_accum, denom, dL_dcamera, antialiasing,
+                                  reinterpret_cast<const SplatRec*>(geom_buffer + gl.rec), dL_dop_eff, dL_dopacity);
     }
     if (e == cudaErrorMemoryAllocation)
         return api.fail(F3DGS_ERR_ALLOC, std::string("cudaMallocAsync for the camera-gradient partials failed: ") +
                                              cudaGetErrorString(e));
     CUDA_TRY(e);
     STAGE_CHECK("preprocess_bwd");
+    if (composite_done && antialiasing) CUDA_TRY(cudaEventRecord(composite_done, stream));
     return 0;
 }
 
@@ -618,7 +675,7 @@ int backward_accum_impl(const char* entry, int P, int D, int M, int R, int C, co
                         float* dL_dsemantic_feature, float* dL_dmean3D, float* dL_dcov3D_precomp, float* dL_dsh,
                         float* dL_dscale, float* dL_drot, float* dL_dmean2D_out, float* grad_accum, float* denom,
                         void* composite_done_event, int debug, void* cuda_stream, bool camera = false,
-                        float* dL_dcamera = nullptr, const FeatureRows& feat = {}) {
+                        float* dL_dcamera = nullptr, const FeatureRows& feat = {}, bool antialiasing = false) {
     const Api api(entry);
     cudaStream_t stream = (cudaStream_t)cuda_stream;
     if (camera && !dL_dcamera) return api.invalid("NULL dL_dcamera");
@@ -642,7 +699,7 @@ int backward_accum_impl(const char* entry, int P, int D, int M, int R, int C, co
         binning_buffer, image_buffer, dL_dpix, dL_dfeaturepix, dL_dfeaturepix_scale, dL_depths, m2d,
         reinterpret_cast<float*>(scratch + sl.conic), dL_dopacity, dcol, dL_dsemantic_feature, dL_dmean3D, dcov, dL_dsh,
         dL_dscale, dL_drot, reinterpret_cast<float*>(scratch + sl.dz), grad_accum, denom, dL_dcamera,
-        (cudaEvent_t)composite_done_event, debug, stream, {scratch, sl.bytes}, feat);
+        (cudaEvent_t)composite_done_event, debug, stream, {scratch, sl.bytes}, feat, antialiasing);
     if (rc < 0) return rc;
     if (dL_dmean2D_out)
         CUDA_TRY(cudaMemcpyAsync(dL_dmean2D_out, m2d, (size_t)P * 3 * sizeof(float), cudaMemcpyDeviceToDevice, stream));
@@ -732,12 +789,13 @@ int f3dgs_backward_accum_cam_f16(int P, int D, int M, int R, int C, const float*
 }  // extern "C"
 
 namespace {
-// The Gaussians' features of a _feature_geometry entry, after the checks every such entry makes before any launch
+// The Gaussians' features of a _feature_geometry or _antialiased entry, after the checks every such entry makes before
+// any launch.  `optional` (the _antialiased entries): a NULL semantic_feature means no feature term.
 int feature_rows(const Api& api, int C, const void* semantic_feature, int semantic_feature_dtype,
-                 int dL_dfeaturepix_dtype, FeatureRows& feat) {
+                 int dL_dfeaturepix_dtype, FeatureRows& feat, bool optional = false) {
     const auto known = [](int t) { return t == F3DGS_F32 || t == F3DGS_F16; };
     if (!known(semantic_feature_dtype) || !known(dL_dfeaturepix_dtype)) return api.invalid("unknown dtype code");
-    if (C > 0 && !semantic_feature) return api.invalid("NULL semantic_feature");
+    if (C > 0 && !semantic_feature && !optional) return api.invalid("NULL semantic_feature");
     feat = {C > 0 ? semantic_feature : nullptr, semantic_feature_dtype == F3DGS_F16};
     return 0;
 }
@@ -798,6 +856,68 @@ int f3dgs_backward_accum_feature_geometry(
                                    dL_dmean3D, dL_dcov3D_precomp, dL_dsh, dL_dscale, dL_drot, dL_dmean2D_out,
                                    grad_accum, denom, composite_done_event, debug, cuda_stream, false, dL_dcamera,
                                    feat);
+    };
+    if (dL_dfeaturepix_dtype == F3DGS_F16)
+        return run(static_cast<const __half*>(dL_dfeaturepix), dL_dfeaturepix_scale);
+    return run(static_cast<const float*>(dL_dfeaturepix), 1.f);
+}
+
+int f3dgs_backward_antialiased(int P, int D, int M, int R, int C, const float* background, int width, int height,
+                               const float* means3D, const float* shs, const float* colors_precomp,
+                               const void* semantic_feature, int semantic_feature_dtype, const float* scales,
+                               float scale_modifier, const float* rotations, const float* cov3D_precomp,
+                               const float* viewmatrix, const float* projmatrix, const float* cam_pos, float tan_fovx,
+                               float tan_fovy, const int* radii, char* geom_buffer, char* binning_buffer,
+                               char* image_buffer, const float* dL_dpix, const void* dL_dfeaturepix,
+                               int dL_dfeaturepix_dtype, float dL_dfeaturepix_scale, const float* dL_depths,
+                               float* dL_dmean2D, float* dL_dconic, float* dL_dopacity, float* dL_dcolor,
+                               float* dL_dsemantic_feature, float* dL_dmean3D, float* dL_dcov3D, float* dL_dsh,
+                               float* dL_dscale, float* dL_drot, float* dL_dz, int debug, void* cuda_stream,
+                               float* dL_dcamera) {
+    (void)colors_precomp;
+    const Api api(__func__);
+    FeatureRows feat;
+    if (const int rc =
+            feature_rows(api, C, semantic_feature, semantic_feature_dtype, dL_dfeaturepix_dtype, feat, true))
+        return rc;
+    const auto run = [&](auto map, float scale) {
+        return backward_impl(api, false, P, D, M, R, C, background, width, height, means3D, shs, scales,
+                             scale_modifier, rotations, cov3D_precomp, viewmatrix, projmatrix, cam_pos, tan_fovx,
+                             tan_fovy, radii, geom_buffer, binning_buffer, image_buffer, dL_dpix, map, scale, dL_depths,
+                             dL_dmean2D, dL_dconic, dL_dopacity, dL_dcolor, dL_dsemantic_feature, dL_dmean3D, dL_dcov3D,
+                             dL_dsh, dL_dscale, dL_drot, dL_dz, nullptr, nullptr, dL_dcamera, nullptr, debug,
+                             (cudaStream_t)cuda_stream, {nullptr, 0}, feat, true);
+    };
+    if (dL_dfeaturepix_dtype == F3DGS_F16)
+        return run(static_cast<const __half*>(dL_dfeaturepix), dL_dfeaturepix_scale);
+    return run(static_cast<const float*>(dL_dfeaturepix), 1.f);
+}
+
+int f3dgs_backward_accum_antialiased(
+    int P, int D, int M, int R, int C, const float* background, int width, int height, const float* means3D,
+    const float* shs, const float* colors_precomp, const void* semantic_feature, int semantic_feature_dtype,
+    const float* scales, float scale_modifier, const float* rotations, const float* cov3D_precomp,
+    const float* viewmatrix, const float* projmatrix, const float* cam_pos, float tan_fovx, float tan_fovy,
+    const int* radii, char* geom_buffer, char* binning_buffer, char* image_buffer, const float* dL_dpix,
+    const void* dL_dfeaturepix, int dL_dfeaturepix_dtype, float dL_dfeaturepix_scale, const float* dL_depths,
+    char* scratch, float* dL_dopacity, float* dL_dcolors_precomp, float* dL_dsemantic_feature, float* dL_dmean3D,
+    float* dL_dcov3D_precomp, float* dL_dsh, float* dL_dscale, float* dL_drot, float* dL_dmean2D_out,
+    float* grad_accum, float* denom, void* composite_done_event, int debug, void* cuda_stream, float* dL_dcamera) {
+    const char* entry = __func__;
+    FeatureRows feat;
+    if (const int rc = feature_rows(Api(entry), C, semantic_feature, semantic_feature_dtype, dL_dfeaturepix_dtype,
+                                    feat, true))
+        return rc;
+    if (P > 0 && overlaps({dL_dopacity, (size_t)P * 4}, {{dL_dmean2D_out, (size_t)P * 3 * 4}}))
+        return Api(entry).invalid("dL_dopacity overlaps another output");
+    const auto run = [&](auto map, float scale) {
+        return backward_accum_impl(entry, P, D, M, R, C, background, width, height, means3D, shs, colors_precomp,
+                                   scales, scale_modifier, rotations, cov3D_precomp, viewmatrix, projmatrix, cam_pos,
+                                   tan_fovx, tan_fovy, radii, geom_buffer, binning_buffer, image_buffer, dL_dpix, map,
+                                   scale, dL_depths, scratch, dL_dopacity, dL_dcolors_precomp, dL_dsemantic_feature,
+                                   dL_dmean3D, dL_dcov3D_precomp, dL_dsh, dL_dscale, dL_drot, dL_dmean2D_out,
+                                   grad_accum, denom, composite_done_event, debug, cuda_stream, false, dL_dcamera,
+                                   feat, true);
     };
     if (dL_dfeaturepix_dtype == F3DGS_F16)
         return run(static_cast<const __half*>(dL_dfeaturepix), dL_dfeaturepix_scale);

@@ -29,17 +29,21 @@ void launch_preprocess_fwd(const ViewParams& vp, const float* means3D, const flo
                            const float* rotations, const float* opacities, const float* shs,
                            const float* cov3D_precomp, const float* colors_precomp, bool prefiltered,
                            int* radii, SplatRec* rec, float* cov3D, uint8_t* clamped,
-                           uint32_t* tiles_touched, cudaStream_t s);
+                           uint32_t* tiles_touched, cudaStream_t s, bool antialiasing = false);
 
 // dL_dcamera (optional, 35 floats: dL/dviewmatrix [16], dL/dprojmatrix [16], dL/dcampos [3]) is ADDED to.  Its
 // float64 block partials come from the default memory pool: cudaErrorMemoryAllocation if that fails.
+// antialiasing: the backward of an antialiased forward, whose records `rec` hold op_eff = opacity * rho.  dL_dop_eff
+// [P] is the composite's dL/dop_eff; dL_dopacity gets rho * dL_dop_eff (assigned, or added with `accumulate`).  In the
+// assigning backward the two may be one buffer, rescaled in place.
 cudaError_t launch_preprocess_bwd(const ViewParams& vp, const float* means3D, const int* radii, const float* shs,
                                   const uint8_t* clamped, const float* scales, const float* rotations,
                                   const float* cov3D, const float* dL_dmean2D, const float* dL_dconic,
                                   float* dL_dmean3D, const float* dL_dcolor, float* dL_dcov3D, float* dL_dsh,
                                   float* dL_dscale, float* dL_drot, const float* dL_dz, cudaStream_t s,
                                   bool accumulate = false, float* grad_accum = nullptr, float* denom = nullptr,
-                                  float* dL_dcamera = nullptr);
+                                  float* dL_dcamera = nullptr, bool antialiasing = false, const SplatRec* rec = nullptr,
+                                  const float* dL_dop_eff = nullptr, float* dL_dopacity = nullptr);
 
 void launch_mark_visible(int P, const float* means3D, const float* viewmatrix, uint8_t* present,
                          cudaStream_t s);

@@ -124,9 +124,11 @@ __device__ __forceinline__ void cov3d_from_scale_rot(const float* __restrict__ s
 }
 
 // EWA projection of the 3-D covariance, reference forward.cu:75-114.  Returns (a, b, c) with the
-// 0.3 dilation applied.  Also hands back the intermediates the backward needs.
+// 0.3 dilation applied, and the undilated diagonal (a0, c0) for antialiasing.  Also hands back the intermediates the
+// backward needs.
 struct Cov2D {
     float a, b, c;
+    float a0, c0;
     float T00, T01, T02, T10, T11, T12;  // T[0][*], T[1][*] of T = W * J (column-major indexing)
     float tx, ty, tz;                    // clamped view-space mean
     float txtz, tytz;                    // unclamped ratios
@@ -147,6 +149,7 @@ __device__ __forceinline__ Cov2D project_cov(F3 mean, const float* __restrict__ 
     const M3 T = Wm * J;
     const M3 Vrk = cols(cv[0], cv[1], cv[2], cv[1], cv[3], cv[4], cv[2], cv[4], cv[5]);
     M3 cov = transpose(T) * transpose(Vrk) * T;
+    o.a0 = cov.c[0][0]; o.c0 = cov.c[1][1];
     cov.c[0][0] += 0.3f;
     cov.c[1][1] += 0.3f;
     o.a = cov.c[0][0]; o.b = cov.c[0][1]; o.c = cov.c[1][1];
@@ -175,10 +178,22 @@ __device__ __forceinline__ void alpha_extent(float A, float B, float C, float op
     ey = sqrtf(tau * A / det) + 0.01f;
 }
 
+// Antialiasing (AA = true): the 0.3 px^2 dilation widens a Gaussian without conserving its integral, so the opacity is
+// scaled by rho = sqrt(max(kAaMinRatio, det0 / det)), det0 = a0 c0 - b^2 of the undilated and det = a c - b^2 of the
+// dilated 2-D covariance; the dilated splat then carries the undilated one's integral.  The ratio is formed from opaque
+// copies of its inputs, so that sharing a product with `det` cannot change how the compiler contracts the default
+// path's arithmetic: conic, radius and everything else keep the bits of AA = false.
+constexpr float kAaMinRatio = 2.5e-5f;
+__device__ __forceinline__ float aa_det0(float a0, float b, float c0) {
+    asm("" : "+f"(a0), "+f"(b), "+f"(c0));
+    return a0 * c0 - b * b;
+}
+
 // shared-memory staging of SH rows (both preprocess kernels)
 constexpr int kBwdBlock = 128;
 __host__ __device__ constexpr int bwd_row_stride(int row_floats) { return row_floats | 1; }  // odd stride: no bank conflicts
 
+template <bool AA>
 __global__ void __launch_bounds__(256)
 preprocess_fwd_kernel(ViewParams vp, const float* __restrict__ means3D, const float* __restrict__ scales,
                       const float* __restrict__ rotations, const float* __restrict__ opacities,
@@ -264,6 +279,7 @@ preprocess_fwd_kernel(ViewParams vp, const float* __restrict__ means3D, const fl
         r.x = ix; r.y = iy;
         r.ca = conA; r.cb = conB; r.cc = conC;
         r.op = opacities[idx];
+        if constexpr (AA) r.op *= sqrtf(fmaxf(kAaMinRatio, aa_det0(c2.a0, c2.b, c2.c0) / det));
         r.depth = depth;
 #ifdef F3DGS_SASS_AUDIT  // build used only to compare the FP instruction mix with the reference kernel
         r.ex = r.ey = 0.f;
@@ -301,6 +317,93 @@ __device__ __forceinline__ F3 dnormvdv3(F3 v, F3 dv) {  // reference auxiliary.h
     return o;
 }
 
+// SH backward of one Gaussian (reference backward.cu:20-139): writes the coefficient gradients dsh (dRGB: the colour
+// gradient, 0 on clamped channels) for the unit view direction (x, y, z) and returns dL/d(x, y, z).
+__device__ __forceinline__ F3 sh_dir_grad(int deg, const float* sh, float* dsh, const float (&dRGB)[3], float x, float y,
+                                          float z) {
+    float ddx = 0.f, ddy = 0.f, ddz = 0.f;  // dL/ddir
+#define SHC(k, c) sh[3 * (k) + (c)]
+#define WR(k, coef)                                                  \
+    do {                                                             \
+    const float cf_ = (coef);                                    \
+    dsh[3 * (k)] = cf_ * dRGB[0];                                \
+    dsh[3 * (k) + 1] = cf_ * dRGB[1];                            \
+    dsh[3 * (k) + 2] = cf_ * dRGB[2];                            \
+    } while (0)
+    WR(0, kSH_C0);
+    if (deg > 0) {
+        WR(1, -kSH_C1 * y);
+        WR(2, kSH_C1 * z);
+        WR(3, -kSH_C1 * x);
+        float dx_[3], dy_[3], dz_[3];
+#pragma unroll
+        for (int ch = 0; ch < 3; ch++) {
+            dx_[ch] = -kSH_C1 * SHC(3, ch);
+            dy_[ch] = -kSH_C1 * SHC(1, ch);
+            dz_[ch] = kSH_C1 * SHC(2, ch);
+        }
+        if (deg > 1) {
+            const float xx = x * x, yy = y * y, zz = z * z;
+            const float xy = x * y, yz = y * z, xz = x * z;
+            WR(4, kSH_C2[0] * xy);
+            WR(5, kSH_C2[1] * yz);
+            WR(6, kSH_C2[2] * (2.f * zz - xx - yy));
+            WR(7, kSH_C2[3] * xz);
+            WR(8, kSH_C2[4] * (xx - yy));
+#pragma unroll
+            for (int ch = 0; ch < 3; ch++) {
+                dx_[ch] += kSH_C2[0] * y * SHC(4, ch) + kSH_C2[2] * 2.f * -x * SHC(6, ch) +
+                           kSH_C2[3] * z * SHC(7, ch) + kSH_C2[4] * 2.f * x * SHC(8, ch);
+                dy_[ch] += kSH_C2[0] * x * SHC(4, ch) + kSH_C2[1] * z * SHC(5, ch) +
+                           kSH_C2[2] * 2.f * -y * SHC(6, ch) + kSH_C2[4] * 2.f * -y * SHC(8, ch);
+                dz_[ch] += kSH_C2[1] * y * SHC(5, ch) + kSH_C2[2] * 2.f * 2.f * z * SHC(6, ch) +
+                           kSH_C2[3] * x * SHC(7, ch);
+            }
+            if (deg > 2) {
+                WR(9, kSH_C3[0] * y * (3.f * xx - yy));
+                WR(10, kSH_C3[1] * xy * z);
+                WR(11, kSH_C3[2] * y * (4.f * zz - xx - yy));
+                WR(12, kSH_C3[3] * z * (2.f * zz - 3.f * xx - 3.f * yy));
+                WR(13, kSH_C3[4] * x * (4.f * zz - xx - yy));
+                WR(14, kSH_C3[5] * z * (xx - yy));
+                WR(15, kSH_C3[6] * x * (xx - 3.f * yy));
+#pragma unroll
+                for (int ch = 0; ch < 3; ch++) {
+                    dx_[ch] += (kSH_C3[0] * SHC(9, ch) * 3.f * 2.f * xy + kSH_C3[1] * SHC(10, ch) * yz +
+                                kSH_C3[2] * SHC(11, ch) * -2.f * xy + kSH_C3[3] * SHC(12, ch) * -3.f * 2.f * xz +
+                                kSH_C3[4] * SHC(13, ch) * (-3.f * xx + 4.f * zz - yy) +
+                                kSH_C3[5] * SHC(14, ch) * 2.f * xz + kSH_C3[6] * SHC(15, ch) * 3.f * (xx - yy));
+                    dy_[ch] += (kSH_C3[0] * SHC(9, ch) * 3.f * (xx - yy) + kSH_C3[1] * SHC(10, ch) * xz +
+                                kSH_C3[2] * SHC(11, ch) * (-3.f * yy + 4.f * zz - xx) +
+                                kSH_C3[3] * SHC(12, ch) * -3.f * 2.f * yz + kSH_C3[4] * SHC(13, ch) * -2.f * xy +
+                                kSH_C3[5] * SHC(14, ch) * -2.f * yz + kSH_C3[6] * SHC(15, ch) * -3.f * 2.f * xy);
+                    dz_[ch] += (kSH_C3[1] * SHC(10, ch) * xy + kSH_C3[2] * SHC(11, ch) * 4.f * 2.f * yz +
+                                kSH_C3[3] * SHC(12, ch) * 3.f * (2.f * zz - xx - yy) +
+                                kSH_C3[4] * SHC(13, ch) * 4.f * 2.f * xz + kSH_C3[5] * SHC(14, ch) * (xx - yy));
+                }
+            }
+        }
+        ddx = dx_[0] * dRGB[0] + dx_[1] * dRGB[1] + dx_[2] * dRGB[2];
+        ddy = dy_[0] * dRGB[0] + dy_[1] * dRGB[1] + dy_[2] * dRGB[2];
+        ddz = dz_[0] * dRGB[0] + dz_[1] * dRGB[1] + dz_[2] * dRGB[2];
+    }
+#undef SHC
+#undef WR
+    return F3{ddx, ddy, ddz};
+}
+
+// The antialiased kernels run the SH backward out of line.  Inlined, ptxas fuses its multiplies and adds differently
+// in each instantiation, so dL_dsh and dL_dmean3D of the camera and accumulating twins would differ in the last bit;
+// one compiled body gives every twin the same bits.  -> dL/dmean through the view direction; *dd = dL/ddir.  (The
+// default kernels keep the inline code, whose instructions their twins already share.)
+__device__ __noinline__ F3 sh_backward_out_of_line(int deg, const float* sh, float* dsh, float r, float g, float b,
+                                                   F3 dir_orig, F3* dd) {
+    const float inv_len = 1.0f / sqrtf(dir_orig.x * dir_orig.x + dir_orig.y * dir_orig.y + dir_orig.z * dir_orig.z);
+    const float dRGB[3] = {r, g, b};
+    *dd = sh_dir_grad(deg, sh, dsh, dRGB, dir_orig.x * inv_len, dir_orig.y * inv_len, dir_orig.z * inv_len);
+    return dnormvdv3(dir_orig, *dd);
+}
+
 // ACCUM = false: the reference's contract -- gradients are ASSIGNED (backward.cu:273, :217-232, :48-97, :323-340) into
 // zero-filled buffers.  ACCUM = true (view batches, f3dgs_backward_accum): every per-parameter gradient is ADDED to what
 // is already there (each Gaussian is written by exactly one thread: plain read-modify-write, no atomics), and the
@@ -328,7 +431,12 @@ __host__ __device__ constexpr int cam_slot(int j) {  // slot -> index in the 35-
                   : j < 24 ? 16 + 4 * ((j - 12) / 3) + ((j - 12) % 3 == 2 ? 3 : (j - 12) % 3) : 32 + (j - 24);
 }
 
-template <bool ACCUM, bool CAM>
+// AA = true: the backward of the antialiased forward.  The composite's opacity gradient g = dL/dop_eff is read from
+// dL_dop_eff; dL_dopacity gets rho g (assigned or added, as every other gradient), and rho's dependence on the 2-D
+// covariance joins dL/d(a, b, c), from where it reaches cov3D, scale, rotation, the mean and the camera.  op_eff is the
+// splat record's op.  dL_dop_eff may be dL_dopacity itself (the assigning backward rescales in place): the two are read
+// and written by the same thread, so neither is __restrict__.
+template <bool ACCUM, bool CAM, bool AA>
 __global__ void __launch_bounds__(kBwdBlock)
 preprocess_bwd_kernel(ViewParams vp, const float* __restrict__ means3D, const int* __restrict__ radii,
                       const float* __restrict__ shs, const uint8_t* __restrict__ clamped,
@@ -338,7 +446,8 @@ preprocess_bwd_kernel(ViewParams vp, const float* __restrict__ means3D, const in
                       const float* __restrict__ dL_dcolor, float* __restrict__ dL_dcov3D,
                       float* __restrict__ dL_dsh, float* __restrict__ dL_dscale, float* __restrict__ dL_drot,
                       const float* __restrict__ dL_dz, float* __restrict__ grad_accum, float* __restrict__ vis_count,
-                      double* __restrict__ cam_part) {
+                      double* __restrict__ cam_part, const SplatRec* __restrict__ rec, const float* dL_dop_eff,
+                      float* dL_dopacity) {
     extern __shared__ float bwd_smem[];
     const int idx = blockIdx.x * blockDim.x + threadIdx.x;
     const int row_floats = vp.M * 3, stride = bwd_row_stride(row_floats);
@@ -395,11 +504,29 @@ preprocess_bwd_kernel(ViewParams vp, const float* __restrict__ means3D, const in
     const float denom2inv = 1.0f / ((denom * denom) + 0.0000001f);
     float dL_da = 0, dL_db = 0, dL_dc = 0;
     const float T00 = c2.T00, T01 = c2.T01, T02 = c2.T02, T10 = c2.T10, T11 = c2.T11, T12 = c2.T12;
+    // AA: h = op_eff g / 2 where rho is not clamped.  Where it is (det0 / det <= kAaMinRatio, a degenerate undilated
+    // covariance among them: det0 = 0 makes 1 / det0 infinite), rho is constant and nothing is added
+    float aa_h = 0.f, det0 = 0.f;
+    bool aa_terms = false;
+    if constexpr (AA) {
+        const float g = dL_dop_eff[idx];
+        det0 = aa_det0(c2.a0, b, c2.c0);
+        const float ratio = det0 / denom;
+        put<ACCUM>(dL_dopacity + idx, sqrtf(fmaxf(kAaMinRatio, ratio)) * g);
+        aa_terms = ratio > kAaMinRatio;
+        if (aa_terms) aa_h = 0.5f * rec[idx].op * g;
+    }
     float dcov[6];
     if (denom2inv != 0) {
         dL_da = denom2inv * (-c * c * dLcx + 2 * b * c * dLcy + (denom - a * c) * dLcz);
         dL_dc = denom2inv * (-a * a * dLcz + 2 * a * b * dLcy + (denom - a * c) * dLcx);
         dL_db = denom2inv * 2 * (b * c * dLcx - (denom + 2 * b * b) * dLcy + a * b * dLcz);
+        if (AA && aa_terms) {
+            // d log rho = (d det0 / det0 - d det / det) / 2, det0 = (a - 0.3)(c - 0.3) - b^2, det = a c - b^2
+            dL_da += aa_h * (c2.c0 / det0 - c / denom);
+            dL_dc += aa_h * (c2.a0 / det0 - a / denom);
+            dL_db += 2.f * aa_h * b * (1.f / denom - 1.f / det0);
+        }
         dcov[0] = (T00 * T00 * dL_da + T00 * T10 * dL_db + T10 * T10 * dL_dc);
         dcov[3] = (T01 * T01 * dL_da + T01 * T11 * dL_db + T11 * T11 * dL_dc);
         dcov[5] = (T02 * T02 * dL_da + T02 * T12 * dL_db + T12 * T12 * dL_dc);
@@ -447,13 +574,21 @@ preprocess_bwd_kernel(ViewParams vp, const float* __restrict__ means3D, const in
         // t_r = xf(vm, r, p) gives dL/dvm[4k + r] = dL/dt_r p_k; T.c[a][k] = sum_r vm[4k + r] J.c[a][r] gives the W term
         // (J.c[0] = (fx/tz, 0, -fx tx/tz^2), J.c[1] = (0, fy/tz, -fy ty/tz^2), J.c[2] = 0)
         const float p[4] = {mx, my, mz, 1.f};
-        const float dT0[3] = {dL_dT00, dL_dT01, dL_dT02}, dT1[3] = {dL_dT10, dL_dT11, dL_dT12};
-        const float J00 = h_x * tz, J11 = h_y * tz, J02 = -h_x * c2.tx * tz2, J12 = -h_y * c2.ty * tz2;
+        float dT0[3] = {dL_dT00, dL_dT01, dL_dT02}, dT1[3] = {dL_dT10, dL_dT11, dL_dT12};
+        float gtx = dL_dtx, gty = dL_dty, gtz = dL_dtz;
+        float fx = h_x, fy = h_y, itz = tz, itz2 = tz2, ctx = c2.tx, cty = c2.ty;
+        if constexpr (AA) {
+            // as for the campos term below: the camera terms read opaque copies, so that a second use of these values
+            // cannot change how the compiler contracts the other outputs of the antialiased kernels
+            asm("" : "+f"(dT0[0]), "+f"(dT0[1]), "+f"(dT0[2]), "+f"(dT1[0]), "+f"(dT1[1]), "+f"(dT1[2]));
+            asm("" : "+f"(gtx), "+f"(gty), "+f"(gtz), "+f"(fx), "+f"(fy), "+f"(itz), "+f"(itz2), "+f"(ctx), "+f"(cty));
+        }
+        const float J00 = fx * itz, J11 = fy * itz, J02 = -fx * ctx * itz2, J12 = -fy * cty * itz2;
 #pragma unroll
         for (int k = 0; k < 4; k++) {
-            cg[3 * k] = dL_dtx * p[k];
-            cg[3 * k + 1] = dL_dty * p[k];
-            cg[3 * k + 2] = dL_dtz * p[k];
+            cg[3 * k] = gtx * p[k];
+            cg[3 * k + 1] = gty * p[k];
+            cg[3 * k + 2] = gtz * p[k];
             if (k < 3) {
                 cg[3 * k] += dT0[k] * J00;
                 cg[3 * k + 1] += dT1[k] * J11;
@@ -481,10 +616,12 @@ preprocess_bwd_kernel(ViewParams vp, const float* __restrict__ means3D, const in
             // proj = (h_0, h_1) m_w with h_r = xf(pm, r, p): dL/dh_0 = m_w d2x, dL/dh_1 = m_w d2y,
             // dL/dh_3 = -(mul1 d2x + mul2 d2y); depth = xf(vm, 2, p)
             const float p[4] = {mx, my, mz, 1.f};
-            const float gh[3] = {m_w * d2x, m_w * d2y, -(mul1 * d2x + mul2 * d2y)};
+            float w = m_w, gx2 = d2x, gy2 = d2y, u1 = mul1, u2 = mul2, gdz = dldz;
+            if constexpr (AA) asm("" : "+f"(w), "+f"(gx2), "+f"(gy2), "+f"(u1), "+f"(u2), "+f"(gdz));  // as above
+            const float gh[3] = {w * gx2, w * gy2, -(u1 * gx2 + u2 * gy2)};
 #pragma unroll
             for (int k = 0; k < 4; k++) {
-                cg[3 * k + 2] += dldz * p[k];
+                cg[3 * k + 2] += gdz * p[k];
 #pragma unroll
                 for (int i = 0; i < 3; i++) cg[12 + 3 * k + i] = gh[i] * p[k];
             }
@@ -504,85 +641,26 @@ preprocess_bwd_kernel(ViewParams vp, const float* __restrict__ means3D, const in
         dRGB[0] = (cb & 1) ? 0.f : dL_dcolor[3 * idx];
         dRGB[1] = (cb & 2) ? 0.f : dL_dcolor[3 * idx + 1];
         dRGB[2] = (cb & 4) ? 0.f : dL_dcolor[3 * idx + 2];
-        float ddx = 0.f, ddy = 0.f, ddz = 0.f;  // dL/ddir
-        const int deg = vp.D;
-#define SHC(k, c) sh[3 * (k) + (c)]
-#define WR(k, coef)                                                  \
-    do {                                                             \
-        const float cf_ = (coef);                                    \
-        dsh[3 * (k)] = cf_ * dRGB[0];                                \
-        dsh[3 * (k) + 1] = cf_ * dRGB[1];                            \
-        dsh[3 * (k) + 2] = cf_ * dRGB[2];                            \
-    } while (0)
-        WR(0, kSH_C0);
-        if (deg > 0) {
-            WR(1, -kSH_C1 * y);
-            WR(2, kSH_C1 * z);
-            WR(3, -kSH_C1 * x);
-            float dx_[3], dy_[3], dz_[3];
-#pragma unroll
-            for (int ch = 0; ch < 3; ch++) {
-                dx_[ch] = -kSH_C1 * SHC(3, ch);
-                dy_[ch] = -kSH_C1 * SHC(1, ch);
-                dz_[ch] = kSH_C1 * SHC(2, ch);
-            }
-            if (deg > 1) {
-                const float xx = x * x, yy = y * y, zz = z * z;
-                const float xy = x * y, yz = y * z, xz = x * z;
-                WR(4, kSH_C2[0] * xy);
-                WR(5, kSH_C2[1] * yz);
-                WR(6, kSH_C2[2] * (2.f * zz - xx - yy));
-                WR(7, kSH_C2[3] * xz);
-                WR(8, kSH_C2[4] * (xx - yy));
-#pragma unroll
-                for (int ch = 0; ch < 3; ch++) {
-                    dx_[ch] += kSH_C2[0] * y * SHC(4, ch) + kSH_C2[2] * 2.f * -x * SHC(6, ch) +
-                               kSH_C2[3] * z * SHC(7, ch) + kSH_C2[4] * 2.f * x * SHC(8, ch);
-                    dy_[ch] += kSH_C2[0] * x * SHC(4, ch) + kSH_C2[1] * z * SHC(5, ch) +
-                               kSH_C2[2] * 2.f * -y * SHC(6, ch) + kSH_C2[4] * 2.f * -y * SHC(8, ch);
-                    dz_[ch] += kSH_C2[1] * y * SHC(5, ch) + kSH_C2[2] * 2.f * 2.f * z * SHC(6, ch) +
-                               kSH_C2[3] * x * SHC(7, ch);
-                }
-                if (deg > 2) {
-                    WR(9, kSH_C3[0] * y * (3.f * xx - yy));
-                    WR(10, kSH_C3[1] * xy * z);
-                    WR(11, kSH_C3[2] * y * (4.f * zz - xx - yy));
-                    WR(12, kSH_C3[3] * z * (2.f * zz - 3.f * xx - 3.f * yy));
-                    WR(13, kSH_C3[4] * x * (4.f * zz - xx - yy));
-                    WR(14, kSH_C3[5] * z * (xx - yy));
-                    WR(15, kSH_C3[6] * x * (xx - 3.f * yy));
-#pragma unroll
-                    for (int ch = 0; ch < 3; ch++) {
-                        dx_[ch] += (kSH_C3[0] * SHC(9, ch) * 3.f * 2.f * xy + kSH_C3[1] * SHC(10, ch) * yz +
-                                    kSH_C3[2] * SHC(11, ch) * -2.f * xy + kSH_C3[3] * SHC(12, ch) * -3.f * 2.f * xz +
-                                    kSH_C3[4] * SHC(13, ch) * (-3.f * xx + 4.f * zz - yy) +
-                                    kSH_C3[5] * SHC(14, ch) * 2.f * xz + kSH_C3[6] * SHC(15, ch) * 3.f * (xx - yy));
-                        dy_[ch] += (kSH_C3[0] * SHC(9, ch) * 3.f * (xx - yy) + kSH_C3[1] * SHC(10, ch) * xz +
-                                    kSH_C3[2] * SHC(11, ch) * (-3.f * yy + 4.f * zz - xx) +
-                                    kSH_C3[3] * SHC(12, ch) * -3.f * 2.f * yz + kSH_C3[4] * SHC(13, ch) * -2.f * xy +
-                                    kSH_C3[5] * SHC(14, ch) * -2.f * yz + kSH_C3[6] * SHC(15, ch) * -3.f * 2.f * xy);
-                        dz_[ch] += (kSH_C3[1] * SHC(10, ch) * xy + kSH_C3[2] * SHC(11, ch) * 4.f * 2.f * yz +
-                                    kSH_C3[3] * SHC(12, ch) * 3.f * (2.f * zz - xx - yy) +
-                                    kSH_C3[4] * SHC(13, ch) * 4.f * 2.f * xz + kSH_C3[5] * SHC(14, ch) * (xx - yy));
-                    }
-                }
-            }
-            ddx = dx_[0] * dRGB[0] + dx_[1] * dRGB[1] + dx_[2] * dRGB[2];
-            ddy = dy_[0] * dRGB[0] + dy_[1] * dRGB[1] + dy_[2] * dRGB[2];
-            ddz = dz_[0] * dRGB[0] + dz_[1] * dRGB[1] + dz_[2] * dRGB[2];
+        F3 dd, dm;
+        if constexpr (AA) {
+            dm = sh_backward_out_of_line(vp.D, sh, dsh, dRGB[0], dRGB[1], dRGB[2], dir_orig, &dd);
+        } else {
+            dd = sh_dir_grad(vp.D, sh, dsh, dRGB, x, y, z);
+            dm = dnormvdv3(dir_orig, dd);
         }
-#undef SHC
-#undef WR
-        const F3 dm = dnormvdv3(dir_orig, F3{ddx, ddy, ddz});
         gx += dm.x; gy += dm.y; gz += dm.z;
         if constexpr (CAM) {
             // dir_orig = p - campos: dL/dcampos = -dm.  dm is recomputed from opaque copies of its inputs rather than
             // read: a second use of dm's products would change how the compiler contracts `gx += dm.x` into FMAs, and
             // so the bits of dL_dmean3D, which must equal those of the CAM = false kernel.
-            F3 v = dir_orig, dv = F3{ddx, ddy, ddz};
-            asm("" : "+f"(v.x), "+f"(v.y), "+f"(v.z), "+f"(dv.x), "+f"(dv.y), "+f"(dv.z));
-            const F3 dmc = dnormvdv3(v, dv);
-            cg[24] = -dmc.x; cg[25] = -dmc.y; cg[26] = -dmc.z;
+            if constexpr (AA) {  // dm comes from the out-of-line call: a second use cannot change its bits
+                cg[24] = -dm.x; cg[25] = -dm.y; cg[26] = -dm.z;
+            } else {
+                F3 v = dir_orig, dv = dd;
+                asm("" : "+f"(v.x), "+f"(v.y), "+f"(v.z), "+f"(dv.x), "+f"(dv.y), "+f"(dv.z));
+                const F3 dmc = dnormvdv3(v, dv);
+                cg[24] = -dmc.x; cg[25] = -dmc.y; cg[26] = -dmc.z;
+            }
         }
     }
     put<ACCUM>(dL_dmean3D + 3 * idx, gx);
@@ -716,13 +794,14 @@ void launch_preprocess_fwd(const ViewParams& vp, const float* means3D, const flo
                            const float* rotations, const float* opacities, const float* shs,
                            const float* cov3D_precomp, const float* colors_precomp, bool prefiltered,
                            int* radii, SplatRec* rec, float* cov3D, uint8_t* clamped,
-                           uint32_t* tiles_touched, cudaStream_t s) {
+                           uint32_t* tiles_touched, cudaStream_t s, bool antialiasing) {
     if (vp.P <= 0) return;
     constexpr int kFwdBlock = 128;
     const size_t smem = shs ? (size_t)kFwdBlock * bwd_row_stride(vp.M * 3) * sizeof(float) : 0;
-    preprocess_fwd_kernel<<<(vp.P + kFwdBlock - 1) / kFwdBlock, kFwdBlock, smem, s>>>(vp, means3D, scales, rotations, opacities, shs,
-                                                           cov3D_precomp, colors_precomp, prefiltered, radii,
-                                                           rec, cov3D, clamped, tiles_touched);
+    const auto kernel = antialiasing ? preprocess_fwd_kernel<true> : preprocess_fwd_kernel<false>;
+    kernel<<<(vp.P + kFwdBlock - 1) / kFwdBlock, kFwdBlock, smem, s>>>(vp, means3D, scales, rotations, opacities, shs,
+                                                                       cov3D_precomp, colors_precomp, prefiltered, radii,
+                                                                       rec, cov3D, clamped, tiles_touched);
     g_launches++;
 }
 
@@ -731,46 +810,42 @@ cudaError_t launch_preprocess_bwd(const ViewParams& vp, const float* means3D, co
                                   const float* cov3D, const float* dL_dmean2D, const float* dL_dconic,
                                   float* dL_dmean3D, const float* dL_dcolor, float* dL_dcov3D, float* dL_dsh,
                                   float* dL_dscale, float* dL_drot, const float* dL_dz, cudaStream_t s, bool accumulate,
-                                  float* grad_accum, float* denom, float* dL_dcamera) {
+                                  float* grad_accum, float* denom, float* dL_dcamera, bool antialiasing,
+                                  const SplatRec* rec, const float* dL_dop_eff, float* dL_dopacity) {
     if (vp.P <= 0) return cudaSuccess;
+    using Kernel = decltype(&preprocess_bwd_kernel<false, false, false>);
+    // [accumulate][camera][antialiasing]
+    static const Kernel kernels[2][2][2] = {
+        {{preprocess_bwd_kernel<false, false, false>, preprocess_bwd_kernel<false, false, true>},
+         {preprocess_bwd_kernel<false, true, false>, preprocess_bwd_kernel<false, true, true>}},
+        {{preprocess_bwd_kernel<true, false, false>, preprocess_bwd_kernel<true, false, true>},
+         {preprocess_bwd_kernel<true, true, false>, preprocess_bwd_kernel<true, true, true>}}};
     const size_t smem = shs ? (size_t)2 * kBwdBlock * bwd_row_stride(vp.M * 3) * sizeof(float) + kBwdBlock : 0;
     static std::atomic<int> attr_set{0};
     int dev = 0;
     cudaGetDevice(&dev);
     if (smem > 48 * 1024 && !((attr_set.load() >> (dev & 31)) & 1)) {  // once per device; harmless if repeated
-        cudaFuncSetAttribute(preprocess_bwd_kernel<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024);
-        cudaFuncSetAttribute(preprocess_bwd_kernel<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024);
-        cudaFuncSetAttribute(preprocess_bwd_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024);
-        cudaFuncSetAttribute(preprocess_bwd_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024);
+        for (const Kernel k : {kernels[0][0][0], kernels[0][0][1], kernels[0][1][0], kernels[0][1][1], kernels[1][0][0],
+                               kernels[1][0][1], kernels[1][1][0], kernels[1][1][1]})
+            cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024);
         attr_set.fetch_or(1 << (dev & 31));
     }
     const int grid = (vp.P + kBwdBlock - 1) / kBwdBlock;
-    if (dL_dcamera == nullptr) {
-        if (accumulate)
-            preprocess_bwd_kernel<true, false><<<grid, kBwdBlock, smem, s>>>(
-                vp, means3D, radii, shs, clamped, scales, rotations, cov3D, dL_dmean2D, dL_dconic, dL_dmean3D,
-                dL_dcolor, dL_dcov3D, dL_dsh, dL_dscale, dL_drot, dL_dz, grad_accum, denom, nullptr);
-        else
-            preprocess_bwd_kernel<false, false><<<grid, kBwdBlock, smem, s>>>(
-                vp, means3D, radii, shs, clamped, scales, rotations, cov3D, dL_dmean2D, dL_dconic, dL_dmean3D,
-                dL_dcolor, dL_dcov3D, dL_dsh, dL_dscale, dL_drot, dL_dz, nullptr, nullptr, nullptr);
-        g_launches++;
-        return cudaSuccess;  // a launch error is left for the caller's cudaGetLastError
-    }
-    // the block partials come from the device's default memory pool, stream-ordered like the launches
+    const bool cam = dL_dcamera != nullptr;
+    // the camera gradient's block partials come from the device's default memory pool, stream-ordered like the launches
     double* part = nullptr;
-    cudaError_t e = cudaMallocAsync((void**)&part, (size_t)grid * kCamTerms * sizeof(double), s);
-    if (e != cudaSuccess) return e;
-    if (accumulate)
-        preprocess_bwd_kernel<true, true><<<grid, kBwdBlock, smem, s>>>(
-            vp, means3D, radii, shs, clamped, scales, rotations, cov3D, dL_dmean2D, dL_dconic, dL_dmean3D, dL_dcolor,
-            dL_dcov3D, dL_dsh, dL_dscale, dL_drot, dL_dz, grad_accum, denom, part);
-    else
-        preprocess_bwd_kernel<false, true><<<grid, kBwdBlock, smem, s>>>(
-            vp, means3D, radii, shs, clamped, scales, rotations, cov3D, dL_dmean2D, dL_dconic, dL_dmean3D, dL_dcolor,
-            dL_dcov3D, dL_dsh, dL_dscale, dL_drot, dL_dz, nullptr, nullptr, part);
+    if (cam) {
+        const cudaError_t e = cudaMallocAsync((void**)&part, (size_t)grid * kCamTerms * sizeof(double), s);
+        if (e != cudaSuccess) return e;
+    }
+    kernels[accumulate][cam][antialiasing]<<<grid, kBwdBlock, smem, s>>>(
+        vp, means3D, radii, shs, clamped, scales, rotations, cov3D, dL_dmean2D, dL_dconic, dL_dmean3D, dL_dcolor,
+        dL_dcov3D, dL_dsh, dL_dscale, dL_drot, dL_dz, accumulate ? grad_accum : nullptr, accumulate ? denom : nullptr,
+        part, rec, dL_dop_eff, dL_dopacity);
+    g_launches++;
+    if (!cam) return cudaSuccess;  // a launch error is left for the caller's cudaGetLastError
     camera_grad_sum_kernel<<<kCamTerms, kCamSumThreads, 0, s>>>(grid, part, dL_dcamera);
-    g_launches += 2;
+    g_launches++;
     return cudaFreeAsync(part, s);
 }
 

@@ -10,7 +10,10 @@
 // plus rasterize_gaussians_backward_camera(same arguments as rasterize_gaussians_backward) -> its 9 gradients +
 // (dL_dviewmatrix [4,4], dL_dprojmatrix [4,4], dL_dcampos [3]) for pose refinement (f3dgs_backward_cam), and
 // rasterize_gaussians_backward_feature_geometry(same arguments, camera) -> the same 12 (the camera three None unless
-// `camera`) with the feature term of dL/dalpha (f3dgs_backward_feature_geometry).
+// `camera`) with the feature term of dL/dalpha (f3dgs_backward_feature_geometry).  Antialiased rendering:
+// rasterize_gaussians_antialiased (rasterize_gaussians' arguments and results, f3dgs_forward_antialiased) and
+// rasterize_gaussians_backward_antialiased(same arguments, camera=False, semantic_feature=None) -> the same 12, with the
+// feature term when semantic_feature is given (f3dgs_backward_antialiased).
 // Differences (all permissive): the feature width is read from semantic_feature.size(-1) at run
 // time (reference: compile-time NUM_SEMANTIC_CHANNELS, config.h:16); an empty / undefined
 // semantic_feature means C = 0; semantic_feature may be float32 or float16, and the feature map
@@ -106,15 +109,22 @@ torch::Tensor scratch_tensor(size_t bytes, const char* fn, const torch::Tensor& 
 
 }  // namespace
 
-std::tuple<int, torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor,
-           torch::Tensor>
-RasterizeGaussiansCUDA(const torch::Tensor& background, const torch::Tensor& means3D, const torch::Tensor& colors,
-                       const torch::Tensor& semantic_feature, const torch::Tensor& opacity,
-                       const torch::Tensor& scales, const torch::Tensor& rotations, const float scale_modifier,
-                       const torch::Tensor& cov3D_precomp, const torch::Tensor& viewmatrix,
-                       const torch::Tensor& projmatrix, const float tan_fovx, const float tan_fovy,
-                       const int image_height, const int image_width, const torch::Tensor& sh, const int degree,
-                       const torch::Tensor& campos, const bool prefiltered, const bool debug) {
+using ForwardResults = std::tuple<int, torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor,
+                                  torch::Tensor, torch::Tensor>;
+
+#define FORWARD_PARAMS                                                                                                 \
+    const torch::Tensor &background, const torch::Tensor &means3D, const torch::Tensor &colors,                       \
+        const torch::Tensor &semantic_feature, const torch::Tensor &opacity, const torch::Tensor &scales,             \
+        const torch::Tensor &rotations, const float scale_modifier, const torch::Tensor &cov3D_precomp,               \
+        const torch::Tensor &viewmatrix, const torch::Tensor &projmatrix, const float tan_fovx, const float tan_fovy, \
+        const int image_height, const int image_width, const torch::Tensor &sh, const int degree,                     \
+        const torch::Tensor &campos, const bool prefiltered, const bool debug
+#define FORWARD_ARGS                                                                                                   \
+    background, means3D, colors, semantic_feature, opacity, scales, rotations, scale_modifier, cov3D_precomp,         \
+        viewmatrix, projmatrix, tan_fovx, tan_fovy, image_height, image_width, sh, degree, campos, prefiltered, debug
+
+// Body of rasterize_gaussians and rasterize_gaussians_antialiased (f3dgs_forward_antialiased)
+static ForwardResults forward(FORWARD_PARAMS, const bool antialiasing) {
     if (means3D.ndimension() != 2 || means3D.size(1) != 3) {
         AT_ERROR("means3D must have dimensions (num_points, 3)");
     }
@@ -157,6 +167,15 @@ RasterizeGaussiansCUDA(const torch::Tensor& background, const torch::Tensor& mea
         auto vm = input(viewmatrix, dev, "viewmatrix"), pm = input(projmatrix, dev, "projmatrix");
         auto shc = input(sh, dev, "shs"), cp = input(campos, dev, "campos");
         cudaStream_t stream = c10::cuda::getCurrentCUDAStream().stream();
+        if (antialiasing) {
+            rendered = f3dgs_forward_antialiased(
+                resize_tensor, &geomBuffer, resize_tensor, &binningBuffer, resize_tensor, &imgBuffer, P, degree, M, C,
+                fptr(bg), W, H, fptr(m3), fptr(shc), fptr(col), has_sf ? sf.data_ptr() : nullptr, dtype_code(sf),
+                fptr(op), fptr(sc), scale_modifier, fptr(rot), fptr(cov), fptr(vm), fptr(pm), fptr(cp), tan_fovx,
+                tan_fovy, prefiltered ? 1 : 0, out_color.data_ptr<float>(), C ? out_feature.data_ptr() : nullptr,
+                out_depth.data_ptr<float>(), radii.data_ptr<int>(), debug ? 1 : 0, (void*)stream);
+            check_rc(rendered, "f3dgs_forward_antialiased");
+        } else
         call_f32_or_f16(sf, f3dgs_forward, "f3dgs_forward", f3dgs_forward_f16, "f3dgs_forward_f16",
                         [&](auto fn, auto sp) {  // sp: float* or uint16_t*, and the feature map is of the same type
                             auto* fm = C ? static_cast<decltype(sp)>(out_feature.data_ptr()) : nullptr;
@@ -172,12 +191,18 @@ RasterizeGaussiansCUDA(const torch::Tensor& background, const torch::Tensor& mea
     return std::make_tuple(rendered, out_color, out_feature, out_depth, radii, geomBuffer, binningBuffer, imgBuffer);
 }
 
+ForwardResults RasterizeGaussiansCUDA(FORWARD_PARAMS) { return forward(FORWARD_ARGS, false); }
+ForwardResults RasterizeGaussiansAntialiasedCUDA(FORWARD_PARAMS) { return forward(FORWARD_ARGS, true); }
+#undef FORWARD_PARAMS
+#undef FORWARD_ARGS
+
 using BackwardGrads = std::tuple<torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor,
                                  torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor>;
 
-// Body of rasterize_gaussians_backward, _camera and _feature_geometry: with a non-NULL camera (35 floats on the device),
-// the _cam entries, which add the camera gradient to it; with feature_geometry, f3dgs_backward_feature_geometry, which
-// reads semantic_feature and takes the camera gradient as an optional argument
+// Body of rasterize_gaussians_backward, _camera, _feature_geometry and _antialiased: with a non-NULL camera (35 floats on
+// the device), the _cam entries, which add the camera gradient to it; with feature_geometry,
+// f3dgs_backward_feature_geometry, which reads semantic_feature and takes the camera gradient as an optional argument;
+// with antialiasing, f3dgs_backward_antialiased, whose feature term reads `features` if that is given
 static BackwardGrads backward_grads(const torch::Tensor& background, const torch::Tensor& means3D,
                                const torch::Tensor& radii, const torch::Tensor& colors,
                                const torch::Tensor& semantic_feature, const torch::Tensor& scales,
@@ -188,7 +213,8 @@ static BackwardGrads backward_grads(const torch::Tensor& background, const torch
                                const torch::Tensor& dL_dout_depth, const torch::Tensor& sh, const int degree,
                                const torch::Tensor& campos, const torch::Tensor& geomBuffer, const int R,
                                const torch::Tensor& binningBuffer, const torch::Tensor& imageBuffer,
-                               const bool debug, float* camera, bool feature_geometry = false) {
+                               const bool debug, float* camera, bool feature_geometry = false,
+                               bool antialiasing = false, const torch::Tensor& features = torch::Tensor()) {
     TORCH_CHECK(means3D.is_cuda(), "means3D must be a CUDA tensor (this build has no CPU path)");
     const c10::cuda::CUDAGuard guard(means3D.device());
     const auto dev = means3D.device();
@@ -256,24 +282,33 @@ static BackwardGrads backward_grads(const torch::Tensor& background, const torch
                 else return run(fn, gp, std::tuple<>(), tail);
             };
         };
-        if (feature_geometry) {
-            // this entry reads the features themselves, not only their shape
-            TORCH_CHECK(!C || semantic_feature.numel() == (int64_t)P * C, "semantic_feature must have P * C = ",
-                        (int64_t)P * C, " elements (got ", semantic_feature.numel(), ")");
-            auto sf = C ? semantic_feature.contiguous() : semantic_feature;
-            check_rc(f3dgs_backward_feature_geometry(
-                         P, degree, M, R, C, fptr(bg), W, H, fptr(m3), fptr(shc), fptr(col), C ? sf.data_ptr() : nullptr,
-                         dtype_code(sf), fptr(sc), scale_modifier, fptr(rot), fptr(cov), fptr(vm), fptr(pm), fptr(cp),
-                         tan_fovx, tan_fovy, rad.data_ptr<int>(), reinterpret_cast<char*>(gb.data_ptr()),
-                         reinterpret_cast<char*>(bb.data_ptr()), reinterpret_cast<char*>(ib.data_ptr()), fptr(gc),
-                         gf.defined() ? gf.data_ptr() : nullptr, dtype_code(gf), 1.0f, fptr(gd),
-                         dL_dmeans2D.data_ptr<float>(), dL_dconic.data_ptr<float>(), dL_dopacity.data_ptr<float>(),
-                         dL_dcolors.data_ptr<float>(), C ? dL_dsemantic_feature.data_ptr<float>() : nullptr,
-                         dL_dmeans3D.data_ptr<float>(), dL_dcov3D.data_ptr<float>(),
-                         M ? dL_dsh.data_ptr<float>() : nullptr, dL_dscales.data_ptr<float>(),
-                         dL_drotations.data_ptr<float>(), dL_dz.data_ptr<float>(), debug ? 1 : 0, (void*)stream, camera),
+        // the _feature_geometry / _antialiased entries: features sf (its element type by code; NULL if absent or C == 0)
+        auto typed_call = [&](auto fn, const torch::Tensor& sf) {
+            return fn(P, degree, M, R, C, fptr(bg), W, H, fptr(m3), fptr(shc), fptr(col),
+                      C && sf.defined() && sf.numel() ? sf.data_ptr() : nullptr, dtype_code(sf), fptr(sc),
+                      scale_modifier, fptr(rot), fptr(cov), fptr(vm), fptr(pm), fptr(cp), tan_fovx, tan_fovy,
+                      rad.data_ptr<int>(), reinterpret_cast<char*>(gb.data_ptr()), reinterpret_cast<char*>(bb.data_ptr()),
+                      reinterpret_cast<char*>(ib.data_ptr()), fptr(gc), gf.defined() ? gf.data_ptr() : nullptr,
+                      dtype_code(gf), 1.0f, fptr(gd), dL_dmeans2D.data_ptr<float>(), dL_dconic.data_ptr<float>(),
+                      dL_dopacity.data_ptr<float>(), dL_dcolors.data_ptr<float>(),
+                      C ? dL_dsemantic_feature.data_ptr<float>() : nullptr, dL_dmeans3D.data_ptr<float>(),
+                      dL_dcov3D.data_ptr<float>(), M ? dL_dsh.data_ptr<float>() : nullptr, dL_dscales.data_ptr<float>(),
+                      dL_drotations.data_ptr<float>(), dL_dz.data_ptr<float>(), debug ? 1 : 0, (void*)stream, camera);
+        };
+        // these entries read the features themselves, not only their shape
+        auto feature_rows = [&](const torch::Tensor& t) {
+            if (!t.defined() || t.numel() == 0) return t;
+            check_features(t, dev);
+            TORCH_CHECK(!C || t.numel() == (int64_t)P * C, "semantic_feature must have P * C = ", (int64_t)P * C,
+                        " elements (got ", t.numel(), ")");
+            return t.contiguous();
+        };
+        if (antialiasing)
+            check_rc(typed_call(f3dgs_backward_antialiased, feature_rows(features)), "f3dgs_backward_antialiased");
+        else if (feature_geometry)
+            check_rc(typed_call(f3dgs_backward_feature_geometry, feature_rows(semantic_feature)),
                      "f3dgs_backward_feature_geometry");
-        } else if (camera)
+        else if (camera)
             call_f32_or_f16(gf, f3dgs_backward_cam, "f3dgs_backward_cam", f3dgs_backward_cam_f16,
                             "f3dgs_backward_cam_f16", dispatch(std::make_tuple(camera)));
         else
@@ -325,6 +360,24 @@ RasterizeGaussiansBackwardFeatureGeometryCUDA(BACKWARD_PARAMS, const bool camera
                           std::make_tuple(cam.narrow(0, 0, 16).view({4, 4}), cam.narrow(0, 16, 16).view({4, 4}),
                                           cam.narrow(0, 32, 3)));
 }
+
+// rasterize_gaussians_backward_feature_geometry's 12 results for the buffers of rasterize_gaussians_antialiased
+// (f3dgs_backward_antialiased): the feature term of dL/dalpha only when `features` (the forward's semantic_feature) is
+// given, the camera gradients only with `camera`
+decltype(std::tuple_cat(BackwardGrads(), std::tuple<torch::Tensor, torch::Tensor, torch::Tensor>()))
+RasterizeGaussiansBackwardAntialiasedCUDA(BACKWARD_PARAMS, const bool camera,
+                                          const std::optional<torch::Tensor>& features) {
+    TORCH_CHECK(means3D.is_cuda(), "means3D must be a CUDA tensor (this build has no CPU path)");
+    const c10::cuda::CUDAGuard guard(means3D.device());
+    const torch::Tensor f = features.has_value() ? *features : torch::Tensor();
+    if (!camera)
+        return std::tuple_cat(backward_grads(BACKWARD_ARGS, nullptr, false, true, f),
+                              std::make_tuple(torch::Tensor(), torch::Tensor(), torch::Tensor()));
+    torch::Tensor cam = torch::zeros({F3DGS_CAMERA_GRAD_FLOATS}, means3D.options().dtype(torch::kFloat32));
+    return std::tuple_cat(backward_grads(BACKWARD_ARGS, cam.data_ptr<float>(), false, true, f),
+                          std::make_tuple(cam.narrow(0, 0, 16).view({4, 4}), cam.narrow(0, 16, 16).view({4, 4}),
+                                          cam.narrow(0, 32, 3)));
+}
 #undef BACKWARD_PARAMS
 #undef BACKWARD_ARGS
 
@@ -332,7 +385,8 @@ RasterizeGaussiansBackwardFeatureGeometryCUDA(BACKWARD_PARAMS, const bool camera
 // caller passes (typically views of one flat gradient buffer, see diff_gaussian_rasterization/parallel.py); nothing is
 // allocated besides one cached scratch tensor per device.  Undefined / empty tensors stand for "not an input".
 // semantic_feature (optional, [P,...,C] float32 or float16): f3dgs_backward_accum_feature_geometry, the feature term of
-// dL/dalpha in the geometric gradients.
+// dL/dalpha in the geometric gradients.  antialiasing: f3dgs_backward_accum_antialiased, for the buffers of
+// rasterize_gaussians_antialiased (with the feature term if semantic_feature is given).
 void RasterizeGaussiansBackwardAccumCUDA(
     const torch::Tensor& background, const torch::Tensor& means3D, const torch::Tensor& radii,
     const torch::Tensor& colors, const torch::Tensor& scales, const torch::Tensor& rotations, const float scale_modifier,
@@ -344,7 +398,8 @@ void RasterizeGaussiansBackwardAccumCUDA(
     torch::Tensor g_semantic_feature, torch::Tensor g_opacities, torch::Tensor g_scales, torch::Tensor g_rotations,
     torch::Tensor g_cov3D, torch::Tensor g_means2D_out, torch::Tensor grad_accum, torch::Tensor denom,
     const int64_t composite_done_event, const bool debug, const double feature_grad_scale,
-    const std::optional<torch::Tensor>& camera_grad, const std::optional<torch::Tensor>& semantic_feature) {
+    const std::optional<torch::Tensor>& camera_grad, const std::optional<torch::Tensor>& semantic_feature,
+    const bool antialiasing) {
     TORCH_CHECK(means3D.is_cuda(), "means3D must be a CUDA tensor (this build has no CPU path)");
     const c10::cuda::CUDAGuard guard(means3D.device());
     const auto dev = means3D.device();
@@ -381,13 +436,18 @@ void RasterizeGaussiansBackwardAccumCUDA(
         cam = in_place(*camera_grad, dev, F3DGS_CAMERA_GRAD_FLOATS, "camera_grad");
     }
     cudaStream_t stream = c10::cuda::getCurrentCUDAStream().stream();
-    if (semantic_feature.has_value() && semantic_feature->defined()) {
-        check_features(*semantic_feature, dev);
-        TORCH_CHECK(semantic_feature->numel() == (int64_t)P * C, "semantic_feature must have P * C = ", (int64_t)P * C,
-                    " elements (got ", semantic_feature->numel(), ")");
-        auto sf = semantic_feature->contiguous();
-        check_rc(f3dgs_backward_accum_feature_geometry(
-                     P, degree, M, R, C, fptr(bg), W, H, fptr(m3), fptr(shc), fptr(col), C ? sf.data_ptr() : nullptr,
+    const bool has_features = semantic_feature.has_value() && semantic_feature->defined();
+    if (has_features || antialiasing) {
+        torch::Tensor sf;
+        if (has_features) {
+            check_features(*semantic_feature, dev);
+            TORCH_CHECK(semantic_feature->numel() == (int64_t)P * C, "semantic_feature must have P * C = ",
+                        (int64_t)P * C, " elements (got ", semantic_feature->numel(), ")");
+            sf = semantic_feature->contiguous();
+        }
+        check_rc((antialiasing ? f3dgs_backward_accum_antialiased : f3dgs_backward_accum_feature_geometry)(
+                     P, degree, M, R, C, fptr(bg), W, H, fptr(m3), fptr(shc), fptr(col),
+                     C && has_features ? sf.data_ptr() : nullptr,
                      dtype_code(sf), fptr(sc), scale_modifier, fptr(rot), fptr(cov), fptr(vm), fptr(pm), fptr(cp),
                      tan_fovx, tan_fovy, rad.data_ptr<int>(), reinterpret_cast<char*>(geomBuffer.data_ptr()),
                      reinterpret_cast<char*>(binningBuffer.data_ptr()),
@@ -404,7 +464,7 @@ void RasterizeGaussiansBackwardAccumCUDA(
                      in_place(grad_accum, dev, P, "grad_accum"), in_place(denom, dev, P, "denom"),
                      reinterpret_cast<void*>(static_cast<intptr_t>(composite_done_event)), debug ? 1 : 0,
                      (void*)stream, cam),
-                 "f3dgs_backward_accum_feature_geometry");
+                 antialiasing ? "f3dgs_backward_accum_antialiased" : "f3dgs_backward_accum_feature_geometry");
         return;
     }
     // scale: the float16 symbol's scale after the map, () for the float32 one; tail: (dL_dcamera) or ()
@@ -973,6 +1033,15 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
               py::arg("g_scales"), py::arg("g_rotations"), py::arg("g_cov3D"), py::arg("g_means2D_out"),
               py::arg("grad_accum"), py::arg("denom"), py::arg("composite_done_event"), py::arg("debug"),
               py::arg("feature_grad_scale") = 1.0, py::arg("camera_grad") = py::none(),
+              py::arg("semantic_feature") = py::none(), py::arg("antialiasing") = false);
+        m.def("rasterize_gaussians_antialiased", &RasterizeGaussiansAntialiasedCUDA);
+        m.def("rasterize_gaussians_backward_antialiased", &RasterizeGaussiansBackwardAntialiasedCUDA,
+              py::arg("background"), py::arg("means3D"), py::arg("radii"), py::arg("colors"), py::arg("features_like"),
+              py::arg("scales"), py::arg("rotations"), py::arg("scale_modifier"), py::arg("cov3D_precomp"),
+              py::arg("viewmatrix"), py::arg("projmatrix"), py::arg("tan_fovx"), py::arg("tan_fovy"),
+              py::arg("dL_dout_color"), py::arg("dL_dout_feature"), py::arg("dL_dout_depth"), py::arg("sh"),
+              py::arg("degree"), py::arg("campos"), py::arg("geomBuffer"), py::arg("R"), py::arg("binningBuffer"),
+              py::arg("imageBuffer"), py::arg("debug"), py::arg("camera") = false,
               py::arg("semantic_feature") = py::none());
     }
     m.def("rasterize_gaussians_backward_camera", &RasterizeGaussiansBackwardCameraCUDA);

@@ -31,6 +31,11 @@ Behavioural notes
     `rasterize_gaussians_feature_geometry` with `rasterize_gaussians`'s arguments, lets a loss on the feature map move
     opacities, means, scales, rotations and the camera too (f3dgs_backward_feature_geometry).  By default the feature
     map feeds dL/dsemantic_feature only, as in the reference (SURVEY D.1).
+  * antialiased rendering (opt-in): `AntialiasedGaussianRasterizer(raster_settings)` multiplies each opacity by
+    sqrt(det(S) / det(S + 0.3 I)), S the 2-D covariance before the rasterizer's 0.3 px^2 dilation, so that a dilated
+    sub-pixel Gaussian keeps the integral of the undilated one (f3dgs_forward_antialiased / f3dgs_backward_antialiased).
+    Renders at a resolution other than the training one (lower-resolution feature targets, lifting at a teacher's
+    resolution) then stay consistent.  By default the opacity is used as it is, as in the reference.
   * `debug=True` keeps the reference semantics: arguments are snapshotted to CPU first and dumped
     to snapshot_fw.dump / snapshot_bw.dump if the native call raises (reference :89-97,:147-155);
     natively it synchronises and checks after every stage.
@@ -56,6 +61,7 @@ __all__ = [
     "GaussianRasterizer",
     "rasterize_gaussians",
     "rasterize_gaussians_feature_geometry",
+    "AntialiasedGaussianRasterizer",
 ]
 
 
@@ -96,16 +102,18 @@ class _RasterizeGaussians(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, means3D, means2D, sh, colors_precomp, semantic_feature, opacities, scales, rotations,
-                cov3Ds_precomp, raster_settings):
+                cov3Ds_precomp, raster_settings, antialiasing=False):
         rs = raster_settings
         if semantic_feature is None:
             semantic_feature = torch.empty(0, device=means3D.device, dtype=means3D.dtype)
         args = (rs.bg, means3D, colors_precomp, semantic_feature, opacities, scales, rotations, rs.scale_modifier,
                 cov3Ds_precomp, rs.viewmatrix, rs.projmatrix, rs.tanfovx, rs.tanfovy, rs.image_height,
                 rs.image_width, sh, rs.sh_degree, rs.campos, rs.prefiltered, rs.debug)
+        fn = _C.rasterize_gaussians_antialiased if antialiasing else _C.rasterize_gaussians
         (num_rendered, color, feature_map, depth, radii, geomBuffer, binningBuffer, imgBuffer) = _call_native(
-            _C.rasterize_gaussians, args, rs.debug, "snapshot_fw.dump", "forward")
+            fn, args, rs.debug, "snapshot_fw.dump", "forward")
         ctx.raster_settings = rs
+        ctx.antialiasing = antialiasing
         ctx.num_rendered = num_rendered
         ctx.save_for_backward(colors_precomp, semantic_feature, means3D, scales, rotations, cov3Ds_precomp, radii,
                               sh, geomBuffer, binningBuffer, imgBuffer)
@@ -114,8 +122,9 @@ class _RasterizeGaussians(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, grad_out_color, grad_out_feature, _grad_radii, grad_depth):
-        grads = _native_backward(ctx, _C.rasterize_gaussians_backward, grad_out_color, grad_out_feature, grad_depth)
-        return grads[:9] + (None,)
+        fn = _antialiased_backward(False, False) if ctx.antialiasing else _C.rasterize_gaussians_backward
+        grads = _native_backward(ctx, fn, grad_out_color, grad_out_feature, grad_depth)
+        return grads[:9] + (None, None)
 
 
 def _native_backward(ctx, fn, grad_out_color, grad_out_feature, grad_depth):
@@ -155,22 +164,32 @@ class _RasterizeGaussiansCamera(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, means3D, means2D, sh, colors_precomp, semantic_feature, opacities, scales, rotations,
-                cov3Ds_precomp, viewmatrix, projmatrix, campos, raster_settings):
+                cov3Ds_precomp, viewmatrix, projmatrix, campos, raster_settings, antialiasing=False):
         rs = raster_settings._replace(viewmatrix=viewmatrix, projmatrix=projmatrix, campos=campos)
         ctx.camera_shapes = (viewmatrix.shape, projmatrix.shape, campos.shape)
         return _RasterizeGaussians.forward(ctx, means3D, means2D, sh, colors_precomp, semantic_feature, opacities,
-                                           scales, rotations, cov3Ds_precomp, rs)
+                                           scales, rotations, cov3Ds_precomp, rs, antialiasing)
 
     @staticmethod
     def backward(ctx, grad_out_color, grad_out_feature, _grad_radii, grad_depth):
-        grads = _native_backward(ctx, _C.rasterize_gaussians_backward_camera, grad_out_color, grad_out_feature,
-                                 grad_depth)
+        fn = _antialiased_backward(True, False) if ctx.antialiasing else _C.rasterize_gaussians_backward_camera
+        grads = _native_backward(ctx, fn, grad_out_color, grad_out_feature, grad_depth)
         cam = tuple(g.reshape(shape) for g, shape in zip(grads[9:], ctx.camera_shapes))
-        return grads[:9] + cam + (None,)
+        return grads[:9] + cam + (None, None)
 
 
-def _feature_geometry_backward(camera):
-    """rasterize_gaussians_backward_feature_geometry with the reference backward's positional arguments"""
+def _antialiased_backward(camera, feature_geometry):
+    """rasterize_gaussians_backward_antialiased with the reference backward's positional arguments; the feature term
+    reads the forward's semantic_feature (the fifth argument)"""
+    return lambda *args: _C.rasterize_gaussians_backward_antialiased(
+        *args, camera=camera, semantic_feature=args[4] if feature_geometry else None)
+
+
+def _feature_geometry_backward(ctx, camera):
+    """rasterize_gaussians_backward_feature_geometry (or its antialiased counterpart, for an antialiased forward) with
+    the reference backward's positional arguments"""
+    if ctx.antialiasing:
+        return _antialiased_backward(camera, True)
     return lambda *args: _C.rasterize_gaussians_backward_feature_geometry(*args, camera)
 
 
@@ -180,8 +199,9 @@ class _RasterizeGaussiansFeatureGeometry(_RasterizeGaussians):
 
     @staticmethod
     def backward(ctx, grad_out_color, grad_out_feature, _grad_radii, grad_depth):
-        grads = _native_backward(ctx, _feature_geometry_backward(False), grad_out_color, grad_out_feature, grad_depth)
-        return grads[:9] + (None,)
+        grads = _native_backward(ctx, _feature_geometry_backward(ctx, False), grad_out_color, grad_out_feature,
+                                 grad_depth)
+        return grads[:9] + (None, None)
 
 
 class _RasterizeGaussiansCameraFeatureGeometry(_RasterizeGaussiansCamera):
@@ -189,9 +209,10 @@ class _RasterizeGaussiansCameraFeatureGeometry(_RasterizeGaussiansCamera):
 
     @staticmethod
     def backward(ctx, grad_out_color, grad_out_feature, _grad_radii, grad_depth):
-        grads = _native_backward(ctx, _feature_geometry_backward(True), grad_out_color, grad_out_feature, grad_depth)
+        grads = _native_backward(ctx, _feature_geometry_backward(ctx, True), grad_out_color, grad_out_feature,
+                                 grad_depth)
         cam = tuple(g.reshape(shape) for g, shape in zip(grads[9:], ctx.camera_shapes))
-        return grads[:9] + cam + (None,)
+        return grads[:9] + cam + (None, None)
 
 
 def _camera_requires_grad(rs):
@@ -199,14 +220,14 @@ def _camera_requires_grad(rs):
 
 
 def _rasterize(means3D, means2D, sh, colors_precomp, semantic_feature, opacities, scales, rotations, cov3Ds_precomp,
-               rs, feature_geometry):
+               rs, feature_geometry, antialiasing=False):
     if torch.is_grad_enabled() and _camera_requires_grad(rs):
         fn = _RasterizeGaussiansCameraFeatureGeometry if feature_geometry else _RasterizeGaussiansCamera
         return fn.apply(means3D, means2D, sh, colors_precomp, semantic_feature, opacities, scales, rotations,
-                        cov3Ds_precomp, rs.viewmatrix, rs.projmatrix, rs.campos, rs)
+                        cov3Ds_precomp, rs.viewmatrix, rs.projmatrix, rs.campos, rs, antialiasing)
     fn = _RasterizeGaussiansFeatureGeometry if feature_geometry else _RasterizeGaussians
     return fn.apply(means3D, means2D, sh, colors_precomp, semantic_feature, opacities, scales, rotations,
-                    cov3Ds_precomp, rs)
+                    cov3Ds_precomp, rs, antialiasing)
 
 
 def rasterize_gaussians(means3D, means2D, sh, colors_precomp, semantic_feature, opacities, scales, rotations,
@@ -227,6 +248,8 @@ def rasterize_gaussians_feature_geometry(means3D, means2D, sh, colors_precomp, s
 class GaussianRasterizer(nn.Module):
     """The reference's rasterizer module.  feature_geometry=True: the backward also feeds the feature map's gradient
     into the geometry (rasterize_gaussians_feature_geometry)."""
+
+    antialiasing = False  # AntialiasedGaussianRasterizer
 
     def __init__(self, raster_settings, feature_geometry=False):
         super().__init__()
@@ -259,4 +282,13 @@ class GaussianRasterizer(nn.Module):
         if cov3D_precomp is None:
             cov3D_precomp = empty
         return _rasterize(means3D, means2D, shs, colors_precomp, semantic_feature, opacities, scales, rotations,
-                          cov3D_precomp, rs, self.feature_geometry)
+                          cov3D_precomp, rs, self.feature_geometry, self.antialiasing)
+
+
+class AntialiasedGaussianRasterizer(GaussianRasterizer):
+    """GaussianRasterizer with antialiased opacities: each opacity is scaled by sqrt(det(S) / det(S + 0.3 I)), S the
+    2-D covariance before the 0.3 px^2 dilation, so that the dilation conserves a Gaussian's integral (see the module
+    docstring).  The render and every gradient are those of the antialiased model; the arguments are
+    GaussianRasterizer's."""
+
+    antialiasing = True

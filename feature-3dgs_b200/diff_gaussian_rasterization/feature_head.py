@@ -315,9 +315,14 @@ class FeatureLift:
     `rs._replace(image_height=Hg, image_width=Wg)`: pixel centres then follow the rasterizer's own projection at that
     resolution (pixel x covers [x, x+1) of Wg, the same field of view).  That is deliberately not the relation of the
     training loss, which resizes the W x H render to Hg x Wg with align_corners=True (corner pixel centres on corner
-    pixel centres); the two differ by up to half a teacher pixel at the image borders.  There is no autograd."""
+    pixel centres); the two differ by up to half a teacher pixel at the image borders.  There is no autograd.
 
-    def __init__(self, means3D, opacities, scales=None, rotations=None, C: int = None, cov3D_precomp=None):
+    A teacher map is usually coarser than the training images, and there the rasterizer's 0.3 px^2 dilation makes
+    small Gaussians blend over more of the map than they cover.  antialiasing=True weights with the antialiased
+    opacities (AntialiasedGaussianRasterizer), which keep each Gaussian's integral at every resolution."""
+
+    def __init__(self, means3D, opacities, scales=None, rotations=None, C: int = None, cov3D_precomp=None,
+                 antialiasing: bool = False):
         if C is None or int(C) < 1 or int(C) > 4096:
             raise ValueError(f"FeatureLift: C must be 1..4096, got {C}")
         if (scales is None or rotations is None) == (cov3D_precomp is None):
@@ -326,6 +331,7 @@ class FeatureLift:
             raise ValueError("FeatureLift: means3D must be a CUDA tensor (there is no CPU path)")
         dev = means3D.device
         self.C, self.P = int(C), int(means3D.shape[0])
+        self.antialiasing = bool(antialiasing)
         e = torch.empty(0, device=dev)
         self._geom = dict(means3D=means3D.detach(), opacities=opacities.detach(),
                           scales=e if scales is None else scales.detach(),
@@ -338,12 +344,12 @@ class FeatureLift:
         self.weight_sum = self.flat[self.P * self.C:]
 
     @classmethod
-    def from_state(cls, state, C: int = None):
+    def from_state(cls, state, C: int = None, antialiasing: bool = False):
         """A lift over the Gaussians of a trainer.GaussianState (its activated geometry); C defaults to the state's
         feature width."""
         act = state.activate()
         C = state.raw["semantic_feature"].shape[-1] if C is None else C
-        return cls(act["means3D"], act["opacities"], act["scales"], act["rotations"], C)
+        return cls(act["means3D"], act["opacities"], act["scales"], act["rotations"], C, antialiasing=antialiasing)
 
     def add(self, raster_settings, feature_map: torch.Tensor):
         """Accumulate one view: feature_map [C,H,W] (float32, or float16 read exactly) with (H, W) ==
@@ -366,7 +372,8 @@ class FeatureLift:
             return
         g, e = self._geom, self._empty
         with torch.no_grad():
-            R, _, _, _, _, geom, binning, img = _C().rasterize_gaussians(
+            fwd = _C().rasterize_gaussians_antialiased if self.antialiasing else _C().rasterize_gaussians
+            R, _, _, _, _, geom, binning, img = fwd(
                 rs.bg, g["means3D"], self._colors, e, g["opacities"], g["scales"], g["rotations"], rs.scale_modifier,
                 g["cov3D"], rs.viewmatrix, rs.projmatrix, rs.tanfovx, rs.tanfovy, H, W, e, rs.sh_degree, rs.campos,
                 rs.prefiltered, rs.debug)

@@ -87,7 +87,7 @@ class CameraGrad(NamedTuple):
 
 
 class _ViewCtx:
-    __slots__ = ("rs", "num_rendered", "radii", "geom", "binning", "img", "inputs")
+    __slots__ = ("rs", "num_rendered", "radii", "geom", "binning", "img", "inputs", "antialiasing")
 
 
 class ViewBatch:
@@ -145,17 +145,20 @@ class ViewBatch:
     def zero_(self):
         self.flat.zero_()
 
-    def forward(self, rs):
-        """One view's forward (no autograd graph).  `rs` is a GaussianRasterizationSettings."""
+    def forward(self, rs, antialiasing: bool = False):
+        """One view's forward (no autograd graph).  `rs` is a GaussianRasterizationSettings.  antialiasing=True renders
+        with the antialiased opacities (AntialiasedGaussianRasterizer); the returned ctx remembers it, so that
+        `backward` differentiates the same model."""
         p = self.params
         e = torch.Tensor([])
         sf = p.get("semantic_feature", self._empty)
-        out = self._C.rasterize_gaussians(rs.bg, p["means3D"], e, sf, p["opacities"], p["scales"], p["rotations"],
-                                          rs.scale_modifier, e, rs.viewmatrix, rs.projmatrix, rs.tanfovx, rs.tanfovy,
-                                          rs.image_height, rs.image_width, p["shs"], rs.sh_degree, rs.campos,
-                                          rs.prefiltered, rs.debug)
+        fn = self._C.rasterize_gaussians_antialiased if antialiasing else self._C.rasterize_gaussians
+        out = fn(rs.bg, p["means3D"], e, sf, p["opacities"], p["scales"], p["rotations"], rs.scale_modifier, e,
+                 rs.viewmatrix, rs.projmatrix, rs.tanfovx, rs.tanfovy, rs.image_height, rs.image_width, p["shs"],
+                 rs.sh_degree, rs.campos, rs.prefiltered, rs.debug)
         ctx = _ViewCtx()
         ctx.rs = rs
+        ctx.antialiasing = bool(antialiasing)
         ctx.num_rendered, color, feat, depth, ctx.radii, ctx.geom, ctx.binning, ctx.img = out
         return color, feat, ctx.radii, depth, ctx
 
@@ -171,7 +174,11 @@ class ViewBatch:
 
         feature_geometry=True also feeds g_feature into dL/dalpha, so that the feature loss reaches the opacities, means,
         scales, rotations, the densification statistics and the camera gradient (f3dgs_backward_accum_feature_geometry,
-        which reads the batch's semantic_feature)."""
+        which reads the batch's semantic_feature).
+
+        A view rendered by forward(rs, antialiasing=True) is differentiated in that mode
+        (f3dgs_backward_accum_antialiased); its opacity gradient is final only after the backward preprocess, so the
+        early bucket of a `last=True` view then starts after it."""
         rs, p, g, e = ctx.rs, self.params, self.grads, torch.Tensor([])
         none = self._empty
         scale = 1.0
@@ -186,7 +193,7 @@ class ViewBatch:
             none, means2D_out if means2D_out is not None else none,
             self.grad_accum if self.grad_accum is not None else none, self.denom if self.denom is not None else none,
             int(self._ev.cuda_event) if (last and self._ev is not None) else 0, rs.debug, float(scale), cam,
-            p.get("semantic_feature") if feature_geometry else None)
+            p.get("semantic_feature") if feature_geometry else None, ctx.antialiasing)
         self._early_pending = bool(last and self._ev is not None)
         if cam is not None:
             return CameraGrad(cam[:16].view(4, 4), cam[16:32].view(4, 4), cam[32:35])

@@ -39,7 +39,7 @@ extern "C" {
 #define F3DGS_MAX_FEATURE_DIM 4096
 #define F3DGS_TILE 16 /* BLOCK_X == BLOCK_Y == 16, reference config.h:18-19 */
 #define F3DGS_CAMERA_GRAD_FLOATS 35 /* dL_dcamera of the _cam backward entries */
-/* element-type codes of the _feature_geometry backward entries */
+/* element-type codes of the _feature_geometry and _antialiased entries */
 #define F3DGS_F32 0 /* IEEE binary32 */
 #define F3DGS_F16 1 /* IEEE binary16 */
 
@@ -160,7 +160,8 @@ int f3dgs_backward_f16(int P, int D, int M, int R, int C,
  *     (scene/gaussian_model.py:436-438): for radii > 0, grad_accum += ||dL_dmean2D.xy||, denom += 1;
  *   - composite_done_event (optional cudaEvent_t): recorded on the stream after the backward composite kernel, i.e. when
  *     dL_dsemantic_feature and dL_dopacity of this view are complete (the backward preprocess does not touch them), so
- *     that a collective on that bucket can start on another stream while the preprocess still runs.
+ *     that a collective on that bucket can start on another stream while the preprocess still runs.  In the
+ *     antialiased entry (below) the preprocess finishes dL_dopacity, so the event is recorded after it.
  */
 size_t f3dgs_backward_scratch_bytes(int P);
 int f3dgs_backward_accum(int P, int D, int M, int R, int C,
@@ -316,8 +317,83 @@ int f3dgs_backward_accum_feature_geometry(int P, int D, int M, int R, int C,
                                           float* dL_drot, float* dL_dmean2D_out, float* grad_accum, float* denom,
                                           void* composite_done_event, int debug, void* cuda_stream, float* dL_dcamera);
 
+/* ---- antialiased rendering (opt-in; no reference counterpart: the reference dilates every 2-D covariance by 0.3 px^2
+ * and keeps the opacity, SURVEY A.2 step 5) ----
+ * The dilation is a low-pass filter that does not conserve energy: a Gaussian at or below a pixel on screen is widened
+ * but keeps its full opacity, so it is too thick and too bright, the more so the lower the rendering resolution.  The
+ * antialiased forward multiplies the opacity by the ratio of the undilated to the dilated splat's integral:
+ *     det0 = a0 c0 - b^2 (2-D covariance S = T V T^T before the dilation),  det = (a0 + 0.3)(c0 + 0.3) - b^2,
+ *     rho = sqrt(max(2.5e-5, det0 / det)),   op_eff = opacity * rho,
+ * and blends op_eff: it is the op of the splat records.  Conic, radii, tiles, depth, colour and everything else are those
+ * of the default forward; the render is bitwise the default forward's with opacities := op_eff.
+ *   f3dgs_forward_antialiased: f3dgs_forward's arguments, except that semantic_feature [P,C] and out_feature_map [C,H,W]
+ *     are of element type semantic_feature_dtype (F3DGS_F32, or F3DGS_F16 as f3dgs_forward_f16).
+ *   f3dgs_backward_antialiased / f3dgs_backward_accum_antialiased: the arguments and contracts of
+ *     f3dgs_backward_feature_geometry / f3dgs_backward_accum_feature_geometry, except that semantic_feature may be NULL
+ *     (no feature term: the counterpart without the feature term); dL_dcamera stays optional.  The composite's opacity
+ *     gradient g = dL/dop_eff becomes dL_dopacity = rho g, and rho's dependence on (a, b, c) joins the conic's gradient:
+ *         h = op_eff g / 2 (0 where rho is clamped),  dL/da += h (c0/det0 - c/det),  dL/dc += h (a0/det0 - a/det),
+ *         dL/db += 2 h b (1/det - 1/det0),
+ *     which reaches dL_dmean3D, dL_dscale, dL_drot, dL_dcov3D and dL_dcamera.  Where rho is clamped (a degenerate
+ *     undilated covariance among those: det0 = 0) it is constant and only dL_dopacity = rho g is added.  With dL_dcamera
+ *     every other output is bitwise that of the call without it, and one view accumulated into zeros gives the
+ *     assigning entry's bits, as for the default entries.  dL_dmean2D, dL_dconic, dL_dcolor,
+ *     dL_dsemantic_feature and dL_dz are the composite's, bitwise those of the counterpart on a forward with
+ *     opacities := op_eff.  The assigning entry lets the composite write g into the zero-filled dL_dopacity and rescales
+ *     it in place; the accumulating entry takes P floats for g from the device's default memory pool (F3DGS_ERR_ALLOC
+ *     if that fails) and adds rho g into dL_dopacity.  f3dgs_backward_scratch_bytes is unchanged.
+ *     composite_done_event is recorded after the backward preprocess, not the composite: only then is dL_dopacity final.
+ *     F3DGS_ERR_INVALID_ARGUMENT, before any launch, for an unknown dtype code, dL_dopacity overlapping another output
+ *     and whatever the counterpart rejects.
+ * Contract (not checkable without a host sync, like R): the buffers of an antialiased forward go to the antialiased
+ * backwards, or to f3dgs_lift_features_accum[_f16], and those of any other forward to the other backwards.  A mismatch
+ * gives wrong gradients, not an error. */
+int f3dgs_forward_antialiased(f3dgs_alloc_fn geometry_alloc, void* geometry_ctx,
+                              f3dgs_alloc_fn binning_alloc, void* binning_ctx,
+                              f3dgs_alloc_fn image_alloc, void* image_ctx,
+                              int P, int D, int M, int C,
+                              const float* background, int width, int height,
+                              const float* means3D, const float* shs, const float* colors_precomp,
+                              const void* semantic_feature, int semantic_feature_dtype, const float* opacities,
+                              const float* scales, float scale_modifier, const float* rotations,
+                              const float* cov3D_precomp,
+                              const float* viewmatrix, const float* projmatrix, const float* cam_pos,
+                              float tan_fovx, float tan_fovy, int prefiltered,
+                              float* out_color, void* out_feature_map, float* out_depth, int* radii,
+                              int debug, void* cuda_stream);
+int f3dgs_backward_antialiased(int P, int D, int M, int R, int C,
+                               const float* background, int width, int height,
+                               const float* means3D, const float* shs, const float* colors_precomp,
+                               const void* semantic_feature, int semantic_feature_dtype,
+                               const float* scales, float scale_modifier, const float* rotations,
+                               const float* cov3D_precomp,
+                               const float* viewmatrix, const float* projmatrix, const float* cam_pos,
+                               float tan_fovx, float tan_fovy, const int* radii,
+                               char* geom_buffer, char* binning_buffer, char* image_buffer,
+                               const float* dL_dpix, const void* dL_dfeaturepix, int dL_dfeaturepix_dtype,
+                               float dL_dfeaturepix_scale, const float* dL_depths,
+                               float* dL_dmean2D, float* dL_dconic, float* dL_dopacity, float* dL_dcolor,
+                               float* dL_dsemantic_feature, float* dL_dmean3D, float* dL_dcov3D,
+                               float* dL_dsh, float* dL_dscale, float* dL_drot, float* dL_dz,
+                               int debug, void* cuda_stream, float* dL_dcamera);
+int f3dgs_backward_accum_antialiased(int P, int D, int M, int R, int C,
+                                     const float* background, int width, int height,
+                                     const float* means3D, const float* shs, const float* colors_precomp,
+                                     const void* semantic_feature, int semantic_feature_dtype,
+                                     const float* scales, float scale_modifier, const float* rotations,
+                                     const float* cov3D_precomp,
+                                     const float* viewmatrix, const float* projmatrix, const float* cam_pos,
+                                     float tan_fovx, float tan_fovy, const int* radii,
+                                     char* geom_buffer, char* binning_buffer, char* image_buffer,
+                                     const float* dL_dpix, const void* dL_dfeaturepix, int dL_dfeaturepix_dtype,
+                                     float dL_dfeaturepix_scale, const float* dL_depths, char* scratch,
+                                     float* dL_dopacity, float* dL_dcolors_precomp, float* dL_dsemantic_feature,
+                                     float* dL_dmean3D, float* dL_dcov3D_precomp, float* dL_dsh, float* dL_dscale,
+                                     float* dL_drot, float* dL_dmean2D_out, float* grad_accum, float* denom,
+                                     void* composite_done_event, int debug, void* cuda_stream, float* dL_dcamera);
+
 /* ---- feature lifting (no reference counterpart): training-free back-projection of 2-D feature maps onto Gaussians ----
- * The buffers and R are those of an f3dgs_forward / f3dgs_forward_f16 of this view at width x height (any C of that
+ * The buffers and R are those of an f3dgs_forward / _f16 / _antialiased of this view at width x height (any C of that
  * forward, 0 included); feature_map [C,H,W] is a map at that resolution, 1 <= C <= F3DGS_MAX_FEATURE_DIM.
  * ACCUMULATES:  feature_sum[P,C] += sum_p w_ip * feature_map[:,p];   weight_sum[P] += sum_p w_ip,
  * w_ip = the blend weight alpha*T of Gaussian i at pixel p (the backward's unwound T: equal to the forward's blend weight
