@@ -224,6 +224,94 @@ def gaussian_ratio(ours, terms, m):
     return float(_ratio((ours.double() - ref).abs(), bar).max()) if ref.numel() else 0.0
 
 
+def colour_depth_dots(rec, Gc, Gd):
+    """dfn for composite_model of the default backward: per pair d = c_g . Gc_p + z_g Gd_p over the records' colour and
+    depth, and the sum of the four products' magnitudes.  Gc [HW, 3], Gd [HW] float32 upstream gradients."""
+    c, z = rec[:, 8:11].double(), rec[:, 11].double()
+    Gc, Gd = Gc.double(), Gd.double().reshape(-1)
+
+    def dfn(gid, pix):
+        cg, gc, t = c[gid], Gc[pix], z[gid] * Gd[pix]
+        return (cg * gc).sum(1) + t, (cg * gc).abs().sum(1) + t.abs()
+
+    return dfn
+
+
+def composite_model(pairs, w, rec, P, dfn, length, bg_dot=None):
+    """Float64 model of the composite's geometric gradients over its own records and its blended pairs (extracted
+    W > 0), in its own pair order:
+        L = sum_p [ sum_{g blended at p} alpha_gp T_gp d_gp + T_final,p bg_dot_p ]
+    with alpha = min(0.99, op exp(power)) (the clamp passes the gradient through, as in the composite), T the product of
+    (1 - alpha) over the pixel's earlier blended pairs and T_final over all of them.  torch autograd gives dL/dmean2D,
+    dL/dconic and dL/dopacity, mapped to the composite's conventions (the mean gradient times W / 2 and H / 2, half the
+    off-diagonal conic gradient).
+
+    dfn(gid, pix) -> (d, dabs): per blended pair the value the walk blends, d = c_g . Gc_p + z_g Gd_p for the default
+    backward (colour_depth_dots) or f_g . Gf_p for the feature term, computed in float64 from the float32 inputs, and the
+    sum of its products' magnitudes.  length: the number of products in d (4 for colour and depth, C for features).
+    bg_dot: None (no background term) or per pixel (bg . Gc_p, sum_i |bg_i Gc_p,i|) [HW] each.
+
+    Bar (per Gaussian and value, in the form of gaussian_ratio).  Per pair the composite forms dL/dalpha = T (d - A) -
+    T_final bg_dot / (1 - alpha), with A the back-to-front recurrence over the pixel's later pairs;
+        |dL/dalpha| <= mag_a = T dabs + S / (1 - alpha) + T_final |bg . Gc| / (1 - alpha),
+    S = sum over later pairs of w dabs.  Its float32 error relative to mag_a is at most u (length + 3 n_p + 6 pi + 10):
+    the dot products (length u; the background's three products are formed once per pixel, within that); the unwound
+    T (2 u per step, as for the weights) and the recurrence's multiply-add per step (3 u n_p together, n_p the pixel's
+    n_contrib); the power (6 u pi, pi as in check_model) through G and alpha; and the few products that form each value
+    (10 u).  Each value is mag_a times the magnitude of its factor (G, dx, dy, the conic, the opacity), and the
+    per-Gaussian sum over its m_g pairs adds m_g u.  With K as for the identities:
+        bar_g = K u (sum_pairs mag (length + 3 n_p + 6 pi + 10) + m_g sum_pairs mag).
+    -> (ref [P, 6], bar [P, 6]) in the order mean2D x, y, conic a, b, c, opacity."""
+    W, H, HW = pairs.W, pairs.H, pairs.HW
+    sel = pairs.widx[w > 0]
+    pix, gid = pairs.pix[sel], pairs.gid[sel]
+    d, dabs = dfn(gid, pix)
+    _, counts = torch.unique_consecutive(pix, return_counts=True)
+    first = torch.repeat_interleave(torch.cumsum(counts, 0) - counts, counts)
+    last = first + torch.repeat_interleave(counts, counts) - 1
+    rec = rec.to(pix.device).double()
+    mean = rec[:, 0:2].clone().requires_grad_()
+    abc = rec[:, 4:7].clone().requires_grad_()
+    op = rec[:, 7].clone().requires_grad_()
+    dx = mean[gid, 0] - (pix % W).double()
+    dy = mean[gid, 1] - (pix // W).double()
+    a, b, c = abc[gid, 0], abc[gid, 1], abc[gid, 2]
+    G = torch.exp(-0.5 * (a * dx * dx + c * dy * dy) - b * dx * dy)
+    av = op[gid] * G
+    alpha = av - (av - ALPHA_MAX).clamp(min=0.0).detach()
+    logf = torch.log1p(-alpha)
+    T = torch.exp(_seg_excl_cumsum(logf, first))
+    L = (alpha * T * d).sum()
+    if bg_dot is not None:
+        bgd, bga = (x.to(pix.device).double().reshape(-1) for x in bg_dot)
+        T_fin = torch.exp(torch.zeros(HW, dtype=torch.float64, device=pix.device).index_add(0, pix, logf))
+        L = L + (T_fin * bgd).sum()
+    gm, gabc, gop = torch.autograd.grad(L, [mean, abc, op])
+    ref = torch.stack([gm[:, 0] * 0.5 * W, gm[:, 1] * 0.5 * H, gabc[:, 0], 0.5 * gabc[:, 1], gabc[:, 2], gop], 1)
+    with torch.no_grad():
+        al, T, G, dx, dy, a, b, c = (x.detach() for x in (alpha, T, G, dx, dy, a, b, c))
+        cs = torch.cumsum(al * T * dabs, 0)
+        mag_a = T * dabs + (cs[last] - cs) / (1 - al)
+        if bg_dot is not None:
+            mag_a = mag_a + T_fin.detach()[pix] * bga[pix] / (1 - al)
+        og = op.detach()[gid] * mag_a * G
+        mag = torch.stack([og * ((dx * a).abs() + (dy * b).abs()) * 0.5 * W,
+                           og * ((dy * c).abs() + (dx * b).abs()) * 0.5 * H,
+                           0.5 * og * dx * dx, 0.5 * og * (dx * dy).abs(), 0.5 * og * dy * dy, G * mag_a], 1)
+        pi = 0.5 * a.abs() * dx * dx + 0.5 * c.abs() * dy * dy + (b * dx * dy).abs()
+        k = length + 3 * pairs.n[pix].double() + 6 * pi + 10
+        an = torch.zeros(P, 6, dtype=torch.float64, device=pix.device).index_add_(0, gid, mag * k[:, None])
+        am = torch.zeros(P, 6, dtype=torch.float64, device=pix.device).index_add_(0, gid, mag)
+        m = torch.zeros(P, dtype=torch.float64, device=pix.device).index_add_(0, gid, torch.ones_like(k))
+        bar = K * U * (an + m[:, None] * am)
+    return ref, bar
+
+
+def geom6(mean2D, conic, opacity):
+    """The composite's six geometric gradients in composite_model's order."""
+    return torch.stack([mean2D[:, 0], mean2D[:, 1], conic[:, 0], conic[:, 1], conic[:, 3], opacity.reshape(-1)], 1)
+
+
 def upstream(H, W, C, seed, dynamic=False):
     """Random upstream gradients (dL/dcolor [3,H,W], dL/dfeature [C,H,W], dL/ddepth [1,H,W]), float32 N(0, 1); dynamic:
     every pixel scaled by 10^U(-6, 0), the range across pixels that a scene-scaled floor hides."""

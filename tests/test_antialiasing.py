@@ -20,6 +20,7 @@ import torch
 
 import camera_grad_model as cgm
 import scenegen
+from camera_grad_model import cov3d_from_scale_rot
 
 torch.set_default_dtype(torch.float32)
 MIN_RATIO = 2.5e-5
@@ -27,20 +28,6 @@ F32, F16 = 0, 1
 
 
 # ------------------------------------------------------------------------------------------------------------ model
-def cov3d_from_scale_rot(scales, rotations, mod=1.0):
-    """Float64 torch twin of the forward's computeCov3D ([P,6] upper triangle), differentiable.  Rc[:, i] is column i of
-    the forward's GLM rotation; GLM's M = S R has M[c][r] = s[r] Rc[c][r], and Sigma = M^T M has
-    Sigma[i][j] = sum_k s_k^2 Rc[i][k] Rc[j][k]."""
-    s = scales * mod
-    r, x, y, z = rotations.unbind(1)
-    Rc = torch.stack([torch.stack([1 - 2 * (y * y + z * z), 2 * (x * y - r * z), 2 * (x * z + r * y)], -1),
-                      torch.stack([2 * (x * y + r * z), 1 - 2 * (x * x + z * z), 2 * (y * z - r * x)], -1),
-                      torch.stack([2 * (x * z - r * y), 2 * (y * z + r * x), 1 - 2 * (x * x + y * y)], -1)], 1)
-    M = Rc * s[:, None, :]
-    S = M @ M.transpose(1, 2)
-    return torch.stack([S[:, 0, 0], S[:, 0, 1], S[:, 0, 2], S[:, 1, 1], S[:, 1, 2], S[:, 2, 2]], 1)
-
-
 def aa_quantities(means3D, cov3D, opacity, vm, pm, campos, W, H, tanfovx, tanfovy, deg=0, shs=None, colors=None):
     """-> (ndc [P,2], conic (A, B, C), op_eff [P], colour [P,3], depth [P], (a0, b, c0)), float64, differentiable.  The
     conventions (clamped Jacobian entries detached, 1e-7 in the screen mean, the conic's 1/(det^2 + 1e-7)) are

@@ -8,7 +8,7 @@ and no background.  So with colours_precomp = X, features = X (or k stacked copi
 backward of (dL/dpix = G, dL/dfeature = 0), camera included.
 
 The independent oracle is a float64 torch autograd model of the term over the composite's own records and blended
-pairs (_feature_model), with a per-Gaussian bar derived as in blend_weights.py; a dropped pair exceeds it.
+pairs (blend_weights.composite_model), with a per-Gaussian bar derived there; a dropped pair exceeds it.
 
 CPU: the entries' argument checks.  GPU: the model against generic random features at C = 1, 5, 40, 130, 132 (scalar and
 16-byte row loads, the 32-, 64- and 128-channel kernels), with the camera gradient against camera_grad_model; the
@@ -229,68 +229,17 @@ def _identity_scene(name):
 
 
 def _feature_model(view, dfn, C):
-    """Float64 model of the feature term's geometric gradients on a view of test_blend_weights.DeviceView, over the
-    composite's own records and its blended pairs (extracted W > 0) in its own pair order.
-
-    dfn(gid, pix) -> (d, dabs): per blended pair the dot product d = f_gid . G_pix of the float32 inputs in float64, and
-    sum_c |f_gid,c G_pix,c|.  The model is L = sum_pairs alpha T d with alpha = min(0.99, op exp(power)) (the clamp
-    passes the gradient through, as in the composite) and T the product of (1 - alpha) over the pixel's earlier
-    blended pairs; torch autograd gives dL/dmean2D, dL/dconic and dL/dopacity, mapped to the composite's conventions
-    (the mean gradient times W / 2 and H / 2, half the off-diagonal conic gradient).
-
-    Bar (per Gaussian and value, in the form of blend_weights.gaussian_ratio).  Per pair, the composite forms
-    dL/dalpha = T (d - A) with A the back-to-front recurrence over the pixel's later pairs, |T (d - A)| <= mag_a =
-    T dabs + S / (1 - alpha), S = sum over later pairs of w dabs.  Its float32 error relative to mag_a is at most
-        u (C + 3 n_p + 6 pi + 10):
-    the C-term dot product (C u); the unwound T (2 u per step, blend_weights) and the recurrence's multiply-add per step
-    (3 u n_p together, n_p the pixel's n_contrib); the power (6 u pi, pi as in blend_weights) through G and alpha; and
-    the few products that form each value (10 u).  Each value is mag_a times the magnitude of its factor (G, dx, dy,
-    the conic, the opacity), and the per-Gaussian sum over its m_g pairs adds m_g u.  With K = 4 as in blend_weights:
-        bar_g = K u (sum_pairs mag (C + 3 n_p + 6 pi + 10) + m_g sum_pairs mag).
-    -> (ref [P, 6], bar [P, 6]) in the order mean2D x, y, conic a, b, c, opacity."""
+    """blend_weights.composite_model of the feature term (no background) on a view of test_blend_weights.DeviceView."""
     import blend_weights as bw
 
-    pr, W, H, P = view.pairs, view.W, view.H, view.P
-    sel = pr.widx[view.w > 0]
-    pix, gid = pr.pix[sel], pr.gid[sel]
-    d, dabs = dfn(gid, pix)
-    _, counts = torch.unique_consecutive(pix, return_counts=True)
-    first = torch.repeat_interleave(torch.cumsum(counts, 0) - counts, counts)
-    last = first + torch.repeat_interleave(counts, counts) - 1
-    rec = view.base["rec"].to(pix.device).double()
-    mean = rec[:, 0:2].clone().requires_grad_()
-    abc = rec[:, 4:7].clone().requires_grad_()
-    op = rec[:, 7].clone().requires_grad_()
-    dx = mean[gid, 0] - (pix % W).double()
-    dy = mean[gid, 1] - (pix // W).double()
-    a, b, c = abc[gid, 0], abc[gid, 1], abc[gid, 2]
-    G = torch.exp(-0.5 * (a * dx * dx + c * dy * dy) - b * dx * dy)
-    av = op[gid] * G
-    alpha = av - (av - bw.ALPHA_MAX).clamp(min=0.0).detach()
-    T = torch.exp(bw._seg_excl_cumsum(torch.log1p(-alpha), first))
-    gm, gabc, gop = torch.autograd.grad((alpha * T * d).sum(), [mean, abc, op])
-    ref = torch.stack([gm[:, 0] * 0.5 * W, gm[:, 1] * 0.5 * H, gabc[:, 0], 0.5 * gabc[:, 1], gabc[:, 2], gop], 1)
-    with torch.no_grad():
-        al, T, G, dx, dy, a, b, c = (x.detach() for x in (alpha, T, G, dx, dy, a, b, c))
-        cs = torch.cumsum(al * T * dabs, 0)
-        mag_a = T * dabs + (cs[last] - cs) / (1 - al)
-        og = op.detach()[gid] * mag_a * G
-        mag = torch.stack([og * ((dx * a).abs() + (dy * b).abs()) * 0.5 * W,
-                           og * ((dy * c).abs() + (dx * b).abs()) * 0.5 * H,
-                           0.5 * og * dx * dx, 0.5 * og * (dx * dy).abs(), 0.5 * og * dy * dy, G * mag_a], 1)
-        pi = 0.5 * a.abs() * dx * dx + 0.5 * c.abs() * dy * dy + (b * dx * dy).abs()
-        k = C + 3 * pr.n[pix].double() + 6 * pi + 10
-        an = torch.zeros(P, 6, dtype=torch.float64, device=pix.device).index_add_(0, gid, mag * k[:, None])
-        am = torch.zeros(P, 6, dtype=torch.float64, device=pix.device).index_add_(0, gid, mag)
-        m = torch.zeros(P, dtype=torch.float64, device=pix.device).index_add_(0, gid, torch.ones_like(k))
-        bar = bw.K * bw.U * (an + m[:, None] * am)
-    return ref, bar
+    return bw.composite_model(view.pairs, view.w, view.base["rec"], view.P, dfn, C)
 
 
 def _geom6(o):
-    """The composite's six geometric gradients of an _assign result, in _feature_model's order."""
-    return torch.stack([o["mean2D"][:, 0], o["mean2D"][:, 1], o["conic"][:, 0], o["conic"][:, 1], o["conic"][:, 3],
-                        o["opacity"][:, 0]], 1)
+    """The composite's six geometric gradients of an _assign result, in composite_model's order."""
+    import blend_weights as bw
+
+    return bw.geom6(o["mean2D"], o["conic"], o["opacity"])
 
 
 def _model_ratio(ours, ref, bar):
