@@ -249,8 +249,10 @@ int f3dgs_get_layout(int P, int width, int height, int R, f3dgs_layout* out) {
 
 namespace {
 
-// Shared body of f3dgs_forward (TF = float), f3dgs_forward_f16 (TF = __half) and f3dgs_forward_antialiased: TF is the
-// element type of semantic_feature and out_feature_map only.  antialiasing: op_eff = opacity * rho in the records.
+// Shared body of f3dgs_forward (TF = float), f3dgs_forward_f16 (TF = __half), f3dgs_forward_antialiased and
+// f3dgs_forward_alpha_invdepth: TF is the element type of semantic_feature and out_feature_map only.  antialiasing:
+// op_eff = opacity * rho in the records.  out_alpha / out_invdepth (f3dgs_forward_alpha_invdepth, which has checked that
+// both are given): the composite also writes the opacity and inverse-depth planes.
 template <typename TF>
 int forward_impl(const char* entry, f3dgs_alloc_fn geometry_alloc, void* geometry_ctx, f3dgs_alloc_fn binning_alloc,
                  void* binning_ctx, f3dgs_alloc_fn image_alloc, void* image_ctx, int P, int D, int M, int C,
@@ -259,7 +261,7 @@ int forward_impl(const char* entry, f3dgs_alloc_fn geometry_alloc, void* geometr
                  float scale_modifier, const float* rotations, const float* cov3D_precomp, const float* viewmatrix,
                  const float* projmatrix, const float* cam_pos, float tan_fovx, float tan_fovy, int prefiltered,
                  float* out_color, TF* out_feature_map, float* out_depth, int* radii, int debug, void* cuda_stream,
-                 bool antialiasing = false) {
+                 bool antialiasing = false, float* out_alpha = nullptr, float* out_invdepth = nullptr) {
     const Api api(entry);
     cudaStream_t stream = (cudaStream_t)cuda_stream;
     if (P < 0 || width <= 0 || height <= 0 || C < 0 || C > F3DGS_MAX_FEATURE_DIM || D < 0 || D > 3)
@@ -277,6 +279,14 @@ int forward_impl(const char* entry, f3dgs_alloc_fn geometry_alloc, void* geometr
     if (C > 0 && (!semantic_feature || !out_feature_map))
         return api.invalid("C > 0 needs semantic_feature and out_feature_map");
     if (shs && M < (D + 1) * (D + 1)) return api.invalid("M < (D+1)^2 SH coefficients");
+    if (out_alpha) {  // the composite writes the planes while it writes the other outputs
+        const size_t hw4 = (size_t)width * height * 4;
+        const Range a{out_alpha, hw4}, i{out_invdepth, hw4};
+        const Range outs[] = {{out_color, 3 * hw4}, {out_feature_map, (size_t)C * width * height * sizeof(TF)},
+                              {out_depth, hw4}, {radii, (size_t)P * 4}};
+        if (overlaps(a, outs) || overlaps(i, outs) || overlaps(a, {i}))
+            return api.invalid("out_alpha / out_invdepth overlap another output");
+    }
 
     const ViewParams vp = make_view(P, D, M, C, width, height, tan_fovx, tan_fovy, scale_modifier, viewmatrix,
                                     projmatrix, cam_pos);
@@ -370,7 +380,7 @@ int forward_impl(const char* entry, f3dgs_alloc_fn geometry_alloc, void* geometr
         StageTimer t(F3DGS_STAGE_COMPOSITE_FWD, stream);
         int* counters = reinterpret_cast<int*>(img + il.counters);
         e = launch_composite_fwd(vp, ranges, point_list, rec, semantic_feature, background, final_T, n_contrib,
-                                 out_color, out_feature_map, out_depth, counters, stream);
+                                 out_color, out_feature_map, out_depth, counters, stream, out_alpha, out_invdepth);
     }
     if (const int rc = api.cuda(e, "composite_fwd launch")) return rc;
     STAGE_CHECK("composite_fwd");
@@ -433,6 +443,31 @@ int f3dgs_forward_antialiased(f3dgs_alloc_fn geometry_alloc, void* geometry_ctx,
     return Api(__func__).invalid("unknown dtype code");
 }
 
+int f3dgs_forward_alpha_invdepth(f3dgs_alloc_fn geometry_alloc, void* geometry_ctx, f3dgs_alloc_fn binning_alloc,
+                                 void* binning_ctx, f3dgs_alloc_fn image_alloc, void* image_ctx, int P, int D, int M,
+                                 int C, const float* background, int width, int height, const float* means3D,
+                                 const float* shs, const float* colors_precomp, const void* semantic_feature,
+                                 int semantic_feature_dtype, const float* opacities, const float* scales,
+                                 float scale_modifier, const float* rotations, const float* cov3D_precomp,
+                                 const float* viewmatrix, const float* projmatrix, const float* cam_pos,
+                                 float tan_fovx, float tan_fovy, int prefiltered, float* out_color,
+                                 void* out_feature_map, float* out_depth, int* radii, int debug, void* cuda_stream,
+                                 int antialiasing, float* out_alpha, float* out_invdepth) {
+    const char* entry = __func__;
+    if (!out_alpha || !out_invdepth) return Api(entry).invalid("NULL out_alpha / out_invdepth");
+    const auto run = [&](auto* features) {
+        using TF = std::remove_const_t<std::remove_pointer_t<decltype(features)>>;
+        return forward_impl(entry, geometry_alloc, geometry_ctx, binning_alloc, binning_ctx, image_alloc, image_ctx,
+                            P, D, M, C, background, width, height, means3D, shs, colors_precomp, features, opacities,
+                            scales, scale_modifier, rotations, cov3D_precomp, viewmatrix, projmatrix, cam_pos, tan_fovx,
+                            tan_fovy, prefiltered, out_color, static_cast<TF*>(out_feature_map), out_depth, radii,
+                            debug, cuda_stream, antialiasing != 0, out_alpha, out_invdepth);
+    };
+    if (semantic_feature_dtype == F3DGS_F32) return run(static_cast<const float*>(semantic_feature));
+    if (semantic_feature_dtype == F3DGS_F16) return run(static_cast<const __half*>(semantic_feature));
+    return Api(entry).invalid("unknown dtype code");
+}
+
 }  // extern "C"
 
 namespace {
@@ -458,7 +493,9 @@ struct ScratchLayout {  // per-view intermediates of the accumulating backward (
 // (the _antialiased entries): the forward's records hold op_eff = opacity * rho, so the composite's opacity gradient is
 // dL/dop_eff and the preprocess backward turns it into dL/dopacity (and rho's geometric terms).  The assigning backward
 // lets the composite write into dL_dopacity and rescales it in place; the accumulating one needs dL/dop_eff of this view
-// alone, so the composite writes into P zeroed floats of the device's default memory pool.
+// alone, so the composite writes into P zeroed floats of the device's default memory pool.  dL_dalpha / dL_dinvdepth
+// (the _alpha_invdepth entries, which have checked that both are given): the gradients of the forward's opacity and
+// inverse-depth planes, added to dL/dalpha and dL/dz by the composite.
 template <typename TG>
 int backward_impl(const Api& api, bool accumulate, int P, int D, int M, int R, int C, const float* background, int width,
                   int height, const float* means3D, const float* shs, const float* scales, float scale_modifier,
@@ -469,7 +506,8 @@ int backward_impl(const Api& api, bool accumulate, int P, int D, int M, int R, i
                   float* dL_dopacity, float* dL_dcolor, float* dL_dsemantic_feature, float* dL_dmean3D, float* dL_dcov3D,
                   float* dL_dsh, float* dL_dscale, float* dL_drot, float* dL_dz, float* grad_accum, float* denom,
                   float* dL_dcamera, cudaEvent_t composite_done, int debug, cudaStream_t stream,
-                  const Range& zero = {nullptr, 0}, const FeatureRows& feat = {}, bool antialiasing = false) {
+                  const Range& zero = {nullptr, 0}, const FeatureRows& feat = {}, bool antialiasing = false,
+                  const float* dL_dalpha = nullptr, const float* dL_dinvdepth = nullptr) {
     if (P < 0 || width <= 0 || height <= 0 || C < 0 || C > F3DGS_MAX_FEATURE_DIM || R < 0)
         return api.invalid("bad sizes");
     if (P == 0) return 0;
@@ -516,6 +554,16 @@ int backward_impl(const Api& api, bool accumulate, int P, int D, int M, int R, i
                               zero};
         if (overlaps({dL_dopacity, p4}, outs)) return api.invalid("dL_dopacity overlaps another output");
     }
+    if (dL_dalpha) {  // read by the composite while it reduces into the outputs
+        const size_t p4 = (size_t)P * 4, hw4 = (size_t)width * height * 4;
+        const Range outs[] = {{dL_dmean2D, 3 * p4}, {dL_dconic, 4 * p4}, {dL_dopacity, p4}, {dL_dcolor, 3 * p4},
+                              {dL_dsemantic_feature, (size_t)C * p4}, {dL_dmean3D, 3 * p4}, {dL_dcov3D, 6 * p4},
+                              {dL_dsh, (size_t)M * 3 * p4}, {dL_dscale, 3 * p4}, {dL_drot, 4 * p4}, {dL_dz, p4},
+                              {grad_accum, p4}, {denom, p4}, {dL_dcamera, F3DGS_CAMERA_GRAD_FLOATS * sizeof(float)},
+                              zero};
+        if (overlaps({dL_dalpha, hw4}, outs) || overlaps({dL_dinvdepth, hw4}, outs))
+            return api.invalid("dL_dalpha / dL_dinvdepth overlap an output");
+    }
     if (zero.p) CUDA_TRY(cudaMemsetAsync(const_cast<void*>(zero.p), 0, zero.bytes, stream));
 
     const ViewParams vp = make_view(P, D, M, C, width, height, tan_fovx, tan_fovy, scale_modifier, viewmatrix,
@@ -547,7 +595,8 @@ int backward_impl(const Api& api, bool accumulate, int P, int D, int M, int R, i
         StageTimer t(F3DGS_STAGE_COMPOSITE_BWD, stream);
         e = launch_composite_bwd(vp, forward_buffers(vp, R, geom_buffer, binning_buffer, image_buffer), background,
                                  dL_dpix, dL_depths, dL_dfeaturepix, dL_dfeaturepix_scale, dL_dmean2D, dL_dconic,
-                                 dL_dop_eff, dL_dcolor, dL_dz, dL_dsemantic_feature, stream, feat);
+                                 dL_dop_eff, dL_dcolor, dL_dz, dL_dsemantic_feature, stream, feat, dL_dalpha,
+                                 dL_dinvdepth);
     }
     if (const int rc = composite_bwd_result(api, e, "composite_bwd launch")) return rc;
     STAGE_CHECK("composite_bwd");
@@ -675,7 +724,8 @@ int backward_accum_impl(const char* entry, int P, int D, int M, int R, int C, co
                         float* dL_dsemantic_feature, float* dL_dmean3D, float* dL_dcov3D_precomp, float* dL_dsh,
                         float* dL_dscale, float* dL_drot, float* dL_dmean2D_out, float* grad_accum, float* denom,
                         void* composite_done_event, int debug, void* cuda_stream, bool camera = false,
-                        float* dL_dcamera = nullptr, const FeatureRows& feat = {}, bool antialiasing = false) {
+                        float* dL_dcamera = nullptr, const FeatureRows& feat = {}, bool antialiasing = false,
+                        const float* dL_dalpha = nullptr, const float* dL_dinvdepth = nullptr) {
     const Api api(entry);
     cudaStream_t stream = (cudaStream_t)cuda_stream;
     if (camera && !dL_dcamera) return api.invalid("NULL dL_dcamera");
@@ -685,6 +735,10 @@ int backward_accum_impl(const char* entry, int P, int D, int M, int R, int C, co
         return api.invalid("dL_dcamera overlaps another output");
     if (overlaps({feat.rows, (size_t)P * C * (feat.f16 ? 2 : 4)}, {{dL_dmean2D_out, (size_t)P * 3 * 4}}))
         return api.invalid("semantic_feature overlaps an output");
+    const size_t hw4 = (size_t)width * height * 4;
+    if (overlaps({dL_dalpha, hw4}, {{dL_dmean2D_out, (size_t)P * 3 * 4}}) ||
+        overlaps({dL_dinvdepth, hw4}, {{dL_dmean2D_out, (size_t)P * 3 * 4}}))
+        return api.invalid("dL_dalpha / dL_dinvdepth overlap an output");
     if ((colors_precomp != nullptr) != (dL_dcolors_precomp != nullptr) ||
         (cov3D_precomp != nullptr) != (dL_dcov3D_precomp != nullptr))
         return api.invalid("dL_dcolors_precomp / dL_dcov3D_precomp go with colors_precomp / cov3D_precomp");
@@ -699,7 +753,8 @@ int backward_accum_impl(const char* entry, int P, int D, int M, int R, int C, co
         binning_buffer, image_buffer, dL_dpix, dL_dfeaturepix, dL_dfeaturepix_scale, dL_depths, m2d,
         reinterpret_cast<float*>(scratch + sl.conic), dL_dopacity, dcol, dL_dsemantic_feature, dL_dmean3D, dcov, dL_dsh,
         dL_dscale, dL_drot, reinterpret_cast<float*>(scratch + sl.dz), grad_accum, denom, dL_dcamera,
-        (cudaEvent_t)composite_done_event, debug, stream, {scratch, sl.bytes}, feat, antialiasing);
+        (cudaEvent_t)composite_done_event, debug, stream, {scratch, sl.bytes}, feat, antialiasing, dL_dalpha,
+        dL_dinvdepth);
     if (rc < 0) return rc;
     if (dL_dmean2D_out)
         CUDA_TRY(cudaMemcpyAsync(dL_dmean2D_out, m2d, (size_t)P * 3 * sizeof(float), cudaMemcpyDeviceToDevice, stream));
@@ -918,6 +973,73 @@ int f3dgs_backward_accum_antialiased(
                                    dL_dmean3D, dL_dcov3D_precomp, dL_dsh, dL_dscale, dL_drot, dL_dmean2D_out,
                                    grad_accum, denom, composite_done_event, debug, cuda_stream, false, dL_dcamera,
                                    feat, true);
+    };
+    if (dL_dfeaturepix_dtype == F3DGS_F16)
+        return run(static_cast<const __half*>(dL_dfeaturepix), dL_dfeaturepix_scale);
+    return run(static_cast<const float*>(dL_dfeaturepix), 1.f);
+}
+
+int f3dgs_backward_alpha_invdepth(int P, int D, int M, int R, int C, const float* background, int width, int height,
+                                  const float* means3D, const float* shs, const float* colors_precomp,
+                                  const void* semantic_feature, int semantic_feature_dtype, const float* scales,
+                                  float scale_modifier, const float* rotations, const float* cov3D_precomp,
+                                  const float* viewmatrix, const float* projmatrix, const float* cam_pos,
+                                  float tan_fovx, float tan_fovy, const int* radii, char* geom_buffer,
+                                  char* binning_buffer, char* image_buffer, const float* dL_dpix,
+                                  const void* dL_dfeaturepix, int dL_dfeaturepix_dtype, float dL_dfeaturepix_scale,
+                                  const float* dL_depths, float* dL_dmean2D, float* dL_dconic, float* dL_dopacity,
+                                  float* dL_dcolor, float* dL_dsemantic_feature, float* dL_dmean3D, float* dL_dcov3D,
+                                  float* dL_dsh, float* dL_dscale, float* dL_drot, float* dL_dz, int debug,
+                                  void* cuda_stream, float* dL_dcamera, int antialiasing, const float* dL_dalpha,
+                                  const float* dL_dinvdepth) {
+    (void)colors_precomp;
+    const Api api(__func__);
+    if (!dL_dalpha || !dL_dinvdepth) return api.invalid("NULL dL_dalpha / dL_dinvdepth");
+    FeatureRows feat;
+    if (const int rc =
+            feature_rows(api, C, semantic_feature, semantic_feature_dtype, dL_dfeaturepix_dtype, feat, true))
+        return rc;
+    const auto run = [&](auto map, float scale) {
+        return backward_impl(api, false, P, D, M, R, C, background, width, height, means3D, shs, scales,
+                             scale_modifier, rotations, cov3D_precomp, viewmatrix, projmatrix, cam_pos, tan_fovx,
+                             tan_fovy, radii, geom_buffer, binning_buffer, image_buffer, dL_dpix, map, scale, dL_depths,
+                             dL_dmean2D, dL_dconic, dL_dopacity, dL_dcolor, dL_dsemantic_feature, dL_dmean3D, dL_dcov3D,
+                             dL_dsh, dL_dscale, dL_drot, dL_dz, nullptr, nullptr, dL_dcamera, nullptr, debug,
+                             (cudaStream_t)cuda_stream, {nullptr, 0}, feat, antialiasing != 0, dL_dalpha,
+                             dL_dinvdepth);
+    };
+    if (dL_dfeaturepix_dtype == F3DGS_F16)
+        return run(static_cast<const __half*>(dL_dfeaturepix), dL_dfeaturepix_scale);
+    return run(static_cast<const float*>(dL_dfeaturepix), 1.f);
+}
+
+int f3dgs_backward_accum_alpha_invdepth(
+    int P, int D, int M, int R, int C, const float* background, int width, int height, const float* means3D,
+    const float* shs, const float* colors_precomp, const void* semantic_feature, int semantic_feature_dtype,
+    const float* scales, float scale_modifier, const float* rotations, const float* cov3D_precomp,
+    const float* viewmatrix, const float* projmatrix, const float* cam_pos, float tan_fovx, float tan_fovy,
+    const int* radii, char* geom_buffer, char* binning_buffer, char* image_buffer, const float* dL_dpix,
+    const void* dL_dfeaturepix, int dL_dfeaturepix_dtype, float dL_dfeaturepix_scale, const float* dL_depths,
+    char* scratch, float* dL_dopacity, float* dL_dcolors_precomp, float* dL_dsemantic_feature, float* dL_dmean3D,
+    float* dL_dcov3D_precomp, float* dL_dsh, float* dL_dscale, float* dL_drot, float* dL_dmean2D_out,
+    float* grad_accum, float* denom, void* composite_done_event, int debug, void* cuda_stream, float* dL_dcamera,
+    int antialiasing, const float* dL_dalpha, const float* dL_dinvdepth) {
+    const char* entry = __func__;
+    if (!dL_dalpha || !dL_dinvdepth) return Api(entry).invalid("NULL dL_dalpha / dL_dinvdepth");
+    FeatureRows feat;
+    if (const int rc = feature_rows(Api(entry), C, semantic_feature, semantic_feature_dtype, dL_dfeaturepix_dtype,
+                                    feat, true))
+        return rc;
+    if (antialiasing && P > 0 && overlaps({dL_dopacity, (size_t)P * 4}, {{dL_dmean2D_out, (size_t)P * 3 * 4}}))
+        return Api(entry).invalid("dL_dopacity overlaps another output");
+    const auto run = [&](auto map, float scale) {
+        return backward_accum_impl(entry, P, D, M, R, C, background, width, height, means3D, shs, colors_precomp,
+                                   scales, scale_modifier, rotations, cov3D_precomp, viewmatrix, projmatrix, cam_pos,
+                                   tan_fovx, tan_fovy, radii, geom_buffer, binning_buffer, image_buffer, dL_dpix, map,
+                                   scale, dL_depths, scratch, dL_dopacity, dL_dcolors_precomp, dL_dsemantic_feature,
+                                   dL_dmean3D, dL_dcov3D_precomp, dL_dsh, dL_dscale, dL_drot, dL_dmean2D_out,
+                                   grad_accum, denom, composite_done_event, debug, cuda_stream, false, dL_dcamera,
+                                   feat, antialiasing != 0, dL_dalpha, dL_dinvdepth);
     };
     if (dL_dfeaturepix_dtype == F3DGS_F16)
         return run(static_cast<const __half*>(dL_dfeaturepix), dL_dfeaturepix_scale);

@@ -19,6 +19,12 @@
 //       replaced each list entry's weights by the pair dot products d_ip = f_i . dL/dF_p; this walk repeats EMIT's, so a
 //       pair's entry is the one EMIT wrote for it, and runs the colour term's scalar recurrence on d (no background:
 //       the feature map has none), reducing the six geometric values into the same dL_dmean2D / dL_dconic / dL_dopacity.
+//   PLANES         (GEOM and EMIT, opt-in) the gradients gA = dL/dA_p and gI = dL/dI_p of the forward's opacity plane
+//       A_p = 1 - T_final and inverse-depth plane I_p = sum_i w_i / z_i.  dA/dalpha_i = T_final / (1 - alpha_i) is the
+//       background term's factor, so gA joins it as bg.dL/dpix - gA; I gets the depth term's recurrence with 1/z_i in
+//       place of z_i (dL/dI_p and one more float per lane), and dL/dz_i gains -w_i gI / z_i^2 in the same reduced value.
+//       The walk reads only what every forward stores (records, final_T, n_contrib), and with gA = gI = 0 each added
+//       term is an exact zero, so every output is bitwise that of the walk without PLANES.
 // 12 warps and a ring without weight slots (RingSlim, 113 KB of shared memory with the reduction tiles): two CTAs per SM,
 // and the alpha warps keep the launch register count (80).
 // As in the reference, the feature loss does not feed dL/dalpha (backward.cu:575 is disabled) unless FEAT is asked for.
@@ -57,6 +63,8 @@ struct BwdArgs {
     float* dL_dz;        // [P]
     InstanceLists lists;  // EMIT and LIFT; w = alpha * T with the backward's unwound T.  FEAT: w = d_ip, read only
     float* weight_sum;    // LIFT: [P] += sum over the view's pixels of w
+    const float* dL_dalpha;     // PLANES: [H,W] gA
+    const float* dL_dinvdepth;  // PLANES: [H,W] gI
 };
 
 // GEOM: geometric gradients; EMIT: and the feature lists; LIFT: the feature lists and the per-Gaussian weight sums;
@@ -85,7 +93,7 @@ __device__ __forceinline__ float* geom_dst(const BwdArgs& args, int v, uint32_t 
     }
 }
 
-template <BwdMode MODE>
+template <BwdMode MODE, bool PLANES = false>
 __global__ void __launch_bounds__(kBwdThreads, kSlimCtas)
 composite_bwd_kernel(const BwdArgs args) {
     constexpr bool EMIT = MODE != BwdMode::GEOM;
@@ -120,6 +128,7 @@ composite_bwd_kernel(const BwdArgs args) {
     struct Px {
         float T, T_final, pxf, pyf, fbx0, fby0, dLp0, dLp1, dLp2, dLd, bg_dot;
         float ar0, ar1, ar2, lc0, lc1, lc2, last_alpha, accum_depth, last_depth;
+        float gI, accum_invd;  // PLANES: dL/dI_p, and the 1/z recurrence's value for the pair the walk reaches next
         uint32_t last_contrib, wmax;
         bool inside;
     } p = Px{};
@@ -186,6 +195,11 @@ composite_bwd_kernel(const BwdArgs args) {
                     p.dLd = args.dL_ddepth[pix];
                 }
                 p.bg_dot = args.bg[0] * p.dLp0 + args.bg[1] * p.dLp1 + args.bg[2] * p.dLp2;
+                if constexpr (PLANES) {
+                    p.gI = p.inside ? args.dL_dinvdepth[pix] : 0.f;
+                    p.bg_dot -= p.inside ? args.dL_dalpha[pix] : 0.f;
+                    p.accum_invd = 0.f;
+                }
             }
             p.ar0 = p.ar1 = p.ar2 = p.lc0 = p.lc1 = p.lc2 = 0.f;
             p.last_alpha = p.accum_depth = p.last_depth = 0.f;
@@ -267,6 +281,15 @@ composite_bwd_kernel(const BwdArgs args) {
                         p.accum_depth = p.last_alpha * p.last_depth + (1.f - p.last_alpha) * p.accum_depth;
                         p.last_depth = r2.w;
                         dL_dalpha += (r2.w - p.accum_depth) * p.dLd;
+                        float dLdz = p.dLd;
+                        if constexpr (PLANES) {
+                            // the depth term's recurrence with 1/z, advanced right away (the depth term advances it
+                            // at the next pair, from last_alpha and last_depth): one register fewer
+                            const float rz = __frcp_rn(r2.w);
+                            dL_dalpha += (rz - p.accum_invd) * p.gI;
+                            p.accum_invd = alpha * rz + (1.f - alpha) * p.accum_invd;
+                            dLdz -= p.gI * (rz * rz);  // dI/dz_i = -w_i / z_i^2
+                        }
                         dL_dalpha *= p.T;
                         p.last_alpha = alpha;
                         dL_dalpha += (-p.T_final * inv_1ma) * p.bg_dot;
@@ -281,7 +304,7 @@ composite_bwd_kernel(const BwdArgs args) {
                         v[3] = -0.5f * gdx * dy * dL_dG;
                         v[4] = -0.5f * gdy * dy * dL_dG;
                         v[5] = Gs * dL_dalpha;
-                        v[6] = wgt * p.dLd;
+                        v[6] = wgt * dLdz;
                     }
                     const uint32_t pm = __ballot_sync(0xffffffffu, contrib);
                     if (pm) {
@@ -344,7 +367,7 @@ static cudaError_t alloc_lists(size_t R, size_t tiles, char** mem, InstanceLists
 // feature_bwd over them, reducing sum_p w * scale * map[:, p] into dst.  `a` brings the mode's outputs.  With features
 // (EMIT only), feature_dot then turns the lists' weights into pair dot products and the FEAT walk adds the feature term
 // to the geometric gradients; the lists are freed after it.
-template <BwdMode MODE, typename TG>
+template <BwdMode MODE, typename TG, bool PLANES = false>
 static cudaError_t run_bwd(BwdArgs a, const ViewParams& vp, const ForwardBuffers& fb, const TG* map, float scale,
                            float* dst, cudaStream_t s, const FeatureRows& feat = {}) {
     a.pa = producer_args(vp, fb.ranges, fb.point_list, fb.rec, fb.n_contrib, fb.counters + kCounterBwdGeom);
@@ -357,7 +380,8 @@ static cudaError_t run_bwd(BwdArgs a, const ViewParams& vp, const ForwardBuffers
     // every instantiation is opted in to the shared memory it needs on the first launch of any of them on a device
     int num_sms = 0;
     cudaError_t e = device_sms<composite_bwd_kernel<BwdMode::GEOM>, composite_bwd_kernel<BwdMode::EMIT>,
-                               composite_bwd_kernel<BwdMode::LIFT>, composite_bwd_kernel<BwdMode::FEAT>>(
+                               composite_bwd_kernel<BwdMode::LIFT>, composite_bwd_kernel<BwdMode::FEAT>,
+                               composite_bwd_kernel<BwdMode::GEOM, true>, composite_bwd_kernel<BwdMode::EMIT, true>>(
         num_sms, sizeof(BwdSmem), kBwdThreads, kSlimCtas);
     const int grid = min(a.pa.num_tiles, kSlimCtas * num_sms);
     auto walk = [&](void (*kernel)(BwdArgs)) {
@@ -367,7 +391,7 @@ static cudaError_t run_bwd(BwdArgs a, const ViewParams& vp, const ForwardBuffers
         g_launches++;
         return cudaGetLastError();
     };
-    if (e == cudaSuccess) e = walk(composite_bwd_kernel<MODE>);
+    if (e == cudaSuccess) e = walk(composite_bwd_kernel<MODE, PLANES>);
     if (MODE != BwdMode::GEOM) {
         if (e == cudaSuccess) e = launch_feature_bwd(vp, fb.ranges, a.lists, map, scale, dst, fb.counters, s);
         if (MODE == BwdMode::EMIT && feat.rows) {
@@ -383,12 +407,16 @@ template <typename TG>
 cudaError_t launch_composite_bwd(const ViewParams& vp, const ForwardBuffers& fb, const float* bg, const float* dL_dpix,
                                  const float* dL_ddepth, const TG* dL_dfeat_pix, float dL_dfeat_pix_scale,
                                  float* dL_dmean2D, float* dL_dconic, float* dL_dopacity, float* dL_dcolor, float* dL_dz,
-                                 float* dL_dfeature, cudaStream_t s, const FeatureRows& feat) {
+                                 float* dL_dfeature, cudaStream_t s, const FeatureRows& feat, const float* dL_dalpha,
+                                 const float* dL_dinvdepth) {
     BwdArgs a{};
     a.bg = bg; a.dL_dpix = dL_dpix; a.dL_ddepth = dL_ddepth;
     a.dL_dmean2D = dL_dmean2D; a.dL_dconic = dL_dconic; a.dL_dopacity = dL_dopacity; a.dL_dcolor = dL_dcolor;
     a.dL_dz = dL_dz;
-    const auto run = vp.C > 0 && fb.R > 0 ? run_bwd<BwdMode::EMIT, TG> : run_bwd<BwdMode::GEOM, TG>;
+    a.dL_dalpha = dL_dalpha; a.dL_dinvdepth = dL_dinvdepth;
+    const bool emit = vp.C > 0 && fb.R > 0;
+    const auto run = dL_dalpha ? (emit ? run_bwd<BwdMode::EMIT, TG, true> : run_bwd<BwdMode::GEOM, TG, true>)
+                               : (emit ? run_bwd<BwdMode::EMIT, TG> : run_bwd<BwdMode::GEOM, TG>);
     return run(a, vp, fb, dL_dfeat_pix, dL_dfeat_pix_scale, dL_dfeature, s, feat);
 }
 
@@ -402,10 +430,10 @@ cudaError_t launch_feature_lift(const ViewParams& vp, const ForwardBuffers& fb, 
 
 template cudaError_t launch_composite_bwd(const ViewParams&, const ForwardBuffers&, const float*, const float*,
                                           const float*, const float*, float, float*, float*, float*, float*, float*,
-                                          float*, cudaStream_t, const FeatureRows&);
+                                          float*, cudaStream_t, const FeatureRows&, const float*, const float*);
 template cudaError_t launch_composite_bwd(const ViewParams&, const ForwardBuffers&, const float*, const float*,
                                           const float*, const __half*, float, float*, float*, float*, float*, float*,
-                                          float*, cudaStream_t, const FeatureRows&);
+                                          float*, cudaStream_t, const FeatureRows&, const float*, const float*);
 template cudaError_t launch_feature_lift(const ViewParams&, const ForwardBuffers&, const float*, float*, float*,
                                          cudaStream_t);
 template cudaError_t launch_feature_lift(const ViewParams&, const ForwardBuffers&, const __half*, float*, float*,

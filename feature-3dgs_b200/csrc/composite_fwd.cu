@@ -33,6 +33,11 @@
 // is bitwise the float32 render of the upcast features followed by .half(), and everything else is bitwise the float32
 // render's (the alpha warps never read features).
 //
+// PLANES (opt-in): the alpha warps also accumulate I = sum_i w_i (1/z_i) beside the depth, with 1/z_i the correctly
+// rounded reciprocal of the record's view depth, and the epilogue writes the opacity plane 1 - T (the T that goes to
+// final_T) and the inverse-depth plane I.  Nothing else the kernel computes or stores changes, so colour, depth, the
+// feature map, final_T and n_contrib are bitwise those of the kernel without the planes.
+//
 // Registers: with features the 28 warps are launched at 72 registers per thread (64512 in the CTA pool); setmaxnreg
 // then gives the producer group 40, the alpha warps 56 and the feature warps 88 (4x32x40 + 8x32x56 + 16x32x88 =
 // 64512).  (setmaxnreg acts per warpgroup of 4 consecutive warps, so the producer group is one unit.)  Without
@@ -61,6 +66,8 @@ struct FwdArgs {
     TF* out_feature;
     float* out_depth;
     int vec_store;
+    float* out_alpha;     // PLANES: [H,W] 1 - final_T
+    float* out_invdepth;  // PLANES: [H,W] sum_i w_i / z_i
 };
 
 // A lane's 4 channels of a staged feature row as loaded (float4, or 8 bytes of float16; to_float4 makes them float32).
@@ -84,7 +91,7 @@ __device__ __forceinline__ void st_run(__half* p, float4 v) {
 __device__ __forceinline__ void st_px(float* p, float v) { *p = v; }
 __device__ __forceinline__ void st_px(__half* p, float v) { *p = __float2half_rn(v); }
 
-template <int CH, typename TF>
+template <int CH, typename TF, bool PLANES>
 __global__ void __launch_bounds__(kFwdThreads<CH>, 1)
 composite_fwd_kernel(const FwdArgs<TF> args) {
     extern __shared__ __align__(128) unsigned char smem_raw[];
@@ -119,6 +126,7 @@ composite_fwd_kernel(const FwdArgs<TF> args) {
         int s = 0, j = 0;
         uint32_t parity = 0, wparity = 1;  // wempty: fresh barrier falls through on parity 1
         float T = 1.f, Cr = 0.f, Cg = 0.f, Cb = 0.f, Dp = 0.f, pxf = 0.f, pyf = 0.f, fbx0 = 0.f, fby0 = 0.f;
+        float Ip = 0.f;  // PLANES
         uint32_t last_contrib = 0;
         int px = 0, py = 0, chunk = 0;
         bool done = true, inside = false, blk_done = true;
@@ -140,6 +148,7 @@ composite_fwd_kernel(const FwdArgs<TF> args) {
                 pxf = (float)px; pyf = (float)py;
                 fbx0 = (float)bx0; fby0 = (float)by0;
                 T = 1.f; Cr = Cg = Cb = Dp = 0.f;
+                if constexpr (PLANES) Ip = 0.f;
                 last_contrib = 0;
                 done = !inside;
                 blk_done = __all_sync(0xffffffffu, done);
@@ -187,6 +196,10 @@ composite_fwd_kernel(const FwdArgs<TF> args) {
                         Cg = blend ? nCg : Cg;
                         Cb = blend ? nCb : Cb;
                         Dp = blend ? nDp : Dp;
+                        if constexpr (PLANES) {
+                            const float nIp = Ip + __frcp_rn(r2.w) * (alpha * T);
+                            Ip = blend ? nIp : Ip;
+                        }
                         T = blend ? test_T : T;
                         last_contrib = blend ? lp : last_contrib;
                         const uint32_t pm = __ballot_sync(0xffffffffu, blend);
@@ -224,6 +237,10 @@ composite_fwd_kernel(const FwdArgs<TF> args) {
                 args.out_color[HW + pix] = Cg + T * args.bg[1];
                 args.out_color[2 * HW + pix] = Cb + T * args.bg[2];
                 args.out_depth[pix] = Dp;
+                if constexpr (PLANES) {
+                    args.out_alpha[pix] = 1.f - T;
+                    args.out_invdepth[pix] = Ip;
+                }
             }
             if (++s == kStages) { s = 0; parity ^= 1; }
             if (CH > 0 && ++j == kWSlots) { j = 0; wparity ^= 1; }
@@ -351,14 +368,14 @@ composite_fwd_kernel(const FwdArgs<TF> args) {
 #undef FEAT_ROW_FMA
 }
 
-template <int CH, typename TF>
+template <int CH, typename TF, bool PLANES>
 static cudaError_t launch_fwd_t(const ViewParams& vp, const uint2* ranges, const uint32_t* point_list,
                                 const SplatRec* rec, const TF* features, const float* bg, float* final_T,
                                 uint32_t* n_contrib, float* out_color, TF* out_feature, float* out_depth,
-                                int* work_counter, cudaStream_t s) {
+                                int* work_counter, cudaStream_t s, float* out_alpha, float* out_invdepth) {
     const size_t smem = sizeof(RingV2<CH, TF>);
     int num_sms = 0;
-    cudaError_t e = device_sms<composite_fwd_kernel<CH, TF>>(num_sms, smem);
+    cudaError_t e = device_sms<composite_fwd_kernel<CH, TF, PLANES>>(num_sms, smem);
     if (e != cudaSuccess) return e;
     FwdArgs<TF> a;
     a.pa = producer_args(vp, ranges, point_list, rec, nullptr, work_counter);
@@ -371,6 +388,7 @@ static cudaError_t launch_fwd_t(const ViewParams& vp, const uint2* ranges, const
     a.pa.use_bulk = (CH > 0 && vp.C % kPer16 == 0 && (reinterpret_cast<uintptr_t>(features) & 15) == 0) ? 1 : 0;
     a.bg = bg; a.final_T = final_T; a.n_contrib = n_contrib;
     a.out_color = out_color; a.out_feature = out_feature; a.out_depth = out_depth;
+    a.out_alpha = out_alpha; a.out_invdepth = out_invdepth;
     // 1: 4-pixel stores (16 B of float, 8 B of half); 2: 8-pixel rows (32 B of float, 16 B of half)
     const uintptr_t out_addr = reinterpret_cast<uintptr_t>(out_feature);
     a.vec_store = (vp.W % 4 == 0 && (out_addr & (4 * sizeof(TF) - 1)) == 0) ? 1 : 0;
@@ -378,7 +396,7 @@ static cudaError_t launch_fwd_t(const ViewParams& vp, const uint2* ranges, const
     e = cudaMemsetAsync(work_counter, 0, sizeof(int), s);
     if (e != cudaSuccess) return e;
     const int grid = min(a.pa.num_tiles * a.pa.chunks, num_sms);
-    composite_fwd_kernel<CH, TF><<<grid, kFwdThreads<CH>, smem, s>>>(a);
+    composite_fwd_kernel<CH, TF, PLANES><<<grid, kFwdThreads<CH>, smem, s>>>(a);
     g_launches++;
     return cudaGetLastError();
 }
@@ -387,23 +405,31 @@ template <typename TF>
 cudaError_t launch_composite_fwd(const ViewParams& vp, const uint2* ranges, const uint32_t* point_list,
                                  const SplatRec* rec, const TF* features, const float* bg,
                                  float* final_T, uint32_t* n_contrib, float* out_color,
-                                 TF* out_feature, float* out_depth, int* counters, cudaStream_t s) {
+                                 TF* out_feature, float* out_depth, int* counters, cudaStream_t s, float* out_alpha,
+                                 float* out_invdepth) {
     int* const work_counter = counters + kCounterFwd;
-    if (vp.C == 0)  // no feature rows or map: one kernel for both element types
-        return launch_fwd_t<0, float>(vp, ranges, point_list, rec, nullptr, bg, final_T, n_contrib, out_color, nullptr,
-                                      out_depth, work_counter, s);
+    if (vp.C == 0) {  // no feature rows or map: one kernel for both element types
+        const auto launch0 = out_alpha ? launch_fwd_t<0, float, true> : launch_fwd_t<0, float, false>;
+        return launch0(vp, ranges, point_list, rec, nullptr, bg, final_T, n_contrib, out_color, nullptr, out_depth,
+                       work_counter, s, out_alpha, out_invdepth);
+    }
     const int ch = channel_chunk(vp.C);
-    const auto launch = ch == 32 ? launch_fwd_t<32, TF> : ch == 64 ? launch_fwd_t<64, TF> : launch_fwd_t<128, TF>;
+    const auto launch = out_alpha ? (ch == 32   ? launch_fwd_t<32, TF, true>
+                                     : ch == 64 ? launch_fwd_t<64, TF, true>
+                                                : launch_fwd_t<128, TF, true>)
+                                  : (ch == 32   ? launch_fwd_t<32, TF, false>
+                                     : ch == 64 ? launch_fwd_t<64, TF, false>
+                                                : launch_fwd_t<128, TF, false>);
     return launch(vp, ranges, point_list, rec, features, bg, final_T, n_contrib, out_color, out_feature, out_depth,
-                  work_counter, s);
+                  work_counter, s, out_alpha, out_invdepth);
 }
 
 template cudaError_t launch_composite_fwd<float>(const ViewParams&, const uint2*, const uint32_t*, const SplatRec*,
                                                  const float*, const float*, float*, uint32_t*, float*, float*, float*,
-                                                 int*, cudaStream_t);
+                                                 int*, cudaStream_t, float*, float*);
 template cudaError_t launch_composite_fwd<__half>(const ViewParams&, const uint2*, const uint32_t*, const SplatRec*,
                                                   const __half*, const float*, float*, uint32_t*, float*, __half*,
-                                                  float*, int*, cudaStream_t);
+                                                  float*, int*, cudaStream_t, float*, float*);
 
 }  // namespace f3dgs
 

@@ -56,12 +56,15 @@ void launch_tile_ranges(int R, const uint64_t* sorted_keys, uint2* ranges, cudaS
 
 // ---- composite_fwd.cu
 // returns cudaSuccess or the launch error.  TF (float or __half) is the element type of features and out_feature: the
-// float16 map is bitwise the float32 map of the exactly upcast features rounded to nearest even
+// float16 map is bitwise the float32 map of the exactly upcast features rounded to nearest even.  With out_alpha (then
+// out_invdepth too, both [H,W]): also the opacity plane 1 - final_T and the inverse-depth plane sum_i w_i / z_i; every
+// other output is bitwise that of the call without them
 template <typename TF>
 cudaError_t launch_composite_fwd(const ViewParams& vp, const uint2* ranges, const uint32_t* point_list,
                                  const SplatRec* rec, const TF* features, const float* bg,
                                  float* final_T, uint32_t* n_contrib, float* out_color,
-                                 TF* out_feature, float* out_depth, int* counters, cudaStream_t s);
+                                 TF* out_feature, float* out_depth, int* counters, cudaStream_t s,
+                                 float* out_alpha = nullptr, float* out_invdepth = nullptr);
 
 // ---- composite_bwd.cu + feature_bwd.cu: the composite backward of a view, from that view's forward buffers
 struct ForwardBuffers {
@@ -83,12 +86,15 @@ struct FeatureRows {
 // instance lists (scratch of the device's default pool, freed on the stream before return), and a second kernel forms
 // dL_dfeature from them.  TG (float or __half) is the element type of dL_dfeat_pix; a __half map stands for
 // dL/dO = scale * float(h) (the scale is not read for a float map).  With feat.rows (and C > 0, R > 0) the feature term
-// of dL/dalpha is added to dL_dmean2D, dL_dconic and dL_dopacity by two more kernels over the same lists.
+// of dL/dalpha is added to dL_dmean2D, dL_dconic and dL_dopacity by two more kernels over the same lists.  With
+// dL_dalpha (then dL_dinvdepth too, both [H,W]): the gradients of the forward's opacity and inverse-depth planes join
+// dL/dalpha and dL_dz in the same geometry walk; with both zero every output is bitwise that of the call without them.
 template <typename TG>
 cudaError_t launch_composite_bwd(const ViewParams& vp, const ForwardBuffers& fb, const float* bg, const float* dL_dpix,
                                  const float* dL_ddepth, const TG* dL_dfeat_pix, float dL_dfeat_pix_scale,
                                  float* dL_dmean2D, float* dL_dconic, float* dL_dopacity, float* dL_dcolor, float* dL_dz,
-                                 float* dL_dfeature, cudaStream_t s, const FeatureRows& feat = {});
+                                 float* dL_dfeature, cudaStream_t s, const FeatureRows& feat = {},
+                                 const float* dL_dalpha = nullptr, const float* dL_dinvdepth = nullptr);
 // Feature lifting, R > 0: weight_sum[P] += the blend weights w = alpha*T of each Gaussian over the view and
 // feature_sum[P, C] += sum_p w * map[:, p], through the same lists.  TF (float or __half) is the element type of map
 template <typename TF>

@@ -13,7 +13,12 @@
 // `camera`) with the feature term of dL/dalpha (f3dgs_backward_feature_geometry).  Antialiased rendering:
 // rasterize_gaussians_antialiased (rasterize_gaussians' arguments and results, f3dgs_forward_antialiased) and
 // rasterize_gaussians_backward_antialiased(same arguments, camera=False, semantic_feature=None) -> the same 12, with the
-// feature term when semantic_feature is given (f3dgs_backward_antialiased).
+// feature term when semantic_feature is given (f3dgs_backward_antialiased).  Opacity and inverse-depth maps:
+// rasterize_gaussians_alpha_invdepth(rasterize_gaussians' arguments, antialiasing=False) -> (num_rendered, color,
+// feature_map, depth, alpha, invdepth, radii, geom, binning, img) (f3dgs_forward_alpha_invdepth) and
+// rasterize_gaussians_backward_alpha_invdepth(the backward's arguments, dL_dout_alpha, dL_dout_invdepth, camera=False,
+// semantic_feature=None, antialiasing=False) -> the same 12 as rasterize_gaussians_backward_antialiased
+// (f3dgs_backward_alpha_invdepth).
 // Differences (all permissive): the feature width is read from semantic_feature.size(-1) at run
 // time (reference: compile-time NUM_SEMANTIC_CHANNELS, config.h:16); an empty / undefined
 // semantic_feature means C = 0; semantic_feature may be float32 or float16, and the feature map
@@ -82,6 +87,14 @@ torch::Tensor feature_grad(const torch::Tensor& t, const torch::Device& dev) {
     return t.contiguous();
 }
 
+// The gradient of an opacity or inverse-depth plane: float32 [1,H,W] (any shape of H*W elements) on `dev`, made
+// contiguous; undefined or empty stands for zeros
+torch::Tensor plane_grad(const torch::Tensor& t, const torch::Device& dev, int64_t H, int64_t W, const char* name) {
+    if (!t.defined() || t.numel() == 0) return torch::zeros({1, H, W}, torch::TensorOptions().device(dev));
+    TORCH_CHECK(t.numel() == H * W, name, " must have H * W = ", H * W, " elements (got ", t.numel(), ")");
+    return input(t, dev, name);
+}
+
 // C-ABI element-type code of a float32 or float16 tensor (absent: float32)
 int dtype_code(const torch::Tensor& t) {
     return t.defined() && t.scalar_type() == torch::kFloat16 ? F3DGS_F16 : F3DGS_F32;
@@ -123,8 +136,10 @@ using ForwardResults = std::tuple<int, torch::Tensor, torch::Tensor, torch::Tens
     background, means3D, colors, semantic_feature, opacity, scales, rotations, scale_modifier, cov3D_precomp,         \
         viewmatrix, projmatrix, tan_fovx, tan_fovy, image_height, image_width, sh, degree, campos, prefiltered, debug
 
-// Body of rasterize_gaussians and rasterize_gaussians_antialiased (f3dgs_forward_antialiased)
-static ForwardResults forward(FORWARD_PARAMS, const bool antialiasing) {
+// Body of rasterize_gaussians, rasterize_gaussians_antialiased (f3dgs_forward_antialiased) and, with `planes` (two
+// tensors it sets to the [1,H,W] opacity and inverse-depth planes), rasterize_gaussians_alpha_invdepth
+// (f3dgs_forward_alpha_invdepth)
+static ForwardResults forward(FORWARD_PARAMS, const bool antialiasing, torch::Tensor* planes = nullptr) {
     if (means3D.ndimension() != 2 || means3D.size(1) != 3) {
         AT_ERROR("means3D must have dimensions (num_points, 3)");
     }
@@ -147,6 +162,8 @@ static ForwardResults forward(FORWARD_PARAMS, const bool antialiasing) {
     torch::Tensor out_depth = P ? torch::empty({1, H, W}, float_opts) : torch::zeros({1, H, W}, float_opts);
     torch::Tensor out_feature = P ? torch::empty({C, H, W}, feat_opts) : torch::zeros({C, H, W}, feat_opts);
     torch::Tensor radii = torch::empty({P}, means3D.options().dtype(torch::kInt32));
+    if (planes)
+        for (int k = 0; k < 2; k++) planes[k] = P ? torch::empty({1, H, W}, float_opts) : torch::zeros({1, H, W}, float_opts);
 
     auto byte_opts = torch::TensorOptions().dtype(torch::kByte).device(dev);
     torch::Tensor geomBuffer = torch::empty({0}, byte_opts);
@@ -167,7 +184,16 @@ static ForwardResults forward(FORWARD_PARAMS, const bool antialiasing) {
         auto vm = input(viewmatrix, dev, "viewmatrix"), pm = input(projmatrix, dev, "projmatrix");
         auto shc = input(sh, dev, "shs"), cp = input(campos, dev, "campos");
         cudaStream_t stream = c10::cuda::getCurrentCUDAStream().stream();
-        if (antialiasing) {
+        if (planes) {
+            rendered = f3dgs_forward_alpha_invdepth(
+                resize_tensor, &geomBuffer, resize_tensor, &binningBuffer, resize_tensor, &imgBuffer, P, degree, M, C,
+                fptr(bg), W, H, fptr(m3), fptr(shc), fptr(col), has_sf ? sf.data_ptr() : nullptr, dtype_code(sf),
+                fptr(op), fptr(sc), scale_modifier, fptr(rot), fptr(cov), fptr(vm), fptr(pm), fptr(cp), tan_fovx,
+                tan_fovy, prefiltered ? 1 : 0, out_color.data_ptr<float>(), C ? out_feature.data_ptr() : nullptr,
+                out_depth.data_ptr<float>(), radii.data_ptr<int>(), debug ? 1 : 0, (void*)stream, antialiasing ? 1 : 0,
+                planes[0].data_ptr<float>(), planes[1].data_ptr<float>());
+            check_rc(rendered, "f3dgs_forward_alpha_invdepth");
+        } else if (antialiasing) {
             rendered = f3dgs_forward_antialiased(
                 resize_tensor, &geomBuffer, resize_tensor, &binningBuffer, resize_tensor, &imgBuffer, P, degree, M, C,
                 fptr(bg), W, H, fptr(m3), fptr(shc), fptr(col), has_sf ? sf.data_ptr() : nullptr, dtype_code(sf),
@@ -193,6 +219,13 @@ static ForwardResults forward(FORWARD_PARAMS, const bool antialiasing) {
 
 ForwardResults RasterizeGaussiansCUDA(FORWARD_PARAMS) { return forward(FORWARD_ARGS, false); }
 ForwardResults RasterizeGaussiansAntialiasedCUDA(FORWARD_PARAMS) { return forward(FORWARD_ARGS, true); }
+std::tuple<int, torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor,
+           torch::Tensor, torch::Tensor>
+RasterizeGaussiansAlphaInvDepthCUDA(FORWARD_PARAMS, const bool antialiasing) {
+    torch::Tensor planes[2];
+    const auto [rendered, color, feature, depth, radii, geom, binning, img] = forward(FORWARD_ARGS, antialiasing, planes);
+    return std::make_tuple(rendered, color, feature, depth, planes[0], planes[1], radii, geom, binning, img);
+}
 #undef FORWARD_PARAMS
 #undef FORWARD_ARGS
 
@@ -202,7 +235,9 @@ using BackwardGrads = std::tuple<torch::Tensor, torch::Tensor, torch::Tensor, to
 // Body of rasterize_gaussians_backward, _camera, _feature_geometry and _antialiased: with a non-NULL camera (35 floats on
 // the device), the _cam entries, which add the camera gradient to it; with feature_geometry,
 // f3dgs_backward_feature_geometry, which reads semantic_feature and takes the camera gradient as an optional argument;
-// with antialiasing, f3dgs_backward_antialiased, whose feature term reads `features` if that is given
+// with antialiasing, f3dgs_backward_antialiased, whose feature term reads `features` if that is given; with `planes`
+// (the gradients of the opacity and inverse-depth planes), f3dgs_backward_alpha_invdepth, with the feature term as under
+// antialiasing and the forward's mode `antialiasing`
 static BackwardGrads backward_grads(const torch::Tensor& background, const torch::Tensor& means3D,
                                const torch::Tensor& radii, const torch::Tensor& colors,
                                const torch::Tensor& semantic_feature, const torch::Tensor& scales,
@@ -214,7 +249,8 @@ static BackwardGrads backward_grads(const torch::Tensor& background, const torch
                                const torch::Tensor& campos, const torch::Tensor& geomBuffer, const int R,
                                const torch::Tensor& binningBuffer, const torch::Tensor& imageBuffer,
                                const bool debug, float* camera, bool feature_geometry = false,
-                               bool antialiasing = false, const torch::Tensor& features = torch::Tensor()) {
+                               bool antialiasing = false, const torch::Tensor& features = torch::Tensor(),
+                               const torch::Tensor* planes = nullptr) {
     TORCH_CHECK(means3D.is_cuda(), "means3D must be a CUDA tensor (this build has no CPU path)");
     const c10::cuda::CUDAGuard guard(means3D.device());
     const auto dev = means3D.device();
@@ -283,7 +319,7 @@ static BackwardGrads backward_grads(const torch::Tensor& background, const torch
             };
         };
         // the _feature_geometry / _antialiased entries: features sf (its element type by code; NULL if absent or C == 0)
-        auto typed_call = [&](auto fn, const torch::Tensor& sf) {
+        auto typed_call = [&](auto fn, const torch::Tensor& sf, auto... tail) {
             return fn(P, degree, M, R, C, fptr(bg), W, H, fptr(m3), fptr(shc), fptr(col),
                       C && sf.defined() && sf.numel() ? sf.data_ptr() : nullptr, dtype_code(sf), fptr(sc),
                       scale_modifier, fptr(rot), fptr(cov), fptr(vm), fptr(pm), fptr(cp), tan_fovx, tan_fovy,
@@ -293,7 +329,8 @@ static BackwardGrads backward_grads(const torch::Tensor& background, const torch
                       dL_dopacity.data_ptr<float>(), dL_dcolors.data_ptr<float>(),
                       C ? dL_dsemantic_feature.data_ptr<float>() : nullptr, dL_dmeans3D.data_ptr<float>(),
                       dL_dcov3D.data_ptr<float>(), M ? dL_dsh.data_ptr<float>() : nullptr, dL_dscales.data_ptr<float>(),
-                      dL_drotations.data_ptr<float>(), dL_dz.data_ptr<float>(), debug ? 1 : 0, (void*)stream, camera);
+                      dL_drotations.data_ptr<float>(), dL_dz.data_ptr<float>(), debug ? 1 : 0, (void*)stream, camera,
+                      tail...);
         };
         // these entries read the features themselves, not only their shape
         auto feature_rows = [&](const torch::Tensor& t) {
@@ -303,7 +340,13 @@ static BackwardGrads backward_grads(const torch::Tensor& background, const torch
                         " elements (got ", t.numel(), ")");
             return t.contiguous();
         };
-        if (antialiasing)
+        if (planes) {
+            auto ga = plane_grad(planes[0], dev, H, W, "dL_dout_alpha"), gi = plane_grad(planes[1], dev, H, W,
+                                                                                       "dL_dout_invdepth");
+            check_rc(typed_call(f3dgs_backward_alpha_invdepth, feature_rows(features), antialiasing ? 1 : 0, fptr(ga),
+                                fptr(gi)),
+                     "f3dgs_backward_alpha_invdepth");
+        } else if (antialiasing)
             check_rc(typed_call(f3dgs_backward_antialiased, feature_rows(features)), "f3dgs_backward_antialiased");
         else if (feature_geometry)
             check_rc(typed_call(f3dgs_backward_feature_geometry, feature_rows(semantic_feature)),
@@ -378,6 +421,25 @@ RasterizeGaussiansBackwardAntialiasedCUDA(BACKWARD_PARAMS, const bool camera,
                           std::make_tuple(cam.narrow(0, 0, 16).view({4, 4}), cam.narrow(0, 16, 16).view({4, 4}),
                                           cam.narrow(0, 32, 3)));
 }
+// rasterize_gaussians_backward_antialiased's 12 results for the buffers of rasterize_gaussians_alpha_invdepth (or of the
+// forward without planes in the same mode), with the gradients of the opacity and inverse-depth planes
+// (f3dgs_backward_alpha_invdepth)
+decltype(std::tuple_cat(BackwardGrads(), std::tuple<torch::Tensor, torch::Tensor, torch::Tensor>()))
+RasterizeGaussiansBackwardAlphaInvDepthCUDA(BACKWARD_PARAMS, const torch::Tensor& dL_dout_alpha,
+                                            const torch::Tensor& dL_dout_invdepth, const bool camera,
+                                            const std::optional<torch::Tensor>& features, const bool antialiasing) {
+    TORCH_CHECK(means3D.is_cuda(), "means3D must be a CUDA tensor (this build has no CPU path)");
+    const c10::cuda::CUDAGuard guard(means3D.device());
+    const torch::Tensor f = features.has_value() ? *features : torch::Tensor();
+    const torch::Tensor planes[2] = {dL_dout_alpha, dL_dout_invdepth};
+    if (!camera)
+        return std::tuple_cat(backward_grads(BACKWARD_ARGS, nullptr, false, antialiasing, f, planes),
+                              std::make_tuple(torch::Tensor(), torch::Tensor(), torch::Tensor()));
+    torch::Tensor cam = torch::zeros({F3DGS_CAMERA_GRAD_FLOATS}, means3D.options().dtype(torch::kFloat32));
+    return std::tuple_cat(backward_grads(BACKWARD_ARGS, cam.data_ptr<float>(), false, antialiasing, f, planes),
+                          std::make_tuple(cam.narrow(0, 0, 16).view({4, 4}), cam.narrow(0, 16, 16).view({4, 4}),
+                                          cam.narrow(0, 32, 3)));
+}
 #undef BACKWARD_PARAMS
 #undef BACKWARD_ARGS
 
@@ -386,7 +448,9 @@ RasterizeGaussiansBackwardAntialiasedCUDA(BACKWARD_PARAMS, const bool camera,
 // allocated besides one cached scratch tensor per device.  Undefined / empty tensors stand for "not an input".
 // semantic_feature (optional, [P,...,C] float32 or float16): f3dgs_backward_accum_feature_geometry, the feature term of
 // dL/dalpha in the geometric gradients.  antialiasing: f3dgs_backward_accum_antialiased, for the buffers of
-// rasterize_gaussians_antialiased (with the feature term if semantic_feature is given).
+// rasterize_gaussians_antialiased (with the feature term if semantic_feature is given).  dL_dout_alpha / dL_dout_invdepth
+// (optional; one given alone: the other is zero): f3dgs_backward_accum_alpha_invdepth, the gradients of the opacity and
+// inverse-depth planes, for the buffers of either forward in the mode `antialiasing`.
 void RasterizeGaussiansBackwardAccumCUDA(
     const torch::Tensor& background, const torch::Tensor& means3D, const torch::Tensor& radii,
     const torch::Tensor& colors, const torch::Tensor& scales, const torch::Tensor& rotations, const float scale_modifier,
@@ -399,7 +463,8 @@ void RasterizeGaussiansBackwardAccumCUDA(
     torch::Tensor g_cov3D, torch::Tensor g_means2D_out, torch::Tensor grad_accum, torch::Tensor denom,
     const int64_t composite_done_event, const bool debug, const double feature_grad_scale,
     const std::optional<torch::Tensor>& camera_grad, const std::optional<torch::Tensor>& semantic_feature,
-    const bool antialiasing) {
+    const bool antialiasing, const std::optional<torch::Tensor>& dL_dout_alpha,
+    const std::optional<torch::Tensor>& dL_dout_invdepth) {
     TORCH_CHECK(means3D.is_cuda(), "means3D must be a CUDA tensor (this build has no CPU path)");
     const c10::cuda::CUDAGuard guard(means3D.device());
     const auto dev = means3D.device();
@@ -437,7 +502,9 @@ void RasterizeGaussiansBackwardAccumCUDA(
     }
     cudaStream_t stream = c10::cuda::getCurrentCUDAStream().stream();
     const bool has_features = semantic_feature.has_value() && semantic_feature->defined();
-    if (has_features || antialiasing) {
+    const bool has_planes = (dL_dout_alpha.has_value() && dL_dout_alpha->defined()) ||
+                            (dL_dout_invdepth.has_value() && dL_dout_invdepth->defined());
+    if (has_features || antialiasing || has_planes) {
         torch::Tensor sf;
         if (has_features) {
             check_features(*semantic_feature, dev);
@@ -445,26 +512,37 @@ void RasterizeGaussiansBackwardAccumCUDA(
                         (int64_t)P * C, " elements (got ", semantic_feature->numel(), ")");
             sf = semantic_feature->contiguous();
         }
-        check_rc((antialiasing ? f3dgs_backward_accum_antialiased : f3dgs_backward_accum_feature_geometry)(
-                     P, degree, M, R, C, fptr(bg), W, H, fptr(m3), fptr(shc), fptr(col),
-                     C && has_features ? sf.data_ptr() : nullptr,
-                     dtype_code(sf), fptr(sc), scale_modifier, fptr(rot), fptr(cov), fptr(vm), fptr(pm), fptr(cp),
-                     tan_fovx, tan_fovy, rad.data_ptr<int>(), reinterpret_cast<char*>(geomBuffer.data_ptr()),
-                     reinterpret_cast<char*>(binningBuffer.data_ptr()),
-                     reinterpret_cast<char*>(imageBuffer.data_ptr()), fptr(gc), gf.defined() ? gf.data_ptr() : nullptr,
-                     dtype_code(gf), (float)feature_grad_scale, fptr(gd), reinterpret_cast<char*>(scratch.data_ptr()),
-                     in_place(g_opacities, dev, P, "g_opacities"),
-                     in_place(g_colors, dev, (int64_t)P * 3, "g_colors_precomp"),
-                     in_place(g_semantic_feature, dev, (int64_t)P * C, "g_semantic_feature"),
-                     in_place(g_means3D, dev, (int64_t)P * 3, "g_means3D"),
-                     in_place(g_cov3D, dev, (int64_t)P * 6, "g_cov3D_precomp"),
-                     in_place(g_sh, dev, (int64_t)P * M * 3, "g_sh"), in_place(g_scales, dev, (int64_t)P * 3, "g_scales"),
-                     in_place(g_rotations, dev, (int64_t)P * 4, "g_rotations"),
-                     in_place(g_means2D_out, dev, (int64_t)P * 3, "g_means2D_out"),
-                     in_place(grad_accum, dev, P, "grad_accum"), in_place(denom, dev, P, "denom"),
-                     reinterpret_cast<void*>(static_cast<intptr_t>(composite_done_event)), debug ? 1 : 0,
-                     (void*)stream, cam),
-                 antialiasing ? "f3dgs_backward_accum_antialiased" : "f3dgs_backward_accum_feature_geometry");
+        // the three entries share their arguments up to dL_dcamera; `tail` is the _alpha_invdepth entry's rest
+        auto call = [&](auto fn, auto... tail) {
+            return fn(P, degree, M, R, C, fptr(bg), W, H, fptr(m3), fptr(shc), fptr(col),
+                      C && has_features ? sf.data_ptr() : nullptr,
+                      dtype_code(sf), fptr(sc), scale_modifier, fptr(rot), fptr(cov), fptr(vm), fptr(pm), fptr(cp),
+                      tan_fovx, tan_fovy, rad.data_ptr<int>(), reinterpret_cast<char*>(geomBuffer.data_ptr()),
+                      reinterpret_cast<char*>(binningBuffer.data_ptr()),
+                      reinterpret_cast<char*>(imageBuffer.data_ptr()), fptr(gc), gf.defined() ? gf.data_ptr() : nullptr,
+                      dtype_code(gf), (float)feature_grad_scale, fptr(gd), reinterpret_cast<char*>(scratch.data_ptr()),
+                      in_place(g_opacities, dev, P, "g_opacities"),
+                      in_place(g_colors, dev, (int64_t)P * 3, "g_colors_precomp"),
+                      in_place(g_semantic_feature, dev, (int64_t)P * C, "g_semantic_feature"),
+                      in_place(g_means3D, dev, (int64_t)P * 3, "g_means3D"),
+                      in_place(g_cov3D, dev, (int64_t)P * 6, "g_cov3D_precomp"),
+                      in_place(g_sh, dev, (int64_t)P * M * 3, "g_sh"),
+                      in_place(g_scales, dev, (int64_t)P * 3, "g_scales"),
+                      in_place(g_rotations, dev, (int64_t)P * 4, "g_rotations"),
+                      in_place(g_means2D_out, dev, (int64_t)P * 3, "g_means2D_out"),
+                      in_place(grad_accum, dev, P, "grad_accum"), in_place(denom, dev, P, "denom"),
+                      reinterpret_cast<void*>(static_cast<intptr_t>(composite_done_event)), debug ? 1 : 0,
+                      (void*)stream, cam, tail...);
+        };
+        if (has_planes) {
+            const torch::Tensor none;
+            auto ga = plane_grad(dL_dout_alpha.value_or(none), dev, H, W, "dL_dout_alpha");
+            auto gi = plane_grad(dL_dout_invdepth.value_or(none), dev, H, W, "dL_dout_invdepth");
+            check_rc(call(f3dgs_backward_accum_alpha_invdepth, antialiasing ? 1 : 0, fptr(ga), fptr(gi)),
+                     "f3dgs_backward_accum_alpha_invdepth");
+        } else
+            check_rc(call(antialiasing ? f3dgs_backward_accum_antialiased : f3dgs_backward_accum_feature_geometry),
+                     antialiasing ? "f3dgs_backward_accum_antialiased" : "f3dgs_backward_accum_feature_geometry");
         return;
     }
     // scale: the float16 symbol's scale after the map, () for the float32 one; tail: (dL_dcamera) or ()
@@ -1033,7 +1111,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
               py::arg("g_scales"), py::arg("g_rotations"), py::arg("g_cov3D"), py::arg("g_means2D_out"),
               py::arg("grad_accum"), py::arg("denom"), py::arg("composite_done_event"), py::arg("debug"),
               py::arg("feature_grad_scale") = 1.0, py::arg("camera_grad") = py::none(),
-              py::arg("semantic_feature") = py::none(), py::arg("antialiasing") = false);
+              py::arg("semantic_feature") = py::none(), py::arg("antialiasing") = false,
+              py::arg("dL_dout_alpha") = py::none(), py::arg("dL_dout_invdepth") = py::none());
         m.def("rasterize_gaussians_antialiased", &RasterizeGaussiansAntialiasedCUDA);
         m.def("rasterize_gaussians_backward_antialiased", &RasterizeGaussiansBackwardAntialiasedCUDA,
               py::arg("background"), py::arg("means3D"), py::arg("radii"), py::arg("colors"), py::arg("features_like"),
@@ -1043,6 +1122,20 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
               py::arg("degree"), py::arg("campos"), py::arg("geomBuffer"), py::arg("R"), py::arg("binningBuffer"),
               py::arg("imageBuffer"), py::arg("debug"), py::arg("camera") = false,
               py::arg("semantic_feature") = py::none());
+        m.def("rasterize_gaussians_alpha_invdepth", &RasterizeGaussiansAlphaInvDepthCUDA, py::arg("background"),
+              py::arg("means3D"), py::arg("colors"), py::arg("semantic_feature"), py::arg("opacity"), py::arg("scales"),
+              py::arg("rotations"), py::arg("scale_modifier"), py::arg("cov3D_precomp"), py::arg("viewmatrix"),
+              py::arg("projmatrix"), py::arg("tan_fovx"), py::arg("tan_fovy"), py::arg("image_height"),
+              py::arg("image_width"), py::arg("sh"), py::arg("degree"), py::arg("campos"), py::arg("prefiltered"),
+              py::arg("debug"), py::arg("antialiasing") = false);
+        m.def("rasterize_gaussians_backward_alpha_invdepth", &RasterizeGaussiansBackwardAlphaInvDepthCUDA,
+              py::arg("background"), py::arg("means3D"), py::arg("radii"), py::arg("colors"), py::arg("features_like"),
+              py::arg("scales"), py::arg("rotations"), py::arg("scale_modifier"), py::arg("cov3D_precomp"),
+              py::arg("viewmatrix"), py::arg("projmatrix"), py::arg("tan_fovx"), py::arg("tan_fovy"),
+              py::arg("dL_dout_color"), py::arg("dL_dout_feature"), py::arg("dL_dout_depth"), py::arg("sh"),
+              py::arg("degree"), py::arg("campos"), py::arg("geomBuffer"), py::arg("R"), py::arg("binningBuffer"),
+              py::arg("imageBuffer"), py::arg("debug"), py::arg("dL_dout_alpha"), py::arg("dL_dout_invdepth"),
+              py::arg("camera") = false, py::arg("semantic_feature") = py::none(), py::arg("antialiasing") = false);
     }
     m.def("rasterize_gaussians_backward_camera", &RasterizeGaussiansBackwardCameraCUDA);
     m.def("rasterize_gaussians_backward_feature_geometry", &RasterizeGaussiansBackwardFeatureGeometryCUDA);

@@ -36,6 +36,11 @@ Behavioural notes
     sub-pixel Gaussian keeps the integral of the undilated one (f3dgs_forward_antialiased / f3dgs_backward_antialiased).
     Renders at a resolution other than the training one (lower-resolution feature targets, lifting at a teacher's
     resolution) then stay consistent.  By default the opacity is used as it is, as in the reference.
+  * opacity and inverse-depth maps (opt-in): `AlphaInvDepthGaussianRasterizer(raster_settings, feature_geometry=False,
+    antialiasing=False)`, or `rasterize_gaussians_alpha_invdepth`, also returns alpha = 1 - T_final (accumulated
+    opacity) and invdepth = sum_i w_i / z_i, both [1,H,W] float32 and differentiable (f3dgs_forward_alpha_invdepth /
+    f3dgs_backward_alpha_invdepth): mask losses, RGBA cut-outs, expected depth depth / alpha and inverse-depth
+    supervision.  Colour, feature map, depth, radii and their gradients are those of the rasterizer without the maps.
   * `debug=True` keeps the reference semantics: arguments are snapshotted to CPU first and dumped
     to snapshot_fw.dump / snapshot_bw.dump if the native call raises (reference :89-97,:147-155);
     natively it synchronises and checks after every stage.
@@ -62,6 +67,8 @@ __all__ = [
     "rasterize_gaussians",
     "rasterize_gaussians_feature_geometry",
     "AntialiasedGaussianRasterizer",
+    "rasterize_gaussians_alpha_invdepth",
+    "AlphaInvDepthGaussianRasterizer",
 ]
 
 
@@ -103,21 +110,10 @@ class _RasterizeGaussians(torch.autograd.Function):
     @staticmethod
     def forward(ctx, means3D, means2D, sh, colors_precomp, semantic_feature, opacities, scales, rotations,
                 cov3Ds_precomp, raster_settings, antialiasing=False):
-        rs = raster_settings
-        if semantic_feature is None:
-            semantic_feature = torch.empty(0, device=means3D.device, dtype=means3D.dtype)
-        args = (rs.bg, means3D, colors_precomp, semantic_feature, opacities, scales, rotations, rs.scale_modifier,
-                cov3Ds_precomp, rs.viewmatrix, rs.projmatrix, rs.tanfovx, rs.tanfovy, rs.image_height,
-                rs.image_width, sh, rs.sh_degree, rs.campos, rs.prefiltered, rs.debug)
         fn = _C.rasterize_gaussians_antialiased if antialiasing else _C.rasterize_gaussians
-        (num_rendered, color, feature_map, depth, radii, geomBuffer, binningBuffer, imgBuffer) = _call_native(
-            fn, args, rs.debug, "snapshot_fw.dump", "forward")
-        ctx.raster_settings = rs
-        ctx.antialiasing = antialiasing
-        ctx.num_rendered = num_rendered
-        ctx.save_for_backward(colors_precomp, semantic_feature, means3D, scales, rotations, cov3Ds_precomp, radii,
-                              sh, geomBuffer, binningBuffer, imgBuffer)
-        ctx.mark_non_differentiable(radii)
+        color, feature_map, depth, radii = _native_forward(ctx, fn, means3D, sh, colors_precomp, semantic_feature,
+                                                           opacities, scales, rotations, cov3Ds_precomp,
+                                                           raster_settings, antialiasing)
         return color, feature_map, radii, depth
 
     @staticmethod
@@ -125,6 +121,27 @@ class _RasterizeGaussians(torch.autograd.Function):
         fn = _antialiased_backward(False, False) if ctx.antialiasing else _C.rasterize_gaussians_backward
         grads = _native_backward(ctx, fn, grad_out_color, grad_out_feature, grad_depth)
         return grads[:9] + (None, None)
+
+
+def _native_forward(ctx, fn, means3D, sh, colors_precomp, semantic_feature, opacities, scales, rotations,
+                    cov3Ds_precomp, rs, antialiasing):
+    """The native forward `fn` with the reference forward's positional arguments; saves on ctx what _native_backward
+    reads -> fn's results between num_rendered and the three buffers, radii last"""
+    if semantic_feature is None:
+        semantic_feature = torch.empty(0, device=means3D.device, dtype=means3D.dtype)
+    args = (rs.bg, means3D, colors_precomp, semantic_feature, opacities, scales, rotations, rs.scale_modifier,
+            cov3Ds_precomp, rs.viewmatrix, rs.projmatrix, rs.tanfovx, rs.tanfovy, rs.image_height,
+            rs.image_width, sh, rs.sh_degree, rs.campos, rs.prefiltered, rs.debug)
+    (num_rendered, *outs, geomBuffer, binningBuffer, imgBuffer) = _call_native(
+        fn, args, rs.debug, "snapshot_fw.dump", "forward")
+    radii = outs[-1]
+    ctx.raster_settings = rs
+    ctx.antialiasing = antialiasing
+    ctx.num_rendered = num_rendered
+    ctx.save_for_backward(colors_precomp, semantic_feature, means3D, scales, rotations, cov3Ds_precomp, radii,
+                          sh, geomBuffer, binningBuffer, imgBuffer)
+    ctx.mark_non_differentiable(radii)
+    return outs
 
 
 def _native_backward(ctx, fn, grad_out_color, grad_out_feature, grad_depth):
@@ -215,6 +232,44 @@ class _RasterizeGaussiansCameraFeatureGeometry(_RasterizeGaussiansCamera):
         return grads[:9] + cam + (None, None)
 
 
+class _RasterizeGaussiansAlphaInvDepth(torch.autograd.Function):
+    """The render with the opacity and inverse-depth planes (f3dgs_forward_alpha_invdepth / f3dgs_backward_alpha_invdepth)
+    in every mode: the camera tensors are always inputs and get gradients when they require grad; feature_geometry
+    adds the feature term of dL/dalpha; antialiasing renders with the antialiased opacities."""
+
+    @staticmethod
+    def forward(ctx, means3D, means2D, sh, colors_precomp, semantic_feature, opacities, scales, rotations,
+                cov3Ds_precomp, viewmatrix, projmatrix, campos, raster_settings, feature_geometry, antialiasing):
+        rs = raster_settings._replace(viewmatrix=viewmatrix, projmatrix=projmatrix, campos=campos)
+        ctx.camera_shapes = (viewmatrix.shape, projmatrix.shape, campos.shape)
+        ctx.feature_geometry = feature_geometry
+        fn = lambda *args: _C.rasterize_gaussians_alpha_invdepth(*args, antialiasing=antialiasing)  # noqa: E731
+        color, feature_map, depth, alpha, invdepth, radii = _native_forward(
+            ctx, fn, means3D, sh, colors_precomp, semantic_feature, opacities, scales, rotations, cov3Ds_precomp, rs,
+            antialiasing)
+        return color, feature_map, radii, depth, alpha, invdepth
+
+    @staticmethod
+    def backward(ctx, grad_out_color, grad_out_feature, _grad_radii, grad_depth, grad_alpha, grad_invdepth):
+        rs = ctx.raster_settings
+        camera = any(ctx.needs_input_grad[9:12])
+        planes = tuple(torch.zeros(1, rs.image_height, rs.image_width, device=rs.bg.device) if g is None else g
+                       for g in (grad_alpha, grad_invdepth))
+        fn = lambda *args: _C.rasterize_gaussians_backward_alpha_invdepth(  # noqa: E731
+            *args, *planes, camera=camera, semantic_feature=args[4] if ctx.feature_geometry else None,
+            antialiasing=ctx.antialiasing)
+        grads = _native_backward(ctx, fn, grad_out_color, grad_out_feature, grad_depth)
+        cam = tuple(None if g is None else g.reshape(shape) for g, shape in zip(grads[9:], ctx.camera_shapes))
+        return grads[:9] + cam + (None, None, None)
+
+
+def _rasterize_alpha_invdepth(means3D, means2D, sh, colors_precomp, semantic_feature, opacities, scales, rotations,
+                              cov3Ds_precomp, rs, feature_geometry, antialiasing=False):
+    return _RasterizeGaussiansAlphaInvDepth.apply(means3D, means2D, sh, colors_precomp, semantic_feature, opacities,
+                                                  scales, rotations, cov3Ds_precomp, rs.viewmatrix, rs.projmatrix,
+                                                  rs.campos, rs, feature_geometry, antialiasing)
+
+
 def _camera_requires_grad(rs):
     return any(isinstance(t, torch.Tensor) and t.requires_grad for t in (rs.viewmatrix, rs.projmatrix, rs.campos))
 
@@ -245,11 +300,24 @@ def rasterize_gaussians_feature_geometry(means3D, means2D, sh, colors_precomp, s
                       cov3Ds_precomp, raster_settings, True)
 
 
+def rasterize_gaussians_alpha_invdepth(means3D, means2D, sh, colors_precomp, semantic_feature, opacities, scales,
+                                       rotations, cov3Ds_precomp, raster_settings, feature_geometry=False,
+                                       antialiasing=False):
+    """rasterize_gaussians (feature_geometry=True: rasterize_gaussians_feature_geometry; antialiasing=True: the
+    antialiased render) that also returns the opacity plane alpha = 1 - T_final and the inverse-depth plane
+    invdepth = sum_i w_i / z_i, [1,H,W] float32 each, and differentiates them ->
+    (color, feature_map, radii, depth, alpha, invdepth).  Everything else, gradients included, is bitwise that of the
+    call without the planes."""
+    return _rasterize_alpha_invdepth(means3D, means2D, sh, colors_precomp, semantic_feature, opacities, scales,
+                                     rotations, cov3Ds_precomp, raster_settings, feature_geometry, antialiasing)
+
+
 class GaussianRasterizer(nn.Module):
     """The reference's rasterizer module.  feature_geometry=True: the backward also feeds the feature map's gradient
     into the geometry (rasterize_gaussians_feature_geometry)."""
 
     antialiasing = False  # AntialiasedGaussianRasterizer
+    _render = staticmethod(_rasterize)  # AlphaInvDepthGaussianRasterizer
 
     def __init__(self, raster_settings, feature_geometry=False):
         super().__init__()
@@ -281,8 +349,8 @@ class GaussianRasterizer(nn.Module):
             rotations = empty
         if cov3D_precomp is None:
             cov3D_precomp = empty
-        return _rasterize(means3D, means2D, shs, colors_precomp, semantic_feature, opacities, scales, rotations,
-                          cov3D_precomp, rs, self.feature_geometry, self.antialiasing)
+        return self._render(means3D, means2D, shs, colors_precomp, semantic_feature, opacities, scales, rotations,
+                            cov3D_precomp, rs, self.feature_geometry, self.antialiasing)
 
 
 class AntialiasedGaussianRasterizer(GaussianRasterizer):
@@ -292,3 +360,16 @@ class AntialiasedGaussianRasterizer(GaussianRasterizer):
     GaussianRasterizer's."""
 
     antialiasing = True
+
+
+class AlphaInvDepthGaussianRasterizer(GaussianRasterizer):
+    """GaussianRasterizer whose forward also returns the opacity and inverse-depth planes:
+    (color, feature_map, radii, depth, alpha, invdepth), alpha = 1 - T_final and invdepth = sum_i w_i / z_i, [1,H,W]
+    float32 each, both differentiable (rasterize_gaussians_alpha_invdepth).  antialiasing=True renders with
+    AntialiasedGaussianRasterizer's opacities."""
+
+    _render = staticmethod(_rasterize_alpha_invdepth)
+
+    def __init__(self, raster_settings, feature_geometry=False, antialiasing=False):
+        super().__init__(raster_settings, feature_geometry)
+        self.antialiasing = antialiasing

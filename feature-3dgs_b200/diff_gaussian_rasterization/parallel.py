@@ -149,21 +149,34 @@ class ViewBatch:
         """One view's forward (no autograd graph).  `rs` is a GaussianRasterizationSettings.  antialiasing=True renders
         with the antialiased opacities (AntialiasedGaussianRasterizer); the returned ctx remembers it, so that
         `backward` differentiates the same model."""
+        fn = self._C.rasterize_gaussians_antialiased if antialiasing else self._C.rasterize_gaussians
+        (color, feat, depth), ctx = self._forward(fn, rs, antialiasing)
+        return color, feat, ctx.radii, depth, ctx
+
+    def forward_alpha_invdepth(self, rs, antialiasing: bool = False):
+        """forward() that also renders the opacity plane alpha = 1 - T_final and the inverse-depth plane
+        invdepth = sum_i w_i / z_i ([1,H,W] float32 each; AlphaInvDepthGaussianRasterizer) ->
+        (color, feat, radii, depth, alpha, invdepth, ctx).  Their gradients go to backward(..., g_alpha=, g_invdepth=)."""
+        fn = lambda *args: self._C.rasterize_gaussians_alpha_invdepth(*args, antialiasing=antialiasing)  # noqa: E731
+        (color, feat, depth, alpha, invdepth), ctx = self._forward(fn, rs, antialiasing)
+        return color, feat, ctx.radii, depth, alpha, invdepth, ctx
+
+    def _forward(self, fn, rs, antialiasing):
+        """The native forward `fn` of one view -> (its images, the view's ctx)"""
         p = self.params
         e = torch.Tensor([])
         sf = p.get("semantic_feature", self._empty)
-        fn = self._C.rasterize_gaussians_antialiased if antialiasing else self._C.rasterize_gaussians
         out = fn(rs.bg, p["means3D"], e, sf, p["opacities"], p["scales"], p["rotations"], rs.scale_modifier, e,
                  rs.viewmatrix, rs.projmatrix, rs.tanfovx, rs.tanfovy, rs.image_height, rs.image_width, p["shs"],
                  rs.sh_degree, rs.campos, rs.prefiltered, rs.debug)
         ctx = _ViewCtx()
         ctx.rs = rs
         ctx.antialiasing = bool(antialiasing)
-        ctx.num_rendered, color, feat, depth, ctx.radii, ctx.geom, ctx.binning, ctx.img = out
-        return color, feat, ctx.radii, depth, ctx
+        ctx.num_rendered, *images, ctx.radii, ctx.geom, ctx.binning, ctx.img = out
+        return images, ctx
 
     def backward(self, ctx, g_color, g_feature, g_depth, means2D_out=None, last: bool = False, camera: bool = False,
-                 feature_geometry: bool = False):
+                 feature_geometry: bool = False, g_alpha=None, g_invdepth=None):
         """Add this view's parameter gradients into the flat buffer.  `last=True` on the rank's last view of the step
         lets all_reduce() start the feature/opacity bucket early.  g_feature: dL/dfeature_map as a float32 or float16
         [C,H,W] tensor, a feature_head.ScaledGrad (a float16 map and its float32 scale), or None.
@@ -178,7 +191,12 @@ class ViewBatch:
 
         A view rendered by forward(rs, antialiasing=True) is differentiated in that mode
         (f3dgs_backward_accum_antialiased); its opacity gradient is final only after the backward preprocess, so the
-        early bucket of a `last=True` view then starts after it."""
+        early bucket of a `last=True` view then starts after it.
+
+        g_alpha / g_invdepth: dL/dalpha and dL/dinvdepth [1,H,W] float32 of forward_alpha_invdepth's planes
+        (f3dgs_backward_accum_alpha_invdepth; one given alone: the other is zero).  The buffers of either forward take
+        them, and they combine with camera, feature_geometry and a ScaledGrad g_feature; with both None the call is the
+        one without them."""
         rs, p, g, e = ctx.rs, self.params, self.grads, torch.Tensor([])
         none = self._empty
         scale = 1.0
@@ -193,7 +211,7 @@ class ViewBatch:
             none, means2D_out if means2D_out is not None else none,
             self.grad_accum if self.grad_accum is not None else none, self.denom if self.denom is not None else none,
             int(self._ev.cuda_event) if (last and self._ev is not None) else 0, rs.debug, float(scale), cam,
-            p.get("semantic_feature") if feature_geometry else None, ctx.antialiasing)
+            p.get("semantic_feature") if feature_geometry else None, ctx.antialiasing, g_alpha, g_invdepth)
         self._early_pending = bool(last and self._ev is not None)
         if cam is not None:
             return CameraGrad(cam[:16].view(4, 4), cam[16:32].view(4, 4), cam[32:35])

@@ -39,7 +39,7 @@ extern "C" {
 #define F3DGS_MAX_FEATURE_DIM 4096
 #define F3DGS_TILE 16 /* BLOCK_X == BLOCK_Y == 16, reference config.h:18-19 */
 #define F3DGS_CAMERA_GRAD_FLOATS 35 /* dL_dcamera of the _cam backward entries */
-/* element-type codes of the _feature_geometry and _antialiased entries */
+/* element-type codes of the _feature_geometry, _antialiased and _alpha_invdepth entries */
 #define F3DGS_F32 0 /* IEEE binary32 */
 #define F3DGS_F16 1 /* IEEE binary16 */
 
@@ -392,9 +392,87 @@ int f3dgs_backward_accum_antialiased(int P, int D, int M, int R, int C,
                                      float* dL_drot, float* dL_dmean2D_out, float* grad_accum, float* denom,
                                      void* composite_done_event, int debug, void* cuda_stream, float* dL_dcamera);
 
+/* ---- opacity and inverse-depth maps (opt-in; no reference counterpart: the upstream 3DGS rasterizer's 2024 update
+ * returns an inverse-depth map, and its image buffer's final transmittance is the opacity map's complement) ----
+ * For pixel p the composite blends pairs i front to back with w_i = alpha_i T_i, exactly as the other forwards do.  The
+ * _alpha_invdepth entries add two float32 planes [1,H,W] (whatever the feature element type):
+ *     alpha     A_p = 1 - T_final,p       written as 1.f - T from the T that goes to final_T: bitwise 1 - final_T;
+ *     invdepth  I_p = sum_i w_i / z_i     z_i the splat record's view depth (the value `depth` blends), 1/z_i the
+ *                                         correctly rounded reciprocal; no background term.
+ * With C > 128 (several channel chunks) chunk 0 writes them, as it writes colour and depth.
+ *   f3dgs_forward_alpha_invdepth: f3dgs_forward_antialiased's arguments, then antialiasing (0: the default forward's
+ *     opacities, else the antialiased forward's op_eff), out_alpha and out_invdepth (both required).  Colour, the
+ *     feature map, depth, radii, the return value and the three buffers are bitwise those of f3dgs_forward / _f16 /
+ *     _antialiased for the same arguments.
+ *   f3dgs_backward_alpha_invdepth / f3dgs_backward_accum_alpha_invdepth: the arguments of f3dgs_backward_antialiased /
+ *     f3dgs_backward_accum_antialiased (semantic_feature optional: given, the feature term of dL/dalpha is added;
+ *     dL_dcamera optional), then antialiasing (0: the composite's opacity gradient goes straight to dL_dopacity, as in
+ *     the default entries; else as in the _antialiased entries), dL_dalpha = dL/dA and dL_dinvdepth = dL/dI ([H,W]
+ *     float32, both required).  With gA_p = dL_dalpha[p], gI_p = dL_dinvdepth[p] the composite adds
+ *         dL/dalpha_i += gA_p T_final,p / (1 - alpha_i)        (the background term with bg.dL/dpix - gA_p),
+ *         dL/dalpha_i += T_i (1/z_i - B_i) gI_p,   B_i = alpha_{i+1} / z_{i+1} + (1 - alpha_{i+1}) B_{i+1},   B_last = 0,
+ *         dL/dz_i     -= sum_p w_ip gI_p / z_i^2,
+ *     which reach dL_dopacity, dL_dmean2D, dL_dconic, dL_dz and through the preprocess dL_dmean3D, dL_dscale, dL_drot,
+ *     dL_dcov3D, dL_dcamera and the densification statistics.  dL_dcolor and dL_dsemantic_feature are unchanged.  With
+ *     dL_dalpha = dL_dinvdepth = 0 every output is bitwise that of the counterpart: f3dgs_backward[_f16], _cam[_f16],
+ *     _feature_geometry or _antialiased (and their _accum twins) for the same remaining arguments.
+ *   F3DGS_ERR_INVALID_ARGUMENT, before any launch, for a NULL plane, a plane overlapping another output (the forward's
+ *     planes: out_color, out_feature_map, out_depth, radii or each other; the backward's plane gradients: any output),
+ *     an unknown dtype code and whatever the counterpart rejects.
+ * Buffers: the backward reads only what every forward stores (splat records, final_T, n_contrib); the planes are not
+ * kept.  So the buffers of f3dgs_forward_alpha_invdepth and those of the counterpart forward with the same antialiasing
+ * go to either backward, with bitwise equal gradients.  The antialiasing flag must match the forward's, as between the
+ * _antialiased entries and the others. */
+int f3dgs_forward_alpha_invdepth(f3dgs_alloc_fn geometry_alloc, void* geometry_ctx,
+                                 f3dgs_alloc_fn binning_alloc, void* binning_ctx,
+                                 f3dgs_alloc_fn image_alloc, void* image_ctx,
+                                 int P, int D, int M, int C,
+                                 const float* background, int width, int height,
+                                 const float* means3D, const float* shs, const float* colors_precomp,
+                                 const void* semantic_feature, int semantic_feature_dtype, const float* opacities,
+                                 const float* scales, float scale_modifier, const float* rotations,
+                                 const float* cov3D_precomp,
+                                 const float* viewmatrix, const float* projmatrix, const float* cam_pos,
+                                 float tan_fovx, float tan_fovy, int prefiltered,
+                                 float* out_color, void* out_feature_map, float* out_depth, int* radii,
+                                 int debug, void* cuda_stream,
+                                 int antialiasing, float* out_alpha, float* out_invdepth);
+int f3dgs_backward_alpha_invdepth(int P, int D, int M, int R, int C,
+                                  const float* background, int width, int height,
+                                  const float* means3D, const float* shs, const float* colors_precomp,
+                                  const void* semantic_feature, int semantic_feature_dtype,
+                                  const float* scales, float scale_modifier, const float* rotations,
+                                  const float* cov3D_precomp,
+                                  const float* viewmatrix, const float* projmatrix, const float* cam_pos,
+                                  float tan_fovx, float tan_fovy, const int* radii,
+                                  char* geom_buffer, char* binning_buffer, char* image_buffer,
+                                  const float* dL_dpix, const void* dL_dfeaturepix, int dL_dfeaturepix_dtype,
+                                  float dL_dfeaturepix_scale, const float* dL_depths,
+                                  float* dL_dmean2D, float* dL_dconic, float* dL_dopacity, float* dL_dcolor,
+                                  float* dL_dsemantic_feature, float* dL_dmean3D, float* dL_dcov3D,
+                                  float* dL_dsh, float* dL_dscale, float* dL_drot, float* dL_dz,
+                                  int debug, void* cuda_stream, float* dL_dcamera,
+                                  int antialiasing, const float* dL_dalpha, const float* dL_dinvdepth);
+int f3dgs_backward_accum_alpha_invdepth(int P, int D, int M, int R, int C,
+                                        const float* background, int width, int height,
+                                        const float* means3D, const float* shs, const float* colors_precomp,
+                                        const void* semantic_feature, int semantic_feature_dtype,
+                                        const float* scales, float scale_modifier, const float* rotations,
+                                        const float* cov3D_precomp,
+                                        const float* viewmatrix, const float* projmatrix, const float* cam_pos,
+                                        float tan_fovx, float tan_fovy, const int* radii,
+                                        char* geom_buffer, char* binning_buffer, char* image_buffer,
+                                        const float* dL_dpix, const void* dL_dfeaturepix, int dL_dfeaturepix_dtype,
+                                        float dL_dfeaturepix_scale, const float* dL_depths, char* scratch,
+                                        float* dL_dopacity, float* dL_dcolors_precomp, float* dL_dsemantic_feature,
+                                        float* dL_dmean3D, float* dL_dcov3D_precomp, float* dL_dsh, float* dL_dscale,
+                                        float* dL_drot, float* dL_dmean2D_out, float* grad_accum, float* denom,
+                                        void* composite_done_event, int debug, void* cuda_stream, float* dL_dcamera,
+                                        int antialiasing, const float* dL_dalpha, const float* dL_dinvdepth);
+
 /* ---- feature lifting (no reference counterpart): training-free back-projection of 2-D feature maps onto Gaussians ----
- * The buffers and R are those of an f3dgs_forward / _f16 / _antialiased of this view at width x height (any C of that
- * forward, 0 included); feature_map [C,H,W] is a map at that resolution, 1 <= C <= F3DGS_MAX_FEATURE_DIM.
+ * The buffers and R are those of an f3dgs_forward / _f16 / _antialiased / _alpha_invdepth of this view at width x height
+ * (any C of that forward, 0 included); feature_map [C,H,W] is a map at that resolution, 1 <= C <= F3DGS_MAX_FEATURE_DIM.
  * ACCUMULATES:  feature_sum[P,C] += sum_p w_ip * feature_map[:,p];   weight_sum[P] += sum_p w_ip,
  * w_ip = the blend weight alpha*T of Gaussian i at pixel p (the backward's unwound T: equal to the forward's blend weight
  * to a few ulp).  Over views, feature_sum / weight_sum is the blend-weighted mean of the maps per Gaussian.  The result
