@@ -1485,6 +1485,55 @@ int f3dgs_adam_step_f16out(int kind, size_t n, int M, float* param, const float*
                                      (cudaStream_t)cuda_stream, reinterpret_cast<__half*>(param_f16)));
 }
 
+}  // extern "C"
+
+namespace {
+// The checks shared by the masked Adam entries: < 0 the rejection, 0 nothing to do (n == 0), 1 launch
+int check_adam_masked(const Api& api, int kind, size_t n, int P, int M, int step, bool null_pointer) {
+    if (kind < F3DGS_PARAM_IDENTITY || kind > F3DGS_PARAM_SH_REST) return api.invalid("unknown parameter kind");
+    if (step < 0) return api.invalid("step < 0");
+    if ((kind == F3DGS_PARAM_SH_DC || kind == F3DGS_PARAM_SH_REST) && M < (kind == F3DGS_PARAM_SH_REST ? 2 : 1))
+        return api.invalid("M < 1 for F3DGS_PARAM_SH_DC or M < 2 for F3DGS_PARAM_SH_REST");
+    if (n == 0) return 0;
+    if (null_pointer) return api.invalid("NULL pointer");
+    if (P < 1 || n % (size_t)P != 0) return api.invalid("P < 1 or n % P != 0");
+    const size_t width = n / (size_t)P;
+    const size_t row[6] = {width, 1, 3, 4, 3, 3 * (size_t)(M - 1)};  // by kind; IDENTITY rows have any width
+    if (width != row[kind])
+        return api.invalid("n / P is not the row width of the kind (SIGMOID 1, EXP 3, NORMALIZE4 4, SH_DC 3, SH_REST "
+                           "3 (M - 1))");
+    return 1;
+}
+}  // namespace
+
+extern "C" {
+
+int f3dgs_adam_step_masked(int kind, size_t n, int P, int M, float* param, const float* grad_activated, float* exp_avg,
+                           float* exp_avg_sq, const uint8_t* visible, float lr, float beta1, float beta2, float eps,
+                           int step, void* cuda_stream) {
+    const Api api(__func__);
+    const int rc =
+        check_adam_masked(api, kind, n, P, M, step, !param || !grad_activated || !exp_avg || !exp_avg_sq || !visible);
+    if (rc <= 0) return rc;
+    return api.cuda(launch_adam_step(kind, n, M, param, grad_activated, exp_avg, exp_avg_sq, lr, beta1, beta2, eps, step,
+                                     (cudaStream_t)cuda_stream, nullptr, visible, P));
+}
+
+int f3dgs_adam_step_masked_f16out(int kind, size_t n, int P, int M, float* param, const float* grad_activated,
+                                  float* exp_avg, float* exp_avg_sq, const uint8_t* visible, uint16_t* param_f16,
+                                  float lr, float beta1, float beta2, float eps, int step, void* cuda_stream) {
+    const Api api(__func__);
+    if (kind != F3DGS_PARAM_IDENTITY) return api.invalid("kind must be F3DGS_PARAM_IDENTITY");
+    const int rc = check_adam_masked(api, kind, n, P, M, step,
+                                     !param || !grad_activated || !exp_avg || !exp_avg_sq || !visible || !param_f16);
+    if (rc <= 0) return rc;
+    if (overlaps({param_f16, n * 2},
+                 {{param, n * 4}, {grad_activated, n * 4}, {exp_avg, n * 4}, {exp_avg_sq, n * 4}, {visible, (size_t)P}}))
+        return api.invalid("param_f16 overlaps param, grad_activated, exp_avg, exp_avg_sq or visible");
+    return api.cuda(launch_adam_step(kind, n, M, param, grad_activated, exp_avg, exp_avg_sq, lr, beta1, beta2, eps, step,
+                                     (cudaStream_t)cuda_stream, reinterpret_cast<__half*>(param_f16), visible, P));
+}
+
 int f3dgs_mark_visible(int P, const float* means3D, const float* viewmatrix, const float* projmatrix,
                        uint8_t* present, void* cuda_stream) {
     (void)projmatrix;  // the reference's frustum side test is commented out (auxiliary.h:160)

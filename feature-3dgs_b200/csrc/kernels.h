@@ -175,9 +175,10 @@ cudaError_t launch_reset_opacity(int P, float* raw_opacity, float* exp_avg, floa
 cudaError_t launch_activate(int P, int M, const float* raw_opacity, const float* raw_scaling, const float* raw_rotation,
                             const float* features_dc, const float* features_rest, float* opacity, float* scales,
                             float* rotations, float* shs, cudaStream_t s);
-// param_f16 (IDENTITY only, may be NULL): also written, half_rn of the updated param
+// param_f16 (IDENTITY only, may be NULL): also written, half_rn of the updated param.  visible (may be NULL): P bytes, the
+// rows of n / P elements to update (nonzero); the others are left untouched.  step == 0: no bias correction
 cudaError_t launch_adam_step(int kind, size_t n, int M, float* param, const float* grad_activated, float* exp_avg,
                              float* exp_avg_sq, float lr, float beta1, float beta2, float eps, int step, cudaStream_t s,
-                             __half* param_f16 = nullptr);
+                             __half* param_f16 = nullptr, const uint8_t* visible = nullptr, int P = 0);
 
 }  // namespace f3dgs

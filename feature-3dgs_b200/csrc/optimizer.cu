@@ -15,6 +15,9 @@
 //                     v <- b2 v + (1 - b2) g^2, p <- p - (lr / (1 - b1^t)) m / (sqrt(v) / sqrt(1 - b2^t) + eps).
 //                     With kHalfOut (IDENTITY groups: float16 feature fields) the same pass also writes the float16
 //                     working copy half_rn(p) of the float32 master, instead of a separate cast pass after the step.
+//                     With kMasked only the rows (Gaussians) marked in `visible` are updated (the sparse Adam of the
+//                     upstream rasterizer's SparseGaussianAdam): any other row's param, m, v and float16 copy are neither
+//                     read nor written, and a visible row gets bitwise the dense step's result.
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -72,11 +75,38 @@ __device__ __forceinline__ void adam_update(float& p, float& m, float& v, float 
     p = p - a.lr_over_bc1 * (m / denom);
 }
 
-template <bool kHalfOut>
-__global__ void __launch_bounds__(256) adam_step_kernel(AdamArgs a, __half* __restrict__ param_f16) {
+// The row of element i of a raw parameter whose rows are `width` elements wide (32-bit division where n allows it)
+__device__ __forceinline__ size_t row_of(size_t i, size_t n, size_t width) {
+    return n <= UINT32_MAX ? (size_t)((uint32_t)i / (uint32_t)width) : i / width;
+}
+
+// Index in the activated gradient of element i of the raw parameter
+__device__ __forceinline__ size_t grad_index(const AdamArgs& a, size_t i) {
+    switch (a.kind) {
+        case F3DGS_PARAM_SH_DC: return (i / 3) * 3 * (size_t)a.M + (i % 3);
+        case F3DGS_PARAM_SH_REST: {
+            const size_t per = 3 * (size_t)(a.M - 1);
+            return (i / per) * 3 * (size_t)a.M + 3 + (i % per);
+        }
+        default: return i;
+    }
+}
+
+constexpr int kMaskedPerThread = 4;
+
+// kMasked: visible [n / width] bytes, nonzero = update the row.  NORMALIZE4 keeps one float4 thread per row.  Every
+// other kind takes kMaskedPerThread elements 256 apart per thread: it reads their rows' mask bytes first and then the
+// visible elements' operands together, so the mask's latency is paid once per kMaskedPerThread elements instead of
+// before each element's loads (with one element per thread, the step with every row visible took 14 % longer than the
+// dense one on an H100 80GB HBM3 at 700 W).  The arithmetic of a visible element is the dense path's, so its results are bitwise the same.
+template <bool kHalfOut, bool kMasked>
+__global__ void __launch_bounds__(256) adam_step_kernel(AdamArgs a, __half* __restrict__ param_f16,
+                                                        const uint8_t* __restrict__ visible, size_t width) {
     const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (a.kind == F3DGS_PARAM_NORMALIZE4) {
         if (i >= a.n / 4) return;
+        if constexpr (kMasked)
+            if (!visible[i]) return;
         float4 r = reinterpret_cast<float4*>(a.param)[i];
         const float4 g = reinterpret_cast<const float4*>(a.grad)[i];
         const float nrm = fmaxf(sqrtf(r.x * r.x + r.y * r.y + r.z * r.z + r.w * r.w), 1e-12f);
@@ -92,6 +122,44 @@ __global__ void __launch_bounds__(256) adam_step_kernel(AdamArgs a, __half* __re
         reinterpret_cast<float4*>(a.param)[i] = r;
         reinterpret_cast<float4*>(a.m)[i] = m;
         reinterpret_cast<float4*>(a.v)[i] = v;
+        return;
+    }
+    if constexpr (kMasked) {
+        constexpr int K = kMaskedPerThread;
+        const size_t i0 = (size_t)blockIdx.x * (256 * K) + threadIdx.x;
+        bool on[K];
+        float p[K], g[K], m[K], v[K];
+#pragma unroll
+        for (int k = 0; k < K; k++) {
+            const size_t j = i0 + 256 * k;
+            on[k] = j < a.n && visible[row_of(j, a.n, width)];
+        }
+#pragma unroll
+        for (int k = 0; k < K; k++) {
+            const size_t j = i0 + 256 * k;
+            if (on[k]) {
+                p[k] = a.param[j];
+                g[k] = a.grad[grad_index(a, j)];
+                m[k] = a.m[j];
+                v[k] = a.v[j];
+            }
+        }
+#pragma unroll
+        for (int k = 0; k < K; k++) {
+            const size_t j = i0 + 256 * k;
+            if (!on[k]) continue;
+            if (a.kind == F3DGS_PARAM_SIGMOID) {
+                const float o = 1.0f / (1.0f + expf(-p[k]));
+                g[k] = g[k] * o * (1.0f - o);
+            } else if (a.kind == F3DGS_PARAM_EXP) {
+                g[k] = g[k] * expf(p[k]);
+            }
+            adam_update(p[k], m[k], v[k], g[k], a);
+            a.param[j] = p[k];
+            a.m[j] = m[k];
+            a.v[j] = v[k];
+            if constexpr (kHalfOut) param_f16[j] = __float2half_rn(p[k]);
+        }
         return;
     }
     if (i >= a.n) return;
@@ -133,19 +201,33 @@ cudaError_t launch_activate(int P, int M, const float* raw_opacity, const float*
 
 cudaError_t launch_adam_step(int kind, size_t n, int M, float* param, const float* grad_activated, float* exp_avg,
                              float* exp_avg_sq, float lr, float beta1, float beta2, float eps, int step, cudaStream_t s,
-                             __half* param_f16) {
+                             __half* param_f16, const uint8_t* visible, int P) {
     AdamArgs a;
     a.param = param; a.grad = grad_activated; a.m = exp_avg; a.v = exp_avg_sq; a.n = n; a.kind = kind; a.M = M;
-    const double bc1 = 1.0 - pow((double)beta1, (double)step), bc2 = 1.0 - pow((double)beta2, (double)step);
-    a.lr_over_bc1 = (float)((double)lr / bc1);
-    a.inv_sqrt_bc2 = (float)(1.0 / sqrt(bc2));
+    if (step == 0) {  // no bias correction
+        a.lr_over_bc1 = lr;
+        a.inv_sqrt_bc2 = 1.0f;
+    } else {
+        const double bc1 = 1.0 - pow((double)beta1, (double)step), bc2 = 1.0 - pow((double)beta2, (double)step);
+        a.lr_over_bc1 = (float)((double)lr / bc1);
+        a.inv_sqrt_bc2 = (float)(1.0 / sqrt(bc2));
+    }
     a.b1 = beta1; a.b2 = beta2; a.eps = eps;
     const size_t threads = kind == F3DGS_PARAM_NORMALIZE4 ? n / 4 : n;
     const unsigned grid = (unsigned)((threads + 255) / 256);
-    if (param_f16)
-        adam_step_kernel<true><<<grid, 256, 0, s>>>(a, param_f16);
-    else
-        adam_step_kernel<false><<<grid, 256, 0, s>>>(a, nullptr);
+    if (visible) {
+        const size_t width = n / (size_t)P;
+        const size_t per_block = kind == F3DGS_PARAM_NORMALIZE4 ? 256 : 256 * kMaskedPerThread;
+        const unsigned grid = (unsigned)((threads + per_block - 1) / per_block);
+        if (param_f16)
+            adam_step_kernel<true, true><<<grid, 256, 0, s>>>(a, param_f16, visible, width);
+        else
+            adam_step_kernel<false, true><<<grid, 256, 0, s>>>(a, nullptr, visible, width);
+    } else if (param_f16) {
+        adam_step_kernel<true, false><<<grid, 256, 0, s>>>(a, param_f16, nullptr, 0);
+    } else {
+        adam_step_kernel<false, false><<<grid, 256, 0, s>>>(a, nullptr, nullptr, 0);
+    }
     g_launches++;
     return cudaGetLastError();
 }

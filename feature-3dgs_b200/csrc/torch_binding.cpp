@@ -1046,10 +1046,11 @@ void activateParams(const torch::Tensor& raw_opacity, const torch::Tensor& raw_s
 }
 
 // param_f16 (optional, IDENTITY groups): a contiguous float16 tensor of param's size, written with param.half() after
-// the step (f3dgs_adam_step_f16out)
+// the step (f3dgs_adam_step_f16out).  visible (optional): a contiguous bool or uint8 tensor of P elements on param's
+// device; only the rows it marks (P rows of numel / P elements) are stepped (f3dgs_adam_step_masked[_f16out])
 void adamStep(int64_t kind, torch::Tensor param, const torch::Tensor& grad_activated, torch::Tensor exp_avg,
               torch::Tensor exp_avg_sq, int64_t M, double lr, double beta1, double beta2, double eps, int64_t step,
-              const c10::optional<torch::Tensor>& param_f16) {
+              const c10::optional<torch::Tensor>& param_f16, const c10::optional<torch::Tensor>& visible) {
     TORCH_CHECK(param.is_cuda(), "parameters must be CUDA tensors (this build has no CPU path)");
     const auto dev = param.device();
     const c10::cuda::CUDAGuard guard(dev);
@@ -1058,13 +1059,35 @@ void adamStep(int64_t kind, torch::Tensor param, const torch::Tensor& grad_activ
     cudaStream_t stream = c10::cuda::getCurrentCUDAStream().stream();
     float* p = in_place(param, dev, n, "param");
     float *m = in_place(exp_avg, dev, n, "exp_avg"), *v = in_place(exp_avg_sq, dev, n, "exp_avg_sq");
+    uint16_t* h16 = nullptr;
     if (param_f16.has_value() && param_f16->defined()) {
         const torch::Tensor& h = *param_f16;
         TORCH_CHECK(h.is_cuda() && h.device() == dev && h.scalar_type() == torch::kFloat16 && h.is_contiguous() &&
                         h.numel() == n,
                     "param_f16 must be a contiguous float16 tensor of ", n, " elements on ", dev);
-        check_rc(f3dgs_adam_step_f16out((int)kind, (size_t)n, (int)M, p, fptr(g), m, v,
-                                        reinterpret_cast<uint16_t*>(h.data_ptr<at::Half>()), (float)lr, (float)beta1,
+        h16 = reinterpret_cast<uint16_t*>(h.data_ptr<at::Half>());
+    }
+    if (visible.has_value() && visible->defined()) {
+        const torch::Tensor& mask = *visible;
+        TORCH_CHECK(mask.is_cuda() && mask.device() == dev &&
+                        (mask.scalar_type() == torch::kBool || mask.scalar_type() == torch::kByte) &&
+                        mask.is_contiguous() && mask.numel() <= INT32_MAX,
+                    "visible must be a contiguous bool or uint8 tensor of P < 2^31 elements on ", dev);
+        const int P = (int)mask.numel();
+        const uint8_t* vis = P ? reinterpret_cast<const uint8_t*>(mask.data_ptr()) : nullptr;
+        if (h16)
+            check_rc(f3dgs_adam_step_masked_f16out((int)kind, (size_t)n, P, (int)M, p, fptr(g), m, v, vis, h16,
+                                                   (float)lr, (float)beta1, (float)beta2, (float)eps, (int)step,
+                                                   (void*)stream),
+                     "f3dgs_adam_step_masked_f16out");
+        else
+            check_rc(f3dgs_adam_step_masked((int)kind, (size_t)n, P, (int)M, p, fptr(g), m, v, vis, (float)lr,
+                                            (float)beta1, (float)beta2, (float)eps, (int)step, (void*)stream),
+                     "f3dgs_adam_step_masked");
+        return;
+    }
+    if (h16) {
+        check_rc(f3dgs_adam_step_f16out((int)kind, (size_t)n, (int)M, p, fptr(g), m, v, h16, (float)lr, (float)beta1,
                                         (float)beta2, (float)eps, (int)step, (void*)stream),
                  "f3dgs_adam_step_f16out");
         return;
@@ -1164,7 +1187,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     m.def("adam_step", &adamStep, pybind11::arg("kind"), pybind11::arg("param"), pybind11::arg("grad_activated"),
           pybind11::arg("exp_avg"), pybind11::arg("exp_avg_sq"), pybind11::arg("M"), pybind11::arg("lr"),
           pybind11::arg("beta1"), pybind11::arg("beta2"), pybind11::arg("eps"), pybind11::arg("step"),
-          pybind11::arg("param_f16") = pybind11::none());
+          pybind11::arg("param_f16") = pybind11::none(), pybind11::arg("visible") = pybind11::none());
     m.def("backward_scratch_bytes", [](int P) { return (unsigned long long)f3dgs_backward_scratch_bytes(P); });
     m.def("debug_views", &debugViews);
     m.def("launch_count", []() { return (unsigned long long)f3dgs_launch_count(); });

@@ -41,6 +41,9 @@ Behavioural notes
     opacity) and invdepth = sum_i w_i / z_i, both [1,H,W] float32 and differentiable (f3dgs_forward_alpha_invdepth /
     f3dgs_backward_alpha_invdepth): mask losses, RGBA cut-outs, expected depth depth / alpha and inverse-depth
     supervision.  Colour, feature map, depth, radii and their gradients are those of the rasterizer without the maps.
+  * sparse Adam (opt-in): `SparseGaussianAdam(params, lr, eps)` with `.step(visibility, N)` is the upstream
+    rasterizer's optimizer of that name: it updates only the Gaussians marked visible (f3dgs_adam_step_masked), without
+    bias correction, and leaves the others' parameters and moments untouched.
   * `debug=True` keeps the reference semantics: arguments are snapshotted to CPU first and dumped
     to snapshot_fw.dump / snapshot_bw.dump if the native call raises (reference :89-97,:147-155);
     natively it synchronises and checks after every stage.
@@ -69,6 +72,7 @@ __all__ = [
     "AntialiasedGaussianRasterizer",
     "rasterize_gaussians_alpha_invdepth",
     "AlphaInvDepthGaussianRasterizer",
+    "SparseGaussianAdam",
 ]
 
 
@@ -373,3 +377,40 @@ class AlphaInvDepthGaussianRasterizer(GaussianRasterizer):
     def __init__(self, raster_settings, feature_geometry=False, antialiasing=False):
         super().__init__(raster_settings, feature_geometry)
         self.antialiasing = antialiasing
+
+
+class SparseGaussianAdam(torch.optim.Adam):
+    """Sparse Adam for the autograd path (GaussianRasterizer on raw parameters): the upstream 3DGS rasterizer's
+    SparseGaussianAdam, called the same way,
+
+        optimizer = SparseGaussianAdam(param_groups, lr=0.0, eps=1e-15)
+        ...
+        optimizer.step(visibility=radii > 0, N=P)
+
+    Each group holds one parameter of N rows (any trailing shape).  step() updates only the rows marked in
+    `visibility` (bool or uint8 [N], on the parameter's device), with betas 0.9 and 0.999 and no bias correction:
+    m = 0.9 m + 0.1 g, v = 0.999 v + 0.001 g^2, p -= lr m / (sqrt(v) + eps), in one native pass per group
+    (f3dgs_adam_step_masked, step 0).  The other rows keep parameter and moments bitwise.  Groups whose parameter has
+    no gradient are skipped.  The moments live in torch Adam's state keys (exp_avg, exp_avg_sq, and step, which stays
+    0), so code that edits optimizer.state[param] directly, as the reference's densification does, keeps working."""
+
+    def __init__(self, params, lr, eps):
+        super().__init__(params=params, lr=lr, eps=eps)
+
+    @torch.no_grad()
+    def step(self, visibility, N):
+        if visibility.numel() != N:
+            raise ValueError(f"visibility has {visibility.numel()} elements, expected N = {N}")
+        for group in self.param_groups:
+            if len(group["params"]) != 1:
+                raise ValueError("SparseGaussianAdam takes one parameter per group")
+            param = group["params"][0]
+            if param.grad is None:
+                continue
+            state = self.state[param]
+            if len(state) == 0:
+                state["step"] = torch.tensor(0.0, dtype=torch.float32)
+                state["exp_avg"] = torch.zeros_like(param, memory_format=torch.preserve_format)
+                state["exp_avg_sq"] = torch.zeros_like(param, memory_format=torch.preserve_format)
+            _C.adam_step(0, param, param.grad, state["exp_avg"], state["exp_avg_sq"], 1, float(group["lr"]), 0.9, 0.999,
+                         float(group["eps"]), 0, None, visibility)

@@ -145,6 +145,14 @@ class ViewBatch:
     def zero_(self):
         self.flat.zero_()
 
+    def visible(self) -> torch.Tensor:
+        """bool [P]: the Gaussians with radii > 0 in at least one view of the step (denom > 0), the rows outside which
+        every gradient slot is exactly zero.  After all_reduce() it is the union over every rank's views, the same on
+        every rank: the mask of GaussianState.step(lrs, visible=...).  Needs densify_stats=True."""
+        if self.denom is None:
+            raise RuntimeError("ViewBatch.visible() needs the densification statistics (densify_stats=True)")
+        return self.denom > 0
+
     def forward(self, rs, antialiasing: bool = False):
         """One view's forward (no autograd graph).  `rs` is a GaussianRasterizationSettings.  antialiasing=True renders
         with the antialiased opacities (AntialiasedGaussianRasterizer); the returned ctx remembers it, so that

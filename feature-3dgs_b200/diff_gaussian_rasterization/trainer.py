@@ -14,6 +14,7 @@ _opacity, _scaling, _rotation, _semantic_feature`, :47-58) as plain CUDA tensors
   step(lrs)             Adam (:163-190: lr per group, eps 1e-15) fused with the activations' Jacobians
                         (f3dgs_adam_step): consumes the all-reduced gradients w.r.t. the ACTIVATED tensors straight from the
                         flat buffer and updates the raw parameters in place -- no autograd graph anywhere;
+                        step(lrs, visible=vb.visible()) is the sparse Adam step on the Gaussians the step's views saw;
   densify_and_prune()   clone / split / prune (:350-434) with the optimizer state carried along, in two native calls
                         (f3dgs_densify_plan / f3dgs_densify_apply) with one host read in between;
   reset_opacity()       :231-234 in one kernel (f3dgs_reset_opacity).
@@ -133,8 +134,14 @@ class GaussianState:
         return self._batch
 
     # ---------------------------------------------------------------------------------------------- optimizer
-    def step(self, lrs: Dict[str, float], grads: Optional[Dict[str, torch.Tensor]] = None):
-        """One Adam step of every group.  `grads`: gradients w.r.t. the activated tensors (default: the ViewBatch's)."""
+    def step(self, lrs: Dict[str, float], grads: Optional[Dict[str, torch.Tensor]] = None,
+             visible: Optional[torch.Tensor] = None):
+        """One Adam step of every group.  `grads`: gradients w.r.t. the activated tensors (default: the ViewBatch's).
+
+        visible: None for the dense step, or a bool [P] CUDA mask (ViewBatch.visible() after all_reduce()) for the sparse
+        Adam step (f3dgs_adam_step_masked): only the marked Gaussians' raw parameters, moments and float16 feature copy
+        change, bitwise as in the dense step; the others stay exactly as they are, so momentum no longer moves Gaussians
+        that no view of the step saw.  Bias correction still uses each group's step count, which advances every step."""
         from . import _C
 
         g = grads if grads is not None else self.batch().grads
@@ -147,7 +154,7 @@ class GaussianState:
             half = name == "semantic_feature" and self.feature_dtype == torch.float16
             copy = self.act["semantic_feature"] if half else None
             _C.adam_step(KIND[name], p, g[GRAD_OF[name]], self.exp_avg[name], self.exp_avg_sq[name], self.M, lrs[name],
-                         self.betas[0], self.betas[1], self.eps, self.steps[name], copy)
+                         self.betas[0], self.betas[1], self.eps, self.steps[name], copy, visible)
 
     # ---------------------------------------------------------------------------------------------- densification
     def update_max_radii(self, radii):

@@ -651,6 +651,23 @@ int f3dgs_adam_step(int kind, size_t n, int M, float* param, const float* grad_a
 int f3dgs_adam_step_f16out(int kind, size_t n, int M, float* param, const float* grad_activated, float* exp_avg,
                            float* exp_avg_sq, uint16_t* param_f16, float lr, float beta1, float beta2, float eps,
                            int step, void* cuda_stream);
+/* Sparse Adam (the upstream 3DGS rasterizer's SparseGaussianAdam): f3dgs_adam_step / f3dgs_adam_step_f16out on the rows
+ * of P Gaussians marked in visible[P] (bytes, nonzero = visible) only.  The raw parameter is P rows of n / P elements:
+ * SIGMOID 1, EXP 3, NORMALIZE4 4, SH_DC 3, SH_REST 3 (M - 1), IDENTITY any width; so P >= 1 and n % P == 0.  A visible
+ * row's param, exp_avg, exp_avg_sq (and param_f16) are bitwise those of the dense entry; every other row is neither read
+ * nor written, whatever its gradient holds.  Bias correction:
+ *   step >= 1  as the dense entries, with the group's step count (it advances on every step, visible or not: one step
+ *              counter per parameter, as torch's SparseAdam);
+ *   step == 0  none (lr / (1 - b1^t) = lr, sqrt(1 - b2^t) = 1): upstream SparseGaussianAdam's update
+ *              m = b1 m + (1 - b1) g, v = b2 v + (1 - b2) g^2, p -= lr m / (sqrt(v) + eps).
+ * n == 0 is a no-op (pointers and P are not checked then).  The _f16out twin takes IDENTITY only, and its param_f16 must
+ * not overlap the other buffers. */
+int f3dgs_adam_step_masked(int kind, size_t n, int P, int M, float* param, const float* grad_activated, float* exp_avg,
+                           float* exp_avg_sq, const uint8_t* visible, float lr, float beta1, float beta2, float eps,
+                           int step, void* cuda_stream);
+int f3dgs_adam_step_masked_f16out(int kind, size_t n, int P, int M, float* param, const float* grad_activated,
+                                  float* exp_avg, float* exp_avg_sq, const uint8_t* visible, uint16_t* param_f16,
+                                  float lr, float beta1, float beta2, float eps, int step, void* cuda_stream);
 
 /* ---- initial scales: reference submodules/simple-knn distCUDA2, used by scene/gaussian_model.py:133-160 ------------
  * out[i] = (d0 + d1 + d2) / 3 in fp32, where d0 <= d1 <= d2 are the three smallest squared distances from points[i] to
