@@ -11,6 +11,7 @@
 #include <cmath>
 #include <cstdio>
 #include <cstring>
+#include <initializer_list>
 #include <mutex>
 #include <string>
 #include <type_traits>
@@ -51,12 +52,12 @@ struct Range {
     size_t bytes;
 };
 
-// Does the output range `out` share a byte with any of the ranges `in`?
+// Does the output range `out` share a byte with any of the ranges `in` other than itself (`out` may be one of them)?
 template <size_t N>
 bool overlaps(const Range& out, const Range (&in)[N]) {
     for (const Range& r : in) {
         const uintptr_t x = (uintptr_t)out.p, y = (uintptr_t)r.p;
-        if (out.p && r.p && x < y + r.bytes && y < x + out.bytes) return true;
+        if (&r != &out && out.p && r.p && x < y + r.bytes && y < x + out.bytes) return true;
     }
     return false;
 }
@@ -249,19 +250,26 @@ int f3dgs_get_layout(int P, int width, int height, int R, f3dgs_layout* out) {
 
 namespace {
 
-// Shared body of f3dgs_forward (TF = float), f3dgs_forward_f16 (TF = __half), f3dgs_forward_antialiased and
-// f3dgs_forward_alpha_invdepth: TF is the element type of semantic_feature and out_feature_map only.  antialiasing:
-// op_eff = opacity * rho in the records.  out_alpha / out_invdepth (f3dgs_forward_alpha_invdepth, which has checked that
-// both are given): the composite also writes the opacity and inverse-depth planes.
-template <typename TF>
+// Every dtype code of a typed entry is F3DGS_F32 or F3DGS_F16
+int check_dtypes(const Api& api, std::initializer_list<int> codes) {
+    for (const int t : codes)
+        if (t != F3DGS_F32 && t != F3DGS_F16) return api.invalid("unknown dtype code");
+    return 0;
+}
+
+// Shared body of f3dgs_forward, f3dgs_forward_f16, f3dgs_forward_antialiased and f3dgs_forward_alpha_invdepth.
+// semantic_feature and out_feature_map are float16 if f16, else float32.  antialiasing: op_eff = opacity * rho in the
+// records.  out_alpha / out_invdepth (f3dgs_forward_alpha_invdepth, which has checked that both are given): the
+// composite also writes the opacity and inverse-depth planes.
 int forward_impl(const char* entry, f3dgs_alloc_fn geometry_alloc, void* geometry_ctx, f3dgs_alloc_fn binning_alloc,
                  void* binning_ctx, f3dgs_alloc_fn image_alloc, void* image_ctx, int P, int D, int M, int C,
                  const float* background, int width, int height, const float* means3D, const float* shs,
-                 const float* colors_precomp, const TF* semantic_feature, const float* opacities, const float* scales,
+                 const float* colors_precomp, const void* semantic_feature, const float* opacities, const float* scales,
                  float scale_modifier, const float* rotations, const float* cov3D_precomp, const float* viewmatrix,
                  const float* projmatrix, const float* cam_pos, float tan_fovx, float tan_fovy, int prefiltered,
-                 float* out_color, TF* out_feature_map, float* out_depth, int* radii, int debug, void* cuda_stream,
-                 bool antialiasing = false, float* out_alpha = nullptr, float* out_invdepth = nullptr) {
+                 float* out_color, void* out_feature_map, float* out_depth, int* radii, int debug, void* cuda_stream,
+                 bool f16 = false, bool antialiasing = false, float* out_alpha = nullptr,
+                 float* out_invdepth = nullptr) {
     const Api api(entry);
     cudaStream_t stream = (cudaStream_t)cuda_stream;
     if (P < 0 || width <= 0 || height <= 0 || C < 0 || C > F3DGS_MAX_FEATURE_DIM || D < 0 || D > 3)
@@ -279,14 +287,12 @@ int forward_impl(const char* entry, f3dgs_alloc_fn geometry_alloc, void* geometr
     if (C > 0 && (!semantic_feature || !out_feature_map))
         return api.invalid("C > 0 needs semantic_feature and out_feature_map");
     if (shs && M < (D + 1) * (D + 1)) return api.invalid("M < (D+1)^2 SH coefficients");
-    if (out_alpha) {  // the composite writes the planes while it writes the other outputs
-        const size_t hw4 = (size_t)width * height * 4;
-        const Range a{out_alpha, hw4}, i{out_invdepth, hw4};
-        const Range outs[] = {{out_color, 3 * hw4}, {out_feature_map, (size_t)C * width * height * sizeof(TF)},
-                              {out_depth, hw4}, {radii, (size_t)P * 4}};
-        if (overlaps(a, outs) || overlaps(i, outs) || overlaps(a, {i}))
-            return api.invalid("out_alpha / out_invdepth overlap another output");
-    }
+    // the composite writes the planes while it writes the other outputs
+    const size_t hw4 = (size_t)width * height * 4;
+    const Range outs[] = {{out_color, 3 * hw4}, {out_feature_map, (size_t)C * width * height * (f16 ? 2 : 4)},
+                          {out_depth, hw4}, {radii, (size_t)P * 4}, {out_alpha, hw4}, {out_invdepth, hw4}};
+    if (overlaps(outs[4], outs) || overlaps(outs[5], outs))
+        return api.invalid("out_alpha / out_invdepth overlap another output");
 
     const ViewParams vp = make_view(P, D, M, C, width, height, tan_fovx, tan_fovy, scale_modifier, viewmatrix,
                                     projmatrix, cam_pos);
@@ -379,8 +385,14 @@ int forward_impl(const char* entry, f3dgs_alloc_fn geometry_alloc, void* geometr
     {
         StageTimer t(F3DGS_STAGE_COMPOSITE_FWD, stream);
         int* counters = reinterpret_cast<int*>(img + il.counters);
-        e = launch_composite_fwd(vp, ranges, point_list, rec, semantic_feature, background, final_T, n_contrib,
-                                 out_color, out_feature_map, out_depth, counters, stream, out_alpha, out_invdepth);
+        if (f16)
+            e = launch_composite_fwd(vp, ranges, point_list, rec, static_cast<const __half*>(semantic_feature),
+                                     background, final_T, n_contrib, out_color, static_cast<__half*>(out_feature_map),
+                                     out_depth, counters, stream, out_alpha, out_invdepth);
+        else
+            e = launch_composite_fwd(vp, ranges, point_list, rec, static_cast<const float*>(semantic_feature),
+                                     background, final_T, n_contrib, out_color, static_cast<float*>(out_feature_map),
+                                     out_depth, counters, stream, out_alpha, out_invdepth);
     }
     if (const int rc = api.cuda(e, "composite_fwd launch")) return rc;
     STAGE_CHECK("composite_fwd");
@@ -414,10 +426,9 @@ int f3dgs_forward_f16(f3dgs_alloc_fn geometry_alloc, void* geometry_ctx, f3dgs_a
                       float tan_fovy, int prefiltered, float* out_color, uint16_t* out_feature_map, float* out_depth,
                       int* radii, int debug, void* cuda_stream) {
     return forward_impl(__func__, geometry_alloc, geometry_ctx, binning_alloc, binning_ctx, image_alloc, image_ctx, P,
-                        D, M, C, background, width, height, means3D, shs, colors_precomp,
-                        reinterpret_cast<const __half*>(semantic_feature), opacities, scales, scale_modifier, rotations,
-                        cov3D_precomp, viewmatrix, projmatrix, cam_pos, tan_fovx, tan_fovy, prefiltered, out_color,
-                        reinterpret_cast<__half*>(out_feature_map), out_depth, radii, debug, cuda_stream);
+                        D, M, C, background, width, height, means3D, shs, colors_precomp, semantic_feature, opacities,
+                        scales, scale_modifier, rotations, cov3D_precomp, viewmatrix, projmatrix, cam_pos, tan_fovx,
+                        tan_fovy, prefiltered, out_color, out_feature_map, out_depth, radii, debug, cuda_stream, true);
 }
 
 int f3dgs_forward_antialiased(f3dgs_alloc_fn geometry_alloc, void* geometry_ctx, f3dgs_alloc_fn binning_alloc,
@@ -429,18 +440,12 @@ int f3dgs_forward_antialiased(f3dgs_alloc_fn geometry_alloc, void* geometry_ctx,
                               const float* viewmatrix, const float* projmatrix, const float* cam_pos, float tan_fovx,
                               float tan_fovy, int prefiltered, float* out_color, void* out_feature_map,
                               float* out_depth, int* radii, int debug, void* cuda_stream) {
-    const char* entry = __func__;
-    const auto run = [&](auto* features) {
-        using TF = std::remove_const_t<std::remove_pointer_t<decltype(features)>>;
-        return forward_impl(entry, geometry_alloc, geometry_ctx, binning_alloc, binning_ctx, image_alloc, image_ctx,
-                            P, D, M, C, background, width, height, means3D, shs, colors_precomp, features, opacities,
-                            scales, scale_modifier, rotations, cov3D_precomp, viewmatrix, projmatrix, cam_pos, tan_fovx,
-                            tan_fovy, prefiltered, out_color, static_cast<TF*>(out_feature_map), out_depth, radii,
-                            debug, cuda_stream, true);
-    };
-    if (semantic_feature_dtype == F3DGS_F32) return run(static_cast<const float*>(semantic_feature));
-    if (semantic_feature_dtype == F3DGS_F16) return run(static_cast<const __half*>(semantic_feature));
-    return Api(__func__).invalid("unknown dtype code");
+    if (const int rc = check_dtypes(Api(__func__), {semantic_feature_dtype})) return rc;
+    return forward_impl(__func__, geometry_alloc, geometry_ctx, binning_alloc, binning_ctx, image_alloc, image_ctx, P,
+                        D, M, C, background, width, height, means3D, shs, colors_precomp, semantic_feature, opacities,
+                        scales, scale_modifier, rotations, cov3D_precomp, viewmatrix, projmatrix, cam_pos, tan_fovx,
+                        tan_fovy, prefiltered, out_color, out_feature_map, out_depth, radii, debug, cuda_stream,
+                        semantic_feature_dtype == F3DGS_F16, true);
 }
 
 int f3dgs_forward_alpha_invdepth(f3dgs_alloc_fn geometry_alloc, void* geometry_ctx, f3dgs_alloc_fn binning_alloc,
@@ -453,19 +458,14 @@ int f3dgs_forward_alpha_invdepth(f3dgs_alloc_fn geometry_alloc, void* geometry_c
                                  float tan_fovx, float tan_fovy, int prefiltered, float* out_color,
                                  void* out_feature_map, float* out_depth, int* radii, int debug, void* cuda_stream,
                                  int antialiasing, float* out_alpha, float* out_invdepth) {
-    const char* entry = __func__;
-    if (!out_alpha || !out_invdepth) return Api(entry).invalid("NULL out_alpha / out_invdepth");
-    const auto run = [&](auto* features) {
-        using TF = std::remove_const_t<std::remove_pointer_t<decltype(features)>>;
-        return forward_impl(entry, geometry_alloc, geometry_ctx, binning_alloc, binning_ctx, image_alloc, image_ctx,
-                            P, D, M, C, background, width, height, means3D, shs, colors_precomp, features, opacities,
-                            scales, scale_modifier, rotations, cov3D_precomp, viewmatrix, projmatrix, cam_pos, tan_fovx,
-                            tan_fovy, prefiltered, out_color, static_cast<TF*>(out_feature_map), out_depth, radii,
-                            debug, cuda_stream, antialiasing != 0, out_alpha, out_invdepth);
-    };
-    if (semantic_feature_dtype == F3DGS_F32) return run(static_cast<const float*>(semantic_feature));
-    if (semantic_feature_dtype == F3DGS_F16) return run(static_cast<const __half*>(semantic_feature));
-    return Api(entry).invalid("unknown dtype code");
+    const Api api(__func__);
+    if (!out_alpha || !out_invdepth) return api.invalid("NULL out_alpha / out_invdepth");
+    if (const int rc = check_dtypes(api, {semantic_feature_dtype})) return rc;
+    return forward_impl(__func__, geometry_alloc, geometry_ctx, binning_alloc, binning_ctx, image_alloc, image_ctx, P,
+                        D, M, C, background, width, height, means3D, shs, colors_precomp, semantic_feature, opacities,
+                        scales, scale_modifier, rotations, cov3D_precomp, viewmatrix, projmatrix, cam_pos, tan_fovx,
+                        tan_fovy, prefiltered, out_color, out_feature_map, out_depth, radii, debug, cuda_stream,
+                        semantic_feature_dtype == F3DGS_F16, antialiasing != 0, out_alpha, out_invdepth);
 }
 
 }  // extern "C"
@@ -485,93 +485,133 @@ struct ScratchLayout {  // per-view intermediates of the accumulating backward (
     }
 };
 
-// Shared body of f3dgs_backward (accumulate = false: the reference's assign-into-zeroed-buffers contract),
-// f3dgs_backward_accum (accumulate = true: += into the caller's per-parameter gradient buffers) and their _f16 twins.
-// TG (float or __half) is the element type of dL_dfeaturepix; a __half map stands for dL/dO = scale * float(h).
-// `zero` (accumulate only): the caller's scratch, zeroed once the arguments are validated.  feat.rows (the _feature_geometry
-// entries only; NULL on every other path): the Gaussians' features, for the feature term of dL/dalpha.  antialiasing
-// (the _antialiased entries): the forward's records hold op_eff = opacity * rho, so the composite's opacity gradient is
-// dL/dop_eff and the preprocess backward turns it into dL/dopacity (and rho's geometric terms).  The assigning backward
-// lets the composite write into dL_dopacity and rescales it in place; the accumulating one needs dL/dop_eff of this view
-// alone, so the composite writes into P zeroed floats of the device's default memory pool.  dL_dalpha / dL_dinvdepth
-// (the _alpha_invdepth entries, which have checked that both are given): the gradients of the forward's opacity and
-// inverse-depth planes, added to dL/dalpha and dL/dz by the composite.
-template <typename TG>
-int backward_impl(const Api& api, bool accumulate, int P, int D, int M, int R, int C, const float* background, int width,
-                  int height, const float* means3D, const float* shs, const float* scales, float scale_modifier,
-                  const float* rotations, const float* cov3D_precomp, const float* viewmatrix, const float* projmatrix,
-                  const float* cam_pos, float tan_fovx, float tan_fovy, const int* radii, char* geom_buffer,
-                  char* binning_buffer, char* image_buffer, const float* dL_dpix, const TG* dL_dfeaturepix,
-                  float dL_dfeaturepix_scale, const float* dL_depths, float* dL_dmean2D, float* dL_dconic,
-                  float* dL_dopacity, float* dL_dcolor, float* dL_dsemantic_feature, float* dL_dmean3D, float* dL_dcov3D,
-                  float* dL_dsh, float* dL_dscale, float* dL_drot, float* dL_dz, float* grad_accum, float* denom,
-                  float* dL_dcamera, cudaEvent_t composite_done, int debug, cudaStream_t stream,
-                  const Range& zero = {nullptr, 0}, const FeatureRows& feat = {}, bool antialiasing = false,
-                  const float* dL_dalpha = nullptr, const float* dL_dinvdepth = nullptr) {
-    if (P < 0 || width <= 0 || height <= 0 || C < 0 || C > F3DGS_MAX_FEATURE_DIM || R < 0)
+// The map gradient dL_dfeaturepix [C,H,W]: float32, or float16 bits h standing for dL/dO = scale * float(h) (the scale
+// is not read for a float32 map)
+struct MapGrad {
+    const void* p;
+    bool f16;
+    float scale;
+};
+
+// One view's backward, as an entry describes it to `backward`.  An entry initialises the fields up to `stream` from
+// its arguments, in f3dgs_backward's order, and the accumulating entries the next group too; every option after that is
+// off unless the entry sets it.
+struct ViewBackward {
+    int P, D, M, R, C;
+    const float* background;
+    int width, height;
+    const float *means3D, *shs, *scales;
+    float scale_modifier;
+    const float *rotations, *cov3D_precomp, *viewmatrix, *projmatrix, *cam_pos;
+    float tan_fovx, tan_fovy;
+    const int* radii;
+    char *geom_buffer, *binning_buffer, *image_buffer;
+    const float* dL_dpix;
+    MapGrad map;
+    const float* dL_depths;
+    float *dL_dmean2D, *dL_dconic, *dL_dopacity, *dL_dcolor, *dL_dsemantic_feature, *dL_dmean3D, *dL_dcov3D, *dL_dsh,
+        *dL_dscale, *dL_drot, *dL_dz;
+    int debug;
+    cudaStream_t stream;
+
+    // The accumulating entries: += into the caller's per-parameter gradient buffers.  Their dL_dmean2D, dL_dconic and
+    // dL_dz are NULL and become per-view intermediates in the scratch; so do dL_dcolor and dL_dcov3D, unless they are
+    // the gradients of the caller's colors_precomp / cov3D_precomp (which accumulate).
+    bool accumulate = false;
+    char* scratch = nullptr;
+    const float* colors_precomp = nullptr;
+    float* dL_dmean2D_out = nullptr;
+    float *grad_accum = nullptr, *denom = nullptr;
+    cudaEvent_t composite_done = nullptr;
+
+    // the _cam entries' 35 floats, added to
+    float* dL_dcamera = nullptr;
+    // the Gaussians' features, for the feature term of dL/dalpha
+    FeatureRows feat;
+    // the forward's records hold op_eff = opacity * rho, so the composite's opacity gradient is dL/dop_eff and the
+    // preprocess backward turns it into dL/dopacity (and rho's geometric terms)
+    bool antialiasing = false;
+    // the gradients of the forward's opacity and inverse-depth planes, added to dL/dalpha and dL/dz by the composite
+    const float *dL_dalpha = nullptr, *dL_dinvdepth = nullptr;
+};
+
+// The features of a _feature_geometry, _antialiased or _alpha_invdepth entry, after the checks every such entry makes
+// before any other.  `required` (the _feature_geometry entries): C > 0 needs features; otherwise a NULL
+// semantic_feature means no feature term.
+int feature_rows(const Api& api, ViewBackward& b, const void* semantic_feature, int semantic_feature_dtype,
+                 int dL_dfeaturepix_dtype, bool required = false) {
+    if (const int rc = check_dtypes(api, {semantic_feature_dtype, dL_dfeaturepix_dtype})) return rc;
+    if (b.C > 0 && !semantic_feature && required) return api.invalid("NULL semantic_feature");
+    b.feat = {b.C > 0 ? semantic_feature : nullptr, semantic_feature_dtype == F3DGS_F16};
+    return 0;
+}
+
+// Shared body of every backward entry: f3dgs_backward (the reference's assign-into-zeroed-buffers contract),
+// f3dgs_backward_accum (b.accumulate) and their float16, _cam, _feature_geometry, _antialiased and _alpha_invdepth
+// twins.  Under antialiasing the assigning backward lets the composite write into dL_dopacity and rescales it in place;
+// the accumulating one needs dL/dop_eff of this view alone, so the composite writes into P zeroed floats of the
+// device's default memory pool.
+int backward(const Api& api, ViewBackward b) {
+    const int P = b.P, C = b.C, debug = b.debug;
+    const cudaStream_t stream = b.stream;
+    if (b.accumulate) {
+        if (P <= 0) return P == 0 ? 0 : api.invalid("bad sizes");
+        if (!b.scratch) return api.invalid("NULL scratch");
+        if ((b.colors_precomp != nullptr) != (b.dL_dcolor != nullptr) ||
+            (b.cov3D_precomp != nullptr) != (b.dL_dcov3D != nullptr))
+            return api.invalid("dL_dcolors_precomp / dL_dcov3D_precomp go with colors_precomp / cov3D_precomp");
+        const ScratchLayout sl((size_t)P);
+        const auto in_scratch = [&](size_t offset) { return reinterpret_cast<float*>(b.scratch + offset); };
+        b.dL_dmean2D = in_scratch(sl.mean2D);
+        b.dL_dconic = in_scratch(sl.conic);
+        b.dL_dz = in_scratch(sl.dz);
+        if (!b.dL_dcolor) b.dL_dcolor = in_scratch(sl.color);
+        if (!b.dL_dcov3D) b.dL_dcov3D = in_scratch(sl.cov3D);
+    }
+    if (P < 0 || b.width <= 0 || b.height <= 0 || C < 0 || C > F3DGS_MAX_FEATURE_DIM || b.R < 0)
         return api.invalid("bad sizes");
     if (P == 0) return 0;
-    if (!geom_buffer || !binning_buffer || !image_buffer) return api.invalid("missing forward buffers");
-    if (!dL_dpix || !dL_depths || (C > 0 && (!dL_dfeaturepix || !dL_dsemantic_feature)) || !dL_dmean2D ||
-        !dL_dconic || !dL_dopacity || !dL_dcolor || !dL_dmean3D || !dL_dcov3D || !dL_dz)
+    if (!b.geom_buffer || !b.binning_buffer || !b.image_buffer) return api.invalid("missing forward buffers");
+    if (!b.dL_dpix || !b.dL_depths || (C > 0 && (!b.map.p || !b.dL_dsemantic_feature)) || !b.dL_dmean2D ||
+        !b.dL_dconic || !b.dL_dopacity || !b.dL_dcolor || !b.dL_dmean3D || !b.dL_dcov3D || !b.dL_dz)
         return api.invalid("NULL gradient pointer");
-    if (shs && !dL_dsh) return api.invalid("shs given but dL_dsh NULL");
-    if (scales && (!rotations || !dL_dscale || !dL_drot))
+    if (b.shs && !b.dL_dsh) return api.invalid("shs given but dL_dsh NULL");
+    if (b.scales && (!b.rotations || !b.dL_dscale || !b.dL_drot))
         return api.invalid("scales given but rotations/dL_dscale/dL_drot NULL");
-    if ((grad_accum == nullptr) != (denom == nullptr)) return api.invalid("grad_accum and denom go together");
-    if constexpr (std::is_same_v<TG, __half>) {
-        if (!std::isfinite(dL_dfeaturepix_scale) || dL_dfeaturepix_scale == 0.f)
+    if ((b.grad_accum == nullptr) != (b.denom == nullptr)) return api.invalid("grad_accum and denom go together");
+    if (b.map.f16) {
+        if (!std::isfinite(b.map.scale) || b.map.scale == 0.f)
             return api.invalid("dL_dfeaturepix_scale must be finite and nonzero");
         // the feature kernel reduces into dL_dsemantic_feature while other warps still read the map
-        if (overlaps({dL_dsemantic_feature, (size_t)P * C * 4}, {{dL_dfeaturepix, (size_t)C * width * height * 2}}))
+        if (overlaps({b.dL_dsemantic_feature, (size_t)P * C * 4}, {{b.map.p, (size_t)C * b.width * b.height * 2}}))
             return api.invalid("dL_dsemantic_feature overlaps dL_dfeaturepix");
     }
-    if (dL_dcamera) {
-        const size_t p4 = (size_t)P * 4;
-        const Range outs[] = {{dL_dmean2D, 3 * p4}, {dL_dconic, 4 * p4}, {dL_dopacity, p4}, {dL_dcolor, 3 * p4},
-                              {dL_dsemantic_feature, (size_t)C * p4}, {dL_dmean3D, 3 * p4}, {dL_dcov3D, 6 * p4},
-                              {dL_dsh, (size_t)M * 3 * p4}, {dL_dscale, 3 * p4}, {dL_drot, 4 * p4}, {dL_dz, p4},
-                              {grad_accum, p4}, {denom, p4}, zero};
-        if (overlaps({dL_dcamera, F3DGS_CAMERA_GRAD_FLOATS * sizeof(float)}, outs))
-            return api.invalid("dL_dcamera overlaps another output");
-    }
-    if (feat.rows) {
-        const size_t p4 = (size_t)P * 4;
-        const Range outs[] = {{dL_dmean2D, 3 * p4}, {dL_dconic, 4 * p4}, {dL_dopacity, p4}, {dL_dcolor, 3 * p4},
-                              {dL_dsemantic_feature, (size_t)C * p4}, {dL_dmean3D, 3 * p4}, {dL_dcov3D, 6 * p4},
-                              {dL_dsh, (size_t)M * 3 * p4}, {dL_dscale, 3 * p4}, {dL_drot, 4 * p4}, {dL_dz, p4},
-                              {grad_accum, p4}, {denom, p4}, {dL_dcamera, F3DGS_CAMERA_GRAD_FLOATS * sizeof(float)},
-                              zero};
-        if (overlaps({feat.rows, (size_t)P * C * (feat.f16 ? 2 : 4)}, outs))
-            return api.invalid("semantic_feature overlaps an output");
-    }
-    if (antialiasing) {  // the preprocess backward writes dL_dopacity while it writes the others
-        const size_t p4 = (size_t)P * 4;
-        const Range outs[] = {{dL_dmean2D, 3 * p4}, {dL_dconic, 4 * p4}, {dL_dcolor, 3 * p4},
-                              {dL_dsemantic_feature, (size_t)C * p4}, {dL_dmean3D, 3 * p4}, {dL_dcov3D, 6 * p4},
-                              {dL_dsh, (size_t)M * 3 * p4}, {dL_dscale, 3 * p4}, {dL_drot, 4 * p4}, {dL_dz, p4},
-                              {grad_accum, p4}, {denom, p4}, {dL_dcamera, F3DGS_CAMERA_GRAD_FLOATS * sizeof(float)},
-                              zero};
-        if (overlaps({dL_dopacity, p4}, outs)) return api.invalid("dL_dopacity overlaps another output");
-    }
-    if (dL_dalpha) {  // read by the composite while it reduces into the outputs
-        const size_t p4 = (size_t)P * 4, hw4 = (size_t)width * height * 4;
-        const Range outs[] = {{dL_dmean2D, 3 * p4}, {dL_dconic, 4 * p4}, {dL_dopacity, p4}, {dL_dcolor, 3 * p4},
-                              {dL_dsemantic_feature, (size_t)C * p4}, {dL_dmean3D, 3 * p4}, {dL_dcov3D, 6 * p4},
-                              {dL_dsh, (size_t)M * 3 * p4}, {dL_dscale, 3 * p4}, {dL_drot, 4 * p4}, {dL_dz, p4},
-                              {grad_accum, p4}, {denom, p4}, {dL_dcamera, F3DGS_CAMERA_GRAD_FLOATS * sizeof(float)},
-                              zero};
-        if (overlaps({dL_dalpha, hw4}, outs) || overlaps({dL_dinvdepth, hw4}, outs))
-            return api.invalid("dL_dalpha / dL_dinvdepth overlap an output");
-    }
-    if (zero.p) CUDA_TRY(cudaMemsetAsync(const_cast<void*>(zero.p), 0, zero.bytes, stream));
+    // Every output; an absent one is NULL.  The optional operands are read or written while the kernels write these,
+    // so none may overlap an output other than itself.
+    const size_t p4 = (size_t)P * 4, hw4 = (size_t)b.width * b.height * 4;
+    const size_t scratch_bytes = b.accumulate ? ScratchLayout((size_t)P).bytes : 0;
+    const Range outs[] = {{b.dL_dmean2D, 3 * p4}, {b.dL_dconic, 4 * p4}, {b.dL_dopacity, p4}, {b.dL_dcolor, 3 * p4},
+                          {b.dL_dsemantic_feature, (size_t)C * p4}, {b.dL_dmean3D, 3 * p4}, {b.dL_dcov3D, 6 * p4},
+                          {b.dL_dsh, (size_t)b.M * 3 * p4}, {b.dL_dscale, 3 * p4}, {b.dL_drot, 4 * p4},
+                          {b.dL_dz, p4}, {b.grad_accum, p4}, {b.denom, p4},
+                          {b.dL_dcamera, F3DGS_CAMERA_GRAD_FLOATS * sizeof(float)}, {b.scratch, scratch_bytes},
+                          {b.dL_dmean2D_out, 3 * p4}};
+    const Range &opacity = outs[2], &camera = outs[13];
+    if (overlaps(camera, outs)) return api.invalid("dL_dcamera overlaps another output");
+    if (overlaps({b.feat.rows, (size_t)P * C * (b.feat.f16 ? 2 : 4)}, outs))
+        return api.invalid("semantic_feature overlaps an output");
+    // the preprocess backward writes dL_dopacity under antialiasing
+    if (b.antialiasing && overlaps(opacity, outs)) return api.invalid("dL_dopacity overlaps another output");
+    if (overlaps({b.dL_dalpha, hw4}, outs) || overlaps({b.dL_dinvdepth, hw4}, outs))
+        return api.invalid("dL_dalpha / dL_dinvdepth overlap an output");
+    if (b.accumulate) CUDA_TRY(cudaMemsetAsync(b.scratch, 0, scratch_bytes, stream));
 
-    const ViewParams vp = make_view(P, D, M, C, width, height, tan_fovx, tan_fovy, scale_modifier, viewmatrix,
-                                    projmatrix, cam_pos);
+    const ViewParams vp = make_view(P, b.D, b.M, C, b.width, b.height, b.tan_fovx, b.tan_fovy, b.scale_modifier,
+                                    b.viewmatrix, b.projmatrix, b.cam_pos);
     const GeomLayout gl((size_t)P);
-    const float* cov3d = cov3D_precomp ? cov3D_precomp : reinterpret_cast<const float*>(geom_buffer + gl.cov3d);
-    const uint8_t* clamped = reinterpret_cast<const uint8_t*>(geom_buffer + gl.clamped);
-    if (radii == nullptr) radii = reinterpret_cast<const int*>(geom_buffer + gl.radii);
+    const float* cov3d = b.cov3D_precomp ? b.cov3D_precomp : reinterpret_cast<const float*>(b.geom_buffer + gl.cov3d);
+    const uint8_t* clamped = reinterpret_cast<const uint8_t*>(b.geom_buffer + gl.clamped);
+    const int* radii = b.radii ? b.radii : reinterpret_cast<const int*>(b.geom_buffer + gl.radii);
 
     cudaError_t e;
     // where the composite puts the opacity gradient: dL/dop_eff under antialiasing (see above)
@@ -582,8 +622,8 @@ int backward_impl(const Api& api, bool accumulate, int P, int D, int M, int R, i
             if (p) cudaFreeAsync(p, s);
         }
     } op_eff_grad{nullptr, stream};
-    float* dL_dop_eff = dL_dopacity;
-    if (antialiasing && accumulate) {
+    float* dL_dop_eff = b.dL_dopacity;
+    if (b.antialiasing && b.accumulate) {
         e = cudaMallocAsync((void**)&op_eff_grad.p, (size_t)P * sizeof(float), stream);
         if (e != cudaSuccess)
             return api.fail(F3DGS_ERR_ALLOC, std::string("cudaMallocAsync for dL/dop_eff failed: ") +
@@ -593,28 +633,34 @@ int backward_impl(const Api& api, bool accumulate, int P, int D, int M, int R, i
     }
     {
         StageTimer t(F3DGS_STAGE_COMPOSITE_BWD, stream);
-        e = launch_composite_bwd(vp, forward_buffers(vp, R, geom_buffer, binning_buffer, image_buffer), background,
-                                 dL_dpix, dL_depths, dL_dfeaturepix, dL_dfeaturepix_scale, dL_dmean2D, dL_dconic,
-                                 dL_dop_eff, dL_dcolor, dL_dz, dL_dsemantic_feature, stream, feat, dL_dalpha,
-                                 dL_dinvdepth);
+        const ForwardBuffers fb = forward_buffers(vp, b.R, b.geom_buffer, b.binning_buffer, b.image_buffer);
+        const auto composite = [&](auto* dL_dfeaturepix) {
+            return launch_composite_bwd(vp, fb, b.background, b.dL_dpix, b.dL_depths, dL_dfeaturepix, b.map.scale,
+                                        b.dL_dmean2D, b.dL_dconic, dL_dop_eff, b.dL_dcolor, b.dL_dz,
+                                        b.dL_dsemantic_feature, stream, b.feat, b.dL_dalpha, b.dL_dinvdepth);
+        };
+        e = b.map.f16 ? composite(static_cast<const __half*>(b.map.p)) : composite(static_cast<const float*>(b.map.p));
     }
     if (const int rc = composite_bwd_result(api, e, "composite_bwd launch")) return rc;
     STAGE_CHECK("composite_bwd");
     // dL_dopacity is final after the composite, or under antialiasing after the preprocess backward
-    if (composite_done && !antialiasing) CUDA_TRY(cudaEventRecord(composite_done, stream));
+    if (b.composite_done && !b.antialiasing) CUDA_TRY(cudaEventRecord(b.composite_done, stream));
     {
         StageTimer t(F3DGS_STAGE_PREPROCESS_BWD, stream);
-        e = launch_preprocess_bwd(vp, means3D, radii, shs, clamped, scales, rotations, cov3d, dL_dmean2D, dL_dconic,
-                                  dL_dmean3D, dL_dcolor, dL_dcov3D, dL_dsh, dL_dscale, dL_drot, dL_dz, stream,
-                                  accumulate, grad_accum, denom, dL_dcamera, antialiasing,
-                                  reinterpret_cast<const SplatRec*>(geom_buffer + gl.rec), dL_dop_eff, dL_dopacity);
+        e = launch_preprocess_bwd(vp, b.means3D, radii, b.shs, clamped, b.scales, b.rotations, cov3d, b.dL_dmean2D,
+                                  b.dL_dconic, b.dL_dmean3D, b.dL_dcolor, b.dL_dcov3D, b.dL_dsh, b.dL_dscale, b.dL_drot,
+                                  b.dL_dz, stream, b.accumulate, b.grad_accum, b.denom, b.dL_dcamera, b.antialiasing,
+                                  reinterpret_cast<const SplatRec*>(b.geom_buffer + gl.rec), dL_dop_eff, b.dL_dopacity);
     }
     if (e == cudaErrorMemoryAllocation)
         return api.fail(F3DGS_ERR_ALLOC, std::string("cudaMallocAsync for the camera-gradient partials failed: ") +
                                              cudaGetErrorString(e));
     CUDA_TRY(e);
     STAGE_CHECK("preprocess_bwd");
-    if (composite_done && antialiasing) CUDA_TRY(cudaEventRecord(composite_done, stream));
+    if (b.composite_done && b.antialiasing) CUDA_TRY(cudaEventRecord(b.composite_done, stream));
+    if (b.dL_dmean2D_out)
+        CUDA_TRY(cudaMemcpyAsync(b.dL_dmean2D_out, b.dL_dmean2D, (size_t)P * 3 * sizeof(float),
+                                 cudaMemcpyDeviceToDevice, stream));
     return 0;
 }
 
@@ -634,11 +680,12 @@ int f3dgs_backward(int P, int D, int M, int R, int C, const float* background, i
                    float* dL_dz, int debug, void* cuda_stream) {
     (void)semantic_feature;  // not needed: dL/dfeature depends only on the blend weights (SURVEY D.1/D.2)
     (void)colors_precomp;    // colours were copied into the per-Gaussian records by the forward
-    return backward_impl(Api(__func__), false, P, D, M, R, C, background, width, height, means3D, shs, scales,
-                         scale_modifier, rotations, cov3D_precomp, viewmatrix, projmatrix, cam_pos, tan_fovx, tan_fovy,
-                         radii, geom_buffer, binning_buffer, image_buffer, dL_dpix, dL_dfeaturepix, 1.f, dL_depths,
-                         dL_dmean2D, dL_dconic, dL_dopacity, dL_dcolor, dL_dsemantic_feature, dL_dmean3D, dL_dcov3D, dL_dsh,
-                         dL_dscale, dL_drot, dL_dz, nullptr, nullptr, nullptr, nullptr, debug, (cudaStream_t)cuda_stream);
+    const ViewBackward b{P, D, M, R, C, background, width, height, means3D, shs, scales, scale_modifier, rotations,
+                         cov3D_precomp, viewmatrix, projmatrix, cam_pos, tan_fovx, tan_fovy, radii, geom_buffer,
+                         binning_buffer, image_buffer, dL_dpix, {dL_dfeaturepix, false, 1.f}, dL_depths, dL_dmean2D,
+                         dL_dconic, dL_dopacity, dL_dcolor, dL_dsemantic_feature, dL_dmean3D, dL_dcov3D, dL_dsh,
+                         dL_dscale, dL_drot, dL_dz, debug, (cudaStream_t)cuda_stream};
+    return backward(Api(__func__), b);
 }
 
 int f3dgs_backward_f16(int P, int D, int M, int R, int C, const float* background, int width, int height,
@@ -653,12 +700,12 @@ int f3dgs_backward_f16(int P, int D, int M, int R, int C, const float* backgroun
                        float* dL_dsh, float* dL_dscale, float* dL_drot, float* dL_dz, int debug, void* cuda_stream) {
     (void)semantic_feature;
     (void)colors_precomp;
-    return backward_impl(Api(__func__), false, P, D, M, R, C, background, width, height, means3D, shs, scales,
-                         scale_modifier, rotations, cov3D_precomp, viewmatrix, projmatrix, cam_pos, tan_fovx, tan_fovy,
-                         radii, geom_buffer, binning_buffer, image_buffer, dL_dpix,
-                         reinterpret_cast<const __half*>(dL_dfeaturepix), dL_dfeaturepix_scale, dL_depths, dL_dmean2D,
-                         dL_dconic, dL_dopacity, dL_dcolor, dL_dsemantic_feature, dL_dmean3D, dL_dcov3D, dL_dsh, dL_dscale,
-                         dL_drot, dL_dz, nullptr, nullptr, nullptr, nullptr, debug, (cudaStream_t)cuda_stream);
+    const ViewBackward b{P, D, M, R, C, background, width, height, means3D, shs, scales, scale_modifier, rotations,
+                         cov3D_precomp, viewmatrix, projmatrix, cam_pos, tan_fovx, tan_fovy, radii, geom_buffer,
+                         binning_buffer, image_buffer, dL_dpix, {dL_dfeaturepix, true, dL_dfeaturepix_scale},
+                         dL_depths, dL_dmean2D, dL_dconic, dL_dopacity, dL_dcolor, dL_dsemantic_feature, dL_dmean3D,
+                         dL_dcov3D, dL_dsh, dL_dscale, dL_drot, dL_dz, debug, (cudaStream_t)cuda_stream};
+    return backward(Api(__func__), b);
 }
 
 int f3dgs_backward_cam(int P, int D, int M, int R, int C, const float* background, int width, int height,
@@ -675,12 +722,13 @@ int f3dgs_backward_cam(int P, int D, int M, int R, int C, const float* backgroun
     (void)colors_precomp;
     const Api api(__func__);
     if (!dL_dcamera) return api.invalid("NULL dL_dcamera");
-    return backward_impl(api, false, P, D, M, R, C, background, width, height, means3D, shs, scales, scale_modifier,
-                         rotations, cov3D_precomp, viewmatrix, projmatrix, cam_pos, tan_fovx, tan_fovy, radii,
-                         geom_buffer, binning_buffer, image_buffer, dL_dpix, dL_dfeaturepix, 1.f, dL_depths, dL_dmean2D,
-                         dL_dconic, dL_dopacity, dL_dcolor, dL_dsemantic_feature, dL_dmean3D, dL_dcov3D, dL_dsh,
-                         dL_dscale, dL_drot, dL_dz, nullptr, nullptr, dL_dcamera, nullptr, debug,
-                         (cudaStream_t)cuda_stream);
+    ViewBackward b{P, D, M, R, C, background, width, height, means3D, shs, scales, scale_modifier, rotations,
+                   cov3D_precomp, viewmatrix, projmatrix, cam_pos, tan_fovx, tan_fovy, radii, geom_buffer,
+                   binning_buffer, image_buffer, dL_dpix, {dL_dfeaturepix, false, 1.f}, dL_depths, dL_dmean2D,
+                   dL_dconic, dL_dopacity, dL_dcolor, dL_dsemantic_feature, dL_dmean3D, dL_dcov3D, dL_dsh, dL_dscale,
+                   dL_drot, dL_dz, debug, (cudaStream_t)cuda_stream};
+    b.dL_dcamera = dL_dcamera;
+    return backward(api, b);
 }
 
 int f3dgs_backward_cam_f16(int P, int D, int M, int R, int C, const float* background, int width, int height,
@@ -698,71 +746,16 @@ int f3dgs_backward_cam_f16(int P, int D, int M, int R, int C, const float* backg
     (void)colors_precomp;
     const Api api(__func__);
     if (!dL_dcamera) return api.invalid("NULL dL_dcamera");
-    return backward_impl(api, false, P, D, M, R, C, background, width, height, means3D, shs, scales, scale_modifier,
-                         rotations, cov3D_precomp, viewmatrix, projmatrix, cam_pos, tan_fovx, tan_fovy, radii,
-                         geom_buffer, binning_buffer, image_buffer, dL_dpix,
-                         reinterpret_cast<const __half*>(dL_dfeaturepix), dL_dfeaturepix_scale, dL_depths, dL_dmean2D,
-                         dL_dconic, dL_dopacity, dL_dcolor, dL_dsemantic_feature, dL_dmean3D, dL_dcov3D, dL_dsh,
-                         dL_dscale, dL_drot, dL_dz, nullptr, nullptr, dL_dcamera, nullptr, debug,
-                         (cudaStream_t)cuda_stream);
+    ViewBackward b{P, D, M, R, C, background, width, height, means3D, shs, scales, scale_modifier, rotations,
+                   cov3D_precomp, viewmatrix, projmatrix, cam_pos, tan_fovx, tan_fovy, radii, geom_buffer,
+                   binning_buffer, image_buffer, dL_dpix, {dL_dfeaturepix, true, dL_dfeaturepix_scale}, dL_depths,
+                   dL_dmean2D, dL_dconic, dL_dopacity, dL_dcolor, dL_dsemantic_feature, dL_dmean3D, dL_dcov3D, dL_dsh,
+                   dL_dscale, dL_drot, dL_dz, debug, (cudaStream_t)cuda_stream};
+    b.dL_dcamera = dL_dcamera;
+    return backward(api, b);
 }
 
 size_t f3dgs_backward_scratch_bytes(int P) { return P > 0 ? ScratchLayout((size_t)P).bytes : 0; }
-
-}  // extern "C"
-
-namespace {
-// Shared body of f3dgs_backward_accum and f3dgs_backward_accum_f16 (TG as in backward_impl)
-template <typename TG>
-int backward_accum_impl(const char* entry, int P, int D, int M, int R, int C, const float* background, int width,
-                        int height, const float* means3D, const float* shs, const float* colors_precomp,
-                        const float* scales, float scale_modifier, const float* rotations, const float* cov3D_precomp,
-                        const float* viewmatrix, const float* projmatrix, const float* cam_pos, float tan_fovx,
-                        float tan_fovy, const int* radii, char* geom_buffer, char* binning_buffer, char* image_buffer,
-                        const float* dL_dpix, const TG* dL_dfeaturepix, float dL_dfeaturepix_scale,
-                        const float* dL_depths, char* scratch, float* dL_dopacity, float* dL_dcolors_precomp,
-                        float* dL_dsemantic_feature, float* dL_dmean3D, float* dL_dcov3D_precomp, float* dL_dsh,
-                        float* dL_dscale, float* dL_drot, float* dL_dmean2D_out, float* grad_accum, float* denom,
-                        void* composite_done_event, int debug, void* cuda_stream, bool camera = false,
-                        float* dL_dcamera = nullptr, const FeatureRows& feat = {}, bool antialiasing = false,
-                        const float* dL_dalpha = nullptr, const float* dL_dinvdepth = nullptr) {
-    const Api api(entry);
-    cudaStream_t stream = (cudaStream_t)cuda_stream;
-    if (camera && !dL_dcamera) return api.invalid("NULL dL_dcamera");
-    if (P <= 0) return P == 0 ? 0 : api.invalid("bad sizes");
-    if (!scratch) return api.invalid("NULL scratch");
-    if (overlaps({dL_dcamera, F3DGS_CAMERA_GRAD_FLOATS * sizeof(float)}, {{dL_dmean2D_out, (size_t)P * 3 * 4}}))
-        return api.invalid("dL_dcamera overlaps another output");
-    if (overlaps({feat.rows, (size_t)P * C * (feat.f16 ? 2 : 4)}, {{dL_dmean2D_out, (size_t)P * 3 * 4}}))
-        return api.invalid("semantic_feature overlaps an output");
-    const size_t hw4 = (size_t)width * height * 4;
-    if (overlaps({dL_dalpha, hw4}, {{dL_dmean2D_out, (size_t)P * 3 * 4}}) ||
-        overlaps({dL_dinvdepth, hw4}, {{dL_dmean2D_out, (size_t)P * 3 * 4}}))
-        return api.invalid("dL_dalpha / dL_dinvdepth overlap an output");
-    if ((colors_precomp != nullptr) != (dL_dcolors_precomp != nullptr) ||
-        (cov3D_precomp != nullptr) != (dL_dcov3D_precomp != nullptr))
-        return api.invalid("dL_dcolors_precomp / dL_dcov3D_precomp go with colors_precomp / cov3D_precomp");
-    const ScratchLayout sl((size_t)P);
-    float* m2d = reinterpret_cast<float*>(scratch + sl.mean2D);
-    // colours / cov3D are intermediates unless they are inputs of the caller (then their gradients accumulate)
-    float* dcol = dL_dcolors_precomp ? dL_dcolors_precomp : reinterpret_cast<float*>(scratch + sl.color);
-    float* dcov = dL_dcov3D_precomp ? dL_dcov3D_precomp : reinterpret_cast<float*>(scratch + sl.cov3D);
-    const int rc = backward_impl(
-        api, true, P, D, M, R, C, background, width, height, means3D, shs, scales, scale_modifier,
-        rotations, cov3D_precomp, viewmatrix, projmatrix, cam_pos, tan_fovx, tan_fovy, radii, geom_buffer,
-        binning_buffer, image_buffer, dL_dpix, dL_dfeaturepix, dL_dfeaturepix_scale, dL_depths, m2d,
-        reinterpret_cast<float*>(scratch + sl.conic), dL_dopacity, dcol, dL_dsemantic_feature, dL_dmean3D, dcov, dL_dsh,
-        dL_dscale, dL_drot, reinterpret_cast<float*>(scratch + sl.dz), grad_accum, denom, dL_dcamera,
-        (cudaEvent_t)composite_done_event, debug, stream, {scratch, sl.bytes}, feat, antialiasing, dL_dalpha,
-        dL_dinvdepth);
-    if (rc < 0) return rc;
-    if (dL_dmean2D_out)
-        CUDA_TRY(cudaMemcpyAsync(dL_dmean2D_out, m2d, (size_t)P * 3 * sizeof(float), cudaMemcpyDeviceToDevice, stream));
-    return 0;
-}
-}  // namespace
-
-extern "C" {
 
 int f3dgs_backward_accum(int P, int D, int M, int R, int C, const float* background, int width, int height,
                          const float* means3D, const float* shs, const float* colors_precomp, const float* scales,
@@ -774,12 +767,14 @@ int f3dgs_backward_accum(int P, int D, int M, int R, int C, const float* backgro
                          float* dL_dcov3D_precomp, float* dL_dsh, float* dL_dscale, float* dL_drot,
                          float* dL_dmean2D_out, float* grad_accum, float* denom, void* composite_done_event, int debug,
                          void* cuda_stream) {
-    return backward_accum_impl(__func__, P, D, M, R, C, background, width, height, means3D, shs, colors_precomp, scales,
-                               scale_modifier, rotations, cov3D_precomp, viewmatrix, projmatrix, cam_pos, tan_fovx,
-                               tan_fovy, radii, geom_buffer, binning_buffer, image_buffer, dL_dpix, dL_dfeaturepix, 1.f,
-                               dL_depths, scratch, dL_dopacity, dL_dcolors_precomp, dL_dsemantic_feature, dL_dmean3D,
-                               dL_dcov3D_precomp, dL_dsh, dL_dscale, dL_drot, dL_dmean2D_out, grad_accum, denom,
-                               composite_done_event, debug, cuda_stream);
+    const ViewBackward b{P, D, M, R, C, background, width, height, means3D, shs, scales, scale_modifier, rotations,
+                         cov3D_precomp, viewmatrix, projmatrix, cam_pos, tan_fovx, tan_fovy, radii, geom_buffer,
+                         binning_buffer, image_buffer, dL_dpix, {dL_dfeaturepix, false, 1.f}, dL_depths, nullptr,
+                         nullptr, dL_dopacity, dL_dcolors_precomp, dL_dsemantic_feature, dL_dmean3D,
+                         dL_dcov3D_precomp, dL_dsh, dL_dscale, dL_drot, nullptr, debug, (cudaStream_t)cuda_stream,
+                         true, scratch, colors_precomp, dL_dmean2D_out, grad_accum, denom,
+                         (cudaEvent_t)composite_done_event};
+    return backward(Api(__func__), b);
 }
 
 int f3dgs_backward_accum_f16(int P, int D, int M, int R, int C, const float* background, int width, int height,
@@ -793,13 +788,14 @@ int f3dgs_backward_accum_f16(int P, int D, int M, int R, int C, const float* bac
                              float* dL_dcov3D_precomp, float* dL_dsh, float* dL_dscale, float* dL_drot,
                              float* dL_dmean2D_out, float* grad_accum, float* denom, void* composite_done_event,
                              int debug, void* cuda_stream) {
-    return backward_accum_impl(__func__, P, D, M, R, C, background, width, height, means3D, shs, colors_precomp, scales,
-                               scale_modifier, rotations, cov3D_precomp, viewmatrix, projmatrix, cam_pos, tan_fovx,
-                               tan_fovy, radii, geom_buffer, binning_buffer, image_buffer, dL_dpix,
-                               reinterpret_cast<const __half*>(dL_dfeaturepix), dL_dfeaturepix_scale, dL_depths, scratch,
-                               dL_dopacity, dL_dcolors_precomp, dL_dsemantic_feature, dL_dmean3D, dL_dcov3D_precomp,
-                               dL_dsh, dL_dscale, dL_drot, dL_dmean2D_out, grad_accum, denom, composite_done_event, debug,
-                               cuda_stream);
+    const ViewBackward b{P, D, M, R, C, background, width, height, means3D, shs, scales, scale_modifier, rotations,
+                         cov3D_precomp, viewmatrix, projmatrix, cam_pos, tan_fovx, tan_fovy, radii, geom_buffer,
+                         binning_buffer, image_buffer, dL_dpix, {dL_dfeaturepix, true, dL_dfeaturepix_scale},
+                         dL_depths, nullptr, nullptr, dL_dopacity, dL_dcolors_precomp, dL_dsemantic_feature,
+                         dL_dmean3D, dL_dcov3D_precomp, dL_dsh, dL_dscale, dL_drot, nullptr, debug,
+                         (cudaStream_t)cuda_stream, true, scratch, colors_precomp, dL_dmean2D_out, grad_accum, denom,
+                         (cudaEvent_t)composite_done_event};
+    return backward(Api(__func__), b);
 }
 
 int f3dgs_backward_accum_cam(int P, int D, int M, int R, int C, const float* background, int width, int height,
@@ -812,12 +808,16 @@ int f3dgs_backward_accum_cam(int P, int D, int M, int R, int C, const float* bac
                              float* dL_dsemantic_feature, float* dL_dmean3D, float* dL_dcov3D_precomp, float* dL_dsh,
                              float* dL_dscale, float* dL_drot, float* dL_dmean2D_out, float* grad_accum, float* denom,
                              void* composite_done_event, int debug, void* cuda_stream, float* dL_dcamera) {
-    return backward_accum_impl(__func__, P, D, M, R, C, background, width, height, means3D, shs, colors_precomp, scales,
-                               scale_modifier, rotations, cov3D_precomp, viewmatrix, projmatrix, cam_pos, tan_fovx,
-                               tan_fovy, radii, geom_buffer, binning_buffer, image_buffer, dL_dpix, dL_dfeaturepix, 1.f,
-                               dL_depths, scratch, dL_dopacity, dL_dcolors_precomp, dL_dsemantic_feature, dL_dmean3D,
-                               dL_dcov3D_precomp, dL_dsh, dL_dscale, dL_drot, dL_dmean2D_out, grad_accum, denom,
-                               composite_done_event, debug, cuda_stream, true, dL_dcamera);
+    const Api api(__func__);
+    if (!dL_dcamera) return api.invalid("NULL dL_dcamera");
+    ViewBackward b{P, D, M, R, C, background, width, height, means3D, shs, scales, scale_modifier, rotations,
+                   cov3D_precomp, viewmatrix, projmatrix, cam_pos, tan_fovx, tan_fovy, radii, geom_buffer,
+                   binning_buffer, image_buffer, dL_dpix, {dL_dfeaturepix, false, 1.f}, dL_depths, nullptr, nullptr,
+                   dL_dopacity, dL_dcolors_precomp, dL_dsemantic_feature, dL_dmean3D, dL_dcov3D_precomp, dL_dsh,
+                   dL_dscale, dL_drot, nullptr, debug, (cudaStream_t)cuda_stream, true, scratch, colors_precomp,
+                   dL_dmean2D_out, grad_accum, denom, (cudaEvent_t)composite_done_event};
+    b.dL_dcamera = dL_dcamera;
+    return backward(api, b);
 }
 
 int f3dgs_backward_accum_cam_f16(int P, int D, int M, int R, int C, const float* background, int width, int height,
@@ -832,31 +832,17 @@ int f3dgs_backward_accum_cam_f16(int P, int D, int M, int R, int C, const float*
                                  float* dL_dsh, float* dL_dscale, float* dL_drot, float* dL_dmean2D_out,
                                  float* grad_accum, float* denom, void* composite_done_event, int debug,
                                  void* cuda_stream, float* dL_dcamera) {
-    return backward_accum_impl(__func__, P, D, M, R, C, background, width, height, means3D, shs, colors_precomp, scales,
-                               scale_modifier, rotations, cov3D_precomp, viewmatrix, projmatrix, cam_pos, tan_fovx,
-                               tan_fovy, radii, geom_buffer, binning_buffer, image_buffer, dL_dpix,
-                               reinterpret_cast<const __half*>(dL_dfeaturepix), dL_dfeaturepix_scale, dL_depths, scratch,
-                               dL_dopacity, dL_dcolors_precomp, dL_dsemantic_feature, dL_dmean3D, dL_dcov3D_precomp,
-                               dL_dsh, dL_dscale, dL_drot, dL_dmean2D_out, grad_accum, denom, composite_done_event, debug,
-                               cuda_stream, true, dL_dcamera);
+    const Api api(__func__);
+    if (!dL_dcamera) return api.invalid("NULL dL_dcamera");
+    ViewBackward b{P, D, M, R, C, background, width, height, means3D, shs, scales, scale_modifier, rotations,
+                   cov3D_precomp, viewmatrix, projmatrix, cam_pos, tan_fovx, tan_fovy, radii, geom_buffer,
+                   binning_buffer, image_buffer, dL_dpix, {dL_dfeaturepix, true, dL_dfeaturepix_scale}, dL_depths,
+                   nullptr, nullptr, dL_dopacity, dL_dcolors_precomp, dL_dsemantic_feature, dL_dmean3D,
+                   dL_dcov3D_precomp, dL_dsh, dL_dscale, dL_drot, nullptr, debug, (cudaStream_t)cuda_stream, true,
+                   scratch, colors_precomp, dL_dmean2D_out, grad_accum, denom, (cudaEvent_t)composite_done_event};
+    b.dL_dcamera = dL_dcamera;
+    return backward(api, b);
 }
-
-}  // extern "C"
-
-namespace {
-// The Gaussians' features of a _feature_geometry or _antialiased entry, after the checks every such entry makes before
-// any launch.  `optional` (the _antialiased entries): a NULL semantic_feature means no feature term.
-int feature_rows(const Api& api, int C, const void* semantic_feature, int semantic_feature_dtype,
-                 int dL_dfeaturepix_dtype, FeatureRows& feat, bool optional = false) {
-    const auto known = [](int t) { return t == F3DGS_F32 || t == F3DGS_F16; };
-    if (!known(semantic_feature_dtype) || !known(dL_dfeaturepix_dtype)) return api.invalid("unknown dtype code");
-    if (C > 0 && !semantic_feature && !optional) return api.invalid("NULL semantic_feature");
-    feat = {C > 0 ? semantic_feature : nullptr, semantic_feature_dtype == F3DGS_F16};
-    return 0;
-}
-}  // namespace
-
-extern "C" {
 
 int f3dgs_backward_feature_geometry(int P, int D, int M, int R, int C, const float* background, int width, int height,
                                     const float* means3D, const float* shs, const float* colors_precomp,
@@ -872,20 +858,16 @@ int f3dgs_backward_feature_geometry(int P, int D, int M, int R, int C, const flo
                                     int debug, void* cuda_stream, float* dL_dcamera) {
     (void)colors_precomp;
     const Api api(__func__);
-    FeatureRows feat;
-    if (const int rc = feature_rows(api, C, semantic_feature, semantic_feature_dtype, dL_dfeaturepix_dtype, feat))
+    ViewBackward b{P, D, M, R, C, background, width, height, means3D, shs, scales, scale_modifier, rotations,
+                   cov3D_precomp, viewmatrix, projmatrix, cam_pos, tan_fovx, tan_fovy, radii, geom_buffer,
+                   binning_buffer, image_buffer, dL_dpix,
+                   {dL_dfeaturepix, dL_dfeaturepix_dtype == F3DGS_F16, dL_dfeaturepix_scale}, dL_depths, dL_dmean2D,
+                   dL_dconic, dL_dopacity, dL_dcolor, dL_dsemantic_feature, dL_dmean3D, dL_dcov3D, dL_dsh, dL_dscale,
+                   dL_drot, dL_dz, debug, (cudaStream_t)cuda_stream};
+    if (const int rc = feature_rows(api, b, semantic_feature, semantic_feature_dtype, dL_dfeaturepix_dtype, true))
         return rc;
-    const auto run = [&](auto map, float scale) {
-        return backward_impl(api, false, P, D, M, R, C, background, width, height, means3D, shs, scales,
-                             scale_modifier, rotations, cov3D_precomp, viewmatrix, projmatrix, cam_pos, tan_fovx,
-                             tan_fovy, radii, geom_buffer, binning_buffer, image_buffer, dL_dpix, map, scale, dL_depths,
-                             dL_dmean2D, dL_dconic, dL_dopacity, dL_dcolor, dL_dsemantic_feature, dL_dmean3D, dL_dcov3D,
-                             dL_dsh, dL_dscale, dL_drot, dL_dz, nullptr, nullptr, dL_dcamera, nullptr, debug,
-                             (cudaStream_t)cuda_stream, {nullptr, 0}, feat);
-    };
-    if (dL_dfeaturepix_dtype == F3DGS_F16)
-        return run(static_cast<const __half*>(dL_dfeaturepix), dL_dfeaturepix_scale);
-    return run(static_cast<const float*>(dL_dfeaturepix), 1.f);
+    b.dL_dcamera = dL_dcamera;
+    return backward(api, b);
 }
 
 int f3dgs_backward_accum_feature_geometry(
@@ -898,23 +880,18 @@ int f3dgs_backward_accum_feature_geometry(
     char* scratch, float* dL_dopacity, float* dL_dcolors_precomp, float* dL_dsemantic_feature, float* dL_dmean3D,
     float* dL_dcov3D_precomp, float* dL_dsh, float* dL_dscale, float* dL_drot, float* dL_dmean2D_out,
     float* grad_accum, float* denom, void* composite_done_event, int debug, void* cuda_stream, float* dL_dcamera) {
-    const char* entry = __func__;
-    FeatureRows feat;
-    if (const int rc = feature_rows(Api(entry), C, semantic_feature, semantic_feature_dtype, dL_dfeaturepix_dtype,
-                                    feat))
+    const Api api(__func__);
+    ViewBackward b{P, D, M, R, C, background, width, height, means3D, shs, scales, scale_modifier, rotations,
+                   cov3D_precomp, viewmatrix, projmatrix, cam_pos, tan_fovx, tan_fovy, radii, geom_buffer,
+                   binning_buffer, image_buffer, dL_dpix,
+                   {dL_dfeaturepix, dL_dfeaturepix_dtype == F3DGS_F16, dL_dfeaturepix_scale}, dL_depths, nullptr,
+                   nullptr, dL_dopacity, dL_dcolors_precomp, dL_dsemantic_feature, dL_dmean3D, dL_dcov3D_precomp,
+                   dL_dsh, dL_dscale, dL_drot, nullptr, debug, (cudaStream_t)cuda_stream, true, scratch,
+                   colors_precomp, dL_dmean2D_out, grad_accum, denom, (cudaEvent_t)composite_done_event};
+    if (const int rc = feature_rows(api, b, semantic_feature, semantic_feature_dtype, dL_dfeaturepix_dtype, true))
         return rc;
-    const auto run = [&](auto map, float scale) {
-        return backward_accum_impl(entry, P, D, M, R, C, background, width, height, means3D, shs, colors_precomp,
-                                   scales, scale_modifier, rotations, cov3D_precomp, viewmatrix, projmatrix, cam_pos,
-                                   tan_fovx, tan_fovy, radii, geom_buffer, binning_buffer, image_buffer, dL_dpix, map,
-                                   scale, dL_depths, scratch, dL_dopacity, dL_dcolors_precomp, dL_dsemantic_feature,
-                                   dL_dmean3D, dL_dcov3D_precomp, dL_dsh, dL_dscale, dL_drot, dL_dmean2D_out,
-                                   grad_accum, denom, composite_done_event, debug, cuda_stream, false, dL_dcamera,
-                                   feat);
-    };
-    if (dL_dfeaturepix_dtype == F3DGS_F16)
-        return run(static_cast<const __half*>(dL_dfeaturepix), dL_dfeaturepix_scale);
-    return run(static_cast<const float*>(dL_dfeaturepix), 1.f);
+    b.dL_dcamera = dL_dcamera;
+    return backward(api, b);
 }
 
 int f3dgs_backward_antialiased(int P, int D, int M, int R, int C, const float* background, int width, int height,
@@ -931,21 +908,16 @@ int f3dgs_backward_antialiased(int P, int D, int M, int R, int C, const float* b
                                float* dL_dcamera) {
     (void)colors_precomp;
     const Api api(__func__);
-    FeatureRows feat;
-    if (const int rc =
-            feature_rows(api, C, semantic_feature, semantic_feature_dtype, dL_dfeaturepix_dtype, feat, true))
-        return rc;
-    const auto run = [&](auto map, float scale) {
-        return backward_impl(api, false, P, D, M, R, C, background, width, height, means3D, shs, scales,
-                             scale_modifier, rotations, cov3D_precomp, viewmatrix, projmatrix, cam_pos, tan_fovx,
-                             tan_fovy, radii, geom_buffer, binning_buffer, image_buffer, dL_dpix, map, scale, dL_depths,
-                             dL_dmean2D, dL_dconic, dL_dopacity, dL_dcolor, dL_dsemantic_feature, dL_dmean3D, dL_dcov3D,
-                             dL_dsh, dL_dscale, dL_drot, dL_dz, nullptr, nullptr, dL_dcamera, nullptr, debug,
-                             (cudaStream_t)cuda_stream, {nullptr, 0}, feat, true);
-    };
-    if (dL_dfeaturepix_dtype == F3DGS_F16)
-        return run(static_cast<const __half*>(dL_dfeaturepix), dL_dfeaturepix_scale);
-    return run(static_cast<const float*>(dL_dfeaturepix), 1.f);
+    ViewBackward b{P, D, M, R, C, background, width, height, means3D, shs, scales, scale_modifier, rotations,
+                   cov3D_precomp, viewmatrix, projmatrix, cam_pos, tan_fovx, tan_fovy, radii, geom_buffer,
+                   binning_buffer, image_buffer, dL_dpix,
+                   {dL_dfeaturepix, dL_dfeaturepix_dtype == F3DGS_F16, dL_dfeaturepix_scale}, dL_depths, dL_dmean2D,
+                   dL_dconic, dL_dopacity, dL_dcolor, dL_dsemantic_feature, dL_dmean3D, dL_dcov3D, dL_dsh, dL_dscale,
+                   dL_drot, dL_dz, debug, (cudaStream_t)cuda_stream};
+    if (const int rc = feature_rows(api, b, semantic_feature, semantic_feature_dtype, dL_dfeaturepix_dtype)) return rc;
+    b.dL_dcamera = dL_dcamera;
+    b.antialiasing = true;
+    return backward(api, b);
 }
 
 int f3dgs_backward_accum_antialiased(
@@ -958,25 +930,18 @@ int f3dgs_backward_accum_antialiased(
     char* scratch, float* dL_dopacity, float* dL_dcolors_precomp, float* dL_dsemantic_feature, float* dL_dmean3D,
     float* dL_dcov3D_precomp, float* dL_dsh, float* dL_dscale, float* dL_drot, float* dL_dmean2D_out,
     float* grad_accum, float* denom, void* composite_done_event, int debug, void* cuda_stream, float* dL_dcamera) {
-    const char* entry = __func__;
-    FeatureRows feat;
-    if (const int rc = feature_rows(Api(entry), C, semantic_feature, semantic_feature_dtype, dL_dfeaturepix_dtype,
-                                    feat, true))
-        return rc;
-    if (P > 0 && overlaps({dL_dopacity, (size_t)P * 4}, {{dL_dmean2D_out, (size_t)P * 3 * 4}}))
-        return Api(entry).invalid("dL_dopacity overlaps another output");
-    const auto run = [&](auto map, float scale) {
-        return backward_accum_impl(entry, P, D, M, R, C, background, width, height, means3D, shs, colors_precomp,
-                                   scales, scale_modifier, rotations, cov3D_precomp, viewmatrix, projmatrix, cam_pos,
-                                   tan_fovx, tan_fovy, radii, geom_buffer, binning_buffer, image_buffer, dL_dpix, map,
-                                   scale, dL_depths, scratch, dL_dopacity, dL_dcolors_precomp, dL_dsemantic_feature,
-                                   dL_dmean3D, dL_dcov3D_precomp, dL_dsh, dL_dscale, dL_drot, dL_dmean2D_out,
-                                   grad_accum, denom, composite_done_event, debug, cuda_stream, false, dL_dcamera,
-                                   feat, true);
-    };
-    if (dL_dfeaturepix_dtype == F3DGS_F16)
-        return run(static_cast<const __half*>(dL_dfeaturepix), dL_dfeaturepix_scale);
-    return run(static_cast<const float*>(dL_dfeaturepix), 1.f);
+    const Api api(__func__);
+    ViewBackward b{P, D, M, R, C, background, width, height, means3D, shs, scales, scale_modifier, rotations,
+                   cov3D_precomp, viewmatrix, projmatrix, cam_pos, tan_fovx, tan_fovy, radii, geom_buffer,
+                   binning_buffer, image_buffer, dL_dpix,
+                   {dL_dfeaturepix, dL_dfeaturepix_dtype == F3DGS_F16, dL_dfeaturepix_scale}, dL_depths, nullptr,
+                   nullptr, dL_dopacity, dL_dcolors_precomp, dL_dsemantic_feature, dL_dmean3D, dL_dcov3D_precomp,
+                   dL_dsh, dL_dscale, dL_drot, nullptr, debug, (cudaStream_t)cuda_stream, true, scratch,
+                   colors_precomp, dL_dmean2D_out, grad_accum, denom, (cudaEvent_t)composite_done_event};
+    if (const int rc = feature_rows(api, b, semantic_feature, semantic_feature_dtype, dL_dfeaturepix_dtype)) return rc;
+    b.dL_dcamera = dL_dcamera;
+    b.antialiasing = true;
+    return backward(api, b);
 }
 
 int f3dgs_backward_alpha_invdepth(int P, int D, int M, int R, int C, const float* background, int width, int height,
@@ -995,22 +960,18 @@ int f3dgs_backward_alpha_invdepth(int P, int D, int M, int R, int C, const float
     (void)colors_precomp;
     const Api api(__func__);
     if (!dL_dalpha || !dL_dinvdepth) return api.invalid("NULL dL_dalpha / dL_dinvdepth");
-    FeatureRows feat;
-    if (const int rc =
-            feature_rows(api, C, semantic_feature, semantic_feature_dtype, dL_dfeaturepix_dtype, feat, true))
-        return rc;
-    const auto run = [&](auto map, float scale) {
-        return backward_impl(api, false, P, D, M, R, C, background, width, height, means3D, shs, scales,
-                             scale_modifier, rotations, cov3D_precomp, viewmatrix, projmatrix, cam_pos, tan_fovx,
-                             tan_fovy, radii, geom_buffer, binning_buffer, image_buffer, dL_dpix, map, scale, dL_depths,
-                             dL_dmean2D, dL_dconic, dL_dopacity, dL_dcolor, dL_dsemantic_feature, dL_dmean3D, dL_dcov3D,
-                             dL_dsh, dL_dscale, dL_drot, dL_dz, nullptr, nullptr, dL_dcamera, nullptr, debug,
-                             (cudaStream_t)cuda_stream, {nullptr, 0}, feat, antialiasing != 0, dL_dalpha,
-                             dL_dinvdepth);
-    };
-    if (dL_dfeaturepix_dtype == F3DGS_F16)
-        return run(static_cast<const __half*>(dL_dfeaturepix), dL_dfeaturepix_scale);
-    return run(static_cast<const float*>(dL_dfeaturepix), 1.f);
+    ViewBackward b{P, D, M, R, C, background, width, height, means3D, shs, scales, scale_modifier, rotations,
+                   cov3D_precomp, viewmatrix, projmatrix, cam_pos, tan_fovx, tan_fovy, radii, geom_buffer,
+                   binning_buffer, image_buffer, dL_dpix,
+                   {dL_dfeaturepix, dL_dfeaturepix_dtype == F3DGS_F16, dL_dfeaturepix_scale}, dL_depths, dL_dmean2D,
+                   dL_dconic, dL_dopacity, dL_dcolor, dL_dsemantic_feature, dL_dmean3D, dL_dcov3D, dL_dsh, dL_dscale,
+                   dL_drot, dL_dz, debug, (cudaStream_t)cuda_stream};
+    if (const int rc = feature_rows(api, b, semantic_feature, semantic_feature_dtype, dL_dfeaturepix_dtype)) return rc;
+    b.dL_dcamera = dL_dcamera;
+    b.antialiasing = antialiasing != 0;
+    b.dL_dalpha = dL_dalpha;
+    b.dL_dinvdepth = dL_dinvdepth;
+    return backward(api, b);
 }
 
 int f3dgs_backward_accum_alpha_invdepth(
@@ -1024,26 +985,21 @@ int f3dgs_backward_accum_alpha_invdepth(
     float* dL_dcov3D_precomp, float* dL_dsh, float* dL_dscale, float* dL_drot, float* dL_dmean2D_out,
     float* grad_accum, float* denom, void* composite_done_event, int debug, void* cuda_stream, float* dL_dcamera,
     int antialiasing, const float* dL_dalpha, const float* dL_dinvdepth) {
-    const char* entry = __func__;
-    if (!dL_dalpha || !dL_dinvdepth) return Api(entry).invalid("NULL dL_dalpha / dL_dinvdepth");
-    FeatureRows feat;
-    if (const int rc = feature_rows(Api(entry), C, semantic_feature, semantic_feature_dtype, dL_dfeaturepix_dtype,
-                                    feat, true))
-        return rc;
-    if (antialiasing && P > 0 && overlaps({dL_dopacity, (size_t)P * 4}, {{dL_dmean2D_out, (size_t)P * 3 * 4}}))
-        return Api(entry).invalid("dL_dopacity overlaps another output");
-    const auto run = [&](auto map, float scale) {
-        return backward_accum_impl(entry, P, D, M, R, C, background, width, height, means3D, shs, colors_precomp,
-                                   scales, scale_modifier, rotations, cov3D_precomp, viewmatrix, projmatrix, cam_pos,
-                                   tan_fovx, tan_fovy, radii, geom_buffer, binning_buffer, image_buffer, dL_dpix, map,
-                                   scale, dL_depths, scratch, dL_dopacity, dL_dcolors_precomp, dL_dsemantic_feature,
-                                   dL_dmean3D, dL_dcov3D_precomp, dL_dsh, dL_dscale, dL_drot, dL_dmean2D_out,
-                                   grad_accum, denom, composite_done_event, debug, cuda_stream, false, dL_dcamera,
-                                   feat, antialiasing != 0, dL_dalpha, dL_dinvdepth);
-    };
-    if (dL_dfeaturepix_dtype == F3DGS_F16)
-        return run(static_cast<const __half*>(dL_dfeaturepix), dL_dfeaturepix_scale);
-    return run(static_cast<const float*>(dL_dfeaturepix), 1.f);
+    const Api api(__func__);
+    if (!dL_dalpha || !dL_dinvdepth) return api.invalid("NULL dL_dalpha / dL_dinvdepth");
+    ViewBackward b{P, D, M, R, C, background, width, height, means3D, shs, scales, scale_modifier, rotations,
+                   cov3D_precomp, viewmatrix, projmatrix, cam_pos, tan_fovx, tan_fovy, radii, geom_buffer,
+                   binning_buffer, image_buffer, dL_dpix,
+                   {dL_dfeaturepix, dL_dfeaturepix_dtype == F3DGS_F16, dL_dfeaturepix_scale}, dL_depths, nullptr,
+                   nullptr, dL_dopacity, dL_dcolors_precomp, dL_dsemantic_feature, dL_dmean3D, dL_dcov3D_precomp,
+                   dL_dsh, dL_dscale, dL_drot, nullptr, debug, (cudaStream_t)cuda_stream, true, scratch,
+                   colors_precomp, dL_dmean2D_out, grad_accum, denom, (cudaEvent_t)composite_done_event};
+    if (const int rc = feature_rows(api, b, semantic_feature, semantic_feature_dtype, dL_dfeaturepix_dtype)) return rc;
+    b.dL_dcamera = dL_dcamera;
+    b.antialiasing = antialiasing != 0;
+    b.dL_dalpha = dL_dalpha;
+    b.dL_dinvdepth = dL_dinvdepth;
+    return backward(api, b);
 }
 
 }  // extern "C"

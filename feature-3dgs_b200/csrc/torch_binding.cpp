@@ -378,67 +378,54 @@ static BackwardGrads backward_grads(const torch::Tensor& background, const torch
 BackwardGrads RasterizeGaussiansBackwardCUDA(BACKWARD_PARAMS) { return backward_grads(BACKWARD_ARGS, nullptr); }
 
 // rasterize_gaussians_backward's 9 gradients + (dL_dviewmatrix [4,4], dL_dprojmatrix [4,4], dL_dcampos [3]), each in the
-// layout of its input (f3dgs_backward_cam / _cam_f16)
-decltype(std::tuple_cat(BackwardGrads(), std::tuple<torch::Tensor, torch::Tensor, torch::Tensor>()))
-RasterizeGaussiansBackwardCameraCUDA(BACKWARD_PARAMS) {
+// layout of its input
+using CameraGrads = decltype(std::tuple_cat(BackwardGrads(), std::tuple<torch::Tensor, torch::Tensor, torch::Tensor>()));
+
+// run(camera) -> the 9 gradients, with `camera` the 35 zeroed floats the camera gradient is added to; without `camera`
+// run(nullptr), and the three camera gradients are None
+template <typename Run>
+static CameraGrads with_camera_grads(const torch::Tensor& means3D, const bool camera, const Run& run) {
     TORCH_CHECK(means3D.is_cuda(), "means3D must be a CUDA tensor (this build has no CPU path)");
     const c10::cuda::CUDAGuard guard(means3D.device());
+    if (!camera) return std::tuple_cat(run(nullptr), std::make_tuple(torch::Tensor(), torch::Tensor(), torch::Tensor()));
     torch::Tensor cam = torch::zeros({F3DGS_CAMERA_GRAD_FLOATS}, means3D.options().dtype(torch::kFloat32));
-    return std::tuple_cat(backward_grads(BACKWARD_ARGS, cam.data_ptr<float>()),
+    return std::tuple_cat(run(cam.data_ptr<float>()),
                           std::make_tuple(cam.narrow(0, 0, 16).view({4, 4}), cam.narrow(0, 16, 16).view({4, 4}),
                                           cam.narrow(0, 32, 3)));
 }
 
+// f3dgs_backward_cam / _cam_f16
+CameraGrads RasterizeGaussiansBackwardCameraCUDA(BACKWARD_PARAMS) {
+    return with_camera_grads(means3D, true, [&](float* cam) { return backward_grads(BACKWARD_ARGS, cam); });
+}
+
 // rasterize_gaussians_backward_camera's 12 results, with the feature term of dL/dalpha in the geometric gradients
 // (f3dgs_backward_feature_geometry); without `camera` the three camera gradients are None and none is computed
-decltype(std::tuple_cat(BackwardGrads(), std::tuple<torch::Tensor, torch::Tensor, torch::Tensor>()))
-RasterizeGaussiansBackwardFeatureGeometryCUDA(BACKWARD_PARAMS, const bool camera) {
-    TORCH_CHECK(means3D.is_cuda(), "means3D must be a CUDA tensor (this build has no CPU path)");
-    const c10::cuda::CUDAGuard guard(means3D.device());
-    if (!camera)
-        return std::tuple_cat(backward_grads(BACKWARD_ARGS, nullptr, true),
-                              std::make_tuple(torch::Tensor(), torch::Tensor(), torch::Tensor()));
-    torch::Tensor cam = torch::zeros({F3DGS_CAMERA_GRAD_FLOATS}, means3D.options().dtype(torch::kFloat32));
-    return std::tuple_cat(backward_grads(BACKWARD_ARGS, cam.data_ptr<float>(), true),
-                          std::make_tuple(cam.narrow(0, 0, 16).view({4, 4}), cam.narrow(0, 16, 16).view({4, 4}),
-                                          cam.narrow(0, 32, 3)));
+CameraGrads RasterizeGaussiansBackwardFeatureGeometryCUDA(BACKWARD_PARAMS, const bool camera) {
+    return with_camera_grads(means3D, camera, [&](float* cam) { return backward_grads(BACKWARD_ARGS, cam, true); });
 }
 
 // rasterize_gaussians_backward_feature_geometry's 12 results for the buffers of rasterize_gaussians_antialiased
 // (f3dgs_backward_antialiased): the feature term of dL/dalpha only when `features` (the forward's semantic_feature) is
 // given, the camera gradients only with `camera`
-decltype(std::tuple_cat(BackwardGrads(), std::tuple<torch::Tensor, torch::Tensor, torch::Tensor>()))
-RasterizeGaussiansBackwardAntialiasedCUDA(BACKWARD_PARAMS, const bool camera,
-                                          const std::optional<torch::Tensor>& features) {
-    TORCH_CHECK(means3D.is_cuda(), "means3D must be a CUDA tensor (this build has no CPU path)");
-    const c10::cuda::CUDAGuard guard(means3D.device());
+CameraGrads RasterizeGaussiansBackwardAntialiasedCUDA(BACKWARD_PARAMS, const bool camera,
+                                                      const std::optional<torch::Tensor>& features) {
     const torch::Tensor f = features.has_value() ? *features : torch::Tensor();
-    if (!camera)
-        return std::tuple_cat(backward_grads(BACKWARD_ARGS, nullptr, false, true, f),
-                              std::make_tuple(torch::Tensor(), torch::Tensor(), torch::Tensor()));
-    torch::Tensor cam = torch::zeros({F3DGS_CAMERA_GRAD_FLOATS}, means3D.options().dtype(torch::kFloat32));
-    return std::tuple_cat(backward_grads(BACKWARD_ARGS, cam.data_ptr<float>(), false, true, f),
-                          std::make_tuple(cam.narrow(0, 0, 16).view({4, 4}), cam.narrow(0, 16, 16).view({4, 4}),
-                                          cam.narrow(0, 32, 3)));
+    return with_camera_grads(means3D, camera,
+                             [&](float* cam) { return backward_grads(BACKWARD_ARGS, cam, false, true, f); });
 }
 // rasterize_gaussians_backward_antialiased's 12 results for the buffers of rasterize_gaussians_alpha_invdepth (or of the
 // forward without planes in the same mode), with the gradients of the opacity and inverse-depth planes
 // (f3dgs_backward_alpha_invdepth)
-decltype(std::tuple_cat(BackwardGrads(), std::tuple<torch::Tensor, torch::Tensor, torch::Tensor>()))
-RasterizeGaussiansBackwardAlphaInvDepthCUDA(BACKWARD_PARAMS, const torch::Tensor& dL_dout_alpha,
-                                            const torch::Tensor& dL_dout_invdepth, const bool camera,
-                                            const std::optional<torch::Tensor>& features, const bool antialiasing) {
-    TORCH_CHECK(means3D.is_cuda(), "means3D must be a CUDA tensor (this build has no CPU path)");
-    const c10::cuda::CUDAGuard guard(means3D.device());
+CameraGrads RasterizeGaussiansBackwardAlphaInvDepthCUDA(BACKWARD_PARAMS, const torch::Tensor& dL_dout_alpha,
+                                                        const torch::Tensor& dL_dout_invdepth, const bool camera,
+                                                        const std::optional<torch::Tensor>& features,
+                                                        const bool antialiasing) {
     const torch::Tensor f = features.has_value() ? *features : torch::Tensor();
     const torch::Tensor planes[2] = {dL_dout_alpha, dL_dout_invdepth};
-    if (!camera)
-        return std::tuple_cat(backward_grads(BACKWARD_ARGS, nullptr, false, antialiasing, f, planes),
-                              std::make_tuple(torch::Tensor(), torch::Tensor(), torch::Tensor()));
-    torch::Tensor cam = torch::zeros({F3DGS_CAMERA_GRAD_FLOATS}, means3D.options().dtype(torch::kFloat32));
-    return std::tuple_cat(backward_grads(BACKWARD_ARGS, cam.data_ptr<float>(), false, antialiasing, f, planes),
-                          std::make_tuple(cam.narrow(0, 0, 16).view({4, 4}), cam.narrow(0, 16, 16).view({4, 4}),
-                                          cam.narrow(0, 32, 3)));
+    return with_camera_grads(means3D, camera, [&](float* cam) {
+        return backward_grads(BACKWARD_ARGS, cam, false, antialiasing, f, planes);
+    });
 }
 #undef BACKWARD_PARAMS
 #undef BACKWARD_ARGS
