@@ -51,26 +51,35 @@ def lib(built):
 
 
 # ------------------------------------------------------------------------------------------------------------ the model
-def planes_dfn(rec, Gc, Gd, GI):
-    """colour_depth_dots with the inverse-depth term: d = c.Gc + z Gd + GI / z per pair (GI [HW] float32)"""
+def planes_dfn(rec, Gc, Gd, GI, F=None, Gf=None):
+    """colour_depth_dots with the inverse-depth term: d = c.Gc + z Gd + GI / z per pair (GI [HW] float32), and with the
+    feature term f.Gf when F [P,C] (the rows the backward reads, as float32 values) and Gf [HW,C] (the map gradient as
+    the composite scales it) are given"""
     base = bw.colour_depth_dots(rec, Gc, Gd)
     rz = 1.0 / rec[:, 11].double()
     GI = GI.double().reshape(-1)
+    if F is not None:
+        F, Gf = F.double().to(GI.device), Gf.double().to(GI.device)
 
     def dfn(gid, pix):
         d, dabs = base(gid, pix)
         t = rz[gid] * GI[pix]
-        return d + t, dabs + t.abs()
+        d, dabs = d + t, dabs + t.abs()
+        if F is not None:
+            fg = F[gid] * Gf[pix]
+            d, dabs = d + fg.sum(1), dabs + fg.abs().sum(1)
+        return d, dabs
 
     return dfn
 
 
-def planes_model(pairs, w, rec, P, bg, Gc, Gd, GA, GI):
-    """(ref, bar) of the six geometric values with the planes' terms.  Gc [HW,3], Gd, GA, GI [HW]."""
+def planes_model(pairs, w, rec, P, bg, Gc, Gd, GA, GI, F=None, Gf=None):
+    """(ref, bar) of the six geometric values with the planes' terms (and the feature term, see planes_dfn).
+    Gc [HW,3], Gd, GA, GI [HW]."""
     bgp = Gc.double() * bg.double().to(Gc.device)
     GA = GA.double().reshape(-1)
-    # 5 products in d, and the reciprocal's rounding
-    return bw.composite_model(pairs, w, rec, P, planes_dfn(rec, Gc, Gd, GI), 6,
+    # 5 products in d, and the reciprocal's rounding; C more with the feature term
+    return bw.composite_model(pairs, w, rec, P, planes_dfn(rec, Gc, Gd, GI, F, Gf), 6 + (0 if F is None else F.shape[1]),
                               (bgp.sum(1) - GA, bgp.abs().sum(1) + GA.abs()))
 
 
@@ -310,28 +319,46 @@ def test_planes_match_the_blend_weight_identities(lib, name):
 
 
 # ----------------------------------------------------------------------------------------------------------- GPU: backward
-def _backward_planes(lib, v, ups, ga, gi, buffers=None, sf=None, aa=0):
-    """f3dgs_backward_alpha_invdepth on the View v (buffers: another forward's dict with geom/binning/img/R/radii)"""
+def _backward_planes(lib, v, ups, ga, gi, buffers=None, sf=None, aa=0, map_scale=None, camera=False, accum=None):
+    """f3dgs_backward_alpha_invdepth on the View v (buffers: another forward's dict with geom/binning/img/R/radii).
+    ups, ga, gi: numpy arrays or tensors.  sf: the feature rows of the feature term (float32 or float16), or None.
+    map_scale: ups[1] is a float16 map h standing for map_scale * float(h) (else a float32 map).  camera: also
+    dL_dcamera (35 floats, "camera").  accum: a dict of buffers to add into with f3dgs_backward_accum_alpha_invdepth
+    instead (opacity, feat, means3D, sh, scales, rotations, mean2D (dL_dmean2D_out), grad_accum, denom; colors /
+    cov3D when precomputed; camera when camera)."""
     dev = torch.device("cuda")
-    gc, gf, gd = (_t(u, dev) for u in ups)
-    ga, gi = _t(ga, dev), _t(gi, dev)
+    gc, gf, gd, ga, gi = (torch.as_tensor(u).to(dev) for u in (*ups, ga, gi))
     P, M = v.P, v.M
     b = v.base if buffers is None else buffers
     z = lambda *s: torch.zeros(*s, device=dev)  # noqa: E731
-    o = dict(mean2D=z(P, 3), conic=z(P, 4), opacity=z(P), color=z(P, 3), feat=z(P, v.C), means3D=z(P, 3),
-             cov3D=z(P, 6), sh=z(P, M, 3), scales=z(P, 3), rotations=z(P, 4), dz=z(P))
     sr = v.scales.numel() > 0
     null = ctypes.c_void_p(0)
     f = ctypes.c_float
+    stream = ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
     args = [P, v.D, M, b["R"], v.C, _ptr(v.bg), v.W, v.H, _ptr(v.d["means3D"]), _ptr(v.shs), _ptr(v.cols),
-            _ptr(sf) if sf is not None else null, F32, _ptr(v.scales), f(v.mod), _ptr(v.rots), _ptr(v.cov), _ptr(v.vm),
-            _ptr(v.pm), _ptr(v.cp), f(v.cam.tanfovx), f(v.cam.tanfovy), _ptr(b["radii"]), _ptr(b["geom"]),
-            _ptr(b["binning"]), _ptr(b["img"]), _ptr(gc), _ptr(gf), F32, f(1.0), _ptr(gd), _ptr(o["mean2D"]),
-            _ptr(o["conic"]), _ptr(o["opacity"]), _ptr(o["color"]), _ptr(o["feat"]), _ptr(o["means3D"]),
-            _ptr(o["cov3D"]), _ptr(o["sh"]) if M else null, _ptr(o["scales"]) if sr else null,
-            _ptr(o["rotations"]) if sr else null, _ptr(o["dz"]), 0,
-            ctypes.c_void_p(torch.cuda.current_stream().cuda_stream), null, aa, _ptr(ga), _ptr(gi)]
-    rc = lib.f3dgs_backward_alpha_invdepth(*args)
+            _ptr(sf), F16 if sf is not None and sf.dtype == torch.float16 else F32, _ptr(v.scales), f(v.mod),
+            _ptr(v.rots), _ptr(v.cov), _ptr(v.vm), _ptr(v.pm), _ptr(v.cp), f(v.cam.tanfovx), f(v.cam.tanfovy),
+            _ptr(b["radii"]), _ptr(b["geom"]), _ptr(b["binning"]), _ptr(b["img"]), _ptr(gc), _ptr(gf),
+            F32 if map_scale is None else F16, f(1.0 if map_scale is None else map_scale), _ptr(gd)]
+    if accum is None:
+        o = dict(mean2D=z(P, 3), conic=z(P, 4), opacity=z(P), color=z(P, 3), feat=z(P, v.C), means3D=z(P, 3),
+                 cov3D=z(P, 6), sh=z(P, M, 3), scales=z(P, 3), rotations=z(P, 4), dz=z(P))
+        if camera:
+            o["camera"] = z(35)
+        args += [_ptr(o["mean2D"]), _ptr(o["conic"]), _ptr(o["opacity"]), _ptr(o["color"]), _ptr(o["feat"]),
+                 _ptr(o["means3D"]), _ptr(o["cov3D"]), _ptr(o["sh"]) if M else null,
+                 _ptr(o["scales"]) if sr else null, _ptr(o["rotations"]) if sr else null, _ptr(o["dz"]), 0, stream]
+        entry = lib.f3dgs_backward_alpha_invdepth
+    else:
+        o = accum
+        scratch = torch.empty(lib.f3dgs_backward_scratch_bytes(P), dtype=torch.uint8, device=dev)
+        args += [_ptr(scratch), _ptr(o["opacity"]), _ptr(o["colors"]) if v.cols.numel() else null, _ptr(o["feat"]),
+                 _ptr(o["means3D"]), _ptr(o["cov3D"]) if v.cov.numel() else null, _ptr(o["sh"]) if M else null,
+                 _ptr(o["scales"]) if sr else null, _ptr(o["rotations"]) if sr else null, _ptr(o["mean2D"]),
+                 _ptr(o["grad_accum"]), _ptr(o["denom"]), null, 0, stream]
+        entry = lib.f3dgs_backward_accum_alpha_invdepth
+    args += [_ptr(o["camera"]) if camera else null, int(aa), _ptr(ga), _ptr(gi)]
+    rc = entry(*args)
     assert rc == 0, lib.f3dgs_last_error()
     torch.cuda.synchronize()
     return o
@@ -427,26 +454,29 @@ def test_zero_plane_gradients_give_the_counterparts_bits(lib, C, aa):
             _equal(new(semantic_feature=sf, camera=True), _C.rasterize_gaussians_backward_feature_geometry(*a, True),
                    "feature geometry camera")
     # the accumulating entry (ViewBatch) with zero planes, and with g_alpha = g_invdepth = None, against the call
-    # without them; the planes forward's buffers against the plain forward's
+    # without them; the planes forward's buffers against the plain forward's.  With and without the camera, and with
+    # features that the feature term leaves out (the _antialiased / plain accumulating counterparts)
     from diff_gaussian_rasterization.parallel import ViewBatch
 
     d = scenegen.to_torch(sc, dev)
     params = dict(means3D=d["means3D"], scales=d["scales"], rotations=d["rotations"], opacities=d["opacities"],
                   shs=d["shs"], semantic_feature=sf if C else None)
     rs = _settings(sc, cam)
-    outs = []
-    for planes in (None, "none", "zeros"):
-        vb = ViewBatch(params)
-        ctx = (vb.forward_alpha_invdepth(rs, antialiasing=aa) if planes else vb.forward(rs, antialiasing=aa))[-1]
-        kw = dict(g_alpha=z, g_invdepth=z) if planes == "zeros" else {}
-        for half in (False, True):
-            g = gf.half() if half else gf
-            cam_g = vb.backward(ctx, gc, g if C else None, gd, camera=True, feature_geometry=bool(C), **kw)
-            outs.append((vb.flat.clone(), torch.cat([cam_g.viewmatrix.reshape(-1), cam_g.projmatrix.reshape(-1),
-                                                     cam_g.campos])))
-    # outs: (without planes, None planes, zero planes) x (float32 map, then float16 map added into the same buffer)
-    for i, o in enumerate(outs[2:]):
-        assert torch.equal(outs[i % 2][0], o[0]) and torch.equal(outs[i % 2][1], o[1]), i
+    for camera, fg in [(True, bool(C)), (False, bool(C))] + ([(True, False)] if C else []):
+        outs = []
+        for planes in (None, "none", "zeros"):
+            vb = ViewBatch(params)
+            ctx = (vb.forward_alpha_invdepth(rs, antialiasing=aa) if planes else vb.forward(rs, antialiasing=aa))[-1]
+            kw = dict(g_alpha=z, g_invdepth=z) if planes == "zeros" else {}
+            for half in (False, True):
+                g = gf.half() if half else gf
+                cam_g = vb.backward(ctx, gc, g if C else None, gd, camera=camera, feature_geometry=fg, **kw)
+                outs.append((vb.flat.clone(), torch.cat([cam_g.viewmatrix.reshape(-1), cam_g.projmatrix.reshape(-1),
+                                                         cam_g.campos]) if camera else None))
+        # outs: (without planes, None planes, zero planes) x (float32 map, then float16 map added into the same buffer)
+        for i, o in enumerate(outs[2:]):
+            assert torch.equal(outs[i % 2][0], o[0]), (camera, fg, i)
+            assert not camera or torch.equal(outs[i % 2][1], o[1]), (camera, fg, i)
 
 
 def _settings(sc, cam, dev="cuda", **over):
@@ -533,9 +563,12 @@ def test_view_batch_sums_three_views(lib):
 
 # ---------------------------------------------------------------------------------------------------------- GPU: autograd
 @pytest.mark.gpu
+@pytest.mark.parametrize("half", [False, True])
+@pytest.mark.parametrize("antialiasing", [False, True])
 @pytest.mark.parametrize("feature_geometry", [False, True])
 @pytest.mark.parametrize("camera", [False, True])
-def test_autograd_equals_the_binding(lib, camera, feature_geometry):
+def test_autograd_equals_the_binding(lib, camera, feature_geometry, antialiasing, half):
+    """half: float16 features, whose float16 feature map's gradient reaches the binding as float16"""
     import diff_gaussian_rasterization as dgr
     from diff_gaussian_rasterization import _C
 
@@ -543,29 +576,38 @@ def test_autograd_equals_the_binding(lib, camera, feature_geometry):
     dev = torch.device("cuda")
     H, W = cam.image_height, cam.image_width
     d = scenegen.to_torch(sc, dev, requires_grad=True)
+    if half:
+        d["semantic_feature"] = d["semantic_feature"].detach().half().requires_grad_()
     rs = _settings(sc, cam)
     if camera:
         rs = rs._replace(viewmatrix=rs.viewmatrix.clone().requires_grad_(), projmatrix=rs.projmatrix.clone(
         ).requires_grad_(), campos=rs.campos.clone().requires_grad_())
     ups = [_t(u, dev) for u in bw.upstream(H, W, sc.C, 8)] + [_t(x, dev) for x in _plane_grads(H, W, 9)]
-    ras = dgr.AlphaInvDepthGaussianRasterizer(rs, feature_geometry=feature_geometry)
+    if half:
+        ups[1] = ups[1].half()
+    ras = dgr.AlphaInvDepthGaussianRasterizer(rs, feature_geometry=feature_geometry, antialiasing=antialiasing)
     outs = ras(means3D=d["means3D"], means2D=torch.zeros_like(d["means3D"]), opacities=d["opacities"], shs=d["shs"],
                semantic_feature=d["semantic_feature"], scales=d["scales"], rotations=d["rotations"])
     color, fmap, radii, depth, alpha, invdepth = outs
-    loss = sum((o * g).sum() for o, g in zip((color, fmap, depth, alpha, invdepth), ups))
+    assert fmap.dtype == d["semantic_feature"].dtype
+    loss = sum((o * g).sum() for o, g in zip((color, depth, alpha, invdepth), ups[:1] + ups[2:]))
+    # the feature map's gradient is ups[1] in the map's own dtype
+    loss = loss + (fmap * ups[1]).sum()
     cam_t = [rs.viewmatrix, rs.projmatrix, rs.campos] if camera else []
     keys = ("means3D", "opacities", "shs", "scales", "rotations", "semantic_feature")
     got = torch.autograd.grad(loss, [d[k] for k in keys] + cam_t)
-    f = _plain_forward(sc, cam, d["semantic_feature"].detach(), False)
+    sf = d["semantic_feature"].detach()
+    f = _plain_forward(sc, cam, sf, antialiasing)
     r = _C.rasterize_gaussians_backward_alpha_invdepth(
-        *_bargs(sc, cam, f, d["semantic_feature"].detach(), ups[:3]), ups[3], ups[4], camera=camera,
-        semantic_feature=d["semantic_feature"].detach() if feature_geometry else None)
+        *_bargs(sc, cam, f, sf, ups[:3]), ups[3], ups[4], camera=camera,
+        semantic_feature=sf if feature_geometry else None, antialiasing=antialiasing)
     want = (r[4], r[3], r[6], r[7], r[8], r[2]) + tuple(r[9:12] if camera else ())
     for k, a, b in zip(keys + ("viewmatrix", "projmatrix", "campos"), got, want):
-        assert torch.equal(a.reshape(b.shape), b), k
+        assert a.dtype == (sf.dtype if k == "semantic_feature" else torch.float32), k
+        assert torch.equal(a.reshape(b.shape), b.to(a.dtype)), k
     # a loss on colour only: GaussianRasterizer's gradients
-    outs2 = dgr.GaussianRasterizer(rs, feature_geometry=feature_geometry)(
-        means3D=d["means3D"], means2D=torch.zeros_like(d["means3D"]), opacities=d["opacities"], shs=d["shs"],
+    outs2 = (dgr.AntialiasedGaussianRasterizer if antialiasing else dgr.GaussianRasterizer)(
+        rs, feature_geometry=feature_geometry)(means3D=d["means3D"], means2D=torch.zeros_like(d["means3D"]), opacities=d["opacities"], shs=d["shs"],
         semantic_feature=d["semantic_feature"], scales=d["scales"], rotations=d["rotations"])
     outs = ras(means3D=d["means3D"], means2D=torch.zeros_like(d["means3D"]), opacities=d["opacities"], shs=d["shs"],
                semantic_feature=d["semantic_feature"], scales=d["scales"], rotations=d["rotations"])

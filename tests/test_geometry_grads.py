@@ -265,9 +265,13 @@ def lib(built):
 class View:
     """One view on the device with the rasterizer's options: its forward, the pairs, the extracted W and what the
     backward entries need.  shs / cov / cols / mod: the SH rows (default the scene's), precomputed covariances or
-    colours, and the scale modifier."""
+    colours, and the scale modifier.  C: the feature width.  planes: render with the forward that also writes the
+    opacity and inverse-depth planes (rasterize_gaussians_alpha_invdepth), with antialiased opacities when
+    antialiasing (the records then hold op_eff)."""
 
-    def __init__(self, sc, cam, shs=None, D=None, cov=None, cols=None, mod=1.0, group=512, weights=True):
+    def __init__(self, sc, cam, shs=None, D=None, cov=None, cols=None, mod=1.0, group=512, weights=True, C=8,
+                 planes=False, antialiasing=False):
+        assert planes or not antialiasing
         dev = torch.device("cuda")
         self.sc, self.cam, self.mod = sc, cam, mod
         self.P, self.W, self.H = sc.P, cam.image_width, cam.image_height
@@ -282,7 +286,7 @@ class View:
         self.vm, self.pm, self.cp = (torch.tensor(a, device=dev).contiguous() for a in (cam.viewmatrix,
                                                                                       cam.projmatrix, cam.campos))
         self.bg = torch.tensor(sc.bg, device=dev)
-        self.C = 8
+        self.C, self.planes, self.antialiasing = C, planes, antialiasing
         self.feats = torch.randn(self.P, 1, self.C, generator=torch.Generator().manual_seed(3)).to(dev)
         self.base = self.forward(self.feats)
         b = self.base
@@ -294,13 +298,19 @@ class View:
     def forward(self, sf):
         from diff_gaussian_rasterization import _C
 
-        R, color, fmap, depth, radii, geom, binning, img = _C.rasterize_gaussians(
-            self.bg, self.d["means3D"], self.cols, sf, self.d["opacities"], self.scales, self.rots, self.mod,
-            self.cov, self.vm, self.pm, self.cam.tanfovx, self.cam.tanfovy, self.H, self.W, self.shs, self.D, self.cp,
-            False, False)
+        args = (self.bg, self.d["means3D"], self.cols, sf, self.d["opacities"], self.scales, self.rots, self.mod,
+                self.cov, self.vm, self.pm, self.cam.tanfovx, self.cam.tanfovy, self.H, self.W, self.shs, self.D,
+                self.cp, False, False)
+        planes = {}
+        if self.planes:
+            R, color, fmap, depth, alpha, invdepth, radii, geom, binning, img = _C.rasterize_gaussians_alpha_invdepth(
+                *args, antialiasing=self.antialiasing)
+            planes = dict(alpha=alpha, invdepth=invdepth)
+        else:
+            R, color, fmap, depth, radii, geom, binning, img = _C.rasterize_gaussians(*args)
         pl, ranges, n_contrib, final_T, rec = _C.debug_views(geom, binning, img, self.P, self.W, self.H, R)
         return dict(R=R, color=color, fmap=fmap, depth=depth, radii=radii, geom=geom, binning=binning, img=img,
-                    point_list=pl, ranges=ranges, n_contrib=n_contrib, final_T=final_T, rec=rec)
+                    point_list=pl, ranges=ranges, n_contrib=n_contrib, final_T=final_T, rec=rec, **planes)
 
     def _onehot(self, g0, C):
         sf = torch.zeros(self.P, 1, C, device="cuda")
