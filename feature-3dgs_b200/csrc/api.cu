@@ -1399,6 +1399,115 @@ int f3dgs_reset_opacity(int P, float* raw_opacity, float* exp_avg, float* exp_av
     return api.cuda(launch_reset_opacity(P, raw_opacity, exp_avg, exp_avg_sq, ceiling, (cudaStream_t)cuda_stream));
 }
 
+}  // extern "C"
+
+namespace {
+// The 21 pointers of f3dgs_gaussian_fields[3] in order, and their byte ranges over `rows` rows; false if a field of
+// nonzero width over rows > 0 is NULL (f_rest has width 0 when M == 1, semantic_feature when C == 0)
+bool gaussian_fields(const f3dgs_gaussian_fields f[3], int M, int C, long long rows, float* out[21], Range ranges[21]) {
+    const size_t width[7] = {3, 3, 3 * (size_t)(M - 1), 1, 3, 4, (size_t)C};
+    for (int g = 0; g < 3; g++) {
+        float* p[7] = {f[g].xyz, f[g].f_dc, f[g].f_rest, f[g].opacity, f[g].scaling, f[g].rotation, f[g].semantic_feature};
+        for (int j = 0; j < 7; j++) {
+            if (width[j] && rows > 0 && !p[j]) return false;
+            out[7 * g + j] = p[j];
+            ranges[7 * g + j] = {p[j], (size_t)rows * width[j] * 4};
+        }
+    }
+    return true;
+}
+
+// Does any of the first `n_out` ranges (the written ones) overlap any other range?
+template <size_t N>
+bool any_overlap(const Range (&r)[N], size_t n_out) {
+    for (size_t i = 0; i < n_out; i++)
+        if (overlaps(r[i], r)) return true;
+    return false;
+}
+
+bool mcmc_sizes_ok(int P, int M, int C) {
+    return P >= 0 && 3 * (long long)P <= INT_MAX && M >= 1 && C >= 0 && C <= F3DGS_MAX_FEATURE_DIM;
+}
+constexpr const char* kMcmcBadSizes = "bad sizes (0 <= 3 P <= INT_MAX, M >= 1, 0 <= C <= F3DGS_MAX_FEATURE_DIM, 0 <= n <= P)";
+}  // namespace
+
+extern "C" {
+
+size_t f3dgs_mcmc_scratch_bytes(int P) {
+    return scratch_bytes(__func__, [=](size_t* b) { return mcmc_scratch_bytes(P, b); });
+}
+
+int f3dgs_mcmc_plan(int P, const float* raw_opacity, float min_opacity, char* scratch, int32_t* n_dead, int32_t* index,
+                    float* alive_opacity, void* cuda_stream) {
+    const Api api(__func__);
+    if (P < 0 || 3 * (long long)P > INT_MAX) return api.invalid("bad sizes (0 <= 3 P <= INT_MAX)");
+    if (!std::isfinite(min_opacity)) return api.invalid("min_opacity must be finite");
+    if (!n_dead || (P > 0 && (!raw_opacity || !scratch || !index || !alive_opacity))) return api.invalid("NULL pointer");
+    const size_t b = (size_t)P * 4;
+    const Range r[5] = {{n_dead, 4}, {index, b}, {alive_opacity, b}, {scratch, mcmc_scratch_fixed_bytes(P)},
+                        {raw_opacity, b}};
+    if (any_overlap(r, 4)) return api.invalid("n_dead, index, alive_opacity, scratch and raw_opacity overlap");
+    return api.cuda(launch_mcmc_plan(P, raw_opacity, min_opacity, scratch, n_dead, index, alive_opacity,
+                                     (cudaStream_t)cuda_stream));
+}
+
+int f3dgs_mcmc_relocate(int P, int M, int C, int n, const int32_t* dead, const int32_t* src, float min_opacity,
+                        const f3dgs_gaussian_fields fields[3], uint16_t* semantic_feature_f16, char* scratch,
+                        void* cuda_stream) {
+    const Api api(__func__);
+    if (!mcmc_sizes_ok(P, M, C) || n < 0 || n > P) return api.invalid(kMcmcBadSizes);
+    if (!std::isfinite(min_opacity)) return api.invalid("min_opacity must be finite");
+    if (!fields) return api.invalid("NULL pointer");
+    Range r[25];
+    float* f[21];
+    if (!gaussian_fields(fields, M, C, P, f, r)) return api.invalid("NULL pointer (a field)");
+    if (n > 0 && (!dead || !src || !scratch)) return api.invalid("NULL pointer");
+    r[21] = {semantic_feature_f16, (size_t)P * C * 2};
+    r[22] = {scratch, mcmc_scratch_fixed_bytes(P)};
+    r[23] = {dead, (size_t)n * 4};
+    r[24] = {src, (size_t)n * 4};
+    if (any_overlap(r, 23)) return api.invalid("fields, semantic_feature_f16, scratch, dead and src overlap");
+    return api.cuda(launch_mcmc_relocate(P, M, C, n, dead, src, min_opacity, f,
+                                         reinterpret_cast<__half*>(semantic_feature_f16), scratch,
+                                         (cudaStream_t)cuda_stream));
+}
+
+int f3dgs_mcmc_add(int P, int M, int C, int n, const int32_t* src, float min_opacity,
+                   const f3dgs_gaussian_fields src_fields[3], const f3dgs_gaussian_fields dst_fields[3], char* scratch,
+                   void* cuda_stream) {
+    const Api api(__func__);
+    if (!mcmc_sizes_ok(P, M, C) || n < 0 || n > P || 3 * ((long long)P + n) > INT_MAX) return api.invalid(kMcmcBadSizes);
+    if (!std::isfinite(min_opacity)) return api.invalid("min_opacity must be finite");
+    if (!src_fields || !dst_fields) return api.invalid("NULL pointer");
+    Range r[44];
+    float *s[21], *d[21];
+    if (!gaussian_fields(dst_fields, M, C, (long long)P + n, d, r) || !gaussian_fields(src_fields, M, C, P, s, r + 21))
+        return api.invalid("NULL pointer (a field)");
+    if (P > 0 && !scratch) return api.invalid("NULL pointer");
+    if (n > 0 && !src) return api.invalid("NULL pointer");
+    r[42] = {scratch, mcmc_scratch_fixed_bytes(P)};
+    r[43] = {src, (size_t)n * 4};
+    // the dst fields and the scratch are written; the src fields may share nothing with them
+    bool bad = false;
+    for (int i = 0; i < 21 && !bad; i++) bad = overlaps(r[i], r);
+    if (bad || overlaps(r[42], r)) return api.invalid("a dst field or the scratch overlaps a field, src or the scratch");
+    return api.cuda(launch_mcmc_add(P, M, C, n, src, min_opacity, s, d, scratch, (cudaStream_t)cuda_stream));
+}
+
+int f3dgs_mcmc_inject_noise(int P, float* xyz, const float* raw_opacity, const float* raw_scaling,
+                            const float* raw_rotation, const float* eps, float scale, void* cuda_stream) {
+    const Api api(__func__);
+    if (P < 0 || 4 * (long long)P > INT_MAX) return api.invalid("bad sizes (0 <= 4 P <= INT_MAX)");
+    if (!std::isfinite(scale)) return api.invalid("scale must be finite");
+    if (P == 0) return 0;
+    if (!xyz || !raw_opacity || !raw_scaling || !raw_rotation || !eps) return api.invalid("NULL pointer");
+    const size_t b = (size_t)P * 4;
+    const Range r[5] = {{xyz, 3 * b}, {raw_opacity, b}, {raw_scaling, 3 * b}, {raw_rotation, 4 * b}, {eps, 3 * b}};
+    if (any_overlap(r, 1)) return api.invalid("xyz overlaps raw_opacity, raw_scaling, raw_rotation or eps");
+    return api.cuda(launch_mcmc_inject_noise(P, xyz, raw_opacity, raw_scaling, raw_rotation, eps, scale,
+                                             (cudaStream_t)cuda_stream));
+}
+
 int f3dgs_activate(int P, int M, const float* raw_opacity, const float* raw_scaling, const float* raw_rotation,
                    const float* features_dc, const float* features_rest, float* opacity, float* scales, float* rotations,
                    float* shs, void* cuda_stream) {

@@ -171,6 +171,21 @@ cudaError_t launch_densify_apply(int P, int M, int C, const char* scratch, const
 cudaError_t launch_reset_opacity(int P, float* raw_opacity, float* exp_avg, float* exp_avg_sq, float ceiling,
                                  cudaStream_t s);
 
+// ---- mcmc.cu: 3DGS-MCMC relocation, growth and position noise (include/f3dgs_b200.h: f3dgs_mcmc_*).  scratch is
+// mcmc_scratch_bytes(P) bytes whose first mcmc_scratch_fixed_bytes(P) need no device query; fields are the 21 fields of
+// f3dgs_gaussian_fields[3] in order
+cudaError_t mcmc_scratch_bytes(int P, size_t* bytes);
+size_t mcmc_scratch_fixed_bytes(int P);
+cudaError_t launch_mcmc_plan(int P, const float* raw_opacity, float min_opacity, char* scratch, int32_t* n_dead,
+                             int32_t* index, float* alive_opacity, cudaStream_t s);
+cudaError_t launch_mcmc_relocate(int P, int M, int C, int n, const int32_t* dead, const int32_t* src, float min_opacity,
+                                 float* const fields[21], __half* feature_f16, char* scratch, cudaStream_t s);
+cudaError_t launch_mcmc_add(int P, int M, int C, int n, const int32_t* src, float min_opacity,
+                            const float* const src_fields[21], float* const dst_fields[21], char* scratch,
+                            cudaStream_t s);
+cudaError_t launch_mcmc_inject_noise(int P, float* xyz, const float* raw_opacity, const float* raw_scaling,
+                                     const float* raw_rotation, const float* eps, float scale, cudaStream_t s);
+
 // ---- optimizer.cu: activation prologue and fused Adam step (include/f3dgs_b200.h: f3dgs_activate / f3dgs_adam_step)
 cudaError_t launch_activate(int P, int M, const float* raw_opacity, const float* raw_scaling, const float* raw_rotation,
                             const float* features_dc, const float* features_rest, float* opacity, float* scales,

@@ -1013,6 +1013,121 @@ void resetOpacity(torch::Tensor raw_opacity, torch::Tensor exp_avg, torch::Tenso
              "f3dgs_reset_opacity");
 }
 
+// ---- fixed-budget densification, 3DGS-MCMC (f3dgs_mcmc_plan / _relocate / _add / _inject_noise)
+namespace {
+// The 21 tensors raw (xyz, f_dc, f_rest, opacity, scaling, rotation, semantic_feature), exp_avg, exp_avg_sq of `rows`
+// rows -> f3dgs_gaussian_fields[3]; M and C are read from the f_rest and semantic_feature shapes of the first group
+void gaussian_fields(const std::vector<torch::Tensor>& t, int64_t rows, int64_t M, int64_t C, f3dgs_gaussian_fields f[3]) {
+    TORCH_CHECK(t.size() == 21, "21 field tensors expected (raw, exp_avg, exp_avg_sq)");
+    const auto dev = t[0].device();
+    const int64_t width[7] = {3, 3, 3 * (M - 1), 1, 3, 4, C};
+    static const char* names[7] = {"xyz", "f_dc", "f_rest", "opacity", "scaling", "rotation", "semantic_feature"};
+    for (int i = 0; i < 21; i++) {
+        f3dgs_gaussian_fields& g = f[i / 7];
+        float** slot[7] = {&g.xyz, &g.f_dc, &g.f_rest, &g.opacity, &g.scaling, &g.rotation, &g.semantic_feature};
+        *slot[i % 7] = in_place(t[i], dev, rows * width[i % 7], names[i % 7]);
+    }
+}
+
+// P, M, C of a group of 21 field tensors
+std::tuple<int64_t, int64_t, int64_t> field_sizes(const std::vector<torch::Tensor>& t) {
+    TORCH_CHECK(t.size() == 21, "21 field tensors expected (raw, exp_avg, exp_avg_sq)");
+    TORCH_CHECK(t[0].is_cuda(), "parameters must be CUDA tensors (this build has no CPU path)");
+    TORCH_CHECK(t[0].dim() == 2 && t[0].size(1) == 3 && t[0].size(0) <= INT32_MAX / 3, "xyz must be [P,3], 3 P < 2^31");
+    TORCH_CHECK(t[2].dim() == 3 && t[6].dim() >= 2, "f_rest must be [P,M-1,3], semantic_feature [P,1,C]");
+    return {t[0].size(0), 1 + t[2].size(1), t[6].size(-1)};
+}
+
+// A contiguous int32 index tensor on `dev` -> its data (nullptr if empty)
+const int32_t* indices(const torch::Tensor& t, const torch::Device& dev, const char* name) {
+    TORCH_CHECK(t.is_cuda() && t.device() == dev && t.scalar_type() == torch::kInt32 && t.is_contiguous() && t.dim() == 1,
+                name, " must be a contiguous 1-D int32 tensor on ", dev);
+    return t.numel() ? t.data_ptr<int32_t>() : nullptr;
+}
+
+char* scratch_ptr(const torch::Tensor& scratch) {
+    return scratch.numel() ? reinterpret_cast<char*>(scratch.data_ptr()) : nullptr;
+}
+}  // namespace
+
+// -> (scratch, n_dead device int32[1], index int32[P]: dead ascending then alive ascending, alive_opacity float[P]: the
+// first P - n_dead are the alive opacities in index order)
+std::tuple<torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor> mcmcPlan(const torch::Tensor& raw_opacity,
+                                                                                double min_opacity) {
+    TORCH_CHECK(raw_opacity.is_cuda(), "parameters must be CUDA tensors (this build has no CPU path)");
+    TORCH_CHECK(raw_opacity.numel() <= INT32_MAX / 3, "mcmc_plan: 3 P must be below 2^31");
+    const auto dev = raw_opacity.device();
+    const c10::cuda::CUDAGuard guard(dev);
+    const int P = (int)raw_opacity.numel();
+    const float* op = in_place(raw_opacity, dev, P, "raw_opacity");
+    torch::Tensor scratch = scratch_tensor(f3dgs_mcmc_scratch_bytes(P), "f3dgs_mcmc_scratch_bytes", raw_opacity);
+    const auto i32 = raw_opacity.options().dtype(torch::kInt32);
+    torch::Tensor n_dead = torch::empty({1}, i32), index = torch::empty({P}, i32);
+    torch::Tensor alive = torch::empty({P}, raw_opacity.options());
+    cudaStream_t stream = c10::cuda::getCurrentCUDAStream().stream();
+    check_rc(f3dgs_mcmc_plan(P, op, (float)min_opacity, scratch_ptr(scratch), n_dead.data_ptr<int32_t>(),
+                             P ? index.data_ptr<int32_t>() : nullptr, P ? alive.data_ptr<float>() : nullptr,
+                             (void*)stream),
+             "f3dgs_mcmc_plan");
+    return std::make_tuple(scratch, n_dead, index, alive);
+}
+
+// fields: the 21 tensors, updated in place; feature_f16: the float16 [P,1,C] copy of the features, or None
+void mcmcRelocate(const torch::Tensor& scratch, const torch::Tensor& dead, const torch::Tensor& src, double min_opacity,
+                  const std::vector<torch::Tensor>& fields, const c10::optional<torch::Tensor>& feature_f16) {
+    const auto [P, M, C] = field_sizes(fields);
+    const auto dev = fields[0].device();
+    const c10::cuda::CUDAGuard guard(dev);
+    TORCH_CHECK(dead.numel() == src.numel(), "mcmc_relocate: dead and src must have the same length");
+    f3dgs_gaussian_fields f[3];
+    gaussian_fields(fields, P, M, C, f);
+    uint16_t* h16 = nullptr;
+    if (feature_f16.has_value() && feature_f16->defined() && feature_f16->numel()) {
+        const torch::Tensor& h = *feature_f16;
+        TORCH_CHECK(h.is_cuda() && h.device() == dev && h.scalar_type() == torch::kFloat16 && h.is_contiguous() &&
+                        h.numel() == P * C,
+                    "feature_f16 must be a contiguous float16 tensor of ", P * C, " elements on ", dev);
+        h16 = reinterpret_cast<uint16_t*>(h.data_ptr<at::Half>());
+    }
+    cudaStream_t stream = c10::cuda::getCurrentCUDAStream().stream();
+    check_rc(f3dgs_mcmc_relocate((int)P, (int)M, (int)C, (int)dead.numel(), indices(dead, dev, "dead"),
+                                 indices(src, dev, "src"), (float)min_opacity, f, h16, scratch_ptr(scratch),
+                                 (void*)stream),
+             "f3dgs_mcmc_relocate");
+}
+
+// src_fields: the 21 tensors of P rows; dst_fields: 21 tensors of P + n rows, written
+void mcmcAdd(const torch::Tensor& scratch, const torch::Tensor& src, double min_opacity,
+             const std::vector<torch::Tensor>& src_fields, const std::vector<torch::Tensor>& dst_fields) {
+    const auto [P, M, C] = field_sizes(src_fields);
+    const auto dev = src_fields[0].device();
+    const c10::cuda::CUDAGuard guard(dev);
+    const int64_t n = src.numel();
+    f3dgs_gaussian_fields s[3], d[3];
+    gaussian_fields(src_fields, P, M, C, s);
+    gaussian_fields(dst_fields, P + n, M, C, d);
+    cudaStream_t stream = c10::cuda::getCurrentCUDAStream().stream();
+    check_rc(f3dgs_mcmc_add((int)P, (int)M, (int)C, (int)n, indices(src, dev, "src"), (float)min_opacity, s, d,
+                            scratch_ptr(scratch), (void*)stream),
+             "f3dgs_mcmc_add");
+}
+
+// xyz [P,3] in place; eps [P,3] the normals
+void mcmcInjectNoise(torch::Tensor xyz, const torch::Tensor& raw_opacity, const torch::Tensor& raw_scaling,
+                     const torch::Tensor& raw_rotation, const torch::Tensor& eps, double scale) {
+    TORCH_CHECK(xyz.is_cuda(), "parameters must be CUDA tensors (this build has no CPU path)");
+    TORCH_CHECK(xyz.dim() == 2 && xyz.size(1) == 3 && xyz.size(0) <= INT32_MAX / 4, "xyz must be [P,3], 4 P < 2^31");
+    const auto dev = xyz.device();
+    const c10::cuda::CUDAGuard guard(dev);
+    const int64_t P = xyz.size(0);
+    cudaStream_t stream = c10::cuda::getCurrentCUDAStream().stream();
+    check_rc(f3dgs_mcmc_inject_noise((int)P, in_place(xyz, dev, 3 * P, "xyz"), in_place(raw_opacity, dev, P, "raw_opacity"),
+                                     in_place(raw_scaling, dev, 3 * P, "raw_scaling"),
+                                     in_place(raw_rotation, dev, 4 * P, "raw_rotation"), in_place(eps, dev, 3 * P, "eps"),
+                                     (float)scale, (void*)stream),
+             "f3dgs_mcmc_inject_noise");
+}
+
 // ---- activation prologue + fused optimizer step (f3dgs_activate / f3dgs_adam_step): in-place on the caller's tensors
 void activateParams(const torch::Tensor& raw_opacity, const torch::Tensor& raw_scaling, const torch::Tensor& raw_rotation,
                     const torch::Tensor& f_dc, const torch::Tensor& f_rest, torch::Tensor opacity, torch::Tensor scales,
@@ -1170,6 +1285,13 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     m.def("densify_apply", &densifyApply);
     m.def("reset_opacity", &resetOpacity, pybind11::arg("raw_opacity"), pybind11::arg("exp_avg"),
           pybind11::arg("exp_avg_sq"), pybind11::arg("ceiling") = 0.01);
+    m.def("mcmc_plan", &mcmcPlan, pybind11::arg("raw_opacity"), pybind11::arg("min_opacity"));
+    m.def("mcmc_relocate", &mcmcRelocate, pybind11::arg("scratch"), pybind11::arg("dead"), pybind11::arg("src"),
+          pybind11::arg("min_opacity"), pybind11::arg("fields"), pybind11::arg("feature_f16") = pybind11::none());
+    m.def("mcmc_add", &mcmcAdd, pybind11::arg("scratch"), pybind11::arg("src"), pybind11::arg("min_opacity"),
+          pybind11::arg("src_fields"), pybind11::arg("dst_fields"));
+    m.def("mcmc_inject_noise", &mcmcInjectNoise, pybind11::arg("xyz"), pybind11::arg("raw_opacity"),
+          pybind11::arg("raw_scaling"), pybind11::arg("raw_rotation"), pybind11::arg("eps"), pybind11::arg("scale"));
     m.def("activate", &activateParams);
     m.def("adam_step", &adamStep, pybind11::arg("kind"), pybind11::arg("param"), pybind11::arg("grad_activated"),
           pybind11::arg("exp_avg"), pybind11::arg("exp_avg_sq"), pybind11::arg("M"), pybind11::arg("lr"),

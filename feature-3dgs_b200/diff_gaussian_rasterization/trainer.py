@@ -17,13 +17,17 @@ _opacity, _scaling, _rotation, _semantic_feature`, :47-58) as plain CUDA tensors
                         step(lrs, visible=vb.visible()) is the sparse Adam step on the Gaussians the step's views saw;
   densify_and_prune()   clone / split / prune (:350-434) with the optimizer state carried along, in two native calls
                         (f3dgs_densify_plan / f3dgs_densify_apply) with one host read in between;
-  reset_opacity()       :231-234 in one kernel (f3dgs_reset_opacity).
+  reset_opacity()       :231-234 in one kernel (f3dgs_reset_opacity);
+  relocate_and_add()    3DGS-MCMC's fixed-budget densification (relocate_gs + add_new_gs) with the optimizer state
+                        carried along (f3dgs_mcmc_plan / _relocate / _add), one host read; inject_noise() and
+                        add_regularizer_grads() its per-step position noise and regulariser gradients.
 
 Float16 feature fields: with feature_dtype=torch.float16 the rasterizer reads a float16 working copy
 act["semantic_feature"] of the float32 master raw["semantic_feature"], so every view renders a float16 map and the feature
 loss hands back a float16 gradient (feature_head `*_and_grad(..., grad_dtype=torch.float16)`).  The master, its Adam
 moments and the accumulated gradient stay float32; the copy is made by one cast at construction and after
-densify_and_prune, and step() refreshes it in the Adam pass itself (f3dgs_adam_step_f16out).
+densify_and_prune, relocate_and_add writes the relocated rows' copies in its own pass, and step() refreshes it in the
+Adam pass itself (f3dgs_adam_step_f16out).
 """
 import math
 from typing import Dict, Optional
@@ -212,6 +216,96 @@ class GaussianState:
         from . import _C
 
         _C.reset_opacity(self.raw["opacity"], self.exp_avg["opacity"], self.exp_avg_sq["opacity"])
+
+    # ---------------------------------------------------------------------------------------------- 3DGS-MCMC
+    def relocate_and_add(self, cap_max: int, min_opacity: float = 0.005, generator=None):
+        """Fixed-budget densification of 3DGS-MCMC (Kheradmand et al., NeurIPS 2024): the official code's relocate_gs
+        followed by add_new_gs; returns (n_relocated, n_added).  Use it in place of densify_and_prune: the cloud grows by
+        at most 5 % per call and never past cap_max, so the memory of a run is set by cap_max.
+
+        Relocation: the Gaussians with sigmoid(opacity) <= min_opacity (dead) are moved onto alive ones, drawn with
+        torch.multinomial(alive opacity / (sum + float32 eps), n_dead, replacement=True, generator=generator).  Addition:
+        n = min(cap_max, int(1.05 P)) - P new rows, drawn the same way over all P opacities, are appended.  A source
+        drawn c times and its copies all take the opacity and scale of the relocation rule (csrc/mcmc.cu: N = min(c + 1,
+        51) copies render like the original did) and zero Adam moments; a dead row keeps its moments, as in the
+        reference.  No draw is made where the reference returns early (nothing dead, nothing alive, no room), so the
+        generator advances exactly as the reference's does.  `steps` is unchanged; the float16 feature copy stays
+        bitwise raw.half().
+
+        Native calls (f3dgs_mcmc_plan, _relocate, _add) and ONE host read, the number of dead rows, besides what
+        torch.multinomial itself does.  Deterministic for equal state and generator state: the draws are made with
+        torch's deterministic algorithms enabled (see _multinomial), so data-parallel replicas stay identical."""
+        from . import _C
+
+        P, r = self.P, self.raw
+        if P == 0:
+            return 0, 0
+        eps = torch.finfo(torch.float32).eps
+        groups = [g[k] for g in (self.raw, self.exp_avg, self.exp_avg_sq) for k in self.NAMES]
+        scratch, n_dead, index, alive_opacity = _C.mcmc_plan(r["opacity"], min_opacity)
+        n_dead = int(n_dead)
+        n_relocated = 0
+        if 0 < n_dead < P:
+            probs = alive_opacity[:P - n_dead]
+            draws = _multinomial(probs / (probs.sum() + eps), n_dead, generator)
+            half = self.feature_dtype == torch.float16 and self.act["semantic_feature"].numel() > 0
+            _C.mcmc_relocate(scratch, index[:n_dead], index[n_dead:][draws], min_opacity, groups,
+                             self.act["semantic_feature"] if half else None)
+            n_relocated = n_dead
+        del index, alive_opacity
+        n_added = min(cap_max, int(1.05 * P)) - P
+        if n_added <= 0:
+            return n_relocated, 0
+        probs = torch.empty(P, 1, device=r["opacity"].device)
+        e = torch.empty(0, device=probs.device)
+        _C.activate(r["opacity"], e, e, e, e, probs, e, e, e)  # torch.sigmoid, bitwise
+        probs = probs.squeeze(-1)
+        src = _multinomial(probs / (probs.sum() + eps), n_added, generator).int()
+        del probs
+        Pn = P + n_added
+        new = [{k: torch.empty((Pn,) + r[k].shape[1:], device=r[k].device) for k in self.NAMES} for _ in range(3)]
+        _C.mcmc_add(scratch, src, min_opacity, groups, [g[k] for g in new for k in self.NAMES])
+        del r, groups, scratch, src
+        self.raw, self.exp_avg, self.exp_avg_sq = new
+        del new
+        self._reset_derived(keep_optimizer_state=True)
+        return n_relocated, n_added
+
+    def inject_noise(self, xyz_lr: float, noise_lr: float = 5e5, generator=None):
+        """3DGS-MCMC's position noise, after every optimizer step: xyz += R diag(s^2) R^T (eps * g * noise_lr * xyz_lr)
+        with eps = torch.randn((P, 3), generator=generator), s = exp(scaling), R the rotation, and the gate
+        g = 1 / (1 + exp(-100 ((1 - opacity) - 0.995))), so only nearly transparent Gaussians move.  One kernel
+        (f3dgs_mcmc_inject_noise), in place, without host sync."""
+        from . import _C
+
+        r = self.raw
+        eps = torch.randn((self.P, 3), generator=generator, device=r["xyz"].device)
+        _C.mcmc_inject_noise(r["xyz"], r["opacity"], r["scaling"], r["rotation"], eps, noise_lr * xyz_lr)
+
+    def add_regularizer_grads(self, opacity_reg: float, scale_reg: float, grads: Optional[Dict[str, torch.Tensor]] = None):
+        """3DGS-MCMC's regularisers opacity_reg * mean(|opacity|) + scale_reg * mean(|scales|) on the activated tensors:
+        adds their gradients, opacity_reg / P to every opacity gradient and scale_reg / (3 P) to every scale gradient
+        (the activations are positive, so d|x|/dx = 1), to `grads` (default: the ViewBatch's).  Call it once per step,
+        after vb.all_reduce() and before step().  The reference adds both terms to the loss of every rendered view, so
+        a step over V views matches it with opacity_reg and scale_reg multiplied by V."""
+        g = grads if grads is not None else self.batch().grads
+        P = self.P
+        if P == 0:
+            return
+        g["opacities"].add_(opacity_reg / P)
+        g["scales"].add_(scale_reg / (3 * P))
+
+
+def _multinomial(probs, n, generator):
+    """torch.multinomial(probs, n, replacement=True, generator=generator), bitwise reproducible: on CUDA its prefix sum
+    over the probabilities is only deterministic with torch's deterministic algorithms on, so they are on for this call
+    (and the caller's setting is restored).  The draws and the generator's advance are those of the plain call."""
+    on, warn_only = torch.are_deterministic_algorithms_enabled(), torch.is_deterministic_algorithms_warn_only_enabled()
+    torch.use_deterministic_algorithms(True, warn_only=True)
+    try:
+        return torch.multinomial(probs, n, replacement=True, generator=generator)
+    finally:
+        torch.use_deterministic_algorithms(on, warn_only=warn_only)
 
 
 def expon_lr(step, lr_init, lr_final, lr_delay_steps=0, lr_delay_mult=1.0, max_steps=1000000):

@@ -720,6 +720,53 @@ int f3dgs_densify_apply(int P, int M, int C, const char* scratch, const int32_t 
                         const f3dgs_gaussian_fields src[3], const f3dgs_gaussian_fields dst[3], void* cuda_stream);
 int f3dgs_reset_opacity(int P, float* raw_opacity, float* exp_avg, float* exp_avg_sq, float ceiling, void* cuda_stream);
 
+/* ---- fixed-budget densification: 3DGS-MCMC (Kheradmand et al., NeurIPS 2024; the official code's relocate_gs,
+ * add_new_gs and position noise, gsplat's MCMCStrategy) ------------------------------------------------------------
+ * Fields as for f3dgs_densify_apply: fields[0] the raw parameters, [1] exp_avg, [2] exp_avg_sq.  The caller draws every
+ * index and normal (e.g. torch.multinomial over alive_opacity / its sum, torch.randn), so a run is reproducible from its
+ * generator.  With o = sigmoid(raw_opacity) (bitwise torch.sigmoid) and s = expf(raw_scaling):
+ *   relocation rule  a source drawn c >= 1 times in a call ends as N = min(c + 1, 51) identical Gaussians, each with
+ *                      o' = 1 - (1 - o)^(1/N)                     (evaluated as -expm1(log1p(-o) / N))
+ *                      s' = s * o / D(o', N),  D(x, N) = sum_{j=1..N} C(N,j) (-1)^(j-1) x^j / sqrt(j)
+ *                    in double; o' is then clamped to [min_opacity, 1 - FLT_EPSILON] (s' keeps the unclamped o'), and
+ *                    raw_opacity = logit(o'), raw_scaling = log(s') are rounded to float once.  1 - (1 - o')^N = o
+ *                    before the clamp.
+ *   f3dgs_mcmc_plan      dead = (o <= min_opacity).  Writes index[P] = the dead indices ascending, then the alive ones
+ *                        ascending; alive_opacity[0 .. P - n_dead) = o of the alive ones in that order; *n_dead (device
+ *                        int32).  index and alive_opacity are P elements each; n_dead is the only count to read back.
+ *   f3dgs_mcmc_relocate  in place, P unchanged: for each of the n draws j, row dead[j] takes every raw field of row
+ *                        src[j] with (o', s'), row src[j] takes (o', s'), and src[j]'s exp_avg and exp_avg_sq are zeroed
+ *                        in all seven fields.  The dead rows' moments are left as they are, as the reference does: it
+ *                        resets the optimizer state of the sources only.  semantic_feature_f16 (NULL, or [P,C] IEEE
+ *                        binary16 bits): the dead rows get their new features rounded to nearest even (torch's .half()).
+ *                        Contract: the dead[] are distinct and no src[j] is a dead row; src[] may repeat.
+ *   f3dgs_mcmc_add       out of place: dst has P + n rows.  Row i < P is src row i, except that a drawn row gets
+ *                        (o', s') and zero moments; row P + j is a copy of src row src[j] with (o', s') and zero moments.
+ *                        Every src element is read at most once and every dst element written once.  No dst field may
+ *                        overlap a src field, src[] or the scratch.
+ *   An index outside [0, P) in dead[] or src[] makes relocate and add write nothing to the caller's buffers (checked on
+ *   the device before the first write).  0 <= n <= P.  scratch: f3dgs_mcmc_scratch_bytes(P) bytes of device memory,
+ *   256-byte aligned, shared by the three calls (not kept between them).
+ *   f3dgs_mcmc_inject_noise  xyz[P,3] += R diag(s^2) R^T (eps * g * scale), g = 1 / (1 + exp(-100 ((1 - o) - 0.995))),
+ *                        R the rotation of the normalised quaternion (w, x, y, z), eps [P,3] the caller's normals;
+ *                        computed in double and rounded once.  The reference's scale is noise_lr * xyz_lr with
+ *                        noise_lr = 5e5, applied after every optimizer step.
+ * All calls are stream-ordered without host sync and bitwise deterministic.  3 P (3 (P + n) for add, 4 P for the
+ * noise) must not exceed INT_MAX; scale and
+ * min_opacity must be finite.  f3dgs_mcmc_scratch_bytes returns 0 for P <= 0, and 0 with f3dgs_last_error() set if the
+ * size query fails. */
+size_t f3dgs_mcmc_scratch_bytes(int P);
+int f3dgs_mcmc_plan(int P, const float* raw_opacity, float min_opacity, char* scratch, int32_t* n_dead, int32_t* index,
+                    float* alive_opacity, void* cuda_stream);
+int f3dgs_mcmc_relocate(int P, int M, int C, int n, const int32_t* dead, const int32_t* src, float min_opacity,
+                        const f3dgs_gaussian_fields fields[3], uint16_t* semantic_feature_f16, char* scratch,
+                        void* cuda_stream);
+int f3dgs_mcmc_add(int P, int M, int C, int n, const int32_t* src, float min_opacity,
+                   const f3dgs_gaussian_fields src_fields[3], const f3dgs_gaussian_fields dst_fields[3], char* scratch,
+                   void* cuda_stream);
+int f3dgs_mcmc_inject_noise(int P, float* xyz, const float* raw_opacity, const float* raw_scaling,
+                            const float* raw_rotation, const float* eps, float scale, void* cuda_stream);
+
 /* ---- markVisible: reference rasterizer_impl.cu:141-153 (checkFrustum :54-66) --------------
  * present[i] = (view-space z of means3D[i] > 0.2).  `present` is P bytes (0/1). */
 int f3dgs_mark_visible(int P, const float* means3D, const float* viewmatrix,
