@@ -1508,6 +1508,67 @@ int f3dgs_mcmc_inject_noise(int P, float* xyz, const float* raw_opacity, const f
                                              (cudaStream_t)cuda_stream));
 }
 
+size_t f3dgs_filter3d_scratch_bytes(int P) { return P > 0 ? kFilter3dScratchBytes : 0; }
+
+int f3dgs_filter3d_compute(int P, int V, const float* means3D, const float* viewmatrices, const float* intrinsics,
+                           float* filter, int32_t* n_seen, char* scratch, void* cuda_stream) {
+    const Api api(__func__);
+    if (P < 0 || 3 * (long long)P > INT_MAX || V < 1 || 16 * (long long)V > INT_MAX)
+        return api.invalid("bad sizes (0 <= 3 P <= INT_MAX, 1 <= 16 V <= INT_MAX)");
+    if (P == 0) return 0;
+    if (!means3D || !viewmatrices || !intrinsics || !filter || !n_seen || !scratch) return api.invalid("NULL pointer");
+    const size_t b = (size_t)P * 4;
+    const Range r[6] = {{filter, b}, {n_seen, 4}, {scratch, kFilter3dScratchBytes}, {means3D, 3 * b},
+                        {viewmatrices, (size_t)V * 64}, {intrinsics, (size_t)V * 16}};
+    if (any_overlap(r, 3)) return api.invalid("filter, n_seen, scratch and the inputs overlap");
+    return api.cuda(launch_filter3d_compute(P, V, means3D, viewmatrices, intrinsics, filter, n_seen, scratch,
+                                            (cudaStream_t)cuda_stream));
+}
+
+int f3dgs_filter3d_apply(int P, const float* opacity, const float* scales, const float* filter, float* opacity_out,
+                         float* scales_out, void* cuda_stream) {
+    const Api api(__func__);
+    if (P < 0 || 3 * (long long)P > INT_MAX) return api.invalid("bad sizes (0 <= 3 P <= INT_MAX)");
+    if (P == 0) return 0;
+    if (!opacity || !scales || !filter || !opacity_out || !scales_out) return api.invalid("NULL pointer");
+    const size_t b = (size_t)P * 4;
+    const Range r[5] = {{opacity_out, b}, {scales_out, 3 * b}, {opacity, b}, {scales, 3 * b}, {filter, b}};
+    if (any_overlap(r, 2)) return api.invalid("opacity_out, scales_out and the inputs overlap");
+    return api.cuda(launch_filter3d_apply(P, opacity, scales, filter, opacity_out, scales_out,
+                                          (cudaStream_t)cuda_stream));
+}
+
+int f3dgs_filter3d_apply_backward(int P, const float* opacity, const float* scales, const float* filter,
+                                  const float* dL_dopacity_f, const float* dL_dscales_f, float* dL_dopacity,
+                                  float* dL_dscales, void* cuda_stream) {
+    const Api api(__func__);
+    if (P < 0 || 3 * (long long)P > INT_MAX) return api.invalid("bad sizes (0 <= 3 P <= INT_MAX)");
+    if (P == 0) return 0;
+    if (!opacity || !scales || !filter || !dL_dopacity_f || !dL_dscales_f || !dL_dopacity || !dL_dscales)
+        return api.invalid("NULL pointer");
+    const size_t b = (size_t)P * 4;
+    // an output that is exactly its own upstream gradient is computed in place: that input's range is then the output's
+    const Range r[7] = {{dL_dopacity, b}, {dL_dscales, 3 * b}, {opacity, b}, {scales, 3 * b}, {filter, b},
+                        {dL_dopacity_f == dL_dopacity ? nullptr : dL_dopacity_f, b},
+                        {dL_dscales_f == dL_dscales ? nullptr : dL_dscales_f, 3 * b}};
+    if (any_overlap(r, 2)) return api.invalid("an output overlaps an input or the other output (other than in place)");
+    return api.cuda(launch_filter3d_apply_backward(P, opacity, scales, filter, dL_dopacity_f, dL_dscales_f, dL_dopacity,
+                                                   dL_dscales, (cudaStream_t)cuda_stream));
+}
+
+int f3dgs_reset_opacity_filter3d(int P, float* raw_opacity, const float* raw_scaling, const float* filter,
+                                 float* exp_avg, float* exp_avg_sq, float ceiling, void* cuda_stream) {
+    const Api api(__func__);
+    if (P < 0 || 3 * (long long)P > INT_MAX) return api.invalid("bad sizes (0 <= 3 P <= INT_MAX)");
+    if (P == 0) return 0;
+    if (!raw_opacity || !raw_scaling || !filter || !exp_avg || !exp_avg_sq) return api.invalid("NULL pointer");
+    const size_t b = (size_t)P * 4;
+    const Range r[5] = {{raw_opacity, b}, {exp_avg, b}, {exp_avg_sq, b}, {raw_scaling, 3 * b}, {filter, b}};
+    if (any_overlap(r, 3)) return api.invalid("raw_opacity, exp_avg, exp_avg_sq and the inputs overlap");
+    return api.cuda(launch_reset_opacity_filter3d(P, raw_opacity, raw_scaling, filter, exp_avg, exp_avg_sq, ceiling,
+                                                  (cudaStream_t)cuda_stream));
+}
+
 int f3dgs_activate(int P, int M, const float* raw_opacity, const float* raw_scaling, const float* raw_rotation,
                    const float* features_dc, const float* features_rest, float* opacity, float* scales, float* rotations,
                    float* shs, void* cuda_stream) {

@@ -186,6 +186,20 @@ cudaError_t launch_mcmc_add(int P, int M, int C, int n, const int32_t* src, floa
 cudaError_t launch_mcmc_inject_noise(int P, float* xyz, const float* raw_opacity, const float* raw_scaling,
                                      const float* raw_rotation, const float* eps, float scale, cudaStream_t s);
 
+// ---- filter3d.cu: Mip-Splatting's 3D smoothing filter (include/f3dgs_b200.h: f3dgs_filter3d_*).  scratch is
+// kFilter3dScratchBytes of device memory (the max seen depth)
+constexpr size_t kFilter3dScratchBytes = 256;
+cudaError_t launch_filter3d_compute(int P, int V, const float* means3D, const float* viewmatrices,
+                                    const float* intrinsics, float* filter, int32_t* n_seen, char* scratch,
+                                    cudaStream_t s);
+cudaError_t launch_filter3d_apply(int P, const float* opacity, const float* scales, const float* filter,
+                                  float* opacity_out, float* scales_out, cudaStream_t s);
+cudaError_t launch_filter3d_apply_backward(int P, const float* opacity, const float* scales, const float* filter,
+                                           const float* dL_dopacity_f, const float* dL_dscales_f, float* dL_dopacity,
+                                           float* dL_dscales, cudaStream_t s);
+cudaError_t launch_reset_opacity_filter3d(int P, float* raw_opacity, const float* raw_scaling, const float* filter,
+                                          float* exp_avg, float* exp_avg_sq, float ceiling, cudaStream_t s);
+
 // ---- optimizer.cu: activation prologue and fused Adam step (include/f3dgs_b200.h: f3dgs_activate / f3dgs_adam_step)
 cudaError_t launch_activate(int P, int M, const float* raw_opacity, const float* raw_scaling, const float* raw_rotation,
                             const float* features_dc, const float* features_rest, float* opacity, float* scales,

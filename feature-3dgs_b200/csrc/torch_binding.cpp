@@ -1128,6 +1128,112 @@ void mcmcInjectNoise(torch::Tensor xyz, const torch::Tensor& raw_opacity, const 
              "f3dgs_mcmc_inject_noise");
 }
 
+// ---- 3D smoothing filter, Mip-Splatting (f3dgs_filter3d_compute / _apply / _apply_backward,
+// f3dgs_reset_opacity_filter3d)
+namespace {
+// An optional output of `numel` float32 elements shaped like `like`: the caller's tensor, or a new one
+torch::Tensor output_or_new(const c10::optional<torch::Tensor>& t, const torch::Tensor& like, const char* name) {
+    if (!t.has_value() || !t->defined()) return torch::empty_like(like, torch::MemoryFormat::Contiguous);
+    in_place(*t, like.device(), like.numel(), name);
+    return *t;
+}
+}  // namespace
+
+// means3D [P,3], viewmatrices [V,4,4] (or [V,16]), intrinsics [V,4] = (fx, fy, W, H) -> (filter [P,1], n_seen device
+// int32[1])
+std::tuple<torch::Tensor, torch::Tensor> filter3dCompute(const torch::Tensor& means3D, const torch::Tensor& viewmatrices,
+                                                         const torch::Tensor& intrinsics) {
+    TORCH_CHECK(means3D.is_cuda(), "means3D must be a CUDA tensor (this build has no CPU path)");
+    TORCH_CHECK(means3D.dim() == 2 && means3D.size(1) == 3 && means3D.size(0) <= INT32_MAX / 3,
+                "means3D must be [P,3], 3 P < 2^31");
+    const auto dev = means3D.device();
+    const c10::cuda::CUDAGuard guard(dev);
+    const int64_t P = means3D.size(0), V = intrinsics.dim() == 2 ? intrinsics.size(0) : -1;
+    TORCH_CHECK(V >= 1 && intrinsics.size(1) == 4 && viewmatrices.numel() == 16 * V,
+                "filter3d_compute: intrinsics must be [V,4] and viewmatrices [V,4,4] with V >= 1");
+    auto m = input(means3D, dev, "means3D"), vm = input(viewmatrices, dev, "viewmatrices");
+    auto in = input(intrinsics, dev, "intrinsics");
+    torch::Tensor filter = torch::empty({P, 1}, m.options());
+    torch::Tensor n_seen = torch::zeros({1}, m.options().dtype(torch::kInt32));
+    if (P == 0) return std::make_tuple(filter, n_seen);
+    torch::Tensor scratch = torch::empty({(int64_t)f3dgs_filter3d_scratch_bytes((int)P)}, m.options().dtype(torch::kUInt8));
+    cudaStream_t stream = c10::cuda::getCurrentCUDAStream().stream();
+    check_rc(f3dgs_filter3d_compute((int)P, (int)V, fptr(m), fptr(vm), fptr(in), filter.data_ptr<float>(),
+                                    n_seen.data_ptr<int32_t>(), scratch_ptr(scratch), (void*)stream),
+             "f3dgs_filter3d_compute");
+    return std::make_tuple(filter, n_seen);
+}
+
+// opacity [P,1], scales [P,3], filter [P,1] -> (opacity_out, scales_out), written into the given tensors or new ones
+std::tuple<torch::Tensor, torch::Tensor> filter3dApply(const torch::Tensor& opacity, const torch::Tensor& scales,
+                                                       const torch::Tensor& filter,
+                                                       const c10::optional<torch::Tensor>& opacity_out,
+                                                       const c10::optional<torch::Tensor>& scales_out) {
+    TORCH_CHECK(scales.is_cuda(), "scales must be a CUDA tensor (this build has no CPU path)");
+    TORCH_CHECK(scales.dim() == 2 && scales.size(1) == 3 && scales.size(0) <= INT32_MAX / 3,
+                "scales must be [P,3], 3 P < 2^31");
+    const auto dev = scales.device();
+    const c10::cuda::CUDAGuard guard(dev);
+    const int64_t P = scales.size(0);
+    TORCH_CHECK(opacity.numel() == P && filter.numel() == P, "filter3d_apply: opacity and filter must have P elements");
+    auto o = input(opacity, dev, "opacity"), s = input(scales, dev, "scales"), f = input(filter, dev, "filter");
+    torch::Tensor oo = output_or_new(opacity_out, o, "opacity_out"), so = output_or_new(scales_out, s, "scales_out");
+    cudaStream_t stream = c10::cuda::getCurrentCUDAStream().stream();
+    check_rc(f3dgs_filter3d_apply((int)P, fptr(o), fptr(s), fptr(f), P ? oo.data_ptr<float>() : nullptr,
+                                  P ? so.data_ptr<float>() : nullptr, (void*)stream),
+             "f3dgs_filter3d_apply");
+    return std::make_tuple(oo, so);
+}
+
+// -> (dL_dopacity, dL_dscales) from the gradients of the filtered tensors; written into the given tensors (which may be
+// the filtered gradients themselves: in place) or new ones
+std::tuple<torch::Tensor, torch::Tensor> filter3dApplyBackward(const torch::Tensor& opacity, const torch::Tensor& scales,
+                                                               const torch::Tensor& filter,
+                                                               const torch::Tensor& dL_dopacity_f,
+                                                               const torch::Tensor& dL_dscales_f,
+                                                               const c10::optional<torch::Tensor>& dL_dopacity,
+                                                               const c10::optional<torch::Tensor>& dL_dscales) {
+    TORCH_CHECK(scales.is_cuda(), "scales must be a CUDA tensor (this build has no CPU path)");
+    TORCH_CHECK(scales.dim() == 2 && scales.size(1) == 3 && scales.size(0) <= INT32_MAX / 3,
+                "scales must be [P,3], 3 P < 2^31");
+    const auto dev = scales.device();
+    const c10::cuda::CUDAGuard guard(dev);
+    const int64_t P = scales.size(0);
+    TORCH_CHECK(opacity.numel() == P && filter.numel() == P && dL_dopacity_f.numel() == P &&
+                    dL_dscales_f.numel() == 3 * P,
+                "filter3d_apply_backward: opacity, filter and dL_dopacity_f must have P elements, dL_dscales_f 3 P");
+    auto o = input(opacity, dev, "opacity"), s = input(scales, dev, "scales"), f = input(filter, dev, "filter");
+    // an in-place output must be the caller's contiguous tensor itself, so the upstream gradients are not copied then
+    const bool go_in_place = dL_dopacity.has_value() && dL_dopacity->defined() && dL_dopacity->is_same(dL_dopacity_f);
+    const bool gs_in_place = dL_dscales.has_value() && dL_dscales->defined() && dL_dscales->is_same(dL_dscales_f);
+    auto gof = go_in_place ? dL_dopacity_f : input(dL_dopacity_f, dev, "dL_dopacity_f");
+    auto gsf = gs_in_place ? dL_dscales_f : input(dL_dscales_f, dev, "dL_dscales_f");
+    torch::Tensor go = output_or_new(dL_dopacity, gof, "dL_dopacity"), gs = output_or_new(dL_dscales, gsf, "dL_dscales");
+    cudaStream_t stream = c10::cuda::getCurrentCUDAStream().stream();
+    check_rc(f3dgs_filter3d_apply_backward((int)P, fptr(o), fptr(s), fptr(f), fptr(gof), fptr(gsf),
+                                           P ? go.data_ptr<float>() : nullptr, P ? gs.data_ptr<float>() : nullptr,
+                                           (void*)stream),
+             "f3dgs_filter3d_apply_backward");
+    return std::make_tuple(go, gs);
+}
+
+void resetOpacityFilter3d(torch::Tensor raw_opacity, const torch::Tensor& raw_scaling, const torch::Tensor& filter,
+                          torch::Tensor exp_avg, torch::Tensor exp_avg_sq, double ceiling) {
+    TORCH_CHECK(raw_opacity.is_cuda(), "parameters must be CUDA tensors (this build has no CPU path)");
+    TORCH_CHECK(raw_opacity.numel() <= INT32_MAX / 3, "reset_opacity_filter3d: 3 P must be below 2^31");
+    const auto dev = raw_opacity.device();
+    const c10::cuda::CUDAGuard guard(dev);
+    const int64_t P = raw_opacity.numel();
+    auto s = input(raw_scaling, dev, "raw_scaling"), f = input(filter, dev, "filter");
+    TORCH_CHECK(raw_scaling.numel() == 3 * P && filter.numel() == P,
+                "reset_opacity_filter3d: raw_scaling must have 3 P elements and filter P");
+    cudaStream_t stream = c10::cuda::getCurrentCUDAStream().stream();
+    check_rc(f3dgs_reset_opacity_filter3d((int)P, in_place(raw_opacity, dev, P, "raw_opacity"), fptr(s), fptr(f),
+                                          in_place(exp_avg, dev, P, "exp_avg"), in_place(exp_avg_sq, dev, P, "exp_avg_sq"),
+                                          (float)ceiling, (void*)stream),
+             "f3dgs_reset_opacity_filter3d");
+}
+
 // ---- activation prologue + fused optimizer step (f3dgs_activate / f3dgs_adam_step): in-place on the caller's tensors
 void activateParams(const torch::Tensor& raw_opacity, const torch::Tensor& raw_scaling, const torch::Tensor& raw_rotation,
                     const torch::Tensor& f_dc, const torch::Tensor& f_rest, torch::Tensor opacity, torch::Tensor scales,
@@ -1292,6 +1398,15 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
           pybind11::arg("src_fields"), pybind11::arg("dst_fields"));
     m.def("mcmc_inject_noise", &mcmcInjectNoise, pybind11::arg("xyz"), pybind11::arg("raw_opacity"),
           pybind11::arg("raw_scaling"), pybind11::arg("raw_rotation"), pybind11::arg("eps"), pybind11::arg("scale"));
+    m.def("filter3d_compute", &filter3dCompute, pybind11::arg("means3D"), pybind11::arg("viewmatrices"),
+          pybind11::arg("intrinsics"));
+    m.def("filter3d_apply", &filter3dApply, pybind11::arg("opacity"), pybind11::arg("scales"), pybind11::arg("filter"),
+          pybind11::arg("opacity_out") = pybind11::none(), pybind11::arg("scales_out") = pybind11::none());
+    m.def("filter3d_apply_backward", &filter3dApplyBackward, pybind11::arg("opacity"), pybind11::arg("scales"),
+          pybind11::arg("filter"), pybind11::arg("dL_dopacity_f"), pybind11::arg("dL_dscales_f"),
+          pybind11::arg("dL_dopacity") = pybind11::none(), pybind11::arg("dL_dscales") = pybind11::none());
+    m.def("reset_opacity_filter3d", &resetOpacityFilter3d, pybind11::arg("raw_opacity"), pybind11::arg("raw_scaling"),
+          pybind11::arg("filter"), pybind11::arg("exp_avg"), pybind11::arg("exp_avg_sq"), pybind11::arg("ceiling") = 0.01);
     m.def("activate", &activateParams);
     m.def("adam_step", &adamStep, pybind11::arg("kind"), pybind11::arg("param"), pybind11::arg("grad_activated"),
           pybind11::arg("exp_avg"), pybind11::arg("exp_avg_sq"), pybind11::arg("M"), pybind11::arg("lr"),

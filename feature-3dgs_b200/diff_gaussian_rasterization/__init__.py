@@ -44,6 +44,12 @@ Behavioural notes
   * sparse Adam (opt-in): `SparseGaussianAdam(params, lr, eps)` with `.step(visibility, N)` is the upstream
     rasterizer's optimizer of that name: it updates only the Gaussians marked visible (f3dgs_adam_step_masked), without
     bias correction, and leaves the others' parameters and moments untouched.
+  * 3D smoothing filter (opt-in, Mip-Splatting): `compute_3d_filter(means3D, train_settings)` gives every Gaussian a
+    world-space filter size from the highest sampling rate any training camera has at it, and
+    `apply_3d_filter(opacities, scales, filter_3D)` returns the filtered opacities and scales to render with, with a
+    native backward (f3dgs_filter3d_*).  Renders closer than or at a higher resolution than the training views then
+    show no Gaussians smaller than the training views could sample.  `GaussianState.compute_3d_filter` turns it on for
+    training.  By default the opacities and scales are used as they are, as in the reference.
   * `debug=True` keeps the reference semantics: arguments are snapshotted to CPU first and dumped
     to snapshot_fw.dump / snapshot_bw.dump if the native call raises (reference :89-97,:147-155);
     natively it synchronises and checks after every stage.
@@ -64,6 +70,8 @@ except ImportError as exc:  # pragma: no cover - exercised only on a broken inst
         "There is no CPU fallback. Original error: %s" % (exc,)
     ) from exc
 
+from .filter3d import apply_3d_filter, compute_3d_filter  # noqa: E402
+
 __all__ = [
     "GaussianRasterizationSettings",
     "GaussianRasterizer",
@@ -73,6 +81,8 @@ __all__ = [
     "rasterize_gaussians_alpha_invdepth",
     "AlphaInvDepthGaussianRasterizer",
     "SparseGaussianAdam",
+    "compute_3d_filter",
+    "apply_3d_filter",
 ]
 
 

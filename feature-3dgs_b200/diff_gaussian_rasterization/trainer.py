@@ -20,7 +20,11 @@ _opacity, _scaling, _rotation, _semantic_feature`, :47-58) as plain CUDA tensors
   reset_opacity()       :231-234 in one kernel (f3dgs_reset_opacity);
   relocate_and_add()    3DGS-MCMC's fixed-budget densification (relocate_gs + add_new_gs) with the optimizer state
                         carried along (f3dgs_mcmc_plan / _relocate / _add), one host read; inject_noise() and
-                        add_regularizer_grads() its per-step position noise and regulariser gradients.
+                        add_regularizer_grads() its per-step position noise and regulariser gradients;
+  compute_3d_filter()   Mip-Splatting's 3D smoothing filter (opt-in, f3dgs_filter3d_*): once on, activate() hands the
+                        rasterizer the filtered opacity and scales, step() takes the filter's backward first,
+                        densification recomputes it, reset_opacity() resets the filtered opacity, and baked_raw()
+                        gives the parameters with the filter folded in, for export.
 
 Float16 feature fields: with feature_dtype=torch.float16 the rasterizer reads a float16 working copy
 act["semantic_feature"] of the float32 master raw["semantic_feature"], so every view renders a float16 map and the feature
@@ -62,6 +66,8 @@ class GaussianState:
             raise ValueError(f"feature_dtype must be torch.float32 or torch.float16, got {feature_dtype}")
         self.betas, self.eps, self.percent_dense = betas, eps, percent_dense
         self.feature_dtype = feature_dtype
+        self.filter_3d: Optional[torch.Tensor] = None  # [P,1] while the 3D filter is on
+        self._filter_cameras = None
         self._reset_derived()
 
     @classmethod
@@ -123,13 +129,22 @@ class GaussianState:
                         rotations=torch.empty(P, 4, device=dev), shs=torch.empty(P, self.M, 3, device=dev),
                         semantic_feature=sf if self.feature_dtype == torch.float32 else sf.to(self.feature_dtype))
         self._batch: Optional[ViewBatch] = None
+        self._unfiltered = None  # the unfiltered opacity [P,1] and scales [P,3] while the 3D filter is on
 
     def activate(self):
+        """The activated tensors the rasterizer reads (self.act), from the raw parameters.  With the 3D filter on,
+        act["opacities"] and act["scales"] hold the filtered values (apply_3d_filter) and the unfiltered ones are kept
+        for step()."""
         from . import _C
 
         a, r = self.act, self.raw
-        _C.activate(r["opacity"], r["scaling"], r["rotation"], r["f_dc"], r["f_rest"], a["opacities"], a["scales"],
-                    a["rotations"], a["shs"])
+        if self.filter_3d is None:
+            _C.activate(r["opacity"], r["scaling"], r["rotation"], r["f_dc"], r["f_rest"], a["opacities"], a["scales"],
+                        a["rotations"], a["shs"])
+            return a
+        o, s = self._unfiltered
+        _C.activate(r["opacity"], r["scaling"], r["rotation"], r["f_dc"], r["f_rest"], o, s, a["rotations"], a["shs"])
+        _C.filter3d_apply(o, s, self.filter_3d, a["opacities"], a["scales"])
         return a
 
     def batch(self) -> ViewBatch:
@@ -145,10 +160,16 @@ class GaussianState:
         visible: None for the dense step, or a bool [P] CUDA mask (ViewBatch.visible() after all_reduce()) for the sparse
         Adam step (f3dgs_adam_step_masked): only the marked Gaussians' raw parameters, moments and float16 feature copy
         change, bitwise as in the dense step; the others stay exactly as they are, so momentum no longer moves Gaussians
-        that no view of the step saw.  Bias correction still uses each group's step count, which advances every step."""
+        that no view of the step saw.  Bias correction still uses each group's step count, which advances every step.
+
+        With the 3D filter on, `grads` holds the gradients w.r.t. the filtered opacity and scales; they are turned into
+        those w.r.t. the unfiltered ones of the last activate(), in place (f3dgs_filter3d_apply_backward), first."""
         from . import _C
 
         g = grads if grads is not None else self.batch().grads
+        if self.filter_3d is not None:
+            o, s = self._unfiltered
+            _C.filter3d_apply_backward(o, s, self.filter_3d, g["opacities"], g["scales"], g["opacities"], g["scales"])
         for name in self.NAMES:
             p = self.raw[name]
             if p.numel() == 0:
@@ -209,13 +230,56 @@ class GaussianState:
         self.raw, self.exp_avg, self.exp_avg_sq = new
         del new
         self._reset_derived(keep_optimizer_state=True)
+        if self.filter_3d is not None:
+            self.compute_3d_filter()
         return self.P
 
     def reset_opacity(self):
-        """scene/gaussian_model.py:231-234: clamp opacity to <= 0.01 and clear its optimizer state, in place."""
+        """scene/gaussian_model.py:231-234: clamp opacity to <= 0.01 and clear its optimizer state, in place.  With the
+        3D filter on, Mip-Splatting's reset: the filtered opacity is clamped and the raw opacity set to match it
+        (f3dgs_reset_opacity_filter3d)."""
         from . import _C
 
-        _C.reset_opacity(self.raw["opacity"], self.exp_avg["opacity"], self.exp_avg_sq["opacity"])
+        r = self.raw
+        if self.filter_3d is not None:
+            _C.reset_opacity_filter3d(r["opacity"], r["scaling"], self.filter_3d, self.exp_avg["opacity"],
+                                      self.exp_avg_sq["opacity"])
+            return
+        _C.reset_opacity(r["opacity"], self.exp_avg["opacity"], self.exp_avg_sq["opacity"])
+
+    # ---------------------------------------------------------------------------------------------- 3D filter
+    def compute_3d_filter(self, cameras=None):
+        """Mip-Splatting's compute_3D_filter (filter3d.compute_3d_filter) on the current means: cameras is a sequence of
+        GaussianRasterizationSettings, the training views.  It turns the 3D filter on; the camera tensors are kept, so
+        that a call without cameras recomputes from the same views (Mip-Splatting recomputes every 100 iterations, and
+        densify_and_prune / relocate_and_add recompute it for the new cloud themselves).  One host read.  Raises
+        ValueError when no Gaussian is seen (or, without cameras, when the filter has never been computed)."""
+        from .filter3d import camera_tensors, compute_from_tensors
+
+        if cameras is not None:
+            self._filter_cameras = camera_tensors(cameras)
+        elif self._filter_cameras is None:
+            raise ValueError("compute_3d_filter: no cameras given and none kept from an earlier call")
+        self.filter_3d = compute_from_tensors(self.raw["xyz"], *self._filter_cameras)
+        dev, P = self.raw["xyz"].device, self.P
+        if self._unfiltered is None or self._unfiltered[0].shape[0] != P:
+            self._unfiltered = (torch.empty(P, 1, device=dev), torch.empty(P, 3, device=dev))
+        return self.filter_3d
+
+    def baked_raw(self) -> Dict[str, torch.Tensor]:
+        """The raw parameters with the 3D filter folded in, Mip-Splatting's save_fused_ply: opacity =
+        inverse_sigmoid(filtered opacity) and scaling = log(filtered scales); the other fields are self.raw's.  A model
+        saved from it (io.save_ply) renders correctly in any 3DGS renderer without the filter.  With the filter off,
+        the raw parameters as they are."""
+        from . import _C
+
+        if self.filter_3d is None:
+            return dict(self.raw)
+        r, P, dev, e = self.raw, self.P, self.raw["xyz"].device, torch.empty(0, device=self.raw["xyz"].device)
+        o, s = torch.empty(P, 1, device=dev), torch.empty(P, 3, device=dev)
+        _C.activate(r["opacity"], r["scaling"], e, e, e, o, s, e, e)
+        o, s = _C.filter3d_apply(o, s, self.filter_3d)
+        return dict(r, opacity=inverse_sigmoid(o), scaling=torch.log(s))
 
     # ---------------------------------------------------------------------------------------------- 3DGS-MCMC
     def relocate_and_add(self, cap_max: int, min_opacity: float = 0.005, generator=None):
@@ -255,6 +319,8 @@ class GaussianState:
         del index, alive_opacity
         n_added = min(cap_max, int(1.05 * P)) - P
         if n_added <= 0:
+            if n_relocated and self.filter_3d is not None:
+                self.compute_3d_filter()
             return n_relocated, 0
         probs = torch.empty(P, 1, device=r["opacity"].device)
         e = torch.empty(0, device=probs.device)
@@ -269,6 +335,8 @@ class GaussianState:
         self.raw, self.exp_avg, self.exp_avg_sq = new
         del new
         self._reset_derived(keep_optimizer_state=True)
+        if self.filter_3d is not None:
+            self.compute_3d_filter()
         return n_relocated, n_added
 
     def inject_noise(self, xyz_lr: float, noise_lr: float = 5e5, generator=None):
@@ -287,7 +355,11 @@ class GaussianState:
         adds their gradients, opacity_reg / P to every opacity gradient and scale_reg / (3 P) to every scale gradient
         (the activations are positive, so d|x|/dx = 1), to `grads` (default: the ViewBatch's).  Call it once per step,
         after vb.all_reduce() and before step().  The reference adds both terms to the loss of every rendered view, so
-        a step over V views matches it with opacity_reg and scale_reg multiplied by V."""
+        a step over V views matches it with opacity_reg and scale_reg multiplied by V.  Raises ValueError while the 3D
+        filter is on: the terms are defined on the unfiltered tensors, but the gradients then belong to filtered ones."""
+        if self.filter_3d is not None:
+            raise ValueError("add_regularizer_grads: not defined with the 3D filter on (the gradients are those of the "
+                             "filtered opacity and scales)")
         g = grads if grads is not None else self.batch().grads
         P = self.P
         if P == 0:

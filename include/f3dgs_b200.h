@@ -767,6 +767,50 @@ int f3dgs_mcmc_add(int P, int M, int C, int n, const int32_t* src, float min_opa
 int f3dgs_mcmc_inject_noise(int P, float* xyz, const float* raw_opacity, const float* raw_scaling,
                             const float* raw_rotation, const float* eps, float scale, void* cuda_stream);
 
+/* ---- 3D smoothing filter: Mip-Splatting (Yu et al., CVPR 2024; the official scene/gaussian_model.py
+ * compute_3D_filter, get_opacity_with_3D_filter, get_scaling_with_3D_filter, reset_opacity) ------------------------
+ * Each Gaussian gets a world-space filter size f from the highest sampling rate any training camera has at it; the
+ * rasterizer is then called with the filtered opacity and scales, so that no Gaussian is smaller than the training
+ * views could sample (no needles when rendering closer or at a higher resolution than any training view).
+ *   f3dgs_filter3d_compute  viewmatrices [V,16] (the rasterizer's viewmatrix, W2C^T), intrinsics [V,4] = (fx, fy, W, H)
+ *                        with fx = W / (2 tanfovx), fy = H / (2 tanfovy) as floats.  For Gaussian i with mean x and
+ *                        camera v: c = x @ vm[:3,:3] + vm[3,:3] (fixed fma order), zc = max(c.z, 0.001),
+ *                        px = c.x / zc * fx + W / 2, py = c.y / zc * fy + H / 2; v sees i when c.z > 0.2 and
+ *                        -0.15 W <= px <= 1.15 W and -0.15 H <= py <= 1.15 H (margins rounded from double once).
+ *                        d_i = min(100000, min over the cameras that see i of zc); a Gaussian no camera sees takes the
+ *                        max d of the seen ones.  filter[i] = d_i * (1 / focal) * sqrt(0.2) in float, focal = max fx
+ *                        (fx only, as the official code).  *n_seen (device int32) = the number of seen Gaussians; when
+ *                        it is 0 the filter is meaningless (the official code fails there).  Bitwise deterministic and
+ *                        independent of the camera order.  scratch: f3dgs_filter3d_scratch_bytes(P) bytes of device
+ *                        memory (returns 0 for P <= 0); filter, n_seen and scratch must not overlap each other or an
+ *                        input.  V >= 1.
+ *   f3dgs_filter3d_apply  o, s the activated opacity [P] and scales [P,3]: opacity_out = o * coef and
+ *                        scales_out = sqrt(s^2 + f^2) per axis, with det1 = s0^2 s1^2 s2^2, det2 = prod (s_k^2 + f^2)
+ *                        and coef = sqrt(det1 / det2): bitwise the official float32 torch formula (torch's .prod(dim=1)
+ *                        order, no contraction).  The outputs must not overlap each other or an input.
+ *   f3dgs_filter3d_apply_backward  the gradients w.r.t. (o, s) from those w.r.t. (opacity_out, scales_out):
+ *                        dL_dopacity = dL_dopacity_f * coef,
+ *                        dL_dscales_k = dL_dscales_f_k * s_k / s_f_k + dL_dopacity_f * o_f * f^2 / (s_k s_f_k^2),
+ *                        the second term 0 where o_f == 0 (an underflowed det1 or s_k == 0 gives no NaN).  The filter
+ *                        gets no gradient.  dL_dopacity may be dL_dopacity_f and dL_dscales may be dL_dscales_f (in
+ *                        place); no other overlap is allowed.
+ *   f3dgs_reset_opacity_filter3d  f3dgs_reset_opacity of the filtered opacity, in place: with o = sigmoid(raw_opacity),
+ *                        s = expf(raw_scaling) and coef as above, raw_opacity <- logit(min(o * coef, ceiling) / coef)
+ *                        (NaN propagates); exp_avg and exp_avg_sq of the opacity [P] are zeroed.  Where coef == 0 the
+ *                        official formula is 0 / 0; there the unfiltered reset's logit(min(o, ceiling)) is written.
+ *                        raw_opacity, exp_avg and exp_avg_sq must not overlap each other, raw_scaling or filter.
+ * All calls are stream-ordered without host sync.  0 <= 3 P <= INT_MAX; P == 0 is a no-op. */
+size_t f3dgs_filter3d_scratch_bytes(int P);
+int f3dgs_filter3d_compute(int P, int V, const float* means3D, const float* viewmatrices, const float* intrinsics,
+                           float* filter, int32_t* n_seen, char* scratch, void* cuda_stream);
+int f3dgs_filter3d_apply(int P, const float* opacity, const float* scales, const float* filter, float* opacity_out,
+                         float* scales_out, void* cuda_stream);
+int f3dgs_filter3d_apply_backward(int P, const float* opacity, const float* scales, const float* filter,
+                                  const float* dL_dopacity_f, const float* dL_dscales_f, float* dL_dopacity,
+                                  float* dL_dscales, void* cuda_stream);
+int f3dgs_reset_opacity_filter3d(int P, float* raw_opacity, const float* raw_scaling, const float* filter,
+                                 float* exp_avg, float* exp_avg_sq, float ceiling, void* cuda_stream);
+
 /* ---- markVisible: reference rasterizer_impl.cu:141-153 (checkFrustum :54-66) --------------
  * present[i] = (view-space z of means3D[i] > 0.2).  `present` is P bytes (0/1). */
 int f3dgs_mark_visible(int P, const float* means3D, const float* viewmatrix,
