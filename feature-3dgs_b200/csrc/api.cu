@@ -1043,6 +1043,25 @@ int f3dgs_lift_features_accum_f16(int P, int R, int C, int width, int height, ch
                      reinterpret_cast<const __half*>(feature_map), feature_sum, weight_sum, cuda_stream);
 }
 
+int f3dgs_gaussian_scores_accum(int P, int R, int width, int height, char* geom_buffer, char* binning_buffer,
+                                char* image_buffer, float* weight_sum, float* max_weight, int64_t* pixel_count,
+                                void* cuda_stream) {
+    const Api api(__func__);
+    if (P < 0 || R < 0 || width <= 0 || height <= 0)
+        return api.invalid("bad sizes (P >= 0, R >= 0, width, height >= 1)");
+    if (P == 0 || R == 0) return 0;  // nothing is blended (a forward with R == 0 may leave an empty binning buffer)
+    if (!geom_buffer || !binning_buffer || !image_buffer) return api.invalid("missing forward buffers");
+    if (!weight_sum || !max_weight || !pixel_count)
+        return api.invalid("NULL pointer (weight_sum, max_weight or pixel_count)");
+    const Range outs[] = {{weight_sum, (size_t)P * 4}, {max_weight, (size_t)P * 4}, {pixel_count, (size_t)P * 8}};
+    for (const Range& r : outs)
+        if (overlaps(r, outs)) return api.invalid("weight_sum, max_weight and pixel_count must not overlap");
+    const ViewParams vp = make_view(P, 0, 0, 0, width, height, 0.f, 0.f, 1.f, nullptr, nullptr, nullptr);
+    return api.cuda(launch_gaussian_scores(vp, forward_buffers(vp, R, geom_buffer, binning_buffer, image_buffer),
+                                           weight_sum, max_weight, pixel_count, (cudaStream_t)cuda_stream),
+                    "score launch");
+}
+
 }  // extern "C"
 
 namespace {
@@ -1355,6 +1374,15 @@ int f3dgs_densify_plan(int P, const float* grad_accum, const float* denom, const
         return api.invalid("counts overlaps scratch");
     return api.cuda(launch_densify_plan(P, grad_accum, denom, raw_opacity, raw_scaling, max_grad, dense_scale,
                                         min_opacity, max_world_scale, scratch, counts, (cudaStream_t)cuda_stream));
+}
+
+int f3dgs_prune_plan(int P, const uint8_t* keep, char* scratch, int32_t* counts, void* cuda_stream) {
+    const Api api(__func__);
+    if (P < 0 || 3 * (long long)P > INT_MAX) return api.invalid("bad sizes (0 <= 3 P <= INT_MAX)");
+    if (!counts || (P > 0 && (!keep || !scratch))) return api.invalid("NULL pointer");
+    const Range flags{scratch, densify_scratch_fixed_bytes(P)};
+    if (overlaps(flags, {{keep, (size_t)P}, {counts, 16}})) return api.invalid("keep or counts overlaps scratch");
+    return api.cuda(launch_prune_plan(P, keep, scratch, counts, (cudaStream_t)cuda_stream));
 }
 
 int f3dgs_densify_apply(int P, int M, int C, const char* scratch, const int32_t counts[4], const float* normals,

@@ -15,6 +15,10 @@
 //   LIFT           feature lifting: the EMIT lists, and instead of the 10 gradient terms the one value w = alpha*T per pair,
 //       reduced into weight_sum[P] through the same tile; no upstream gradient or background is read.  feature_bwd.cu
 //       then forms sum_p w * map[:, p] over the lists with the teacher map in place of dL/dfeature_map.
+//   SCORE          per-Gaussian scores of the view: LIFT's weights without the lists, three values per pair (w, 1, w)
+//       parked in the same tile; the flush adds the first row sum into weight_sum, the second (a count of 0/1 floats,
+//       at most 32 per row, exact) into pixel_count with an integer atomic, and takes the third row's max into
+//       max_weight with an integer atomicMax on the float bits (w > 0, so the bits order as the floats do).
 //   FEAT           the feature term of dL/dalpha (opt-in, after EMIT and feature_bwd): feature_dot (feature_bwd.cu) has
 //       replaced each list entry's weights by the pair dot products d_ip = f_i . dL/dF_p; this walk repeats EMIT's, so a
 //       pair's entry is the one EMIT wrote for it, and runs the colour term's scalar recurrence on d (no background:
@@ -65,11 +69,14 @@ struct BwdArgs {
     float* weight_sum;    // LIFT: [P] += sum over the view's pixels of w
     const float* dL_dalpha;     // PLANES: [H,W] gA
     const float* dL_dinvdepth;  // PLANES: [H,W] gI
+    float* max_weight;          // SCORE: [P] = max(max_weight, the largest w of the view)
+    int64_t* pixel_count;       // SCORE: [P] += the number of pixels the Gaussian blended into
 };
 
 // GEOM: geometric gradients; EMIT: and the feature lists; LIFT: the feature lists and the per-Gaussian weight sums;
-// FEAT: the feature term of the geometric gradients, from the lists' pair dot products
-enum class BwdMode { GEOM, EMIT, LIFT, FEAT };
+// FEAT: the feature term of the geometric gradients, from the lists' pair dot products; SCORE: LIFT's weights without
+// the lists, reduced into the per-Gaussian weight sum, largest weight and blended-pixel count
+enum class BwdMode { GEOM, EMIT, LIFT, FEAT, SCORE };
 // Namespace-scope constants: as constexpr locals of the kernel they changed the register allocation of the EMIT
 // instantiation, which is meant to stay instruction-for-instruction what it was before lifting existed.
 template <BwdMode M>
@@ -77,7 +84,9 @@ constexpr bool kLift = M == BwdMode::LIFT;
 template <BwdMode M>
 constexpr bool kFeat = M == BwdMode::FEAT;
 template <BwdMode M>
-constexpr int kVals = kLift<M> ? 1 : (kFeat<M> ? 6 : kRedVals);  // values reduced per pair: FEAT has no depth or colour
+constexpr bool kScore = M == BwdMode::SCORE;
+template <BwdMode M>  // values reduced per pair: FEAT has no depth or colour, SCORE reduces w, 1 and w
+constexpr int kVals = kLift<M> ? 1 : (kFeat<M> ? 6 : (kScore<M> ? 3 : kRedVals));
 
 // destination of reduced value v (0..9) of Gaussian gid: reference backward.cu:560-610 (atomicAdd targets)
 __device__ __forceinline__ float* geom_dst(const BwdArgs& args, int v, uint32_t gid) {
@@ -93,10 +102,33 @@ __device__ __forceinline__ float* geom_dst(const BwdArgs& args, int v, uint32_t 
     }
 }
 
+// SCORE: one parked row of Gaussian gid (32 lanes, 0 where the pair did not blend) into its score v: 0 the weight sum,
+// 1 the blended-pixel count, 2 the largest weight
+__device__ __forceinline__ void score_flush_row(const BwdArgs& args, int v, uint32_t gid, const float* r) {
+    float s0 = 0.f, s1 = 0.f, s2 = 0.f, s3 = 0.f, m = 0.f;
+    const float4* row = reinterpret_cast<const float4*>(r);
+#pragma unroll
+    for (int jj = 0; jj < 8; jj++) {
+        const float4 q = row[jj];
+        s0 += q.x;
+        s1 += q.y;
+        s2 += q.z;
+        s3 += q.w;
+        m = fmaxf(m, fmaxf(fmaxf(q.x, q.y), fmaxf(q.z, q.w)));
+    }
+    if (v == 0)
+        red_add_f1(args.weight_sum + gid, (s0 + s1) + (s2 + s3));
+    else if (v == 1)
+        atomicAdd(reinterpret_cast<unsigned long long*>(args.pixel_count + gid),
+                  (unsigned long long)((s0 + s1) + (s2 + s3)));
+    else
+        atomicMax(reinterpret_cast<int*>(args.max_weight + gid), __float_as_int(m));
+}
+
 template <BwdMode MODE, bool PLANES = false>
 __global__ void __launch_bounds__(kBwdThreads, kSlimCtas)
 composite_bwd_kernel(const BwdArgs args) {
-    constexpr bool EMIT = MODE != BwdMode::GEOM;
+    constexpr bool EMIT = MODE != BwdMode::GEOM && MODE != BwdMode::SCORE;
     extern __shared__ __align__(128) unsigned char smem_raw[];
     BwdSmem& sm = *reinterpret_cast<BwdSmem*>(smem_raw);
     RingSlim& ring = sm.ring;
@@ -141,7 +173,9 @@ composite_bwd_kernel(const BwdArgs args) {
         __syncwarp();
         for (int r = lane; r < kVals<MODE> * kRedSlots; r += 32) {
             const int slot = r % kRedSlots, v = r / kRedSlots;
-            if (slot < (int)nslots) {
+            if constexpr (kScore<MODE>) {
+                if (slot < (int)nslots) score_flush_row(args, v, red_gid[slot], red[r]);
+            } else if (slot < (int)nslots) {
                 float s0 = 0.f, s1 = 0.f, s2 = 0.f, s3 = 0.f;
                 const float4* row = reinterpret_cast<const float4*>(red[r]);
 #pragma unroll
@@ -187,7 +221,7 @@ composite_bwd_kernel(const BwdArgs args) {
             p.T = p.T_final;
             p.last_contrib = p.inside ? args.n_contrib[pix] : 0u;
             p.dLp0 = p.dLp1 = p.dLp2 = p.dLd = 0.f;
-            if constexpr (!kLift<MODE> && !kFeat<MODE>) {
+            if constexpr (!kLift<MODE> && !kFeat<MODE> && !kScore<MODE>) {
                 if (p.inside) {
                     p.dLp0 = args.dL_dpix[pix];
                     p.dLp1 = args.dL_dpix[HW + pix];
@@ -237,11 +271,15 @@ composite_bwd_kernel(const BwdArgs args) {
                     float v[kRedVals];
 #pragma unroll
                     for (int i = 0; i < kRedVals; i++) v[i] = 0.f;
-                    if constexpr (kLift<MODE>) {
+                    if constexpr (kLift<MODE> || kScore<MODE>) {
                         if (contrib) {  // the T unwind below, without the gradient terms
                             p.T = p.T * rcp_approx(1.f - alpha);
                             wgt = alpha * p.T;
                             v[0] = wgt;
+                            if constexpr (kScore<MODE>) {
+                                v[1] = 1.f;
+                                v[2] = wgt;
+                            }
                         }
                     } else if constexpr (kFeat<MODE>) {
                         if (contrib) {  // the colour term below with the one channel d_ip and no background
@@ -364,7 +402,7 @@ static cudaError_t alloc_lists(size_t R, size_t tiles, char** mem, InstanceLists
 }
 
 // The geometry kernel in mode MODE over the view's forward buffers; for EMIT and LIFT also the instance lists and then
-// feature_bwd over them, reducing sum_p w * scale * map[:, p] into dst.  `a` brings the mode's outputs.  With features
+// feature_bwd over them (SCORE has neither), reducing sum_p w * scale * map[:, p] into dst.  `a` brings the mode's outputs.  With features
 // (EMIT only), feature_dot then turns the lists' weights into pair dot products and the FEAT walk adds the feature term
 // to the geometric gradients; the lists are freed after it.
 template <BwdMode MODE, typename TG, bool PLANES = false>
@@ -372,8 +410,9 @@ static cudaError_t run_bwd(BwdArgs a, const ViewParams& vp, const ForwardBuffers
                            float* dst, cudaStream_t s, const FeatureRows& feat = {}) {
     a.pa = producer_args(vp, fb.ranges, fb.point_list, fb.rec, fb.n_contrib, fb.counters + kCounterBwdGeom);
     a.final_T = fb.final_T; a.n_contrib = fb.n_contrib;
+    constexpr bool lists = MODE == BwdMode::EMIT || MODE == BwdMode::LIFT;
     char* mem = nullptr;
-    if (MODE != BwdMode::GEOM) {
+    if (lists) {
         const cudaError_t e = alloc_lists((size_t)fb.R, (size_t)a.pa.num_tiles, &mem, a.lists, s);
         if (e != cudaSuccess) return e;
     }
@@ -381,7 +420,8 @@ static cudaError_t run_bwd(BwdArgs a, const ViewParams& vp, const ForwardBuffers
     int num_sms = 0;
     cudaError_t e = device_sms<composite_bwd_kernel<BwdMode::GEOM>, composite_bwd_kernel<BwdMode::EMIT>,
                                composite_bwd_kernel<BwdMode::LIFT>, composite_bwd_kernel<BwdMode::FEAT>,
-                               composite_bwd_kernel<BwdMode::GEOM, true>, composite_bwd_kernel<BwdMode::EMIT, true>>(
+                               composite_bwd_kernel<BwdMode::GEOM, true>, composite_bwd_kernel<BwdMode::EMIT, true>,
+                               composite_bwd_kernel<BwdMode::SCORE>>(
         num_sms, sizeof(BwdSmem), kBwdThreads, kSlimCtas);
     const int grid = min(a.pa.num_tiles, kSlimCtas * num_sms);
     auto walk = [&](void (*kernel)(BwdArgs)) {
@@ -392,7 +432,7 @@ static cudaError_t run_bwd(BwdArgs a, const ViewParams& vp, const ForwardBuffers
         return cudaGetLastError();
     };
     if (e == cudaSuccess) e = walk(composite_bwd_kernel<MODE, PLANES>);
-    if (MODE != BwdMode::GEOM) {
+    if (lists) {
         if (e == cudaSuccess) e = launch_feature_bwd(vp, fb.ranges, a.lists, map, scale, dst, fb.counters, s);
         if (MODE == BwdMode::EMIT && feat.rows) {
             if (e == cudaSuccess) e = launch_feature_dot(vp, fb.ranges, a.lists, feat, map, scale, fb.counters, s);
@@ -426,6 +466,13 @@ cudaError_t launch_feature_lift(const ViewParams& vp, const ForwardBuffers& fb, 
     BwdArgs a{};
     a.weight_sum = weight_sum;
     return run_bwd<BwdMode::LIFT>(a, vp, fb, map, 1.f, feature_sum, s);
+}
+
+cudaError_t launch_gaussian_scores(const ViewParams& vp, const ForwardBuffers& fb, float* weight_sum, float* max_weight,
+                                   int64_t* pixel_count, cudaStream_t s) {
+    BwdArgs a{};
+    a.weight_sum = weight_sum; a.max_weight = max_weight; a.pixel_count = pixel_count;
+    return run_bwd<BwdMode::SCORE, float>(a, vp, fb, nullptr, 1.f, nullptr, s);
 }
 
 template cudaError_t launch_composite_bwd(const ViewParams&, const ForwardBuffers&, const float*, const float*,

@@ -20,6 +20,8 @@
 //      and its two child rows (moments: zeros for the new rows).  Child xyz = R(q) (z * std) + parent xyz with z the
 //      caller's normals, child scaling as above.  Every new row is written exactly once; no atomics, so the result is
 //      bitwise reproducible.
+// A prune from the caller's mask (f3dgs_prune_plan) replaces step 1 by prune_classify_kernel, flags {keep != 0, 0, 0, 0};
+// the scan and apply_kernel are the same, with totals {A, 0, 0, 0} and no normals.
 #include <cub/cub.cuh>
 
 #include <cmath>
@@ -40,6 +42,19 @@ cudaError_t scan_bytes(int P, size_t* bytes) {
     *bytes = 0;
     return cub::DeviceScan::ExclusiveScan(nullptr, *bytes, (int4*)nullptr, (int4*)nullptr, Add4(), make_int4(0, 0, 0, 0),
                                           P + 1);
+}
+
+// step 2 after a classify launch: the flags scanned in place, their totals copied to counts
+cudaError_t scan_flags(int P, char* scratch, int32_t* counts, cudaStream_t s) {
+    cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) return e;
+    size_t sb = 0;
+    if ((e = scan_bytes(P, &sb)) != cudaSuccess) return e;
+    int4* flags = reinterpret_cast<int4*>(scratch);
+    if ((e = cub::DeviceScan::ExclusiveScan(scratch + densify_scratch_fixed_bytes(P), sb, flags, flags, Add4(),
+                                            make_int4(0, 0, 0, 0), P + 1, s)) != cudaSuccess)
+        return e;
+    return cudaMemcpyAsync(counts, flags + P, 4 * sizeof(int32_t), cudaMemcpyDeviceToDevice, s);
 }
 
 // torch's max over a dimension: NaN propagates
@@ -83,6 +98,12 @@ __global__ void __launch_bounds__(256) classify_kernel(const __grid_constant__ C
         child = !(transparent || cmax > a.max_world_scale);
     }
     a.flags[i] = make_int4(!split && !prune, clone && !prune, child, split);
+}
+
+__global__ void __launch_bounds__(256) prune_classify_kernel(int P, const uint8_t* __restrict__ keep, int4* flags) {
+    const long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x;
+    if (i > P) return;
+    flags[i] = make_int4(i < P && keep[i] != 0, 0, 0, 0);
 }
 
 // One segment per (group, field): group 0 the raw parameters, 1 exp_avg, 2 exp_avg_sq; fields in
@@ -204,9 +225,6 @@ cudaError_t launch_densify_plan(int P, const float* grad_accum, const float* den
                                 const float* raw_scaling, float max_grad, float dense_scale, float min_opacity,
                                 float max_world_scale, char* scratch, int32_t* counts, cudaStream_t s) {
     if (P == 0) return cudaMemsetAsync(counts, 0, 4 * sizeof(int32_t), s);
-    size_t sb = 0;
-    cudaError_t e = scan_bytes(P, &sb);
-    if (e != cudaSuccess) return e;
     int4* flags = reinterpret_cast<int4*>(scratch);
     ClassifyArgs c;
     c.P = P; c.grad_accum = grad_accum; c.denom = denom; c.raw_opacity = raw_opacity; c.raw_scaling = raw_scaling;
@@ -214,11 +232,14 @@ cudaError_t launch_densify_plan(int P, const float* grad_accum, const float* den
     c.split_inv = densify_split_inv(); c.flags = flags;
     classify_kernel<<<blocks_for((long long)P + 1), 256, 0, s>>>(c);
     g_launches++;
-    if ((e = cudaGetLastError()) != cudaSuccess) return e;
-    if ((e = cub::DeviceScan::ExclusiveScan(scratch + densify_scratch_fixed_bytes(P), sb, flags, flags, Add4(),
-                                            make_int4(0, 0, 0, 0), P + 1, s)) != cudaSuccess)
-        return e;
-    return cudaMemcpyAsync(counts, flags + P, 4 * sizeof(int32_t), cudaMemcpyDeviceToDevice, s);
+    return scan_flags(P, scratch, counts, s);
+}
+
+cudaError_t launch_prune_plan(int P, const uint8_t* keep, char* scratch, int32_t* counts, cudaStream_t s) {
+    if (P == 0) return cudaMemsetAsync(counts, 0, 4 * sizeof(int32_t), s);
+    prune_classify_kernel<<<blocks_for((long long)P + 1), 256, 0, s>>>(P, keep, reinterpret_cast<int4*>(scratch));
+    g_launches++;
+    return scan_flags(P, scratch, counts, s);
 }
 
 cudaError_t launch_densify_apply(int P, int M, int C, const char* scratch, const int32_t counts[4], const float* normals,

@@ -100,6 +100,11 @@ cudaError_t launch_composite_bwd(const ViewParams& vp, const ForwardBuffers& fb,
 template <typename TF>
 cudaError_t launch_feature_lift(const ViewParams& vp, const ForwardBuffers& fb, const TF* map, float* feature_sum,
                                 float* weight_sum, cudaStream_t s);
+// Per-Gaussian scores, R > 0, from the same walk without lists or feature kernel: weight_sum[P] += sum_p w,
+// max_weight[P] = max(max_weight, max_p w) (max_weight >= 0, compared as float bits), pixel_count[P] += the number of
+// pixels the Gaussian blended into.  Allocates nothing
+cudaError_t launch_gaussian_scores(const ViewParams& vp, const ForwardBuffers& fb, float* weight_sum, float* max_weight,
+                                   int64_t* pixel_count, cudaStream_t s);
 
 // ---- feature_head.cu (a float16 map or target gives the result of the float32 one upcast exactly; a float16 gradient
 // is half_rn(out_scale * the float32 one), out_scale not read for a float gradient)
@@ -166,6 +171,8 @@ size_t densify_scratch_fixed_bytes(int P);
 cudaError_t launch_densify_plan(int P, const float* grad_accum, const float* denom, const float* raw_opacity,
                                 const float* raw_scaling, float max_grad, float dense_scale, float min_opacity,
                                 float max_world_scale, char* scratch, int32_t* counts, cudaStream_t s);
+// prune from a mask: the plan of launch_densify_apply that keeps row i iff keep[i] != 0, counts {A, 0, 0, 0}
+cudaError_t launch_prune_plan(int P, const uint8_t* keep, char* scratch, int32_t* counts, cudaStream_t s);
 cudaError_t launch_densify_apply(int P, int M, int C, const char* scratch, const int32_t counts[4], const float* normals,
                                  const float* const src[21], float* const dst[21], cudaStream_t s);
 cudaError_t launch_reset_opacity(int P, float* raw_opacity, float* exp_avg, float* exp_avg_sq, float ceiling,

@@ -603,6 +603,35 @@ void liftFeaturesAccum(const torch::Tensor& geomBuffer, const int R, const torch
                     });
 }
 
+// Per-Gaussian scores (f3dgs_gaussian_scores_accum): the buffers and R of a forward of this view at width x height;
+// weight_sum [P] float32, max_weight [P] float32 (>= 0) and pixel_count [P] int64, contiguous, accumulated in place
+void gaussianScoresAccum(const torch::Tensor& geomBuffer, const int R, const torch::Tensor& binningBuffer,
+                         const torch::Tensor& imageBuffer, const int64_t width, const int64_t height,
+                         torch::Tensor weight_sum, torch::Tensor max_weight, torch::Tensor pixel_count) {
+    TORCH_CHECK(weight_sum.is_cuda(), "gaussian_scores_accum: weight_sum must be a CUDA tensor");
+    const auto dev = weight_sum.device();
+    const c10::cuda::CUDAGuard guard(dev);
+    TORCH_CHECK(weight_sum.numel() <= INT32_MAX && width <= INT32_MAX && height <= INT32_MAX,
+                "gaussian_scores_accum: sizes too large");
+    const int64_t P = weight_sum.numel();
+    float* ws = in_place(weight_sum, dev, P, "gaussian_scores_accum: weight_sum");
+    float* mw = in_place(max_weight, dev, P, "gaussian_scores_accum: max_weight");
+    TORCH_CHECK(pixel_count.is_cuda() && pixel_count.device() == dev && pixel_count.scalar_type() == torch::kInt64 &&
+                    pixel_count.is_contiguous() && pixel_count.numel() == P,
+                "gaussian_scores_accum: pixel_count must be a contiguous int64 tensor of ", P, " elements on ", dev);
+    for (const torch::Tensor* b : {&geomBuffer, &binningBuffer, &imageBuffer})
+        TORCH_CHECK(b->device() == dev && b->scalar_type() == torch::kByte && b->is_contiguous(),
+                    "gaussian_scores_accum: the forward buffers must be contiguous uint8 tensors on ", dev);
+    if (P == 0) return;
+    cudaStream_t stream = c10::cuda::getCurrentCUDAStream().stream();
+    check_rc(f3dgs_gaussian_scores_accum((int)P, R, (int)width, (int)height,
+                                         reinterpret_cast<char*>(geomBuffer.data_ptr()),
+                                         reinterpret_cast<char*>(binningBuffer.data_ptr()),
+                                         reinterpret_cast<char*>(imageBuffer.data_ptr()), ws, mw,
+                                         pixel_count.data_ptr<int64_t>(), (void*)stream),
+             "f3dgs_gaussian_scores_accum");
+}
+
 torch::Tensor markVisible(torch::Tensor& means3D, torch::Tensor& viewmatrix, torch::Tensor& projmatrix) {
     TORCH_CHECK(means3D.is_cuda(), "means3D must be a CUDA tensor (this build has no CPU path)");
     const c10::cuda::CUDAGuard guard(means3D.device());
@@ -966,6 +995,26 @@ std::tuple<torch::Tensor, torch::Tensor> densifyPlan(const torch::Tensor& grad_a
                                 scratch.numel() ? reinterpret_cast<char*>(scratch.data_ptr()) : nullptr,
                                 counts.data_ptr<int32_t>(), (void*)stream),
              "f3dgs_densify_plan");
+    return std::make_tuple(scratch, counts);
+}
+
+// keep: bool or uint8 [P] CUDA mask -> (scratch, counts): counts = device int32[4] {rows kept, 0, 0, 0}, the plan of a
+// densify_apply that keeps the marked rows
+std::tuple<torch::Tensor, torch::Tensor> prunePlan(const torch::Tensor& keep) {
+    TORCH_CHECK(keep.is_cuda(), "prune_plan: keep must be a CUDA tensor (this build has no CPU path)");
+    TORCH_CHECK(keep.dim() == 1 && (keep.scalar_type() == torch::kBool || keep.scalar_type() == torch::kByte),
+                "prune_plan: keep must be a bool or uint8 tensor [P]");
+    TORCH_CHECK(keep.size(0) <= INT32_MAX / 3, "prune_plan: 3 P must be below 2^31");
+    const c10::cuda::CUDAGuard guard(keep.device());
+    auto k = keep.contiguous();
+    const int P = (int)k.size(0);
+    torch::Tensor scratch = scratch_tensor(f3dgs_densify_scratch_bytes(P), "f3dgs_densify_scratch_bytes", k);
+    torch::Tensor counts = torch::empty({4}, k.options().dtype(torch::kInt32));
+    cudaStream_t stream = c10::cuda::getCurrentCUDAStream().stream();
+    check_rc(f3dgs_prune_plan(P, P ? reinterpret_cast<const uint8_t*>(k.data_ptr()) : nullptr,
+                              scratch.numel() ? reinterpret_cast<char*>(scratch.data_ptr()) : nullptr,
+                              counts.data_ptr<int32_t>(), (void*)stream),
+             "f3dgs_prune_plan");
     return std::make_tuple(scratch, counts);
 }
 
@@ -1373,6 +1422,9 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     m.def("lift_features_accum", &liftFeaturesAccum, pybind11::arg("geomBuffer"), pybind11::arg("R"),
           pybind11::arg("binningBuffer"), pybind11::arg("imageBuffer"), pybind11::arg("feature_map"),
           pybind11::arg("feature_sum"), pybind11::arg("weight_sum"));
+    m.def("gaussian_scores_accum", &gaussianScoresAccum, pybind11::arg("geomBuffer"), pybind11::arg("R"),
+          pybind11::arg("binningBuffer"), pybind11::arg("imageBuffer"), pybind11::arg("width"), pybind11::arg("height"),
+          pybind11::arg("weight_sum"), pybind11::arg("max_weight"), pybind11::arg("pixel_count"));
     m.def("feature_resize_fwd", &featureResizeFwd);
     m.def("feature_resize_bwd", &featureResizeBwd, pybind11::arg("dout"), pybind11::arg("H"), pybind11::arg("W"),
           pybind11::arg("dtype") = torch::kFloat32, pybind11::arg("out_scale") = 1.0);
@@ -1389,6 +1441,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     m.def("knn_mean_dist", &knnMeanDist);
     m.def("densify_plan", &densifyPlan);
     m.def("densify_apply", &densifyApply);
+    m.def("prune_plan", &prunePlan, pybind11::arg("keep"));
     m.def("reset_opacity", &resetOpacity, pybind11::arg("raw_opacity"), pybind11::arg("exp_avg"),
           pybind11::arg("exp_avg_sq"), pybind11::arg("ceiling") = 0.01);
     m.def("mcmc_plan", &mcmcPlan, pybind11::arg("raw_opacity"), pybind11::arg("min_opacity"));

@@ -50,6 +50,10 @@ Behavioural notes
     native backward (f3dgs_filter3d_*).  Renders closer than or at a higher resolution than the training views then
     show no Gaussians smaller than the training views could sample.  `GaussianState.compute_3d_filter` turns it on for
     training.  By default the opacities and scales are used as they are, as in the reference.
+  * compaction (opt-in): `GaussianScores(means3D, opacities, scales, rotations)` accumulates each Gaussian's blend-weight
+    sum, largest blend weight and blended-pixel count over views (f3dgs_gaussian_scores_accum), and
+    `GaussianState.prune(keep)` / `prune_by_importance(scores, ratio)` remove rows with the Adam state carried along
+    (f3dgs_prune_plan + f3dgs_densify_apply).
   * `debug=True` keeps the reference semantics: arguments are snapshotted to CPU first and dumped
     to snapshot_fw.dump / snapshot_bw.dump if the native call raises (reference :89-97,:147-155);
     natively it synchronises and checks after every stage.
@@ -71,6 +75,7 @@ except ImportError as exc:  # pragma: no cover - exercised only on a broken inst
     ) from exc
 
 from .filter3d import apply_3d_filter, compute_3d_filter  # noqa: E402
+from .scores import GaussianScores  # noqa: E402
 
 __all__ = [
     "GaussianRasterizationSettings",
@@ -83,6 +88,7 @@ __all__ = [
     "SparseGaussianAdam",
     "compute_3d_filter",
     "apply_3d_filter",
+    "GaussianScores",
 ]
 
 

@@ -295,6 +295,18 @@ def decoded_feature_l1_loss(feature_map: torch.Tensor, gt: torch.Tensor, weight:
     return _DecodedL1.apply(feature_map, weight, bias, gt, float(loss_weight))
 
 
+def _weights_forward(g, colors, e, antialiasing, rs, H, W):
+    """The forward whose buffers FeatureLift and GaussianScores walk: C = 0 with zero colors_precomp (no SH work), at
+    H x W, antialiased or not.  g holds means3D, opacities, scales, rotations and cov3D (e, empty, where absent).
+    -> (R, geom, binning, img)"""
+    fwd = _C().rasterize_gaussians_antialiased if antialiasing else _C().rasterize_gaussians
+    R, _, _, _, _, geom, binning, img = fwd(
+        rs.bg, g["means3D"], colors, e, g["opacities"], g["scales"], g["rotations"], rs.scale_modifier, g["cov3D"],
+        rs.viewmatrix, rs.projmatrix, rs.tanfovx, rs.tanfovy, H, W, e, rs.sh_degree, rs.campos, rs.prefiltered,
+        rs.debug)
+    return R, geom, binning, img
+
+
 class FeatureLift:
     """Lift 2-D feature maps onto Gaussians without training (blend-weighted back-projection over views):
 
@@ -370,13 +382,8 @@ class FeatureLift:
             raise ValueError(f"FeatureLift.add: feature_map must be on {self.flat.device}, got {feature_map.device}")
         if self.P == 0:
             return
-        g, e = self._geom, self._empty
         with torch.no_grad():
-            fwd = _C().rasterize_gaussians_antialiased if self.antialiasing else _C().rasterize_gaussians
-            R, _, _, _, _, geom, binning, img = fwd(
-                rs.bg, g["means3D"], self._colors, e, g["opacities"], g["scales"], g["rotations"], rs.scale_modifier,
-                g["cov3D"], rs.viewmatrix, rs.projmatrix, rs.tanfovx, rs.tanfovy, H, W, e, rs.sh_degree, rs.campos,
-                rs.prefiltered, rs.debug)
+            R, geom, binning, img = _weights_forward(self._geom, self._colors, self._empty, self.antialiasing, rs, H, W)
             _C().lift_features_accum(geom, R, binning, img, feature_map, self.feature_sum, self.weight_sum)
 
     def result(self, min_weight: float = 0.0, dtype=torch.float32):

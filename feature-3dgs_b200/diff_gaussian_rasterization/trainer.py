@@ -24,7 +24,10 @@ _opacity, _scaling, _rotation, _semantic_feature`, :47-58) as plain CUDA tensors
   compute_3d_filter()   Mip-Splatting's 3D smoothing filter (opt-in, f3dgs_filter3d_*): once on, activate() hands the
                         rasterizer the filtered opacity and scales, step() takes the filter's backward first,
                         densification recomputes it, reset_opacity() resets the filtered opacity, and baked_raw()
-                        gives the parameters with the filter folded in, for export.
+                        gives the parameters with the filter folded in, for export;
+  prune(keep)           removes the rows a mask drops, with the optimizer state carried along (f3dgs_prune_plan /
+                        f3dgs_densify_apply), one host read; prune_by_importance() drops the lowest blend-weight
+                        scores (scores.GaussianScores), LightGaussian's rule.
 
 Float16 feature fields: with feature_dtype=torch.float16 the rasterizer reads a float16 working copy
 act["semantic_feature"] of the float32 master raw["semantic_feature"], so every view renders a float16 map and the feature
@@ -233,6 +236,69 @@ class GaussianState:
         if self.filter_3d is not None:
             self.compute_3d_filter()
         return self.P
+
+    def prune(self, keep: torch.Tensor) -> int:
+        """Keep the rows where `keep` (a bool or uint8 CUDA tensor [P], any nonzero byte keeps) is set; returns the new P.
+
+        Every raw field and its exp_avg and exp_avg_sq become bitwise t[keep], in order; `steps` is unchanged, the
+        float16 feature copy is bitwise raw.half() and max_radii2D is compacted with the rows, as the reference's
+        prune_points does.  The ViewBatch is rebuilt, and the 3D filter, when on, is recomputed for the new means (its
+        own host read).  Per-row statistics the caller keeps (densification statistics, scores) are the caller's to
+        index with `keep`.
+
+        Two native calls (csrc/densify.cu: the mask plan, then densify_apply's compaction) and ONE host read, the
+        number of rows kept, which sizes the new tensors."""
+        from . import _C
+
+        P = self.P
+        dev = self.raw["xyz"].device
+        if not isinstance(keep, torch.Tensor) or keep.dtype not in (torch.bool, torch.uint8) or keep.shape != (P,):
+            raise ValueError(f"prune: keep must be a bool or uint8 tensor [{P}], got "
+                             f"{getattr(keep, 'dtype', type(keep))} {tuple(getattr(keep, 'shape', ()))}")
+        if keep.device != dev:
+            raise ValueError(f"prune: keep must be on {dev}, got {keep.device}")
+        keep = keep if keep.dtype == torch.bool else keep != 0
+        scratch, counts = _C.prune_plan(keep)
+        # max_radii2D's new position: the rank among the kept rows, slot A for the dropped ones
+        rank = torch.cumsum(keep, 0, dtype=torch.int64) - 1
+        A = int(counts[0])
+        radii = torch.empty(A + 1, device=dev).scatter_(0, torch.where(keep, rank, A), self.max_radii2D)[:A]
+        del rank
+        groups = (self.raw, self.exp_avg, self.exp_avg_sq)
+        r = self.raw
+        new = [{k: torch.empty((A,) + r[k].shape[1:], device=dev) for k in self.NAMES} for _ in groups]
+        _C.densify_apply(scratch, [A, 0, 0, 0], torch.empty(0, device=dev), [g[k] for g in groups for k in self.NAMES],
+                         [g[k] for g in new for k in self.NAMES])
+        del r, groups, scratch
+        self.raw, self.exp_avg, self.exp_avg_sq = new
+        del new
+        self._reset_derived(keep_optimizer_state=True)
+        self.max_radii2D = radii
+        if self.filter_3d is not None:
+            self.compute_3d_filter()
+        return self.P
+
+    def prune_by_importance(self, scores, prune_ratio: float, volume_power: float = 0.1) -> int:
+        """LightGaussian's global-significance pruning: remove exactly n = int(prune_ratio * P) rows, those with the
+        smallest v = scores.weight_sum * V ** volume_power, V the product of the three activated scales (the filtered
+        ones with the 3D filter on).  Ties go to the lower index first (a stable sort).  LightGaussian also divides V by
+        a reference volume; a constant factor does not change the ranking, so it is left out.  `scores` is a
+        scores.GaussianScores of this state's Gaussians (all_reduce'd first when data-parallel).  Returns the new P; one
+        host read, prune's.
+
+        RadSplat's rule needs no method: state.prune(scores.max_weight >= tau).  Mini-Splatting's importance is
+        volume_power=0."""
+        P = self.P
+        if not 0.0 <= prune_ratio <= 1.0:
+            raise ValueError(f"prune_by_importance: prune_ratio must be in [0, 1], got {prune_ratio}")
+        w = scores.weight_sum
+        if w.shape != (P,):
+            raise ValueError(f"prune_by_importance: the scores are of {w.shape[0]} Gaussians, the state has {P}")
+        n = int(prune_ratio * P)
+        v = w * self.activate()["scales"].prod(dim=1) ** volume_power
+        keep = torch.ones(P, dtype=torch.bool, device=w.device)
+        keep[torch.sort(v, stable=True).indices[:n]] = False
+        return self.prune(keep)
 
     def reset_opacity(self):
         """scene/gaussian_model.py:231-234: clamp opacity to <= 0.01 and clear its optimizer state, in place.  With the

@@ -490,6 +490,24 @@ int f3dgs_lift_features_accum_f16(int P, int R, int C, int width, int height, ch
                                   char* image_buffer, const uint16_t* feature_map, float* feature_sum,
                                   float* weight_sum, void* cuda_stream);
 
+/* ---- per-Gaussian blend-weight scores (no reference counterpart): the statistics compaction methods prune by -------
+ * The buffers and R are those of an f3dgs_forward / _f16 / _antialiased / _alpha_invdepth of this view at width x height
+ * (any C of that forward, 0 included; an antialiased forward scores the antialiased model).  ACCUMULATES:
+ *   weight_sum[P]  += sum_p w_ip                          (LightGaussian's global significance without its volume
+ *                                                          factor, Mini-Splatting's importance)
+ *   max_weight[P]   = max(max_weight, max_p w_ip)         (RadSplat's score)
+ *   pixel_count[P] += #{p : Gaussian i blended into p}    (LightGaussian's hit count), exact
+ * w_ip = the blend weight alpha*T of Gaussian i at pixel p (the backward's unwound T, the value
+ * f3dgs_lift_features_accum's weight_sum adds: equal to the forward's blend weight to a few ulp); the pairs counted are
+ * exactly those the forward composited.  max_weight must hold values >= 0 (zeros to start): it is updated with an
+ * integer max on the float bits, so it is exact and does not depend on the order of the views.  weight_sum equals
+ * f3dgs_lift_features_accum's on the same buffers up to the order of the float reductions.  The three outputs must not
+ * overlap.  P == 0 or R == 0 launches nothing.  The call allocates nothing: one kernel, the geometry walk of the
+ * backward without its instance lists or feature kernel, and no upstream gradient is read. */
+int f3dgs_gaussian_scores_accum(int P, int R, int width, int height, char* geom_buffer, char* binning_buffer,
+                                char* image_buffer, float* weight_sum, float* max_weight, int64_t* pixel_count,
+                                void* cuda_stream);
+
 /* ==== callers either side of the rasterizer (SURVEY.md section 8 f): additive entry points ======================= */
 
 /* ---- post-raster feature head: reference train.py:98-104 ---------------------------------------------------------
@@ -707,6 +725,12 @@ int f3dgs_knn_mean_dist(int P, const float* points, float* out, char* scratch, v
  * Both calls are stream-ordered without host sync and bitwise deterministic.  3 P must not exceed INT_MAX.
  * f3dgs_densify_scratch_bytes returns 0 for P <= 0, and 0 with f3dgs_last_error() set if the size query fails.
  *
+ * Pruning from a caller's mask is the same pair with another plan:
+ *   f3dgs_prune_plan     keeps row i iff keep[i] != 0 (keep: P bytes of device memory, any nonzero byte keeps) and
+ *                        writes counts = {A, 0, 0, 0}, A the rows kept.  scratch is f3dgs_densify_scratch_bytes(P)
+ *                        bytes; keep and counts must not overlap its flags.  f3dgs_densify_apply with the host copy
+ *                        of counts and normals == NULL then writes the A kept rows of every field, in order, bitwise.
+ *
  * f3dgs_reset_opacity: raw_opacity <- logf(x / (1 - x)) with x = min(sigmoid(raw_opacity), ceiling) (NaN propagates, as
  * torch.minimum), in place; exp_avg and exp_avg_sq of the opacity [P] are zeroed.  The reference's ceiling is 0.01f. */
 typedef struct f3dgs_gaussian_fields {
@@ -718,6 +742,7 @@ int f3dgs_densify_plan(int P, const float* grad_accum, const float* denom, const
                        float max_world_scale, char* scratch, int32_t* counts, void* cuda_stream);
 int f3dgs_densify_apply(int P, int M, int C, const char* scratch, const int32_t counts[4], const float* normals,
                         const f3dgs_gaussian_fields src[3], const f3dgs_gaussian_fields dst[3], void* cuda_stream);
+int f3dgs_prune_plan(int P, const uint8_t* keep, char* scratch, int32_t* counts, void* cuda_stream);
 int f3dgs_reset_opacity(int P, float* raw_opacity, float* exp_avg, float* exp_avg_sq, float ceiling, void* cuda_stream);
 
 /* ---- fixed-budget densification: 3DGS-MCMC (Kheradmand et al., NeurIPS 2024; the official code's relocate_gs,
