@@ -533,6 +533,10 @@ struct ViewBackward {
     bool antialiasing = false;
     // the gradients of the forward's opacity and inverse-depth planes, added to dL/dalpha and dL/dz by the composite
     const float *dL_dalpha = nullptr, *dL_dinvdepth = nullptr;
+    // the _absgrad entries: AbsGS's per-view statistic [P,3] (required there; the accumulating entry zeroes it), and the
+    // accumulating entry's grad_accum_abs [P] (optional)
+    bool absgrad = false;
+    float *dL_dmean2D_abs = nullptr, *grad_accum_abs = nullptr;
 };
 
 // The features of a _feature_geometry, _antialiased or _alpha_invdepth entry, after the checks every such entry makes
@@ -579,6 +583,8 @@ int backward(const Api& api, ViewBackward b) {
     if (b.scales && (!b.rotations || !b.dL_dscale || !b.dL_drot))
         return api.invalid("scales given but rotations/dL_dscale/dL_drot NULL");
     if ((b.grad_accum == nullptr) != (b.denom == nullptr)) return api.invalid("grad_accum and denom go together");
+    if (b.absgrad && !b.dL_dmean2D_abs) return api.invalid("NULL dL_dmean2D_abs");
+    if (b.grad_accum_abs && !b.grad_accum) return api.invalid("grad_accum_abs needs grad_accum and denom");
     if (b.map.f16) {
         if (!std::isfinite(b.map.scale) || b.map.scale == 0.f)
             return api.invalid("dL_dfeaturepix_scale must be finite and nonzero");
@@ -595,8 +601,10 @@ int backward(const Api& api, ViewBackward b) {
                           {b.dL_dsh, (size_t)b.M * 3 * p4}, {b.dL_dscale, 3 * p4}, {b.dL_drot, 4 * p4},
                           {b.dL_dz, p4}, {b.grad_accum, p4}, {b.denom, p4},
                           {b.dL_dcamera, F3DGS_CAMERA_GRAD_FLOATS * sizeof(float)}, {b.scratch, scratch_bytes},
-                          {b.dL_dmean2D_out, 3 * p4}};
-    const Range &opacity = outs[2], &camera = outs[13];
+                          {b.dL_dmean2D_out, 3 * p4}, {b.dL_dmean2D_abs, 3 * p4}, {b.grad_accum_abs, p4}};
+    const Range &opacity = outs[2], &camera = outs[13], &mean2D_abs = outs[16], &accum_abs = outs[17];
+    if (overlaps(accum_abs, outs)) return api.invalid("grad_accum_abs overlaps another output");
+    if (overlaps(mean2D_abs, outs)) return api.invalid("dL_dmean2D_abs overlaps another output");
     if (overlaps(camera, outs)) return api.invalid("dL_dcamera overlaps another output");
     if (overlaps({b.feat.rows, (size_t)P * C * (b.feat.f16 ? 2 : 4)}, outs))
         return api.invalid("semantic_feature overlaps an output");
@@ -605,6 +613,7 @@ int backward(const Api& api, ViewBackward b) {
     if (overlaps({b.dL_dalpha, hw4}, outs) || overlaps({b.dL_dinvdepth, hw4}, outs))
         return api.invalid("dL_dalpha / dL_dinvdepth overlap an output");
     if (b.accumulate) CUDA_TRY(cudaMemsetAsync(b.scratch, 0, scratch_bytes, stream));
+    if (b.accumulate && b.dL_dmean2D_abs) CUDA_TRY(cudaMemsetAsync(b.dL_dmean2D_abs, 0, 3 * p4, stream));
 
     const ViewParams vp = make_view(P, b.D, b.M, C, b.width, b.height, b.tan_fovx, b.tan_fovy, b.scale_modifier,
                                     b.viewmatrix, b.projmatrix, b.cam_pos);
@@ -637,7 +646,8 @@ int backward(const Api& api, ViewBackward b) {
         const auto composite = [&](auto* dL_dfeaturepix) {
             return launch_composite_bwd(vp, fb, b.background, b.dL_dpix, b.dL_depths, dL_dfeaturepix, b.map.scale,
                                         b.dL_dmean2D, b.dL_dconic, dL_dop_eff, b.dL_dcolor, b.dL_dz,
-                                        b.dL_dsemantic_feature, stream, b.feat, b.dL_dalpha, b.dL_dinvdepth);
+                                        b.dL_dsemantic_feature, stream, b.feat, b.dL_dalpha, b.dL_dinvdepth,
+                                        b.dL_dmean2D_abs);
         };
         e = b.map.f16 ? composite(static_cast<const __half*>(b.map.p)) : composite(static_cast<const float*>(b.map.p));
     }
@@ -650,7 +660,8 @@ int backward(const Api& api, ViewBackward b) {
         e = launch_preprocess_bwd(vp, b.means3D, radii, b.shs, clamped, b.scales, b.rotations, cov3d, b.dL_dmean2D,
                                   b.dL_dconic, b.dL_dmean3D, b.dL_dcolor, b.dL_dcov3D, b.dL_dsh, b.dL_dscale, b.dL_drot,
                                   b.dL_dz, stream, b.accumulate, b.grad_accum, b.denom, b.dL_dcamera, b.antialiasing,
-                                  reinterpret_cast<const SplatRec*>(b.geom_buffer + gl.rec), dL_dop_eff, b.dL_dopacity);
+                                  reinterpret_cast<const SplatRec*>(b.geom_buffer + gl.rec), dL_dop_eff, b.dL_dopacity,
+                                  b.dL_dmean2D_abs, b.grad_accum_abs);
     }
     if (e == cudaErrorMemoryAllocation)
         return api.fail(F3DGS_ERR_ALLOC, std::string("cudaMallocAsync for the camera-gradient partials failed: ") +
@@ -999,6 +1010,70 @@ int f3dgs_backward_accum_alpha_invdepth(
     b.antialiasing = antialiasing != 0;
     b.dL_dalpha = dL_dalpha;
     b.dL_dinvdepth = dL_dinvdepth;
+    return backward(api, b);
+}
+
+int f3dgs_backward_absgrad(int P, int D, int M, int R, int C, const float* background, int width, int height,
+                           const float* means3D, const float* shs, const float* colors_precomp,
+                           const void* semantic_feature, int semantic_feature_dtype, const float* scales,
+                           float scale_modifier, const float* rotations, const float* cov3D_precomp,
+                           const float* viewmatrix, const float* projmatrix, const float* cam_pos, float tan_fovx,
+                           float tan_fovy, const int* radii, char* geom_buffer, char* binning_buffer,
+                           char* image_buffer, const float* dL_dpix, const void* dL_dfeaturepix,
+                           int dL_dfeaturepix_dtype, float dL_dfeaturepix_scale, const float* dL_depths,
+                           float* dL_dmean2D, float* dL_dconic, float* dL_dopacity, float* dL_dcolor,
+                           float* dL_dsemantic_feature, float* dL_dmean3D, float* dL_dcov3D, float* dL_dsh,
+                           float* dL_dscale, float* dL_drot, float* dL_dz, int debug, void* cuda_stream,
+                           float* dL_dcamera, int antialiasing, const float* dL_dalpha, const float* dL_dinvdepth,
+                           float* dL_dmean2D_abs) {
+    (void)colors_precomp;
+    const Api api(__func__);
+    if ((dL_dalpha == nullptr) != (dL_dinvdepth == nullptr)) return api.invalid("dL_dalpha and dL_dinvdepth go together");
+    ViewBackward b{P, D, M, R, C, background, width, height, means3D, shs, scales, scale_modifier, rotations,
+                   cov3D_precomp, viewmatrix, projmatrix, cam_pos, tan_fovx, tan_fovy, radii, geom_buffer,
+                   binning_buffer, image_buffer, dL_dpix,
+                   {dL_dfeaturepix, dL_dfeaturepix_dtype == F3DGS_F16, dL_dfeaturepix_scale}, dL_depths, dL_dmean2D,
+                   dL_dconic, dL_dopacity, dL_dcolor, dL_dsemantic_feature, dL_dmean3D, dL_dcov3D, dL_dsh, dL_dscale,
+                   dL_drot, dL_dz, debug, (cudaStream_t)cuda_stream};
+    if (const int rc = feature_rows(api, b, semantic_feature, semantic_feature_dtype, dL_dfeaturepix_dtype)) return rc;
+    b.dL_dcamera = dL_dcamera;
+    b.antialiasing = antialiasing != 0;
+    b.dL_dalpha = dL_dalpha;
+    b.dL_dinvdepth = dL_dinvdepth;
+    b.absgrad = true;
+    b.dL_dmean2D_abs = dL_dmean2D_abs;
+    return backward(api, b);
+}
+
+int f3dgs_backward_accum_absgrad(
+    int P, int D, int M, int R, int C, const float* background, int width, int height, const float* means3D,
+    const float* shs, const float* colors_precomp, const void* semantic_feature, int semantic_feature_dtype,
+    const float* scales, float scale_modifier, const float* rotations, const float* cov3D_precomp,
+    const float* viewmatrix, const float* projmatrix, const float* cam_pos, float tan_fovx, float tan_fovy,
+    const int* radii, char* geom_buffer, char* binning_buffer, char* image_buffer, const float* dL_dpix,
+    const void* dL_dfeaturepix, int dL_dfeaturepix_dtype, float dL_dfeaturepix_scale, const float* dL_depths,
+    char* scratch, float* dL_dopacity, float* dL_dcolors_precomp, float* dL_dsemantic_feature, float* dL_dmean3D,
+    float* dL_dcov3D_precomp, float* dL_dsh, float* dL_dscale, float* dL_drot, float* dL_dmean2D_out,
+    float* grad_accum, float* denom, void* composite_done_event, int debug, void* cuda_stream, float* dL_dcamera,
+    int antialiasing, const float* dL_dalpha, const float* dL_dinvdepth, float* dL_dmean2D_abs,
+    float* grad_accum_abs) {
+    const Api api(__func__);
+    if ((dL_dalpha == nullptr) != (dL_dinvdepth == nullptr)) return api.invalid("dL_dalpha and dL_dinvdepth go together");
+    ViewBackward b{P, D, M, R, C, background, width, height, means3D, shs, scales, scale_modifier, rotations,
+                   cov3D_precomp, viewmatrix, projmatrix, cam_pos, tan_fovx, tan_fovy, radii, geom_buffer,
+                   binning_buffer, image_buffer, dL_dpix,
+                   {dL_dfeaturepix, dL_dfeaturepix_dtype == F3DGS_F16, dL_dfeaturepix_scale}, dL_depths, nullptr,
+                   nullptr, dL_dopacity, dL_dcolors_precomp, dL_dsemantic_feature, dL_dmean3D, dL_dcov3D_precomp,
+                   dL_dsh, dL_dscale, dL_drot, nullptr, debug, (cudaStream_t)cuda_stream, true, scratch,
+                   colors_precomp, dL_dmean2D_out, grad_accum, denom, (cudaEvent_t)composite_done_event};
+    if (const int rc = feature_rows(api, b, semantic_feature, semantic_feature_dtype, dL_dfeaturepix_dtype)) return rc;
+    b.dL_dcamera = dL_dcamera;
+    b.antialiasing = antialiasing != 0;
+    b.dL_dalpha = dL_dalpha;
+    b.dL_dinvdepth = dL_dinvdepth;
+    b.absgrad = true;
+    b.dL_dmean2D_abs = dL_dmean2D_abs;
+    b.grad_accum_abs = grad_accum_abs;
     return backward(api, b);
 }
 
@@ -1374,6 +1449,21 @@ int f3dgs_densify_plan(int P, const float* grad_accum, const float* denom, const
         return api.invalid("counts overlaps scratch");
     return api.cuda(launch_densify_plan(P, grad_accum, denom, raw_opacity, raw_scaling, max_grad, dense_scale,
                                         min_opacity, max_world_scale, scratch, counts, (cudaStream_t)cuda_stream));
+}
+
+int f3dgs_densify_plan_absgrad(int P, const float* grad_accum, const float* denom, const float* raw_opacity,
+                               const float* raw_scaling, float max_grad, float dense_scale, float min_opacity,
+                               float max_world_scale, char* scratch, int32_t* counts, void* cuda_stream,
+                               const float* grad_accum_abs, float abs_grad) {
+    const Api api(__func__);
+    if (P < 0 || 3 * (long long)P > INT_MAX) return api.invalid("bad sizes (0 <= 3 P <= INT_MAX)");
+    if (!counts || (P > 0 && (!grad_accum || !denom || !grad_accum_abs || !raw_opacity || !raw_scaling || !scratch)))
+        return api.invalid("NULL pointer");
+    if (overlaps({counts, 16}, {{scratch, densify_scratch_fixed_bytes(P)}}))
+        return api.invalid("counts overlaps scratch");
+    return api.cuda(launch_densify_plan(P, grad_accum, denom, raw_opacity, raw_scaling, max_grad, dense_scale,
+                                        min_opacity, max_world_scale, scratch, counts, (cudaStream_t)cuda_stream,
+                                        grad_accum_abs, abs_grad));
 }
 
 int f3dgs_prune_plan(int P, const uint8_t* keep, char* scratch, int32_t* counts, void* cuda_stream) {

@@ -29,9 +29,15 @@
 //       place of z_i (dL/dI_p and one more float per lane), and dL/dz_i gains -w_i gI / z_i^2 in the same reduced value.
 //       The walk reads only what every forward stores (records, final_T, n_contrib), and with gA = gI = 0 each added
 //       term is an exact zero, so every output is bitwise that of the walk without PLANES.
+//   ABS            (GEOM, EMIT and FEAT, opt-in) AbsGS's densification statistic: the flush of each parked 2-D mean row
+//       (values 0 and 1) also sums the absolute values of its 32 per-pixel terms and adds that with one more
+//       red.global.add into dL_dmean2D_abs[P,3].  The per-pair loop, the parking and the shared memory are those of the
+//       walk without it, so every other output is bitwise unchanged.  With features and FEAT the re-walk flushes its
+//       own terms the same way: the statistic is then sum_p |colour-walk term| + sum_p |feature-walk term|.
 // 12 warps and a ring without weight slots (RingSlim, 113 KB of shared memory with the reduction tiles): two CTAs per SM,
 // and the alpha warps keep the launch register count (80).
 // As in the reference, the feature loss does not feed dL/dalpha (backward.cu:575 is disabled) unless FEAT is asked for.
+#include <cassert>  // F3DGS_DEBUG_LISTS
 #include <mutex>
 
 #include "composite_common.cuh"
@@ -71,6 +77,7 @@ struct BwdArgs {
     const float* dL_dinvdepth;  // PLANES: [H,W] gI
     float* max_weight;          // SCORE: [P] = max(max_weight, the largest w of the view)
     int64_t* pixel_count;       // SCORE: [P] += the number of pixels the Gaussian blended into
+    float* dL_dmean2D_abs;      // ABS: [P,3] += sum over the view's pixels of |2-D mean term| (x, y; z untouched)
 };
 
 // GEOM: geometric gradients; EMIT: and the feature lists; LIFT: the feature lists and the per-Gaussian weight sums;
@@ -125,7 +132,7 @@ __device__ __forceinline__ void score_flush_row(const BwdArgs& args, int v, uint
         atomicMax(reinterpret_cast<int*>(args.max_weight + gid), __float_as_int(m));
 }
 
-template <BwdMode MODE, bool PLANES = false>
+template <BwdMode MODE, bool PLANES = false, bool ABS = false>
 __global__ void __launch_bounds__(kBwdThreads, kSlimCtas)
 composite_bwd_kernel(const BwdArgs args) {
     constexpr bool EMIT = MODE != BwdMode::GEOM && MODE != BwdMode::SCORE;
@@ -190,6 +197,19 @@ composite_bwd_kernel(const BwdArgs args) {
                     red_add_f1(args.weight_sum + red_gid[slot], (s0 + s1) + (s2 + s3));
                 else
                     red_add_f1(geom_dst(args, v, red_gid[slot]), (s0 + s1) + (s2 + s3));
+                if constexpr (ABS) {
+                    // the 2-D mean rows: the same 32 terms again, as absolute values.  One accumulator: with four, the
+                    // EMIT + PLANES walk spilled 16 bytes more than without ABS
+                    if (v < 2) {
+                        float t = 0.f;
+#pragma unroll
+                        for (int jj = 0; jj < 8; jj++) {
+                            const float4 q = row[jj];
+                            t += (fabsf(q.x) + fabsf(q.y)) + (fabsf(q.z) + fabsf(q.w));
+                        }
+                        red_add_f1(args.dL_dmean2D_abs + 3 * (size_t)red_gid[slot] + v, t);
+                    }
+                }
             }
         }
         __syncwarp();
@@ -401,11 +421,12 @@ static cudaError_t alloc_lists(size_t R, size_t tiles, char** mem, InstanceLists
     return e;
 }
 
-// The geometry kernel in mode MODE over the view's forward buffers; for EMIT and LIFT also the instance lists and then
+// The geometry kernel in mode MODE (with ABS: and the absolute 2-D mean sums, in the FEAT walk too) over the view's
+// forward buffers; for EMIT and LIFT also the instance lists and then
 // feature_bwd over them (SCORE has neither), reducing sum_p w * scale * map[:, p] into dst.  `a` brings the mode's outputs.  With features
 // (EMIT only), feature_dot then turns the lists' weights into pair dot products and the FEAT walk adds the feature term
 // to the geometric gradients; the lists are freed after it.
-template <BwdMode MODE, typename TG, bool PLANES = false>
+template <BwdMode MODE, typename TG, bool PLANES = false, bool ABS = false>
 static cudaError_t run_bwd(BwdArgs a, const ViewParams& vp, const ForwardBuffers& fb, const TG* map, float scale,
                            float* dst, cudaStream_t s, const FeatureRows& feat = {}) {
     a.pa = producer_args(vp, fb.ranges, fb.point_list, fb.rec, fb.n_contrib, fb.counters + kCounterBwdGeom);
@@ -421,7 +442,11 @@ static cudaError_t run_bwd(BwdArgs a, const ViewParams& vp, const ForwardBuffers
     cudaError_t e = device_sms<composite_bwd_kernel<BwdMode::GEOM>, composite_bwd_kernel<BwdMode::EMIT>,
                                composite_bwd_kernel<BwdMode::LIFT>, composite_bwd_kernel<BwdMode::FEAT>,
                                composite_bwd_kernel<BwdMode::GEOM, true>, composite_bwd_kernel<BwdMode::EMIT, true>,
-                               composite_bwd_kernel<BwdMode::SCORE>>(
+                               composite_bwd_kernel<BwdMode::SCORE>, composite_bwd_kernel<BwdMode::GEOM, false, true>,
+                               composite_bwd_kernel<BwdMode::EMIT, false, true>,
+                               composite_bwd_kernel<BwdMode::GEOM, true, true>,
+                               composite_bwd_kernel<BwdMode::EMIT, true, true>,
+                               composite_bwd_kernel<BwdMode::FEAT, false, true>>(
         num_sms, sizeof(BwdSmem), kBwdThreads, kSlimCtas);
     const int grid = min(a.pa.num_tiles, kSlimCtas * num_sms);
     auto walk = [&](void (*kernel)(BwdArgs)) {
@@ -431,12 +456,12 @@ static cudaError_t run_bwd(BwdArgs a, const ViewParams& vp, const ForwardBuffers
         g_launches++;
         return cudaGetLastError();
     };
-    if (e == cudaSuccess) e = walk(composite_bwd_kernel<MODE, PLANES>);
+    if (e == cudaSuccess) e = walk(composite_bwd_kernel<MODE, PLANES, ABS>);
     if (lists) {
         if (e == cudaSuccess) e = launch_feature_bwd(vp, fb.ranges, a.lists, map, scale, dst, fb.counters, s);
         if (MODE == BwdMode::EMIT && feat.rows) {
             if (e == cudaSuccess) e = launch_feature_dot(vp, fb.ranges, a.lists, feat, map, scale, fb.counters, s);
-            if (e == cudaSuccess) e = walk(composite_bwd_kernel<BwdMode::FEAT>);
+            if (e == cudaSuccess) e = walk(composite_bwd_kernel<BwdMode::FEAT, false, ABS>);
         }
         cudaFreeAsync(mem, s);
     }
@@ -448,15 +473,20 @@ cudaError_t launch_composite_bwd(const ViewParams& vp, const ForwardBuffers& fb,
                                  const float* dL_ddepth, const TG* dL_dfeat_pix, float dL_dfeat_pix_scale,
                                  float* dL_dmean2D, float* dL_dconic, float* dL_dopacity, float* dL_dcolor, float* dL_dz,
                                  float* dL_dfeature, cudaStream_t s, const FeatureRows& feat, const float* dL_dalpha,
-                                 const float* dL_dinvdepth) {
+                                 const float* dL_dinvdepth, float* dL_dmean2D_abs) {
     BwdArgs a{};
     a.bg = bg; a.dL_dpix = dL_dpix; a.dL_ddepth = dL_ddepth;
     a.dL_dmean2D = dL_dmean2D; a.dL_dconic = dL_dconic; a.dL_dopacity = dL_dopacity; a.dL_dcolor = dL_dcolor;
     a.dL_dz = dL_dz;
     a.dL_dalpha = dL_dalpha; a.dL_dinvdepth = dL_dinvdepth;
+    a.dL_dmean2D_abs = dL_dmean2D_abs;
     const bool emit = vp.C > 0 && fb.R > 0;
-    const auto run = dL_dalpha ? (emit ? run_bwd<BwdMode::EMIT, TG, true> : run_bwd<BwdMode::GEOM, TG, true>)
-                               : (emit ? run_bwd<BwdMode::EMIT, TG> : run_bwd<BwdMode::GEOM, TG>);
+    const auto run =
+        dL_dmean2D_abs
+            ? (dL_dalpha ? (emit ? run_bwd<BwdMode::EMIT, TG, true, true> : run_bwd<BwdMode::GEOM, TG, true, true>)
+                         : (emit ? run_bwd<BwdMode::EMIT, TG, false, true> : run_bwd<BwdMode::GEOM, TG, false, true>))
+            : (dL_dalpha ? (emit ? run_bwd<BwdMode::EMIT, TG, true> : run_bwd<BwdMode::GEOM, TG, true>)
+                         : (emit ? run_bwd<BwdMode::EMIT, TG> : run_bwd<BwdMode::GEOM, TG>));
     return run(a, vp, fb, dL_dfeat_pix, dL_dfeat_pix_scale, dL_dfeature, s, feat);
 }
 
@@ -477,10 +507,12 @@ cudaError_t launch_gaussian_scores(const ViewParams& vp, const ForwardBuffers& f
 
 template cudaError_t launch_composite_bwd(const ViewParams&, const ForwardBuffers&, const float*, const float*,
                                           const float*, const float*, float, float*, float*, float*, float*, float*,
-                                          float*, cudaStream_t, const FeatureRows&, const float*, const float*);
+                                          float*, cudaStream_t, const FeatureRows&, const float*, const float*,
+                                          float*);
 template cudaError_t launch_composite_bwd(const ViewParams&, const ForwardBuffers&, const float*, const float*,
                                           const float*, const __half*, float, float*, float*, float*, float*, float*,
-                                          float*, cudaStream_t, const FeatureRows&, const float*, const float*);
+                                          float*, cudaStream_t, const FeatureRows&, const float*, const float*,
+                                          float*);
 template cudaError_t launch_feature_lift(const ViewParams&, const ForwardBuffers&, const float*, float*, float*,
                                          cudaStream_t);
 template cudaError_t launch_feature_lift(const ViewParams&, const ForwardBuffers&, const __half*, float*, float*,

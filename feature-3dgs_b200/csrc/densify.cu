@@ -7,6 +7,7 @@
 //   g = grad_accum / denom (NaN -> 0), smax = max over 3 of expf(raw_scaling), o = sigmoid(raw_opacity)
 //   clone  g >= max_grad && smax <= dense_scale
 //   split  g >= max_grad && smax >  dense_scale
+//          (AbsGS, with grad_accum_abs: ga >= abs_grad && smax > dense_scale, ga = grad_accum_abs / denom, NaN -> 0)
 //   prune  o < min_opacity || smax > max_world_scale   (each row with its own scaling; a child's is
 //                                                        logf(expf(raw) * (1 / 1.6f)), the reference's log(s / (0.8 N)))
 // Both split copies share scaling and opacity, so they are kept or pruned together.
@@ -73,8 +74,11 @@ struct ClassifyArgs {
     const float *grad_accum, *denom, *raw_opacity, *raw_scaling;
     float max_grad, dense_scale, min_opacity, max_world_scale, split_inv;
     int4* flags;
+    const float* grad_accum_abs;  // ABS
+    float abs_grad;               // ABS
 };
 
+template <bool ABS = false>
 __global__ void __launch_bounds__(256) classify_kernel(const __grid_constant__ ClassifyArgs a) {
     const long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x;
     if (i > a.P) return;
@@ -89,7 +93,13 @@ __global__ void __launch_bounds__(256) classify_kernel(const __grid_constant__ C
     const float o = 1.0f / (1.0f + expf(-a.raw_opacity[i]));  // torch.sigmoid
     const bool transparent = o < a.min_opacity;
     const bool sel = g >= a.max_grad;
-    const bool clone = sel && smax <= a.dense_scale, split = sel && smax > a.dense_scale;
+    bool split_sel = sel;
+    if constexpr (ABS) {
+        float ga = a.grad_accum_abs[i] / a.denom[i];
+        if (ga != ga) ga = 0.0f;
+        split_sel = ga >= a.abs_grad;
+    }
+    const bool clone = sel && smax <= a.dense_scale, split = split_sel && smax > a.dense_scale;
     const bool prune = transparent || smax > a.max_world_scale;  // the clone shares the original's scaling
     int child = 0;
     if (split) {
@@ -223,14 +233,19 @@ float densify_split_inv() { return 1.0f / (float)(0.8 * 2); }  // as torch: opma
 
 cudaError_t launch_densify_plan(int P, const float* grad_accum, const float* denom, const float* raw_opacity,
                                 const float* raw_scaling, float max_grad, float dense_scale, float min_opacity,
-                                float max_world_scale, char* scratch, int32_t* counts, cudaStream_t s) {
+                                float max_world_scale, char* scratch, int32_t* counts, cudaStream_t s,
+                                const float* grad_accum_abs, float abs_grad) {
     if (P == 0) return cudaMemsetAsync(counts, 0, 4 * sizeof(int32_t), s);
     int4* flags = reinterpret_cast<int4*>(scratch);
-    ClassifyArgs c;
+    ClassifyArgs c{};
     c.P = P; c.grad_accum = grad_accum; c.denom = denom; c.raw_opacity = raw_opacity; c.raw_scaling = raw_scaling;
     c.max_grad = max_grad; c.dense_scale = dense_scale; c.min_opacity = min_opacity; c.max_world_scale = max_world_scale;
     c.split_inv = densify_split_inv(); c.flags = flags;
-    classify_kernel<<<blocks_for((long long)P + 1), 256, 0, s>>>(c);
+    c.grad_accum_abs = grad_accum_abs; c.abs_grad = abs_grad;
+    if (grad_accum_abs)
+        classify_kernel<true><<<blocks_for((long long)P + 1), 256, 0, s>>>(c);
+    else
+        classify_kernel<<<blocks_for((long long)P + 1), 256, 0, s>>>(c);
     g_launches++;
     return scan_flags(P, scratch, counts, s);
 }

@@ -35,7 +35,8 @@ void launch_preprocess_fwd(const ViewParams& vp, const float* means3D, const flo
 // float64 block partials come from the default memory pool: cudaErrorMemoryAllocation if that fails.
 // antialiasing: the backward of an antialiased forward, whose records `rec` hold op_eff = opacity * rho.  dL_dop_eff
 // [P] is the composite's dL/dop_eff; dL_dopacity gets rho * dL_dop_eff (assigned, or added with `accumulate`).  In the
-// assigning backward the two may be one buffer, rescaled in place.
+// assigning backward the two may be one buffer, rescaled in place.  grad_accum_abs (accumulate with grad_accum only):
+// += ||dL_dmean2D_abs.xy|| for every Gaussian with radii > 0, next to grad_accum's own update.
 cudaError_t launch_preprocess_bwd(const ViewParams& vp, const float* means3D, const int* radii, const float* shs,
                                   const uint8_t* clamped, const float* scales, const float* rotations,
                                   const float* cov3D, const float* dL_dmean2D, const float* dL_dconic,
@@ -43,7 +44,8 @@ cudaError_t launch_preprocess_bwd(const ViewParams& vp, const float* means3D, co
                                   float* dL_dscale, float* dL_drot, const float* dL_dz, cudaStream_t s,
                                   bool accumulate = false, float* grad_accum = nullptr, float* denom = nullptr,
                                   float* dL_dcamera = nullptr, bool antialiasing = false, const SplatRec* rec = nullptr,
-                                  const float* dL_dop_eff = nullptr, float* dL_dopacity = nullptr);
+                                  const float* dL_dop_eff = nullptr, float* dL_dopacity = nullptr,
+                                  const float* dL_dmean2D_abs = nullptr, float* grad_accum_abs = nullptr);
 
 void launch_mark_visible(int P, const float* means3D, const float* viewmatrix, uint8_t* present,
                          cudaStream_t s);
@@ -89,12 +91,16 @@ struct FeatureRows {
 // of dL/dalpha is added to dL_dmean2D, dL_dconic and dL_dopacity by two more kernels over the same lists.  With
 // dL_dalpha (then dL_dinvdepth too, both [H,W]): the gradients of the forward's opacity and inverse-depth planes join
 // dL/dalpha and dL_dz in the same geometry walk; with both zero every output is bitwise that of the call without them.
+// With dL_dmean2D_abs ([P,3], added to; the third column untouched): AbsGS's statistic, the sums over the view's pixels
+// of |x| and |y| of each pixel's 2-D mean term, from the same walk (and the feature walk's own terms with feat.rows);
+// every other output is bitwise that of the call without it.
 template <typename TG>
 cudaError_t launch_composite_bwd(const ViewParams& vp, const ForwardBuffers& fb, const float* bg, const float* dL_dpix,
                                  const float* dL_ddepth, const TG* dL_dfeat_pix, float dL_dfeat_pix_scale,
                                  float* dL_dmean2D, float* dL_dconic, float* dL_dopacity, float* dL_dcolor, float* dL_dz,
                                  float* dL_dfeature, cudaStream_t s, const FeatureRows& feat = {},
-                                 const float* dL_dalpha = nullptr, const float* dL_dinvdepth = nullptr);
+                                 const float* dL_dalpha = nullptr, const float* dL_dinvdepth = nullptr,
+                                 float* dL_dmean2D_abs = nullptr);
 // Feature lifting, R > 0: weight_sum[P] += the blend weights w = alpha*T of each Gaussian over the view and
 // feature_sum[P, C] += sum_p w * map[:, p], through the same lists.  TF (float or __half) is the element type of map
 template <typename TF>
@@ -168,9 +174,11 @@ cudaError_t launch_knn_mean_dist(int P, const float* points, float* out, char* s
 // src / dst are the 21 fields of f3dgs_gaussian_fields[3] in order
 cudaError_t densify_scratch_bytes(int P, size_t* bytes);
 size_t densify_scratch_fixed_bytes(int P);
+// grad_accum_abs (optional): AbsGS's split rule, split when grad_accum_abs / denom >= abs_grad (instead of g >= max_grad)
 cudaError_t launch_densify_plan(int P, const float* grad_accum, const float* denom, const float* raw_opacity,
                                 const float* raw_scaling, float max_grad, float dense_scale, float min_opacity,
-                                float max_world_scale, char* scratch, int32_t* counts, cudaStream_t s);
+                                float max_world_scale, char* scratch, int32_t* counts, cudaStream_t s,
+                                const float* grad_accum_abs = nullptr, float abs_grad = 0.f);
 // prune from a mask: the plan of launch_densify_apply that keeps row i iff keep[i] != 0, counts {A, 0, 0, 0}
 cudaError_t launch_prune_plan(int P, const uint8_t* keep, char* scratch, int32_t* counts, cudaStream_t s);
 cudaError_t launch_densify_apply(int P, int M, int C, const char* scratch, const int32_t counts[4], const float* normals,

@@ -436,7 +436,8 @@ __host__ __device__ constexpr int cam_slot(int j) {  // slot -> index in the 35-
 // covariance joins dL/d(a, b, c), from where it reaches cov3D, scale, rotation, the mean and the camera.  op_eff is the
 // splat record's op.  dL_dop_eff may be dL_dopacity itself (the assigning backward rescales in place): the two are read
 // and written by the same thread, so neither is __restrict__.
-template <bool ACCUM, bool CAM, bool AA>
+// ABS = true (ACCUM only): AbsGS's statistic grad_accum_abs += ||dL_dmean2D_abs.xy||, gated and formed as grad_accum is.
+template <bool ACCUM, bool CAM, bool AA, bool ABS = false>
 __global__ void __launch_bounds__(kBwdBlock)
 preprocess_bwd_kernel(ViewParams vp, const float* __restrict__ means3D, const int* __restrict__ radii,
                       const float* __restrict__ shs, const uint8_t* __restrict__ clamped,
@@ -447,7 +448,8 @@ preprocess_bwd_kernel(ViewParams vp, const float* __restrict__ means3D, const in
                       float* __restrict__ dL_dsh, float* __restrict__ dL_dscale, float* __restrict__ dL_drot,
                       const float* __restrict__ dL_dz, float* __restrict__ grad_accum, float* __restrict__ vis_count,
                       double* __restrict__ cam_part, const SplatRec* __restrict__ rec, const float* dL_dop_eff,
-                      float* dL_dopacity) {
+                      float* dL_dopacity, const float* __restrict__ dL_dmean2D_abs,
+                      float* __restrict__ grad_accum_abs) {
     extern __shared__ float bwd_smem[];
     const int idx = blockIdx.x * blockDim.x + threadIdx.x;
     const int row_floats = vp.M * 3, stride = bwd_row_stride(row_floats);
@@ -485,6 +487,10 @@ preprocess_bwd_kernel(ViewParams vp, const float* __restrict__ means3D, const in
         const float ux = dL_dmean2D[3 * idx], uy = dL_dmean2D[3 * idx + 1];
         grad_accum[idx] += sqrtf(ux * ux + uy * uy);
         vis_count[idx] += 1.0f;
+        if constexpr (ABS) {
+            const float ax = dL_dmean2D_abs[3 * idx], ay = dL_dmean2D_abs[3 * idx + 1];
+            grad_accum_abs[idx] += sqrtf(ax * ax + ay * ay);
+        }
     }
     const float* vm = vp.viewmatrix;
     const float* proj = vp.projmatrix;
@@ -811,7 +817,8 @@ cudaError_t launch_preprocess_bwd(const ViewParams& vp, const float* means3D, co
                                   float* dL_dmean3D, const float* dL_dcolor, float* dL_dcov3D, float* dL_dsh,
                                   float* dL_dscale, float* dL_drot, const float* dL_dz, cudaStream_t s, bool accumulate,
                                   float* grad_accum, float* denom, float* dL_dcamera, bool antialiasing,
-                                  const SplatRec* rec, const float* dL_dop_eff, float* dL_dopacity) {
+                                  const SplatRec* rec, const float* dL_dop_eff, float* dL_dopacity,
+                                  const float* dL_dmean2D_abs, float* grad_accum_abs) {
     if (vp.P <= 0) return cudaSuccess;
     using Kernel = decltype(&preprocess_bwd_kernel<false, false, false>);
     // [accumulate][camera][antialiasing]
@@ -820,13 +827,18 @@ cudaError_t launch_preprocess_bwd(const ViewParams& vp, const float* means3D, co
          {preprocess_bwd_kernel<false, true, false>, preprocess_bwd_kernel<false, true, true>}},
         {{preprocess_bwd_kernel<true, false, false>, preprocess_bwd_kernel<true, false, true>},
          {preprocess_bwd_kernel<true, true, false>, preprocess_bwd_kernel<true, true, true>}}};
+    // the accumulating backward with AbsGS's statistic: [camera][antialiasing]
+    static const Kernel abs_kernels[2][2] = {
+        {preprocess_bwd_kernel<true, false, false, true>, preprocess_bwd_kernel<true, false, true, true>},
+        {preprocess_bwd_kernel<true, true, false, true>, preprocess_bwd_kernel<true, true, true, true>}};
     const size_t smem = shs ? (size_t)2 * kBwdBlock * bwd_row_stride(vp.M * 3) * sizeof(float) + kBwdBlock : 0;
     static std::atomic<int> attr_set{0};
     int dev = 0;
     cudaGetDevice(&dev);
     if (smem > 48 * 1024 && !((attr_set.load() >> (dev & 31)) & 1)) {  // once per device; harmless if repeated
         for (const Kernel k : {kernels[0][0][0], kernels[0][0][1], kernels[0][1][0], kernels[0][1][1], kernels[1][0][0],
-                               kernels[1][0][1], kernels[1][1][0], kernels[1][1][1]})
+                               kernels[1][0][1], kernels[1][1][0], kernels[1][1][1], abs_kernels[0][0],
+                               abs_kernels[0][1], abs_kernels[1][0], abs_kernels[1][1]})
             cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024);
         attr_set.fetch_or(1 << (dev & 31));
     }
@@ -838,10 +850,11 @@ cudaError_t launch_preprocess_bwd(const ViewParams& vp, const float* means3D, co
         const cudaError_t e = cudaMallocAsync((void**)&part, (size_t)grid * kCamTerms * sizeof(double), s);
         if (e != cudaSuccess) return e;
     }
-    kernels[accumulate][cam][antialiasing]<<<grid, kBwdBlock, smem, s>>>(
+    const bool abs = accumulate && grad_accum && grad_accum_abs;
+    (abs ? abs_kernels[cam][antialiasing] : kernels[accumulate][cam][antialiasing])<<<grid, kBwdBlock, smem, s>>>(
         vp, means3D, radii, shs, clamped, scales, rotations, cov3D, dL_dmean2D, dL_dconic, dL_dmean3D, dL_dcolor,
         dL_dcov3D, dL_dsh, dL_dscale, dL_drot, dL_dz, accumulate ? grad_accum : nullptr, accumulate ? denom : nullptr,
-        part, rec, dL_dop_eff, dL_dopacity);
+        part, rec, dL_dop_eff, dL_dopacity, abs ? dL_dmean2D_abs : nullptr, abs ? grad_accum_abs : nullptr);
     g_launches++;
     if (!cam) return cudaSuccess;  // a launch error is left for the caller's cudaGetLastError
     camera_grad_sum_kernel<<<kCamTerms, kCamSumThreads, 0, s>>>(grid, part, dL_dcamera);

@@ -18,7 +18,9 @@
 // feature_map, depth, alpha, invdepth, radii, geom, binning, img) (f3dgs_forward_alpha_invdepth) and
 // rasterize_gaussians_backward_alpha_invdepth(the backward's arguments, dL_dout_alpha, dL_dout_invdepth, camera=False,
 // semantic_feature=None, antialiasing=False) -> the same 12 as rasterize_gaussians_backward_antialiased
-// (f3dgs_backward_alpha_invdepth).
+// (f3dgs_backward_alpha_invdepth).  AbsGS's densification statistic:
+// rasterize_gaussians_backward_absgrad(the backward's arguments, dL_dout_alpha=None, dL_dout_invdepth=None, camera=False,
+// semantic_feature=None, antialiasing=False) -> the same 12 and dL_dmeans2D_abs [P,3] (f3dgs_backward_absgrad).
 // Differences (all permissive): the feature width is read from semantic_feature.size(-1) at run
 // time (reference: compile-time NUM_SEMANTIC_CHANNELS, config.h:16); an empty / undefined
 // semantic_feature means C = 0; semantic_feature may be float32 or float16, and the feature map
@@ -237,7 +239,8 @@ using BackwardGrads = std::tuple<torch::Tensor, torch::Tensor, torch::Tensor, to
 // f3dgs_backward_feature_geometry, which reads semantic_feature and takes the camera gradient as an optional argument;
 // with antialiasing, f3dgs_backward_antialiased, whose feature term reads `features` if that is given; with `planes`
 // (the gradients of the opacity and inverse-depth planes), f3dgs_backward_alpha_invdepth, with the feature term as under
-// antialiasing and the forward's mode `antialiasing`
+// antialiasing and the forward's mode `antialiasing`; with `abs_out` (set to the [P,3] statistic), f3dgs_backward_absgrad,
+// with the planes when `planes` is given, and otherwise as f3dgs_backward_alpha_invdepth
 static BackwardGrads backward_grads(const torch::Tensor& background, const torch::Tensor& means3D,
                                const torch::Tensor& radii, const torch::Tensor& colors,
                                const torch::Tensor& semantic_feature, const torch::Tensor& scales,
@@ -250,7 +253,7 @@ static BackwardGrads backward_grads(const torch::Tensor& background, const torch
                                const torch::Tensor& binningBuffer, const torch::Tensor& imageBuffer,
                                const bool debug, float* camera, bool feature_geometry = false,
                                bool antialiasing = false, const torch::Tensor& features = torch::Tensor(),
-                               const torch::Tensor* planes = nullptr) {
+                               const torch::Tensor* planes = nullptr, torch::Tensor* abs_out = nullptr) {
     TORCH_CHECK(means3D.is_cuda(), "means3D must be a CUDA tensor (this build has no CPU path)");
     const c10::cuda::CUDAGuard guard(means3D.device());
     const auto dev = means3D.device();
@@ -274,6 +277,7 @@ static BackwardGrads backward_grads(const torch::Tensor& background, const torch
     torch::Tensor dL_dscales = torch::zeros({P, 3}, o);
     torch::Tensor dL_drotations = torch::zeros({P, 4}, o);
     torch::Tensor dL_dz = torch::zeros({P, 1}, o);
+    if (abs_out) *abs_out = torch::zeros({P, 3}, o);
 
     if (P != 0) {
         // only semantic_feature's shape is used: dL/dfeature depends on the blend weights alone (f3dgs_backward does
@@ -340,7 +344,16 @@ static BackwardGrads backward_grads(const torch::Tensor& background, const torch
                         " elements (got ", t.numel(), ")");
             return t.contiguous();
         };
-        if (planes) {
+        if (abs_out) {
+            torch::Tensor ga, gi;
+            if (planes) {
+                ga = plane_grad(planes[0], dev, H, W, "dL_dout_alpha");
+                gi = plane_grad(planes[1], dev, H, W, "dL_dout_invdepth");
+            }
+            check_rc(typed_call(f3dgs_backward_absgrad, feature_rows(features), antialiasing ? 1 : 0, fptr(ga), fptr(gi),
+                                abs_out->data_ptr<float>()),
+                     "f3dgs_backward_absgrad");
+        } else if (planes) {
             auto ga = plane_grad(planes[0], dev, H, W, "dL_dout_alpha"), gi = plane_grad(planes[1], dev, H, W,
                                                                                        "dL_dout_invdepth");
             check_rc(typed_call(f3dgs_backward_alpha_invdepth, feature_rows(features), antialiasing ? 1 : 0, fptr(ga),
@@ -427,6 +440,23 @@ CameraGrads RasterizeGaussiansBackwardAlphaInvDepthCUDA(BACKWARD_PARAMS, const t
         return backward_grads(BACKWARD_ARGS, cam, false, antialiasing, f, planes);
     });
 }
+// rasterize_gaussians_backward_alpha_invdepth's 12 results, the planes optional (both None: none; one alone: the other
+// is zero), and dL_dmeans2D_abs [P,3]: AbsGS's per-view sums of |per-pixel 2-D mean terms| (f3dgs_backward_absgrad)
+std::tuple<torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor,
+           torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor>
+RasterizeGaussiansBackwardAbsGradCUDA(BACKWARD_PARAMS, const std::optional<torch::Tensor>& dL_dout_alpha,
+                                      const std::optional<torch::Tensor>& dL_dout_invdepth, const bool camera,
+                                      const std::optional<torch::Tensor>& features, const bool antialiasing) {
+    const torch::Tensor f = features.has_value() ? *features : torch::Tensor();
+    const torch::Tensor none;
+    const torch::Tensor planes[2] = {dL_dout_alpha.value_or(none), dL_dout_invdepth.value_or(none)};
+    const bool has_planes = planes[0].defined() || planes[1].defined();
+    torch::Tensor abs;
+    auto grads = with_camera_grads(means3D, camera, [&](float* cam) {
+        return backward_grads(BACKWARD_ARGS, cam, false, antialiasing, f, has_planes ? planes : nullptr, &abs);
+    });
+    return std::tuple_cat(grads, std::make_tuple(abs));
+}
 #undef BACKWARD_PARAMS
 #undef BACKWARD_ARGS
 
@@ -437,7 +467,9 @@ CameraGrads RasterizeGaussiansBackwardAlphaInvDepthCUDA(BACKWARD_PARAMS, const t
 // dL/dalpha in the geometric gradients.  antialiasing: f3dgs_backward_accum_antialiased, for the buffers of
 // rasterize_gaussians_antialiased (with the feature term if semantic_feature is given).  dL_dout_alpha / dL_dout_invdepth
 // (optional; one given alone: the other is zero): f3dgs_backward_accum_alpha_invdepth, the gradients of the opacity and
-// inverse-depth planes, for the buffers of either forward in the mode `antialiasing`.
+// inverse-depth planes, for the buffers of either forward in the mode `antialiasing`.  dL_dmean2D_abs (optional, [P,3]
+// contiguous float32): f3dgs_backward_accum_absgrad with any of the above, which writes the view's AbsGS statistic into
+// it and, with grad_accum_abs ([P], needs grad_accum and denom), adds its norm there.
 void RasterizeGaussiansBackwardAccumCUDA(
     const torch::Tensor& background, const torch::Tensor& means3D, const torch::Tensor& radii,
     const torch::Tensor& colors, const torch::Tensor& scales, const torch::Tensor& rotations, const float scale_modifier,
@@ -451,11 +483,15 @@ void RasterizeGaussiansBackwardAccumCUDA(
     const int64_t composite_done_event, const bool debug, const double feature_grad_scale,
     const std::optional<torch::Tensor>& camera_grad, const std::optional<torch::Tensor>& semantic_feature,
     const bool antialiasing, const std::optional<torch::Tensor>& dL_dout_alpha,
-    const std::optional<torch::Tensor>& dL_dout_invdepth) {
+    const std::optional<torch::Tensor>& dL_dout_invdepth, const std::optional<torch::Tensor>& dL_dmean2D_abs,
+    const std::optional<torch::Tensor>& grad_accum_abs) {
     TORCH_CHECK(means3D.is_cuda(), "means3D must be a CUDA tensor (this build has no CPU path)");
     const c10::cuda::CUDAGuard guard(means3D.device());
     const auto dev = means3D.device();
     const int P = means3D.size(0);
+    const bool has_abs = dL_dmean2D_abs.has_value() && dL_dmean2D_abs->defined();
+    TORCH_CHECK(has_abs || !(grad_accum_abs.has_value() && grad_accum_abs->defined()),
+                "grad_accum_abs needs dL_dmean2D_abs");
     if (P == 0) return;
     const int H = dL_dout_color.size(1), W = dL_dout_color.size(2);
     int M = 0;
@@ -491,7 +527,7 @@ void RasterizeGaussiansBackwardAccumCUDA(
     const bool has_features = semantic_feature.has_value() && semantic_feature->defined();
     const bool has_planes = (dL_dout_alpha.has_value() && dL_dout_alpha->defined()) ||
                             (dL_dout_invdepth.has_value() && dL_dout_invdepth->defined());
-    if (has_features || antialiasing || has_planes) {
+    if (has_features || antialiasing || has_planes || has_abs) {
         torch::Tensor sf;
         if (has_features) {
             check_features(*semantic_feature, dev);
@@ -521,8 +557,18 @@ void RasterizeGaussiansBackwardAccumCUDA(
                       reinterpret_cast<void*>(static_cast<intptr_t>(composite_done_event)), debug ? 1 : 0,
                       (void*)stream, cam, tail...);
         };
-        if (has_planes) {
-            const torch::Tensor none;
+        const torch::Tensor none;
+        if (has_abs) {
+            torch::Tensor ga, gi;
+            if (has_planes) {
+                ga = plane_grad(dL_dout_alpha.value_or(none), dev, H, W, "dL_dout_alpha");
+                gi = plane_grad(dL_dout_invdepth.value_or(none), dev, H, W, "dL_dout_invdepth");
+            }
+            check_rc(call(f3dgs_backward_accum_absgrad, antialiasing ? 1 : 0, fptr(ga), fptr(gi),
+                          in_place(*dL_dmean2D_abs, dev, (int64_t)P * 3, "dL_dmean2D_abs"),
+                          in_place(grad_accum_abs.value_or(none), dev, P, "grad_accum_abs")),
+                     "f3dgs_backward_accum_absgrad");
+        } else if (has_planes) {
             auto ga = plane_grad(dL_dout_alpha.value_or(none), dev, H, W, "dL_dout_alpha");
             auto gi = plane_grad(dL_dout_invdepth.value_or(none), dev, H, W, "dL_dout_invdepth");
             check_rc(call(f3dgs_backward_accum_alpha_invdepth, antialiasing ? 1 : 0, fptr(ga), fptr(gi)),
@@ -972,10 +1018,13 @@ torch::Tensor knnMeanDist(const torch::Tensor& points) {
 // ---- densification (f3dgs_densify_plan / f3dgs_densify_apply / f3dgs_reset_opacity)
 
 // -> (scratch, counts): counts = device int32[4] {originals kept, clones kept, children kept per copy, split}
+// grad_accum_abs (optional, [P]): AbsGS's split rule with threshold abs_grad (f3dgs_densify_plan_absgrad)
 std::tuple<torch::Tensor, torch::Tensor> densifyPlan(const torch::Tensor& grad_accum, const torch::Tensor& denom,
                                                      const torch::Tensor& raw_opacity, const torch::Tensor& raw_scaling,
                                                      double max_grad, double dense_scale, double min_opacity,
-                                                     double max_world_scale) {
+                                                     double max_world_scale,
+                                                     const std::optional<torch::Tensor>& grad_accum_abs,
+                                                     double abs_grad) {
     TORCH_CHECK(raw_scaling.is_cuda(), "parameters must be CUDA tensors (this build has no CPU path)");
     TORCH_CHECK(raw_scaling.dim() == 2 && raw_scaling.size(1) == 3, "raw_scaling must be [P,3]");
     TORCH_CHECK(raw_scaling.size(0) <= INT32_MAX / 3, "densify: 3 P must be below 2^31");
@@ -990,11 +1039,17 @@ std::tuple<torch::Tensor, torch::Tensor> densifyPlan(const torch::Tensor& grad_a
     torch::Tensor scratch = scratch_tensor(f3dgs_densify_scratch_bytes(P), "f3dgs_densify_scratch_bytes", raw_scaling);
     torch::Tensor counts = torch::empty({4}, raw_scaling.options().dtype(torch::kInt32));
     cudaStream_t stream = c10::cuda::getCurrentCUDAStream().stream();
-    check_rc(f3dgs_densify_plan(P, gp, dp, op, sp, (float)max_grad, (float)dense_scale, (float)min_opacity,
-                                (float)max_world_scale,
-                                scratch.numel() ? reinterpret_cast<char*>(scratch.data_ptr()) : nullptr,
-                                counts.data_ptr<int32_t>(), (void*)stream),
-             "f3dgs_densify_plan");
+    char* sc = scratch.numel() ? reinterpret_cast<char*>(scratch.data_ptr()) : nullptr;
+    if (grad_accum_abs.has_value() && grad_accum_abs->defined()) {
+        auto gaa = grad_accum_abs->contiguous();
+        check_rc(f3dgs_densify_plan_absgrad(P, gp, dp, op, sp, (float)max_grad, (float)dense_scale, (float)min_opacity,
+                                            (float)max_world_scale, sc, counts.data_ptr<int32_t>(), (void*)stream,
+                                            in_place(gaa, dev, P, "grad_accum_abs"), (float)abs_grad),
+                 "f3dgs_densify_plan_absgrad");
+    } else
+        check_rc(f3dgs_densify_plan(P, gp, dp, op, sp, (float)max_grad, (float)dense_scale, (float)min_opacity,
+                                    (float)max_world_scale, sc, counts.data_ptr<int32_t>(), (void*)stream),
+                 "f3dgs_densify_plan");
     return std::make_tuple(scratch, counts);
 }
 
@@ -1392,7 +1447,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
               py::arg("grad_accum"), py::arg("denom"), py::arg("composite_done_event"), py::arg("debug"),
               py::arg("feature_grad_scale") = 1.0, py::arg("camera_grad") = py::none(),
               py::arg("semantic_feature") = py::none(), py::arg("antialiasing") = false,
-              py::arg("dL_dout_alpha") = py::none(), py::arg("dL_dout_invdepth") = py::none());
+              py::arg("dL_dout_alpha") = py::none(), py::arg("dL_dout_invdepth") = py::none(),
+              py::arg("dL_dmean2D_abs") = py::none(), py::arg("grad_accum_abs") = py::none());
         m.def("rasterize_gaussians_antialiased", &RasterizeGaussiansAntialiasedCUDA);
         m.def("rasterize_gaussians_backward_antialiased", &RasterizeGaussiansBackwardAntialiasedCUDA,
               py::arg("background"), py::arg("means3D"), py::arg("radii"), py::arg("colors"), py::arg("features_like"),
@@ -1415,6 +1471,14 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
               py::arg("dL_dout_color"), py::arg("dL_dout_feature"), py::arg("dL_dout_depth"), py::arg("sh"),
               py::arg("degree"), py::arg("campos"), py::arg("geomBuffer"), py::arg("R"), py::arg("binningBuffer"),
               py::arg("imageBuffer"), py::arg("debug"), py::arg("dL_dout_alpha"), py::arg("dL_dout_invdepth"),
+              py::arg("camera") = false, py::arg("semantic_feature") = py::none(), py::arg("antialiasing") = false);
+        m.def("rasterize_gaussians_backward_absgrad", &RasterizeGaussiansBackwardAbsGradCUDA, py::arg("background"),
+              py::arg("means3D"), py::arg("radii"), py::arg("colors"), py::arg("features_like"), py::arg("scales"),
+              py::arg("rotations"), py::arg("scale_modifier"), py::arg("cov3D_precomp"), py::arg("viewmatrix"),
+              py::arg("projmatrix"), py::arg("tan_fovx"), py::arg("tan_fovy"), py::arg("dL_dout_color"),
+              py::arg("dL_dout_feature"), py::arg("dL_dout_depth"), py::arg("sh"), py::arg("degree"), py::arg("campos"),
+              py::arg("geomBuffer"), py::arg("R"), py::arg("binningBuffer"), py::arg("imageBuffer"), py::arg("debug"),
+              py::arg("dL_dout_alpha") = py::none(), py::arg("dL_dout_invdepth") = py::none(),
               py::arg("camera") = false, py::arg("semantic_feature") = py::none(), py::arg("antialiasing") = false);
     }
     m.def("rasterize_gaussians_backward_camera", &RasterizeGaussiansBackwardCameraCUDA);
@@ -1439,7 +1503,10 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     m.def("feature_pca_range", &featurePcaRange);
     m.def("feature_pca_image", &featurePcaImage);
     m.def("knn_mean_dist", &knnMeanDist);
-    m.def("densify_plan", &densifyPlan);
+    m.def("densify_plan", &densifyPlan, pybind11::arg("grad_accum"), pybind11::arg("denom"),
+          pybind11::arg("raw_opacity"), pybind11::arg("raw_scaling"), pybind11::arg("max_grad"),
+          pybind11::arg("dense_scale"), pybind11::arg("min_opacity"), pybind11::arg("max_world_scale"),
+          pybind11::arg("grad_accum_abs") = pybind11::none(), pybind11::arg("abs_grad") = 0.0);
     m.def("densify_apply", &densifyApply);
     m.def("prune_plan", &prunePlan, pybind11::arg("keep"));
     m.def("reset_opacity", &resetOpacity, pybind11::arg("raw_opacity"), pybind11::arg("exp_avg"),

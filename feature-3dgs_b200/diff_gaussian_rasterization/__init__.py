@@ -54,6 +54,14 @@ Behavioural notes
     sum, largest blend weight and blended-pixel count over views (f3dgs_gaussian_scores_accum), and
     `GaussianState.prune(keep)` / `prune_by_importance(scores, ratio)` remove rows with the Adam state carried along
     (f3dgs_prune_plan + f3dgs_densify_apply).
+  * absolute-gradient densification (opt-in, AbsGS): `AbsGradGaussianRasterizer(raster_settings, feature_geometry=False,
+    antialiasing=False)` takes AbsGS's `screenspace_points_abs` as `forward(..., means2D_abs=...)`, a [P,3] tensor that
+    requires grad, and gives it the view's per-Gaussian sums over pixels of |x| and |y| of each pixel's dL/dmean2D term
+    as its `.grad` (f3dgs_backward_absgrad).  A large Gaussian over fine texture, whose per-pixel terms cancel in
+    dL/dmean2D, keeps a large statistic there, so AbsGS's split rule splits it.  The render and every other gradient
+    are GaussianRasterizer's (AntialiasedGaussianRasterizer's with antialiasing).  `ViewBatch(absgrad=True)` and
+    `GaussianState(absgrad=True)` accumulate the statistic natively, and `densify_and_prune(abs_grad=...)` applies
+    the split rule.
   * `debug=True` keeps the reference semantics: arguments are snapshotted to CPU first and dumped
     to snapshot_fw.dump / snapshot_bw.dump if the native call raises (reference :89-97,:147-155);
     natively it synchronises and checks after every stage.
@@ -89,6 +97,7 @@ __all__ = [
     "compute_3d_filter",
     "apply_3d_filter",
     "GaussianScores",
+    "AbsGradGaussianRasterizer",
 ]
 
 
@@ -290,6 +299,44 @@ def _rasterize_alpha_invdepth(means3D, means2D, sh, colors_precomp, semantic_fea
                                                   rs.campos, rs, feature_geometry, antialiasing)
 
 
+class _RasterizeGaussiansAbsGrad(torch.autograd.Function):
+    """The default or antialiased render whose backward also gives means2D_abs AbsGS's statistic, the view's sums over
+    pixels of |x| and |y| of each pixel's dL/dmean2D term (f3dgs_backward_absgrad), in every mode: the camera tensors
+    are always inputs and get gradients when they require grad; feature_geometry adds the feature term of dL/dalpha
+    (and its walk's own absolute terms); antialiasing renders with the antialiased opacities."""
+
+    @staticmethod
+    def forward(ctx, means3D, means2D, sh, colors_precomp, semantic_feature, opacities, scales, rotations,
+                cov3Ds_precomp, means2D_abs, viewmatrix, projmatrix, campos, raster_settings, feature_geometry,
+                antialiasing):
+        rs = raster_settings._replace(viewmatrix=viewmatrix, projmatrix=projmatrix, campos=campos)
+        ctx.camera_shapes = (viewmatrix.shape, projmatrix.shape, campos.shape)
+        ctx.feature_geometry = feature_geometry
+        fn = _C.rasterize_gaussians_antialiased if antialiasing else _C.rasterize_gaussians
+        color, feature_map, depth, radii = _native_forward(ctx, fn, means3D, sh, colors_precomp, semantic_feature,
+                                                           opacities, scales, rotations, cov3Ds_precomp, rs,
+                                                           antialiasing)
+        return color, feature_map, radii, depth
+
+    @staticmethod
+    def backward(ctx, grad_out_color, grad_out_feature, _grad_radii, grad_depth):
+        camera = any(ctx.needs_input_grad[10:13])
+        fn = lambda *args: _C.rasterize_gaussians_backward_absgrad(  # noqa: E731
+            *args, camera=camera, semantic_feature=args[4] if ctx.feature_geometry else None,
+            antialiasing=ctx.antialiasing)
+        grads = _native_backward(ctx, fn, grad_out_color, grad_out_feature, grad_depth)
+        cam = tuple(None if g is None else g.reshape(shape) for g, shape in zip(grads[9:12], ctx.camera_shapes))
+        return grads[:9] + (grads[12],) + cam + (None, None, None)
+
+
+def _rasterize_absgrad(means3D, means2D, means2D_abs, sh, colors_precomp, semantic_feature, opacities, scales,
+                       rotations, cov3Ds_precomp, rs, feature_geometry, antialiasing=False):
+    # means2D_abs after the reference's nine inputs: _native_backward reads semantic_feature's needs_input_grad at 4
+    return _RasterizeGaussiansAbsGrad.apply(means3D, means2D, sh, colors_precomp, semantic_feature, opacities, scales,
+                                            rotations, cov3Ds_precomp, means2D_abs, rs.viewmatrix, rs.projmatrix,
+                                            rs.campos, rs, feature_geometry, antialiasing)
+
+
 def _camera_requires_grad(rs):
     return any(isinstance(t, torch.Tensor) and t.requires_grad for t in (rs.viewmatrix, rs.projmatrix, rs.campos))
 
@@ -393,6 +440,34 @@ class AlphaInvDepthGaussianRasterizer(GaussianRasterizer):
     def __init__(self, raster_settings, feature_geometry=False, antialiasing=False):
         super().__init__(raster_settings, feature_geometry)
         self.antialiasing = antialiasing
+
+
+class AbsGradGaussianRasterizer(GaussianRasterizer):
+    """GaussianRasterizer for AbsGS (Ye et al., ACM MM 2024): forward(..., means2D_abs=screenspace_points_abs) takes a
+    second [P,3] screen-space tensor that requires grad, and the backward gives it the view's per-Gaussian sums over
+    pixels of |x| and |y| of each pixel's dL/dmean2D term (third column 0), the statistic of AbsGS's split rule.  The
+    render and every other gradient are GaussianRasterizer's (AntialiasedGaussianRasterizer's with antialiasing=True);
+    with feature_geometry the feature walk's terms are summed on their own and added (see f3dgs_backward_absgrad).
+    Without means2D_abs the call is GaussianRasterizer's."""
+
+    def __init__(self, raster_settings, feature_geometry=False, antialiasing=False):
+        super().__init__(raster_settings, feature_geometry)
+        self.antialiasing = antialiasing
+        self._means2D_abs = None
+
+    def forward(self, means3D, means2D, opacities, shs=None, semantic_feature=None, colors_precomp=None,
+                scales=None, rotations=None, cov3D_precomp=None, means2D_abs=None):
+        self._means2D_abs = means2D_abs  # read by _render, which GaussianRasterizer.forward calls
+        try:
+            return super().forward(means3D, means2D, opacities, shs, semantic_feature, colors_precomp, scales,
+                                   rotations, cov3D_precomp)
+        finally:
+            self._means2D_abs = None
+
+    def _render(self, means3D, means2D, *args):
+        if self._means2D_abs is None:
+            return _rasterize(means3D, means2D, *args)
+        return _rasterize_absgrad(means3D, means2D, self._means2D_abs, *args)
 
 
 class SparseGaussianAdam(torch.optim.Adam):

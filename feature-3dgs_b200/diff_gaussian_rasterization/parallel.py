@@ -106,11 +106,17 @@ class ViewBatch:
 
     `semantic_feature` may be float16 (a float16 feature field): the forward then renders a float16 map, and the
     feature gradient still accumulates in float32, in a slot of the same shape.
+
+    absgrad=True (needs densify_stats) also accumulates AbsGS's statistic: every backward writes the view's per-Gaussian
+    sums over pixels of |x| and |y| of each pixel's dL/dmean2D term into `mean2D_abs` [P,3] and adds its norm to
+    `grad_accum_abs` [P] where radii > 0, as grad_accum gets ||dL/dmean2D|| (f3dgs_backward_accum_absgrad).
+    grad_accum_abs is a third slice of the flat buffer after denom, so all_reduce()'s collective covers it; the other
+    offsets do not move.
     """
 
     ORDER = ("semantic_feature", "opacities", "means3D", "shs", "scales", "rotations")
 
-    def __init__(self, params: dict, densify_stats: bool = True):
+    def __init__(self, params: dict, densify_stats: bool = True, absgrad: bool = False):
         from . import _C  # deferred: this module must stay importable without the extension (bench reference arm)
 
         self._C = _C
@@ -120,7 +126,9 @@ class ViewBatch:
         dev = params["means3D"].device
         self.P = P
         sizes = [self.params[k].numel() for k in self.names]
-        extra = 2 * P if densify_stats else 0
+        if absgrad and not densify_stats:
+            raise ValueError("ViewBatch: absgrad needs the densification statistics (densify_stats=True)")
+        extra = (3 if absgrad else 2) * P if densify_stats else 0
         # every view starts on a 16-byte boundary: the backward and the optimizer move the rotation gradient as float4,
         # and P, which sets the offsets, is arbitrary once densification has run
         offs, o = [], 0
@@ -133,6 +141,8 @@ class ViewBatch:
         self.early = next((s for k, s in zip(self.names, offs) if k not in ("semantic_feature", "opacities")), o)
         self.grad_accum = self.flat[o:o + P] if densify_stats else None
         self.denom = self.flat[o + P:o + 2 * P] if densify_stats else None
+        self.grad_accum_abs = self.flat[o + 2 * P:o + 3 * P] if absgrad else None
+        self.mean2D_abs = torch.zeros(P, 3, device=dev, dtype=torch.float32) if absgrad else None
         self.scratch = torch.empty(int(_C.backward_scratch_bytes(P)), dtype=torch.uint8, device=dev)
         self._empty = torch.empty(0, device=dev)
         self._side = torch.cuda.Stream(device=dev) if dev.type == "cuda" else None
@@ -204,7 +214,11 @@ class ViewBatch:
         g_alpha / g_invdepth: dL/dalpha and dL/dinvdepth [1,H,W] float32 of forward_alpha_invdepth's planes
         (f3dgs_backward_accum_alpha_invdepth; one given alone: the other is zero).  The buffers of either forward take
         them, and they combine with camera, feature_geometry and a ScaledGrad g_feature; with both None the call is the
-        one without them."""
+        one without them.
+
+        With absgrad the call goes through f3dgs_backward_accum_absgrad whatever the other options: mean2D_abs then
+        holds this view's AbsGS statistic and grad_accum_abs has its norm added; everything else is bitwise the call
+        without it."""
         rs, p, g, e = ctx.rs, self.params, self.grads, torch.Tensor([])
         none = self._empty
         scale = 1.0
@@ -219,7 +233,8 @@ class ViewBatch:
             none, means2D_out if means2D_out is not None else none,
             self.grad_accum if self.grad_accum is not None else none, self.denom if self.denom is not None else none,
             int(self._ev.cuda_event) if (last and self._ev is not None) else 0, rs.debug, float(scale), cam,
-            p.get("semantic_feature") if feature_geometry else None, ctx.antialiasing, g_alpha, g_invdepth)
+            p.get("semantic_feature") if feature_geometry else None, ctx.antialiasing, g_alpha, g_invdepth,
+            self.mean2D_abs, self.grad_accum_abs)
         self._early_pending = bool(last and self._ev is not None)
         if cam is not None:
             return CameraGrad(cam[:16].view(4, 4), cam[16:32].view(4, 4), cam[32:35])

@@ -16,7 +16,8 @@ _opacity, _scaling, _rotation, _semantic_feature`, :47-58) as plain CUDA tensors
                         flat buffer and updates the raw parameters in place -- no autograd graph anywhere;
                         step(lrs, visible=vb.visible()) is the sparse Adam step on the Gaussians the step's views saw;
   densify_and_prune()   clone / split / prune (:350-434) with the optimizer state carried along, in two native calls
-                        (f3dgs_densify_plan / f3dgs_densify_apply) with one host read in between;
+                        (f3dgs_densify_plan / f3dgs_densify_apply) with one host read in between; with absgrad=True
+                        the batch also accumulates AbsGS's statistic and densify_and_prune(abs_grad=...) splits on it;
   reset_opacity()       :231-234 in one kernel (f3dgs_reset_opacity);
   relocate_and_add()    3DGS-MCMC's fixed-budget densification (relocate_gs + add_new_gs) with the optimizer state
                         carried along (f3dgs_mcmc_plan / _relocate / _add), one host read; inject_noise() and
@@ -57,7 +58,7 @@ class GaussianState:
     NAMES = ("xyz", "f_dc", "f_rest", "opacity", "scaling", "rotation", "semantic_feature")
 
     def __init__(self, xyz, features_dc, features_rest, opacity, scaling, rotation, semantic_feature,
-                 betas=(0.9, 0.999), eps=1e-15, percent_dense=0.01, feature_dtype=torch.float32):
+                 betas=(0.9, 0.999), eps=1e-15, percent_dense=0.01, feature_dtype=torch.float32, absgrad=False):
         self.raw: Dict[str, torch.Tensor] = dict(
             xyz=xyz.contiguous(), f_dc=features_dc.contiguous(), f_rest=features_rest.contiguous(),
             opacity=opacity.contiguous(), scaling=scaling.contiguous(), rotation=rotation.contiguous(),
@@ -69,6 +70,7 @@ class GaussianState:
             raise ValueError(f"feature_dtype must be torch.float32 or torch.float16, got {feature_dtype}")
         self.betas, self.eps, self.percent_dense = betas, eps, percent_dense
         self.feature_dtype = feature_dtype
+        self.absgrad = absgrad  # the batch also accumulates AbsGS's statistic (ViewBatch(absgrad=True))
         self.filter_3d: Optional[torch.Tensor] = None  # [P,1] while the 3D filter is on
         self._filter_cameras = None
         self._reset_derived()
@@ -83,7 +85,7 @@ class GaussianState:
         three nearest neighbours)), isotropic, from the native distCUDA2 (csrc/knn.cu).  Every other field is computed
         with the reference's own tensor operations, so it is bitwise what create_from_pcd builds.  With `speedup` the
         feature width is int(semantic_feature_size / 4), as there.  Raises ValueError on mismatched shapes or a
-        non-finite coordinate.  kwargs (feature_dtype among them) go to the constructor."""
+        non-finite coordinate.  kwargs (feature_dtype and absgrad among them) go to the constructor."""
         from . import _C
 
         def as_f32(a):
@@ -152,7 +154,7 @@ class GaussianState:
 
     def batch(self) -> ViewBatch:
         if self._batch is None:
-            self._batch = ViewBatch(self.act, densify_stats=True)
+            self._batch = ViewBatch(self.act, densify_stats=True, absgrad=self.absgrad)
         return self._batch
 
     # ---------------------------------------------------------------------------------------------- optimizer
@@ -189,7 +191,8 @@ class GaussianState:
         """train.py:131, without a host sync: max_radii2D = max(max_radii2D, radii) where radii > 0."""
         self.max_radii2D = torch.where(radii > 0, torch.maximum(self.max_radii2D, radii.float()), self.max_radii2D)
 
-    def densify_and_prune(self, max_grad, min_opacity, extent, max_screen_size, grad_accum=None, denom=None, generator=None):
+    def densify_and_prune(self, max_grad, min_opacity, extent, max_screen_size, grad_accum=None, denom=None, generator=None,
+                          abs_grad=None, grad_accum_abs=None):
         """scene/gaussian_model.py:420-434 (clone :407-418, split :381-405, prune :316-330); returns the new P.
 
         With g = grad_accum / denom (0 where that is NaN) and smax the largest of exp(scaling), a Gaussian is cloned when
@@ -206,22 +209,37 @@ class GaussianState:
         reference's tensor code computes, except the split children's xyz, which agree within float rounding (the
         reference's torch.bmm has no defined summation order).
 
+        abs_grad (AbsGS's split rule, Ye et al., ACM MM 2024): with ga = grad_accum_abs / denom (0 where NaN), a
+        Gaussian is split when ga >= abs_grad and smax > percent_dense * extent; cloning and pruning are unchanged.
+        grad_accum_abs defaults to the batch's (GaussianState(absgrad=True)); ValueError when abs_grad is given and
+        there is none.  With abs_grad=None the statistic is not read and the result is that of the call without it.
+        gsplat's variant, the abs statistic for both decisions, needs no option:
+        densify_and_prune(0.0008, ..., grad_accum=vb.grad_accum_abs).
+
         Two native calls (csrc/densify.cu) and ONE host sync, the read of the four output counts that size the new
         tensors and the normal draw.  Deterministic: identical state, statistics and generator state give bitwise-
         identical output, so data-parallel replicas that densify from the same all-reduced statistics with the same seed
         stay identical."""
         from . import _C
 
-        if grad_accum is None or denom is None:
+        if grad_accum is None or denom is None or (abs_grad is not None and grad_accum_abs is None):
             vb = self.batch()
             grad_accum = vb.grad_accum if grad_accum is None else grad_accum
             denom = vb.denom if denom is None else denom
+            if abs_grad is not None and grad_accum_abs is None:
+                grad_accum_abs = vb.grad_accum_abs
             del vb
+        if abs_grad is None:
+            grad_accum_abs = None
+        elif grad_accum_abs is None:
+            raise ValueError("densify_and_prune: abs_grad needs AbsGS's statistic: pass grad_accum_abs, or build the "
+                             "state with absgrad=True")
         r = self.raw
         scratch, counts = _C.densify_plan(grad_accum, denom, r["opacity"], r["scaling"], max_grad,
                                           self.percent_dense * extent, min_opacity,
-                                          0.1 * extent if max_screen_size else math.inf)
-        del grad_accum, denom
+                                          0.1 * extent if max_screen_size else math.inf, grad_accum_abs,
+                                          0.0 if abs_grad is None else abs_grad)
+        del grad_accum, denom, grad_accum_abs
         A, B, Cc, Ns = counts.tolist()
         normals = torch.randn((2 * Ns, 3), generator=generator, device=r["xyz"].device)
         Pn = A + B + 2 * Cc

@@ -470,6 +470,61 @@ int f3dgs_backward_accum_alpha_invdepth(int P, int D, int M, int R, int C,
                                         void* composite_done_event, int debug, void* cuda_stream, float* dL_dcamera,
                                         int antialiasing, const float* dL_dalpha, const float* dL_dinvdepth);
 
+/* ---- absolute-gradient densification statistic (opt-in; AbsGS, Ye et al., ACM MM 2024; gsplat's absgrad=True) ----
+ * dL/dmean2D_i is a sum over the pixels p a view blends Gaussian i into of per-pixel terms t_ip = (t_x, t_y), in
+ * dL_dmean2D's units (the 0.5 W, 0.5 H of the reference).  Terms of opposite sign cancel there, so a large Gaussian over
+ * fine texture keeps a small ||dL/dmean2D|| and is never split ("gradient collision").  The _absgrad entries also give
+ *     dL_dmean2D_abs[i] = ( sum_p |t_x|, sum_p |t_y|, 0 )                                   [P,3] float32
+ *     grad_accum_abs[i] += sqrt(ax^2 + ay^2)   for radii_i > 0, (ax, ay) the first two columns   (accumulating entry)
+ * from the backward composite's own reduction (each parked row of 32 per-pixel terms is summed twice, once as it is and
+ * once as absolute values).  With the plane gradients t_ip includes their terms.  With the feature term of dL/dalpha
+ * (semantic_feature given, C > 0) the colour walk and the feature walk each reduce their own terms, so the statistic is
+ * sum_p |colour-walk term| + sum_p |feature-walk term|, which is AbsGS's value wherever one of the two is zero.
+ *   f3dgs_backward_absgrad / f3dgs_backward_accum_absgrad: the arguments of f3dgs_backward_alpha_invdepth /
+ *     f3dgs_backward_accum_alpha_invdepth, except that dL_dalpha and dL_dinvdepth may both be NULL (no planes; one
+ *     alone is invalid), then dL_dmean2D_abs ([P,3], required).  The assigning entry adds into dL_dmean2D_abs as it
+ *     adds into dL_dmean2D (the caller zeroes it; the third column stays 0).  The accumulating entry zeroes it itself
+ *     and leaves this view's values in it, and takes grad_accum_abs ([P], optional; it needs grad_accum and denom),
+ *     added to as grad_accum is.  Every other output is bitwise that of the counterpart entry: _alpha_invdepth with
+ *     planes, otherwise f3dgs_backward[_f16], _cam[_f16], _feature_geometry or _antialiased (and their _accum twins).
+ *   F3DGS_ERR_INVALID_ARGUMENT, before any launch, for a NULL dL_dmean2D_abs, a dL_dmean2D_abs or grad_accum_abs
+ *     overlapping another output, grad_accum_abs without grad_accum / denom, one plane alone, and whatever the
+ *     counterpart rejects. */
+int f3dgs_backward_absgrad(int P, int D, int M, int R, int C,
+                           const float* background, int width, int height,
+                           const float* means3D, const float* shs, const float* colors_precomp,
+                           const void* semantic_feature, int semantic_feature_dtype,
+                           const float* scales, float scale_modifier, const float* rotations,
+                           const float* cov3D_precomp,
+                           const float* viewmatrix, const float* projmatrix, const float* cam_pos,
+                           float tan_fovx, float tan_fovy, const int* radii,
+                           char* geom_buffer, char* binning_buffer, char* image_buffer,
+                           const float* dL_dpix, const void* dL_dfeaturepix, int dL_dfeaturepix_dtype,
+                           float dL_dfeaturepix_scale, const float* dL_depths,
+                           float* dL_dmean2D, float* dL_dconic, float* dL_dopacity, float* dL_dcolor,
+                           float* dL_dsemantic_feature, float* dL_dmean3D, float* dL_dcov3D,
+                           float* dL_dsh, float* dL_dscale, float* dL_drot, float* dL_dz,
+                           int debug, void* cuda_stream, float* dL_dcamera,
+                           int antialiasing, const float* dL_dalpha, const float* dL_dinvdepth,
+                           float* dL_dmean2D_abs);
+int f3dgs_backward_accum_absgrad(int P, int D, int M, int R, int C,
+                                 const float* background, int width, int height,
+                                 const float* means3D, const float* shs, const float* colors_precomp,
+                                 const void* semantic_feature, int semantic_feature_dtype,
+                                 const float* scales, float scale_modifier, const float* rotations,
+                                 const float* cov3D_precomp,
+                                 const float* viewmatrix, const float* projmatrix, const float* cam_pos,
+                                 float tan_fovx, float tan_fovy, const int* radii,
+                                 char* geom_buffer, char* binning_buffer, char* image_buffer,
+                                 const float* dL_dpix, const void* dL_dfeaturepix, int dL_dfeaturepix_dtype,
+                                 float dL_dfeaturepix_scale, const float* dL_depths, char* scratch,
+                                 float* dL_dopacity, float* dL_dcolors_precomp, float* dL_dsemantic_feature,
+                                 float* dL_dmean3D, float* dL_dcov3D_precomp, float* dL_dsh, float* dL_dscale,
+                                 float* dL_drot, float* dL_dmean2D_out, float* grad_accum, float* denom,
+                                 void* composite_done_event, int debug, void* cuda_stream, float* dL_dcamera,
+                                 int antialiasing, const float* dL_dalpha, const float* dL_dinvdepth,
+                                 float* dL_dmean2D_abs, float* grad_accum_abs);
+
 /* ---- feature lifting (no reference counterpart): training-free back-projection of 2-D feature maps onto Gaussians ----
  * The buffers and R are those of an f3dgs_forward / _f16 / _antialiased / _alpha_invdepth of this view at width x height
  * (any C of that forward, 0 included); feature_map [C,H,W] is a map at that resolution, 1 <= C <= F3DGS_MAX_FEATURE_DIM.
@@ -725,6 +780,13 @@ int f3dgs_knn_mean_dist(int P, const float* points, float* out, char* scratch, v
  * Both calls are stream-ordered without host sync and bitwise deterministic.  3 P must not exceed INT_MAX.
  * f3dgs_densify_scratch_bytes returns 0 for P <= 0, and 0 with f3dgs_last_error() set if the size query fails.
  *
+ * AbsGS's split rule is the same pair with another plan:
+ *   f3dgs_densify_plan_absgrad  f3dgs_densify_plan's arguments, then grad_accum_abs ([P], required; the statistic of
+ *                        f3dgs_backward_accum_absgrad) and abs_grad.  With ga = grad_accum_abs / denom (0 where NaN):
+ *                          split  ga >= abs_grad && smax > dense_scale
+ *                        clone and prune are unchanged.  (gsplat's variant, the abs statistic for both decisions, is
+ *                        f3dgs_densify_plan with grad_accum_abs in place of grad_accum.)
+ *
  * Pruning from a caller's mask is the same pair with another plan:
  *   f3dgs_prune_plan     keeps row i iff keep[i] != 0 (keep: P bytes of device memory, any nonzero byte keeps) and
  *                        writes counts = {A, 0, 0, 0}, A the rows kept.  scratch is f3dgs_densify_scratch_bytes(P)
@@ -740,6 +802,10 @@ size_t f3dgs_densify_scratch_bytes(int P);
 int f3dgs_densify_plan(int P, const float* grad_accum, const float* denom, const float* raw_opacity,
                        const float* raw_scaling, float max_grad, float dense_scale, float min_opacity,
                        float max_world_scale, char* scratch, int32_t* counts, void* cuda_stream);
+int f3dgs_densify_plan_absgrad(int P, const float* grad_accum, const float* denom, const float* raw_opacity,
+                               const float* raw_scaling, float max_grad, float dense_scale, float min_opacity,
+                               float max_world_scale, char* scratch, int32_t* counts, void* cuda_stream,
+                               const float* grad_accum_abs, float abs_grad);
 int f3dgs_densify_apply(int P, int M, int C, const char* scratch, const int32_t counts[4], const float* normals,
                         const f3dgs_gaussian_fields src[3], const f3dgs_gaussian_fields dst[3], void* cuda_stream);
 int f3dgs_prune_plan(int P, const uint8_t* keep, char* scratch, int32_t* counts, void* cuda_stream);
