@@ -1790,3 +1790,90 @@ int f3dgs_mark_visible(int P, const float* means3D, const float* viewmatrix, con
 }
 
 }  // extern "C"
+
+namespace {
+bool vq_sizes_ok(int P, int K, int D) { return P >= 0 && K >= 1 && K <= kVqMaxK && D >= 1 && D <= kVqMaxD; }
+constexpr const char* kVqBadSizes = "bad sizes (P >= 0, 1 <= K <= 65536, 1 <= D <= 4096)";
+
+// the checks shared by update and codebook_grad: < 0 the rejection, 0 nothing to do (P == 0), 1 launch
+int check_vq_reduce(const Api& api, int P, int K, int D, const float* x, const float* weights, const char* scratch,
+                    const float* out) {
+    if (!vq_sizes_ok(P, K, D)) return api.invalid(kVqBadSizes);
+    if (P == 0) return 0;
+    if (!x || !scratch || !out) return api.invalid("NULL pointer");
+    const size_t row = (size_t)D * 4;
+    const Range r[4] = {{out, (size_t)K * row}, {x, (size_t)P * row}, {weights, (size_t)P * 4},
+                        {scratch, vq_scratch_fixed_bytes(P, K)}};
+    if (any_overlap(r, 1)) return api.invalid("the output overlaps x, weights or the scratch");
+    return 1;
+}
+
+template <typename T>
+int vq_decode_impl(const char* entry, int P, int K, int D, const float* codebook, const int32_t* code, T* out,
+                   void* cuda_stream) {
+    const Api api(entry);
+    if (!vq_sizes_ok(P, K, D)) return api.invalid(kVqBadSizes);
+    if (P == 0) return 0;
+    if (!codebook || !code || !out) return api.invalid("NULL pointer");
+    const Range r[3] = {{out, (size_t)P * D * sizeof(T)}, {codebook, (size_t)K * D * 4}, {code, (size_t)P * 4}};
+    if (any_overlap(r, 1)) return api.invalid("out overlaps the codebook or code");
+    return api.cuda(launch_vq_decode(P, K, D, codebook, code, out, (cudaStream_t)cuda_stream));
+}
+}  // namespace
+
+extern "C" {
+
+size_t f3dgs_vq_scratch_bytes(int P, int K) {
+    if (K < 1 || K > kVqMaxK) return 0;
+    return scratch_bytes(__func__, [=](size_t* b) { return vq_scratch_bytes(P, K, b); });
+}
+
+int f3dgs_vq_assign(int P, int K, int D, const float* x, const float* codebook, int32_t* code, void* cuda_stream) {
+    const Api api(__func__);
+    if (!vq_sizes_ok(P, K, D)) return api.invalid(kVqBadSizes);
+    if (P == 0) return 0;
+    if (!x || !codebook || !code) return api.invalid("NULL pointer");
+    const Range r[3] = {{code, (size_t)P * 4}, {x, (size_t)P * D * 4}, {codebook, (size_t)K * D * 4}};
+    if (any_overlap(r, 1)) return api.invalid("code overlaps x or the codebook");
+    return api.cuda(launch_vq_assign(P, K, D, x, codebook, code, (cudaStream_t)cuda_stream));
+}
+
+int f3dgs_vq_plan(int P, int K, const int32_t* code, char* scratch, void* cuda_stream) {
+    const Api api(__func__);
+    if (!vq_sizes_ok(P, K, 1)) return api.invalid(kVqBadSizes);
+    if (P == 0) return 0;
+    if (!code || !scratch) return api.invalid("NULL pointer");
+    const Range r[2] = {{scratch, vq_scratch_fixed_bytes(P, K)}, {code, (size_t)P * 4}};
+    if (any_overlap(r, 1)) return api.invalid("scratch overlaps code");
+    size_t sb = 0;
+    CUDA_TRY(vq_scratch_bytes(P, K, &sb));  // the sort's share of the scratch is sized by CUB for the current device
+    if (overlaps({code, (size_t)P * 4}, {{scratch, sb}})) return api.invalid("scratch overlaps code");
+    return api.cuda(launch_vq_plan(P, K, code, scratch, (cudaStream_t)cuda_stream));
+}
+
+int f3dgs_vq_update(int P, int K, int D, const float* x, const float* weights, const char* scratch, float* codebook,
+                    void* cuda_stream) {
+    const Api api(__func__);
+    const int rc = check_vq_reduce(api, P, K, D, x, weights, scratch, codebook);
+    if (rc <= 0) return rc;
+    return api.cuda(launch_vq_reduce(P, K, D, x, weights, scratch, codebook, true, (cudaStream_t)cuda_stream));
+}
+
+int f3dgs_vq_codebook_grad(int P, int K, int D, const float* dL_dx, const char* scratch, float* dL_dcodebook,
+                           void* cuda_stream) {
+    const Api api(__func__);
+    const int rc = check_vq_reduce(api, P, K, D, dL_dx, nullptr, scratch, dL_dcodebook);
+    if (rc <= 0) return rc;
+    return api.cuda(launch_vq_reduce(P, K, D, dL_dx, nullptr, scratch, dL_dcodebook, false, (cudaStream_t)cuda_stream));
+}
+
+int f3dgs_vq_decode(int P, int K, int D, const float* codebook, const int32_t* code, float* out, void* cuda_stream) {
+    return vq_decode_impl(__func__, P, K, D, codebook, code, out, cuda_stream);
+}
+
+int f3dgs_vq_decode_f16out(int P, int K, int D, const float* codebook, const int32_t* code, uint16_t* out,
+                           void* cuda_stream) {
+    return vq_decode_impl(__func__, P, K, D, codebook, code, reinterpret_cast<__half*>(out), cuda_stream);
+}
+
+}  // extern "C"

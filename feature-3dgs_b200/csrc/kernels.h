@@ -215,6 +215,21 @@ cudaError_t launch_filter3d_apply_backward(int P, const float* opacity, const fl
 cudaError_t launch_reset_opacity_filter3d(int P, float* raw_opacity, const float* raw_scaling, const float* filter,
                                           float* exp_avg, float* exp_avg_sq, float ceiling, cudaStream_t s);
 
+// ---- vq.cu: vector quantisation, codebook [K,D] and codes [P] (include/f3dgs_b200.h: f3dgs_vq_*).  scratch (the plan) is
+// vq_scratch_bytes(P, K) bytes whose first vq_scratch_fixed_bytes(P, K) need no device query; assign and reduce take
+// their temporaries from the device's default memory pool
+constexpr int kVqMaxD = 4096, kVqMaxK = 65536;
+cudaError_t vq_scratch_bytes(int P, int K, size_t* bytes);
+size_t vq_scratch_fixed_bytes(int P, int K);
+cudaError_t launch_vq_assign(int P, int K, int D, const float* x, const float* codebook, int32_t* code, cudaStream_t s);
+cudaError_t launch_vq_plan(int P, int K, const int32_t* code, char* scratch, cudaStream_t s);
+// mean: out[k] = sum w x / sum w over the plan's rows of code k where sum w > 0 (weights NULL: all ones), other rows
+// untouched; else out[k] = sum x over those rows for every k (weights not read)
+cudaError_t launch_vq_reduce(int P, int K, int D, const float* x, const float* weights, const char* scratch, float* out,
+                             bool mean, cudaStream_t s);
+template <typename T>  // float or __half (rounded to nearest even)
+cudaError_t launch_vq_decode(int P, int K, int D, const float* codebook, const int32_t* code, T* out, cudaStream_t s);
+
 // ---- optimizer.cu: activation prologue and fused Adam step (include/f3dgs_b200.h: f3dgs_activate / f3dgs_adam_step)
 cudaError_t launch_activate(int P, int M, const float* raw_opacity, const float* raw_scaling, const float* raw_rotation,
                             const float* features_dc, const float* features_rest, float* opacity, float* scales,

@@ -1338,6 +1338,111 @@ void resetOpacityFilter3d(torch::Tensor raw_opacity, const torch::Tensor& raw_sc
              "f3dgs_reset_opacity_filter3d");
 }
 
+// ---- vector quantisation (f3dgs_vq_*): x [P,D] rows, codebook [K,D], code int32 [P]
+namespace {
+// a float32 matrix [rows, D] on a CUDA device, made contiguous; rows and D must fit an int (the C ABI checks D)
+torch::Tensor vq_matrix(const torch::Tensor& t, const char* name) {
+    TORCH_CHECK(t.is_cuda(), name, " must be a CUDA tensor (this build has no CPU path)");
+    TORCH_CHECK(t.scalar_type() == torch::kFloat32, name, " must be float32 (got ", t.scalar_type(), ")");
+    TORCH_CHECK(t.dim() == 2 && t.size(0) <= INT32_MAX && t.size(1) <= INT32_MAX, name, " must be a [rows, D] matrix");
+    return t.contiguous();
+}
+}  // namespace
+
+// x [P,D], codebook [K,D] -> code int32 [P]
+torch::Tensor vqAssign(const torch::Tensor& x, const torch::Tensor& codebook) {
+    const torch::Tensor xc = vq_matrix(x, "x"), cc = vq_matrix(codebook, "codebook");
+    TORCH_CHECK(xc.dim() == 2 && cc.dim() == 2 && xc.size(1) == cc.size(1) && xc.device() == cc.device(),
+                "vq_assign: x must be [P,D] and codebook [K,D] on one device");
+    const c10::cuda::CUDAGuard guard(xc.device());
+    torch::Tensor code = torch::empty({xc.size(0)}, xc.options().dtype(torch::kInt32));
+    cudaStream_t stream = c10::cuda::getCurrentCUDAStream().stream();
+    check_rc(f3dgs_vq_assign((int)xc.size(0), (int)cc.size(0), (int)xc.size(1), fptr(xc), fptr(cc),
+                             code.numel() ? code.data_ptr<int32_t>() : nullptr, (void*)stream),
+             "f3dgs_vq_assign");
+    return code;
+}
+
+// code int32 [P] -> the plan (a uint8 scratch tensor)
+torch::Tensor vqPlan(const torch::Tensor& code, int64_t K) {
+    TORCH_CHECK(code.is_cuda() && code.scalar_type() == torch::kInt32 && code.dim() == 1 && code.is_contiguous() &&
+                    code.numel() <= INT32_MAX,
+                "vq_plan: code must be a contiguous 1-D int32 CUDA tensor");
+    TORCH_CHECK(K >= 1 && K <= 65536, "vq_plan: K must be in [1, 65536]");
+    const c10::cuda::CUDAGuard guard(code.device());
+    const int P = (int)code.numel();
+    torch::Tensor scratch = scratch_tensor(f3dgs_vq_scratch_bytes(P, (int)K), "f3dgs_vq_scratch_bytes", code);
+    cudaStream_t stream = c10::cuda::getCurrentCUDAStream().stream();
+    check_rc(f3dgs_vq_plan(P, (int)K, P ? code.data_ptr<int32_t>() : nullptr,
+                           scratch.numel() ? reinterpret_cast<char*>(scratch.data_ptr()) : nullptr, (void*)stream),
+             "f3dgs_vq_plan");
+    return scratch;
+}
+
+// codebook [K,D] updated in place (contiguous float32) from x [P,D] over the plan of the codes; weights [P] or None
+void vqUpdate(const torch::Tensor& x, const c10::optional<torch::Tensor>& weights, const torch::Tensor& scratch,
+              torch::Tensor codebook) {
+    const torch::Tensor xc = vq_matrix(x, "x");
+    TORCH_CHECK(xc.dim() == 2 && codebook.dim() == 2 && codebook.size(1) == xc.size(1),
+                "vq_update: x must be [P,D] and codebook [K,D]");
+    const auto dev = xc.device();
+    const c10::cuda::CUDAGuard guard(dev);
+    const int64_t P = xc.size(0), K = codebook.size(0), D = xc.size(1);
+    float* cb = in_place(codebook, dev, K * D, "codebook");
+    torch::Tensor w;
+    if (weights.has_value() && weights->defined()) {
+        w = input(*weights, dev, "weights");
+        TORCH_CHECK(w.numel() == P, "vq_update: weights must have P elements");
+    }
+    cudaStream_t stream = c10::cuda::getCurrentCUDAStream().stream();
+    check_rc(f3dgs_vq_update((int)P, (int)K, (int)D, fptr(xc), w.defined() ? fptr(w) : nullptr,
+                             scratch_ptr(scratch), cb, (void*)stream),
+             "f3dgs_vq_update");
+}
+
+// dL_dx [P,D] -> dL_dcodebook [K,D] over the plan of the codes
+torch::Tensor vqCodebookGrad(const torch::Tensor& dL_dx, const torch::Tensor& scratch, int64_t K) {
+    const torch::Tensor g = vq_matrix(dL_dx, "dL_dx");
+    TORCH_CHECK(g.dim() == 2, "vq_codebook_grad: dL_dx must be [P,D]");
+    const c10::cuda::CUDAGuard guard(g.device());
+    torch::Tensor out = torch::empty({K, g.size(1)}, g.options());
+    if (g.size(0) == 0) return out.zero_();
+    cudaStream_t stream = c10::cuda::getCurrentCUDAStream().stream();
+    check_rc(f3dgs_vq_codebook_grad((int)g.size(0), (int)K, (int)g.size(1), fptr(g), scratch_ptr(scratch),
+                                    out.numel() ? out.data_ptr<float>() : nullptr, (void*)stream),
+             "f3dgs_vq_codebook_grad");
+    return out;
+}
+
+// codebook [K,D], code int32 [P] -> [P,D] float32, or float16 (half_rn) with `half`; out (optional) is written instead
+torch::Tensor vqDecode(const torch::Tensor& codebook, const torch::Tensor& code, bool half,
+                       const c10::optional<torch::Tensor>& out) {
+    const torch::Tensor cc = vq_matrix(codebook, "codebook");
+    TORCH_CHECK(cc.dim() == 2, "vq_decode: codebook must be [K,D]");
+    const auto dev = cc.device();
+    const c10::cuda::CUDAGuard guard(dev);
+    const int32_t* ci = indices(code, dev, "code");
+    const int64_t P = code.numel(), K = cc.size(0), D = cc.size(1);
+    const auto dtype = half ? torch::kFloat16 : torch::kFloat32;
+    torch::Tensor o;
+    if (out.has_value() && out->defined()) {
+        o = *out;
+        TORCH_CHECK(o.device() == dev && o.scalar_type() == dtype && o.is_contiguous() && o.numel() == P * D,
+                    "vq_decode: out must be a contiguous tensor of P D elements of the output dtype on ", dev);
+    } else {
+        o = torch::empty({P, D}, cc.options().dtype(dtype));
+    }
+    cudaStream_t stream = c10::cuda::getCurrentCUDAStream().stream();
+    if (half)
+        check_rc(f3dgs_vq_decode_f16out((int)P, (int)K, (int)D, fptr(cc), ci,
+                                        P ? reinterpret_cast<uint16_t*>(o.data_ptr<at::Half>()) : nullptr, (void*)stream),
+                 "f3dgs_vq_decode_f16out");
+    else
+        check_rc(f3dgs_vq_decode((int)P, (int)K, (int)D, fptr(cc), ci, P ? o.data_ptr<float>() : nullptr, (void*)stream),
+                 "f3dgs_vq_decode");
+    return o;
+}
+
 // ---- activation prologue + fused optimizer step (f3dgs_activate / f3dgs_adam_step): in-place on the caller's tensors
 void activateParams(const torch::Tensor& raw_opacity, const torch::Tensor& raw_scaling, const torch::Tensor& raw_rotation,
                     const torch::Tensor& f_dc, const torch::Tensor& f_rest, torch::Tensor opacity, torch::Tensor scales,
@@ -1527,6 +1632,13 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
           pybind11::arg("dL_dopacity") = pybind11::none(), pybind11::arg("dL_dscales") = pybind11::none());
     m.def("reset_opacity_filter3d", &resetOpacityFilter3d, pybind11::arg("raw_opacity"), pybind11::arg("raw_scaling"),
           pybind11::arg("filter"), pybind11::arg("exp_avg"), pybind11::arg("exp_avg_sq"), pybind11::arg("ceiling") = 0.01);
+    m.def("vq_assign", &vqAssign, pybind11::arg("x"), pybind11::arg("codebook"));
+    m.def("vq_plan", &vqPlan, pybind11::arg("code"), pybind11::arg("K"));
+    m.def("vq_update", &vqUpdate, pybind11::arg("x"), pybind11::arg("weights"), pybind11::arg("scratch"),
+          pybind11::arg("codebook"));
+    m.def("vq_codebook_grad", &vqCodebookGrad, pybind11::arg("dL_dx"), pybind11::arg("scratch"), pybind11::arg("K"));
+    m.def("vq_decode", &vqDecode, pybind11::arg("codebook"), pybind11::arg("code"), pybind11::arg("half") = false,
+          pybind11::arg("out") = pybind11::none());
     m.def("activate", &activateParams);
     m.def("adam_step", &adamStep, pybind11::arg("kind"), pybind11::arg("param"), pybind11::arg("grad_activated"),
           pybind11::arg("exp_avg"), pybind11::arg("exp_avg_sq"), pybind11::arg("M"), pybind11::arg("lr"),

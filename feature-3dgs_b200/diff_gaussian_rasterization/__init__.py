@@ -62,6 +62,11 @@ Behavioural notes
     are GaussianRasterizer's (AntialiasedGaussianRasterizer's with antialiasing).  `ViewBatch(absgrad=True)` and
     `GaussianState(absgrad=True)` accumulate the statistic natively, and `densify_and_prune(abs_grad=...)` applies
     the split rule.
+  * vector-quantised feature fields (LightGaussian, CompGS): `kmeans(x, K)` fits a codebook [K,D] and int32 codes on the
+    GPU (a TF32 tensor-core assignment with the argmin fused into the GEMM, float64 segment means), `decode(codebook,
+    code)` gathers the rows back (float32 or float16), and `CodePlan(code, K)` gives the codebook gradient of the
+    gather.  `GaussianState.quantize_features(K)` trains the codebook in place of per-Gaussian features, and io.save_ply
+    stores it with one ushort code per Gaussian.
   * `debug=True` keeps the reference semantics: arguments are snapshotted to CPU first and dumped
     to snapshot_fw.dump / snapshot_bw.dump if the native call raises (reference :89-97,:147-155);
     natively it synchronises and checks after every stage.
@@ -83,6 +88,7 @@ except ImportError as exc:  # pragma: no cover - exercised only on a broken inst
     ) from exc
 
 from .filter3d import apply_3d_filter, compute_3d_filter  # noqa: E402
+from .codebook import CodePlan, decode, kmeans  # noqa: E402
 from .scores import GaussianScores  # noqa: E402
 
 __all__ = [
@@ -98,6 +104,9 @@ __all__ = [
     "apply_3d_filter",
     "GaussianScores",
     "AbsGradGaussianRasterizer",
+    "kmeans",
+    "decode",
+    "CodePlan",
 ]
 
 

@@ -28,7 +28,11 @@ _opacity, _scaling, _rotation, _semantic_feature`, :47-58) as plain CUDA tensors
                         gives the parameters with the filter folded in, for export;
   prune(keep)           removes the rows a mask drops, with the optimizer state carried along (f3dgs_prune_plan /
                         f3dgs_densify_apply), one host read; prune_by_importance() drops the lowest blend-weight
-                        scores (scores.GaussianScores), LightGaussian's rule.
+                        scores (scores.GaussianScores), LightGaussian's rule;
+  quantize_features()   LightGaussian's / CompGS's vector quantisation of the feature field (codebook.kmeans): the state
+                        then trains a codebook [K,C] in place of per-Gaussian features, activate() decodes codebook[code]
+                        for the rasterizer and step() takes the codebook gradient of that gather; dequantize() returns
+                        to per-Gaussian features.
 
 Float16 feature fields: with feature_dtype=torch.float16 the rasterizer reads a float16 working copy
 act["semantic_feature"] of the float32 master raw["semantic_feature"], so every view renders a float16 map and the feature
@@ -73,6 +77,10 @@ class GaussianState:
         self.absgrad = absgrad  # the batch also accumulates AbsGS's statistic (ViewBatch(absgrad=True))
         self.filter_3d: Optional[torch.Tensor] = None  # [P,1] while the 3D filter is on
         self._filter_cameras = None
+        # quantised features (quantize_features): codebook [K,C] with its own Adam state, code [P] int32 and its plan
+        self.codebook: Optional[torch.Tensor] = None
+        self.code: Optional[torch.Tensor] = None
+        self._code_plan = None
         self._reset_derived()
 
     @classmethod
@@ -130,19 +138,23 @@ class GaussianState:
             self.steps = {k: 0 for k in self.raw}
         self.max_radii2D = torch.zeros(P, device=dev)
         sf = self.raw["semantic_feature"]
+        if self.code is not None:  # the decoded field, rewritten by every activate()
+            sf = self._decode_features()
         self.act = dict(means3D=self.raw["xyz"], opacities=torch.empty(P, 1, device=dev), scales=torch.empty(P, 3, device=dev),
                         rotations=torch.empty(P, 4, device=dev), shs=torch.empty(P, self.M, 3, device=dev),
-                        semantic_feature=sf if self.feature_dtype == torch.float32 else sf.to(self.feature_dtype))
+                        semantic_feature=sf if sf.dtype == self.feature_dtype else sf.to(self.feature_dtype))
         self._batch: Optional[ViewBatch] = None
         self._unfiltered = None  # the unfiltered opacity [P,1] and scales [P,3] while the 3D filter is on
 
     def activate(self):
         """The activated tensors the rasterizer reads (self.act), from the raw parameters.  With the 3D filter on,
         act["opacities"] and act["scales"] hold the filtered values (apply_3d_filter) and the unfiltered ones are kept
-        for step()."""
+        for step().  With quantised features, act["semantic_feature"] is rewritten with codebook[code]."""
         from . import _C
 
         a, r = self.act, self.raw
+        if self.code is not None:
+            self._decode_features(a["semantic_feature"])
         if self.filter_3d is None:
             _C.activate(r["opacity"], r["scaling"], r["rotation"], r["f_dc"], r["f_rest"], a["opacities"], a["scales"],
                         a["rotations"], a["shs"])
@@ -167,6 +179,10 @@ class GaussianState:
         change, bitwise as in the dense step; the others stay exactly as they are, so momentum no longer moves Gaussians
         that no view of the step saw.  Bias correction still uses each group's step count, which advances every step.
 
+        With quantised features the codebook takes a dense step (a code is shared by rows in and out of view) from the
+        exact gradient of the gather, the per-code sum of grads["semantic_feature"] (CodePlan.grad), with its own
+        moments and step count.
+
         With the 3D filter on, `grads` holds the gradients w.r.t. the filtered opacity and scales; they are turned into
         those w.r.t. the unfiltered ones of the last activate(), in place (f3dgs_filter3d_apply_backward), first."""
         from . import _C
@@ -175,6 +191,11 @@ class GaussianState:
         if self.filter_3d is not None:
             o, s = self._unfiltered
             _C.filter3d_apply_backward(o, s, self.filter_3d, g["opacities"], g["scales"], g["opacities"], g["scales"])
+        if self.code is not None:
+            self.codebook_steps += 1
+            _C.adam_step(KIND["semantic_feature"], self.codebook, self._code_plan.grad(g["semantic_feature"]),
+                         self.codebook_exp_avg, self.codebook_exp_avg_sq, self.M, lrs["semantic_feature"], self.betas[0],
+                         self.betas[1], self.eps, self.codebook_steps, None, None)
         for name in self.NAMES:
             p = self.raw[name]
             if p.numel() == 0:
@@ -222,6 +243,7 @@ class GaussianState:
         stay identical."""
         from . import _C
 
+        self._refuse_quantized("densify_and_prune")
         if grad_accum is None or denom is None or (abs_grad is not None and grad_accum_abs is None):
             vb = self.batch()
             grad_accum = vb.grad_accum if grad_accum is None else grad_accum
@@ -260,8 +282,9 @@ class GaussianState:
 
         Every raw field and its exp_avg and exp_avg_sq become bitwise t[keep], in order; `steps` is unchanged, the
         float16 feature copy is bitwise raw.half() and max_radii2D is compacted with the rows, as the reference's
-        prune_points does.  The ViewBatch is rebuilt, and the 3D filter, when on, is recomputed for the new means (its
-        own host read).  Per-row statistics the caller keeps (densification statistics, scores) are the caller's to
+        prune_points does.  With quantised features the codes are compacted the same way (the codebook is unchanged)
+        and their plan rebuilt, without another host read.  The ViewBatch is rebuilt, and the 3D filter, when on, is
+        recomputed for the new means (its own host read).  Per-row statistics the caller keeps (densification statistics, scores) are the caller's to
         index with `keep`.
 
         Two native calls (csrc/densify.cu: the mask plan, then densify_apply's compaction) and ONE host read, the
@@ -280,8 +303,12 @@ class GaussianState:
         # max_radii2D's new position: the rank among the kept rows, slot A for the dropped ones
         rank = torch.cumsum(keep, 0, dtype=torch.int64) - 1
         A = int(counts[0])
-        radii = torch.empty(A + 1, device=dev).scatter_(0, torch.where(keep, rank, A), self.max_radii2D)[:A]
-        del rank
+        slot = torch.where(keep, rank, A)
+        radii = torch.empty(A + 1, device=dev).scatter_(0, slot, self.max_radii2D)[:A]
+        if self.code is not None:
+            self.code = torch.empty(A + 1, dtype=torch.int32, device=dev).scatter_(0, slot, self.code)[:A].contiguous()
+            self._code_plan = None
+        del rank, slot
         groups = (self.raw, self.exp_avg, self.exp_avg_sq)
         r = self.raw
         new = [{k: torch.empty((A,) + r[k].shape[1:], device=dev) for k in self.NAMES} for _ in groups]
@@ -290,6 +317,10 @@ class GaussianState:
         del r, groups, scratch
         self.raw, self.exp_avg, self.exp_avg_sq = new
         del new
+        if self.code is not None:
+            from .codebook import CodePlan
+
+            self._code_plan = CodePlan(self.code, self.codebook.shape[0])
         self._reset_derived(keep_optimizer_state=True)
         self.max_radii2D = radii
         if self.filter_3d is not None:
@@ -330,6 +361,83 @@ class GaussianState:
                                       self.exp_avg_sq["opacity"])
             return
         _C.reset_opacity(r["opacity"], self.exp_avg["opacity"], self.exp_avg_sq["opacity"])
+
+    # ---------------------------------------------------------------------------------------------- quantised features
+    def quantize_features(self, K: int, iters: int = 10, weights: Optional[torch.Tensor] = None, generator=None):
+        """Replace the per-Gaussian features by a k-means codebook [K,C] and one code per Gaussian (LightGaussian's and
+        CompGS's vector quantisation; codebook.kmeans on raw["semantic_feature"], `iters` rounds, seeded by
+        `generator`).  weights=scores.weight_sum (scores.GaussianScores) weights each Gaussian by how much it renders.
+
+        Afterwards self.codebook [K,C] is trained with its own exp_avg, exp_avg_sq and step count, self.code [P] int32
+        stays fixed, and raw["semantic_feature"] with its two moments is released (kept as [P,1,0]).  activate() decodes
+        codebook[code] into act["semantic_feature"] (float16 with feature_dtype=torch.float16, half_rn of the float32
+        codebook), so ViewBatch, the rasterizer and the feature losses are unchanged; step() trains the codebook (see
+        step()).  prune() carries the codes; densify_and_prune and relocate_and_add raise ValueError, as they would need a
+        code for every new row.  dequantize() goes back.
+
+        Returns the bytes held for the feature field before and after (dict before=, after=): the per-row features,
+        their moments and working copy before; the codebook, its moments, the codes, their plan and the decoded field
+        after.  ValueError when already quantised, without features (C == 0), or from kmeans (K > P, bad weights)."""
+        from .codebook import CodePlan, kmeans
+
+        if self.code is not None:
+            raise ValueError("quantize_features: the features are already quantised")
+        P, sf = self.P, self.raw["semantic_feature"]
+        C = sf.shape[-1]
+        if C == 0:
+            raise ValueError("quantize_features: the state has no features (C == 0)")
+        before = self._feature_bytes()
+        codebook, code = kmeans(sf.reshape(P, C), K, iters=iters, weights=weights, generator=generator)
+        self.codebook, self.code, self._code_plan = codebook, code, CodePlan(code, K)
+        self.codebook_exp_avg, self.codebook_exp_avg_sq = torch.zeros_like(codebook), torch.zeros_like(codebook)
+        self.codebook_steps = 0
+        del sf
+        for group in (self.raw, self.exp_avg, self.exp_avg_sq):
+            group["semantic_feature"] = torch.empty(P, 1, 0, device=codebook.device)
+        radii = self.max_radii2D
+        self._reset_derived(keep_optimizer_state=True)
+        self.max_radii2D = radii
+        return dict(before=before, after=self._feature_bytes())
+
+    def dequantize(self):
+        """Back to per-Gaussian features: raw["semantic_feature"] = codebook[code] as [P,1,C] float32, with zero Adam
+        moments and step count; the codebook, its state and the codes are dropped."""
+        if self.code is None:
+            raise ValueError("dequantize: the features are not quantised")
+        from .codebook import decode
+
+        P = self.P
+        sf = decode(self.codebook, self.code).reshape(P, 1, -1)
+        self.raw["semantic_feature"] = sf
+        self.exp_avg["semantic_feature"] = torch.zeros_like(sf)
+        self.exp_avg_sq["semantic_feature"] = torch.zeros_like(sf)
+        self.steps["semantic_feature"] = 0
+        self.codebook = self.code = self._code_plan = None
+        self.codebook_exp_avg = self.codebook_exp_avg_sq = None
+        radii = self.max_radii2D
+        self._reset_derived(keep_optimizer_state=True)
+        self.max_radii2D = radii
+
+    def _decode_features(self, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """codebook[code] as [P,1,C] of feature_dtype, written into `out` when given"""
+        from .codebook import decode
+
+        P, C = self.P, self.codebook.shape[1]
+        return decode(self.codebook, self.code, self.feature_dtype, out=out).view(P, 1, C)
+
+    def _feature_bytes(self) -> int:
+        """bytes of the distinct tensors that hold the feature field and its optimizer state"""
+        ts = [self.raw["semantic_feature"], self.exp_avg["semantic_feature"], self.exp_avg_sq["semantic_feature"],
+              self.act["semantic_feature"]]
+        if self.code is not None:
+            ts += [self.codebook, self.codebook_exp_avg, self.codebook_exp_avg_sq, self.code, self._code_plan.scratch]
+        seen = {t.data_ptr(): t.numel() * t.element_size() for t in ts if t.numel()}
+        return sum(seen.values())
+
+    def _refuse_quantized(self, what: str):
+        if self.code is not None:
+            raise ValueError(f"{what}: not available while the features are quantised (new rows would need codes); "
+                             "call dequantize() first")
 
     # ---------------------------------------------------------------------------------------------- 3D filter
     def compute_3d_filter(self, cameras=None):
@@ -385,6 +493,7 @@ class GaussianState:
         torch's deterministic algorithms enabled (see _multinomial), so data-parallel replicas stay identical."""
         from . import _C
 
+        self._refuse_quantized("relocate_and_add")
         P, r = self.P, self.raw
         if P == 0:
             return 0, 0

@@ -902,6 +902,53 @@ int f3dgs_filter3d_apply_backward(int P, const float* opacity, const float* scal
 int f3dgs_reset_opacity_filter3d(int P, float* raw_opacity, const float* raw_scaling, const float* filter,
                                  float* exp_avg, float* exp_avg_sq, float ceiling, void* cuda_stream);
 
+/* ---- vector quantisation: k-means codebooks of per-row features (LightGaussian, NeurIPS 2024; CompGS, ECCV 2024) ----
+ * Rows x [P,D] float32, a codebook c [K,D] float32 and codes code [P] int32, all row-major.  1 <= D <= 4096,
+ * 1 <= K <= 65536, P >= 0; P == 0 launches nothing.
+ *   f3dgs_vq_assign      code[i] = argmin_k (||c_k||^2 - 2 x_i . c_k).  The products run on the tensor cores in TF32:
+ *                        x and c rounded to nearest (cvt.rna), fp32 accumulation, as f3dgs_feature_query; ||c_k||^2 is
+ *                        summed in fp32 from the unrounded codebook.  Ties go to the lower index.  A NaN score loses to
+ *                        every number, so a row whose scores are all NaN (a NaN in x) gets code 0.  Only the codes reach
+ *                        memory.  Error bound: with d(x, c) = ||x - c||^2 in exact arithmetic on the float32 inputs,
+ *                        cmax = max_k ||c_k||, u = 2^-11 (TF32 rounding) and g = (D + 8) 2^-22 (the fp32 sums of D
+ *                        terms as the tensor cores form them, products exact and each k8 block added with alignment
+ *                        and truncation; the norm sum; the final subtraction), every row satisfies
+ *                          d(x, c_code) - min_k d(x, c_k) <= (4 (2u + u^2) + 4 g (1 + u)^2) ||x|| cmax + 2 g cmax^2
+ *                        i.e. (2^-8 + 2^-20 + 4 g (1 + 2^-11)^2) ||x|| cmax + 2 g cmax^2: twice (for the chosen code and
+ *                        the best one) the rounding of two products x . c (Cauchy-Schwarz) plus the fp32 sums.  code
+ *                        must not overlap x or the codebook.  The rounded codebook (K D floats, padded) comes from the
+ *                        device's default memory pool.
+ *   f3dgs_vq_plan        a stable sort of the row indices by code and the segment offsets of each code, written to
+ *                        scratch (f3dgs_vq_scratch_bytes(P, K) bytes of device memory, 256-byte aligned).  The plan stays
+ *                        valid while the codes do not change: update and codebook_grad only read it.  A code outside
+ *                        [0, K) is detected on the device: every update or codebook_grad over that plan then writes
+ *                        nothing.  scratch must not overlap code.
+ *   f3dgs_vq_update      in place: c_k = sum w_i x_i / sum w_i over the plan's rows of code k, the sums in double,
+ *                        rounded once; weights [P] (NULL: all ones) must be finite and >= 0: otherwise (checked on the
+ *                        device before any write) the call writes nothing.  A code with zero total weight keeps its row
+ *                        bitwise.
+ *   f3dgs_vq_codebook_grad  dL_dcodebook[k] = sum dL_dx_i over the plan's rows of code k, in double, rounded once,
+ *                        written (0 for an empty code): the chain rule of decode's gather.
+ *   Both reductions use no float atomics and a fixed order (set by P and the codes), and spread every code's rows over
+ *   CTAs of at most 512 rows, one code holding every row included.  Their partial sums (8 D (P / 256 + 1) bytes) come
+ *   from the device's default memory pool.  codebook (update) and dL_dcodebook must not overlap an input or the scratch.
+ *   f3dgs_vq_decode      out[i, :] = c[code[i], :], float32; f3dgs_vq_decode_f16out writes the IEEE binary16 bits of
+ *                        half_rn(c[code[i], :]), bitwise torch's c.half()[code].  A code outside [0, K) decodes to a NaN
+ *                        row.  out must not overlap the codebook or code.
+ * F3DGS_ERR_INVALID_ARGUMENT, before any CUDA call, for sizes out of range, a NULL pointer (with P > 0) or an overlap.
+ * Stream-ordered without host sync; every result is bitwise reproducible.  f3dgs_vq_scratch_bytes returns 0 for P <= 0
+ * or K out of range, and 0 with f3dgs_last_error() set if the size query fails. */
+size_t f3dgs_vq_scratch_bytes(int P, int K);
+int f3dgs_vq_assign(int P, int K, int D, const float* x, const float* codebook, int32_t* code, void* cuda_stream);
+int f3dgs_vq_plan(int P, int K, const int32_t* code, char* scratch, void* cuda_stream);
+int f3dgs_vq_update(int P, int K, int D, const float* x, const float* weights, const char* scratch, float* codebook,
+                    void* cuda_stream);
+int f3dgs_vq_codebook_grad(int P, int K, int D, const float* dL_dx, const char* scratch, float* dL_dcodebook,
+                           void* cuda_stream);
+int f3dgs_vq_decode(int P, int K, int D, const float* codebook, const int32_t* code, float* out, void* cuda_stream);
+int f3dgs_vq_decode_f16out(int P, int K, int D, const float* codebook, const int32_t* code, uint16_t* out,
+                           void* cuda_stream);
+
 /* ---- markVisible: reference rasterizer_impl.cu:141-153 (checkFrustum :54-66) --------------
  * present[i] = (view-space z of means3D[i] > 0.2).  `present` is P bytes (0/1). */
 int f3dgs_mark_visible(int P, const float* means3D, const float* viewmatrix,
