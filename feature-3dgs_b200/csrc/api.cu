@@ -1877,3 +1877,88 @@ int f3dgs_vq_decode_f16out(int P, int K, int D, const float* codebook, const int
 }
 
 }  // extern "C"
+
+namespace {
+bool knn_graph_sizes_ok(int P, int k) { return P >= 0 && k >= 1 && k <= 32 && (long long)P * k <= INT_MAX; }
+constexpr const char* kKnnGraphBadSizes = "bad sizes (P >= 0, 1 <= k <= 32, P k <= 2^31 - 1)";
+}  // namespace
+
+extern "C" {
+
+size_t f3dgs_knn_graph_scratch_bytes(int P, int k) {
+    if (!knn_graph_sizes_ok(P, k)) return 0;
+    return scratch_bytes(__func__, [=](size_t* b) { return knn_graph_scratch_bytes(P, k, b); });
+}
+
+int f3dgs_knn_graph(int P, int k, const float* points, int32_t* idx, float* dist2, int32_t* order, char* scratch,
+                    void* cuda_stream) {
+    const Api api(__func__);
+    if (!knn_graph_sizes_ok(P, k)) return api.invalid(kKnnGraphBadSizes);
+    if (P == 0) return 0;
+    if (!points || !idx || !dist2 || !order || !scratch) return api.invalid("NULL pointer");
+    const size_t E = (size_t)P * k;
+    Range r[5] = {{idx, E * 4}, {dist2, E * 4}, {order, (size_t)P * 4}, {points, (size_t)P * 12},
+                  {scratch, knn_graph_scratch_fixed_bytes(P, k)}};
+    if (any_overlap(r, 3)) return api.invalid("idx, dist2 and order overlap each other, points or scratch");
+    size_t sb = 0;
+    CUDA_TRY(knn_graph_scratch_bytes(P, k, &sb));  // the sorts' share of the scratch is sized by CUB for the device
+    r[4].bytes = sb;
+    if (any_overlap(r, 3)) return api.invalid("idx, dist2 and order overlap each other, points or scratch");
+    return api.cuda(launch_knn_graph(P, k, points, idx, dist2, order, scratch, (cudaStream_t)cuda_stream));
+}
+
+int f3dgs_knn_reverse(int P, int k, const int32_t* idx, int32_t* offsets, int32_t* sources, char* scratch,
+                      void* cuda_stream) {
+    const Api api(__func__);
+    if (!knn_graph_sizes_ok(P, k)) return api.invalid(kKnnGraphBadSizes);
+    if (P == 0) return 0;
+    if (!idx || !offsets || !sources || !scratch) return api.invalid("NULL pointer");
+    const size_t E = (size_t)P * k;
+    Range r[4] = {{offsets, ((size_t)P + 1) * 4}, {sources, E * 4}, {idx, E * 4},
+                  {scratch, knn_graph_scratch_fixed_bytes(P, k)}};
+    if (any_overlap(r, 2)) return api.invalid("offsets and sources overlap each other, idx or scratch");
+    size_t sb = 0;
+    CUDA_TRY(knn_graph_scratch_bytes(P, k, &sb));
+    r[3].bytes = sb;
+    if (any_overlap(r, 2)) return api.invalid("offsets and sources overlap each other, idx or scratch");
+    return api.cuda(launch_knn_reverse(P, k, idx, offsets, sources, scratch, (cudaStream_t)cuda_stream));
+}
+
+int f3dgs_feature_tv_accum(int P, int k, int C, const float* features, const int32_t* idx, const int32_t* offsets,
+                           const int32_t* sources, const int32_t* order, double weight, long long n_edges, float* grad,
+                           double* loss, void* cuda_stream) {
+    const Api api(__func__);
+    if (!knn_graph_sizes_ok(P, k) || C < 1 || C > F3DGS_MAX_FEATURE_DIM || n_edges < 0 || n_edges > (long long)P * k)
+        return api.invalid("bad sizes (P >= 0, 1 <= k <= 32, P k <= 2^31 - 1, 1 <= C <= F3DGS_MAX_FEATURE_DIM, "
+                           "0 <= n_edges <= P k)");
+    if (!std::isfinite(weight)) return api.invalid("weight must be finite");
+    if (P == 0) return 0;
+    if (!features || !idx || !offsets || !sources || !grad || !loss) return api.invalid("NULL pointer");
+    const size_t E = (size_t)P * k, row = (size_t)C * 4;
+    const Range r[7] = {{grad, (size_t)P * row}, {loss, 8}, {features, (size_t)P * row}, {idx, E * 4},
+                        {offsets, ((size_t)P + 1) * 4}, {sources, E * 4}, {order, (size_t)P * 4}};
+    if (any_overlap(r, 2)) return api.invalid("grad and loss overlap each other or an input");
+    const cudaError_t e = launch_feature_tv_accum(P, k, C, features, idx, offsets, sources, order, weight, n_edges,
+                                                  grad, loss, (cudaStream_t)cuda_stream);
+    if (e == cudaErrorMemoryAllocation)
+        return api.fail(F3DGS_ERR_ALLOC, std::string("cudaMallocAsync for the partial sums failed: ") +
+                                             cudaGetErrorString(e));
+    return api.cuda(e);
+}
+
+int f3dgs_feature_fill(int P, int k, int C, const float* features, const float* weights, const int32_t* idx,
+                       float min_weight, float* out, void* cuda_stream) {
+    const Api api(__func__);
+    if (!knn_graph_sizes_ok(P, k) || C < 1 || C > F3DGS_MAX_FEATURE_DIM)
+        return api.invalid("bad sizes (P >= 0, 1 <= k <= 32, P k <= 2^31 - 1, 1 <= C <= F3DGS_MAX_FEATURE_DIM)");
+    if (std::isnan(min_weight)) return api.invalid("min_weight must not be NaN");
+    if (P == 0) return 0;
+    if (!features || !weights || !idx || !out) return api.invalid("NULL pointer");
+    const size_t row = (size_t)C * 4;
+    const Range r[4] = {{out, (size_t)P * row}, {features, (size_t)P * row}, {weights, (size_t)P * 4},
+                        {idx, (size_t)P * k * 4}};
+    if (any_overlap(r, 1)) return api.invalid("out overlaps features, weights or idx");
+    return api.cuda(launch_feature_fill(P, k, C, features, weights, idx, min_weight, out, (cudaStream_t)cuda_stream));
+}
+
+}  // extern "C"

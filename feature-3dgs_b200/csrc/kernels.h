@@ -168,6 +168,23 @@ cudaError_t launch_pca_image(int C, int N, const X* x, const float* mean, const 
 cudaError_t knn_scratch_bytes(int P, size_t* bytes);
 size_t knn_scratch_fixed_bytes(int P);
 cudaError_t launch_knn_mean_dist(int P, const float* points, float* out, char* scratch, cudaStream_t s);
+// exact k-NN graph (1 <= k <= 32): idx / dist2 [P,k] in input row order, order [P] the Morton order of the walk; and its
+// reverse lists (CSR offsets [P+1], sources [P k]).  Both take knn_graph_scratch_bytes(P, k) bytes of scratch whose first
+// knn_graph_scratch_fixed_bytes(P, k) need no device query
+cudaError_t knn_graph_scratch_bytes(int P, int k, size_t* bytes);
+size_t knn_graph_scratch_fixed_bytes(int P, int k);
+cudaError_t launch_knn_graph(int P, int k, const float* points, int32_t* idx, float* dist2, int32_t* order,
+                             char* scratch, cudaStream_t s);
+cudaError_t launch_knn_reverse(int P, int k, const int32_t* idx, int32_t* offsets, int32_t* sources, char* scratch,
+                               cudaStream_t s);
+
+// ---- neighbors.cu: total variation of features [P,C] over a k-NN graph (grad added to, loss [1] double written; its
+// P + 1024 doubles of partial sums come from the device's default memory pool) and the neighbour fill of low-weight rows
+cudaError_t launch_feature_tv_accum(int P, int k, int C, const float* features, const int32_t* idx,
+                                    const int32_t* offsets, const int32_t* sources, const int32_t* order, double weight,
+                                    long long n_edges, float* grad, double* loss, cudaStream_t s);
+cudaError_t launch_feature_fill(int P, int k, int C, const float* features, const float* weight, const int32_t* idx,
+                                float min_weight, float* out, cudaStream_t s);
 
 // ---- densify.cu: clone / split / prune (densify_and_prune) and reset_opacity.  scratch is densify_scratch_bytes(P)
 // bytes whose first densify_scratch_fixed_bytes(P) (the scanned per-Gaussian flags apply reads) need no device query;

@@ -23,6 +23,17 @@
 // of the input order: every pair distance is one fixed expression of (query, candidate), the best-3 multiset of values
 // does not depend on visiting order, and the sum is (d0 + d1) + d2 in ascending order.  No float atomics touch the
 // result.
+//
+// Exact k-NN graph (launch_knn_graph, 1 <= k <= 32): steps 1-5 unchanged (build_tree), then graph_kernel, the same walk
+// with a best-K list of (squared distance, input index) pairs per lane, K in {4, 8, 16, 32} the next size up from k, kept
+// in registers by an unrolled compare-and-swap insertion.  Row i of idx / dist2 [P,k] is ascending by the pair
+// (dist2, index) compared lexicographically, so ties go to the lower index; the point itself is excluded by index, and
+// entries past P - 1 are (-1, +inf).  Exactness: a box is pruned only if its distance is ABOVE the current k-th distance
+// (a box at exactly that distance may still hold a tie with a lower index).  By the argument above the box distance is
+// a lower bound on the computed distance of every point inside, so each of them would come after the k-th pair.  The
+// order of (distance, index) pairs is total, so the first k pairs are one set whatever the visiting order: results are
+// bitwise reproducible, and a permutation of the input permutes the rows (and renames the indices) without changing
+// dist2.  launch_knn_reverse builds the transpose in CSR form from idx with a stable radix sort of (neighbour, source).
 #include <cub/cub.cuh>
 
 #include <algorithm>
@@ -296,6 +307,176 @@ __global__ void __launch_bounds__(256) query_kernel(int P, int top, long long to
     if (active) out[order[self]] = __fdiv_rn(__fadd_rn(__fadd_rn(d0, d1), d2), 3.f);
 }
 
+// ---- exact k-NN graph: the same walk with a best-K list of (distance, index) pairs per lane
+
+// (d, i) before (e, j) in a row of the graph: by distance, ties to the lower index (an empty slot, index 0xffffffff and
+// +inf, comes after every point)
+__device__ __forceinline__ bool pair_less(float d, uint32_t i, float e, uint32_t j) {
+    return d < e || (d == e && i < j);
+}
+
+// The best pairs of one lane in K registers each for distances and indices (every index below is a compile-time
+// constant).  For k < K the first K - k slots hold the sentinel (-inf, 0), which no pair comes before, so the k wanted
+// pairs sit ascending in slots [K - k, K) and the last slot is the k-th.
+template <int K>
+struct BestK {
+    float d[K];
+    uint32_t i[K];
+};
+
+template <int K>
+__device__ __forceinline__ void best_init(BestK<K>& b, int k) {
+#pragma unroll
+    for (int j = 0; j < K; j++) {
+        b.d[j] = __int_as_float(j < K - k ? 0xff800000 : 0x7f800000);
+        b.i[j] = j < K - k ? 0u : 0xffffffffu;
+    }
+}
+
+// a pair before the k-th replaces it and sinks by one compare-and-swap per slot
+template <int K>
+__device__ __forceinline__ void best_insert(BestK<K>& b, float dv, uint32_t iv) {
+    if (pair_less(dv, iv, b.d[K - 1], b.i[K - 1])) {
+        b.d[K - 1] = dv;
+        b.i[K - 1] = iv;
+#pragma unroll
+        for (int j = K - 1; j > 0; j--) {
+            const float d0 = b.d[j - 1], d1 = b.d[j];
+            const uint32_t i0 = b.i[j - 1], i1 = b.i[j];
+            const bool sw = pair_less(d1, i1, d0, i0);
+            b.d[j - 1] = sw ? d1 : d0;
+            b.d[j] = sw ? d0 : d1;
+            b.i[j - 1] = sw ? i1 : i0;
+            b.i[j] = sw ? i0 : i1;
+        }
+    }
+}
+
+// best-K update of every lane against the points of one leaf; candidates carry their input index
+template <int K>
+__device__ __forceinline__ void scan_leaf_k(int P, long long leaf, const float4* __restrict__ sorted,
+                                            const uint32_t* __restrict__ order, int lane, long long self, float3 q,
+                                            bool active, BestK<K>& best) {
+    const long long base = leaf * kLeaf;
+    const int cnt = (int)min((long long)kLeaf, (long long)P - base);
+    float4 c = make_float4(0.f, 0.f, 0.f, 0.f);
+    uint32_t ci = 0;
+    if (lane < cnt) {
+        c = sorted[base + lane];
+        ci = order[base + lane];
+    }
+    for (int j = 0; j < cnt; j++) {
+        const float cx = __shfl_sync(0xffffffffu, c.x, j);
+        const float cy = __shfl_sync(0xffffffffu, c.y, j);
+        const float cz = __shfl_sync(0xffffffffu, c.z, j);
+        const uint32_t cj = __shfl_sync(0xffffffffu, ci, j);
+        if (active && base + j != self) best_insert<K>(best, sq3(__fsub_rn(cx, q.x), __fsub_rn(cy, q.y), __fsub_rn(cz, q.z)), cj);
+    }
+}
+
+template <int K>
+__global__ void __launch_bounds__(256) graph_kernel(int P, int k, int top, long long top_off,
+                                                    const float4* __restrict__ sorted, const uint32_t* __restrict__ order,
+                                                    const float4* __restrict__ box_lo, const float4* __restrict__ box_hi,
+                                                    int32_t* __restrict__ idx, float* __restrict__ dist2) {
+    const int lane = threadIdx.x & 31;
+    const long long leaf = (blockIdx.x * (long long)blockDim.x + threadIdx.x) >> 5;
+    if (leaf * kLeaf >= P) return;  // warp-uniform
+    const long long self = leaf * kLeaf + lane;
+    const bool active = self < P;
+    float3 q = make_float3(0.f, 0.f, 0.f);
+    if (active) {
+        const float4 p = sorted[self];
+        q = make_float3(p.x, p.y, p.z);
+    }
+    BestK<K> best;
+    best_init<K>(best, k);
+    scan_leaf_k<K>(P, leaf, sorted, order, lane, self, q, active, best);
+
+    // query_kernel's walk; a box is entered unless its distance is above the k-th distance (a box at that distance can
+    // still hold a tie with a lower index)
+    int l = top;
+    long long n = 0, off = top_off, cnt = 1;
+    while (true) {
+        const bool need = active && box_dist(q, box_lo[off + n], box_hi[off + n]) <= best.d[K - 1];
+        if (__any_sync(0xffffffffu, need)) {
+            if (l > 0) {
+                l--;
+                n *= kLeaf;
+                cnt = level_count(P, l);
+                off -= cnt;
+                continue;
+            }
+            if (n != leaf) scan_leaf_k<K>(P, n, sorted, order, lane, self, q, active, best);
+        }
+        while (l < top && ((n & (kLeaf - 1)) == kLeaf - 1 || n + 1 >= cnt)) {
+            off += cnt;
+            l++;
+            n >>= 5;
+            cnt = level_count(P, l);
+        }
+        if (l == top) break;
+        n++;
+    }
+    if (!active) return;
+    const size_t row = (size_t)order[self] * k;
+    const int skip = K - k;
+#pragma unroll
+    for (int j = 0; j < K; j++)
+        if (j >= skip) {
+            idx[row + j - skip] = (int32_t)best.i[j];
+            dist2[row + j - skip] = best.d[j];
+        }
+}
+
+// ---- reverse lists: a stable sort of the (neighbour, source) pairs by neighbour; -1 (or any index outside [0, P))
+// sorts last as key P and is dropped
+struct ReverseLayout {
+    size_t keys_in, keys_out, vals_in, sort_tmp, fixed_bytes;
+    explicit ReverseLayout(size_t E) {
+        size_t o = 0;
+        keys_in = o;   o = align_up(o + E * sizeof(uint32_t));
+        keys_out = o;  o = align_up(o + E * sizeof(uint32_t));
+        vals_in = o;   o = align_up(o + E * sizeof(int32_t));
+        sort_tmp = o;
+        fixed_bytes = o;
+    }
+};
+
+int key_bits(int P) {  // keys are in [0, P]
+    int b = 0;
+    for (uint32_t n = (uint32_t)P; n; n >>= 1) b++;
+    return b;
+}
+
+cudaError_t reverse_sort_bytes(int P, int k, size_t* bytes) {
+    *bytes = 0;
+    return cub::DeviceRadixSort::SortPairs(nullptr, *bytes, (const uint32_t*)nullptr, (uint32_t*)nullptr,
+                                           (const int32_t*)nullptr, (int32_t*)nullptr, P * k, 0, key_bits(P));
+}
+
+__global__ void __launch_bounds__(256) reverse_keys_kernel(int P, int k, const int32_t* __restrict__ idx,
+                                                           uint32_t* __restrict__ keys, int32_t* __restrict__ vals) {
+    const long long e = blockIdx.x * (long long)blockDim.x + threadIdx.x;
+    if (e >= (long long)P * k) return;
+    const int32_t j = idx[e];
+    keys[e] = (j >= 0 && j < P) ? (uint32_t)j : (uint32_t)P;
+    vals[e] = (int32_t)(e / k);
+}
+
+// offsets[n] = the first sorted position whose key is >= n, for n in [0, P]; dropped entries become -1
+__global__ void __launch_bounds__(256) reverse_offsets_kernel(int P, int E, const uint32_t* __restrict__ keys,
+                                                              int32_t* __restrict__ sources, int32_t* __restrict__ offsets) {
+    const int e = blockIdx.x * blockDim.x + threadIdx.x;
+    if (e >= E) return;
+    const uint32_t key = keys[e];
+    const long long prev = e ? (long long)keys[e - 1] : -1;
+    for (long long n = prev + 1; n <= key; n++) offsets[n] = e;
+    if (e == E - 1)
+        for (long long n = (long long)key + 1; n <= P; n++) offsets[n] = E;
+    if (key == (uint32_t)P) sources[e] = -1;
+}
+
 }  // namespace
 
 cudaError_t knn_scratch_bytes(int P, size_t* bytes) {
@@ -310,9 +491,11 @@ cudaError_t knn_scratch_bytes(int P, size_t* bytes) {
 
 size_t knn_scratch_fixed_bytes(int P) { return P > 0 ? KnnLayout(P).fixed_bytes : 0; }
 
-cudaError_t launch_knn_mean_dist(int P, const float* points, float* out, char* scratch, cudaStream_t s) {
-    if (P <= 0) return cudaSuccess;
-    const KnnLayout ly(P);
+namespace {
+
+// Steps 1-5 of the pipeline, shared by every query: the sorted points, the Morton order idx_out and the boxes of every
+// level, in `scratch` as laid out by `ly`
+cudaError_t build_tree(int P, const float* points, char* scratch, const KnnLayout& ly, cudaStream_t s) {
     size_t sb = 0;
     cudaError_t e = sort_bytes(P, &sb);
     if (e != cudaSuccess) return e;
@@ -343,8 +526,84 @@ cudaError_t launch_knn_mean_dist(int P, const float* points, float* out, char* s
                                                                           hi + L.off[l - 1], lo + L.off[l], hi + L.off[l]);
         g_launches++;
     }
-    query_kernel<<<blocks_for((long long)L.count[0] * 32), 256, 0, s>>>(P, L.n - 1, L.off[L.n - 1], sorted, idx_out, lo,
-                                                                        hi, out);
+    return cudaGetLastError();
+}
+
+}  // namespace
+
+cudaError_t launch_knn_mean_dist(int P, const float* points, float* out, char* scratch, cudaStream_t s) {
+    if (P <= 0) return cudaSuccess;
+    const KnnLayout ly(P);
+    cudaError_t e = build_tree(P, points, scratch, ly, s);
+    if (e != cudaSuccess) return e;
+    const KnnLevels& L = ly.lv;
+    query_kernel<<<blocks_for((long long)L.count[0] * 32), 256, 0, s>>>(
+        P, L.n - 1, L.off[L.n - 1], reinterpret_cast<const float4*>(scratch + ly.pts),
+        reinterpret_cast<const uint32_t*>(scratch + ly.idx_out), reinterpret_cast<const float4*>(scratch + ly.box_lo),
+        reinterpret_cast<const float4*>(scratch + ly.box_hi), out);
+    g_launches++;
+    return cudaGetLastError();
+}
+
+cudaError_t knn_graph_scratch_bytes(int P, int k, size_t* bytes) {
+    *bytes = 0;
+    if (P <= 0) return cudaSuccess;
+    size_t a = 0, b = 0;
+    cudaError_t e = knn_scratch_bytes(P, &a);
+    if (e != cudaSuccess) return e;
+    if ((e = reverse_sort_bytes(P, k, &b)) != cudaSuccess) return e;
+    *bytes = std::max(a, ReverseLayout((size_t)P * k).fixed_bytes + align_up(b));
+    return cudaSuccess;
+}
+
+size_t knn_graph_scratch_fixed_bytes(int P, int k) {
+    return P > 0 ? std::max(KnnLayout(P).fixed_bytes, ReverseLayout((size_t)P * k).fixed_bytes) : 0;
+}
+
+cudaError_t launch_knn_graph(int P, int k, const float* points, int32_t* idx, float* dist2, int32_t* order,
+                             char* scratch, cudaStream_t s) {
+    if (P <= 0) return cudaSuccess;
+    const KnnLayout ly(P);
+    cudaError_t e = build_tree(P, points, scratch, ly, s);
+    if (e != cudaSuccess) return e;
+    const KnnLevels& L = ly.lv;
+    const float4* sorted = reinterpret_cast<const float4*>(scratch + ly.pts);
+    const uint32_t* ord = reinterpret_cast<const uint32_t*>(scratch + ly.idx_out);
+    const float4* lo = reinterpret_cast<const float4*>(scratch + ly.box_lo);
+    const float4* hi = reinterpret_cast<const float4*>(scratch + ly.box_hi);
+    const unsigned grid = blocks_for((long long)L.count[0] * 32);
+    if (k <= 4)
+        graph_kernel<4><<<grid, 256, 0, s>>>(P, k, L.n - 1, L.off[L.n - 1], sorted, ord, lo, hi, idx, dist2);
+    else if (k <= 8)
+        graph_kernel<8><<<grid, 256, 0, s>>>(P, k, L.n - 1, L.off[L.n - 1], sorted, ord, lo, hi, idx, dist2);
+    else if (k <= 16)
+        graph_kernel<16><<<grid, 256, 0, s>>>(P, k, L.n - 1, L.off[L.n - 1], sorted, ord, lo, hi, idx, dist2);
+    else
+        graph_kernel<32><<<grid, 256, 0, s>>>(P, k, L.n - 1, L.off[L.n - 1], sorted, ord, lo, hi, idx, dist2);
+    g_launches++;
+    if ((e = cudaGetLastError()) != cudaSuccess) return e;
+    return cudaMemcpyAsync(order, ord, (size_t)P * sizeof(int32_t), cudaMemcpyDeviceToDevice, s);
+}
+
+cudaError_t launch_knn_reverse(int P, int k, const int32_t* idx, int32_t* offsets, int32_t* sources, char* scratch,
+                               cudaStream_t s) {
+    if (P <= 0) return cudaSuccess;
+    const int E = P * k;
+    const ReverseLayout ly((size_t)E);
+    size_t sb = 0;
+    cudaError_t e = reverse_sort_bytes(P, k, &sb);
+    if (e != cudaSuccess) return e;
+    uint32_t* keys_in = reinterpret_cast<uint32_t*>(scratch + ly.keys_in);
+    uint32_t* keys_out = reinterpret_cast<uint32_t*>(scratch + ly.keys_out);
+    int32_t* vals_in = reinterpret_cast<int32_t*>(scratch + ly.vals_in);
+    reverse_keys_kernel<<<blocks_for(E), 256, 0, s>>>(P, k, idx, keys_in, vals_in);
+    g_launches++;
+    if ((e = cudaGetLastError()) != cudaSuccess) return e;
+    // the radix sort is stable: each neighbour's sources stay in ascending row order
+    if ((e = cub::DeviceRadixSort::SortPairs(scratch + ly.sort_tmp, sb, keys_in, keys_out, vals_in, sources, E, 0,
+                                             key_bits(P), s)) != cudaSuccess)
+        return e;
+    reverse_offsets_kernel<<<blocks_for(E), 256, 0, s>>>(P, E, keys_out, sources, offsets);
     g_launches++;
     return cudaGetLastError();
 }

@@ -1443,6 +1443,110 @@ torch::Tensor vqDecode(const torch::Tensor& codebook, const torch::Tensor& code,
     return o;
 }
 
+// ---- neighbour graphs (f3dgs_knn_graph / _reverse, f3dgs_feature_tv_accum, f3dgs_feature_fill)
+namespace {
+// a contiguous int32 [P,k] CUDA tensor on `dev`
+const int32_t* graph_idx(const torch::Tensor& idx, const torch::Device& dev) {
+    TORCH_CHECK(idx.is_cuda() && idx.device() == dev && idx.scalar_type() == torch::kInt32 && idx.dim() == 2 &&
+                    idx.is_contiguous(),
+                "idx must be a contiguous int32 [P,k] tensor on ", dev);
+    return idx.numel() ? idx.data_ptr<int32_t>() : nullptr;
+}
+}  // namespace
+
+// points [P,3] -> (idx int32 [P,k], dist2 float32 [P,k], order int32 [P])
+std::tuple<torch::Tensor, torch::Tensor, torch::Tensor> knnGraph(const torch::Tensor& points, int64_t k) {
+    TORCH_CHECK(points.is_cuda(), "points must be a CUDA tensor (this build has no CPU path)");
+    TORCH_CHECK(points.scalar_type() == torch::kFloat32 && points.dim() == 2 && points.size(1) == 3,
+                "points must be a float32 tensor [P,3]");
+    TORCH_CHECK(k >= 1 && k <= 32 && points.size(0) * k <= INT32_MAX, "knn_graph: need 1 <= k <= 32 and P k < 2^31");
+    const c10::cuda::CUDAGuard guard(points.device());
+    auto p = points.contiguous();
+    const int P = (int)p.size(0);
+    torch::Tensor idx = torch::empty({P, k}, p.options().dtype(torch::kInt32));
+    torch::Tensor dist2 = torch::empty({P, k}, p.options());
+    torch::Tensor order = torch::empty({P}, p.options().dtype(torch::kInt32));
+    if (P == 0) return std::make_tuple(idx, dist2, order);
+    torch::Tensor scratch = scratch_tensor(f3dgs_knn_graph_scratch_bytes(P, (int)k), "f3dgs_knn_graph_scratch_bytes", p);
+    cudaStream_t stream = c10::cuda::getCurrentCUDAStream().stream();
+    check_rc(f3dgs_knn_graph(P, (int)k, fptr(p), idx.data_ptr<int32_t>(), dist2.data_ptr<float>(),
+                             order.data_ptr<int32_t>(), scratch_ptr(scratch), (void*)stream),
+             "f3dgs_knn_graph");
+    return std::make_tuple(idx, dist2, order);
+}
+
+// idx int32 [P,k] -> (offsets int32 [P+1], sources int32 [P k])
+std::tuple<torch::Tensor, torch::Tensor> knnReverse(const torch::Tensor& idx) {
+    TORCH_CHECK(idx.is_cuda(), "idx must be a CUDA tensor (this build has no CPU path)");
+    const auto dev = idx.device();
+    const c10::cuda::CUDAGuard guard(dev);
+    const int32_t* ip = graph_idx(idx, dev);
+    const int64_t P = idx.size(0), k = idx.size(1);
+    TORCH_CHECK(k >= 1 && k <= 32 && P * k <= INT32_MAX, "knn_reverse: need 1 <= k <= 32 and P k < 2^31");
+    torch::Tensor offsets = torch::zeros({P + 1}, idx.options());
+    torch::Tensor sources = torch::empty({P * k}, idx.options());
+    if (P == 0) return std::make_tuple(offsets, sources);
+    torch::Tensor scratch =
+        scratch_tensor(f3dgs_knn_graph_scratch_bytes((int)P, (int)k), "f3dgs_knn_graph_scratch_bytes", idx);
+    cudaStream_t stream = c10::cuda::getCurrentCUDAStream().stream();
+    check_rc(f3dgs_knn_reverse((int)P, (int)k, ip, offsets.data_ptr<int32_t>(), sources.data_ptr<int32_t>(),
+                               scratch_ptr(scratch), (void*)stream),
+             "f3dgs_knn_reverse");
+    return std::make_tuple(offsets, sources);
+}
+
+// features [P,C] (any shape of P C floats, contiguous), the graph, grad (contiguous float32, P C elements) added to in
+// place -> the loss, a float64 CUDA scalar
+torch::Tensor featureTvAccum(const torch::Tensor& features, const torch::Tensor& idx, const torch::Tensor& offsets,
+                             const torch::Tensor& sources, const c10::optional<torch::Tensor>& order, double weight,
+                             int64_t n_edges, torch::Tensor grad) {
+    TORCH_CHECK(features.is_cuda(), "features must be a CUDA tensor (this build has no CPU path)");
+    const auto dev = features.device();
+    const c10::cuda::CUDAGuard guard(dev);
+    const int32_t* ip = graph_idx(idx, dev);
+    const int64_t P = idx.size(0), k = idx.size(1);
+    TORCH_CHECK(P > 0 ? features.numel() % P == 0 : features.numel() == 0, "features must have P rows");
+    const int64_t C = P ? features.numel() / P : 0;
+    const torch::Tensor f = input(features, dev, "features");
+    float* gp = in_place(grad, dev, P * C, "grad");
+    const int32_t* op = indices(offsets, dev, "offsets");
+    const int32_t* sp = indices(sources, dev, "sources");
+    TORCH_CHECK(offsets.numel() == P + 1 && sources.numel() == P * k, "offsets must be [P+1] and sources [P k]");
+    const int32_t* orp = nullptr;
+    if (order.has_value() && order->defined()) {
+        orp = indices(*order, dev, "order");
+        TORCH_CHECK(order->numel() == P, "order must be [P]");
+    }
+    torch::Tensor loss = torch::zeros({}, features.options().dtype(torch::kFloat64));
+    if (P == 0) return loss;
+    cudaStream_t stream = c10::cuda::getCurrentCUDAStream().stream();
+    check_rc(f3dgs_feature_tv_accum((int)P, (int)k, (int)C, fptr(f), ip, op, sp, orp, weight, n_edges, gp,
+                                    loss.data_ptr<double>(), (void*)stream),
+             "f3dgs_feature_tv_accum");
+    return loss;
+}
+
+// features [P,C] (any shape of P C floats), weights [P], idx [P,k] -> a new [P,C]-shaped tensor (features' shape)
+torch::Tensor featureFill(const torch::Tensor& features, const torch::Tensor& weights, const torch::Tensor& idx,
+                          double min_weight) {
+    TORCH_CHECK(features.is_cuda(), "features must be a CUDA tensor (this build has no CPU path)");
+    const auto dev = features.device();
+    const c10::cuda::CUDAGuard guard(dev);
+    const int32_t* ip = graph_idx(idx, dev);
+    const int64_t P = idx.size(0), k = idx.size(1);
+    TORCH_CHECK(P > 0 ? features.numel() % P == 0 : features.numel() == 0, "features must have P rows");
+    const int64_t C = P ? features.numel() / P : 0;
+    const torch::Tensor f = input(features, dev, "features"), w = input(weights, dev, "weights");
+    TORCH_CHECK(weights.numel() == P, "weights must have P elements");
+    torch::Tensor out = torch::empty_like(f);
+    if (P == 0 || C == 0) return out;
+    cudaStream_t stream = c10::cuda::getCurrentCUDAStream().stream();
+    check_rc(f3dgs_feature_fill((int)P, (int)k, (int)C, fptr(f), fptr(w), ip, (float)min_weight, out.data_ptr<float>(),
+                                (void*)stream),
+             "f3dgs_feature_fill");
+    return out;
+}
+
 // ---- activation prologue + fused optimizer step (f3dgs_activate / f3dgs_adam_step): in-place on the caller's tensors
 void activateParams(const torch::Tensor& raw_opacity, const torch::Tensor& raw_scaling, const torch::Tensor& raw_rotation,
                     const torch::Tensor& f_dc, const torch::Tensor& f_rest, torch::Tensor opacity, torch::Tensor scales,
@@ -1639,6 +1743,13 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     m.def("vq_codebook_grad", &vqCodebookGrad, pybind11::arg("dL_dx"), pybind11::arg("scratch"), pybind11::arg("K"));
     m.def("vq_decode", &vqDecode, pybind11::arg("codebook"), pybind11::arg("code"), pybind11::arg("half") = false,
           pybind11::arg("out") = pybind11::none());
+    m.def("knn_graph", &knnGraph, pybind11::arg("points"), pybind11::arg("k"));
+    m.def("knn_reverse", &knnReverse, pybind11::arg("idx"));
+    m.def("feature_tv_accum", &featureTvAccum, pybind11::arg("features"), pybind11::arg("idx"),
+          pybind11::arg("offsets"), pybind11::arg("sources"), pybind11::arg("order"), pybind11::arg("weight"),
+          pybind11::arg("n_edges"), pybind11::arg("grad"));
+    m.def("feature_fill", &featureFill, pybind11::arg("features"), pybind11::arg("weights"), pybind11::arg("idx"),
+          pybind11::arg("min_weight"));
     m.def("activate", &activateParams);
     m.def("adam_step", &adamStep, pybind11::arg("kind"), pybind11::arg("param"), pybind11::arg("grad_activated"),
           pybind11::arg("exp_avg"), pybind11::arg("exp_avg_sq"), pybind11::arg("M"), pybind11::arg("lr"),

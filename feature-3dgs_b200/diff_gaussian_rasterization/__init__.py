@@ -67,6 +67,11 @@ Behavioural notes
     code)` gathers the rows back (float32 or float16), and `CodePlan(code, K)` gives the codebook gradient of the
     gather.  `GaussianState.quantize_features(K)` trains the codebook in place of per-Gaussian features, and io.save_ply
     stores it with one ushort code per Gaussian.
+  * neighbour graphs of Gaussians: `knn_graph(points, k)` is the exact k-NN graph (f3dgs_knn_graph, int32 indices and
+    squared distances, ties to the lower index).  Over it, `feature_tv_loss(features, graph, weight)` is the total
+    variation of the feature field (Gaussian Grouping's 3-D neighbour term, in L1), `fill_features(features, weight,
+    graph)` gives rows no view blended their neighbours' weighted mean, and `outlier_mask(graph, std_ratio)` is
+    statistical outlier removal.  `GaussianState.add_feature_tv_grads` and `remove_outliers` use them in training.
   * `debug=True` keeps the reference semantics: arguments are snapshotted to CPU first and dumped
     to snapshot_fw.dump / snapshot_bw.dump if the native call raises (reference :89-97,:147-155);
     natively it synchronises and checks after every stage.
@@ -90,6 +95,8 @@ except ImportError as exc:  # pragma: no cover - exercised only on a broken inst
 from .filter3d import apply_3d_filter, compute_3d_filter  # noqa: E402
 from .codebook import CodePlan, decode, kmeans  # noqa: E402
 from .scores import GaussianScores  # noqa: E402
+from .neighbors import (KnnGraph, feature_tv_loss, feature_tv_loss_and_grad, fill_features, knn_graph,  # noqa: E402
+                        outlier_mask)
 
 __all__ = [
     "GaussianRasterizationSettings",
@@ -107,6 +114,12 @@ __all__ = [
     "kmeans",
     "decode",
     "CodePlan",
+    "KnnGraph",
+    "knn_graph",
+    "feature_tv_loss",
+    "feature_tv_loss_and_grad",
+    "fill_features",
+    "outlier_mask",
 ]
 
 

@@ -32,7 +32,10 @@ _opacity, _scaling, _rotation, _semantic_feature`, :47-58) as plain CUDA tensors
   quantize_features()   LightGaussian's / CompGS's vector quantisation of the feature field (codebook.kmeans): the state
                         then trains a codebook [K,C] in place of per-Gaussian features, activate() decodes codebook[code]
                         for the rasterizer and step() takes the codebook gradient of that gather; dequantize() returns
-                        to per-Gaussian features.
+                        to per-Gaussian features;
+  neighbor_graph(k)     the exact k-NN graph of the means (neighbors.knn_graph), cached until the rows change;
+                        add_feature_tv_grads() adds the gradient of the feature field's total variation over it, and
+                        remove_outliers() prunes statistical outliers.
 
 Float16 feature fields: with feature_dtype=torch.float16 the rasterizer reads a float16 working copy
 act["semantic_feature"] of the float32 master raw["semantic_feature"], so every view renders a float16 map and the feature
@@ -144,6 +147,7 @@ class GaussianState:
                         rotations=torch.empty(P, 4, device=dev), shs=torch.empty(P, self.M, 3, device=dev),
                         semantic_feature=sf if sf.dtype == self.feature_dtype else sf.to(self.feature_dtype))
         self._batch: Optional[ViewBatch] = None
+        self._graph = None  # neighbor_graph()'s cache: the rows it was built on are gone or reordered
         self._unfiltered = None  # the unfiltered opacity [P,1] and scales [P,3] while the 3D filter is on
 
     def activate(self):
@@ -509,6 +513,7 @@ class GaussianState:
             _C.mcmc_relocate(scratch, index[:n_dead], index[n_dead:][draws], min_opacity, groups,
                              self.act["semantic_feature"] if half else None)
             n_relocated = n_dead
+            self._graph = None  # the relocated rows moved (and _reset_derived is not reached without additions)
         del index, alive_opacity
         n_added = min(cap_max, int(1.05 * P)) - P
         if n_added <= 0:
@@ -559,6 +564,40 @@ class GaussianState:
             return
         g["opacities"].add_(opacity_reg / P)
         g["scales"].add_(scale_reg / (3 * P))
+
+    # ---------------------------------------------------------------------------------------------- neighbour graph
+    def neighbor_graph(self, k: int, rebuild: bool = False):
+        """The exact k-NN graph of raw["xyz"] (neighbors.knn_graph, one host read for its finiteness check), cached.
+        Densification, prune, relocate_and_add and quantisation drop the cache; while the means move under step() it is
+        the caller's choice when to pass rebuild=True (or call again with another k)."""
+        from .neighbors import knn_graph
+
+        if rebuild or self._graph is None or self._graph.k != k:
+            self._graph = knn_graph(self.raw["xyz"], k)
+        return self._graph
+
+    def add_feature_tv_grads(self, weight: float, k: int = 8, grads: Optional[Dict[str, torch.Tensor]] = None):
+        """Adds the gradient of the feature field's total variation over the k-NN graph, weight / (|E| C) * sum over
+        edges (i, j) of ||f_i - f_j||_1 (neighbors.feature_tv_loss_and_grad) on the float32 master raw["semantic_feature"],
+        to grads["semantic_feature"] (default: the ViewBatch's).  Gaussian Grouping's 3-D neighbour term, in L1: it pulls
+        the features of Gaussians that the 2-D loss barely reaches (inside objects, occluded, nearly transparent)
+        towards their neighbours'.  Call it once per step after vb.all_reduce() and before step().  Returns the loss (a
+        CUDA scalar; no host read besides the graph's).  Raises ValueError while the features are quantised."""
+        from .neighbors import feature_tv_loss_and_grad
+
+        if self.code is not None:
+            raise ValueError("add_feature_tv_grads: not available while the features are quantised; call dequantize() "
+                             "first")
+        g = grads if grads is not None else self.batch().grads
+        sf = self.raw["semantic_feature"]
+        return feature_tv_loss_and_grad(sf, self.neighbor_graph(k), weight, g["semantic_feature"])
+
+    def remove_outliers(self, k: int = 16, std_ratio: float = 2.0) -> int:
+        """Statistical outlier removal (neighbors.outlier_mask over the k-NN graph of the means): prune(mask), with the
+        optimizer state carried along as prune() does.  Returns the new P."""
+        from .neighbors import outlier_mask
+
+        return self.prune(outlier_mask(self.neighbor_graph(k), std_ratio))
 
 
 def _multinomial(probs, n, generator):

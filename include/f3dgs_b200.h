@@ -949,6 +949,55 @@ int f3dgs_vq_decode(int P, int K, int D, const float* codebook, const int32_t* c
 int f3dgs_vq_decode_f16out(int P, int K, int D, const float* codebook, const int32_t* code, uint16_t* out,
                            void* cuda_stream);
 
+/* ---- neighbour graphs of Gaussians: exact k-NN, its reverse lists, total variation of a feature field over it, and
+ * the neighbour fill of low-weight rows ---------------------------------------------------------------------------
+ * P points [P,3] float32, 1 <= k <= 32, P k <= 2^31 - 1; P == 0 launches nothing.  Graph arrays are row-major [P,k].
+ *   f3dgs_knn_graph      idx [P,k] int32 and dist2 [P,k] float32 in input row order: row i holds the k nearest points
+ *                        j != i (exclusion by index, so a coincident point is a neighbour at distance 0), ascending by the
+ *                        pair (dist2, j) compared lexicographically, so ties go to the lower index.  dist2 is
+ *                        f3dgs_knn_mean_dist's one expression, fma(dz, dz, fma(dy, dy, dx * dx)) of the rounded
+ *                        differences candidate - query per axis.  Entries past P - 1 are idx = -1, dist2 = +inf.  order
+ *                        [P] int32 receives the Morton order of the search (a permutation of [0, P)), in which rows
+ *                        close in space are close in memory.  The result is EXACT: the search prunes a box only when its
+ *                        distance, a lower bound on the rounded distance of every point inside (rounding is monotone),
+ *                        is above the current k-th distance.  No float atomics: bitwise reproducible, and a permutation
+ *                        of the points permutes the rows (dist2 is unchanged).  Results are specified for finite
+ *                        coordinates only.  idx, dist2 and order must not overlap each other, points or scratch.
+ *   f3dgs_knn_reverse    the transpose of idx in CSR form: sources[offsets[n] .. offsets[n+1]) are the rows i with n in
+ *                        idx[i], ascending (a stable radix sort of the (neighbour, source) pairs).  Entries of idx outside
+ *                        [0, P), -1 among them, are dropped; offsets[P] is the number of valid entries and sources past it
+ *                        are -1.  offsets [P+1] and sources [P k] int32 must not overlap each other, idx or scratch.
+ *   Both take scratch of f3dgs_knn_graph_scratch_bytes(P, k) bytes of device memory, 256-byte aligned (0 for sizes out
+ *   of range, and 0 with f3dgs_last_error() set if a size query of the device sort fails).
+ *   f3dgs_feature_tv_accum  total variation of features f [P,C] float32 (1 <= C <= F3DGS_MAX_FEATURE_DIM) over the graph's
+ *                        valid edges E (n_edges = |E|, given by the caller):
+ *                          L = weight / (|E| C) * sum_{(i,j) in E} sum_c |f_ic - f_jc|
+ *                          grad_i += float(n_i) * s,   s = (float)(weight / (|E| C)),
+ *                          n_i = sum_{j in N(i)} sign(f_i - f_j) - sum_{i' in R(i)} sign(f_i' - f_i),  sign(0) = 0
+ *                        with N from idx and R from the reverse lists (offsets, sources).  n_i is an integer counted
+ *                        exactly; the product and the add are each rounded to nearest (no fma), so grad is defined
+ *                        bitwise and is ADDED to.  *loss (device double) = L, from per-row float64 sums reduced in a fixed
+ *                        order.  order [P] (may be NULL: row order) is the walk order over rows; the results do not
+ *                        depend on it.  n_edges == 0: *loss = 0 and grad is untouched.  P + 1024 doubles of partial sums
+ *                        come from the device's default memory pool (F3DGS_ERR_ALLOC if that fails).  grad and loss must
+ *                        not overlap each other or an input; weight must be finite.
+ *   f3dgs_feature_fill   out [P,C] = features, except that a row i with weights[i] <= min_weight and at least one
+ *                        neighbour j with weights[j] > min_weight becomes sum_j w_j f_j / sum_j w_j over those
+ *                        neighbours, both sums in double in neighbour order, the quotient rounded once to float32.
+ *                        weights [P] float32; min_weight must not be NaN; out must not overlap features, weights or idx.
+ * F3DGS_ERR_INVALID_ARGUMENT, before any CUDA call, for sizes out of range, a NULL pointer (with P > 0) or an overlap.
+ * Stream-ordered without host sync; every result is bitwise reproducible. */
+size_t f3dgs_knn_graph_scratch_bytes(int P, int k);
+int f3dgs_knn_graph(int P, int k, const float* points, int32_t* idx, float* dist2, int32_t* order, char* scratch,
+                    void* cuda_stream);
+int f3dgs_knn_reverse(int P, int k, const int32_t* idx, int32_t* offsets, int32_t* sources, char* scratch,
+                      void* cuda_stream);
+int f3dgs_feature_tv_accum(int P, int k, int C, const float* features, const int32_t* idx, const int32_t* offsets,
+                           const int32_t* sources, const int32_t* order, double weight, long long n_edges, float* grad,
+                           double* loss, void* cuda_stream);
+int f3dgs_feature_fill(int P, int k, int C, const float* features, const float* weights, const int32_t* idx,
+                       float min_weight, float* out, void* cuda_stream);
+
 /* ---- markVisible: reference rasterizer_impl.cu:141-153 (checkFrustum :54-66) --------------
  * present[i] = (view-space z of means3D[i] > 0.2).  `present` is P bytes (0/1). */
 int f3dgs_mark_visible(int P, const float* means3D, const float* viewmatrix,
