@@ -27,6 +27,11 @@ steps the forward rounded once each: <= 4 u n_p = 2u (2 n_p); its sum over the G
 products 2u.  k = 4 covers the largest of these coefficients (the unwind's 2u per unit of 2 n_p) with room for the
 order in which atomics or a hierarchical reduction add the terms; no bar is scaled by a scene-wide maximum.
 
+Windows.  Pairs(..., tiles=) restricts the pairs to the pixels of some tiles, and extract_ids reads the weights of the
+Gaussians in their lists only, so that a view of any size is checked exactly where it is checked: every weight and
+every per-pixel identity at those pixels, and the per-Gaussian identities of the Gaussians `contained` in the tiles
+(all of whose instances lie in them, so all of whose blended pixels are among the pairs).
+
 Every check returns worst ratios |err| / bar (<= 1 passes) so that the margin can be printed.
 """
 import numpy as np
@@ -52,30 +57,58 @@ def _seg_excl_cumsum(x, first):
 
 class Pairs:
     """Every (pixel, list entry) pair of a view: for each pixel inside the image, every instance of its tile's list in list
-    order.  pix (y * W + x), pos (1-based list position), gid; walked = pos <= n_contrib of the pixel."""
+    order.  pix (y * W + x), pos (1-based list position), gid; walked = pos <= n_contrib of the pixel.
 
-    def __init__(self, point_list, ranges, n_contrib, W, H):
+    tiles: None (every pixel of the image) or a 1-D tensor of tile ids (row-major over the 16x16 tile grid): then only the
+    pixels of those tiles get pairs, the same pairs, in the same order, as the whole image's rows for them.  pixels holds
+    the pixels that have pairs, ascending; HW stays the image's, and per-pixel tensors ([HW]) are indexed by pixel id."""
+
+    def __init__(self, point_list, ranges, n_contrib, W, H, tiles=None):
         dev = point_list.device
         self.W, self.H, self.HW = W, H, W * H
         p = torch.arange(W * H, device=dev)
         py, px = p // W, p % W
         tile = (py // 16) * ((W + 15) // 16) + px // 16
+        if tiles is not None:
+            keep = torch.isin(tile, torch.as_tensor(tiles, device=dev).long())
+            p, tile = p[keep], tile[keep]
+        self.pixels = p
         ranges = ranges.long()
         start = ranges[tile, 0]
         L = ranges[tile, 1] - start
         self.n = n_contrib.reshape(-1).long()
-        assert bool((self.n <= L).all())
+        assert bool((self.n[p] <= L).all())
         first = torch.cumsum(L, 0) - L
         self.pix = torch.repeat_interleave(p, L)
         self.first = torch.repeat_interleave(first, L)  # index of the first pair of the same pixel
         off = torch.arange(self.pix.numel(), device=dev) - self.first
         self.pos = off + 1
-        self.gid = point_list.long()[start[self.pix] + off]
+        self.gid = point_list.long()[torch.repeat_interleave(start, L) + off]
         self.walked = self.pos <= self.n[self.pix]
         self.widx = torch.nonzero(self.walked).reshape(-1)  # walked pairs, in pair order
         self.wgid = self.gid[self.widx]
         self.order = torch.argsort(self.wgid, stable=True)  # walked pairs by Gaussian, for the group gathers
         self.sorted_gid = self.wgid[self.order]
+
+
+def contained(point_list, ranges, P, tiles):
+    """bool [P]: the Gaussians that have instances in point_list and every one of them in a tile of `tiles`.  Only
+    such a Gaussian blends no pixel outside those tiles, so only its per-Gaussian sums are complete over windowed
+    Pairs.  Each instance's tile is the tile whose range [start, end) holds it."""
+    dev = point_list.device
+    ranges = ranges.long()
+    start, L = ranges[:, 0], ranges[:, 1] - ranges[:, 0]
+    first = torch.cumsum(L, 0) - L
+    n = int(L.sum())
+    inst = torch.repeat_interleave(start - first, L) + torch.arange(n, device=dev)  # list index of each range entry
+    inst_tile = torch.full((point_list.numel(),), -1, dtype=torch.long, device=dev)
+    inst_tile[inst] = torch.repeat_interleave(torch.arange(L.numel(), device=dev), L)
+    assert n == point_list.numel() and bool((inst_tile >= 0).all()), "the ranges do not cover the list once"
+    inside = torch.isin(inst_tile, torch.as_tensor(tiles, device=dev).long())
+    gid = point_list.long()
+    total = torch.zeros(P, dtype=torch.long, device=dev).index_add_(0, gid, torch.ones_like(gid))
+    outside = torch.zeros(P, dtype=torch.long, device=dev).index_add_(0, gid, (~inside).long())
+    return (total > 0) & (outside == 0)
 
 
 def extract(pairs, P, render, group):
@@ -97,9 +130,41 @@ def extract(pairs, P, render, group):
     return w
 
 
+def extract_ids(pairs, P, render, gids, group):
+    """-> float32 weight of every walked pair whose Gaussian is in gids (distinct ids), 0 for the other pairs.
+    render(sf) -> [C, H*W] float32 map of the features sf [P, C]: for the group k0 .. k0+C-1 of gids, row gids[k0 + k]
+    is one-hot e_k and every other row 0.  Only the pairs' pixels are read: at them, a weight outside the walked pairs
+    fails, as does a negative or non-finite value anywhere in the map."""
+    dev = pairs.pix.device
+    gids = torch.as_tensor(gids, device=dev).long()
+    assert torch.unique(gids).numel() == gids.numel()
+    w = torch.zeros(pairs.widx.numel(), dtype=torch.float32, device=dev)
+    wpix = pairs.pix[pairs.widx]
+    slot = torch.full((P,), -1, dtype=torch.long, device=dev)
+    for k0 in range(0, gids.numel(), group):
+        g = gids[k0:k0 + group]
+        C = g.numel()
+        sf = torch.zeros(P, C, dtype=torch.float32, device=dev)
+        sf[g, torch.arange(C, device=dev)] = 1.0
+        m = render(sf)
+        del sf
+        assert m.shape == (C, pairs.HW) and m.dtype == torch.float32
+        slot[g] = torch.arange(C, device=dev)
+        k = slot[pairs.wgid]
+        slot[g] = -1
+        idx = torch.nonzero(k >= 0).reshape(-1)
+        v = m[k[idx], wpix[idx]]
+        w[idx] = v
+        # no weight at the pairs' pixels outside the walked pairs, none negative or non-finite
+        assert int(torch.count_nonzero(m[:, pairs.pixels])) == int(torch.count_nonzero(v)), (k0, C)
+        assert bool(m.min() >= 0) and bool(torch.isfinite(m.sum()))  # a NaN fails the first, an inf the second
+        del m
+    return w
+
+
 def check_model(pairs, w, rec, final_T):
-    """Part 2: every weight against the float64 model built from the records (see the module docstring).
-    -> dict(weight=worst ratio, final_T=worst ratio, bad_*: counts of failed pairs / pixels, ...)."""
+    """Part 2: every weight against the float64 model built from the records (see the module docstring), and final_T
+    at the pairs' pixels.  -> dict(weight=worst ratio, final_T=worst ratio, bad_*: counts of failed pairs / pixels, ...)."""
     dev = pairs.pix.device
     f64 = torch.float64
     rec = rec.to(dev)
@@ -136,7 +201,9 @@ def check_model(pairs, w, rec, final_T):
     rep["weight"] = float(rw[blended].max()) if bool(blended.any()) else 0.0
     rep["n_blended"] = int(blended.sum())
     # final_T: the product over every blended pair
-    rep["final_T"] = float(_ratio((final_T.reshape(-1).to(dev).double() - T_fin).abs(), rho_fin * T_fin + U * T_fin).max())
+    px = pairs.pixels
+    rep["final_T"] = float(_ratio((final_T.reshape(-1).to(dev).double()[px] - T_fin[px]).abs(),
+                                  (rho_fin * T_fin + U * T_fin)[px]).max())
     # blend decisions before n_contrib
     walked = pairs.walked
     rep["bad_blended_but_fails_thresholds"] = int((blended & clear_skip).sum())
@@ -167,7 +234,9 @@ def check_model(pairs, w, rec, final_T):
 
 
 class Weights:
-    """W as sparse [P, HW] float64 matrices over the blended pairs, with the per-pixel and per-Gaussian bar terms."""
+    """W as sparse [P, HW] float64 matrices over the blended pairs, with the per-pixel and per-Gaussian bar terms.  The
+    per-pixel checks cover the pairs' pixels (every pixel, or those of windowed Pairs); a per-Gaussian sum is complete
+    only for a Gaussian that blends no pixel outside them (contained), which `rows` selects."""
 
     def __init__(self, pairs, w, P):
         keep = w > 0
@@ -175,34 +244,40 @@ class Weights:
         g, p = pairs.gid[idx], pairs.pix[idx]
         v = w[keep].double()
         self.P, self.HW = P, pairs.HW
+        self.pixels = pairs.pixels
         self.n = pairs.n.double()
-        self.W = torch.sparse_coo_tensor(torch.stack([g, p]), v, (P, self.HW)).coalesce()
-        self.Wt = torch.sparse_coo_tensor(torch.stack([p, g]), v, (self.HW, P)).coalesce()
-        self.Wn = torch.sparse_coo_tensor(torch.stack([g, p]), v * (2 * self.n[p] + 4), (P, self.HW)).coalesce()
+        # pixels are indexed in the order of self.pixels (ascending): the whole image or the windows
+        q = torch.searchsorted(self.pixels, p)
+        n = self.pixels.numel()
+        self.W = torch.sparse_coo_tensor(torch.stack([g, q]), v, (P, n)).coalesce()
+        self.Wt = torch.sparse_coo_tensor(torch.stack([q, g]), v, (n, P)).coalesce()
+        self.Wn = torch.sparse_coo_tensor(torch.stack([g, q]), v * (2 * self.n[p] + 4), (P, n)).coalesce()
         self.m = torch.zeros(P, dtype=torch.float64, device=v.device).index_add_(0, g, torch.ones_like(v))
 
     def per_pixel(self, ours, x, extra=None, extra_mag=None):
-        """ours [HW, C] against sum_g w x[g] (+ extra) -> worst ratio.  A float16 `ours` is one rounding of the float32
-        sum: its error is what remains after the half spacing on the side of the reference."""
+        """ours [HW, C] against sum_g w x[g] (+ extra [HW, .]) at the pairs' pixels -> worst ratio.  A float16 `ours` is
+        one rounding of the float32 sum: its error is what remains after the half spacing on the side of the reference."""
+        px = self.pixels
         x = x.double()
         ref = torch.sparse.mm(self.Wt, x)
         mag = torch.sparse.mm(self.Wt, x.abs())
         if extra is not None:
-            ref, mag = ref + extra, mag + extra_mag
-        bar = K * U * (self.n[:, None] + 2) * mag
+            ref, mag = ref + extra[px], mag + extra_mag[px]
+        bar = K * U * (self.n[px, None] + 2) * mag
+        ours = ours[px]
         err = (ours.double() - ref).abs()
         if ours.dtype == torch.float16:
             err = torch.clamp(err - half_rounding(ours.double(), ref), min=0.0)
         return float(_ratio(err, bar).max()) if ref.numel() else 0.0
 
     def terms(self, G):
-        """(sum_p w G, sum_p w |G|, sum_p w |G| (2 n_p + 4)) over the pixels, [P, C] each."""
-        G = G.double()
+        """(sum_p w G, sum_p w |G|, sum_p w |G| (2 n_p + 4)) over the pixels, [P, C] each.  G: [HW, C]."""
+        G = G[self.pixels].double()
         return torch.sparse.mm(self.W, G), torch.sparse.mm(self.W, G.abs()), torch.sparse.mm(self.Wn, G.abs())
 
-    def per_gaussian(self, ours, G):
-        """ours [P, C] against sum_p w G[p] -> worst ratio."""
-        return gaussian_ratio(ours, self.terms(G), self.m)
+    def per_gaussian(self, ours, G, rows=None):
+        """ours [P, C] against sum_p w G[p] -> worst ratio over the Gaussians `rows` (default all)."""
+        return gaussian_ratio(ours, self.terms(G), self.m, rows)
 
 
 def half_rounding(y, ref):
@@ -216,10 +291,13 @@ def half_rounding(y, ref):
     return torch.where(larger | (y == 0), up, down) / 2
 
 
-def gaussian_ratio(ours, terms, m):
+def gaussian_ratio(ours, terms, m, rows=None):
     """Worst |ours - ref| / bar for Weights.terms (summed over views where several add into one result) and the
-    summation lengths m (the pixels each Gaussian blends, over those views)."""
+    summation lengths m (the pixels each Gaussian blends, over those views), over the Gaussians `rows` (index or bool
+    mask; default all)."""
     ref, a, an = terms
+    if rows is not None:
+        ours, ref, a, an, m = ours[rows], ref[rows], a[rows], an[rows], m[rows]
     bar = K * U * (an + m[:, None] * a)
     return float(_ratio((ours.double() - ref).abs(), bar).max()) if ref.numel() else 0.0
 
