@@ -315,6 +315,26 @@ def colour_depth_dots(rec, Gc, Gd):
     return dfn
 
 
+PAIR_CHUNK = 1 << 25  # float64 elements of one [pairs, C] product in pair_dots
+
+
+def pair_dots(F, G, gid, pix):
+    """(sum_c F[gid, c] G[pix, c], sum_c |F[gid, c] G[pix, c]|) per pair in float64, F [P, C] and G [HW, C] of any
+    float type.  The [pairs, C] products are formed over chunks of pairs: a bench-sized window walks millions of pairs,
+    and at C = 256 one product over all of them is several GB."""
+    n = gid.numel()
+    step = max(1, PAIR_CHUNK // max(F.shape[1], 1))
+    if n <= step:
+        fg = F[gid].double() * G[pix].double()
+        return fg.sum(1), fg.abs().sum(1)
+    s = torch.empty(n, dtype=torch.float64, device=gid.device)
+    a = torch.empty_like(s)
+    for i in range(0, n, step):
+        fg = F[gid[i:i + step]].double() * G[pix[i:i + step]].double()
+        s[i:i + step], a[i:i + step] = fg.sum(1), fg.abs().sum(1)
+    return s, a
+
+
 def composite_model(pairs, w, rec, P, dfn, length, bg_dot=None):
     """Float64 model of the composite's geometric gradients over its own records and its blended pairs (extracted
     W > 0), in its own pair order:

@@ -16,9 +16,10 @@ import blend_weights as bw
 from ref_densify import _append, _select, build_rotation
 
 
-def abs_mean2d_model(pairs, w, rec, P, dfn, bg_dot=None):
+def abs_mean2d_model(pairs, w, rec, P, dfn, bg_dot=None, signed=False):
     """[P, 2] float64: per Gaussian, sum over its blended pairs of |t_x| and |t_y|, t the pair's term of dL/dmean2D in
-    the composite's units (0.5 W, 0.5 H), for composite_model's loss with the same dfn and bg_dot."""
+    the composite's units (0.5 W, 0.5 H), for composite_model's loss with the same dfn and bg_dot.  signed: also the
+    pairs' own t [n, 2] and their Gaussians [n], in the order of the blended pairs."""
     W, H, HW = pairs.W, pairs.H, pairs.HW
     sel = pairs.widx[w > 0]
     pix, gid = pairs.pix[sel], pairs.gid[sel]
@@ -41,8 +42,9 @@ def abs_mean2d_model(pairs, w, rec, P, dfn, bg_dot=None):
         T_fin = torch.exp(torch.zeros(HW, dtype=torch.float64, device=pix.device).index_add(0, pix, logf))
         L = L + (T_fin * bgd).sum()
     (gm,) = torch.autograd.grad(L, [mean])
-    t = torch.stack([gm[:, 0] * 0.5 * W, gm[:, 1] * 0.5 * H], 1).abs()
-    return torch.zeros(P, 2, dtype=torch.float64, device=pix.device).index_add_(0, gid, t)
+    t = torch.stack([gm[:, 0] * 0.5 * W, gm[:, 1] * 0.5 * H], 1)
+    out = torch.zeros(P, 2, dtype=torch.float64, device=pix.device).index_add_(0, gid, t.abs())
+    return (out, t, gid) if signed else out
 
 
 def planes_dfn(rec, Gc, Gd, gI):
@@ -60,11 +62,11 @@ def planes_dfn(rec, Gc, Gd, gI):
 
 def feature_dfn(feats, Gf):
     """dfn of the feature walk: d = f_g . Gf_p (feats [P, C], Gf [C, HW])."""
-    F, G = feats.double(), Gf.double()
-
     def dfn(gid, pix):
-        t = F[gid] * G[:, pix].t()
-        return t.sum(1), t.abs().sum(1)
+        if gid.numel() * Gf.shape[0] <= bw.PAIR_CHUNK:
+            t = feats.double()[gid] * Gf.double()[:, pix].t()
+            return t.sum(1), t.abs().sum(1)
+        return bw.pair_dots(feats, Gf.t(), gid, pix)  # bench-sized windows: over chunks of pairs
 
     return dfn
 

@@ -59,15 +59,15 @@ def planes_dfn(rec, Gc, Gd, GI, F=None, Gf=None):
     rz = 1.0 / rec[:, 11].double()
     GI = GI.double().reshape(-1)
     if F is not None:
-        F, Gf = F.double().to(GI.device), Gf.double().to(GI.device)
+        F, Gf = F.to(GI.device), Gf.to(GI.device)
 
     def dfn(gid, pix):
         d, dabs = base(gid, pix)
         t = rz[gid] * GI[pix]
         d, dabs = d + t, dabs + t.abs()
         if F is not None:
-            fg = F[gid] * Gf[pix]
-            d, dabs = d + fg.sum(1), dabs + fg.abs().sum(1)
+            fs, fa = bw.pair_dots(F, Gf, gid, pix)
+            d, dabs = d + fs, dabs + fa
         return d, dabs
 
     return dfn
@@ -83,14 +83,15 @@ def planes_model(pairs, w, rec, P, bg, Gc, Gd, GA, GI, F=None, Gf=None):
                               (bgp.sum(1) - GA, bgp.abs().sum(1) + GA.abs()))
 
 
-def dz_check(Wt, rec, ours, Gd, GI):
-    """dL/dz_g = sum_p w (Gd_p - GI_p / z_g^2) per Gaussian -> worst ratio"""
+def dz_check(Wt, rec, ours, Gd, GI, rows=None):
+    """dL/dz_g = sum_p w (Gd_p - GI_p / z_g^2) per Gaussian -> worst ratio over the Gaussians `rows` (default all)"""
     P = ours.numel()
     r1, a1, n1 = Wt.terms(Gd.reshape(-1, 1))
     r2, a2, n2 = Wt.terms(GI.reshape(-1, 1))
     z = rec[:, 11].double().reshape(-1, 1).to(r1.device)
     iz2 = torch.where(z > 0, 1.0 / (z * z), torch.zeros_like(z))  # culled Gaussians: z = 0 in the record, no pairs
-    return bw.gaussian_ratio(ours.reshape(P, 1), (r1 - r2 * iz2, a1 + a2 * iz2, n1 + n2 * iz2), Wt.m)
+    return bw.gaussian_ratio(ours.reshape(P, 1).to(r1.device), (r1 - r2 * iz2, a1 + a2 * iz2, n1 + n2 * iz2), Wt.m,
+                             rows)
 
 
 def test_negative_controls_the_model_flags_a_dropped_term():

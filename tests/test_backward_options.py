@@ -140,46 +140,61 @@ class Reference:
                                             F=F, Gf=self.Gf if F is not None else None)
         self.Wt = bw.Weights(v.pairs, v.w, v.P)
 
-    def composite(self, o, rho=None, opacity=True):
-        """Worst ratios of the composite's outputs in o (an assigning entry's); rho: antialiased dL_dopacity."""
+    def composite(self, o, rho=None, opacity=True, rows=None):
+        """Worst ratios of the composite's outputs in o (an assigning entry's); rho: antialiased dL_dopacity.  rows:
+        the Gaussians judged (bool mask or index; default all), the contained ones of windowed pairs."""
         assert bool((o["mean2D"][:, 2] == 0).all()) and bool((o["conic"][:, 2] == 0).all())
         g6 = bw.geom6(o["mean2D"], o["conic"], o["opacity"]).double().to(self.ref6.device)
-        r = bw._ratio((g6 - self.ref6).abs(), self.bar6).max(0).values
+        r = bw._ratio((g6 - self.ref6).abs(), self.bar6)
+        r = (r if rows is None else r[rows]).max(0).values
         worst = {k: float(x) for k, x in zip(("dL_dmean2D.x", "dL_dmean2D.y", "dL_dconic.a", "dL_dconic.b",
                                               "dL_dconic.c"), r)}
         if opacity:
-            worst["dL_dopacity"] = self.opacity(o["opacity"], rho)
+            worst["dL_dopacity"] = self.opacity(o["opacity"], rho, rows)
         P = self.ref6.shape[0]
-        worst["dL_dcolor"] = self.Wt.per_gaussian(o["color"].reshape(P, 3), self.Gc)
-        worst["dL_dz"] = dz_check(self.Wt, self.rec, o["dz"], self.Gd, self.GI)
+        worst["dL_dcolor"] = self.Wt.per_gaussian(o["color"].reshape(P, 3), self.Gc, rows)
+        worst["dL_dz"] = dz_check(self.Wt, self.rec, o["dz"], self.Gd, self.GI, rows)
         return worst
 
-    def opacity(self, ours, rho=None):
+    def opacity(self, ours, rho=None, rows=None):
         ref, bar = self.ref6[:, 5].cpu(), self.bar6[:, 5].cpu()
         ours = ours.reshape(-1).cpu().double()
+        keep = torch.ones_like(ref, dtype=torch.bool) if rows is None else _mask(rows, ref.numel())
         if rho is None:
-            return float(bw._ratio((ours - ref).abs(), bar).max())
+            r = bw._ratio((ours - ref).abs(), bar)[keep]
+            return float(r.max()) if r.numel() else 0.0
         ref, bar = rho_opacity(ref, bar, rho["rho"], rho["cond"])
-        r = bw._ratio((ours - ref).abs(), bar)[~rho["needle"]]
+        r = bw._ratio((ours - ref).abs(), bar)[~rho["needle"] & keep]
         return float(r.max()) if r.numel() else 0.0
 
-    def features(self, feat):
+    def features(self, feat, rows=None):
         P = self.ref6.shape[0]
-        return self.Wt.per_gaussian(feat.reshape(P, -1), self.Gf) if self.Gf.shape[1] else 0.0
+        return self.Wt.per_gaussian(feat.reshape(P, -1), self.Gf, rows) if self.Gf.shape[1] else 0.0
 
-    def accumulated(self, o, rho=None):
+    def accumulated(self, o, rho=None, rows=None):
         """The accumulating entry's own outputs, accumulated into zeros: dL_dopacity, dL_dmean2D_out (every term of
         the composite's dL/dmean2D), grad_accum (|dL/dmean2D.xy| of the full model: the model's bars and the sqrt's
-        and the add's rounding) and denom."""
+        and the add's rounding) and denom.  rows: as for composite."""
         ref, bar = self.ref6.cpu(), self.bar6.cpu()
         m2 = o["mean2D"].cpu().double()
         assert bool((m2[:, 2] == 0).all())
-        worst = {"dL_dopacity": self.opacity(o["opacity"], rho),
-                 "dL_dmean2D_out": float(bw._ratio((m2[:, :2] - ref[:, :2]).abs(), bar[:, :2]).max())}
+        keep = torch.ones(ref.shape[0], dtype=torch.bool) if rows is None else _mask(rows, ref.shape[0])
+        worst = {"dL_dopacity": self.opacity(o["opacity"], rho, rows),
+                 "dL_dmean2D_out": float(bw._ratio((m2[:, :2] - ref[:, :2]).abs(), bar[:, :2])[keep].max())}
         n = ref[:, :2].norm(dim=1)
         gbar = bar[:, :2].sum(1) + 2 * bw.U * n
-        worst["grad_accum"] = float(bw._ratio((o["grad_accum"].cpu().double().reshape(-1) - n).abs(), gbar).max())
+        worst["grad_accum"] = float(bw._ratio((o["grad_accum"].cpu().double().reshape(-1) - n).abs(), gbar)[keep].max())
         return worst
+
+
+def _mask(rows, P):
+    """rows (bool mask or index, any device) -> bool [P] on the CPU"""
+    rows = torch.as_tensor(rows).cpu()
+    if rows.dtype == torch.bool:
+        return rows
+    m = torch.zeros(P, dtype=torch.bool)
+    m[rows] = True
+    return m
 
 
 def _inputs(v, ups, feat, mp):

@@ -183,11 +183,12 @@ def test_containment_on_a_hand_made_list():
 # ============================================================================================== GPU
 class BenchView:
     """One camera of a bench scene on the device: test_geometry_grads.View rendering the scene's own features (its
-    forward is bench.py's: _C.rasterize_gaussians), the data-driven windows, and per window the pairs, the weights of
-    the Gaussians in its lists and the contained Gaussians."""
+    forward is bench.py's: _C.rasterize_gaussians; with planes, rasterize_gaussians_alpha_invdepth, antialiased when
+    antialiasing), the data-driven windows, and per window the pairs, the weights of the Gaussians in its lists and the
+    contained Gaussians."""
 
-    def __init__(self, sc, cam, n_windows, group=128, backward=True):
-        v = View(sc, cam, C=sc.C, weights=False)
+    def __init__(self, sc, cam, n_windows, group=128, backward=True, planes=False, antialiasing=False):
+        v = View(sc, cam, C=sc.C, weights=False, planes=planes, antialiasing=antialiasing)
         v.feats = v.d["semantic_feature"]
         v.base = v.forward(v.feats)
         if not backward:  # the forward's buffers are for the backward only; the extraction renders hold their own
@@ -255,8 +256,8 @@ _VIEWS = {}
 
 
 def _bench_view(name, cam, n_windows, **kw):
-    """One BenchView per (config, camera), built once; another config frees the previous one's."""
-    key = (name, cam)
+    """One BenchView per (config, camera, options), built once; another config frees the previous one's."""
+    key = (name, cam) + tuple(sorted(kw.items()))
     if key not in _VIEWS:
         for k in [k for k in _VIEWS if k[0] != name]:
             del _VIEWS[k]
