@@ -257,10 +257,11 @@ int check_dtypes(const Api& api, std::initializer_list<int> codes) {
     return 0;
 }
 
-// Shared body of f3dgs_forward, f3dgs_forward_f16, f3dgs_forward_antialiased and f3dgs_forward_alpha_invdepth.
-// semantic_feature and out_feature_map are float16 if f16, else float32.  antialiasing: op_eff = opacity * rho in the
-// records.  out_alpha / out_invdepth (f3dgs_forward_alpha_invdepth, which has checked that both are given): the
-// composite also writes the opacity and inverse-depth planes.
+// Shared body of f3dgs_forward, f3dgs_forward_f16, f3dgs_forward_antialiased, f3dgs_forward_alpha_invdepth and
+// f3dgs_forward_distortion.  semantic_feature and out_feature_map are float16 if f16, else float32.  antialiasing:
+// op_eff = opacity * rho in the records.  out_alpha / out_invdepth (f3dgs_forward_alpha_invdepth, which has checked that
+// both are given): the composite also writes the opacity and inverse-depth planes.  out_distortion
+// (f3dgs_forward_distortion): the composite also writes the depth distortion plane.
 int forward_impl(const char* entry, f3dgs_alloc_fn geometry_alloc, void* geometry_ctx, f3dgs_alloc_fn binning_alloc,
                  void* binning_ctx, f3dgs_alloc_fn image_alloc, void* image_ctx, int P, int D, int M, int C,
                  const float* background, int width, int height, const float* means3D, const float* shs,
@@ -269,7 +270,7 @@ int forward_impl(const char* entry, f3dgs_alloc_fn geometry_alloc, void* geometr
                  const float* projmatrix, const float* cam_pos, float tan_fovx, float tan_fovy, int prefiltered,
                  float* out_color, void* out_feature_map, float* out_depth, int* radii, int debug, void* cuda_stream,
                  bool f16 = false, bool antialiasing = false, float* out_alpha = nullptr,
-                 float* out_invdepth = nullptr) {
+                 float* out_invdepth = nullptr, float* out_distortion = nullptr) {
     const Api api(entry);
     cudaStream_t stream = (cudaStream_t)cuda_stream;
     if (P < 0 || width <= 0 || height <= 0 || C < 0 || C > F3DGS_MAX_FEATURE_DIM || D < 0 || D > 3)
@@ -290,9 +291,11 @@ int forward_impl(const char* entry, f3dgs_alloc_fn geometry_alloc, void* geometr
     // the composite writes the planes while it writes the other outputs
     const size_t hw4 = (size_t)width * height * 4;
     const Range outs[] = {{out_color, 3 * hw4}, {out_feature_map, (size_t)C * width * height * (f16 ? 2 : 4)},
-                          {out_depth, hw4}, {radii, (size_t)P * 4}, {out_alpha, hw4}, {out_invdepth, hw4}};
+                          {out_depth, hw4}, {radii, (size_t)P * 4}, {out_alpha, hw4}, {out_invdepth, hw4},
+                          {out_distortion, hw4}};
     if (overlaps(outs[4], outs) || overlaps(outs[5], outs))
         return api.invalid("out_alpha / out_invdepth overlap another output");
+    if (overlaps(outs[6], outs)) return api.invalid("out_distortion overlaps another output");
 
     const ViewParams vp = make_view(P, D, M, C, width, height, tan_fovx, tan_fovy, scale_modifier, viewmatrix,
                                     projmatrix, cam_pos);
@@ -388,11 +391,11 @@ int forward_impl(const char* entry, f3dgs_alloc_fn geometry_alloc, void* geometr
         if (f16)
             e = launch_composite_fwd(vp, ranges, point_list, rec, static_cast<const __half*>(semantic_feature),
                                      background, final_T, n_contrib, out_color, static_cast<__half*>(out_feature_map),
-                                     out_depth, counters, stream, out_alpha, out_invdepth);
+                                     out_depth, counters, stream, out_alpha, out_invdepth, out_distortion);
         else
             e = launch_composite_fwd(vp, ranges, point_list, rec, static_cast<const float*>(semantic_feature),
                                      background, final_T, n_contrib, out_color, static_cast<float*>(out_feature_map),
-                                     out_depth, counters, stream, out_alpha, out_invdepth);
+                                     out_depth, counters, stream, out_alpha, out_invdepth, out_distortion);
     }
     if (const int rc = api.cuda(e, "composite_fwd launch")) return rc;
     STAGE_CHECK("composite_fwd");
@@ -468,6 +471,26 @@ int f3dgs_forward_alpha_invdepth(f3dgs_alloc_fn geometry_alloc, void* geometry_c
                         semantic_feature_dtype == F3DGS_F16, antialiasing != 0, out_alpha, out_invdepth);
 }
 
+int f3dgs_forward_distortion(f3dgs_alloc_fn geometry_alloc, void* geometry_ctx, f3dgs_alloc_fn binning_alloc,
+                             void* binning_ctx, f3dgs_alloc_fn image_alloc, void* image_ctx, int P, int D, int M,
+                             int C, const float* background, int width, int height, const float* means3D,
+                             const float* shs, const float* colors_precomp, const void* semantic_feature,
+                             int semantic_feature_dtype, const float* opacities, const float* scales,
+                             float scale_modifier, const float* rotations, const float* cov3D_precomp,
+                             const float* viewmatrix, const float* projmatrix, const float* cam_pos, float tan_fovx,
+                             float tan_fovy, int prefiltered, float* out_color, void* out_feature_map,
+                             float* out_depth, int* radii, int debug, void* cuda_stream, int antialiasing,
+                             float* out_distortion) {
+    const Api api(__func__);
+    if (!out_distortion) return api.invalid("NULL out_distortion");
+    if (const int rc = check_dtypes(api, {semantic_feature_dtype})) return rc;
+    return forward_impl(__func__, geometry_alloc, geometry_ctx, binning_alloc, binning_ctx, image_alloc, image_ctx, P,
+                        D, M, C, background, width, height, means3D, shs, colors_precomp, semantic_feature, opacities,
+                        scales, scale_modifier, rotations, cov3D_precomp, viewmatrix, projmatrix, cam_pos, tan_fovx,
+                        tan_fovy, prefiltered, out_color, out_feature_map, out_depth, radii, debug, cuda_stream,
+                        semantic_feature_dtype == F3DGS_F16, antialiasing != 0, nullptr, nullptr, out_distortion);
+}
+
 }  // extern "C"
 
 namespace {
@@ -537,6 +560,9 @@ struct ViewBackward {
     // accumulating entry's grad_accum_abs [P] (optional)
     bool absgrad = false;
     float *dL_dmean2D_abs = nullptr, *grad_accum_abs = nullptr;
+    // the _distortion entries: the forward's depth plane and the gradient of its depth distortion, added to dL/dalpha
+    // and dL/dz by the composite
+    const float *depth = nullptr, *dL_ddistortion = nullptr;
 };
 
 // The features of a _feature_geometry, _antialiased or _alpha_invdepth entry, after the checks every such entry makes
@@ -612,6 +638,8 @@ int backward(const Api& api, ViewBackward b) {
     if (b.antialiasing && overlaps(opacity, outs)) return api.invalid("dL_dopacity overlaps another output");
     if (overlaps({b.dL_dalpha, hw4}, outs) || overlaps({b.dL_dinvdepth, hw4}, outs))
         return api.invalid("dL_dalpha / dL_dinvdepth overlap an output");
+    if (overlaps({b.depth, hw4}, outs) || overlaps({b.dL_ddistortion, hw4}, outs))
+        return api.invalid("depth / dL_ddistortion overlap an output");
     if (b.accumulate) CUDA_TRY(cudaMemsetAsync(b.scratch, 0, scratch_bytes, stream));
     if (b.accumulate && b.dL_dmean2D_abs) CUDA_TRY(cudaMemsetAsync(b.dL_dmean2D_abs, 0, 3 * p4, stream));
 
@@ -647,7 +675,7 @@ int backward(const Api& api, ViewBackward b) {
             return launch_composite_bwd(vp, fb, b.background, b.dL_dpix, b.dL_depths, dL_dfeaturepix, b.map.scale,
                                         b.dL_dmean2D, b.dL_dconic, dL_dop_eff, b.dL_dcolor, b.dL_dz,
                                         b.dL_dsemantic_feature, stream, b.feat, b.dL_dalpha, b.dL_dinvdepth,
-                                        b.dL_dmean2D_abs);
+                                        b.dL_dmean2D_abs, b.depth, b.dL_ddistortion);
         };
         e = b.map.f16 ? composite(static_cast<const __half*>(b.map.p)) : composite(static_cast<const float*>(b.map.p));
     }
@@ -1072,6 +1100,70 @@ int f3dgs_backward_accum_absgrad(
     b.dL_dalpha = dL_dalpha;
     b.dL_dinvdepth = dL_dinvdepth;
     b.absgrad = true;
+    b.dL_dmean2D_abs = dL_dmean2D_abs;
+    b.grad_accum_abs = grad_accum_abs;
+    return backward(api, b);
+}
+
+int f3dgs_backward_distortion(int P, int D, int M, int R, int C, const float* background, int width, int height,
+                              const float* means3D, const float* shs, const float* colors_precomp,
+                              const void* semantic_feature, int semantic_feature_dtype, const float* scales,
+                              float scale_modifier, const float* rotations, const float* cov3D_precomp,
+                              const float* viewmatrix, const float* projmatrix, const float* cam_pos, float tan_fovx,
+                              float tan_fovy, const int* radii, char* geom_buffer, char* binning_buffer,
+                              char* image_buffer, const float* dL_dpix, const void* dL_dfeaturepix,
+                              int dL_dfeaturepix_dtype, float dL_dfeaturepix_scale, const float* dL_depths,
+                              float* dL_dmean2D, float* dL_dconic, float* dL_dopacity, float* dL_dcolor,
+                              float* dL_dsemantic_feature, float* dL_dmean3D, float* dL_dcov3D, float* dL_dsh,
+                              float* dL_dscale, float* dL_drot, float* dL_dz, int debug, void* cuda_stream,
+                              float* dL_dcamera, int antialiasing, const float* depth, const float* dL_ddistortion,
+                              float* dL_dmean2D_abs) {
+    (void)colors_precomp;
+    const Api api(__func__);
+    if (!depth || !dL_ddistortion) return api.invalid("NULL depth / dL_ddistortion");
+    ViewBackward b{P, D, M, R, C, background, width, height, means3D, shs, scales, scale_modifier, rotations,
+                   cov3D_precomp, viewmatrix, projmatrix, cam_pos, tan_fovx, tan_fovy, radii, geom_buffer,
+                   binning_buffer, image_buffer, dL_dpix,
+                   {dL_dfeaturepix, dL_dfeaturepix_dtype == F3DGS_F16, dL_dfeaturepix_scale}, dL_depths, dL_dmean2D,
+                   dL_dconic, dL_dopacity, dL_dcolor, dL_dsemantic_feature, dL_dmean3D, dL_dcov3D, dL_dsh, dL_dscale,
+                   dL_drot, dL_dz, debug, (cudaStream_t)cuda_stream};
+    if (const int rc = feature_rows(api, b, semantic_feature, semantic_feature_dtype, dL_dfeaturepix_dtype)) return rc;
+    b.dL_dcamera = dL_dcamera;
+    b.antialiasing = antialiasing != 0;
+    b.depth = depth;
+    b.dL_ddistortion = dL_ddistortion;
+    b.absgrad = dL_dmean2D_abs != nullptr;
+    b.dL_dmean2D_abs = dL_dmean2D_abs;
+    return backward(api, b);
+}
+
+int f3dgs_backward_accum_distortion(
+    int P, int D, int M, int R, int C, const float* background, int width, int height, const float* means3D,
+    const float* shs, const float* colors_precomp, const void* semantic_feature, int semantic_feature_dtype,
+    const float* scales, float scale_modifier, const float* rotations, const float* cov3D_precomp,
+    const float* viewmatrix, const float* projmatrix, const float* cam_pos, float tan_fovx, float tan_fovy,
+    const int* radii, char* geom_buffer, char* binning_buffer, char* image_buffer, const float* dL_dpix,
+    const void* dL_dfeaturepix, int dL_dfeaturepix_dtype, float dL_dfeaturepix_scale, const float* dL_depths,
+    char* scratch, float* dL_dopacity, float* dL_dcolors_precomp, float* dL_dsemantic_feature, float* dL_dmean3D,
+    float* dL_dcov3D_precomp, float* dL_dsh, float* dL_dscale, float* dL_drot, float* dL_dmean2D_out,
+    float* grad_accum, float* denom, void* composite_done_event, int debug, void* cuda_stream, float* dL_dcamera,
+    int antialiasing, const float* depth, const float* dL_ddistortion, float* dL_dmean2D_abs, float* grad_accum_abs) {
+    const Api api(__func__);
+    if (!depth || !dL_ddistortion) return api.invalid("NULL depth / dL_ddistortion");
+    if (grad_accum_abs && !dL_dmean2D_abs) return api.invalid("grad_accum_abs needs dL_dmean2D_abs");
+    ViewBackward b{P, D, M, R, C, background, width, height, means3D, shs, scales, scale_modifier, rotations,
+                   cov3D_precomp, viewmatrix, projmatrix, cam_pos, tan_fovx, tan_fovy, radii, geom_buffer,
+                   binning_buffer, image_buffer, dL_dpix,
+                   {dL_dfeaturepix, dL_dfeaturepix_dtype == F3DGS_F16, dL_dfeaturepix_scale}, dL_depths, nullptr,
+                   nullptr, dL_dopacity, dL_dcolors_precomp, dL_dsemantic_feature, dL_dmean3D, dL_dcov3D_precomp,
+                   dL_dsh, dL_dscale, dL_drot, nullptr, debug, (cudaStream_t)cuda_stream, true, scratch,
+                   colors_precomp, dL_dmean2D_out, grad_accum, denom, (cudaEvent_t)composite_done_event};
+    if (const int rc = feature_rows(api, b, semantic_feature, semantic_feature_dtype, dL_dfeaturepix_dtype)) return rc;
+    b.dL_dcamera = dL_dcamera;
+    b.antialiasing = antialiasing != 0;
+    b.depth = depth;
+    b.dL_ddistortion = dL_ddistortion;
+    b.absgrad = dL_dmean2D_abs != nullptr;
     b.dL_dmean2D_abs = dL_dmean2D_abs;
     b.grad_accum_abs = grad_accum_abs;
     return backward(api, b);

@@ -34,6 +34,20 @@
 //       red.global.add into dL_dmean2D_abs[P,3].  The per-pair loop, the parking and the shared memory are those of the
 //       walk without it, so every other output is bitwise unchanged.  With features and FEAT the re-walk flushes its
 //       own terms the same way: the statistic is then sum_p |colour-walk term| + sum_p |feature-walk term|.
+//   DIST           (GEOM and EMIT, opt-in, not with PLANES) the gradient g = dL/dL_p of the forward's depth distortion
+//       L_p = sum_ij w_i w_j |z_i - z_j| = 2 sum_i w_i (z_i A_i - D_i), A_i = 1 - T_i, D_i = sum_{j<i} w_j z_j.  With
+//       Abar_i = sum_{j>i} w_j = T_{i+1} - T_final and Dbar_i = sum_{j>i} w_j z_j (one running register), and D_i
+//       = D_tot - Dbar_i - w_i z_i from the forward's depth plane D_tot:
+//         c_i = dL_p/dw_i = 2 [z_i (A_i - Abar_i) + Dbar_i - D_i]
+//         dL/dalpha_i += T_i (c_i - B_i) g,  B_i = alpha_{i+1} c_{i+1} + (1 - alpha_{i+1}) B_{i+1},  B_last = 0
+//         dL/dz_i     += 2 w_i (A_i - Abar_i) g
+//       The walk keeps E_i = Dbar_i - D_i - w_i z_i = 2 Dbar_i - D_tot in one register (from -D_tot, += 2 w_i z_i per
+//       pair), so c_i = 2 [z_i (A_i - Abar_i) + E_i + w_i z_i]; B is the colour term's recurrence on c, advanced right
+//       away as PLANES advances its 1/z one (three floats per lane with g).  At ties in z the
+//       walk takes the subgradient of blend order: of two pairs at one depth, the later counts as the farther.  The terms
+//       join dL/dalpha and dL/dz, so under ABS the 2-D mean terms include the distortion's share.  The walk reads only
+//       what every forward stores plus the depth plane, and with g = 0 every added term is an exact zero, so every
+//       output is bitwise that of the walk without DIST.
 // 12 warps and a ring without weight slots (RingSlim, 113 KB of shared memory with the reduction tiles): two CTAs per SM,
 // and the alpha warps keep the launch register count (80).
 // As in the reference, the feature loss does not feed dL/dalpha (backward.cu:575 is disabled) unless FEAT is asked for.
@@ -78,6 +92,8 @@ struct BwdArgs {
     float* max_weight;          // SCORE: [P] = max(max_weight, the largest w of the view)
     int64_t* pixel_count;       // SCORE: [P] += the number of pixels the Gaussian blended into
     float* dL_dmean2D_abs;      // ABS: [P,3] += sum over the view's pixels of |2-D mean term| (x, y; z untouched)
+    const float* depth;           // DIST: [H,W] the forward's depth plane D_tot
+    const float* dL_ddistortion;  // DIST: [H,W] g
 };
 
 // GEOM: geometric gradients; EMIT: and the feature lists; LIFT: the feature lists and the per-Gaussian weight sums;
@@ -132,7 +148,7 @@ __device__ __forceinline__ void score_flush_row(const BwdArgs& args, int v, uint
         atomicMax(reinterpret_cast<int*>(args.max_weight + gid), __float_as_int(m));
 }
 
-template <BwdMode MODE, bool PLANES = false, bool ABS = false>
+template <BwdMode MODE, bool PLANES = false, bool ABS = false, bool DIST = false>
 __global__ void __launch_bounds__(kBwdThreads, kSlimCtas)
 composite_bwd_kernel(const BwdArgs args) {
     constexpr bool EMIT = MODE != BwdMode::GEOM && MODE != BwdMode::SCORE;
@@ -168,6 +184,7 @@ composite_bwd_kernel(const BwdArgs args) {
         float T, T_final, pxf, pyf, fbx0, fby0, dLp0, dLp1, dLp2, dLd, bg_dot;
         float ar0, ar1, ar2, lc0, lc1, lc2, last_alpha, accum_depth, last_depth;
         float gI, accum_invd;  // PLANES: dL/dI_p, and the 1/z recurrence's value for the pair the walk reaches next
+        float gD, Ed, Bd;  // DIST: dL/dL_p, and E and B of the pair the walk reaches next
         uint32_t last_contrib, wmax;
         bool inside;
     } p = Px{};
@@ -254,6 +271,11 @@ composite_bwd_kernel(const BwdArgs args) {
                     p.bg_dot -= p.inside ? args.dL_dalpha[pix] : 0.f;
                     p.accum_invd = 0.f;
                 }
+                if constexpr (DIST) {
+                    p.gD = p.inside ? args.dL_ddistortion[pix] : 0.f;
+                    p.Ed = p.inside ? -args.depth[pix] : 0.f;
+                    p.Bd = 0.f;
+                }
             }
             p.ar0 = p.ar1 = p.ar2 = p.lc0 = p.lc1 = p.lc2 = 0.f;
             p.last_alpha = p.accum_depth = p.last_depth = 0.f;
@@ -328,6 +350,7 @@ composite_bwd_kernel(const BwdArgs args) {
                         // the background term, where the reference divides twice (backward.cu:541,583); the
                         // unwound T differs from the reference's by a few ulp after a whole tile list.
                         const float inv_1ma = rcp_approx(1.f - alpha);
+                        [[maybe_unused]] const float T_next = p.T;  // DIST: T_{i+1}
                         p.T = p.T * inv_1ma;
                         wgt = alpha * p.T;
                         float dL_dalpha;
@@ -347,6 +370,15 @@ composite_bwd_kernel(const BwdArgs args) {
                             dL_dalpha += (rz - p.accum_invd) * p.gI;
                             p.accum_invd = alpha * rz + (1.f - alpha) * p.accum_invd;
                             dLdz -= p.gI * (rz * rz);  // dI/dz_i = -w_i / z_i^2
+                        }
+                        if constexpr (DIST) {
+                            const float dA = (1.f - p.T) - (T_next - p.T_final);  // A_i - Abar_i
+                            const float wz = wgt * r2.w;
+                            const float c = 2.f * (r2.w * dA + (p.Ed + wz));  // dL_p/dw_i
+                            dL_dalpha += (c - p.Bd) * p.gD;
+                            p.Bd = alpha * c + (1.f - alpha) * p.Bd;
+                            p.Ed += 2.f * wz;
+                            dLdz += 2.f * dA * p.gD;
                         }
                         dL_dalpha *= p.T;
                         p.last_alpha = alpha;
@@ -426,7 +458,7 @@ static cudaError_t alloc_lists(size_t R, size_t tiles, char** mem, InstanceLists
 // feature_bwd over them (SCORE has neither), reducing sum_p w * scale * map[:, p] into dst.  `a` brings the mode's outputs.  With features
 // (EMIT only), feature_dot then turns the lists' weights into pair dot products and the FEAT walk adds the feature term
 // to the geometric gradients; the lists are freed after it.
-template <BwdMode MODE, typename TG, bool PLANES = false, bool ABS = false>
+template <BwdMode MODE, typename TG, bool PLANES = false, bool ABS = false, bool DIST = false>
 static cudaError_t run_bwd(BwdArgs a, const ViewParams& vp, const ForwardBuffers& fb, const TG* map, float scale,
                            float* dst, cudaStream_t s, const FeatureRows& feat = {}) {
     a.pa = producer_args(vp, fb.ranges, fb.point_list, fb.rec, fb.n_contrib, fb.counters + kCounterBwdGeom);
@@ -446,7 +478,11 @@ static cudaError_t run_bwd(BwdArgs a, const ViewParams& vp, const ForwardBuffers
                                composite_bwd_kernel<BwdMode::EMIT, false, true>,
                                composite_bwd_kernel<BwdMode::GEOM, true, true>,
                                composite_bwd_kernel<BwdMode::EMIT, true, true>,
-                               composite_bwd_kernel<BwdMode::FEAT, false, true>>(
+                               composite_bwd_kernel<BwdMode::FEAT, false, true>,
+                               composite_bwd_kernel<BwdMode::GEOM, false, false, true>,
+                               composite_bwd_kernel<BwdMode::EMIT, false, false, true>,
+                               composite_bwd_kernel<BwdMode::GEOM, false, true, true>,
+                               composite_bwd_kernel<BwdMode::EMIT, false, true, true>>(
         num_sms, sizeof(BwdSmem), kBwdThreads, kSlimCtas);
     const int grid = min(a.pa.num_tiles, kSlimCtas * num_sms);
     auto walk = [&](void (*kernel)(BwdArgs)) {
@@ -456,7 +492,7 @@ static cudaError_t run_bwd(BwdArgs a, const ViewParams& vp, const ForwardBuffers
         g_launches++;
         return cudaGetLastError();
     };
-    if (e == cudaSuccess) e = walk(composite_bwd_kernel<MODE, PLANES, ABS>);
+    if (e == cudaSuccess) e = walk(composite_bwd_kernel<MODE, PLANES, ABS, DIST>);
     if (lists) {
         if (e == cudaSuccess) e = launch_feature_bwd(vp, fb.ranges, a.lists, map, scale, dst, fb.counters, s);
         if (MODE == BwdMode::EMIT && feat.rows) {
@@ -473,16 +509,23 @@ cudaError_t launch_composite_bwd(const ViewParams& vp, const ForwardBuffers& fb,
                                  const float* dL_ddepth, const TG* dL_dfeat_pix, float dL_dfeat_pix_scale,
                                  float* dL_dmean2D, float* dL_dconic, float* dL_dopacity, float* dL_dcolor, float* dL_dz,
                                  float* dL_dfeature, cudaStream_t s, const FeatureRows& feat, const float* dL_dalpha,
-                                 const float* dL_dinvdepth, float* dL_dmean2D_abs) {
+                                 const float* dL_dinvdepth, float* dL_dmean2D_abs, const float* depth,
+                                 const float* dL_ddistortion) {
     BwdArgs a{};
     a.bg = bg; a.dL_dpix = dL_dpix; a.dL_ddepth = dL_ddepth;
     a.dL_dmean2D = dL_dmean2D; a.dL_dconic = dL_dconic; a.dL_dopacity = dL_dopacity; a.dL_dcolor = dL_dcolor;
     a.dL_dz = dL_dz;
     a.dL_dalpha = dL_dalpha; a.dL_dinvdepth = dL_dinvdepth;
     a.dL_dmean2D_abs = dL_dmean2D_abs;
+    a.depth = depth; a.dL_ddistortion = dL_ddistortion;
     const bool emit = vp.C > 0 && fb.R > 0;
     const auto run =
-        dL_dmean2D_abs
+        dL_ddistortion
+            ? (dL_dmean2D_abs
+                   ? (emit ? run_bwd<BwdMode::EMIT, TG, false, true, true> : run_bwd<BwdMode::GEOM, TG, false, true, true>)
+                   : (emit ? run_bwd<BwdMode::EMIT, TG, false, false, true>
+                           : run_bwd<BwdMode::GEOM, TG, false, false, true>))
+        : dL_dmean2D_abs
             ? (dL_dalpha ? (emit ? run_bwd<BwdMode::EMIT, TG, true, true> : run_bwd<BwdMode::GEOM, TG, true, true>)
                          : (emit ? run_bwd<BwdMode::EMIT, TG, false, true> : run_bwd<BwdMode::GEOM, TG, false, true>))
             : (dL_dalpha ? (emit ? run_bwd<BwdMode::EMIT, TG, true> : run_bwd<BwdMode::GEOM, TG, true>)
@@ -508,11 +551,11 @@ cudaError_t launch_gaussian_scores(const ViewParams& vp, const ForwardBuffers& f
 template cudaError_t launch_composite_bwd(const ViewParams&, const ForwardBuffers&, const float*, const float*,
                                           const float*, const float*, float, float*, float*, float*, float*, float*,
                                           float*, cudaStream_t, const FeatureRows&, const float*, const float*,
-                                          float*);
+                                          float*, const float*, const float*);
 template cudaError_t launch_composite_bwd(const ViewParams&, const ForwardBuffers&, const float*, const float*,
                                           const float*, const __half*, float, float*, float*, float*, float*, float*,
                                           float*, cudaStream_t, const FeatureRows&, const float*, const float*,
-                                          float*);
+                                          float*, const float*, const float*);
 template cudaError_t launch_feature_lift(const ViewParams&, const ForwardBuffers&, const float*, float*, float*,
                                          cudaStream_t);
 template cudaError_t launch_feature_lift(const ViewParams&, const ForwardBuffers&, const __half*, float*, float*,

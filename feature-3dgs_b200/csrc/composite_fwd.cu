@@ -38,6 +38,12 @@
 // final_T) and the inverse-depth plane I.  Nothing else the kernel computes or stores changes, so colour, depth, the
 // feature map, final_T and n_contrib are bitwise those of the kernel without the planes.
 //
+// DIST (opt-in, not with PLANES): the alpha warps also accumulate the depth distortion loss
+// L_p = sum_ij w_i w_j |z_i - z_j| = 2 sum_i w_i (z_i A_i - D_i), A_i = 1 - T_i, D_i = sum_{j<i} w_j z_j, with z_i the
+// record's view depth.  The tile sort key orders each tile list by z, so this prefix-sum form is the pairwise sum.  Per
+// blended pair Q += w (z (1 - T) - Dp) before Dp takes the pair, and the epilogue writes 2Q.  As with PLANES nothing else
+// changes, so every other output is bitwise that of the kernel without it.
+//
 // Registers: with features the 28 warps are launched at 72 registers per thread (64512 in the CTA pool); setmaxnreg
 // then gives the producer group 40, the alpha warps 56 and the feature warps 88 (4x32x40 + 8x32x56 + 16x32x88 =
 // 64512).  (setmaxnreg acts per warpgroup of 4 consecutive warps, so the producer group is one unit.)  Without
@@ -68,6 +74,7 @@ struct FwdArgs {
     int vec_store;
     float* out_alpha;     // PLANES: [H,W] 1 - final_T
     float* out_invdepth;  // PLANES: [H,W] sum_i w_i / z_i
+    float* out_distortion;  // DIST: [H,W] sum_ij w_i w_j |z_i - z_j|
 };
 
 // A lane's 4 channels of a staged feature row as loaded (float4, or 8 bytes of float16; to_float4 makes them float32).
@@ -91,7 +98,7 @@ __device__ __forceinline__ void st_run(__half* p, float4 v) {
 __device__ __forceinline__ void st_px(float* p, float v) { *p = v; }
 __device__ __forceinline__ void st_px(__half* p, float v) { *p = __float2half_rn(v); }
 
-template <int CH, typename TF, bool PLANES>
+template <int CH, typename TF, bool PLANES, bool DIST = false>
 __global__ void __launch_bounds__(kFwdThreads<CH>, 1)
 composite_fwd_kernel(const FwdArgs<TF> args) {
     extern __shared__ __align__(128) unsigned char smem_raw[];
@@ -127,6 +134,7 @@ composite_fwd_kernel(const FwdArgs<TF> args) {
         uint32_t parity = 0, wparity = 1;  // wempty: fresh barrier falls through on parity 1
         float T = 1.f, Cr = 0.f, Cg = 0.f, Cb = 0.f, Dp = 0.f, pxf = 0.f, pyf = 0.f, fbx0 = 0.f, fby0 = 0.f;
         float Ip = 0.f;  // PLANES
+        float Q = 0.f;   // DIST: half the distortion so far
         uint32_t last_contrib = 0;
         int px = 0, py = 0, chunk = 0;
         bool done = true, inside = false, blk_done = true;
@@ -149,6 +157,7 @@ composite_fwd_kernel(const FwdArgs<TF> args) {
                 fbx0 = (float)bx0; fby0 = (float)by0;
                 T = 1.f; Cr = Cg = Cb = Dp = 0.f;
                 if constexpr (PLANES) Ip = 0.f;
+                if constexpr (DIST) Q = 0.f;
                 last_contrib = 0;
                 done = !inside;
                 blk_done = __all_sync(0xffffffffu, done);
@@ -192,6 +201,10 @@ composite_fwd_kernel(const FwdArgs<TF> args) {
                         const float nCg = Cg + r2.y * alpha * T;
                         const float nCb = Cb + r2.z * alpha * T;
                         const float nDp = Dp + r2.w * (alpha * T);
+                        if constexpr (DIST) {  // before Dp takes this pair: Dp = D_i, 1 - T = A_i
+                            const float nQ = Q + (alpha * T) * (r2.w * (1.f - T) - Dp);
+                            Q = blend ? nQ : Q;
+                        }
                         Cr = blend ? nCr : Cr;
                         Cg = blend ? nCg : Cg;
                         Cb = blend ? nCb : Cb;
@@ -241,6 +254,7 @@ composite_fwd_kernel(const FwdArgs<TF> args) {
                     args.out_alpha[pix] = 1.f - T;
                     args.out_invdepth[pix] = Ip;
                 }
+                if constexpr (DIST) args.out_distortion[pix] = 2.f * Q;
             }
             if (++s == kStages) { s = 0; parity ^= 1; }
             if (CH > 0 && ++j == kWSlots) { j = 0; wparity ^= 1; }
@@ -368,14 +382,15 @@ composite_fwd_kernel(const FwdArgs<TF> args) {
 #undef FEAT_ROW_FMA
 }
 
-template <int CH, typename TF, bool PLANES>
+template <int CH, typename TF, bool PLANES, bool DIST = false>
 static cudaError_t launch_fwd_t(const ViewParams& vp, const uint2* ranges, const uint32_t* point_list,
                                 const SplatRec* rec, const TF* features, const float* bg, float* final_T,
                                 uint32_t* n_contrib, float* out_color, TF* out_feature, float* out_depth,
-                                int* work_counter, cudaStream_t s, float* out_alpha, float* out_invdepth) {
+                                int* work_counter, cudaStream_t s, float* out_alpha, float* out_invdepth,
+                                float* out_distortion) {
     const size_t smem = sizeof(RingV2<CH, TF>);
     int num_sms = 0;
-    cudaError_t e = device_sms<composite_fwd_kernel<CH, TF, PLANES>>(num_sms, smem);
+    cudaError_t e = device_sms<composite_fwd_kernel<CH, TF, PLANES, DIST>>(num_sms, smem);
     if (e != cudaSuccess) return e;
     FwdArgs<TF> a;
     a.pa = producer_args(vp, ranges, point_list, rec, nullptr, work_counter);
@@ -388,7 +403,7 @@ static cudaError_t launch_fwd_t(const ViewParams& vp, const uint2* ranges, const
     a.pa.use_bulk = (CH > 0 && vp.C % kPer16 == 0 && (reinterpret_cast<uintptr_t>(features) & 15) == 0) ? 1 : 0;
     a.bg = bg; a.final_T = final_T; a.n_contrib = n_contrib;
     a.out_color = out_color; a.out_feature = out_feature; a.out_depth = out_depth;
-    a.out_alpha = out_alpha; a.out_invdepth = out_invdepth;
+    a.out_alpha = out_alpha; a.out_invdepth = out_invdepth; a.out_distortion = out_distortion;
     // 1: 4-pixel stores (16 B of float, 8 B of half); 2: 8-pixel rows (32 B of float, 16 B of half)
     const uintptr_t out_addr = reinterpret_cast<uintptr_t>(out_feature);
     a.vec_store = (vp.W % 4 == 0 && (out_addr & (4 * sizeof(TF) - 1)) == 0) ? 1 : 0;
@@ -396,7 +411,7 @@ static cudaError_t launch_fwd_t(const ViewParams& vp, const uint2* ranges, const
     e = cudaMemsetAsync(work_counter, 0, sizeof(int), s);
     if (e != cudaSuccess) return e;
     const int grid = min(a.pa.num_tiles * a.pa.chunks, num_sms);
-    composite_fwd_kernel<CH, TF, PLANES><<<grid, kFwdThreads<CH>, smem, s>>>(a);
+    composite_fwd_kernel<CH, TF, PLANES, DIST><<<grid, kFwdThreads<CH>, smem, s>>>(a);
     g_launches++;
     return cudaGetLastError();
 }
@@ -406,30 +421,35 @@ cudaError_t launch_composite_fwd(const ViewParams& vp, const uint2* ranges, cons
                                  const SplatRec* rec, const TF* features, const float* bg,
                                  float* final_T, uint32_t* n_contrib, float* out_color,
                                  TF* out_feature, float* out_depth, int* counters, cudaStream_t s, float* out_alpha,
-                                 float* out_invdepth) {
+                                 float* out_invdepth, float* out_distortion) {
     int* const work_counter = counters + kCounterFwd;
     if (vp.C == 0) {  // no feature rows or map: one kernel for both element types
-        const auto launch0 = out_alpha ? launch_fwd_t<0, float, true> : launch_fwd_t<0, float, false>;
+        const auto launch0 = out_distortion ? launch_fwd_t<0, float, false, true>
+                             : out_alpha    ? launch_fwd_t<0, float, true>
+                                            : launch_fwd_t<0, float, false>;
         return launch0(vp, ranges, point_list, rec, nullptr, bg, final_T, n_contrib, out_color, nullptr, out_depth,
-                       work_counter, s, out_alpha, out_invdepth);
+                       work_counter, s, out_alpha, out_invdepth, out_distortion);
     }
     const int ch = channel_chunk(vp.C);
-    const auto launch = out_alpha ? (ch == 32   ? launch_fwd_t<32, TF, true>
-                                     : ch == 64 ? launch_fwd_t<64, TF, true>
-                                                : launch_fwd_t<128, TF, true>)
-                                  : (ch == 32   ? launch_fwd_t<32, TF, false>
-                                     : ch == 64 ? launch_fwd_t<64, TF, false>
-                                                : launch_fwd_t<128, TF, false>);
+    const auto launch = out_distortion ? (ch == 32   ? launch_fwd_t<32, TF, false, true>
+                                          : ch == 64 ? launch_fwd_t<64, TF, false, true>
+                                                     : launch_fwd_t<128, TF, false, true>)
+                        : out_alpha    ? (ch == 32   ? launch_fwd_t<32, TF, true>
+                                          : ch == 64 ? launch_fwd_t<64, TF, true>
+                                                     : launch_fwd_t<128, TF, true>)
+                                       : (ch == 32   ? launch_fwd_t<32, TF, false>
+                                          : ch == 64 ? launch_fwd_t<64, TF, false>
+                                                     : launch_fwd_t<128, TF, false>);
     return launch(vp, ranges, point_list, rec, features, bg, final_T, n_contrib, out_color, out_feature, out_depth,
-                  work_counter, s, out_alpha, out_invdepth);
+                  work_counter, s, out_alpha, out_invdepth, out_distortion);
 }
 
 template cudaError_t launch_composite_fwd<float>(const ViewParams&, const uint2*, const uint32_t*, const SplatRec*,
                                                  const float*, const float*, float*, uint32_t*, float*, float*, float*,
-                                                 int*, cudaStream_t, float*, float*);
+                                                 int*, cudaStream_t, float*, float*, float*);
 template cudaError_t launch_composite_fwd<__half>(const ViewParams&, const uint2*, const uint32_t*, const SplatRec*,
                                                   const __half*, const float*, float*, uint32_t*, float*, __half*,
-                                                  float*, int*, cudaStream_t, float*, float*);
+                                                  float*, int*, cudaStream_t, float*, float*, float*);
 
 }  // namespace f3dgs
 

@@ -60,13 +60,15 @@ void launch_tile_ranges(int R, const uint64_t* sorted_keys, uint2* ranges, cudaS
 // returns cudaSuccess or the launch error.  TF (float or __half) is the element type of features and out_feature: the
 // float16 map is bitwise the float32 map of the exactly upcast features rounded to nearest even.  With out_alpha (then
 // out_invdepth too, both [H,W]): also the opacity plane 1 - final_T and the inverse-depth plane sum_i w_i / z_i; every
-// other output is bitwise that of the call without them
+// other output is bitwise that of the call without them.  With out_distortion ([H,W], not with out_alpha): also the depth
+// distortion sum_ij w_i w_j |z_i - z_j| per pixel, every other output again bitwise unchanged
 template <typename TF>
 cudaError_t launch_composite_fwd(const ViewParams& vp, const uint2* ranges, const uint32_t* point_list,
                                  const SplatRec* rec, const TF* features, const float* bg,
                                  float* final_T, uint32_t* n_contrib, float* out_color,
                                  TF* out_feature, float* out_depth, int* counters, cudaStream_t s,
-                                 float* out_alpha = nullptr, float* out_invdepth = nullptr);
+                                 float* out_alpha = nullptr, float* out_invdepth = nullptr,
+                                 float* out_distortion = nullptr);
 
 // ---- composite_bwd.cu + feature_bwd.cu: the composite backward of a view, from that view's forward buffers
 struct ForwardBuffers {
@@ -93,14 +95,17 @@ struct FeatureRows {
 // dL/dalpha and dL_dz in the same geometry walk; with both zero every output is bitwise that of the call without them.
 // With dL_dmean2D_abs ([P,3], added to; the third column untouched): AbsGS's statistic, the sums over the view's pixels
 // of |x| and |y| of each pixel's 2-D mean term, from the same walk (and the feature walk's own terms with feat.rows);
-// every other output is bitwise that of the call without it.
+// every other output is bitwise that of the call without it.  With dL_ddistortion (then depth too, both [H,W]; not with
+// dL_dalpha): the gradient of the forward's depth distortion, from the forward's depth plane `depth`, joins dL/dalpha
+// and dL_dz in the same walk; with it zero every output is bitwise that of the call without it.
 template <typename TG>
 cudaError_t launch_composite_bwd(const ViewParams& vp, const ForwardBuffers& fb, const float* bg, const float* dL_dpix,
                                  const float* dL_ddepth, const TG* dL_dfeat_pix, float dL_dfeat_pix_scale,
                                  float* dL_dmean2D, float* dL_dconic, float* dL_dopacity, float* dL_dcolor, float* dL_dz,
                                  float* dL_dfeature, cudaStream_t s, const FeatureRows& feat = {},
                                  const float* dL_dalpha = nullptr, const float* dL_dinvdepth = nullptr,
-                                 float* dL_dmean2D_abs = nullptr);
+                                 float* dL_dmean2D_abs = nullptr, const float* depth = nullptr,
+                                 const float* dL_ddistortion = nullptr);
 // Feature lifting, R > 0: weight_sum[P] += the blend weights w = alpha*T of each Gaussian over the view and
 // feature_sum[P, C] += sum_p w * map[:, p], through the same lists.  TF (float or __half) is the element type of map
 template <typename TF>

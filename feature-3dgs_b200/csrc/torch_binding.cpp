@@ -20,7 +20,12 @@
 // semantic_feature=None, antialiasing=False) -> the same 12 as rasterize_gaussians_backward_antialiased
 // (f3dgs_backward_alpha_invdepth).  AbsGS's densification statistic:
 // rasterize_gaussians_backward_absgrad(the backward's arguments, dL_dout_alpha=None, dL_dout_invdepth=None, camera=False,
-// semantic_feature=None, antialiasing=False) -> the same 12 and dL_dmeans2D_abs [P,3] (f3dgs_backward_absgrad).
+// semantic_feature=None, antialiasing=False) -> the same 12 and dL_dmeans2D_abs [P,3] (f3dgs_backward_absgrad).  Depth
+// distortion: rasterize_gaussians_distortion(rasterize_gaussians' arguments, antialiasing=False) -> (num_rendered, color,
+// feature_map, depth, distortion, radii, geom, binning, img) (f3dgs_forward_distortion) and
+// rasterize_gaussians_backward_distortion(the backward's arguments, depth, dL_ddistortion, camera=False,
+// semantic_feature=None, antialiasing=False, dL_dmean2D_abs=None) -> the same 12 as
+// rasterize_gaussians_backward_antialiased (f3dgs_backward_distortion; dL_dmean2D_abs [P,3] is added to).
 // Differences (all permissive): the feature width is read from semantic_feature.size(-1) at run
 // time (reference: compile-time NUM_SEMANTIC_CHANNELS, config.h:16); an empty / undefined
 // semantic_feature means C = 0; semantic_feature may be float32 or float16, and the feature map
@@ -138,10 +143,12 @@ using ForwardResults = std::tuple<int, torch::Tensor, torch::Tensor, torch::Tens
     background, means3D, colors, semantic_feature, opacity, scales, rotations, scale_modifier, cov3D_precomp,         \
         viewmatrix, projmatrix, tan_fovx, tan_fovy, image_height, image_width, sh, degree, campos, prefiltered, debug
 
-// Body of rasterize_gaussians, rasterize_gaussians_antialiased (f3dgs_forward_antialiased) and, with `planes` (two
-// tensors it sets to the [1,H,W] opacity and inverse-depth planes), rasterize_gaussians_alpha_invdepth
-// (f3dgs_forward_alpha_invdepth)
-static ForwardResults forward(FORWARD_PARAMS, const bool antialiasing, torch::Tensor* planes = nullptr) {
+// Body of rasterize_gaussians, rasterize_gaussians_antialiased (f3dgs_forward_antialiased), with `planes` (two
+// tensors it sets to the [1,H,W] opacity and inverse-depth planes) rasterize_gaussians_alpha_invdepth
+// (f3dgs_forward_alpha_invdepth), and with `distortion` (set to the [1,H,W] distortion plane)
+// rasterize_gaussians_distortion (f3dgs_forward_distortion)
+static ForwardResults forward(FORWARD_PARAMS, const bool antialiasing, torch::Tensor* planes = nullptr,
+                              torch::Tensor* distortion = nullptr) {
     if (means3D.ndimension() != 2 || means3D.size(1) != 3) {
         AT_ERROR("means3D must have dimensions (num_points, 3)");
     }
@@ -166,6 +173,7 @@ static ForwardResults forward(FORWARD_PARAMS, const bool antialiasing, torch::Te
     torch::Tensor radii = torch::empty({P}, means3D.options().dtype(torch::kInt32));
     if (planes)
         for (int k = 0; k < 2; k++) planes[k] = P ? torch::empty({1, H, W}, float_opts) : torch::zeros({1, H, W}, float_opts);
+    if (distortion) *distortion = P ? torch::empty({1, H, W}, float_opts) : torch::zeros({1, H, W}, float_opts);
 
     auto byte_opts = torch::TensorOptions().dtype(torch::kByte).device(dev);
     torch::Tensor geomBuffer = torch::empty({0}, byte_opts);
@@ -195,6 +203,15 @@ static ForwardResults forward(FORWARD_PARAMS, const bool antialiasing, torch::Te
                 out_depth.data_ptr<float>(), radii.data_ptr<int>(), debug ? 1 : 0, (void*)stream, antialiasing ? 1 : 0,
                 planes[0].data_ptr<float>(), planes[1].data_ptr<float>());
             check_rc(rendered, "f3dgs_forward_alpha_invdepth");
+        } else if (distortion) {
+            rendered = f3dgs_forward_distortion(
+                resize_tensor, &geomBuffer, resize_tensor, &binningBuffer, resize_tensor, &imgBuffer, P, degree, M, C,
+                fptr(bg), W, H, fptr(m3), fptr(shc), fptr(col), has_sf ? sf.data_ptr() : nullptr, dtype_code(sf),
+                fptr(op), fptr(sc), scale_modifier, fptr(rot), fptr(cov), fptr(vm), fptr(pm), fptr(cp), tan_fovx,
+                tan_fovy, prefiltered ? 1 : 0, out_color.data_ptr<float>(), C ? out_feature.data_ptr() : nullptr,
+                out_depth.data_ptr<float>(), radii.data_ptr<int>(), debug ? 1 : 0, (void*)stream, antialiasing ? 1 : 0,
+                distortion->data_ptr<float>());
+            check_rc(rendered, "f3dgs_forward_distortion");
         } else if (antialiasing) {
             rendered = f3dgs_forward_antialiased(
                 resize_tensor, &geomBuffer, resize_tensor, &binningBuffer, resize_tensor, &imgBuffer, P, degree, M, C,
@@ -228,6 +245,14 @@ RasterizeGaussiansAlphaInvDepthCUDA(FORWARD_PARAMS, const bool antialiasing) {
     const auto [rendered, color, feature, depth, radii, geom, binning, img] = forward(FORWARD_ARGS, antialiasing, planes);
     return std::make_tuple(rendered, color, feature, depth, planes[0], planes[1], radii, geom, binning, img);
 }
+std::tuple<int, torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor,
+           torch::Tensor>
+RasterizeGaussiansDistortionCUDA(FORWARD_PARAMS, const bool antialiasing) {
+    torch::Tensor distortion;
+    const auto [rendered, color, feature, depth, radii, geom, binning, img] =
+        forward(FORWARD_ARGS, antialiasing, nullptr, &distortion);
+    return std::make_tuple(rendered, color, feature, depth, distortion, radii, geom, binning, img);
+}
 #undef FORWARD_PARAMS
 #undef FORWARD_ARGS
 
@@ -240,7 +265,8 @@ using BackwardGrads = std::tuple<torch::Tensor, torch::Tensor, torch::Tensor, to
 // with antialiasing, f3dgs_backward_antialiased, whose feature term reads `features` if that is given; with `planes`
 // (the gradients of the opacity and inverse-depth planes), f3dgs_backward_alpha_invdepth, with the feature term as under
 // antialiasing and the forward's mode `antialiasing`; with `abs_out` (set to the [P,3] statistic), f3dgs_backward_absgrad,
-// with the planes when `planes` is given, and otherwise as f3dgs_backward_alpha_invdepth
+// with the planes when `planes` is given, and otherwise as f3dgs_backward_alpha_invdepth; with `dist` (the forward's depth
+// plane and the distortion's gradient), f3dgs_backward_distortion, adding AbsGS's statistic into `dist_abs` if given
 static BackwardGrads backward_grads(const torch::Tensor& background, const torch::Tensor& means3D,
                                const torch::Tensor& radii, const torch::Tensor& colors,
                                const torch::Tensor& semantic_feature, const torch::Tensor& scales,
@@ -253,7 +279,8 @@ static BackwardGrads backward_grads(const torch::Tensor& background, const torch
                                const torch::Tensor& binningBuffer, const torch::Tensor& imageBuffer,
                                const bool debug, float* camera, bool feature_geometry = false,
                                bool antialiasing = false, const torch::Tensor& features = torch::Tensor(),
-                               const torch::Tensor* planes = nullptr, torch::Tensor* abs_out = nullptr) {
+                               const torch::Tensor* planes = nullptr, torch::Tensor* abs_out = nullptr,
+                               const torch::Tensor* dist = nullptr, float* dist_abs = nullptr) {
     TORCH_CHECK(means3D.is_cuda(), "means3D must be a CUDA tensor (this build has no CPU path)");
     const c10::cuda::CUDAGuard guard(means3D.device());
     const auto dev = means3D.device();
@@ -344,7 +371,15 @@ static BackwardGrads backward_grads(const torch::Tensor& background, const torch
                         " elements (got ", t.numel(), ")");
             return t.contiguous();
         };
-        if (abs_out) {
+        if (dist) {
+            auto depth = input(dist[0], dev, "depth");
+            TORCH_CHECK(depth.defined() && depth.numel() == (int64_t)H * W, "depth must have H * W = ", (int64_t)H * W,
+                        " elements (got ", depth.defined() ? depth.numel() : 0, ")");
+            auto gD = plane_grad(dist[1], dev, H, W, "dL_ddistortion");
+            check_rc(typed_call(f3dgs_backward_distortion, feature_rows(features), antialiasing ? 1 : 0, fptr(depth),
+                                fptr(gD), dist_abs),
+                     "f3dgs_backward_distortion");
+        } else if (abs_out) {
             torch::Tensor ga, gi;
             if (planes) {
                 ga = plane_grad(planes[0], dev, H, W, "dL_dout_alpha");
@@ -457,6 +492,23 @@ RasterizeGaussiansBackwardAbsGradCUDA(BACKWARD_PARAMS, const std::optional<torch
     });
     return std::tuple_cat(grads, std::make_tuple(abs));
 }
+// rasterize_gaussians_backward_antialiased's 12 results for the buffers of rasterize_gaussians_distortion (or of the
+// forward without it in the same mode) and that forward's depth plane, with the gradient of the depth distortion
+// (f3dgs_backward_distortion); dL_dmean2D_abs (optional, [P,3] contiguous float32) is added AbsGS's statistic
+CameraGrads RasterizeGaussiansBackwardDistortionCUDA(BACKWARD_PARAMS, const torch::Tensor& depth,
+                                                     const torch::Tensor& dL_ddistortion, const bool camera,
+                                                     const std::optional<torch::Tensor>& features,
+                                                     const bool antialiasing,
+                                                     const std::optional<torch::Tensor>& dL_dmean2D_abs) {
+    const torch::Tensor f = features.has_value() ? *features : torch::Tensor();
+    const torch::Tensor dist[2] = {depth, dL_ddistortion};
+    float* abs = dL_dmean2D_abs.has_value() && dL_dmean2D_abs->defined()
+                     ? in_place(*dL_dmean2D_abs, means3D.device(), means3D.size(0) * 3, "dL_dmean2D_abs")
+                     : nullptr;
+    return with_camera_grads(means3D, camera, [&](float* cam) {
+        return backward_grads(BACKWARD_ARGS, cam, false, antialiasing, f, nullptr, nullptr, dist, abs);
+    });
+}
 #undef BACKWARD_PARAMS
 #undef BACKWARD_ARGS
 
@@ -469,7 +521,9 @@ RasterizeGaussiansBackwardAbsGradCUDA(BACKWARD_PARAMS, const std::optional<torch
 // (optional; one given alone: the other is zero): f3dgs_backward_accum_alpha_invdepth, the gradients of the opacity and
 // inverse-depth planes, for the buffers of either forward in the mode `antialiasing`.  dL_dmean2D_abs (optional, [P,3]
 // contiguous float32): f3dgs_backward_accum_absgrad with any of the above, which writes the view's AbsGS statistic into
-// it and, with grad_accum_abs ([P], needs grad_accum and denom), adds its norm there.
+// it and, with grad_accum_abs ([P], needs grad_accum and denom), adds its norm there.  depth and g_distortion (optional,
+// together, [H*W] float32, not with the planes): f3dgs_backward_accum_distortion, the gradient of the depth distortion
+// from the forward's depth plane, with the AbsGS statistic as above.
 void RasterizeGaussiansBackwardAccumCUDA(
     const torch::Tensor& background, const torch::Tensor& means3D, const torch::Tensor& radii,
     const torch::Tensor& colors, const torch::Tensor& scales, const torch::Tensor& rotations, const float scale_modifier,
@@ -484,7 +538,8 @@ void RasterizeGaussiansBackwardAccumCUDA(
     const std::optional<torch::Tensor>& camera_grad, const std::optional<torch::Tensor>& semantic_feature,
     const bool antialiasing, const std::optional<torch::Tensor>& dL_dout_alpha,
     const std::optional<torch::Tensor>& dL_dout_invdepth, const std::optional<torch::Tensor>& dL_dmean2D_abs,
-    const std::optional<torch::Tensor>& grad_accum_abs) {
+    const std::optional<torch::Tensor>& grad_accum_abs, const std::optional<torch::Tensor>& depth,
+    const std::optional<torch::Tensor>& g_distortion) {
     TORCH_CHECK(means3D.is_cuda(), "means3D must be a CUDA tensor (this build has no CPU path)");
     const c10::cuda::CUDAGuard guard(means3D.device());
     const auto dev = means3D.device();
@@ -527,7 +582,11 @@ void RasterizeGaussiansBackwardAccumCUDA(
     const bool has_features = semantic_feature.has_value() && semantic_feature->defined();
     const bool has_planes = (dL_dout_alpha.has_value() && dL_dout_alpha->defined()) ||
                             (dL_dout_invdepth.has_value() && dL_dout_invdepth->defined());
-    if (has_features || antialiasing || has_planes || has_abs) {
+    const bool has_depth = depth.has_value() && depth->defined();
+    const bool has_dist = g_distortion.has_value() && g_distortion->defined();
+    TORCH_CHECK(has_depth == has_dist, "depth and g_distortion go together");
+    TORCH_CHECK(!(has_dist && has_planes), "g_distortion does not combine with dL_dout_alpha / dL_dout_invdepth");
+    if (has_features || antialiasing || has_planes || has_abs || has_dist) {
         torch::Tensor sf;
         if (has_features) {
             check_features(*semantic_feature, dev);
@@ -558,7 +617,16 @@ void RasterizeGaussiansBackwardAccumCUDA(
                       (void*)stream, cam, tail...);
         };
         const torch::Tensor none;
-        if (has_abs) {
+        if (has_dist) {
+            // the depth plane is an input, not a gradient: an empty one must not stand for zeros
+            TORCH_CHECK(depth->numel() == (int64_t)H * W, "depth must have H * W = ", (int64_t)H * W, " elements (got ",
+                        depth->numel(), ")");
+            auto dp = input(*depth, dev, "depth"), gD = plane_grad(*g_distortion, dev, H, W, "g_distortion");
+            check_rc(call(f3dgs_backward_accum_distortion, antialiasing ? 1 : 0, fptr(dp), fptr(gD),
+                          has_abs ? in_place(*dL_dmean2D_abs, dev, (int64_t)P * 3, "dL_dmean2D_abs") : nullptr,
+                          in_place(grad_accum_abs.value_or(none), dev, P, "grad_accum_abs")),
+                     "f3dgs_backward_accum_distortion");
+        } else if (has_abs) {
             torch::Tensor ga, gi;
             if (has_planes) {
                 ga = plane_grad(dL_dout_alpha.value_or(none), dev, H, W, "dL_dout_alpha");
@@ -1657,7 +1725,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
               py::arg("feature_grad_scale") = 1.0, py::arg("camera_grad") = py::none(),
               py::arg("semantic_feature") = py::none(), py::arg("antialiasing") = false,
               py::arg("dL_dout_alpha") = py::none(), py::arg("dL_dout_invdepth") = py::none(),
-              py::arg("dL_dmean2D_abs") = py::none(), py::arg("grad_accum_abs") = py::none());
+              py::arg("dL_dmean2D_abs") = py::none(), py::arg("grad_accum_abs") = py::none(),
+              py::arg("depth") = py::none(), py::arg("g_distortion") = py::none());
         m.def("rasterize_gaussians_antialiased", &RasterizeGaussiansAntialiasedCUDA);
         m.def("rasterize_gaussians_backward_antialiased", &RasterizeGaussiansBackwardAntialiasedCUDA,
               py::arg("background"), py::arg("means3D"), py::arg("radii"), py::arg("colors"), py::arg("features_like"),
@@ -1689,6 +1758,21 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
               py::arg("geomBuffer"), py::arg("R"), py::arg("binningBuffer"), py::arg("imageBuffer"), py::arg("debug"),
               py::arg("dL_dout_alpha") = py::none(), py::arg("dL_dout_invdepth") = py::none(),
               py::arg("camera") = false, py::arg("semantic_feature") = py::none(), py::arg("antialiasing") = false);
+        m.def("rasterize_gaussians_distortion", &RasterizeGaussiansDistortionCUDA, py::arg("background"),
+              py::arg("means3D"), py::arg("colors"), py::arg("semantic_feature"), py::arg("opacity"), py::arg("scales"),
+              py::arg("rotations"), py::arg("scale_modifier"), py::arg("cov3D_precomp"), py::arg("viewmatrix"),
+              py::arg("projmatrix"), py::arg("tan_fovx"), py::arg("tan_fovy"), py::arg("image_height"),
+              py::arg("image_width"), py::arg("sh"), py::arg("degree"), py::arg("campos"), py::arg("prefiltered"),
+              py::arg("debug"), py::arg("antialiasing") = false);
+        m.def("rasterize_gaussians_backward_distortion", &RasterizeGaussiansBackwardDistortionCUDA,
+              py::arg("background"), py::arg("means3D"), py::arg("radii"), py::arg("colors"), py::arg("features_like"),
+              py::arg("scales"), py::arg("rotations"), py::arg("scale_modifier"), py::arg("cov3D_precomp"),
+              py::arg("viewmatrix"), py::arg("projmatrix"), py::arg("tan_fovx"), py::arg("tan_fovy"),
+              py::arg("dL_dout_color"), py::arg("dL_dout_feature"), py::arg("dL_dout_depth"), py::arg("sh"),
+              py::arg("degree"), py::arg("campos"), py::arg("geomBuffer"), py::arg("R"), py::arg("binningBuffer"),
+              py::arg("imageBuffer"), py::arg("debug"), py::arg("depth"), py::arg("dL_ddistortion"),
+              py::arg("camera") = false, py::arg("semantic_feature") = py::none(), py::arg("antialiasing") = false,
+              py::arg("dL_dmean2D_abs") = py::none());
     }
     m.def("rasterize_gaussians_backward_camera", &RasterizeGaussiansBackwardCameraCUDA);
     m.def("rasterize_gaussians_backward_feature_geometry", &RasterizeGaussiansBackwardFeatureGeometryCUDA);

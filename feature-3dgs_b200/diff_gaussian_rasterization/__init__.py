@@ -62,6 +62,18 @@ Behavioural notes
     are GaussianRasterizer's (AntialiasedGaussianRasterizer's with antialiasing).  `ViewBatch(absgrad=True)` and
     `GaussianState(absgrad=True)` accumulate the statistic natively, and `densify_and_prune(abs_grad=...)` applies
     the split rule.
+  * depth distortion loss (opt-in; Mip-NeRF 360's term as 2DGS and gsplat's `distloss` use it, in its L1 form on view
+    depth): `DistortionGaussianRasterizer(raster_settings, feature_geometry=False, antialiasing=False)`, or
+    `rasterize_gaussians_distortion`, also returns, per pixel p over the pairs i it blends in blend order,
+        distortion_p = sum_i sum_j w_i w_j |z_i - z_j| = 2 sum_i w_i (z_i A_i - D_i),
+        A_i = sum_{j<i} w_j = 1 - T_i,   D_i = sum_{j<i} w_j z_j,
+    with w_i = alpha_i T_i and z_i the view depth the depth plane blends ([1,H,W] float32, differentiable;
+    f3dgs_forward_distortion / f3dgs_backward_distortion).  Each tile list is sorted by depth, so the prefix sums equal
+    the pairwise sum.  The loss pulls each pixel's blend weights together along the ray, which removes semi-transparent
+    floaters.  Its weight, and any normalisation by scene scale, is the caller's.  At ties in z the backward orders the
+    tied pairs by blend order.  Colour, feature map, depth, radii and their gradients are those of the rasterizer
+    without it.  `ViewBatch.forward_distortion` and `ViewBatch.backward(..., g_distortion=)` do the same without
+    autograd.
   * vector-quantised feature fields (LightGaussian, CompGS): `kmeans(x, K)` fits a codebook [K,D] and int32 codes on the
     GPU (a TF32 tensor-core assignment with the argmin fused into the GEMM, float64 segment means), `decode(codebook,
     code)` gathers the rows back (float32 or float16), and `CodePlan(code, K)` gives the codebook gradient of the
@@ -106,6 +118,8 @@ __all__ = [
     "AntialiasedGaussianRasterizer",
     "rasterize_gaussians_alpha_invdepth",
     "AlphaInvDepthGaussianRasterizer",
+    "rasterize_gaussians_distortion",
+    "DistortionGaussianRasterizer",
     "SparseGaussianAdam",
     "compute_3d_filter",
     "apply_3d_filter",
@@ -175,9 +189,10 @@ class _RasterizeGaussians(torch.autograd.Function):
 
 
 def _native_forward(ctx, fn, means3D, sh, colors_precomp, semantic_feature, opacities, scales, rotations,
-                    cov3Ds_precomp, rs, antialiasing):
+                    cov3Ds_precomp, rs, antialiasing, save_depth=False):
     """The native forward `fn` with the reference forward's positional arguments; saves on ctx what _native_backward
-    reads -> fn's results between num_rendered and the three buffers, radii last"""
+    reads (save_depth: and the depth plane, last) -> fn's results between num_rendered and the three buffers, radii
+    last"""
     if semantic_feature is None:
         semantic_feature = torch.empty(0, device=means3D.device, dtype=means3D.dtype)
     args = (rs.bg, means3D, colors_precomp, semantic_feature, opacities, scales, rotations, rs.scale_modifier,
@@ -190,7 +205,7 @@ def _native_forward(ctx, fn, means3D, sh, colors_precomp, semantic_feature, opac
     ctx.antialiasing = antialiasing
     ctx.num_rendered = num_rendered
     ctx.save_for_backward(colors_precomp, semantic_feature, means3D, scales, rotations, cov3Ds_precomp, radii,
-                          sh, geomBuffer, binningBuffer, imgBuffer)
+                          sh, geomBuffer, binningBuffer, imgBuffer, *((outs[2],) if save_depth else ()))
     ctx.mark_non_differentiable(radii)
     return outs
 
@@ -201,7 +216,7 @@ def _native_backward(ctx, fn, grad_out_color, grad_out_feature, grad_depth):
     whatever else `fn` returns."""
     rs = ctx.raster_settings
     (colors_precomp, semantic_feature, means3D, scales, rotations, cov3Ds_precomp, radii, sh, geomBuffer,
-     binningBuffer, imgBuffer) = ctx.saved_tensors
+     binningBuffer, imgBuffer) = ctx.saved_tensors[:11]
     # autograd hands None/undefined for outputs that did not take part in the loss
     if grad_out_color is None:
         grad_out_color = torch.zeros(3, rs.image_height, rs.image_width, device=means3D.device)
@@ -321,6 +336,46 @@ def _rasterize_alpha_invdepth(means3D, means2D, sh, colors_precomp, semantic_fea
                                                   rs.campos, rs, feature_geometry, antialiasing)
 
 
+class _RasterizeGaussiansDistortion(torch.autograd.Function):
+    """The render with the depth distortion plane (f3dgs_forward_distortion / f3dgs_backward_distortion) in every mode:
+    the camera tensors are always inputs and get gradients when they require grad; feature_geometry adds the feature
+    term of dL/dalpha; antialiasing renders with the antialiased opacities.  The depth plane is saved: the backward
+    reads it."""
+
+    @staticmethod
+    def forward(ctx, means3D, means2D, sh, colors_precomp, semantic_feature, opacities, scales, rotations,
+                cov3Ds_precomp, viewmatrix, projmatrix, campos, raster_settings, feature_geometry, antialiasing):
+        rs = raster_settings._replace(viewmatrix=viewmatrix, projmatrix=projmatrix, campos=campos)
+        ctx.camera_shapes = (viewmatrix.shape, projmatrix.shape, campos.shape)
+        ctx.feature_geometry = feature_geometry
+        fn = lambda *args: _C.rasterize_gaussians_distortion(*args, antialiasing=antialiasing)  # noqa: E731
+        color, feature_map, depth, distortion, radii = _native_forward(
+            ctx, fn, means3D, sh, colors_precomp, semantic_feature, opacities, scales, rotations, cov3Ds_precomp, rs,
+            antialiasing, save_depth=True)
+        return color, feature_map, radii, depth, distortion
+
+    @staticmethod
+    def backward(ctx, grad_out_color, grad_out_feature, _grad_radii, grad_depth, grad_distortion):
+        rs = ctx.raster_settings
+        camera = any(ctx.needs_input_grad[9:12])
+        depth = ctx.saved_tensors[11]
+        if grad_distortion is None:
+            grad_distortion = torch.zeros(1, rs.image_height, rs.image_width, device=rs.bg.device)
+        fn = lambda *args: _C.rasterize_gaussians_backward_distortion(  # noqa: E731
+            *args, depth, grad_distortion, camera=camera, semantic_feature=args[4] if ctx.feature_geometry else None,
+            antialiasing=ctx.antialiasing)
+        grads = _native_backward(ctx, fn, grad_out_color, grad_out_feature, grad_depth)
+        cam = tuple(None if g is None else g.reshape(shape) for g, shape in zip(grads[9:], ctx.camera_shapes))
+        return grads[:9] + cam + (None, None, None)
+
+
+def _rasterize_distortion(means3D, means2D, sh, colors_precomp, semantic_feature, opacities, scales, rotations,
+                          cov3Ds_precomp, rs, feature_geometry, antialiasing=False):
+    return _RasterizeGaussiansDistortion.apply(means3D, means2D, sh, colors_precomp, semantic_feature, opacities,
+                                               scales, rotations, cov3Ds_precomp, rs.viewmatrix, rs.projmatrix,
+                                               rs.campos, rs, feature_geometry, antialiasing)
+
+
 class _RasterizeGaussiansAbsGrad(torch.autograd.Function):
     """The default or antialiased render whose backward also gives means2D_abs AbsGS's statistic, the view's sums over
     pixels of |x| and |y| of each pixel's dL/dmean2D term (f3dgs_backward_absgrad), in every mode: the camera tensors
@@ -401,6 +456,17 @@ def rasterize_gaussians_alpha_invdepth(means3D, means2D, sh, colors_precomp, sem
                                      rotations, cov3Ds_precomp, raster_settings, feature_geometry, antialiasing)
 
 
+def rasterize_gaussians_distortion(means3D, means2D, sh, colors_precomp, semantic_feature, opacities, scales,
+                                   rotations, cov3Ds_precomp, raster_settings, feature_geometry=False,
+                                   antialiasing=False):
+    """rasterize_gaussians (feature_geometry=True: rasterize_gaussians_feature_geometry; antialiasing=True: the
+    antialiased render) that also returns the depth distortion plane sum_ij w_i w_j |z_i - z_j| ([1,H,W] float32, see
+    the module docstring) and differentiates it -> (color, feature_map, radii, depth, distortion).  Everything else,
+    gradients included, is bitwise that of the call without it."""
+    return _rasterize_distortion(means3D, means2D, sh, colors_precomp, semantic_feature, opacities, scales,
+                                 rotations, cov3Ds_precomp, raster_settings, feature_geometry, antialiasing)
+
+
 class GaussianRasterizer(nn.Module):
     """The reference's rasterizer module.  feature_geometry=True: the backward also feeds the feature map's gradient
     into the geometry (rasterize_gaussians_feature_geometry)."""
@@ -458,6 +524,19 @@ class AlphaInvDepthGaussianRasterizer(GaussianRasterizer):
     AntialiasedGaussianRasterizer's opacities."""
 
     _render = staticmethod(_rasterize_alpha_invdepth)
+
+    def __init__(self, raster_settings, feature_geometry=False, antialiasing=False):
+        super().__init__(raster_settings, feature_geometry)
+        self.antialiasing = antialiasing
+
+
+class DistortionGaussianRasterizer(GaussianRasterizer):
+    """GaussianRasterizer whose forward also returns the depth distortion plane:
+    (color, feature_map, radii, depth, distortion), distortion = sum_ij w_i w_j |z_i - z_j| per pixel, [1,H,W] float32
+    and differentiable (rasterize_gaussians_distortion).  antialiasing=True renders with AntialiasedGaussianRasterizer's
+    opacities."""
+
+    _render = staticmethod(_rasterize_distortion)
 
     def __init__(self, raster_settings, feature_geometry=False, antialiasing=False):
         super().__init__(raster_settings, feature_geometry)

@@ -87,7 +87,7 @@ class CameraGrad(NamedTuple):
 
 
 class _ViewCtx:
-    __slots__ = ("rs", "num_rendered", "radii", "geom", "binning", "img", "inputs", "antialiasing")
+    __slots__ = ("rs", "num_rendered", "radii", "geom", "binning", "img", "inputs", "antialiasing", "depth")
 
 
 class ViewBatch:
@@ -179,6 +179,15 @@ class ViewBatch:
         (color, feat, depth, alpha, invdepth), ctx = self._forward(fn, rs, antialiasing)
         return color, feat, ctx.radii, depth, alpha, invdepth, ctx
 
+    def forward_distortion(self, rs, antialiasing: bool = False):
+        """forward() that also renders the depth distortion plane sum_ij w_i w_j |z_i - z_j| ([1,H,W] float32;
+        DistortionGaussianRasterizer) -> (color, feat, radii, depth, distortion, ctx).  ctx keeps the depth plane, which
+        the backward reads; the distortion's gradient goes to backward(..., g_distortion=)."""
+        fn = lambda *args: self._C.rasterize_gaussians_distortion(*args, antialiasing=antialiasing)  # noqa: E731
+        (color, feat, depth, distortion), ctx = self._forward(fn, rs, antialiasing)
+        ctx.depth = depth
+        return color, feat, ctx.radii, depth, distortion, ctx
+
     def _forward(self, fn, rs, antialiasing):
         """The native forward `fn` of one view -> (its images, the view's ctx)"""
         p = self.params
@@ -190,11 +199,12 @@ class ViewBatch:
         ctx = _ViewCtx()
         ctx.rs = rs
         ctx.antialiasing = bool(antialiasing)
+        ctx.depth = None
         ctx.num_rendered, *images, ctx.radii, ctx.geom, ctx.binning, ctx.img = out
         return images, ctx
 
     def backward(self, ctx, g_color, g_feature, g_depth, means2D_out=None, last: bool = False, camera: bool = False,
-                 feature_geometry: bool = False, g_alpha=None, g_invdepth=None):
+                 feature_geometry: bool = False, g_distortion=None, g_alpha=None, g_invdepth=None):
         """Add this view's parameter gradients into the flat buffer.  `last=True` on the rank's last view of the step
         lets all_reduce() start the feature/opacity bucket early.  g_feature: dL/dfeature_map as a float32 or float16
         [C,H,W] tensor, a feature_head.ScaledGrad (a float16 map and its float32 scale), or None.
@@ -216,9 +226,19 @@ class ViewBatch:
         them, and they combine with camera, feature_geometry and a ScaledGrad g_feature; with both None the call is the
         one without them.
 
+        g_distortion: dL/ddistortion [1,H,W] float32 of forward_distortion's plane (f3dgs_backward_accum_distortion,
+        from the depth plane ctx kept).  It needs a ctx of forward_distortion, does not combine with g_alpha /
+        g_invdepth (ValueError), and combines with camera, feature_geometry, antialiasing, float16 features, a
+        ScaledGrad g_feature and absgrad; None is the call without it.  Pass it by keyword, as the plane gradients.
+
         With absgrad the call goes through f3dgs_backward_accum_absgrad whatever the other options: mean2D_abs then
         holds this view's AbsGS statistic and grad_accum_abs has its norm added; everything else is bitwise the call
         without it."""
+        if g_distortion is not None:
+            if ctx.depth is None:
+                raise ValueError("ViewBatch.backward: g_distortion needs the ctx of forward_distortion (it keeps depth)")
+            if g_alpha is not None or g_invdepth is not None:
+                raise ValueError("ViewBatch.backward: g_distortion does not combine with g_alpha / g_invdepth")
         rs, p, g, e = ctx.rs, self.params, self.grads, torch.Tensor([])
         none = self._empty
         scale = 1.0
@@ -234,7 +254,7 @@ class ViewBatch:
             self.grad_accum if self.grad_accum is not None else none, self.denom if self.denom is not None else none,
             int(self._ev.cuda_event) if (last and self._ev is not None) else 0, rs.debug, float(scale), cam,
             p.get("semantic_feature") if feature_geometry else None, ctx.antialiasing, g_alpha, g_invdepth,
-            self.mean2D_abs, self.grad_accum_abs)
+            self.mean2D_abs, self.grad_accum_abs, ctx.depth if g_distortion is not None else None, g_distortion)
         self._early_pending = bool(last and self._ev is not None)
         if cam is not None:
             return CameraGrad(cam[:16].view(4, 4), cam[16:32].view(4, 4), cam[32:35])

@@ -525,6 +525,90 @@ int f3dgs_backward_accum_absgrad(int P, int D, int M, int R, int C,
                                  int antialiasing, const float* dL_dalpha, const float* dL_dinvdepth,
                                  float* dL_dmean2D_abs, float* grad_accum_abs);
 
+/* ---- depth distortion loss (opt-in; Mip-NeRF 360's distortion term as 2DGS and gsplat's `distloss` use it on splats,
+ * here in its L1 form on view depth) ----
+ * For pixel p take the pairs i = 1..n the composite blends, in blend order, with w_i = alpha_i T_i and z_i the splat
+ * record's view depth (the value `depth` blends).  Each tile list is sorted by z (the sort key's low word is the float
+ * bits of z > 0), so z_i is non-decreasing along i and
+ *     L_p = sum_i sum_j w_i w_j |z_i - z_j| = 2 sum_i w_i (z_i A_i - D_i),   A_i = sum_{j<i} w_j = 1 - T_i,
+ *                                                                          D_i = sum_{j<i} w_j z_j.
+ * It pulls each pixel's blend weights together along the ray, which removes semi-transparent floaters.  Ties in z add 0.
+ * The loss weight, and any normalisation by scene scale, is the caller's.  With C > 128 chunk 0 writes the plane.
+ *   f3dgs_forward_distortion: f3dgs_forward_antialiased's arguments, then antialiasing (as in
+ *     f3dgs_forward_alpha_invdepth) and out_distortion ([H,W] float32, required).  Per blended pair the composite adds
+ *     w (z (1 - T) - D) before D takes the pair, and writes twice the sum.  Colour, the feature map, depth, radii, the
+ *     return value and the three buffers are bitwise those of the counterpart forward for the same arguments.
+ *   f3dgs_backward_distortion / f3dgs_backward_accum_distortion: the arguments of f3dgs_backward_antialiased /
+ *     f3dgs_backward_accum_antialiased (semantic_feature optional: given, the feature term of dL/dalpha is added;
+ *     dL_dcamera optional), then antialiasing (as in the _alpha_invdepth entries), depth (the forward's depth plane
+ *     [H,W], required), dL_ddistortion = dL/dL_p ([H,W] float32, required), dL_dmean2D_abs ([P,3], optional: NULL means
+ *     no AbsGS statistic; otherwise as in the _absgrad entries) and, for the accumulating entry, grad_accum_abs ([P],
+ *     optional, as in f3dgs_backward_accum_absgrad; it needs dL_dmean2D_abs).  With g = dL_ddistortion[p],
+ *     Abar_i = sum_{j>i} w_j = T_{i+1} - T_final and Dbar_i = sum_{j>i} w_j z_j, the composite adds
+ *         c_i = dL_p/dw_i = 2 [z_i (A_i - Abar_i) + Dbar_i - D_i],   D_i = depth[p] - Dbar_i - w_i z_i,
+ *         dL/dalpha_i += T_i (c_i - B_i) g,   B_i = alpha_{i+1} c_{i+1} + (1 - alpha_{i+1}) B_{i+1},   B_last = 0,
+ *         dL/dz_i     += 2 w_i (A_i - Abar_i) g.
+ *     At ties in z this is the subgradient that orders the tied pairs by blend order (the later one counts as the
+ *     farther).  The terms reach dL_dopacity, dL_dmean2D, dL_dconic, dL_dz and through the preprocess dL_dmean3D,
+ *     dL_dscale, dL_drot, dL_dcov3D, dL_dcamera and the densification statistics; under AbsGS each pixel's 2-D mean term
+ *     includes the distortion's share.  dL_dcolor and dL_dsemantic_feature are unchanged.  With dL_ddistortion = 0
+ *     every output is bitwise that of the counterpart: f3dgs_backward[_f16], _cam[_f16], _feature_geometry or
+ *     _antialiased (and their _accum twins), or the _absgrad entries without planes when dL_dmean2D_abs is given.
+ *     Distortion and the _alpha_invdepth planes do not combine in one call.
+ *   F3DGS_ERR_INVALID_ARGUMENT, before any launch, for a NULL out_distortion, depth or dL_ddistortion, an out_distortion
+ *     overlapping another output, a depth or dL_ddistortion overlapping an output, grad_accum_abs without
+ *     dL_dmean2D_abs, and whatever the counterpart rejects.
+ * Buffers: the backward reads only what every forward stores, plus `depth`.  So the buffers of any forward with the
+ * same antialiasing go to it, with that forward's depth plane. */
+int f3dgs_forward_distortion(f3dgs_alloc_fn geometry_alloc, void* geometry_ctx,
+                             f3dgs_alloc_fn binning_alloc, void* binning_ctx,
+                             f3dgs_alloc_fn image_alloc, void* image_ctx,
+                             int P, int D, int M, int C,
+                             const float* background, int width, int height,
+                             const float* means3D, const float* shs, const float* colors_precomp,
+                             const void* semantic_feature, int semantic_feature_dtype, const float* opacities,
+                             const float* scales, float scale_modifier, const float* rotations,
+                             const float* cov3D_precomp,
+                             const float* viewmatrix, const float* projmatrix, const float* cam_pos,
+                             float tan_fovx, float tan_fovy, int prefiltered,
+                             float* out_color, void* out_feature_map, float* out_depth, int* radii,
+                             int debug, void* cuda_stream,
+                             int antialiasing, float* out_distortion);
+int f3dgs_backward_distortion(int P, int D, int M, int R, int C,
+                              const float* background, int width, int height,
+                              const float* means3D, const float* shs, const float* colors_precomp,
+                              const void* semantic_feature, int semantic_feature_dtype,
+                              const float* scales, float scale_modifier, const float* rotations,
+                              const float* cov3D_precomp,
+                              const float* viewmatrix, const float* projmatrix, const float* cam_pos,
+                              float tan_fovx, float tan_fovy, const int* radii,
+                              char* geom_buffer, char* binning_buffer, char* image_buffer,
+                              const float* dL_dpix, const void* dL_dfeaturepix, int dL_dfeaturepix_dtype,
+                              float dL_dfeaturepix_scale, const float* dL_depths,
+                              float* dL_dmean2D, float* dL_dconic, float* dL_dopacity, float* dL_dcolor,
+                              float* dL_dsemantic_feature, float* dL_dmean3D, float* dL_dcov3D,
+                              float* dL_dsh, float* dL_dscale, float* dL_drot, float* dL_dz,
+                              int debug, void* cuda_stream, float* dL_dcamera,
+                              int antialiasing, const float* depth, const float* dL_ddistortion,
+                              float* dL_dmean2D_abs);
+int f3dgs_backward_accum_distortion(int P, int D, int M, int R, int C,
+                                    const float* background, int width, int height,
+                                    const float* means3D, const float* shs, const float* colors_precomp,
+                                    const void* semantic_feature, int semantic_feature_dtype,
+                                    const float* scales, float scale_modifier, const float* rotations,
+                                    const float* cov3D_precomp,
+                                    const float* viewmatrix, const float* projmatrix, const float* cam_pos,
+                                    float tan_fovx, float tan_fovy, const int* radii,
+                                    char* geom_buffer, char* binning_buffer, char* image_buffer,
+                                    const float* dL_dpix, const void* dL_dfeaturepix, int dL_dfeaturepix_dtype,
+                                    float dL_dfeaturepix_scale, const float* dL_depths, char* scratch,
+                                    float* dL_dopacity, float* dL_dcolors_precomp, float* dL_dsemantic_feature,
+                                    float* dL_dmean3D, float* dL_dcov3D_precomp, float* dL_dsh, float* dL_dscale,
+                                    float* dL_drot, float* dL_dmean2D_out, float* grad_accum, float* denom,
+                                    void* composite_done_event, int debug, void* cuda_stream, float* dL_dcamera,
+                                    int antialiasing, const float* depth, const float* dL_ddistortion,
+                                    float* dL_dmean2D_abs, float* grad_accum_abs);
+
 /* ---- feature lifting (no reference counterpart): training-free back-projection of 2-D feature maps onto Gaussians ----
  * The buffers and R are those of an f3dgs_forward / _f16 / _antialiased / _alpha_invdepth of this view at width x height
  * (any C of that forward, 0 included); feature_map [C,H,W] is a map at that resolution, 1 <= C <= F3DGS_MAX_FEATURE_DIM.
